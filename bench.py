@@ -60,6 +60,42 @@ CONFIGS = {
 SAMPLES_PER_GPU = CONFIGS[3]["samples"]
 
 
+H100_HBM_GBS, H100_F16_TFLOPS = 3350.0, 989.0  # H100 SXM data sheet (700 W): HBM3 bandwidth, dense f16 tensor rate
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, n_all, P, world, d_flags, d_scores, d_gath):
+    """What the timed path handed its caller in the last step, as float32: pose_flags [samples, P] and candidate_scores, the scores
+    of the classified poses (flags VALID | FILTERED) in (sample, pose) order — the result's pose_scores holds exactly these and
+    NaN at every other pose. Every sample, or a fixed seeded sample of them with their indices in `rows` when the whole would
+    exceed 64 MB."""
+    if world == 1:
+        scores = d_scores.view(n_all, P).cpu().numpy()
+        flags = d_flags.view(n_all, P).cpu().numpy()
+    else:  # the all-gathered slots: [scores f32 slot_samples*P][flags u8 slot_samples*P, padded to 16 B] per rank
+        from gpd_b200 import lib
+        g = d_gath.cpu().numpy()
+        slot_samples = lib.shard_bounds(n_all, 0, world)[2]
+        slot_b = lib.slot_bytes(slot_samples, P)
+        scores, flags = np.zeros((n_all, P), np.float32), np.zeros((n_all, P), np.uint8)
+        for r in range(world):
+            lo, hi, _ = lib.shard_bounds(n_all, r, world)
+            base = r * slot_b
+            scores[lo:hi] = g[base:base + (hi - lo) * P * 4].view(np.float32).reshape(hi - lo, P)
+            flags[lo:hi] = g[base + slot_samples * P * 4:base + slot_samples * P * 4 + (hi - lo) * P].reshape(hi - lo, P)
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    max_rows = (DUMP_MAX_BYTES - (1 << 20)) // (P * 4 * 3)  # scores + flags + row index per sample, with room to spare
+    if n_all > max_rows:
+        rows = np.sort(np.random.default_rng(0).choice(n_all, max_rows, replace=False))
+        scores, flags = scores[rows], flags[rows]
+        arrays["rows"] = rows.astype(np.float64)
+    arrays["pose_flags"] = flags.astype(np.float32)
+    arrays["candidate_scores"] = scores[(flags & 3) == 3].astype(np.float32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def flops_per_image(ch):
     return {"conv1": 2 * 56 * 56 * 20 * 25 * ch, "conv2": 2 * 24 * 24 * 50 * 500, "ip1": 2 * 7200 * 500 + 2 * 500 * 2}
 
@@ -91,7 +127,7 @@ def bench_params(config, **over):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -282,6 +318,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--lenet-impl", type=int, default=0)
     ap.add_argument("--no-preprocess", action="store_true", help="skip the secondary gpdb_preprocess measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's pose flags / candidate scores as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -339,7 +376,7 @@ def main():
     else:
         d_flags = torch.zeros(n * P, dtype=torch.uint8, device=dev)
         d_scores = torch.zeros(n * P, dtype=torch.float32, device=dev)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)  # > the 50 MB L2 of an H100
     stats = abi.Result()
 
     def step_resident():
@@ -370,6 +407,9 @@ def main():
     if world > 1:
         dist.barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, n_all, P, world, d_flags if world == 1 else None, d_scores if world == 1 else None,
+                     d_gath if world > 1 else None)
     # per-stage device times from a SERIAL pass (outside the timed region): in the timed steps the hand search of the chunks
     # ahead runs concurrently with images / LeNet of the current chunk, so its stage timers overlap the others
     ctx.set_overlap(0)
@@ -471,13 +511,14 @@ def main():
     if rank == 0:
         st = stage_ms / args.steps  # per step, this rank
         peaks = {}
-        try:
+        try:  # peaks measured on this machine, when present, over the data sheet's
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
-        tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+        hbm_peak = peaks.get("hbm_gbs", H100_HBM_GBS)
+        tf_peak = peaks.get("bf16_tflops_sustained", H100_F16_TFLOPS)
+        peak_src = ("measured (MEASURED_PEAKS.json)" if peaks else
+                    "fallback: H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense f16")
         # neighbourhood statistics for the algorithmic byte counts (SURVEY.md 8(d)), from the oracle's grid
         from oracle import oracle
         oc = oracle.OracleCloud(cloud["xyz"], cloud["normals"], cloud["cam_source"], cloud["view_points"])
@@ -494,26 +535,17 @@ def main():
         }
         dom = max(kernels, key=lambda k: kernels[k]["ms"])
         kd = kernels[dom]
-        # measured DRAM traffic (ncu --set full capture, profiles/traffic.json: bytes per image / per sample) scaled to
-        # the units of one step, like `achieved` (which sums all launches of the kernel in the step)
-        traffic = None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(dom)
-            if tj:
-                traffic = tj["bytes_per_unit"] * (n if tj["unit"] == "sample" else ncand)
-        except Exception:
-            pass
         if kd["bound"] == "hbm":
             ach = kd["bytes"] / (kd["ms"] * 1e-3) / 1e9
             roof = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s",
-                    "frac": ach / hbm_peak, "traffic": traffic, "peak_source": peak_src,
-                    "per": "step: all launches of the kernel summed (algorithmic bytes, CUDA-event time, ncu DRAM bytes)",
+                    "frac": ach / hbm_peak, "peak_source": peak_src,
+                    "per": "step: all launches of the kernel summed (algorithmic bytes, CUDA-event time)",
                     "algorithmic_bytes": kd["bytes"]}
         else:
             ach = kd["flops"] / (kd["ms"] * 1e-3) / 1e12
             roof = {"kernel": dom, "bound": "tensor", "achieved": ach, "peak": tf_peak, "unit": "TFLOP/s",
-                    "frac": ach / tf_peak, "traffic": traffic, "peak_source": peak_src,
-                    "per": "step: all launches of the kernel summed (algorithmic flops, CUDA-event time, ncu DRAM bytes)",
+                    "frac": ach / tf_peak, "peak_source": peak_src,
+                    "per": "step: all launches of the kernel summed (algorithmic flops, CUDA-event time)",
                     "algorithmic_flops": kd["flops"]}
         per_kernel = {}
         for k, v in kernels.items():
@@ -523,11 +555,10 @@ def main():
             else:
                 a = v["flops"] / max(v["ms"], 1e-9) / 1e9
                 per_kernel[k] = {"ms_per_step": round(v["ms"], 3), "TFLOP/s": round(a, 2), "frac_tensor": round(a / tf_peak, 4)}
-        # conv1 issues tcgen05 kind::i8 (3 int8 digit planes stacked along N): its instruction peak, measured on B200 with
-        # tools/umma_rate.cu, is 8192 MAC / clock / SM = twice the f16 / bf16 rate (profiles/r02_umma_rate.txt)
+        # conv1 issues wgmma u8 x s8 (3 int8 digit planes stacked along N): the H100 data sheet's dense int8 rate is twice the f16 rate
         per_kernel["lenet_conv1"]["frac_tensor_int8"] = round(per_kernel["lenet_conv1"]["frac_tensor"] / 2.0, 4)
-        per_kernel["lenet_conv1"]["note"] = ("kind::i8: frac_tensor is against the bf16 peak (reference scale), frac_tensor_int8 against "
-                                             "2 x that, the measured int8 instruction rate")
+        per_kernel["lenet_conv1"]["note"] = ("u8 x s8: frac_tensor is against the f16 peak (reference scale), frac_tensor_int8 against "
+                                             "2 x that, the data sheet's int8 rate")
         line = {
             "metric": cfg["metric"], "value": value, "unit": UNIT, "n_gpus": n_gpus, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": cfg["scaling"], "vs_baseline": None,

@@ -1,4 +1,4 @@
-"""gpd_b200 — the grasp-candidate hot path of atenpas/gpd on B200 (sm_100a).
+"""gpd_b200 — the grasp-candidate hot path of atenpas/gpd on H100 (sm_90a).
 
 The product is the C-ABI library gpd_b200/libgpd_b200.so (include/gpd_b200.h); this package is its ctypes binding
 (`lib`), the ctypes mirror of the boundary structs (`abi`), seeded input generators (`scenes`) and the multi-GPU

@@ -252,9 +252,9 @@ void gpdb_params_default(gpdb_params *p) {
 }
 
 const char *gpdb_build_info(void) {
-  return "gpd_b200 v1, sm_100a, kernels: k_frames k_hands k_images k_normals (fp64 / PCL-order fp32, -fmad=false), lenet: "
-         "conv1 tcgen05 kind::i8 implicit GEMM (uint8 image x 3 int8 weight digit planes, exact int32 in TMEM), conv2 tcgen05 "
-         "f16 implicit GEMM + ip1 TMA-fed tcgen05 GEMM (fp16 hi/lo split operands, fp32 accumulate in TMEM), ip2 simt; "
+  return "gpd_b200 v1, sm_90a, kernels: k_frames k_hands k_images k_normals (fp64 / PCL-order fp32, -fmad=false), lenet: "
+         "conv1 wgmma u8 x s8 implicit GEMM (uint8 image x 3 int8 weight digit planes, exact int32 accumulators), conv2 wgmma "
+         "f16 implicit GEMM + ip1 TMA-fed wgmma GEMM (fp16 hi/lo split operands, fp32 accumulate), ip2 simt; "
          "lenet_impl=1 forces the simt-fp32 kernels";
 }
 
@@ -277,8 +277,8 @@ int gpdb_create(const gpdb_params *params, gpdb_ctx **ctx_out) {
     return GPDB_ERR_INVALID;
   }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, params->device) != cudaSuccess || prop.major != 10) {
-    gpdb_set_error(nullptr, GPDB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a (B200) only",
+  if (cudaGetDeviceProperties(&prop, params->device) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+    gpdb_set_error(nullptr, GPDB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only",
                    params->device, prop.major, prop.minor);
     return GPDB_ERR_CUDA;
   }

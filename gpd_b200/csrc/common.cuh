@@ -1,4 +1,4 @@
-// common.cuh — shared declarations of libgpd_b200.so (sm_100a only).
+// common.cuh — shared declarations of libgpd_b200.so (sm_90a only).
 //
 // HBM layout of one context (see DESIGN.md "data layout"):
 //   cloud   pts4   float4[N]  points SORTED BY GRID CELL: x,y,z + original index bits  (4.8 MB @300k)
@@ -99,7 +99,7 @@ struct LenetWeights {  // device pointers, layouts documented in lenet_simt.cu
 struct C1Affine {  // conv1 epilogue: per-filter weight scale and bias (kernel parameter = constant bank)
   float scale[20], bias[20];
 };
-struct LenetTc {  // tensor-core (tcgen05) weight blobs, lenet_tc.cu
+struct LenetTc {  // tensor-core (wgmma) weight blobs, lenet_tc.cu
   void *b1, *b2, *b3;
   C1Affine c1_aff;
   int npl, nch1;
@@ -211,7 +211,7 @@ int pre_cam_expand(gpdb_ctx *ctx, int *d_out);
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);
 int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits);
 
-// lenet_tc.cu (tcgen05 conv1 / conv2)
+// lenet_tc.cu (wgmma conv1 / conv2 / ip1)
 int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]);
 struct __half;
 int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, __half *xc, float *h3);

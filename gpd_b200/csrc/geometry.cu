@@ -1,4 +1,4 @@
-// geometry.cu — the point-geometry kernels of the grasp-candidate path (sm_100a).
+// geometry.cu — the point-geometry kernels of the grasp-candidate path (sm_90a).
 //
 //   k_frames  : FrameEstimator::calculateLocalFrames  (frame_estimator.cpp:6-86, local_frame.cpp:14-41)
 //   k_hands   : HandSearch::evalHands / HandSet::evalHands / FingerHand / Antipodal / Hand::construct
@@ -1168,7 +1168,7 @@ __global__ void k_clusters(const gpdb_pose *__restrict__ hands, int n, int min_i
 // the reference's for every input.
 //
 // Pixel layout written to HBM ("P16"): one 16-byte group per pixel = channels 0..C-1 in the reference's order, bytes
-// C..15 zero, pixels row-major — exactly the K-chunk the tcgen05 conv1 reads (lenet_tc.cu), so the classifier
+// C..15 zero, pixels row-major — exactly the K-chunk the tensor-core conv1 reads (lenet_tc.cu), so the classifier
 // bulk-copies an image straight into its operand plane; k_p16_to_hwc produces the cv::Mat layout for callers that
 // want the images themselves (gpdb_images, keep_images).
 // ------------------------------------------------------------------------------------------------
@@ -2072,7 +2072,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
       for (int g = tid; g < S * RW; g += NT_IMG) {
         const int row = g / RW, c4 = g - row * RW;
         // 3x3 max of 4 pixels x 1 channel per word. Bytes are split into their even / odd 16-bit lanes (E = [b0, b2],
-        // O = [b1, b3]) so that every max is ONE native VIMNMX3.U16x2 (the 8-bit SIMD max is emulated on sm_100): vertical
+        // O = [b1, b3]) so that every max is ONE native VIMNMX3.U16x2 (the 8-bit SIMD max is emulated): vertical
         // max of the three rows first (centre word: E and O; left word: only O, whose high lane is pixel -1; right word:
         // only E, whose low lane is pixel +4), then the horizontal neighbours by lane shifts.
         unsigned res[16];

@@ -1,4 +1,4 @@
-// grid.cuh — the uniform-grid neighbour search shared by geometry.cu and preprocess.cu (sm_100a).
+// grid.cuh — the uniform-grid neighbour search shared by geometry.cu and preprocess.cu (sm_90a).
 // Cells are ordered x-fastest, so a row of cells is ONE contiguous segment of the cell-sorted point array; the
 // predicate is FLANN L2_Simple<float> (frame_estimator.cpp:74, hand_search.cpp:178, image_generator.cpp:61 and
 // pcl::search::KdTree inside pcl::NormalEstimationOMP, cloud.cpp:497-535).

@@ -1,26 +1,26 @@
-// lenet_tc.cu — LeNet conv1 / conv2 (A14) on the sm_100a tensor cores (tcgen05.mma, accumulators in TMEM).
+// lenet_tc.cu — LeNet conv1 / conv2 / ip1 (A14) on the sm_90a tensor cores (warpgroup wgmma.mma_async, accumulators in
+// registers).
 //
 // Both convolutions are IM2COL-FREE implicit GEMMs. The activations of one image live in shared memory as
 // "channel planes": plane p holds channels 8p..8p+7 of every pixel as one 16-byte group, pixels in row-major
 // order. For output pixel m = y*W + x (W = input width) and filter tap (kh, kw) the 8 channels it needs are the
 // 16-byte group  plane_p[m + kh*W + kw]  — so the A operand of the GEMM (rows = output pixels, K = taps x
 // channels) is a Hankel matrix over that plane: row stride 16 B, K-chunk stride 16 B. This is exactly a K-major
-// no-swizzle UMMA shared-memory descriptor with SBO = 128 B (8 rows x 16 B) and LBO = the byte distance between
-// the two 8-element K-chunks of one K=16 instruction (tools/umma_probe.cu T2/T4 verify this addressing on B200).
-// No patch matrix is ever materialised; every tcgen05.mma reads the plane directly.
+// no-swizzle wgmma shared-memory descriptor with SBO = 128 B (8 rows x 16 B) and LBO = the byte distance between
+// the two K-chunks of one instruction. No patch matrix is ever materialised; every wgmma reads the plane directly.
 //
 // Precision: the reference computes in float32 on raw 0..255 inputs (logits ~1e3), tolerance 1e-4 relative.
-//   conv1: integer path (kind::i8): the uint8 image is the A operand as it is; each weight is a 24-bit integer times
-//          a per-filter scale, split into three balanced int8 digits stacked along N (rows 0..19 | 20..39 | 40..59
-//          of a N = 64 B operand) so ONE instruction stream reads A once; the int32 dot products are exact and the
-//          epilogue recombines the three 20-column groups in float32 (see k_conv1_i8 below).
+//   conv1: integer path (u8 x s8 -> s32): the uint8 image is the A operand as it is; each weight is a 24-bit integer times
+//          a per-filter scale, split into three balanced int8 digits stacked along N (60 of the 64 B rows, see c1_col) so
+//          ONE instruction stream reads A once; the int32 dot products are exact and the epilogue recombines the three
+//          digits in float32 (see k_conv1_i8 below).
 //   conv2: activations a and weights w are scaled by powers of two (exact) and split in two fp16 terms each;
 //          D[:, 0:64] += a_hi w_hi + a_lo w_hi, D[:, 64:128] += a_hi w_lo  (error ~2^-22), summed in the epilogue.
 // Output pixels with x beyond the valid width are computed and discarded (7 % / 14 % of the rows).
 //
-// One CTA per SM, persistent over images; weights stay resident in shared memory (76.8 KB / 155.6 KB).
-// The 2x2 max-pool + bias (+ReLU for the 12-channel net) is fused into the epilogue: TMEM -> registers ->
-// x-pair max by shuffle -> small smem stage -> y-pair max -> global.
+// A tile of 128 GEMM rows is computed by two warpgroups (rows 0..63 | 64..127), each issuing m64 instructions; the
+// weights stay resident in shared memory (26.6 KB / 135 KB). The 2x2 max-pool + bias (+ReLU for the 12-channel net) is
+// fused into the epilogue: registers -> x-pair max by shuffle -> small smem stage -> y-pair max -> global.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -29,221 +29,140 @@
 #include <vector>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int NF1 = 20, NF2 = 50, NH = 500;
 
-struct MmaTab {  // per-instruction operand offsets (bytes) relative to tile row 0
-  uint32_t a_off, a_lbo;
-};
-
 // ---------------------------------------------------------------------------------------------------------
 // conv1: image 60x60 P16 (16-byte pixels: C uint8 channels, zero padded) -> P1 [784 px][20] float32 (pixel-major), 2x2 max-pooled.
-// Integer tensor-core path (tcgen05.mma kind::i8, int32 accumulators in TMEM): the uint8 image IS the A operand —
-// one pixel = one 16-byte K-chunk (C <= 16 channels, zero padded), so an instruction (K = 32) covers two filter taps.
+// Integer tensor-core path (wgmma .s32.u8.s8, int32 accumulators): the uint8 image IS the A operand — one pixel = one 16-byte
+// K-chunk (C <= 16 channels, zero padded), so an instruction (K = 32) covers two filter taps.
 // Weights: w = s_o * W, W a 24-bit signed integer (s_o = max|w_o| / 8.3e6 per filter), W = 65536 d0 + 256 d1 + d2 with
-// balanced int8 digits; the three digit planes are stacked along N (rows 0..19 | 20..39 | 40..59 of N = 64). The
-// dot products are EXACT integers; the epilogue recombines them in float32 (error ~1e-7 relative, like float32 itself).
+// balanced int8 digits; the three digit planes are B rows (accumulator columns) c1_col(o, digit), chosen so that the thread
+// holding a row holds all three digits of its filters. The dot products are EXACT integers; the epilogue recombines them in
+// float32 (error ~1e-7 relative, like float32 itself).
 // tiles: 28 per image, tile t = output rows 2t, 2t+1 = GEMM rows m0 = 120 t .. +119 (of 128): 120 CONSECUTIVE pixels, so the
-// sixteen 8-row core matrices of an A chunk are one contiguous 2 KB range (SBO = 128 B) and an unaligned start costs one extra
-// 128-byte wavefront per chunk. tcgen05.mma streams its operands from shared memory at the 128 B / clock the LSU also uses
-// (tools/umma_rate.cu on B200: kind::i8 128x64x32 = 48 clocks = 6 KB / 128 B with fixed descriptors, 716 clocks per 13-MMA
-// tile with this kernel's descriptors and nothing else running; a 16 x 8-pixel tile whose core matrices lie one image row apart,
-// SBO = 960 B, pools with two shuffles and needs no stage, but its scattered core matrices cost 804 clocks per tile — tried,
-// no gain). Every shared-memory access of the epilogue therefore takes a cycle from the operand stream: the 2x2 max-pool
-// stages only the UPPER output row of a tile (x-pair max by shuffle first), 28 pixels x 20 floats moved as float4 (conflict
-// free), and the lower row's threads finish the pixel (max, scale and bias from the constant bank, store): ~90 wavefronts
-// per tile instead of ~290 (both rows staged with scalar stores + a pooled pass reading stage, scale and bias from shared memory).
-// warps [0, 4 NG): NG epilogue groups (tile t -> group t % NG, TMEM buffer t % NG); warps 4 NG ..: MMA issuers (NMW);
-// last warp: producer — the images arrive from k_images already as 16-byte pixels (P16), so ONE bulk-async copy
-// (cp.async.bulk, mbarrier complete_tx) drops the next image straight into the free operand plane (double-buffered); no
-// thread ever touches the pixels.
+// 8-row core matrices of an A chunk are one contiguous range (SBO = 128 B).
+// Two CTAs per SM (88 KB of shared memory each): while one waits for its next image (one bulk-async copy of the P16 image into
+// its operand plane) or runs its epilogue, the other's instructions keep the tensor cores busy.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int C1_W = 60, C1_NPIX = 3616, C1_PLANE = C1_NPIX * 16, C1_TILES = 28, C1_TILE_ROWS = 120;
-constexpr int C1_N = 64, C1_BCHUNK = C1_N * 16;  // B rows: digit0 0..19 | digit1 20..39 | digit2 40..59 | 4 zero rows
+constexpr int C1_N = 64, C1_BCHUNK = C1_N * 16;  // B rows: 3 digits x 20 filters (c1_col) + 4 zero rows
 constexpr int C1_NCH = 25, C1_NMMA = 13;         // chunk c = kh*5 + kw (+1 zero-weight chunk)
-// measured on B200 (50.6 k images): 4 groups 4.90 ms, 5 groups 4.73 ms, 6 groups 4.97 ms, 7 groups 4.95 ms
-#ifndef GPDB_C1_NG
-#define GPDB_C1_NG 5
-#endif
-constexpr int C1_NG = GPDB_C1_NG;                 // epilogue groups = TMEM accumulator buffers
-constexpr int C1_TMEM_COLS = 64 * C1_NG <= 256 ? 256 : 512;  // allocation: a power of two
-// MMA issuer warps per CTA: with two, tiles alternate between them and the descriptor set-up of one tile (~100 dependent
-// uniform-datapath instructions) overlaps the other warp's tile. Measured (B200, 50.6 k images): conv2 (76 instructions per
-// tile) 5.73 -> 5.45 ms with two; conv1 (13 per tile) 4.80 -> 4.91 ms, so it keeps one.
-#ifndef GPDB_C1_MMA_WARPS
-#define GPDB_C1_MMA_WARPS 1
-#endif
-#ifndef GPDB_C2_MMA_WARPS
-#define GPDB_C2_MMA_WARPS 2
-#endif
-constexpr int NMW = GPDB_C1_MMA_WARPS, NMW2 = GPDB_C2_MMA_WARPS;
-constexpr int C1_MMA_WARP = 4 * C1_NG, C1_CONV_WARP0 = C1_MMA_WARP + NMW, C1_NT = (C1_CONV_WARP0 + 1) * 32;
+constexpr int C1_NT = 256, C1_CTAS_PER_SM = 2;
 constexpr int C1_IMG_BYTES = C1_W * C1_W * 16;  // one P16 image
 constexpr int C1_B_BYTES = 2 * C1_NMMA * C1_BCHUNK;
-static_assert(C1_TILES % NMW == 0 && C1_NG % NMW == 0 && (NMW == 1 || NMW == 2) && (NMW2 == 1 || NMW2 == 2), "tiles alternate between the MMA warps");
+constexpr int C1_STAGE_FLOATS = 28 * NF1;       // x-pooled upper output row of a tile
 
 // chunk c -> byte offset of row 0 inside the plane (monotonic in c)
 __host__ __device__ constexpr uint32_t c1_off(int c) {
   return (uint32_t)((((c >= C1_NCH ? C1_NCH - 1 : c) / 5) * C1_W + (c >= C1_NCH ? C1_NCH - 1 : c) % 5) * 16);
 }
-__host__ __device__ constexpr uint32_t instr_desc_i8(int M, int N) {  // D = s32, A = u8, B = s8, K-major both
-  return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// accumulator column (= B row) of digit tm of filter o: filter o = 4 f + q lives in the columns of lane quad q (8 j + 2 q + e),
+// its digits in slots s = 3 f + tm (j = s / 2, e = s % 2) — thread slot s is accumulator value 4 (s / 2) + (s % 2) (+2: row + 8)
+__host__ __device__ constexpr int c1_col(int o, int tm) {
+  return 8 * ((3 * (o >> 2) + tm) >> 1) + 2 * (o & 3) + ((3 * (o >> 2) + tm) & 1);
 }
+__device__ __forceinline__ constexpr int c1_slot_reg(int s, int h) { return 4 * (s >> 1) + 2 * h + (s & 1); }
 
-__global__ void __launch_bounds__(C1_NT, 1) k_conv1_i8(const uint8_t *__restrict__ images /* P16 */, int n,
-                                                       const uint8_t *__restrict__ wblob, const C1Affine aff /* constant bank */,
-                                                       int relu, float *__restrict__ p1) {
+__global__ void __launch_bounds__(C1_NT, C1_CTAS_PER_SM) k_conv1_i8(const uint8_t *__restrict__ images /* P16 */, int n,
+                                                                    const uint8_t *__restrict__ wblob,
+                                                                    const C1Affine aff /* constant bank */, int relu,
+                                                                    float *__restrict__ p1) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t full[C1_NG], empty[C1_NG], pl_full[2], pl_empty[2];
-  __shared__ uint32_t tmem_base;
-  uint8_t *sB = smem;                                   // 26 chunks x 64 rows x 16 B (int8)
-  uint8_t *sPl = sB + C1_B_BYTES;                       // 2 planes of 3616 px x 16 B (uint8)
-  float *stage = reinterpret_cast<float *>(sPl + 2 * C1_PLANE);        // NG x [28][20]: x-pooled upper row of a tile
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // provably warp-uniform
+  __shared__ uint64_t pl_full;
+  uint8_t *sB = smem;                                            // 26 chunks x 64 rows x 16 B (int8)
+  uint8_t *sPl = sB + C1_B_BYTES;                                // 3616 px x 16 B (uint8)
+  float *stage = reinterpret_cast<float *>(sPl + C1_PLANE);      // 2 x [28][20], alternating between tiles
+  const int tid = threadIdx.x, wg_id = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
 
   for (int i = tid; i < C1_B_BYTES / 16; i += C1_NT) reinterpret_cast<uint4 *>(sB)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
-  for (int i = tid; i < 2 * C1_PLANE / 16; i += C1_NT) reinterpret_cast<uint4 *>(sPl)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = C1_IMG_BYTES / 16 + tid; i < C1_PLANE / 16; i += C1_NT) reinterpret_cast<uint4 *>(sPl)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
-    for (int b = 0; b < C1_NG; b++) {
-      umma::mbar_init(&full[b], 1);   // tcgen05.commit of the MMA warp
-      umma::mbar_init(&empty[b], 4);  // one arrival per epilogue warp
-    }
-    for (int b = 0; b < 2; b++) {
-      umma::mbar_init(&pl_full[b], 1);   // the producer's expect_tx arrival + the bulk copy's bytes
-      umma::mbar_init(&pl_empty[b], NMW);  // tcgen05.commit of every MMA warp after its last tile of the image
-    }
-    umma::fence_mbar_init();
+    wg::mbar_init(&pl_full, 1);  // the expect_tx arrival + the bulk copy's bytes
+    wg::fence_mbar_init();
   }
-  if (warp == 0) umma::tmem_alloc(&tmem_base, C1_TMEM_COLS);
-  umma::fence_async_smem();  // the zero fill of the planes (generic proxy) before the bulk copies / MMAs (async proxy)
-  umma::fence_before_sync();
+  wg::fence_async_smem();  // weights and the zero tail (generic proxy) before the tensor-core reads (async proxy)
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tb = tmem_base;
 
-  if (warp >= C1_CONV_WARP0) {
-    // ===== producer: image `it` of this CTA -> plane (it & 1) as soon as the MMAs of image it-2 have released it
-    if (umma::elect_one()) {
-      int it = 0;
-      for (int im = blockIdx.x; im < n; im += gridDim.x, it++) {
-        const int buf = it & 1;
-        umma::mbar_wait(&pl_empty[buf], ((it >> 1) & 1) ^ 1);
-        umma::mbar_expect_tx(&pl_full[buf], C1_IMG_BYTES);
-        umma::bulk_g2s(sPl + (size_t)buf * C1_PLANE, images + (size_t)im * C1_IMG_BYTES, C1_IMG_BYTES, &pl_full[buf]);
-      }
+  const uint32_t sB_u = wg::smem_u32(sB), sPl_u = wg::smem_u32(sPl) + (uint32_t)wg_id * 64 * 16;
+  int it = 0;
+  for (int im = blockIdx.x; im < n; im += gridDim.x, it++) {
+    if (tid == 0) {
+      wg::mbar_expect_tx(&pl_full, C1_IMG_BYTES);
+      wg::bulk_g2s(sPl, images + (size_t)im * C1_IMG_BYTES, C1_IMG_BYTES, &pl_full);
     }
-    __syncwarp();
-  } else if (warp >= C1_MMA_WARP) {
-    // ===== MMA issuer warps (tile t belongs to warp t % NMW; C1_TILES and C1_NG are multiples of NMW): tile t accumulates into TMEM columns [64 (gt % NG), +64) as soon as that buffer has been
-    // drained. The whole warp runs the (fully unrolled) loop so that every descriptor is a uniform-register
-    // expression base + compile-time constant; one elected lane issues the instructions.
-    const uint32_t sB_u = umma::smem_u32(sB);
-    constexpr uint32_t idesc = instr_desc_i8(128, C1_N);
-    int gt = 0, it = 0;
-    for (int im = blockIdx.x; im < n; im += gridDim.x, it++) {
-      const int buf = it & 1;
-      umma::mbar_wait(&pl_full[buf], (it >> 1) & 1);
-      umma::fence_after_sync();
-      const uint32_t sPl_u = umma::smem_u32(sPl) + (uint32_t)buf * C1_PLANE;
-      for (int t = 0; t < C1_TILES; t++, gt++) {
-        if (t % NMW != warp - C1_MMA_WARP) continue;
-        const int b = gt % C1_NG;
-        umma::mbar_wait(&empty[b], ((gt / C1_NG) & 1) ^ 1);
-        umma::fence_after_sync();
-        const uint32_t arow = sPl_u + (uint32_t)(t * C1_TILE_ROWS) * 16;
-        const uint32_t dcol = tb + (uint32_t)b * 64;
-        if (umma::elect_one()) {
+    wg::mbar_wait(&pl_full, it & 1);
+    float *out = p1 + (size_t)im * 784 * NF1;
+    for (int t = 0; t < C1_TILES; t++) {
+      int32_t d[32];
+      const uint32_t arow = sPl_u + (uint32_t)(t * C1_TILE_ROWS) * 16;
+      wg::fence();
 #pragma unroll
-          for (int i = 0; i < C1_NMMA; i++) {
-            const uint32_t a0 = c1_off(2 * i), a1 = c1_off(2 * i + 1);
-            const uint32_t lbo = (2 * i + 1 >= C1_NCH) ? 16u : (a1 - a0);
-            umma::mma_i8(dcol, umma::desc_from(arow + a0, lbo, 128), umma::desc_from(sB_u + (uint32_t)(2 * i) * C1_BCHUNK, C1_BCHUNK, 128),
-                         idesc, i > 0);
-          }
-          umma::commit(&full[b]);
-          if (t >= C1_TILES - NMW) umma::commit(&pl_empty[buf]);  // every MMA of this warp that reads the plane has completed
-        }
-        __syncwarp();
+      for (int i = 0; i < C1_NMMA; i++) {
+        const uint32_t a0 = c1_off(2 * i), a1 = c1_off(2 * i + 1);
+        const uint32_t lbo = (2 * i + 1 >= C1_NCH) ? 16u : (a1 - a0);
+        wg::mma_u8s8_n64(d, wg::desc(arow + a0, lbo, 128), wg::desc(sB_u + (uint32_t)(2 * i) * C1_BCHUNK, C1_BCHUNK, 128), i > 0);
       }
-    }
-  } else {
-    // ===== epilogue groups drain the tiles round-robin: TMEM -> registers (recombine the three digit planes) -> x-pair max
-    // by shuffle -> the upper row's even threads stage their 20 values -> the lower row's even threads take the max with
-    // them, scale, add the bias and store the pooled pixel. Group g owns TMEM buffer g, stage g, named barrier 1 + g.
-    const int grp = warp >> 2, r = tid & 127;  // r = GEMM row = pixel (dy, x): dy = r / 60, x = r % 60
-    const int dy = r >= C1_W ? 1 : 0, x = r - dy * C1_W;
-    const bool pooled = (x & 1) == 0 && x < 56 && r < C1_TILE_ROWS;  // left pixel of a valid x-pair
-    float4 *stg = reinterpret_cast<float4 *>(stage + grp * (28 * NF1)) + (x >> 1) * (NF1 / 4);
-    int gt = 0;
-    for (int im = blockIdx.x; im < n; im += gridDim.x) {
-      float *out = p1 + (size_t)im * 784 * NF1;
-      for (int t = 0; t < C1_TILES; t++, gt++) {
-        const int b = gt % C1_NG;
-        if (b != grp) continue;
-        umma::mbar_wait_relaxed(&full[b], (gt / C1_NG) & 1);
-        umma::fence_after_sync();
-        const uint32_t trow = tb + (uint32_t)b * 64 + ((uint32_t)((warp & 3) * 32) << 16);
-        float d[64];
+      wg::commit();
+      wg::wait<0>();
+      wg::reg_fence(d);
+      // recombine the three digits of this thread's 5 filters (o = 4 f + q) for its two rows, then the x-pair max: rows r, r + 1
+      // are lanes l, l ^ 4
+      float v[2][5];
 #pragma unroll
-        for (int cb = 0; cb < 4; cb++) umma::tmem_ld16(trow + cb * 16, d + cb * 16);
-        umma::tmem_ld_wait();
-        umma::fence_before_sync();
-        __syncwarp();
-        if ((tid & 31) == 0) umma::mbar_arrive(&empty[b]);  // the buffer may be overwritten by tile t + NG
-        float v[NF1];
+      for (int h = 0; h < 2; h++)
 #pragma unroll
-        for (int j = 0; j < NF1; j++) {
-          const float f0 = (float)__float_as_int(d[j]), f1 = (float)__float_as_int(d[NF1 + j]), f2 = (float)__float_as_int(d[2 * NF1 + j]);
-          v[j] = fmaf(f0, 65536.0f, fmaf(f1, 256.0f, f2));
-          v[j] = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
+        for (int f = 0; f < 5; f++) {
+          const float f0 = (float)d[c1_slot_reg(3 * f, h)], f1 = (float)d[c1_slot_reg(3 * f + 1, h)],
+                      f2 = (float)d[c1_slot_reg(3 * f + 2, h)];
+          v[h][f] = fmaf(f0, 65536.0f, fmaf(f1, 256.0f, f2));
+          v[h][f] = fmaxf(v[h][f], __shfl_xor_sync(0xffffffffu, v[h][f], 4));
         }
-        umma::named_bar_sync(1 + grp, 128);  // the previous tile's reads of this stage are done
-        if (pooled && dy == 0) {
+      float *stg = stage + (t & 1) * C1_STAGE_FLOATS;
 #pragma unroll
-          for (int j4 = 0; j4 < NF1 / 4; j4++) stg[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
+      for (int h = 0; h < 2; h++) {
+        const int r = wg_id * 64 + warp * 16 + (lane >> 2) + 8 * h, x = r >= C1_W ? r - C1_W : r;
+        if (r < C1_W && (x & 1) == 0 && x < 56) {
+#pragma unroll
+          for (int f = 0; f < 5; f++) stg[(x >> 1) * NF1 + 4 * f + q] = v[h][f];
         }
-        umma::named_bar_sync(1 + grp, 128);
-        if (pooled && dy == 1) {
-          float4 *o = reinterpret_cast<float4 *>(out + (size_t)(t * 28 + (x >> 1)) * NF1);
+      }
+      __syncthreads();  // the upper row is staged; a stage buffer is rewritten two tiles later, after the next barrier
 #pragma unroll
-          for (int j4 = 0; j4 < NF1 / 4; j4++) {
-            const float4 u = stg[j4];
-            float m[4] = {fmaxf(v[4 * j4], u.x), fmaxf(v[4 * j4 + 1], u.y), fmaxf(v[4 * j4 + 2], u.z), fmaxf(v[4 * j4 + 3], u.w)};
+      for (int h = 0; h < 2; h++) {
+        const int r = wg_id * 64 + warp * 16 + (lane >> 2) + 8 * h, x = r - C1_W;
+        if (r >= C1_W && r < C1_TILE_ROWS && (x & 1) == 0 && x < 56) {
+          float *o = out + (size_t)(t * 28 + (x >> 1)) * NF1;
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-              m[k] = fmaf(m[k], aff.scale[4 * j4 + k], aff.bias[4 * j4 + k]);
-              if (relu) m[k] = fmaxf(m[k], 0.0f);
-            }
-            o[j4] = make_float4(m[0], m[1], m[2], m[3]);
+          for (int f = 0; f < 5; f++) {
+            const int ch = 4 * f + q;
+            float m = fmaxf(v[h][f], stg[(x >> 1) * NF1 + ch]);
+            m = fmaf(m, aff.scale[ch], aff.bias[ch]);
+            if (relu) m = fmaxf(m, 0.0f);
+            o[ch] = m;
           }
         }
       }
     }
+    __syncthreads();  // every instruction of this image has read the plane before the next bulk copy overwrites it
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tb, C1_TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // conv2: P1 [784 px][20] f32 -> P2 [j = 12x12][50] f32 (k = c + 50 j, the ip1 input order), max-pooled.
 // Tile T (6 per image) = output rows 4T .. 4T+3 = GEMM rows m = y*28 + x (112 of 128) over the EIGHT input rows
-// 4T .. 4T+7, held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two pixels, see c2_off) of 232 pixels. The planes are DOUBLE-BUFFERED and
-// written by four dedicated converter warps (float32 -> scaled fp16 hi/lo), so that the conversion of tile T+1 — and
-// the global loads of tile T+2, prefetched into registers — overlap the MMAs of tile T; no CTA-wide barrier exists in
-// the steady state (round 1 converted half an image with the whole CTA between two __syncthreads: 7.6 ms against an
-// MMA floor of 4.2 ms per 50 k images). The 4 halo rows of a tile are converted twice (converters have the slack).
-//   warps 0-7: two epilogue groups (TMEM buffer = tile parity); warps 8..: MMA issuers (tiles alternate); then 4 converter warps
-//   barriers: pl_full[2] (4 converter-warp arrivals) / pl_empty[2] (tcgen05.commit); full[2] / empty[2] for TMEM
+// 4T .. 4T+7, held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two pixels, see c2_off) of 232 pixels. The
+// planes are DOUBLE-BUFFERED: the instructions of tile T are issued asynchronously, and while the tensor cores work on them
+// the same threads convert tile T+1 (float32 -> scaled fp16 hi/lo) into the other buffer. The 4 halo rows of a tile are
+// converted twice. One CTA per SM (the weights alone take 135 KB).
 // ---------------------------------------------------------------------------------------------------------
 constexpr int C2_W = 28, C2_NPIX = 232, C2_PLANE = C2_NPIX * 16, C2_NCH = 65, C2_NMMA = 33;
 constexpr int C2_BCHUNK = 128 * 16;
 constexpr int C2_TILES = 6, C2_TILE_PIX = 8 * C2_W;  // 224 input pixels per tile
-
-constexpr int C2_MMA_WARP = 8, C2_CONV_WARP0 = C2_MMA_WARP + NMW2, C2_NCONV = 4 * 32, C2_NT = (C2_CONV_WARP0 + 4) * 32;
+constexpr int C2_NT = 256;
 constexpr int IP_K = 7200, IP_KCH = IP_K / 8;  // ip1 reduction length, in 8-element chunks
 // K-chunks (8 fp16 = 16 B per GEMM row): c < 50: plane p = c / 25 (channels 8p .. 8p+7), tap (kh, kw) = c % 25.
 // c >= 50: plane 2 holds, per pixel, channels 16..19 of that pixel AND of its right neighbour, so one chunk covers the two
@@ -259,274 +178,195 @@ __global__ void __launch_bounds__(C2_NT, 1) k_conv2_tc(const float *__restrict__
                                                        const float *__restrict__ bias, float a_scale, float out_scale, int relu,
                                                        float *__restrict__ p2, __half *__restrict__ xc, float x_scale) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t full[2], empty[2], pl_full[2], pl_empty[2];
-  __shared__ uint32_t tmem_base;
   __shared__ float sbias[64];
-  uint8_t *sB = smem;                                      // 76 chunks x 128 rows x 16 B
+  uint8_t *sB = smem;                                      // 66 chunks x 128 rows x 16 B
   uint8_t *sPl = sB + (size_t)(2 * C2_NMMA) * C2_BCHUNK;   // 2 buffers x 6 planes: hi p0..2, lo p0..2
-  float *stage = reinterpret_cast<float *>(sPl + 2 * 6 * C2_PLANE);  // 2 x [56][50]
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  float *stg = reinterpret_cast<float *>(sPl + 2 * 6 * C2_PLANE);  // [56][50]: x-pooled rows of a tile
+  const int tid = threadIdx.x, wg_id = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
 
   for (int i = tid; i < (2 * C2_NMMA) * C2_BCHUNK / 16; i += C2_NT) reinterpret_cast<uint4 *>(sB)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
   for (int i = tid; i < 2 * 6 * C2_PLANE / 16; i += C2_NT) reinterpret_cast<uint4 *>(sPl)[i] = make_uint4(0, 0, 0, 0);
   if (tid < 64) sbias[tid] = tid < NF2 ? bias[tid] : 0.0f;
-  if (tid == 0) {
-    for (int b = 0; b < 2; b++) {
-      umma::mbar_init(&full[b], 1);
-      umma::mbar_init(&empty[b], 4);
-      umma::mbar_init(&pl_full[b], 4);
-      umma::mbar_init(&pl_empty[b], 1);
-    }
-    umma::fence_mbar_init();
-  }
-  if (warp == 0) umma::tmem_alloc(&tmem_base, 256);
-  umma::fence_async_smem();
-  umma::fence_before_sync();
-  __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tb = tmem_base;
-  const uint32_t idesc_hi = umma::instr_desc(128, 128, umma::F16), idesc_lo = umma::instr_desc(128, 64, umma::F16);
 
-  if (warp >= C2_CONV_WARP0) {
-    // ===== converters: tile gt -> plane buffer gt & 1. (pixel, plane) items of a tile: 224 x 3, 6 per thread (last partial)
-    const int ct = tid - C2_CONV_WARP0 * 32;  // 0..127
-    constexpr int ITEMS = (C2_TILE_PIX * 3 + C2_NCONV - 1) / C2_NCONV;
-    float4 pre[ITEMS][2];
-    auto issue_loads = [&](int im2, int T2) {
+  // (pixel, plane) items of a tile: 224 x 3; plane 2 takes channels 16..19 of the pixel and of its right neighbour
+  auto convert = [&](int im, int T, int buf) {
+    uint8_t *pl = sPl + (size_t)buf * 6 * C2_PLANE;
+    for (int i = tid; i < C2_TILE_PIX * 3; i += C2_NT) {
+      const int lp = i / 3, p = i - lp * 3;
+      const float *src = p1 + (size_t)im * 784 * NF1 + (size_t)(4 * T * C2_W + lp) * NF1 + p * 8;
+      const float4 x0 = __ldg(reinterpret_cast<const float4 *>(src));
+      float4 x1 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p < 2) x1 = __ldg(reinterpret_cast<const float4 *>(src + 4));
+      else if (lp + 1 < C2_TILE_PIX) x1 = __ldg(reinterpret_cast<const float4 *>(src + NF1));
+      const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+      __half hi[8], lo[8];
 #pragma unroll
-      for (int j = 0; j < ITEMS; j++) {
-        const int i = ct + j * C2_NCONV;
-        pre[j][0] = make_float4(0.f, 0.f, 0.f, 0.f);
-        pre[j][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (i < C2_TILE_PIX * 3 && im2 < n) {
-          const int lp = i / 3, p = i - lp * 3;
-          const float *src = p1 + (size_t)im2 * 784 * NF1 + (size_t)(4 * T2 * C2_W + lp) * NF1 + p * 8;
-          pre[j][0] = __ldg(reinterpret_cast<const float4 *>(src));
-          if (p < 2) pre[j][1] = __ldg(reinterpret_cast<const float4 *>(src + 4));
-          else if (lp + 1 < C2_TILE_PIX) pre[j][1] = __ldg(reinterpret_cast<const float4 *>(src + NF1));  // right neighbour, channels 16..19
-        }
+      for (int e = 0; e < 8; e++) {
+        float a = x[e] * a_scale;
+        hi[e] = __float2half_rn(a);
+        lo[e] = __float2half_rn(a - __half2float(hi[e]));
       }
-    };
-    issue_loads(blockIdx.x, 0);
-    int gt = 0;
-    for (int im = blockIdx.x; im < n; im += gridDim.x) {
-      for (int T = 0; T < C2_TILES; T++, gt++) {
-        const int buf = gt & 1;
-        umma::mbar_wait(&pl_empty[buf], ((gt >> 1) & 1) ^ 1);  // the MMAs of tile gt-2 have read this buffer
-        uint8_t *pl = sPl + (size_t)buf * 6 * C2_PLANE;
-#pragma unroll
-        for (int j = 0; j < ITEMS; j++) {
-          const int i = ct + j * C2_NCONV;
-          if (i >= C2_TILE_PIX * 3) continue;
-          const int lp = i / 3, p = i - lp * 3;
-          const float x[8] = {pre[j][0].x, pre[j][0].y, pre[j][0].z, pre[j][0].w, pre[j][1].x, pre[j][1].y, pre[j][1].z, pre[j][1].w};
-          __half hi[8], lo[8];
-#pragma unroll
-          for (int e = 0; e < 8; e++) {
-            float a = x[e] * a_scale;
-            hi[e] = __float2half_rn(a);
-            lo[e] = __float2half_rn(a - __half2float(hi[e]));
-          }
-          *reinterpret_cast<uint4 *>(pl + (size_t)p * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(hi);
-          *reinterpret_cast<uint4 *>(pl + (size_t)(3 + p) * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(lo);
-        }
-        // the loads of the NEXT tile fly while the tensor cores work on this one
-        if (T + 1 < C2_TILES) issue_loads(im, T + 1);
-        else issue_loads(im + gridDim.x, 0);
-        umma::fence_async_smem();
-        __syncwarp();
-        if ((tid & 31) == 0) umma::mbar_arrive(&pl_full[buf]);
-      }
+      *reinterpret_cast<uint4 *>(pl + (size_t)p * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(hi);
+      *reinterpret_cast<uint4 *>(pl + (size_t)(3 + p) * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(lo);
     }
-  } else if (warp >= C2_MMA_WARP) {  // tile gt belongs to MMA warp gt % NMW2 (= its plane / TMEM buffer when NMW2 = 2)
-    const uint32_t sPl_u = umma::smem_u32(sPl), sB_u = umma::smem_u32(sB);
-    int gt = 0;
-    for (int im = blockIdx.x; im < n; im += gridDim.x) {
-      for (int T = 0; T < C2_TILES; T++, gt++) {
-        if (gt % NMW2 != warp - C2_MMA_WARP) continue;
-        const int b = gt & 1;
-        umma::mbar_wait(&pl_full[b], (gt >> 1) & 1);
-        umma::mbar_wait(&empty[b], ((gt >> 1) & 1) ^ 1);
-        umma::fence_after_sync();
-        const uint32_t arow = sPl_u + (uint32_t)b * 6 * C2_PLANE;
-        const uint32_t dcol = tb + (uint32_t)b * 128;
-        if (umma::elect_one()) {
+  };
+  __syncthreads();  // the zero fill is complete before any thread converts into the planes
+  if (blockIdx.x < n) convert(blockIdx.x, 0, 0);
+  wg::fence_async_smem();
+  __syncthreads();
+
+  const uint32_t sPl_u = wg::smem_u32(sPl) + (uint32_t)wg_id * 64 * 16, sB_u = wg::smem_u32(sB);
+  int gt = 0;
+  for (int im = blockIdx.x; im < n; im += gridDim.x) {
+    float *out = p2 + (size_t)im * 7200;
+    for (int T = 0; T < C2_TILES; T++, gt++) {
+      const int b = gt & 1;
+      const uint32_t arow = sPl_u + (uint32_t)b * 6 * C2_PLANE;
+      float d[64];
+      wg::fence();
 #pragma unroll
-          for (int i = 0; i < C2_NMMA; i++) {  // a_hi x [w_hi | w_lo]
-            const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
-            const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-            umma::mma_f16(dcol, umma::desc_from(arow + a0, lbo, 128),
-                          umma::desc_from(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), idesc_hi, i > 0);
-          }
-#pragma unroll
-          for (int i = 0; i < C2_NMMA; i++) {  // a_lo x w_hi
-            const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
-            const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-            umma::mma_f16(dcol, umma::desc_from(arow + 3 * C2_PLANE + a0, lbo, 128),
-                          umma::desc_from(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), idesc_lo, true);
-          }
-          umma::commit(&full[b]);      // accumulator of this tile complete
-          umma::commit(&pl_empty[b]);  // ... and its planes may be rewritten
-        }
-        __syncwarp();
+      for (int i = 0; i < C2_NMMA; i++) {  // a_hi x [w_hi | w_lo]
+        const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
+        const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
+        wg::mma_f16_n128(d, wg::desc(arow + a0, lbo, 128), wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), i > 0);
       }
-    }
-  } else {
-    const int grp = warp >> 2, r = tid & 127;
-    float *stg = stage + grp * (56 * NF2);
-    int gt = 0;
-    for (int im = blockIdx.x; im < n; im += gridDim.x) {
-      float *out = p2 + (size_t)im * 7200;
-      for (int T = 0; T < C2_TILES; T++, gt++) {
-        const int b = gt & 1;
-        if (b != grp) continue;
-        umma::mbar_wait_relaxed(&full[b], (gt >> 1) & 1);
-        umma::fence_after_sync();
-        const uint32_t trow = tb + (uint32_t)b * 128 + ((uint32_t)((warp & 3) * 32) << 16);
-        const int rr = r >> 1;  // [dy 0..3][x/2 0..13]
+#pragma unroll
+      for (int i = 0; i < C2_NMMA; i++) {  // a_lo x w_hi
+        const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
+        const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
+        wg::mma_f16_n64(d, wg::desc(arow + 3 * C2_PLANE + a0, lbo, 128),
+                        wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), true);
+      }
+      wg::commit();
+      // the operands of the next tile go into the other buffer while the tensor cores work on this one (that buffer's
+      // instructions completed before the barrier that ended the previous tile)
+      const int nim = T + 1 < C2_TILES ? im : im + gridDim.x, nT = T + 1 < C2_TILES ? T + 1 : 0;
+      if (nim < n) convert(nim, nT, b ^ 1);
+      wg::wait<0>();
+      wg::reg_fence(d);
+      // columns c and 64 + c are values i and i + 32 of the same thread; rows r, r + 1 are lanes l, l ^ 4
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int r = wg_id * 64 + warp * 16 + (lane >> 2) + 8 * h, rr = r >> 1;  // rr = [dy 0..3][x/2 0..13]
         const bool wr = (r & 1) == 0 && r < 112 && (rr % 14) < 12;
-        umma::named_bar_sync(1 + grp, 128);  // the previous tile's pooled reads of this stage are done
 #pragma unroll
-        for (int cb = 0; cb < 4; cb++) {
-          float a[16], bq[16];
-          umma::tmem_ld16(trow + cb * 16, a);
-          umma::tmem_ld16(trow + 64 + cb * 16, bq);
-          umma::tmem_ld_wait();
-          if (cb == 3) {
-            umma::fence_before_sync();
-            __syncwarp();
-            if ((tid & 31) == 0) umma::mbar_arrive(&empty[b]);
-          }
+        for (int j = 0; j < 8; j++)
 #pragma unroll
-          for (int j = 0; j < 16; j++) {
-            float v = (a[j] + bq[j]) * out_scale;
-            v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-            if (wr && cb * 16 + j < NF2) stg[rr * NF2 + cb * 16 + j] = v;
+          for (int e = 0; e < 2; e++) {
+            const int i = 4 * j + 2 * h + e, c = 8 * j + 2 * q + e;
+            float v = (d[i] + d[i + 32]) * out_scale;
+            v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+            if (wr && c < NF2) stg[rr * NF2 + c] = v;
           }
-        }
-        umma::named_bar_sync(1 + grp, 128);
-        for (int i = r; i < 2 * 12 * NF2; i += 128) {
-          int ch = i % NF2, px = (i / NF2) % 12, q = i / (NF2 * 12);
-          float m = fmaxf(stg[((2 * q) * 14 + px) * NF2 + ch], stg[((2 * q + 1) * 14 + px) * NF2 + ch]) + sbias[ch];
-          if (relu) m = fmaxf(m, 0.0f);
-          int j = (2 * T + q) * 12 + px;
-          if (p2) out[(size_t)j * NF2 + ch] = m;
-          if (xc) {  // ip1's A operand: [tile im/128][hi|lo][k/8][row im%128][k%8] fp16, scaled by 2^-8
-            const int k = ch + NF2 * j;
-            const float a = m * x_scale;
-            const __half hi = __float2half_rn(a);
-            const __half lo = __float2half_rn(a - __half2float(hi));
-            const size_t base = ((size_t)(im >> 7) * 2 * IP_KCH + (size_t)(k >> 3)) * 128 * 8 + (size_t)(im & 127) * 8 + (k & 7);
-            xc[base] = hi;
-            xc[base + (size_t)IP_KCH * 128 * 8] = lo;
-          }
+      }
+      __syncthreads();
+      for (int i = tid; i < 2 * 12 * NF2; i += C2_NT) {
+        int ch = i % NF2, px = (i / NF2) % 12, qq = i / (NF2 * 12);
+        float m = fmaxf(stg[((2 * qq) * 14 + px) * NF2 + ch], stg[((2 * qq + 1) * 14 + px) * NF2 + ch]) + sbias[ch];
+        if (relu) m = fmaxf(m, 0.0f);
+        int j = (2 * T + qq) * 12 + px;
+        if (p2) out[(size_t)j * NF2 + ch] = m;
+        if (xc) {  // ip1's A operand: [tile im/128][hi|lo][k/8][row im%128][k%8] fp16, scaled by 2^-8
+          const int k = ch + NF2 * j;
+          const float a = m * x_scale;
+          const __half hi = __float2half_rn(a);
+          const __half lo = __float2half_rn(a - __half2float(hi));
+          const size_t base = ((size_t)(im >> 7) * 2 * IP_KCH + (size_t)(k >> 3)) * 128 * 8 + (size_t)(im & 127) * 8 + (k & 7);
+          xc[base] = hi;
+          xc[base + (size_t)IP_KCH * 128 * 8] = lo;
         }
       }
+      wg::fence_async_smem();  // the converted planes of the next tile -> tensor-core reads
+      __syncthreads();         // ... and the stage is free again
     }
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tb, 256);
 }
 
 
 // ---------------------------------------------------------------------------------------------------------
-// ip1: H3[n x 500] = relu(X[n x 7200] W[7200 x 500] + b) as a TMA-fed tcgen05 GEMM.
+// ip1: H3[n x 500] = relu(X[n x 7200] W[7200 x 500] + b) as a TMA-fed wgmma GEMM.
 // CTA tile: 128 images x 128 outputs; X arrives as fp16 hi/lo in the canonical K-major layout written by conv2's
 // epilogue, W as a host-prepared fp16 hi/lo blob — both are plain contiguous byte ranges per K-block, so the
 // operand ring is filled by 1-D bulk copies (no tensor map needed).
 // D[:, 0:128] += x_hi w_hi + x_lo w_hi ; D[:, 128:256] += x_hi w_lo ; summed and rescaled in the epilogue.
-// warp 4: MMA issuer, warp 5: bulk-copy producer, warps 0-3: epilogue.
+// warps 0-7: two consumer warpgroups (images 0..63 | 64..127 of the tile, 128 accumulators per thread), warp 8: producer.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int IP_KB_CH = 6, IP_NKB = IP_KCH / IP_KB_CH, IP_STAGES = 4;     // 48-element K-blocks, 150 of them
 constexpr int IP_A_BYTES = IP_KB_CH * 128 * 16, IP_B_BYTES = IP_KB_CH * 256 * 16;
 constexpr int IP_STAGE_BYTES = 2 * IP_A_BYTES + IP_B_BYTES;                 // 49152
-constexpr int IP_NT = 192;
+constexpr int IP_NT = 288;
 
 __global__ void __launch_bounds__(IP_NT, 1) k_ip1_tc(const __half *__restrict__ xc, int n, const uint8_t *__restrict__ wblob,
                                                      const float *__restrict__ bias, float out_scale, float *__restrict__ h3) {
   extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t full[IP_STAGES], empty[IP_STAGES], done;
-  __shared__ uint32_t tmem_base;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  __shared__ uint64_t full[IP_STAGES], empty[IP_STAGES];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mt = blockIdx.x, ob = blockIdx.y;
   if (tid == 0) {
     for (int s = 0; s < IP_STAGES; s++) {
-      umma::mbar_init(&full[s], 1);
-      umma::mbar_init(&empty[s], 1);
+      wg::mbar_init(&full[s], 1);
+      wg::mbar_init(&empty[s], 8);  // one arrival per consumer warp
     }
-    umma::mbar_init(&done, 1);
-    umma::fence_mbar_init();
+    wg::fence_mbar_init();
   }
-  if (warp == 0) umma::tmem_alloc(&tmem_base, 256);
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tb = tmem_base;
-  if (warp == 5) {
+  if (warp == 8) {
     // ===== producer: one elected lane streams the K-blocks through the ring
-    if (umma::elect_one()) {
+    if (wg::elect_one()) {
       const uint8_t *xa_hi = reinterpret_cast<const uint8_t *>(xc) + (size_t)mt * 2 * IP_KCH * 128 * 16;
       const uint8_t *xa_lo = xa_hi + (size_t)IP_KCH * 128 * 16;
       const uint8_t *wb = wblob + (size_t)ob * IP_NKB * IP_B_BYTES;
       for (int kb = 0; kb < IP_NKB; kb++) {
         const int s = kb % IP_STAGES;
-        umma::mbar_wait(&empty[s], ((kb / IP_STAGES) & 1) ^ 1);
+        wg::mbar_wait(&empty[s], ((kb / IP_STAGES) & 1) ^ 1);
         uint8_t *st = smem + (size_t)s * IP_STAGE_BYTES;
-        umma::mbar_expect_tx(&full[s], IP_STAGE_BYTES);
-        umma::bulk_g2s(st, xa_hi + (size_t)kb * IP_A_BYTES, IP_A_BYTES, &full[s]);
-        umma::bulk_g2s(st + IP_A_BYTES, xa_lo + (size_t)kb * IP_A_BYTES, IP_A_BYTES, &full[s]);
-        umma::bulk_g2s(st + 2 * IP_A_BYTES, wb + (size_t)kb * IP_B_BYTES, IP_B_BYTES, &full[s]);
+        wg::mbar_expect_tx(&full[s], IP_STAGE_BYTES);
+        wg::bulk_g2s(st, xa_hi + (size_t)kb * IP_A_BYTES, IP_A_BYTES, &full[s]);
+        wg::bulk_g2s(st + IP_A_BYTES, xa_lo + (size_t)kb * IP_A_BYTES, IP_A_BYTES, &full[s]);
+        wg::bulk_g2s(st + 2 * IP_A_BYTES, wb + (size_t)kb * IP_B_BYTES, IP_B_BYTES, &full[s]);
       }
     }
     __syncwarp();
-  } else if (warp == 4) {
-    // ===== MMA issuer
-    const uint32_t idesc_hi = umma::instr_desc(128, 256, umma::F16), idesc_lo = umma::instr_desc(128, 128, umma::F16);
-    const uint32_t sm_u = umma::smem_u32(smem);
-    for (int kb = 0; kb < IP_NKB; kb++) {
-      const int s = kb % IP_STAGES;
-      umma::mbar_wait(&full[s], (kb / IP_STAGES) & 1);
-      umma::fence_after_sync();
-      const uint32_t st = sm_u + (uint32_t)s * IP_STAGE_BYTES;
-      if (umma::elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < IP_KB_CH / 2; ks++) {
-          const uint64_t da_hi = umma::desc_from(st + (uint32_t)(2 * ks) * 128 * 16, 128 * 16, 128);
-          const uint64_t da_lo = umma::desc_from(st + IP_A_BYTES + (uint32_t)(2 * ks) * 128 * 16, 128 * 16, 128);
-          const uint64_t db = umma::desc_from(st + 2 * IP_A_BYTES + (uint32_t)(2 * ks) * 256 * 16, 256 * 16, 128);
-          umma::mma_f16(tb, da_hi, db, idesc_hi, (kb | ks) != 0);  // x_hi x [w_hi | w_lo]
-          umma::mma_f16(tb, da_lo, db, idesc_lo, true);            // x_lo x w_hi
-        }
-        umma::commit(&empty[s]);                    // the stage may be refilled once these MMAs have read it
-        if (kb == IP_NKB - 1) umma::commit(&done);  // accumulator complete
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===== epilogue: rows = images of this M-tile
-    umma::mbar_wait(&done, 0);
-    umma::fence_after_sync();
-    const int im = mt * 128 + tid;
-    const uint32_t trow = tb + ((uint32_t)(warp * 32) << 16);
-#pragma unroll
-    for (int cb = 0; cb < 8; cb++) {
-      float a[16], b[16];
-      umma::tmem_ld16(trow + cb * 16, a);
-      umma::tmem_ld16(trow + 128 + cb * 16, b);
-      umma::tmem_ld_wait();
-      if (im < n) {
-#pragma unroll
-        for (int j = 0; j < 16; j++) {
-          const int o = ob * 128 + cb * 16 + j;
-          if (o < NH) h3[(size_t)im * NH + o] = fmaxf((a[j] + b[j]) * out_scale + __ldg(bias + o), 0.0f);
-        }
-      }
-    }
-    umma::fence_before_sync();
+    return;
   }
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tb, 256);
+  // ===== consumers
+  const int wg_id = warp >> 2, q = lane & 3;
+  const uint32_t sm_u = wg::smem_u32(smem), a_row = (uint32_t)wg_id * 64 * 16;
+  float d[128];
+#pragma unroll
+  for (int i = 0; i < 128; i++) d[i] = 0.0f;
+  for (int kb = 0; kb < IP_NKB; kb++) {
+    const int s = kb % IP_STAGES;
+    wg::mbar_wait(&full[s], (kb / IP_STAGES) & 1);
+    const uint32_t st = sm_u + (uint32_t)s * IP_STAGE_BYTES;
+    wg::fence();
+#pragma unroll
+    for (int ks = 0; ks < IP_KB_CH / 2; ks++) {
+      const uint64_t da_hi = wg::desc(st + a_row + (uint32_t)(2 * ks) * 128 * 16, 128 * 16, 128);
+      const uint64_t da_lo = wg::desc(st + IP_A_BYTES + a_row + (uint32_t)(2 * ks) * 128 * 16, 128 * 16, 128);
+      const uint64_t db = wg::desc(st + 2 * IP_A_BYTES + (uint32_t)(2 * ks) * 256 * 16, 256 * 16, 128);
+      wg::mma_f16_n256(d, da_hi, db, (kb | ks) != 0);  // x_hi x [w_hi | w_lo]
+      wg::mma_f16_n128(d, da_lo, db, true);            // x_lo x w_hi
+    }
+    wg::commit();
+    wg::wait<1>();  // the instructions of K-block kb - 1 have read their stage: it may be refilled
+    if (kb > 0 && lane == 0) wg::mbar_arrive(&empty[(kb - 1) % IP_STAGES]);
+  }
+  wg::wait<0>();
+  wg::reg_fence(d);
+  // columns c and 128 + c are values i and i + 64 of the same thread
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int im = mt * 128 + wg_id * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    if (im >= n) continue;
+#pragma unroll
+    for (int j = 0; j < 16; j++)
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        const int i = 4 * j + 2 * h + e, o = ob * 128 + 8 * j + 2 * q + e;
+        if (o < NH) h3[(size_t)im * NH + o] = fmaxf((d[i] + d[i + 64]) * out_scale + __ldg(bias + o), 0.0f);
+      }
+  }
 }
 
 }  // namespace
@@ -552,7 +392,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
   LenetTc &t = ctx->tc;
   t.npl = 1;
   t.nch1 = C1_NCH;
-  // conv1 blob: [chunk c = kh*5+kw (26, last zero)][row n = digit*20 + o (64)][16 x int8: channel e], then 20 float scales
+  // conv1 blob: [chunk c = kh*5+kw (26, last zero)][row n = c1_col(o, digit) (64)][16 x int8: channel e], then 20 float scales
   std::vector<int8_t> b1((size_t)C1_B_BYTES + NF1 * sizeof(float), 0);
   {
     float *scales = reinterpret_cast<float *>(b1.data() + C1_B_BYTES);
@@ -576,7 +416,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
             }
             dg[0] = (int)std::max(-128L, std::min(127L, W));
             const int c = kh * 5 + kw;
-            for (int tm = 0; tm < 3; tm++) b1[((size_t)c * C1_N + tm * NF1 + o) * 16 + ch] = (int8_t)dg[tm];
+            for (int tm = 0; tm < 3; tm++) b1[((size_t)c * C1_N + c1_col(o, tm)) * 16 + ch] = (int8_t)dg[tm];
           }
     }
   }
@@ -663,18 +503,18 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
   return GPDB_OK;
 }
 
-// conv1 + pool, conv2 + pool and ip1 + ReLU on tcgen05; p1 [n][784][20] f32, xc = fp16 hi/lo ip1 operand, h3 [n][500]
+// conv1 + pool, conv2 + pool and ip1 + ReLU on wgmma; p1 [n][784][20] f32, xc = fp16 hi/lo ip1 operand, h3 [n][500]
 int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, __half *xc, float *h3) {
   const LenetTc &t = ctx->tc;
   const int relu = ctx->prm.relu_after_conv;
-  size_t sm1 = (size_t)C1_B_BYTES + 2 * (size_t)C1_PLANE + C1_NG * 28 * NF1 * sizeof(float) + 32;
-  size_t sm2 = (size_t)(2 * C2_NMMA) * C2_BCHUNK + 2 * 6 * C2_PLANE + 2 * 56 * NF2 * sizeof(float);
+  size_t sm1 = (size_t)C1_B_BYTES + C1_PLANE + 2 * C1_STAGE_FLOATS * sizeof(float);
+  size_t sm2 = (size_t)(2 * C2_NMMA) * C2_BCHUNK + 2 * 6 * C2_PLANE + 56 * NF2 * sizeof(float);
   size_t sm3 = (size_t)IP_STAGES * IP_STAGE_BYTES;
   CUDA_TRY(cudaFuncSetAttribute(k_conv1_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
   CUDA_TRY(cudaFuncSetAttribute(k_conv2_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
   CUDA_TRY(cudaFuncSetAttribute(k_ip1_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm3));
   cudaEvent_t e1 = gpdb_st_begin(ctx);
-  k_conv1_i8<<<std::min(n, ctx->sm_count), C1_NT, sm1, ctx->stream>>>(d_images, n, (const uint8_t *)t.b1, t.c1_aff, relu, p1);
+  k_conv1_i8<<<std::min(n, C1_CTAS_PER_SM * ctx->sm_count), C1_NT, sm1, ctx->stream>>>(d_images, n, (const uint8_t *)t.b1, t.c1_aff, relu, p1);
   LAUNCH_CHECK();
   gpdb_st_end(ctx, 5, e1);
   cudaEvent_t e2 = gpdb_st_begin(ctx);

@@ -336,7 +336,7 @@ bool preprocessParamsFromConfig(const std::string &config_filename, gpdb_preproc
 
 // ---- the reference's own C interface for Python callers (src/detect_grasps_python.cpp:49-65,431-549,598-607; the two
 // calcGraspDescriptors* entry points write HDF5 through cv::hdf and are not provided),
-// same names, argument order and struct layout, over the B200 path (exported by libgpd_host.so) -----------------
+// same names, argument order and struct layout, over the GPU path (exported by libgpd_host.so) -----------------
 extern "C" {
 struct Grasp {       // detect_grasps_python.cpp:49-56
   double *pos;       // Hand position (3)

@@ -1,5 +1,5 @@
 // detect_grasps CONFIG_FILE PCD_FILE [NORMALS_FILE] — the reference's command line (src/detect_grasps.cpp:20-94) over
-// the B200 path. A cloud without normals is preprocessed on the device (workspace filter, voxelisation, normal
+// the GPU path. A cloud without normals is preprocessed on the device (workspace filter, voxelisation, normal
 // estimation: GraspDetector::preprocessPointCloud -> gpdb_preprocess); normals given as PCD fields or as a
 // NORMALS_FILE are kept.
 // --dump-config prints the parsed parameters as JSON and exits (used by the CPU tests).

@@ -803,7 +803,7 @@ void GraspDetector::preprocessPointCloud(util::Cloud &cloud) {
   double ms[6];
   gpdb_preprocess_timings(ctx_, ms);
   if (pp.voxelize) printf("Voxelized cloud: %d\n", n);
-  if (pp.estimate_normals) printf("Calculated %d surface normals in %3.4fs (mode: B200).\n", n, ms[4] * 1e-3);
+  if (pp.estimate_normals) printf("Calculated %d surface normals in %3.4fs (mode: GPU).\n", n, ms[4] * 1e-3);
   std::vector<float> xyz(3 * (size_t)n);
   std::vector<double> nrm(3 * (size_t)n);
   std::vector<int> cam((size_t)n * cloud.numCameras());

@@ -2,7 +2,7 @@
 
 The library is built in-tree (gpd_b200/csrc/Makefile, __graft_entry__.build()). There is no CPU
 fallback: if the shared object is missing this module raises, and every compute call returns
-GPDB_ERR_CUDA when no sm_100 device is present.
+GPDB_ERR_CUDA when no sm_90 device is present.
 """
 import ctypes as C
 import os
@@ -40,7 +40,7 @@ def lib():
     if not os.path.exists(SO_PATH):
         raise RuntimeError(
             f"{SO_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). gpd_b200 has no CPU fallback.")
+            "(nvcc, sm_90a). gpd_b200 has no CPU fallback.")
     L = C.CDLL(SO_PATH)
     vp = C.c_void_p
     L.gpdb_params_default.argtypes = [C.POINTER(abi.Params)]

@@ -1,5 +1,5 @@
 /*
- * gpd_b200.h — C-ABI of libgpd_b200.so: the B200-native grasp-candidate hot path.
+ * gpd_b200.h — C-ABI of libgpd_b200.so: the H100-native grasp-candidate hot path.
  *
  * This is the drop-in boundary for the ONE path of atenpas/gpd that this repo
  * accelerates (GraspDetector::detectGrasps steps 1-4, reference
@@ -22,7 +22,7 @@
  * `GraspDetector::detectGrasps` shims) a maintainer would add.
  *
  * There is NO CPU fallback behind these symbols: every compute entry point
- * returns GPDB_ERR_CUDA when no sm_100 device is usable.
+ * returns GPDB_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef GPD_B200_H_
 #define GPD_B200_H_
@@ -99,7 +99,7 @@ typedef struct gpdb_params {
   int32_t device;           /* CUDA device ordinal                                    */
   int32_t chunk_samples;    /* samples per device pass; 0 = library default           */
   int32_t keep_images;      /* gpdb_detect also returns the grasp images              */
-  int32_t lenet_impl;       /* 0 = default (tcgen05 when built), 1 = force SIMT fp32  */
+  int32_t lenet_impl;       /* 0 = default (wgmma tensor cores), 1 = force SIMT fp32  */
 } gpdb_params;
 
 /* One grasp candidate = candidate::Hand (include/gpd/candidate/hand.h:267-276). */

@@ -119,7 +119,7 @@ def test_images_entry_point_other_channel_counts(ch):
     ctx.close()
 
 
-@pytest.mark.parametrize("impl", [0, 1])  # 0 = tcgen05 convolutions, 1 = SIMT float32
+@pytest.mark.parametrize("impl", [0, 1])  # 0 = wgmma convolutions, 1 = SIMT float32
 @pytest.mark.parametrize("name,ch", [("lenet_caffe_15ch", 15), ("lenet_caffe_3ch", 3), ("lenet_ir_12ch", 12)])
 def test_classifier_against_reference_model_goldens(golden_dir, name, ch, impl):
     import os
@@ -208,7 +208,7 @@ def test_full_size_properties_config3():
 
 @pytest.mark.parametrize("ch", [15, 3, 12])
 def test_tensor_core_lenet_matches_simt_and_oracle_on_many_images(ch):
-    """tcgen05 implicit-GEMM convolutions (bf16x3 / fp16x2 split operands) vs the float32 SIMT kernels vs the oracle
+    """wgmma implicit-GEMM convolutions (int8 digit planes / fp16x2 split operands) vs the float32 SIMT kernels vs the oracle
     on a few thousand images, random-init weights of the reference's architecture and scale."""
     rng = np.random.default_rng(ch)
     n = 1500

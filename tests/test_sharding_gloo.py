@@ -1,6 +1,6 @@
 """world_size-2 gloo test (CPU) of the multi-GPU host logic: contiguous slices of the sample indices over a
 broadcast cloud, one all-gather of fixed-stride score slots (gpd_b200/sharding.py). The per-rank compute is
-stood in by the oracle here (no GPU in this container); on the B200 box the same code runs with NCCL."""
+stood in by the oracle here (no GPU in this container); on a GPU machine the same code runs with NCCL."""
 import os
 import socket
 

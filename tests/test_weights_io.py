@@ -1,19 +1,23 @@
 """Weight import from the reference's other backends' formats (SURVEY.md 8(f).2): `.caffemodel` (Caffe backend) and
 OpenVINO IR `.xml` + `.bin` -> the .bin parameter-directory layout (gpdb_read_weights_file / gpdb_load_weights_file).
 
-CPU: the wire-level parsers against files written by this test (a minimal protobuf encoder / an IR skeleton) and — in
-the build container, where /root/reference exists — against the reference's own model files, which must reproduce the
-shipped .bin parameters bit for bit. GPU: a context loaded from a .caffemodel scores like one given the arrays."""
+CPU: the wire-level parsers against files written by this test (a minimal protobuf encoder / an IR skeleton) and against
+the reference's own model files, rebuilt byte for byte from the shipped weights and tests/golden/model_skeletons.npz
+(tools/make_model_skeletons.py), which must reproduce the shipped .bin parameters bit for bit. GPU: a context loaded from a .caffemodel scores like one given the arrays."""
+import hashlib
 import os
 import struct
 
 import numpy as np
 import pytest
 
-from conftest import load_weights
 from gpd_b200 import lib
 
-REF = "/root/reference/models"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# the reference's model files (paths under its models/ directory) and the net whose weights they hold
+MODEL_FILES = {"caffe15": (15, "caffe/15channels/two_views_15_channels_90_deg_no_flipping.caffemodel"),
+               "caffe3": (3, "caffe/3channels/bottles_boxes_cans_5xNeg.caffemodel"),
+               "ir12": (12, "openvino/two_views_12_channels_curv_axis.bin")}
 NAMES = ["conv1_weights", "conv1_biases", "conv2_weights", "conv2_biases", "ip1_weights", "ip1_biases", "ip2_weights", "ip2_biases"]
 
 
@@ -104,16 +108,42 @@ def test_openvino_ir_parser(tmp_path):
             assert np.array_equal(a, e)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference's model files exist only in the build container")
-def test_reference_model_files_reproduce_the_bin_parameters():
-    for ch, path in ((15, f"{REF}/caffe/15channels/two_views_15_channels_90_deg_no_flipping.caffemodel"),
-                     (3, f"{REF}/caffe/3channels/bottles_boxes_cans_5xNeg.caffemodel")):
-        arrs, _ = lib.read_weights_file(path, ch)
-        ref = [np.fromfile(f"{REF}/lenet/{ch}channels/params/{n}.bin", dtype=np.float32) for n in NAMES]
-        assert all(np.array_equal(a, r) for a, r in zip(arrs, ref)), ch
-    arrs, relu = lib.read_weights_file(f"{REF}/openvino/two_views_12_channels_curv_axis.bin", 12)
-    w12, _ = load_weights(12)
-    assert relu == 3 and all(np.array_equal(a, np.ravel(r)) for a, r in zip(arrs, w12))
+def framework_order(bin_arrays):
+    """Inverse of expected_bin_layout: the eight arrays flat, in the order Caffe / the OpenVINO IR store them."""
+    c1w, c1b, c2w, c2b, ip1, f1b, ip2, f2b = [np.ravel(np.asarray(a, np.float32)) for a in bin_arrays]
+    f1w = ip1.reshape(144, 50, 500).transpose(2, 1, 0)  # [o + 500 (c + 50 j)] -> W[o, c 144 + j]
+    return [np.ascontiguousarray(a).ravel() for a in (c1w, c1b, c2w, c2b, f1w, f1b, ip2.reshape(500, 2).T, f2b)]
+
+
+def shipped_weights(ch):
+    z = np.load(os.path.join(ROOT, "gpd_b200", "weights", f"lenet_{ch}ch.npz"))
+    return [np.ravel(z[n]) for n in NAMES]
+
+
+def rebuild_model_file(key, out_dir):
+    """The reference's model file `key`, byte for byte: its stored skeleton with the shipped weights put back in place."""
+    g = np.load(os.path.join(ROOT, "tests", "golden", "model_skeletons.npz"))
+    ch, rel = MODEL_FILES[key]
+    skel, data, pos = g[key + "_skeleton"].tobytes(), bytearray(), 0
+    for off, a in zip(g[key + "_offsets"], framework_order(shipped_weights(ch))):
+        data += skel[pos:off] + a.tobytes()
+        pos = int(off)
+    data += skel[pos:]
+    assert hashlib.sha256(data).hexdigest() == str(g[key + "_sha256"]), key
+    path = out_dir / os.path.basename(rel)
+    path.write_bytes(bytes(data))
+    if key + "_xml" in g.files:
+        path.with_suffix(".xml").write_bytes(g[key + "_xml"].tobytes())
+    return str(path)
+
+
+def test_reference_model_files_reproduce_the_bin_parameters(tmp_path):
+    for key in ("caffe15", "caffe3", "ir12"):
+        ch = MODEL_FILES[key][0]
+        arrs, relu = lib.read_weights_file(rebuild_model_file(key, tmp_path), ch)
+        assert all(np.array_equal(a, r) for a, r in zip(arrs, shipped_weights(ch))), key
+        if key == "ir12":
+            assert relu == 3
 
 
 @pytest.mark.gpu
