@@ -15,11 +15,12 @@
 //          ONE instruction stream reads A once; the int32 dot products are exact and the epilogue recombines the three
 //          digits in float32 (see k_conv1_i8 below).
 //   conv2: activations a and weights w are scaled by powers of two (exact) and split in two fp16 terms each;
-//          D[:, 0:64] += a_hi w_hi + a_lo w_hi, D[:, 64:128] += a_hi w_lo  (error ~2^-22), summed in the epilogue.
+//          D[:, 0:56] += a_hi w_hi + a_lo w_hi, D[:, 56:112] += a_hi w_lo  (error ~2^-22), summed in the epilogue.
 // Output pixels with x beyond the valid width are computed and discarded (7 % / 14 % of the rows).
 //
-// A tile of 128 GEMM rows is computed by two warpgroups (rows 0..63 | 64..127), each issuing m64 instructions; the
-// weights stay resident in shared memory (26.6 KB / 135 KB). The 2x2 max-pool + bias (+ReLU for the 12-channel net) is
+// conv1 computes a tile of 128 GEMM rows with two warpgroups (rows 0..63 | 64..127); conv2 is warp-specialised: a converter
+// warpgroup feeds two consumer warpgroups that each own whole 128-row tiles and alternate on the tensor cores. The
+// weights stay resident in shared memory (26.6 KB / 115.5 KB). The 2x2 max-pool + bias (+ReLU for the 12-channel net) is
 // fused into the epilogue: registers -> x-pair max by shuffle -> small smem stage -> y-pair max -> global.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -152,17 +153,26 @@ __global__ void __launch_bounds__(C1_NT, C1_CTAS_PER_SM) k_conv1_i8(const uint8_
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// conv2: P1 [784 px][20] f32 -> P2 [j = 12x12][50] f32 (k = c + 50 j, the ip1 input order), max-pooled.
+// conv2: P1 [784 px][20] f32 -> ip1's fp16 hi/lo operand xc (k = c + 50 j, j = 12x12 pooled pixel), max-pooled.
 // Tile T (6 per image) = output rows 4T .. 4T+3 = GEMM rows m = y*28 + x (112 of 128) over the EIGHT input rows
-// 4T .. 4T+7, held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two pixels, see c2_off) of 232 pixels. The
-// planes are DOUBLE-BUFFERED: the instructions of tile T are issued asynchronously, and while the tensor cores work on them
-// the same threads convert tile T+1 (float32 -> scaled fp16 hi/lo) into the other buffer. The 4 halo rows of a tile are
-// converted twice. One CTA per SM (the weights alone take 135 KB).
+// 4T .. 4T+7 (224 consecutive P1 pixels, 17.5 KB), held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two
+// pixels, see c2_off) of 232 pixels. The 4 halo rows of a tile are converted twice. One CTA per SM, three warpgroups:
+//   warpgroup 0, converter: one bulk copy per tile brings its float32 pixels into a raw buffer (two, filled two tiles
+//     ahead); the warpgroup converts them to the scaled fp16 hi/lo planes of a plane stage and arrives on its `full` barrier.
+//   warpgroups 1, 2, consumers: consumer c owns the tiles g = c, c + 2, ... of the CTA's sequence (and plane stage c) and
+//     issues both m64 halves of each. Named barriers order the two consumers' instruction batches (ping-pong), so the
+//     tensor cores run one consumer's tile while the other runs its epilogue (x-pair max by shuffle -> own stage ->
+//     y-pair max + bias -> 16-byte stores of 8 consecutive k of xc).
+// N = 112 + 56: D[:, 0:56] += a_hi w_hi + a_lo w_hi, D[:, 56:112] += a_hi w_lo (w rows 50..55 / 106..111 are zero).
 // ---------------------------------------------------------------------------------------------------------
 constexpr int C2_W = 28, C2_NPIX = 232, C2_PLANE = C2_NPIX * 16, C2_NCH = 65, C2_NMMA = 33;
-constexpr int C2_BCHUNK = 128 * 16;
+constexpr int C2_N = 112, C2_BCHUNK = C2_N * 16;  // B rows per K-chunk: 0..55 w_hi, 56..111 w_lo
+constexpr int C2_B_BYTES = 2 * C2_NMMA * C2_BCHUNK;
 constexpr int C2_TILES = 6, C2_TILE_PIX = 8 * C2_W;  // 224 input pixels per tile
-constexpr int C2_NT = 256;
+constexpr int C2_STAGE = 6 * C2_PLANE;               // one plane stage: hi p0..2, lo p0..2
+constexpr int C2_RAW_BYTES = C2_TILE_PIX * 20 * 4;   // a tile's float32 input pixels
+constexpr int C2_STG_FLOATS = 56 * 50;               // x-pooled rows of a tile [dy 0..3][x/2 0..13][50]
+constexpr int C2_NT = 384;
 constexpr int IP_K = 7200, IP_KCH = IP_K / 8;  // ip1 reduction length, in 8-element chunks
 // K-chunks (8 fp16 = 16 B per GEMM row): c < 50: plane p = c / 25 (channels 8p .. 8p+7), tap (kh, kw) = c % 25.
 // c >= 50: plane 2 holds, per pixel, channels 16..19 of that pixel AND of its right neighbour, so one chunk covers the two
@@ -176,112 +186,159 @@ __host__ __device__ constexpr uint32_t c2_off(int c) {
 
 __global__ void __launch_bounds__(C2_NT, 1) k_conv2_tc(const float *__restrict__ p1, int n, const uint8_t *__restrict__ wblob,
                                                        const float *__restrict__ bias, float a_scale, float out_scale, int relu,
-                                                       float *__restrict__ p2, __half *__restrict__ xc, float x_scale) {
+                                                       __half *__restrict__ xc, float x_scale) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ float sbias[64];
-  uint8_t *sB = smem;                                      // 66 chunks x 128 rows x 16 B
-  uint8_t *sPl = sB + (size_t)(2 * C2_NMMA) * C2_BCHUNK;   // 2 buffers x 6 planes: hi p0..2, lo p0..2
-  float *stg = reinterpret_cast<float *>(sPl + 2 * 6 * C2_PLANE);  // [56][50]: x-pooled rows of a tile
-  const int tid = threadIdx.x, wg_id = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+  __shared__ uint64_t raw_full[2], full[2], empty[2];
+  uint8_t *sB = smem;                    // 66 chunks x 112 rows x 16 B
+  uint8_t *sPl = sB + C2_B_BYTES;        // 2 plane stages
+  // the x-pooled stages of the two consumers follow the planes: the unused GEMM rows 112..127 of the last plane read up to
+  // 192 B past the plane stages, and those bytes must exist (the values only reach discarded rows)
+  float *stg = reinterpret_cast<float *>(sPl + 2 * C2_STAGE);
+  float *raw = stg + 2 * C2_STG_FLOATS;  // 2 x [224 px][20] float32
+  const int tid = threadIdx.x, wg_id = tid >> 7, wt = tid & 127, warp = wt >> 5, lane = tid & 31, q = lane & 3;
 
-  for (int i = tid; i < (2 * C2_NMMA) * C2_BCHUNK / 16; i += C2_NT) reinterpret_cast<uint4 *>(sB)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
-  for (int i = tid; i < 2 * 6 * C2_PLANE / 16; i += C2_NT) reinterpret_cast<uint4 *>(sPl)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < C2_B_BYTES / 16; i += C2_NT) reinterpret_cast<uint4 *>(sB)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
+  // the 8-pixel tail of every plane is read by valid rows (as zero A elements) and never written again
+  for (int i = tid; i < 2 * 6 * 8; i += C2_NT)
+    reinterpret_cast<uint4 *>(sPl + (i >> 3) * C2_PLANE + (C2_TILE_PIX + (i & 7)) * 16)[0] = make_uint4(0, 0, 0, 0);
   if (tid < 64) sbias[tid] = tid < NF2 ? bias[tid] : 0.0f;
+  if (tid == 0) {
+    for (int s = 0; s < 2; s++) {
+      wg::mbar_init(&raw_full[s], 1);  // the expect_tx arrival + the bulk copy's bytes
+      wg::mbar_init(&full[s], 128);    // every converter thread, after its own proxy fence
+      wg::mbar_init(&empty[s], 4);     // one arrival per consumer warp
+    }
+    wg::fence_mbar_init();
+  }
+  wg::fence_async_smem();  // weights and zero tails (generic proxy) before the tensor-core reads (async proxy)
+  __syncthreads();
 
-  // (pixel, plane) items of a tile: 224 x 3; plane 2 takes channels 16..19 of the pixel and of its right neighbour
-  auto convert = [&](int im, int T, int buf) {
-    uint8_t *pl = sPl + (size_t)buf * 6 * C2_PLANE;
-    for (int i = tid; i < C2_TILE_PIX * 3; i += C2_NT) {
-      const int lp = i / 3, p = i - lp * 3;
-      const float *src = p1 + (size_t)im * 784 * NF1 + (size_t)(4 * T * C2_W + lp) * NF1 + p * 8;
-      const float4 x0 = __ldg(reinterpret_cast<const float4 *>(src));
-      float4 x1 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p < 2) x1 = __ldg(reinterpret_cast<const float4 *>(src + 4));
-      else if (lp + 1 < C2_TILE_PIX) x1 = __ldg(reinterpret_cast<const float4 *>(src + NF1));
-      const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+  // the CTA's tiles g = 0 .. G-1: image blockIdx.x + (g / 6) * gridDim.x, tile g % 6
+  const int G = C2_TILES * ((n - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x);
+  auto tile_image = [&](int g) { return (int)blockIdx.x + (g / C2_TILES) * (int)gridDim.x; };
+
+  if (wg_id == 0) {
+    // ===== converter
+    wg::setmaxnreg_dec<40>();
+    auto fetch = [&](int g) {
+      const int s = g & 1;
+      wg::mbar_expect_tx(&raw_full[s], C2_RAW_BYTES);
+      wg::bulk_g2s(raw + s * (C2_RAW_BYTES / 4),
+                   p1 + (size_t)tile_image(g) * 784 * NF1 + (size_t)(g % C2_TILES) * 4 * C2_W * NF1, C2_RAW_BYTES,
+                   &raw_full[s]);
+    };
+    if (wt == 0)
+      for (int g = 0; g < 2 && g < G; g++) fetch(g);
+    for (int g = 0; g < G; g++) {
+      const int s = g & 1;
+      const float *rs = raw + s * (C2_RAW_BYTES / 4);
+      uint8_t *pl = sPl + s * C2_STAGE;
+      wg::mbar_wait(&raw_full[s], (g >> 1) & 1);
+      wg::mbar_wait(&empty[s], ((g >> 1) & 1) ^ 1);
+      // (pixel, plane) items: 224 x 3; plane 2 takes channels 16..19 of the pixel and of its right neighbour
+      for (int i = wt; i < C2_TILE_PIX * 3; i += 128) {
+        const int lp = i / 3, p = i - lp * 3;
+        const float *src = rs + lp * NF1 + p * 8;
+        const float4 x0 = *reinterpret_cast<const float4 *>(src);
+        float4 x1 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (p < 2) x1 = *reinterpret_cast<const float4 *>(src + 4);
+        else if (lp + 1 < C2_TILE_PIX) x1 = *reinterpret_cast<const float4 *>(src + NF1);
+        const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+        __half hi[8], lo[8];
+#pragma unroll
+        for (int e = 0; e < 8; e++) {
+          float a = x[e] * a_scale;
+          hi[e] = __float2half_rn(a);
+          lo[e] = __float2half_rn(a - __half2float(hi[e]));
+        }
+        *reinterpret_cast<uint4 *>(pl + (size_t)p * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(hi);
+        *reinterpret_cast<uint4 *>(pl + (size_t)(3 + p) * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(lo);
+      }
+      wg::fence_async_smem();  // this thread's plane writes -> the tensor-core reads
+      wg::mbar_arrive(&full[s]);
+      if (g + 2 < G) {
+        wg::bar_sync(5, 128);  // every converter thread has read raw buffer s before the copy overwrites it
+        if (wt == 0) fetch(g + 2);
+      }
+    }
+    return;
+  }
+
+  // ===== consumers
+  wg::setmaxnreg_inc<232>();
+  const int c = wg_id - 1;
+  const uint32_t arow = wg::smem_u32(sPl) + (uint32_t)c * C2_STAGE, sB_u = wg::smem_u32(sB);
+  float *st = stg + c * C2_STG_FLOATS;
+  for (int g = c; g < G; g += 2) {
+    const int im = tile_image(g), T = g % C2_TILES;
+    // this consumer's batch goes after the other's previous one; the barrier also orders the previous epilogue's stage
+    // reads (all 128 threads) before this tile's stage writes
+    if (g > 0) wg::bar_sync(1 + c, 256);
+    wg::mbar_wait(&full[c], (g >> 1) & 1);
+    float d[2][56];
+    wg::fence();
+#pragma unroll
+    for (int i = 0; i < C2_NMMA; i++) {  // a_hi x [w_hi | w_lo]
+      const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
+      const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
+      const uint64_t db = wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128);
+#pragma unroll
+      for (int hh = 0; hh < 2; hh++) wg::mma_f16_n112(d[hh], wg::desc(arow + hh * 64 * 16 + a0, lbo, 128), db, i > 0);
+    }
+#pragma unroll
+    for (int i = 0; i < C2_NMMA; i++) {  // a_lo x w_hi
+      const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
+      const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
+      const uint64_t db = wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128);
+#pragma unroll
+      for (int hh = 0; hh < 2; hh++)
+        wg::mma_f16_n56(d[hh], wg::desc(arow + 3 * C2_PLANE + hh * 64 * 16 + a0, lbo, 128), db, true);
+    }
+    wg::commit();
+    if (g + 1 < G) wg::bar_arrive(2 - c, 256);  // the other consumer may issue its next batch
+    wg::wait<0>();
+    wg::reg_fence(d[0]);
+    wg::reg_fence(d[1]);
+    if (lane == 0) wg::mbar_arrive(&empty[c]);
+    // columns c and 56 + c are values i and i + 28 of the same thread; rows r, r + 1 are lanes l, l ^ 4
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int r = hh * 64 + warp * 16 + (lane >> 2) + 8 * h, rr = r >> 1;  // rr = [dy 0..3][x/2 0..13]
+        const bool wr = (r & 1) == 0 && r < 112 && (rr % 14) < 12;
+#pragma unroll
+        for (int j = 0; j < 7; j++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int i = 4 * j + 2 * h + e, ch = 8 * j + 2 * q + e;
+            float v = (d[hh][i] + d[hh][i + 28]) * out_scale;
+            v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+            if (wr && ch < NF2) st[rr * NF2 + ch] = v;
+          }
+      }
+    wg::bar_sync(3 + c, 128);
+    // the tile's 2 x 12 x 50 = 1200 consecutive k (from 1200 T) are 150 whole 8-element chunks of ip1's A operand:
+    // [tile im/128][hi|lo][k/8][row im%128][k%8] fp16, scaled by x_scale
+    __half *xrow = xc + (size_t)(im >> 7) * 2 * IP_KCH * 128 * 8 + (size_t)(im & 127) * 8;
+    for (int ci = wt; ci < 150; ci += 128) {
       __half hi[8], lo[8];
 #pragma unroll
       for (int e = 0; e < 8; e++) {
-        float a = x[e] * a_scale;
+        const int kk = 8 * ci + e, qq = kk / 600, px = (kk % 600) / NF2, ch = kk % NF2;  // kk = 600 qq + 50 px + ch
+        float m = fmaxf(st[((2 * qq) * 14 + px) * NF2 + ch], st[((2 * qq + 1) * 14 + px) * NF2 + ch]) + sbias[ch];
+        if (relu) m = fmaxf(m, 0.0f);
+        const float a = m * x_scale;
         hi[e] = __float2half_rn(a);
         lo[e] = __float2half_rn(a - __half2float(hi[e]));
       }
-      *reinterpret_cast<uint4 *>(pl + (size_t)p * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(hi);
-      *reinterpret_cast<uint4 *>(pl + (size_t)(3 + p) * C2_PLANE + (size_t)lp * 16) = *reinterpret_cast<uint4 *>(lo);
-    }
-  };
-  __syncthreads();  // the zero fill is complete before any thread converts into the planes
-  if (blockIdx.x < n) convert(blockIdx.x, 0, 0);
-  wg::fence_async_smem();
-  __syncthreads();
-
-  const uint32_t sPl_u = wg::smem_u32(sPl) + (uint32_t)wg_id * 64 * 16, sB_u = wg::smem_u32(sB);
-  int gt = 0;
-  for (int im = blockIdx.x; im < n; im += gridDim.x) {
-    float *out = p2 + (size_t)im * 7200;
-    for (int T = 0; T < C2_TILES; T++, gt++) {
-      const int b = gt & 1;
-      const uint32_t arow = sPl_u + (uint32_t)b * 6 * C2_PLANE;
-      float d[64];
-      wg::fence();
-#pragma unroll
-      for (int i = 0; i < C2_NMMA; i++) {  // a_hi x [w_hi | w_lo]
-        const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
-        const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-        wg::mma_f16_n128(d, wg::desc(arow + a0, lbo, 128), wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), i > 0);
-      }
-#pragma unroll
-      for (int i = 0; i < C2_NMMA; i++) {  // a_lo x w_hi
-        const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
-        const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-        wg::mma_f16_n64(d, wg::desc(arow + 3 * C2_PLANE + a0, lbo, 128),
-                        wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128), true);
-      }
-      wg::commit();
-      // the operands of the next tile go into the other buffer while the tensor cores work on this one (that buffer's
-      // instructions completed before the barrier that ended the previous tile)
-      const int nim = T + 1 < C2_TILES ? im : im + gridDim.x, nT = T + 1 < C2_TILES ? T + 1 : 0;
-      if (nim < n) convert(nim, nT, b ^ 1);
-      wg::wait<0>();
-      wg::reg_fence(d);
-      // columns c and 64 + c are values i and i + 32 of the same thread; rows r, r + 1 are lanes l, l ^ 4
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int r = wg_id * 64 + warp * 16 + (lane >> 2) + 8 * h, rr = r >> 1;  // rr = [dy 0..3][x/2 0..13]
-        const bool wr = (r & 1) == 0 && r < 112 && (rr % 14) < 12;
-#pragma unroll
-        for (int j = 0; j < 8; j++)
-#pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int i = 4 * j + 2 * h + e, c = 8 * j + 2 * q + e;
-            float v = (d[i] + d[i + 32]) * out_scale;
-            v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
-            if (wr && c < NF2) stg[rr * NF2 + c] = v;
-          }
-      }
-      __syncthreads();
-      for (int i = tid; i < 2 * 12 * NF2; i += C2_NT) {
-        int ch = i % NF2, px = (i / NF2) % 12, qq = i / (NF2 * 12);
-        float m = fmaxf(stg[((2 * qq) * 14 + px) * NF2 + ch], stg[((2 * qq + 1) * 14 + px) * NF2 + ch]) + sbias[ch];
-        if (relu) m = fmaxf(m, 0.0f);
-        int j = (2 * T + qq) * 12 + px;
-        if (p2) out[(size_t)j * NF2 + ch] = m;
-        if (xc) {  // ip1's A operand: [tile im/128][hi|lo][k/8][row im%128][k%8] fp16, scaled by 2^-8
-          const int k = ch + NF2 * j;
-          const float a = m * x_scale;
-          const __half hi = __float2half_rn(a);
-          const __half lo = __float2half_rn(a - __half2float(hi));
-          const size_t base = ((size_t)(im >> 7) * 2 * IP_KCH + (size_t)(k >> 3)) * 128 * 8 + (size_t)(im & 127) * 8 + (k & 7);
-          xc[base] = hi;
-          xc[base + (size_t)IP_KCH * 128 * 8] = lo;
-        }
-      }
-      wg::fence_async_smem();  // the converted planes of the next tile -> tensor-core reads
-      __syncthreads();         // ... and the stage is free again
+      __half *dst = xrow + (size_t)(150 * T + ci) * 128 * 8;
+      *reinterpret_cast<uint4 *>(dst) = *reinterpret_cast<uint4 *>(hi);
+      *reinterpret_cast<uint4 *>(dst + (size_t)IP_KCH * 128 * 8) = *reinterpret_cast<uint4 *>(lo);
     }
   }
 }
-
 
 // ---------------------------------------------------------------------------------------------------------
 // ip1: H3[n x 500] = relu(X[n x 7200] W[7200 x 500] + b) as a TMA-fed wgmma GEMM.
@@ -301,7 +358,7 @@ __global__ void __launch_bounds__(IP_NT, 1) k_ip1_tc(const __half *__restrict__ 
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t full[IP_STAGES], empty[IP_STAGES];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int mt = blockIdx.x, ob = blockIdx.y;
+  const int ob = blockIdx.x, mt = blockIdx.y;
   if (tid == 0) {
     for (int s = 0; s < IP_STAGES; s++) {
       wg::mbar_init(&full[s], 1);
@@ -420,7 +477,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
           }
     }
   }
-  // conv2 blob: [chunk c][row n: 0..63 = w_hi (50 used), 64..127 = w_lo][8 x fp16], weights scaled by 2^k
+  // conv2 blob: [chunk c][row n: 0..55 = w_hi (50 used), 56..111 = w_lo][8 x fp16], weights scaled by 2^k
   float mx = 0.0f;
   for (size_t i = 0; i < (size_t)NF2 * NF1 * 25; i++) mx = std::fmax(mx, std::fabs(w[2][i]));
   t.w2_scale = pow2_scale(mx, 16.0f);
@@ -446,7 +503,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
     return sc;
   };
   t.a2_scale = safe_scale(a1_bound, 1.0f / 16.0f);
-  std::vector<__half> b2((size_t)(2 * C2_NMMA) * 128 * 8, __float2half(0.0f));
+  std::vector<__half> b2((size_t)(2 * C2_NMMA) * C2_N * 8, __float2half(0.0f));
   for (int c = 0; c < C2_NCH; c++) {
     for (int o = 0; o < NF2; o++)
       for (int e = 0; e < 8; e++) {
@@ -460,8 +517,8 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
         float wv = w[2][(((size_t)o * NF1 + ch) * 5 + kh) * 5 + kw] * t.w2_scale;
         __half hi = __float2half_rn(wv);
         __half lo = __float2half_rn(wv - __half2float(hi));
-        b2[((size_t)c * 128 + o) * 8 + e] = hi;
-        b2[((size_t)c * 128 + 64 + o) * 8 + e] = lo;
+        b2[((size_t)c * C2_N + o) * 8 + e] = hi;
+        b2[((size_t)c * C2_N + C2_N / 2 + o) * 8 + e] = lo;
       }
   }
   // ip1 blob: [o-block 4][K-block 150][chunk 6][row 256: 0..127 w_hi(o), 128..255 w_lo(o)][8 x fp16], W(o,k) = w[4][o + 500 k]
@@ -508,7 +565,7 @@ int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, _
   const LenetTc &t = ctx->tc;
   const int relu = ctx->prm.relu_after_conv;
   size_t sm1 = (size_t)C1_B_BYTES + C1_PLANE + 2 * C1_STAGE_FLOATS * sizeof(float);
-  size_t sm2 = (size_t)(2 * C2_NMMA) * C2_BCHUNK + 2 * 6 * C2_PLANE + 56 * NF2 * sizeof(float);
+  size_t sm2 = (size_t)C2_B_BYTES + 2 * C2_STAGE + 2 * C2_STG_FLOATS * sizeof(float) + 2 * C2_RAW_BYTES;
   size_t sm3 = (size_t)IP_STAGES * IP_STAGE_BYTES;
   CUDA_TRY(cudaFuncSetAttribute(k_conv1_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
   CUDA_TRY(cudaFuncSetAttribute(k_conv2_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
@@ -519,12 +576,11 @@ int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, _
   gpdb_st_end(ctx, 5, e1);
   cudaEvent_t e2 = gpdb_st_begin(ctx);
   k_conv2_tc<<<std::min(n, ctx->sm_count), C2_NT, sm2, ctx->stream>>>(p1, n, (const uint8_t *)t.b2, ctx->w.c2b, t.a2_scale,
-                                                                       1.0f / (t.a2_scale * t.w2_scale), relu, nullptr, xc,
-                                                                       t.x3_scale);
+                                                                       1.0f / (t.a2_scale * t.w2_scale), relu, xc, t.x3_scale);
   LAUNCH_CHECK();
   gpdb_st_end(ctx, 6, e2);
   cudaEvent_t e3 = gpdb_st_begin(ctx);
-  dim3 g3((n + 127) / 128, 4);
+  dim3 g3(4, (n + 127) / 128);  // the four output blocks of an image tile run together and share its X through L2
   k_ip1_tc<<<g3, IP_NT, sm3, ctx->stream>>>(xc, n, (const uint8_t *)t.b3, ctx->w.i1b, 1.0f / (t.x3_scale * t.w3_scale), h3);
   LAUNCH_CHECK();
   gpdb_st_end(ctx, 7, e3);
