@@ -1946,6 +1946,9 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         }
       }
       for (int k = tid; k < (3 * SS) >> 1; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);
+      // odd image size: the 16-byte stores stop one cell short of tile C's end (its last pixel would keep the ball /
+      // draw list or the previous image's sums); the bitmaps follow, so no store may go further
+      if ((SS & 1) && tid == 0) tileA[3 * SS - 1] = 0ull;
       __syncthreads();
       // compact the set bits into a list (behind bitmap 0, in the dead box-list region) so that the per-voxel work
       // is spread evenly: shadow voxels are spatially clustered, a thread-per-word loop would be badly unbalanced
@@ -2122,7 +2125,8 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
 //     projection 2 (cell + fixed-point coordinate) is stashed next to the voxel code and summed in a second, cheap pass;
 //   * the quantised POINT channels are scattered straight into the image's own (still unused) 57.6 KB of HBM / L2 as twelve
 //     byte planes and read back into the dead tiles before the dilation; only the three shadow planes stay in shared memory.
-// Requires image_size 60 and at most two cameras (otherwise k_images does all the work). Results are bit-identical to
+// Requires image_size 60 and, at 15 channels, at most two cameras whose shadow bitmaps fit the box list with 2 KB to spare
+// (see geo_images; otherwise k_images does all the work). Results are bit-identical to
 // k_images (tests/test_gpu_parity.py::test_image_kernels_agree).
 // ------------------------------------------------------------------------------------------------
 constexpr int BOX_CAP2 = 1024;
@@ -2947,7 +2951,8 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
 // `d_p16`: nc images of S*S 16-byte pixels (see k_images). Fast path: k_images2 (two CTAs per SM) over every image, then
 // k_images over the images whose box list (1 024 points) overflowed, then its global-list instance over the images whose box
 // holds more than 2 048 points (up to 32 768; the overflow lists are usually empty: those launches return at once);
-// k_images alone when the geometry is outside the fast path's limits (image_size != 60, more than two cameras) or when
+// k_images alone when the geometry is outside the fast path's limits (image_size != 60; at 15 channels more than two
+// cameras, or shadow bitmaps that leave less than 2 KB of the box list: two cameras at the default image volume) or when
 // GPD_B200_IMAGES_KERNEL=1 forces it (tests compare the kernels).
 int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
   if (nc <= 0) return GPDB_OK;

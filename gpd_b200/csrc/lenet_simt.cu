@@ -283,8 +283,8 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
   if (n <= 0) return GPDB_OK;
   const int S = ctx->prm.image_size, C = ctx->prm.image_num_channels;
   const int P1 = (S - 4) / 2, P2 = (P1 - 4) / 2, K = NF2 * P2 * P2;
-  if (K != 7200) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "LeNet expects image_size 60 (ip1 input 7200), got %d", K);
+  if (S != 60) {  // 61..63 would also give ip1 7200 inputs, but the reference's network is built for 60 x 60
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "LeNet expects image_size 60 (ip1 input 7200), got %d (ip1 input %d)", S, K);
     return GPDB_ERR_INVALID;
   }
   const LenetWeights &w = ctx->w;

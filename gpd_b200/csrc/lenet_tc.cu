@@ -483,8 +483,10 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
   t.w2_scale = pow2_scale(mx, 16.0f);
   // Activation scales of the fp16 hi/lo split. The hi term must stay below the fp16 maximum (65504) for ANY input image:
   // bound the activations from the weights (pool1 <= max_o sum_i |w1[o,i]| * 255 + |b1[o]|, propagated through conv2 for
-  // pool2) and shrink the default power-of-two scales (tuned on the reference's three weight sets) when another model's
-  // weights need it, so that scores can never silently become inf / NaN.
+  // pool2), so that scores can never silently become inf / NaN. The scale is the LARGEST power of two that keeps
+  // scale * bound <= 60000, in both directions: a fixed scale would push the lo term of small activations (a model with
+  // small conv1 weights) into fp16 subnormals, an absolute error of ~2^-25 / scale that no longer shrinks with the
+  // activations. Scaling conv1's weights and all biases by 2^k then scales every logit by exactly 2^k.
   double a1_bound = 0.0;
   for (int o = 0; o < NF1; o++) {
     double sabs = 0.0;
@@ -497,12 +499,17 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
     for (size_t i = 0; i < (size_t)NF1 * 25; i++) sabs += std::fabs((double)w[2][(size_t)o * NF1 * 25 + i]);
     a2_bound = std::max(a2_bound, sabs * a1_bound + std::fabs((double)w[3][o]));
   }
-  auto safe_scale = [](double bound, float preferred) {
-    float sc = preferred;
-    while ((double)sc * bound > 60000.0) sc *= 0.5f;
-    return sc;
+  // The epilogue multiplies by 1 / (scale * w_scale): 2^j is also held to |j + log2 w_scale| <= 120, which keeps that
+  // factor a normal float (weights whose bound would need more are ~2^100 away from any trained net).
+  auto safe_scale = [](double bound, float w_scale) {
+    const int we = std::ilogb(w_scale), lo = std::max(-126, -120 - we), hi = std::min(127, 120 - we);
+    if (!(bound > 0.0)) return std::ldexp(1.0f, std::max(lo, std::min(hi, 0)));  // all-zero layer: any scale is exact
+    int j = (int)std::floor(std::log2(60000.0 / bound));
+    while (j > lo && std::ldexp(1.0, j) * bound > 60000.0) j--;  // log2 rounding, either way
+    while (j < hi && std::ldexp(1.0, j + 1) * bound <= 60000.0) j++;
+    return std::ldexp(1.0f, std::max(lo, std::min(hi, j)));
   };
-  t.a2_scale = safe_scale(a1_bound, 1.0f / 16.0f);
+  t.a2_scale = safe_scale(a1_bound, t.w2_scale);
   std::vector<__half> b2((size_t)(2 * C2_NMMA) * C2_N * 8, __float2half(0.0f));
   for (int c = 0; c < C2_NCH; c++) {
     for (int o = 0; o < NF2; o++)
@@ -525,7 +532,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
   mx = 0.0f;
   for (size_t i = 0; i < (size_t)NH * IP_K; i++) mx = std::fmax(mx, std::fabs(w[4][i]));
   t.w3_scale = pow2_scale(mx, 16.0f);
-  t.x3_scale = safe_scale(a2_bound, 1.0f / 256.0f);
+  t.x3_scale = safe_scale(a2_bound, t.w3_scale);
   std::vector<__half> b3((size_t)4 * IP_NKB * IP_KB_CH * 256 * 8, __float2half(0.0f));
   for (int ob = 0; ob < 4; ob++)
     for (int kc = 0; kc < IP_KCH; kc++) {

@@ -167,17 +167,25 @@ def synthetic_raw_scene(seed, n_points=300000, two_cameras=False, step=0.002, na
     return d
 
 
-def synthetic_table_scene(seed, n_points=300000, two_cameras=False, step=0.003, _raw=False):
+def synthetic_table_scene(seed, n_points=300000, two_cameras=False, step=0.003, _raw=False, cameras=None,
+                          mark_all_cameras=False):
     """Config 3/4/5 cloud: a table plane at z ~ 0.9 m in front of a camera at the origin looking
     along +z, 30-60 boxes / cylinders / spheres (5-25 cm) resting on it, surfaces on a 3 mm
     lattice with sigma = 0.5 mm noise, hidden-surface culled per camera, voxelised at 0.003 and
     cut to exactly n_points. Normals are the analytic surface normals perturbed by ~3 degrees of
     noise (stand-in for PCA r=0.03), flipped towards the seeing camera, stored as float32 values.
+
+    `cameras` ([K, 3] positions, looking along +z from z < 0.9) replaces the default camera set (the origin, plus
+    (0.6, 0, 0) with `two_cameras`). cam_source marks the first camera that sees a point, or every camera that sees
+    it with `mark_all_cameras`; normals are flipped towards the first one either way.
     """
     rng = np.random.default_rng(seed)
     scale = (n_points / 300000.0) ** 0.5
     tx, ty, tz = 2.0 * scale, 1.5 * scale, 0.9
-    cams = [np.zeros(3)] + ([np.array([0.6, 0.0, 0.0])] if two_cameras else [])
+    if cameras is None:
+        cams = [np.zeros(3)] + ([np.array([0.6, 0.0, 0.0])] if two_cameras else [])
+    else:
+        cams = [np.asarray(c, dtype=np.float64).reshape(3) for c in cameras]
     table = _lattice_rect(np.array([-tx / 2, -ty / 2, tz]), np.array([1.0, 0, 0]), np.array([0, 1.0, 0]), tx, ty, step)
     P, Nn = [table], [np.tile([0.0, 0.0, -1.0], (len(table), 1))]
     n_obj = int(rng.integers(30, 61) * scale * scale) + 1
@@ -202,6 +210,8 @@ def synthetic_table_scene(seed, n_points=300000, two_cameras=False, step=0.003, 
         firstcam = np.argmax(seen, axis=1)
         cam_source = np.zeros((len(pts), len(cams)), np.int32)
         cam_source[np.arange(len(pts)), firstcam] = 1
+        if mark_all_cameras:
+            cam_source = seen.astype(np.int32)
         return {"xyz": np.ascontiguousarray(pts.astype(np.float32)), "cam_source": cam_source,
                 "view_points": np.array(cams, dtype=np.float64)}
     xyz, first = voxelize(pts.astype(np.float32), step)
@@ -215,6 +225,8 @@ def synthetic_table_scene(seed, n_points=300000, two_cameras=False, step=0.003, 
     firstcam = np.argmax(seen, axis=1)
     cam_source = np.zeros((n_points, len(cams)), np.int32)
     cam_source[np.arange(n_points), firstcam] = 1
+    if mark_all_cameras:
+        cam_source = seen.astype(np.int32)
     vp = np.array(cams, dtype=np.float64)
     to_cam = vp[firstcam] - xyz.astype(np.float64)
     flip = (to_cam * nrm).sum(1) < 0

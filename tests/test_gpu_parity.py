@@ -470,16 +470,19 @@ def test_result_arena_is_reused_and_outlives_the_context():
 def test_image_kernels_agree(ch, two_cams, monkeypatch):
     """The two image kernels — k_images2 (fast path: two CTAs per SM, 1024-point box list, two-pass shadow sums, point
     planes parked in the image's own memory) and k_images (general tier, also the overflow tier of the fast path) — must
-    produce bit-identical images; both are compared with the oracle elsewhere."""
+    produce bit-identical images; both are compared with the oracle elsewhere. The fast path must actually have run: it
+    launches one kernel more per image batch (one batch here) than the general tier alone. Two cameras' 15-channel shadow
+    bitmaps fit k_images2 only at an image depth below the default 0.06 (DESIGN §4)."""
     s = scenes.synthetic_table_scene(5 if two_cams else 7, n_points=60000, two_cameras=two_cams)
-    p, ctx, oc, w = make(s, ch)
-    poses = ctx.hand_search(scenes.sample_indices(3, 60000, 1500))["candidates"]
-    assert len(poses) > 300
+    p, ctx, oc, w = make(s, ch, keep_images=1, **({"volume_depth": 0.05} if ch == 15 and two_cams else {}))
+    sidx = scenes.sample_indices(3, 60000, 1500)
     monkeypatch.setenv("GPD_B200_IMAGES_KERNEL", "1")
-    general = ctx.images(poses)
+    general = ctx.detect(sidx)
     monkeypatch.delenv("GPD_B200_IMAGES_KERNEL")
-    fast = ctx.images(poses)
-    assert np.array_equal(general, fast)
+    fast = ctx.detect(sidx)
+    assert general["n_candidates"] > 300
+    assert fast["kernel_launches"] == general["kernel_launches"] + 1
+    assert np.array_equal(general["images"], fast["images"])
     ctx.close()
 
 
