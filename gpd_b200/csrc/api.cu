@@ -438,7 +438,8 @@ int gpdb_install_device_cloud(gpdb_ctx *ctx, int N, int K, const double *view_po
   float lo[3], hi[3];
   int *d_bounds = (int *)gpdb_scratch(ctx, 4, sizeof(double) * 6 + sizeof(int) * 8);
   if (!d_bounds) return GPDB_ERR_CUDA;
-  int rc = pre_bounds(ctx, ctx->d_xyz, N, d_bounds, lo, hi);
+  int rc = pre_nonunit(ctx);  // before the grid build, which uploads ctx->hp
+  if (rc == GPDB_OK) rc = pre_bounds(ctx, ctx->d_xyz, N, d_bounds, lo, hi);
   if (rc == GPDB_OK) rc = geo_build_grid(ctx, lo, hi, N);
   if (rc != GPDB_OK) return rc;
   ctx->cloud_set = true;
@@ -517,13 +518,24 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
   cudaEvent_t ev[6];
   for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
   auto drop_events = [&]() { for (auto &e : ev) cudaEventDestroy(e); };
-  // ---- upload the raw cloud (camera source packed to one bit per camera, as gpdb_set_cloud does)
+  // ---- upload the raw cloud (camera source packed to one bit per camera). A camera sees a point when its entry is
+  // exactly 1: the reference's voxelisation keeps only those entries (cloud.cpp:327) and its normal estimation and
+  // reverseNormals test == 1 (cloud.cpp:581,611). Without voxelisation the reference keeps the raw values, which its
+  // normals read as == 1 and the grasp path as >= 1; one bit cannot hold both, so other values are rejected there.
   std::vector<uint8_t> cam((size_t)M, (uint8_t)((1u << K) - 1));
   if (cam_source)
     for (int i = 0; i < M; i++) {
       uint8_t m = 0;
-      for (int k = 0; k < K; k++)
-        if (cam_source[(size_t)i * K + k] > 0) m |= (uint8_t)(1u << k);
+      for (int k = 0; k < K; k++) {
+        const int32_t v = cam_source[(size_t)i * K + k];
+        if (!pp->voxelize && v != 0 && v != 1) {
+          gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess: cam_source[%d][%d] = %d; without voxelisation entries "
+                         "must be 0 or 1", i, k, (int)v);
+          drop_events();
+          return GPDB_ERR_INVALID;
+        }
+        if (v == 1) m |= (uint8_t)(1u << k);
+      }
       cam[i] = m;
     }
   const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
@@ -571,6 +583,10 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
     rc = pre_normals(ctx, pp->normals_radius);
     if (rc != GPDB_OK) { drop_events(); return rc; }
   }
+  // zero normals (points no camera sees) and voxel averages of supplied normals are not of unit length
+  rc = pre_nonunit(ctx);
+  if (rc != GPDB_OK) { drop_events(); return rc; }
+  CUDA_TRY(cudaMemcpyAsync(ctx->dp, &ctx->hp, sizeof(DevParams), cudaMemcpyHostToDevice, ctx->stream));
   cudaEventRecord(ev[5], ctx->stream);
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   float t;

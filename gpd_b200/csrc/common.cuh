@@ -60,10 +60,21 @@ struct DevParams {
   // cloud
   int N, K;
   int all_seen;                // every point is seen by every camera (cam mask complete): the per-point masks need not be read
+  int nonunit;                 // some normal is not of unit length (unit_normal): images holding one fold their cells exactly
   double vp[GPDB_MAX_CAMERAS][3];
   // LeNet
   int relu_after_conv;
 };
+
+// A normal of unit length up to float32 rounding. createNormalsImage folds every point of a grasp-image cell into the
+// cell as v += (|n| - v) / ||v|| (image_strategy.cpp:136-141); while every normal has unit length the result is the last
+// writer's |n|, which is what the image kernels store. A zero normal (a point no camera sees) or a voxel average of
+// supplied normals is not of unit length, and neither is a NaN normal (the fold keeps a cell NaN once a NaN writer
+// reached it); images holding one replay the fold exactly.
+__host__ __device__ __forceinline__ bool unit_normal(const double *n) {
+  const double l2 = n[0] * n[0] + n[1] * n[1] + n[2] * n[2];
+  return fabs(l2 - 1.0) <= 1e-5;
+}
 
 struct DevCloud {
   const float4 *pts4;
@@ -205,6 +216,7 @@ int pre_bounds(gpdb_ctx *ctx, const float *d_xyz, int n, int *d_bounds, float lo
 int pre_filter_voxelize(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_cam_raw, const double *d_nrm_raw, int M,
                         const gpdb_preprocess_params &pp, int *n_out, cudaEvent_t ev_filter_done);
 int pre_normals(gpdb_ctx *ctx, double radius);
+int pre_nonunit(gpdb_ctx *ctx);
 int pre_cam_expand(gpdb_ctx *ctx, int *d_out);
 
 // lenet_simt.cu

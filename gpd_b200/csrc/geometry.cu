@@ -1496,6 +1496,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
     double *rcp = &sm.red[0][0];  // the scan's reduction scratch is idle from here to the next image: reciprocal table (cell_mean)
     if (tid < RCP_N) rcp[tid] = 1.0 / ((double)tid * 4294967296.0);  // visible after the barrier that ends the box-point pass
     // dense pass over the box points: hand-frame coordinates -> unit cube, cell indices, |R^T n| (all lanes busy)
+    bool nonunit = false;
     for (int k = tid; k < bn; k += NT_IMG) {
       const double px = (double)__uint_as_float(bq[k]), py = (double)__uint_as_float(bq[BC + k]),
                    pz = (double)__uint_as_float(bq[2 * BC + k]);
@@ -1515,8 +1516,10 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
       bnrm[k] = (float)fabs(n0);
       bnrm[BC + k] = (float)fabs(n1);
       bnrm[2 * BC + k] = (float)fabs(n2);
+      if (!unit_normal(nn)) nonunit = true;
     }
-    __syncthreads();
+    // a normal of other than unit length in the box: the cells replay createNormalsImage's fold (unit_normal, common.cuh)
+    const bool exact_fold = __syncthreads_or(nonunit) != 0;
 
     // ---- points phase: per projection rasterise normals (arg-max key = last writer in (dist, index)
     // order, createNormalsImage :124-143) and depth (per-cell mean, createDepthImage :158-176)
@@ -1544,6 +1547,46 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         n0 = bnrm[k];
         n1 = bnrm[BC + k];
         n2 = bnrm[2 * BC + k];
+        if (exact_fold) {
+          // replay the cell's writers in ascending key ((dist, index)) order, ending with this winner: v = |n| into an
+          // empty cell, else v += (|n| - v) * (1 / sqrt(v.v)) in the oracle's float / double steps. O(writers x bn), only
+          // for images that hold a normal of other than unit length.
+          float v0 = 0.0f, v1 = 0.0f, v2 = 0.0f;
+          unsigned long long cur = 0ull;
+          bool first = true;
+          for (;;) {
+            unsigned long long nxt = ~0ull;
+            int jn = k;
+            for (int j = 0; j < bn; j++) {
+              const unsigned cj = bcell[j];
+              const unsigned long long kj = bkeys[j];
+              if ((S - 1 - (int)((cj >> (8 * a0)) & 255)) * S + (int)((cj >> (8 * a1)) & 255) == pix && (first || kj > cur) &&
+                  kj < nxt) {
+                nxt = kj;
+                jn = j;
+              }
+            }
+            const float b0 = bnrm[jn], b1 = bnrm[BC + jn], b2 = bnrm[2 * BC + jn];
+            if (v0 == 0.0f && v1 == 0.0f && v2 == 0.0f) {
+              v0 = b0;
+              v1 = b1;
+              v2 = b2;
+            } else {
+              const double f = 1.0 / (double)sqrtf(v0 * v0 + v1 * v1 + v2 * v2);
+              const float d0 = (float)((double)(b0 - v0) * f), d1 = (float)((double)(b1 - v1) * f),
+                          d2 = (float)((double)(b2 - v2) * f);
+              v0 += d0;
+              v1 += d1;
+              v2 += d2;
+            }
+            if (jn == k) break;
+            cur = nxt;
+            first = false;
+          }
+          n0 = v0;
+          n1 = v1;
+          n2 = v2;
+        }
         const float avg = (float)cell_mean(tileB[pix], rcp);
         dv = (float)(1.0 - (double)avg);
         return true;
@@ -2140,6 +2183,7 @@ struct Img2Smem {
   unsigned occf[MAXPIX / 32 + 2];
   unsigned lcgA[GPDB_MAX_NSP], lcgC[GPDB_MAX_NSP];
   int cam_or, n_img, box_n, wl_n, dl_n, st_n;
+  int nonunit;  // a box point has a normal of other than unit length: the image is redone by k_images (exact fold)
   int bm_org[3], bm_dims[3];
   float fred[NT_IMG / 32][8];
 };
@@ -2186,6 +2230,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       sm.cam_or = 0;
       sm.n_img = 0;
       sm.box_n = 0;
+      sm.nonunit = 0;
     }
     uint8_t *gimg = p16 + (size_t)b * SS * 16;  // the image's own memory: first the point planes, finally the pixels
     for (int k = tid; k < (npp * PLB) >> 4; k += NT_IMG) reinterpret_cast<uint4 *>(gimg)[k] = make_uint4(0, 0, 0, 0);
@@ -2218,6 +2263,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           if (in_image_box(P, h, x, y, z)) {
             inb = true;
             key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)idx;
+            if (P.nonunit && !unit_normal(cl.nrm + 3 * (size_t)idx)) sm.nonunit = 1;
           }
         }
       }
@@ -2264,11 +2310,11 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       sm.center[0] = a0 / nn;
       sm.center[1] = a1 / nn;
       sm.center[2] = a2 / nn;
-      if (sm.box_n > BOX_CAP2) ovf[atomicAdd(ovf_count, 1)] = b;  // redone by k_images (larger list)
+      if (sm.box_n > BOX_CAP2 || sm.nonunit) ovf[atomicAdd(ovf_count, 1)] = b;  // redone by k_images (larger list / exact fold)
     }
     __syncthreads();
     PHASE(2);
-    if (sm.box_n > BOX_CAP2) continue;  // uniform
+    if (sm.box_n > BOX_CAP2 || sm.nonunit) continue;  // uniform
     const int bn = sm.box_n;
     double *rcp = &sm.red[0][0];  // the scan's reduction scratch is idle from here to the next image: reciprocal table (cell_mean)
     if (tid < RCP_N) rcp[tid] = 1.0 / ((double)tid * 4294967296.0);  // visible after the barrier that ends the box-point pass

@@ -450,6 +450,12 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
   out[2] = nd[2];
 }
 
+// any normal of the cloud not of unit length (unit_normal, common.cuh) -> *flag = 1
+__global__ void k_nonunit(const double *nrm, int N, int *flag) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N && !unit_normal(nrm + 3 * (size_t)i)) *flag = 1;
+}
+
 __global__ void k_cam_expand(const uint8_t *cam, int N, int K, int *out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -526,8 +532,8 @@ int pre_normals(gpdb_ctx *ctx, double radius) {
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (e4) {
       CUDA_TRY(cudaMemsetAsync(ctx->d_err + 4, 0, sizeof(int), ctx->stream));
-      gpdb_set_error(ctx, GPDB_ERR_CAPACITY, "normal estimation: %d points have more than %d neighbours within normals_radius",
-                     e4, NRM_CAP2);
+      gpdb_set_error(ctx, GPDB_ERR_CAPACITY, "normal estimation: %d points have more than %d neighbours within normals_radius %g",
+                     e4, NRM_CAP2, radius);
       return GPDB_ERR_CAPACITY;
     }
   }
@@ -630,6 +636,22 @@ int pre_filter_voxelize(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_
     tr.mark("reserve + emit");
   }
   *n_out = U;
+  return GPDB_OK;
+}
+
+// ctx->hp.nonunit of the installed cloud (ctx->d_nrm, ctx->N points); the caller uploads ctx->hp
+int pre_nonunit(gpdb_ctx *ctx) {
+  // the spare last int of slot 4 (workspace bounds, grid bounds, voxel error), idle between the synchronous steps
+  int *flag = (int *)gpdb_scratch(ctx, 4, sizeof(double) * 6 + sizeof(int) * 8);
+  if (!flag) return GPDB_ERR_CUDA;
+  flag = (int *)((double *)flag + 6) + 7;
+  CUDA_TRY(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+  k_nonunit<<<(ctx->N + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_nrm, ctx->N, flag);
+  LAUNCH_CHECK();
+  int h = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  ctx->hp.nonunit = h;
   return GPDB_OK;
 }
 

@@ -269,6 +269,12 @@ void gpdb_preprocess_params_default(gpdb_preprocess_params *p);
  * on the device, and installs the processed cloud in the context exactly as gpdb_set_cloud would (the neighbour
  * grid is built from the device copy). Inputs as gpdb_set_cloud (raw cloud, n_points may be millions); `normals`
  * may be NULL when estimate_normals = 1. Returns the number of processed points N' (>= 0) or a negative error.
+ * A camera sees a point when its cam_source entry is exactly 1, as in the reference's voxelisation and normal
+ * estimation (cloud.cpp:327,581,611); with voxelize = 0 any entry other than 0 or 1 is GPDB_ERR_INVALID (the
+ * reference would keep it raw and read it as == 1 for the normals but >= 1 in the grasp path). More than 8 192
+ * neighbours within normals_radius at one point is GPDB_ERR_CAPACITY; a voxel index of 2^21 or more on any axis
+ * (cloud extent / voxel_size) is GPDB_ERR_INVALID. After either error, or a rejected cam_source, the context holds
+ * no cloud until the next successful gpdb_set_cloud / gpdb_preprocess.
  * Not covered: refine_normals_k, remove_outliers, sample_above_plane (PCL filters outside the default cfg) and
  * Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect).
  * Semantics that differ from the reference by specification (DESIGN.md "preprocessing"): the voxel set is an

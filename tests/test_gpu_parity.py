@@ -26,9 +26,11 @@ def make(cloud, ch, **over):
     return p, ctx, oc, oracle.WeightPack(w)
 
 
-def assert_parity(ro, rg, ch):
+def assert_parity(ro, rg, ch, equal_nan=False):
+    """equal_nan: frames may be NaN (clouds with NaN normals), at the same entries on both sides."""
     assert np.array_equal(ro["frame_valid"], rg["frame_valid"])
-    assert np.allclose(ro["frames"], rg["frames"], atol=1e-9, rtol=0)
+    assert np.array_equal(np.isnan(ro["frames"]), np.isnan(rg["frames"]))
+    assert np.allclose(ro["frames"], rg["frames"], atol=1e-9, rtol=0, equal_nan=equal_nan)
     assert np.array_equal(ro["pose_flags"], rg["pose_flags"])
     assert ro["n_candidates"] == rg["n_candidates"]
     co, cg = ro["candidates"], rg["candidates"]
