@@ -338,6 +338,15 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->d_samples);
   cudaFree(ctx->d_sel);
   cudaFree(ctx->d_cell_start);
+  cudaFree(ctx->d_bpts4);
+  cudaFree(ctx->d_bxyz);
+  cudaFree(ctx->d_bnrm);
+  cudaFree(ctx->d_bcam);
+  cudaFree(ctx->d_bcell_start);
+  cudaFree(ctx->d_bdesc);
+  cudaFree(ctx->d_bsoff);
+  free(ctx->b_off);
+  free(ctx->b_sel);
   float *w[8] = {ctx->w.c1w, ctx->w.c1b, ctx->w.c2w, ctx->w.c2b, ctx->w.i1w, ctx->w.i1b, ctx->w.i2w, ctx->w.i2b};
   for (float *p : w) cudaFree(p);
   cudaFree(ctx->tc.b1);
@@ -601,6 +610,11 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
 
 int gpdb_set_samples(gpdb_ctx *ctx, const double *samples, int32_t n) {
   if (!ctx || n < 0 || (n > 0 && !samples)) return GPDB_ERR_INVALID;
+  if (!ctx->cloud_set && ctx->b_n > 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_samples: sample positions address the single cloud; a batch of clouds "
+                   "(gpdb_set_clouds) takes cloud-local point indices only");
+    return GPDB_ERR_INVALID;
+  }
   if (!ctx->cloud_set) {
     gpdb_set_error(ctx, GPDB_ERR_STATE, "no point cloud: call gpdb_set_cloud / gpdb_preprocess first");
     return GPDB_ERR_STATE;
@@ -825,7 +839,7 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_
   const size_t psz = (size_t)S * S * 16;   // one image in the device layout (16-byte pixels, see k_images)
   out->n_samples = n;
   out->poses_per_sample = P;
-  if (!resident)
+  if (!resident && !ctx->run.n)
     for (int i = 0; i < n; i++)
       if (sample_idx[i] < 0 || sample_idx[i] >= ctx->N + ctx->n_samples) {
         gpdb_set_error(ctx, GPDB_ERR_INVALID, "sample index %d at position %d outside the cloud (N = %d, + %d sample positions)",
@@ -1031,7 +1045,20 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_
     }
   }
   int n_sel = 0;
-  if (selecting) {
+  if (selecting && ctx->run.n) {  // a batch: the top select_k of every cloud
+    gpdb_pose *d_top = nullptr;
+    rc = geo_select_batch(ctx, ctx->d_sel, total_nc, select_k, ctx->b_sel, &d_top);
+    if (rc < 0) return finish(rc);
+    n_sel = rc;
+    if (n_sel > 0) {
+      PIPE_CUDA(cudaStreamSynchronize(ps.copy));
+      if (!arena_reserve(ar, 1, sizeof(gpdb_pose) * (size_t)n_sel, 0)) {
+        gpdb_set_error(ctx, GPDB_ERR_CUDA, "cudaHostAlloc of the candidate arena failed");
+        return finish(GPDB_ERR_CUDA);
+      }
+      PIPE_CUDA(cudaMemcpyAsync(ar->buf[1], d_top, sizeof(gpdb_pose) * (size_t)n_sel, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+  } else if (selecting) {
     n_sel = std::min(select_k, total_nc);
     if (n_sel > 0) {
       gpdb_pose *d_top = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)std::max(n_sel, cmax * P));
@@ -1102,6 +1129,203 @@ int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n, 
     return GPDB_ERR_INVALID;
   }
   return run_pipeline(ctx, d_sample_idx, n, stats, true, true, d_flags_out, d_scores_out);
+}
+
+int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
+                    const int32_t *cam_source, const int32_t *n_cameras, const double *view_points) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  ctx->b_n = 0;  // a failed call leaves no batch behind; the single cloud is untouched either way
+  if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !normals || !view_points || point_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, "
+                   "normals, view_points");
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < n_clouds; b++) {
+    if (point_offsets[b + 1] <= point_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: cloud %d has %d points (offsets must increase)", b,
+                     point_offsets[b + 1] - point_offsets[b]);
+      return GPDB_ERR_INVALID;
+    }
+    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: cloud %d has %d cameras (1 <= cameras <= %d)", b, n_cameras[b],
+                     GPDB_MAX_CAMERAS);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  const int N = point_offsets[n_clouds];
+  for (size_t i = 0; i < 3 * (size_t)N; i++)
+    if (!std::isfinite(xyz[i])) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: point %zu has a non-finite coordinate (run removeNans / "
+                     "gpdb_preprocess first)", i / 3);
+      return GPDB_ERR_INVALID;
+    }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  // host side: camera masks (a camera sees a point when its entry is > 0, as gpdb_set_cloud) and the descriptors' cloud fields
+  std::vector<uint8_t> cam((size_t)N);
+  std::vector<CloudDesc> desc((size_t)n_clouds);
+  size_t cs = 0, vs = 0;  // running offsets into cam_source (N_b x K_b blocks) and view_points (3 x K_b blocks)
+  int maxk = 0;
+  for (int b = 0; b < n_clouds; b++) {
+    CloudDesc &D = desc[b];
+    memset(&D, 0, sizeof(D));
+    D.off = point_offsets[b];
+    D.N = point_offsets[b + 1] - D.off;
+    D.K = n_cameras[b];
+    maxk = std::max(maxk, D.K);
+    for (int k = 0; k < D.K; k++)
+      for (int r = 0; r < 3; r++) D.vp[k][r] = view_points[vs + 3 * k + r];
+    vs += 3 * (size_t)D.K;
+    const uint8_t all = (uint8_t)((1u << D.K) - 1);
+    bool all_seen = true;
+    for (int i = 0; i < D.N; i++) {
+      uint8_t m = all;
+      if (cam_source) {
+        m = 0;
+        for (int k = 0; k < D.K; k++)
+          if (cam_source[cs + (size_t)i * D.K + k] > 0) m |= (uint8_t)(1u << k);
+      }
+      cam[(size_t)D.off + i] = m;
+      all_seen = all_seen && m == all;
+    }
+    cs += (size_t)D.N * D.K;
+    D.all_seen = all_seen ? 1 : 0;
+  }
+  // grow-only arenas
+  if ((size_t)N > ctx->bcloud_cap) {
+    cudaFree(ctx->d_bpts4); ctx->d_bpts4 = nullptr;
+    cudaFree(ctx->d_bxyz); ctx->d_bxyz = nullptr;
+    cudaFree(ctx->d_bnrm); ctx->d_bnrm = nullptr;
+    cudaFree(ctx->d_bcam); ctx->d_bcam = nullptr;
+    ctx->bcloud_cap = 0;
+    const size_t cap = (size_t)N + N / 8 + 1024;
+    CUDA_TRY(cudaMalloc(&ctx->d_bpts4, sizeof(float4) * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bxyz, sizeof(float) * 3 * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bnrm, sizeof(double) * 3 * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bcam, cap));
+    ctx->bcloud_cap = cap;
+  }
+  if ((size_t)n_clouds + 1 > ctx->bdesc_cap) {
+    cudaFree(ctx->d_bdesc); ctx->d_bdesc = nullptr;
+    cudaFree(ctx->d_bsoff); ctx->d_bsoff = nullptr;
+    free(ctx->b_off); ctx->b_off = nullptr;
+    free(ctx->b_sel); ctx->b_sel = nullptr;
+    ctx->bdesc_cap = 0;
+    const size_t cap = (size_t)n_clouds + 1 + n_clouds / 4;
+    CUDA_TRY(cudaMalloc(&ctx->d_bdesc, sizeof(CloudDesc) * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bsoff, sizeof(int) * cap));
+    ctx->b_off = (int *)malloc(sizeof(int) * cap);
+    ctx->b_sel = (int *)malloc(sizeof(int) * cap);
+    if (!ctx->b_off || !ctx->b_sel) {
+      gpdb_set_error(ctx, GPDB_ERR_CUDA, "gpdb_set_clouds: host allocation failed");
+      return GPDB_ERR_CUDA;
+    }
+    ctx->bdesc_cap = cap;
+  }
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bxyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bnrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bcam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bdesc, desc.data(), sizeof(CloudDesc) * (size_t)n_clouds, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->bcloud.pts4 = ctx->d_bpts4;
+  ctx->bcloud.xyz = ctx->d_bxyz;
+  ctx->bcloud.nrm = ctx->d_bnrm;
+  ctx->bcloud.cam = ctx->d_bcam;
+  ctx->bcloud.samples = nullptr;
+  ctx->bcloud.n_points = N;
+  ctx->b_n = n_clouds;
+  int rc = geo_build_grid_batch(ctx, N);
+  if (rc != GPDB_OK) {
+    ctx->b_n = 0;
+    return rc;
+  }
+  memcpy(ctx->b_off, point_offsets, sizeof(int) * ((size_t)n_clouds + 1));
+  ctx->b_maxk = maxk;
+  return n_clouds;
+}
+
+}  // extern "C"
+
+namespace {
+
+// gpdb_detect_batch / gpdb_detect_batch_select: checks the CSR sample lists against the installed batch and runs them as
+// ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back with cloud-local
+// sample slots, grouped by cloud (offsets_out).
+int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out, int32_t *offsets_out,
+              int select_k, const char *name) {
+  int rc = gpdb_check_state(ctx, false, true);
+  if (rc != GPDB_OK) return rc;
+  if (ctx->b_n == 0) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds first", name);
+    return GPDB_ERR_STATE;
+  }
+  const int B = ctx->b_n;
+  if (!out || !sample_offsets || sample_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need out and sample_offsets[%d] starting at 0", name, B + 1);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++)
+    if (sample_offsets[b + 1] < sample_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample_offsets decrease at cloud %d", name, b);
+      return GPDB_ERR_INVALID;
+    }
+  const int n = sample_offsets[B];
+  if (n > 0 && !sample_idx) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null sample_idx", name);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++) {
+    const int nb = ctx->b_off[b + 1] - ctx->b_off[b];
+    for (int i = sample_offsets[b]; i < sample_offsets[b + 1]; i++)
+      if (sample_idx[i] < 0 || sample_idx[i] >= nb) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d)", name, sample_idx[i],
+                       i, b, nb);
+        return GPDB_ERR_INVALID;
+      }
+  }
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bsoff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  ctx->run = CloudTable{ctx->d_bdesc, ctx->d_bsoff, B};
+  rc = gpdb_run_pipeline(ctx, sample_idx, n, out, true, false, nullptr, nullptr, select_k, 0);
+  ctx->run = CloudTable{nullptr, nullptr, 0};
+  if (rc < 0) return rc;
+  // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
+  if (select_k >= 0) {
+    for (int b = 0; b < B; b++) {
+      offsets_out[b] = ctx->b_sel[b];
+      for (int j = ctx->b_sel[b]; j < ctx->b_sel[b + 1]; j++) out->candidates[j].sample_slot -= sample_offsets[b];
+    }
+    offsets_out[B] = ctx->b_sel[B];
+  } else {
+    int b = 0;
+    offsets_out[0] = 0;
+    for (int j = 0; j < out->n_candidates; j++) {
+      while (out->candidates[j].sample_slot >= sample_offsets[b + 1]) offsets_out[++b] = j;
+      out->candidates[j].sample_slot -= sample_offsets[b];
+    }
+    while (b < B) offsets_out[++b] = out->n_candidates;
+  }
+  return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gpdb_detect_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out,
+                      int32_t *cand_offsets_out) {
+  if (ctx && !cand_offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch: null cand_offsets_out");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, sample_idx, out, cand_offsets_out, -1, "gpdb_detect_batch");
+}
+
+int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, int32_t num_selected,
+                             gpdb_result *out, int32_t *sel_offsets_out) {
+  if (ctx && (!sel_offsets_out || num_selected < 0)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch_select: need sel_offsets_out and num_selected >= 0");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, sample_idx, out, sel_offsets_out, num_selected, "gpdb_detect_batch_select");
 }
 
 int gpdb_set_overlap(gpdb_ctx *ctx, int32_t enable) {

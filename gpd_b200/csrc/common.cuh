@@ -87,6 +87,25 @@ struct DevCloud {
   int n_points;
 };
 
+// One cloud of a batch (gpdb_set_clouds): the fields of DevParams that are per cloud, under the same names, so that the
+// grid helpers (grid.cuh) and the kernels read either. The clouds' arrays are concatenated; pts4 is sorted by
+// (cloud, cell) and its w bits hold the CLOUD-LOCAL index, so keys, shadow seeds and pose records match a single-cloud run.
+struct CloudDesc {
+  float lo[3], inv_cell;
+  int dim[3];
+  int cell_base;              // first entry of this cloud's cells in the batch's cell_start
+  int off, N, K;              // first point in the concatenated arrays, points, cameras
+  int all_seen, nonunit;
+  double vp[GPDB_MAX_CAMERAS][3];
+};
+// The clouds of the current batch call: d[n] descriptors, soff[n+1] the CSR offsets of the call's samples per cloud
+// (a sample's position in the call = its sample slot). n == 0: the single cloud of the context.
+struct CloudTable {
+  const CloudDesc *d;
+  const int *soff;
+  int n;
+};
+
 // device error counters: [0] LRF capacity, [1] hand-search capacity (final tier), [2] image box list,
 // [3] hand-search tier-1 overflow count (informational), [4] normal-estimation capacity (final tier)
 #define GPDB_NERR 8
@@ -165,6 +184,20 @@ struct gpdb_ctx {
   int *d_src;         // raw index of each processed point (valid after gpdb_preprocess: has_src)
   bool has_src;
   cudaEvent_t ev[8];
+  // batch of clouds (gpdb_set_clouds), held beside the single cloud; grow-only arenas as the cloud arrays
+  DevCloud bcloud;    // the concatenated arrays (xyz / nrm / cam by concatenated index, pts4 sorted by (cloud, cell))
+  float4 *d_bpts4;
+  float *d_bxyz;
+  double *d_bnrm;
+  uint8_t *d_bcam;
+  int *d_bcell_start;
+  CloudDesc *d_bdesc;
+  int *d_bsoff;       // [B+1] sample offsets of the running batch call
+  size_t bcloud_cap, bcell_cap, bdesc_cap;
+  int b_n, b_maxk;    // clouds installed (0: none), largest camera count
+  int *b_off;         // host copy of the point offsets [b_n + 1]
+  int *b_sel;         // host: per-cloud offsets of the last batch selection [b_n + 1]
+  CloudTable run;     // n > 0 while a batch call runs: the geometry launchers use the batch instantiations
 };
 
 void gpdb_set_error(gpdb_ctx *ctx, int code, const char *fmt, ...);
@@ -188,6 +221,11 @@ int gpdb_install_device_cloud(gpdb_ctx *ctx, int N, int K, const double *view_po
 // geometry.cu
 // builds the neighbour grid over ctx->d_xyz (N points) whose per-axis bounds are lo / hi
 int geo_build_grid(gpdb_ctx *ctx, const float lo[3], const float hi[3], int N);
+// builds the per-cloud grids of the installed batch (N concatenated points, ctx->b_n clouds) and its descriptor table
+int geo_build_grid_batch(gpdb_ctx *ctx, int N);
+// the top k of every cloud of the running batch among the n candidate records (sample-slot order, scores filled) ->
+// *d_out (device scratch); sel_off[b_n + 1] (host) receives the per-cloud output offsets. Returns the total or an error.
+int geo_select_batch(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, int *sel_off, gpdb_pose **d_out);
 int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid);
 int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
               gpdb_pose *d_poses, uint8_t *d_flags);

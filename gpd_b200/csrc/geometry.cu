@@ -22,7 +22,9 @@
 // All float64 geometry is evaluated in the oracle's operation order; this file is compiled with
 // -fmad=false so that no multiply-add is contracted (strict '<' on doubles, SURVEY.md 9.3).
 #include <cfloat>
+#include <climits>
 #include <cstdlib>
+#include <vector>
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -75,8 +77,8 @@ struct SegScan {
   int prefix[NT + 1];
 };
 // fills seg.start/prefix for rows [row0, row0+NT) ; returns batch total. Contains __syncthreads.
-template <int NT>
-__device__ __forceinline__ int seg_batch(const DevParams &P, const int *cell_start, const SegRange &s, int row0,
+template <int NT, class G>
+__device__ __forceinline__ int seg_batch(const G &P, const int *cell_start, const SegRange &s, int row0,
                                          SegScan<NT> &seg) {
   int row = row0 + threadIdx.x, st = 0, len = 0;
   if (row < s.nrows) seg_row(P, cell_start, s, row, st, len);
@@ -93,8 +95,8 @@ __device__ __forceinline__ int seg_batch(const DevParams &P, const int *cell_sta
 // (rows are contiguous segments of the cell-sorted point array -> coalesced float4 loads, no per-candidate search).
 // body(in_range, point, position in the cell-sorted array) is called by all 32 lanes together. Contains __syncthreads:
 // call from uniform control flow.
-template <int NT, class F>
-__device__ __forceinline__ void scan_balanced(const DevParams &P, const DevCloud &cl, const SegRange &sr, SegScan<NT> &seg,
+template <int NT, class G, class F>
+__device__ __forceinline__ void scan_balanced(const G &P, const DevCloud &cl, const SegRange &sr, SegScan<NT> &seg,
                                               F &&body) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int NW = NT / 32;
@@ -317,11 +319,13 @@ __device__ void eigen3(const double *Min, double *eval, double *Q) {
 // goes to `ovf2` and tier 2, whose lists live in a per-warp slice of global memory (`gkeys`, LRF_CAP_GLOBAL keys, a
 // grid-stride loop over the list). Beyond that: err[0]. The reference has no limit (frame_estimator.cpp:6-86); a voxelised
 // cloud never leaves tier 0 (at most ~155 voxels of 3 mm in a 1 cm ball).
-__device__ __forceinline__ bool lrf_sample(const DevParams &P, const DevCloud &cl, const int *sidx, int i, unsigned long long *keys,
-                                           unsigned long long *sorted, int cap, bool last, double *frames, uint8_t *valid, int *err,
-                                           double *s_acc_w);
+template <bool BATCH>
+__device__ __forceinline__ bool lrf_sample(const DevParams &P, const DevCloud &cl, const CloudTable &tab, const int *sidx, int i,
+                                           unsigned long long *keys, unsigned long long *sorted, int cap, bool last, double *frames,
+                                           uint8_t *valid, int *err, double *s_acc_w);
 
-__global__ void __launch_bounds__(LRF_WARPS * 32) k_frames(const DevParams *Pp, DevCloud cl, const int *sidx, int n,
+template <bool BATCH>
+__global__ void __launch_bounds__(LRF_WARPS * 32) k_frames(const DevParams *Pp, DevCloud cl, CloudTable tab, const int *sidx, int n,
                                                             double *frames, uint8_t *valid, int *err, int cap, int *ovf,
                                                             int *ovf_count, int *ovf2, int *ovf2_count, unsigned long long *gkeys,
                                                             int tier) {
@@ -333,7 +337,7 @@ __global__ void __launch_bounds__(LRF_WARPS * 32) k_frames(const DevParams *Pp, 
     const int gw = blockIdx.x * LRF_WARPS + warp, nw = gridDim.x * LRF_WARPS, cnt2 = *ovf2_count;
     unsigned long long *keys = gkeys + (size_t)gw * 2 * cap;
     for (int j = gw; j < cnt2; j += nw) {
-      lrf_sample(P, cl, sidx, ovf2[j], keys, keys + cap, cap, true, frames, valid, err, s_acc[warp]);
+      lrf_sample<BATCH>(P, cl, tab, sidx, ovf2[j], keys, keys + cap, cap, true, frames, valid, err, s_acc[warp]);
       __syncwarp();
     }
     return;
@@ -347,26 +351,29 @@ __global__ void __launch_bounds__(LRF_WARPS * 32) k_frames(const DevParams *Pp, 
   }
   unsigned long long *keys = reinterpret_cast<unsigned long long *>(lrf_dyn) + (size_t)warp * cap;
   unsigned long long *sorted = reinterpret_cast<unsigned long long *>(lrf_dyn) + (size_t)(LRF_WARPS + warp) * cap;
-  if (!lrf_sample(P, cl, sidx, i, keys, sorted, cap, false, frames, valid, err, s_acc[warp]) && lane == 0) {
+  if (!lrf_sample<BATCH>(P, cl, tab, sidx, i, keys, sorted, cap, false, frames, valid, err, s_acc[warp]) && lane == 0) {
     if (tier == 0) ovf[atomicAdd(ovf_count, 1)] = i;  // re-run with the large list
     else ovf2[atomicAdd(ovf2_count, 1)] = i;          // ... with the global-memory list
   }
 }
 
 // one sample by one warp; false when the ball holds more than `cap` points and this is not the last tier (nothing written)
-__device__ __forceinline__ bool lrf_sample(const DevParams &P, const DevCloud &cl, const int *sidx, int i, unsigned long long *keys,
-                                           unsigned long long *sorted, int cap, bool last, double *frames, uint8_t *valid, int *err,
-                                           double *s_acc_w) {
+template <bool BATCH>
+__device__ __forceinline__ bool lrf_sample(const DevParams &P, const DevCloud &cl0, const CloudTable &tab, const int *sidx, int i,
+                                           unsigned long long *keys, unsigned long long *sorted, int cap, bool last, double *frames,
+                                           uint8_t *valid, int *err, double *s_acc_w) {
   const int lane = threadIdx.x & 31;
   const int si = sidx[i];
+  const auto &G = CloudSel<BATCH>::get(P, tab, i);  // geo_frames runs over the whole call: slot = i
+  const DevCloud cl = local_cloud(G, cl0);
   double sp[3];
   sample_position(cl, si, sp);
   float q[3] = {(float)sp[0], (float)sp[1], (float)sp[2]};
-  SegRange sr = seg_range(P, q, P.rf_lrf);
+  SegRange sr = seg_range(G, q, P.rf_lrf);
   int cnt = 0;
   for (int row = 0; row < sr.nrows; row++) {
     int st, len;
-    seg_row(P, cl.cell_start, sr, row, st, len);
+    seg_row(G, cl.cell_start, sr, row, st, len);
     for (int k0 = 0; k0 < len; k0 += 32) {
       int k = k0 + lane;
       bool hit = false;
@@ -495,7 +502,8 @@ struct HandsSmem {
 // tiers: in_list == nullptr: every sample, else the samples in_list[0 .. *in_count) (the overflow of the previous tier);
 // samples whose slab does not fit `cap` go to out_list (next tier) or, in the last tier (out_list == nullptr), are an error.
 // glist != nullptr: the staged neighbourhood lives in a per-CTA slice of global memory (last tier, any density up to cap).
-__global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevCloud cl, const int *sidx, int n, int slot0,
+template <bool BATCH>
+__global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevCloud cl0, CloudTable tab, const int *sidx, int n, int slot0,
                                                     const double *frames, const uint8_t *fvalid, gpdb_pose *poses,
                                                     uint8_t *flags, int cap, const int *in_list, const int *in_count,
                                                     int *out_list, int *out_count, float4 *glist, int *err) {
@@ -512,6 +520,8 @@ __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevC
   for (int w = blockIdx.x; w < work_n; w += gridDim.x) {
     const int i = in_list ? in_list[w] : w;
     const int si = sidx[i];
+    const auto &G = CloudSel<BATCH>::get(P, tab, slot0 + i);
+    const DevCloud cl = local_cloud(G, cl0);
     __syncthreads();
     if (tid == 0) {
       S.count = 0;
@@ -541,11 +551,11 @@ __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevC
     // ---- stage the neighbourhood: ball r = nn_radius_hs, kept if inside the (slightly widened)
     // height slab when every rotation axis is the curvature axis (z is then pose independent)
     float q[3] = {(float)S.sample[0], (float)S.sample[1], (float)S.sample[2]};
-    SegRange sr = seg_range(P, q, P.rf_hs);
+    SegRange sr = seg_range(G, q, P.rf_hs);
     const double hz = P.hand_height * 1.001 + 1e-9;
     unsigned long long best = ~0ull;
     int nball = 0;
-    scan_balanced<NT_HANDS>(P, cl, sr, S.seg, [&](bool in, const float4 &p, int) {
+    scan_balanced<NT_HANDS>(G, cl, sr, S.seg, [&](bool in, const float4 &p, int) {
       bool keep = false;
       if (in) {
         float d = l2_simple(q, p.x, p.y, p.z);
@@ -1331,8 +1341,8 @@ __device__ __noinline__ float dilated_min(const float *F, int S) {
 // GL = true is the last tier: the box list (and the float images of the general min path) live in a per-CTA slice of global
 // memory (`gl_base`, `gl_cap` points: L2-resident scratch) instead of shared memory, for clouds so dense that an image box
 // holds more than BOX_CAP points (the reference has no limit; image_generator.cpp:54-64).
-template <int S_T, bool GL>
-__global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCloud cl, const gpdb_pose *cand, int nc,
+template <int S_T, bool GL, bool BATCH>
+__global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCloud cl0, CloudTable tab, const gpdb_pose *cand, int nc,
                                                       uint8_t *p16, const double *qtab, int *err, int plane_bytes,
                                                       int list_bytes, unsigned long long *prof, const int *work,
                                                       const int *work_n, unsigned char *gl_base, int gl_cap, int *ovf2,
@@ -1394,16 +1404,18 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
     for (int k = tid; k < SS; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);  // tiles A, B: clean
     __syncthreads();
     PHASE(1);   // image start
-    const bool need_cam = (C == 15) && !P.all_seen;  // the camera set of the neighbourhood is only read by the shadow
+    const auto &G = CloudSel<BATCH>::get(P, tab, sm.h.sample_slot);
+    const DevCloud cl = local_cloud(G, cl0);
+    const bool need_cam = (C == 15) && !G.all_seen;  // the camera set of the neighbourhood is only read by the shadow
     const gpdb_pose &h = sm.h;
     const double inv_d = 1.0 / P.vol_d, inv_w = 1.0 / P.vol_w, inv_h = 1.0 / (2.0 * P.vol_h);
     float q[3] = {(float)h.sample[0], (float)h.sample[1], (float)h.sample[2]};
-    SegRange sr = seg_range(P, q, P.rf_img);
+    SegRange sr = seg_range(G, q, P.rf_img);
     // ---- ball scan 1: neighbourhood centre + camera set (HandSet::calculateShadow, hand_set.cpp:131-136)
     //      and the list of points inside the image box (ImageStrategy::transformToUnitImage)
     double sx = 0, sy = 0, sz = 0;
     int cnt = 0, cam_or = 0;
-    scan_balanced<NT_IMG>(P, cl, sr, sm.seg, [&](bool in, const float4 &p, int where) {
+    scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int where) {
       // the scan only APPENDS the raw box points (few lanes qualify: doing the per-point work here would run it at
       // ~6 % lane utilisation); unit coordinates, cells and normals are computed densely after the scan
       bool inb = false, inball = false;
@@ -1477,7 +1489,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         a2 += sm.red[w][2];
       }
       double nn = (double)sm.n_img;
-      if (!need_cam && sm.n_img > 0) sm.cam_or = (1 << P.K) - 1;  // every point is seen by every camera (set at upload)
+      if (!need_cam && sm.n_img > 0) sm.cam_or = (1 << G.K) - 1;  // every point is seen by every camera (set at upload)
       sm.center[0] = a0 / nn;
       sm.center[1] = a1 / nn;
       sm.center[2] = a2 / nn;
@@ -1734,7 +1746,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
     PHASE(3);  // points phase (3 projections) done
     // ---- shadow phase (15 channels): HandSet::calculateShadow, deterministic variant
     if (C == 15) {
-      const int K = P.K;
+      const int K = G.K;
       const int bmd = P.bm_dim;
       const int bm_words = 2 * bmd * bmd;  // rows of 64 bits along x (bm_dim <= 64)
       const double gmax = qtab[GPDB_QTAB_SIZE - 1];
@@ -1763,7 +1775,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
       }
       if (tid < K) {
         // shadow_vec = shadow_length * (center - view_point) / norm (hand_set.cpp:146-150)
-        double s0 = sm.center[0] - P.vp[tid][0], s1 = sm.center[1] - P.vp[tid][1], s2 = sm.center[2] - P.vp[tid][2];
+        double s0 = sm.center[0] - G.vp[tid][0], s1 = sm.center[1] - G.vp[tid][1], s2 = sm.center[2] - G.vp[tid][2];
         double nn = sqrt((s0 * s0 + s1 * s1) + s2 * s2);
         sm.sv[tid][0] = P.shadow_length * s0 / nn;
         sm.sv[tid][1] = P.shadow_length * s1 / nn;
@@ -1907,7 +1919,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
             append(ok, p, rg);
           }
         } else {  // more in-ball points than the list holds: walk the grid again
-          scan_balanced<NT_IMG>(P, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
+          scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
             unsigned rg = 0;
             const bool ok = in && l2_simple(q, p.x, p.y, p.z) < P.r2_img && cull(p, rg);
             append(ok, p, rg);
@@ -2188,7 +2200,8 @@ struct Img2Smem {
   float fred[NT_IMG / 32][8];
 };
 
-__global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevCloud cl, const gpdb_pose *cand, int nc,
+template <bool BATCH>
+__global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevCloud cl0, CloudTable tab, const gpdb_pose *cand, int nc,
                                                        uint8_t *p16, const double *qtab, int *ovf, int *ovf_count,
                                                        unsigned long long *prof) {
   long long t_phase = 0;
@@ -2239,14 +2252,16 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
     __syncthreads();
     PHASE(1);
     const gpdb_pose &h = sm.h;
-    const bool need_cam = (C == 15) && !P.all_seen;
+    const auto &G = CloudSel<BATCH>::get(P, tab, h.sample_slot);
+    const DevCloud cl = local_cloud(G, cl0);
+    const bool need_cam = (C == 15) && !G.all_seen;
     const double inv_d = 1.0 / P.vol_d, inv_w = 1.0 / P.vol_w, inv_h = 1.0 / (2.0 * P.vol_h);
     float q[3] = {(float)h.sample[0], (float)h.sample[1], (float)h.sample[2]};
-    SegRange sr = seg_range(P, q, P.rf_img);
+    SegRange sr = seg_range(G, q, P.rf_img);
     // ---- ball scan 1: neighbourhood centre, camera set, raw box points
     double sx = 0, sy = 0, sz = 0;
     int cnt = 0, cam_or = 0;
-    scan_balanced<NT_IMG>(P, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
+    scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
       bool inb = false;
       unsigned long long key = 0;
       if (in) {
@@ -2263,7 +2278,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           if (in_image_box(P, h, x, y, z)) {
             inb = true;
             key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)idx;
-            if (P.nonunit && !unit_normal(cl.nrm + 3 * (size_t)idx)) sm.nonunit = 1;
+            if (G.nonunit && !unit_normal(cl.nrm + 3 * (size_t)idx)) sm.nonunit = 1;
           }
         }
       }
@@ -2306,7 +2321,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         a2 += sm.red[w][2];
       }
       double nn = (double)sm.n_img;
-      if (!need_cam && sm.n_img > 0) sm.cam_or = (1 << P.K) - 1;
+      if (!need_cam && sm.n_img > 0) sm.cam_or = (1 << G.K) - 1;
       sm.center[0] = a0 / nn;
       sm.center[1] = a1 / nn;
       sm.center[2] = a2 / nn;
@@ -2435,7 +2450,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
 
     // ---- shadow phase (15 channels)
     if (C == 15) {
-      const int K = P.K;
+      const int K = G.K;
       const int bmd = P.bm_dim;
       const int bm_words = 2 * bmd * bmd;
       const double gmax = qtab[GPDB_QTAB_SIZE - 1];
@@ -2462,7 +2477,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         }
       }
       if (tid < K) {
-        double s0 = sm.center[0] - P.vp[tid][0], s1 = sm.center[1] - P.vp[tid][1], s2 = sm.center[2] - P.vp[tid][2];
+        double s0 = sm.center[0] - G.vp[tid][0], s1 = sm.center[1] - G.vp[tid][1], s2 = sm.center[2] - G.vp[tid][2];
         double nn = sqrt((s0 * s0 + s1 * s1) + s2 * s2);
         sm.sv[tid][0] = P.shadow_length * s0 / nn;
         sm.sv[tid][1] = P.shadow_length * s1 / nn;
@@ -2553,7 +2568,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           rg = (unsigned)r0 | ((unsigned)r1 << 16);
           return true;
         };
-        scan_balanced<NT_IMG>(P, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
+        scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
           unsigned rg = 0;
           const bool ok = in && l2_simple(q, p.x, p.y, p.z) < P.r2_img && cull(p, rg);
           const unsigned mk = __ballot_sync(0xffffffffu, ok);
@@ -2850,6 +2865,140 @@ __global__ void k_hwc_to_p16(const uint8_t *__restrict__ hwc, size_t npix, int C
   reinterpret_cast<uint4 *>(p16)[i] = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
+// ------------------------------------------------------------------------------------------------
+// batch of clouds (gpdb_set_clouds): one grid per cloud, built for all clouds in one segmented pass
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int b_f2ord(float f) {  // order-preserving int image of a float (as pre_bounds)
+  int i = __float_as_int(f);
+  return i >= 0 ? i : i ^ 0x7fffffff;
+}
+// the cloud holding concatenated point g: largest b with d[b].off <= g (clouds are not empty)
+__device__ __forceinline__ int b_cloud_of_point(const CloudDesc *d, int B, int g) {
+  int lo = 0, hi = B;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (d[mid].off <= g) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+// one CTA per cloud: bounds, then the grid geo_build_grid derives from them (same float32 steps), and whether any normal
+// is off unit length (pre_nonunit). ncell[b] = cells of cloud b.
+__global__ void __launch_bounds__(256) k_batch_desc(const float *xyz, const double *nrm, CloudDesc *d, long long *ncell) {
+  __shared__ int s_mn[3], s_mx[3], s_nonunit;
+  CloudDesc &D = d[blockIdx.x];
+  if (threadIdx.x < 3) {
+    s_mn[threadIdx.x] = INT_MAX;
+    s_mx[threadIdx.x] = INT_MIN;
+  }
+  if (threadIdx.x == 0) s_nonunit = 0;
+  __syncthreads();
+  int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
+  bool nonunit = false;
+  for (int i = D.off + threadIdx.x; i < D.off + D.N; i += blockDim.x) {
+    for (int a = 0; a < 3; a++) {
+      const int o = b_f2ord(xyz[3 * (size_t)i + a]);
+      mn[a] = min(mn[a], o);
+      mx[a] = max(mx[a], o);
+    }
+    if (!unit_normal(nrm + 3 * (size_t)i)) nonunit = true;
+  }
+  for (int a = 0; a < 3; a++) {
+    mn[a] = __reduce_min_sync(0xffffffffu, mn[a]);
+    mx[a] = __reduce_max_sync(0xffffffffu, mx[a]);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    for (int a = 0; a < 3; a++) {
+      atomicMin(s_mn + a, mn[a]);
+      atomicMax(s_mx + a, mx[a]);
+    }
+  }
+  if (nonunit) s_nonunit = 1;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  float lo[3], hi[3];
+  for (int a = 0; a < 3; a++) {
+    lo[a] = __int_as_float(s_mn[a] >= 0 ? s_mn[a] : s_mn[a] ^ 0x7fffffff);
+    hi[a] = __int_as_float(s_mx[a] >= 0 ? s_mx[a] : s_mx[a] ^ 0x7fffffff);
+  }
+  float cell = 0.02f;
+  double nc;
+  for (;;) {
+    nc = 1;
+    for (int a = 0; a < 3; a++) {
+      D.dim[a] = (int)floorf((hi[a] - lo[a]) / cell) + 2;
+      nc *= D.dim[a];
+    }
+    if (nc <= 48e6) break;
+    cell *= 1.5f;
+  }
+  for (int a = 0; a < 3; a++) D.lo[a] = lo[a];
+  D.inv_cell = 1.0f / cell;
+  D.nonunit = s_nonunit;
+  ncell[blockIdx.x] = (long long)nc;
+}
+__global__ void k_batch_base(CloudDesc *d, const long long *base, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) d[b].cell_base = (int)base[b];
+}
+// cell id of every point in the batch-wide numbering (cloud b's cells start at its cell_base): sorting by it orders the
+// points by (cloud, cell), stable in point order
+__global__ void k_batch_cell_ids(const float *xyz, const CloudDesc *d, int B, int N, int *cid, int *idx, int *counts) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= N) return;
+  const CloudDesc &D = d[b_cloud_of_point(d, B, g)];
+  const int c = D.cell_base +
+                (cell_of(D, xyz[3 * g + 2], 2) * D.dim[1] + cell_of(D, xyz[3 * g + 1], 1)) * D.dim[0] + cell_of(D, xyz[3 * g], 0);
+  cid[g] = c;
+  idx[g] = g;
+  atomicAdd(counts + c + 1, 1);
+}
+__global__ void k_batch_fill_sorted(const float *xyz, const int *idx_sorted, const CloudDesc *d, int B, int N, float4 *pts4) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= N) return;
+  const int g = idx_sorted[k];
+  const int local = g - d[b_cloud_of_point(d, B, g)].off;
+  pts4[k] = make_float4(xyz[3 * g], xyz[3 * g + 1], xyz[3 * g + 2], __int_as_float(local));
+}
+// first candidate of every cloud: candidates are in sample-slot order, cloud b owns the slots [soff[b], soff[b+1])
+__global__ void k_batch_cand_off(const gpdb_pose *cand, int n, const int *soff, int B, int *cand_off) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > B) return;
+  const int slot = soff[b];
+  int lo = 0, hi = n;  // first candidate with sample_slot >= slot
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (cand[mid].sample_slot < slot) lo = mid + 1; else hi = mid;
+  }
+  cand_off[b] = lo;
+}
+// selection keys of a batch: cloud in the high word (clouds in order), descending score below (as k_select_keys); one
+// stable device-wide radix sort then orders every cloud's candidates as gpdb_detect_select would, ties in candidate order
+__global__ void k_batch_select_keys(const gpdb_pose *cand, int n, const int *soff, int B, unsigned long long *keys, int *vals) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int slot = cand[i].sample_slot;
+  int lo = 0, hi = B;  // largest b with soff[b] <= slot
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (soff[mid] <= slot) lo = mid; else hi = mid;
+  }
+  unsigned u = __float_as_uint(cand[i].score);
+  u ^= (u >> 31) ? 0xFFFFFFFFu : 0x80000000u;
+  keys[i] = ((unsigned long long)lo << 32) | ~u;
+  vals[i] = i;
+}
+// the selected records in output order: the first sel_off[b+1] - sel_off[b] of cloud b's sorted segment
+__global__ void k_batch_sel_order(const int *sorted_vals, const int *cand_off, const int *sel_off, int B, int k, int *order) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= k) return;
+  int lo = 0, hi = B;  // largest b with sel_off[b] <= j
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (sel_off[mid] <= j) lo = mid; else hi = mid;
+  }
+  order[j] = sorted_vals[cand_off[lo] + (j - sel_off[lo])];
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -2913,12 +3062,12 @@ int geo_build_grid(gpdb_ctx *ctx, const float lo[3], const float hi[3], int N) {
   return GPDB_OK;
 }
 
-int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
-  if (n <= 0) return GPDB_OK;
+template <bool BATCH>
+static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
   const int cap0 = 128;  // ~44 points at the default nn_radius on a 3 mm cloud
   const size_t smem0 = (size_t)2 * LRF_WARPS * cap0 * sizeof(unsigned long long);
   const size_t smem1 = (size_t)2 * LRF_WARPS * LRF_CAP * sizeof(unsigned long long);
-  CUDA_TRY(cudaFuncSetAttribute(k_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+  CUDA_TRY(cudaFuncSetAttribute(k_frames<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
   int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * 2 * ((size_t)n + 1));
   const int g2 = 37;  // tier 2: 148 warps, 2 x 8 B x LRF_CAP_GLOBAL each (38 MB of scratch)
   unsigned long long *gkeys =
@@ -2927,48 +3076,65 @@ int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
+  const CloudTable tab = ctx->run;
   const int grid = (n + LRF_WARPS - 1) / LRF_WARPS;
-  k_frames<<<grid, LRF_WARPS * 32, smem0, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, d_frames, d_valid, ctx->d_err, cap0, ovf,
-                                                       ovf_count, ovf2, ovf2_count, nullptr, 0);
+  k_frames<BATCH><<<grid, LRF_WARPS * 32, smem0, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, d_frames, d_valid, ctx->d_err, cap0,
+                                                                ovf, ovf_count, ovf2, ovf2_count, nullptr, 0);
   LAUNCH_CHECK();
   // overflow tiers over the (usually empty) lists: the tier-1 grid is sized for the worst case (every sample overflowed) so
   // no host round trip is needed; warps beyond the list length exit at once
-  k_frames<<<grid, LRF_WARPS * 32, smem1, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, d_frames, d_valid, ctx->d_err, LRF_CAP, ovf,
-                                                       ovf_count, ovf2, ovf2_count, nullptr, 1);
+  k_frames<BATCH><<<grid, LRF_WARPS * 32, smem1, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, d_frames, d_valid, ctx->d_err,
+                                                                LRF_CAP, ovf, ovf_count, ovf2, ovf2_count, nullptr, 1);
   LAUNCH_CHECK();
-  k_frames<<<g2, LRF_WARPS * 32, 0, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, d_frames, d_valid, ctx->d_err, LRF_CAP_GLOBAL, ovf,
-                                                 ovf_count, ovf2, ovf2_count, gkeys, 2);
+  k_frames<BATCH><<<g2, LRF_WARPS * 32, 0, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, d_frames, d_valid, ctx->d_err,
+                                                          LRF_CAP_GLOBAL, ovf, ovf_count, ovf2, ovf2_count, gkeys, 2);
   LAUNCH_CHECK();
   return GPDB_OK;
+}
+
+int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
+  if (n <= 0) return GPDB_OK;
+  return ctx->run.n ? launch_frames<true>(ctx, ctx->bcloud, d_sidx, n, d_frames, d_valid)
+                    : launch_frames<false>(ctx, ctx->cloud, d_sidx, n, d_frames, d_valid);
 }
 
 static const int HANDS_CAP1 = 2176, HANDS_CAP2 = 12800;  // tier 1: 4 CTAs per SM (34 KB + 20 KB static each, <= 64 registers)
 static const int HANDS_CAP3 = 131072;                    // last tier: neighbourhood staged in global memory (2 MB per CTA)
 
-int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
-              gpdb_pose *d_poses, uint8_t *d_flags) {
-  if (n <= 0) return GPDB_OK;
+template <bool BATCH>
+static int launch_hands(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, int n, int slot0, const double *d_frames,
+                        const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags) {
   // per call, not once per process: function attributes belong to the current device's context (one context per GPU)
-  CUDA_TRY(cudaFuncSetAttribute(k_hands, cudaFuncAttributeMaxDynamicSharedMemorySize, HANDS_CAP2 * 16));
+  CUDA_TRY(cudaFuncSetAttribute(k_hands<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, HANDS_CAP2 * 16));
   int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * 2 * ((size_t)n + 1));
   float4 *glist = (float4 *)gpdb_scratch(ctx, 21, sizeof(float4) * (size_t)HANDS_CAP3 * ctx->sm_count);
   if (!ovf || !glist) return GPDB_ERR_CUDA;
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
-  k_hands<<<n, NT_HANDS, HANDS_CAP1 * 16, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, slot0, d_frames, d_valid, d_poses,
-                                                         d_flags, HANDS_CAP1, nullptr, nullptr, ovf, ovf_count, nullptr, ctx->d_err);
+  const CloudTable tab = ctx->run;
+  k_hands<BATCH><<<n, NT_HANDS, HANDS_CAP1 * 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames, d_valid, d_poses,
+                                                                d_flags, HANDS_CAP1, nullptr, nullptr, ovf, ovf_count, nullptr,
+                                                                ctx->d_err);
   LAUNCH_CHECK();
   // large-tile pass over the samples whose neighbourhood did not fit tier 1 (persistent CTAs) ...
-  k_hands<<<ctx->sm_count, NT_HANDS, HANDS_CAP2 * 16, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, slot0, d_frames,
-                                                                     d_valid, d_poses, d_flags, HANDS_CAP2, ovf, ovf_count,
-                                                                     ovf2, ovf2_count, nullptr, ctx->d_err);
+  k_hands<BATCH><<<ctx->sm_count, NT_HANDS, HANDS_CAP2 * 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames,
+                                                                            d_valid, d_poses, d_flags, HANDS_CAP2, ovf,
+                                                                            ovf_count, ovf2, ovf2_count, nullptr, ctx->d_err);
   LAUNCH_CHECK();
   // ... and the last tier over what did not fit that either: neighbourhood in global memory (usually an empty list)
-  k_hands<<<ctx->sm_count, NT_HANDS, 16, ctx->stream>>>(ctx->dp, ctx->cloud, d_sidx, n, slot0, d_frames, d_valid, d_poses,
-                                                        d_flags, HANDS_CAP3, ovf2, ovf2_count, nullptr, nullptr, glist, ctx->d_err);
+  k_hands<BATCH><<<ctx->sm_count, NT_HANDS, 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames, d_valid, d_poses,
+                                                               d_flags, HANDS_CAP3, ovf2, ovf2_count, nullptr, nullptr, glist,
+                                                               ctx->d_err);
   LAUNCH_CHECK();
   return GPDB_OK;
+}
+
+int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
+              gpdb_pose *d_poses, uint8_t *d_flags) {
+  if (n <= 0) return GPDB_OK;
+  return ctx->run.n ? launch_hands<true>(ctx, ctx->bcloud, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags)
+                    : launch_hands<false>(ctx, ctx->cloud, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags);
 }
 
 int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags, int n_poses, gpdb_pose *d_cand,
@@ -3000,13 +3166,15 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
 // k_images alone when the geometry is outside the fast path's limits (image_size != 60; at 15 channels more than two
 // cameras, or shadow bitmaps that leave less than 2 KB of the box list: two cameras at the default image volume) or when
 // GPD_B200_IMAGES_KERNEL=1 forces it (tests compare the kernels).
-int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
-  if (nc <= 0) return GPDB_OK;
+template <bool BATCH>
+static int launch_images(gpdb_ctx *ctx, const DevCloud &cl, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
   const DevParams &hp = ctx->hp;
+  const int K = BATCH ? ctx->b_maxk : hp.K;  // a batch is sized for its largest camera count
+  const CloudTable tab = ctx->run;
   const int S = hp.S, RS = (S + 3) & ~3;
   const size_t plane_bytes = ((size_t)hp.C * S * RS + 15) / 16 * 16;
   const size_t tiles = (size_t)3 * 8 * S * S;
-  const size_t bm = (size_t)hp.K * (2 * (size_t)hp.bm_dim * hp.bm_dim) * 4;
+  const size_t bm = (size_t)K * (2 * (size_t)hp.bm_dim * hp.bm_dim) * 4;
   // shadow phase: the bitmaps alias the box list and the compacted voxel list follows them: room for >= 4 k voxels
   const size_t list_bytes = (std::max((size_t)BOX_CAP * 36, hp.C == 15 ? bm + 4096 * 4 : (size_t)0) + 15) / 16 * 16;
   const size_t smem = plane_bytes + tiles + list_bytes;
@@ -3015,7 +3183,7 @@ int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
     return GPDB_ERR_INVALID;
   }
   const char *force = getenv("GPD_B200_IMAGES_KERNEL");
-  const bool fast = S == 60 && (hp.C != 15 || (hp.K <= 2 && bm + 2048 <= (size_t)BOX_CAP2 * 36)) && !(force && force[0] == '1');
+  const bool fast = S == 60 && (hp.C != 15 || (K <= 2 && bm + 2048 <= (size_t)BOX_CAP2 * 36)) && !(force && force[0] == '1');
   const int *d_work = nullptr, *d_work_n = nullptr;
   if (fast) {
     int *ovf = (int *)gpdb_scratch(ctx, 22, sizeof(int) * ((size_t)nc + 1));  // not slot 2: the hand search of the next chunk
@@ -3023,8 +3191,8 @@ int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
     int *ovf_count = ovf + nc;
     CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
     const size_t smem2 = (size_t)2 * 8 * S * S + (size_t)3 * S * S + (size_t)BOX_CAP2 * 36;
-    CUDA_TRY(cudaFuncSetAttribute(k_images2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    k_images2<<<std::min(nc, ctx->sm_count * 64), NT_IMG, smem2, ctx->stream>>>(ctx->dp, ctx->cloud, d_cand, nc, d_p16, ctx->d_qtab, ovf,
+    CUDA_TRY(cudaFuncSetAttribute(k_images2<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    k_images2<BATCH><<<std::min(nc, ctx->sm_count * 64), NT_IMG, smem2, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ovf,
                                                                                ovf_count, ctx->d_prof);
     LAUNCH_CHECK();
     d_work = ovf;
@@ -3041,29 +3209,35 @@ int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
   const int grid = fast ? ctx->sm_count : std::min(nc, ctx->sm_count * 64);
   if (S == 60) {
-    CUDA_TRY(cudaFuncSetAttribute(k_images<60, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_TRY(cudaFuncSetAttribute(k_images<60, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_images<60, false><<<grid, NT_IMG, smem, ctx->stream>>>(ctx->dp, ctx->cloud, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
+    CUDA_TRY(cudaFuncSetAttribute(k_images<60, false, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(cudaFuncSetAttribute(k_images<60, true, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_images<60, false, BATCH><<<grid, NT_IMG, smem, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
                                                              (int)plane_bytes, (int)list_bytes, ctx->d_prof, d_work, d_work_n,
                                                              nullptr, 0, ovf2, ovf2_count);
     LAUNCH_CHECK();
     // ... which the last tier redoes with the box list in global memory (32 768 points; beyond: GPDB_ERR_CAPACITY)
-    k_images<60, true><<<ctx->sm_count, NT_IMG, smem, ctx->stream>>>(ctx->dp, ctx->cloud, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
+    k_images<60, true, BATCH><<<ctx->sm_count, NT_IMG, smem, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
                                                                      (int)plane_bytes, (int)list_bytes, ctx->d_prof, ovf2, ovf2_count,
                                                                      gl, gl_cap, nullptr, nullptr);
   } else {
-    CUDA_TRY(cudaFuncSetAttribute(k_images<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_TRY(cudaFuncSetAttribute(k_images<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_images<0, false><<<grid, NT_IMG, smem, ctx->stream>>>(ctx->dp, ctx->cloud, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
+    CUDA_TRY(cudaFuncSetAttribute(k_images<0, false, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(cudaFuncSetAttribute(k_images<0, true, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_images<0, false, BATCH><<<grid, NT_IMG, smem, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
                                                             (int)plane_bytes, (int)list_bytes, ctx->d_prof, d_work, d_work_n,
                                                             nullptr, 0, ovf2, ovf2_count);
     LAUNCH_CHECK();
-    k_images<0, true><<<ctx->sm_count, NT_IMG, smem, ctx->stream>>>(ctx->dp, ctx->cloud, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
+    k_images<0, true, BATCH><<<ctx->sm_count, NT_IMG, smem, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ctx->d_err,
                                                                     (int)plane_bytes, (int)list_bytes, ctx->d_prof, ovf2, ovf2_count,
                                                                     gl, gl_cap, nullptr, nullptr);
   }
   LAUNCH_CHECK();
   return GPDB_OK;
+}
+
+int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
+  if (nc <= 0) return GPDB_OK;
+  return ctx->run.n ? launch_images<true>(ctx, ctx->bcloud, d_cand, nc, d_p16)
+                    : launch_images<false>(ctx, ctx->cloud, d_cand, nc, d_p16);
 }
 
 int geo_p16_to_hwc(gpdb_ctx *ctx, const uint8_t *d_p16, int n, uint8_t *d_hwc) {
@@ -3121,4 +3295,106 @@ int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_sc
   k_scatter_scores<<<(nc + 255) / 256, 256, 0, ctx->stream>>>(d_cand, d_scores, nc, slot0, P, d_pose_scores, d_cand_out);
   LAUNCH_CHECK();
   return GPDB_OK;
+}
+
+// The grids of the batch installed in ctx->d_bxyz / d_bnrm (N points, ctx->b_n clouds whose descriptors hold off / N / K /
+// all_seen / vp): bounds, dims, cell bases and non-unit flags on the device, one sort over (cloud, cell) for all clouds.
+int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
+  const int B = ctx->b_n;
+  long long *ncell = (long long *)gpdb_scratch(ctx, 5, sizeof(long long) * 2 * ((size_t)B + 1));
+  if (!ncell) return GPDB_ERR_CUDA;
+  long long *base = ncell + B + 1;
+  CUDA_TRY(cudaMemsetAsync(ncell + B, 0, sizeof(long long), ctx->stream));
+  k_batch_desc<<<B, 256, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bnrm, ctx->d_bdesc, ncell);
+  LAUNCH_CHECK();
+  size_t tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ncell, base, B + 1, ctx->stream);
+  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  if (!tmp) return GPDB_ERR_CUDA;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, ncell, base, B + 1, ctx->stream));
+  ctx->launches += 1;
+  long long total = 0;
+  CUDA_TRY(cudaMemcpyAsync(&total, base + B, sizeof(total), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (total + 1 > (long long)INT_MAX) {
+    gpdb_set_error(ctx, GPDB_ERR_CAPACITY, "gpdb_set_clouds: the grids of the batch need %lld cells (max %d)", total, INT_MAX - 1);
+    return GPDB_ERR_CAPACITY;
+  }
+  k_batch_base<<<(B + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_bdesc, base, B);
+  LAUNCH_CHECK();
+  const size_t ncells = (size_t)total;
+  if (ncells + 1 > ctx->bcell_cap) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(ctx->d_bcell_start);
+    ctx->d_bcell_start = nullptr;
+    ctx->bcell_cap = 0;
+    CUDA_TRY(cudaMalloc(&ctx->d_bcell_start, sizeof(int) * (ncells + 1 + ncells / 4)));
+    ctx->bcell_cap = ncells + 1 + ncells / 4;
+  }
+  CUDA_TRY(cudaMemsetAsync(ctx->d_bcell_start, 0, sizeof(int) * (ncells + 1), ctx->stream));
+  int *cid = (int *)gpdb_scratch(ctx, 0, sizeof(int) * (size_t)N * 4);
+  if (!cid) return GPDB_ERR_CUDA;
+  int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
+  const int tb = 256, gb = (N + tb - 1) / tb;
+  k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bdesc, B, N, cid, idx, ctx->d_bcell_start);
+  LAUNCH_CHECK();
+  size_t tmp2 = 0;
+  tmp_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream);
+  cub::DeviceScan::InclusiveSum(nullptr, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream);
+  tmp = gpdb_scratch(ctx, 1, std::max(tmp_bytes, tmp2));
+  if (!tmp) return GPDB_ERR_CUDA;
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream));
+  ctx->launches += 4;
+  k_batch_fill_sorted<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, idx2, ctx->d_bdesc, B, N, ctx->d_bpts4);
+  LAUNCH_CHECK();
+  CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream));
+  ctx->launches += 2;
+  ctx->bcloud.cell_start = ctx->d_bcell_start;
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return GPDB_OK;
+}
+
+// gpdb_detect_select per cloud of the running batch: the n classified candidates (sample-slot order) are sorted by
+// (cloud, descending score) with one stable device-wide radix sort, so ties keep candidate order and one large cloud is
+// sorted by the whole device; the first min(k, count) of every cloud are gathered to d_out in cloud order.
+// sel_off[B+1] (host) receives the output offsets; returns the total.
+int geo_select_batch(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, int *sel_off, gpdb_pose **d_out) {
+  const int B = ctx->run.n;
+  *d_out = nullptr;
+  unsigned long long *keys = (unsigned long long *)gpdb_scratch(
+      ctx, 3, sizeof(unsigned long long) * 2 * (size_t)n + sizeof(int) * (3 * (size_t)n + 2 * ((size_t)B + 1)));
+  if (!keys) return GPDB_ERR_CUDA;
+  unsigned long long *keys2 = keys + n;
+  int *vals = (int *)(keys2 + n), *vals2 = vals + n, *order = vals2 + n, *cand_off = order + n, *d_sel_off = cand_off + B + 1;
+  k_batch_cand_off<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, ctx->run.soff, B, cand_off);
+  LAUNCH_CHECK();
+  std::vector<int> coff((size_t)B + 1);
+  CUDA_TRY(cudaMemcpyAsync(coff.data(), cand_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  if (n > 0) {
+    k_batch_select_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, ctx->run.soff, B, keys, vals);
+    LAUNCH_CHECK();
+    int cloud_bits = 0;
+    while ((1ll << cloud_bits) < B) cloud_bits++;
+    size_t tmp_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32 + cloud_bits, ctx->stream);
+    void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+    if (!tmp) return GPDB_ERR_CUDA;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32 + cloud_bits, ctx->stream));
+    ctx->launches += 4;
+  }
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  sel_off[0] = 0;
+  for (int b = 0; b < B; b++) sel_off[b + 1] = sel_off[b] + std::min(k, coff[b + 1] - coff[b]);
+  const int total = sel_off[B];
+  if (total == 0) return 0;
+  CUDA_TRY(cudaMemcpyAsync(d_sel_off, sel_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  k_batch_sel_order<<<(total + 255) / 256, 256, 0, ctx->stream>>>(vals2, cand_off, d_sel_off, B, total, order);
+  LAUNCH_CHECK();
+  gpdb_pose *out = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)total);
+  if (!out) return GPDB_ERR_CUDA;
+  k_gather_poses<<<(total * 32 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, order, total, out);
+  LAUNCH_CHECK();
+  *d_out = out;
+  return total;
 }

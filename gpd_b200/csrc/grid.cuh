@@ -7,7 +7,9 @@
 
 namespace {
 
-__device__ __forceinline__ int cell_of(const DevParams &P, float v, int a) {
+// G: DevParams (the single cloud) or CloudDesc (one cloud of a batch): both carry lo / inv_cell / dim
+template <class G>
+__device__ __forceinline__ int cell_of(const G &P, float v, int a) {
   int c = (int)floorf((v - P.lo[a]) * P.inv_cell);
   return min(max(c, 0), P.dim[a] - 1);
 }
@@ -27,6 +29,35 @@ __device__ __forceinline__ void sample_position(const DevCloud &cl, int si, doub
   }
 }
 
+// The cloud of a sample slot. Single cloud (BATCH = false): DevParams itself, so that instantiation compiles to the code
+// it always was. Batch: the descriptor of the cloud whose CSR sample range holds the slot (binary search over soff).
+template <bool BATCH>
+struct CloudSel {
+  static __device__ __forceinline__ const DevParams &get(const DevParams &P, const CloudTable &, int) { return P; }
+};
+template <>
+struct CloudSel<true> {
+  static __device__ __forceinline__ const CloudDesc &get(const DevParams &, const CloudTable &t, int slot) {
+    int lo = 0, hi = t.n;  // largest b with soff[b] <= slot
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (__ldg(t.soff + mid) <= slot) lo = mid; else hi = mid;
+    }
+    return t.d[lo];
+  }
+};
+// The arrays of that cloud: indices (sample indices, pts4 w bits) are local to it; pts4 positions and cell_start values
+// stay batch-wide.
+__device__ __forceinline__ DevCloud local_cloud(const DevParams &, const DevCloud &cl) { return cl; }
+__device__ __forceinline__ DevCloud local_cloud(const CloudDesc &D, DevCloud cl) {
+  cl.xyz += 3 * (size_t)D.off;
+  cl.nrm += 3 * (size_t)D.off;
+  cl.cam += D.off;
+  cl.cell_start += D.cell_base;
+  cl.n_points = D.N;
+  return cl;
+}
+
 // FLANN L2_Simple<float> (float32, accumulated x,y,z in order)
 __device__ __forceinline__ float l2_simple(const float q[3], float x, float y, float z) {
   float dx = q[0] - x, dy = q[1] - y, dz = q[2] - z;
@@ -44,7 +75,8 @@ __device__ __forceinline__ float l2_simple(const float q[3], float x, float y, f
 struct SegRange {
   int c0[3], c1[3], ny, nrows;
 };
-__device__ __forceinline__ SegRange seg_range(const DevParams &P, const float q[3], float rf) {
+template <class G>
+__device__ __forceinline__ SegRange seg_range(const G &P, const float q[3], float rf) {
   SegRange s;
 #pragma unroll
   for (int a = 0; a < 3; a++) {
@@ -55,7 +87,8 @@ __device__ __forceinline__ SegRange seg_range(const DevParams &P, const float q[
   s.nrows = s.ny * (s.c1[2] - s.c0[2] + 1);
   return s;
 }
-__device__ __forceinline__ void seg_row(const DevParams &P, const int *cell_start, const SegRange &s, int row, int &start,
+template <class G>
+__device__ __forceinline__ void seg_row(const G &P, const int *cell_start, const SegRange &s, int row, int &start,
                                         int &len) {
   int cy = s.c0[1] + row % s.ny, cz = s.c0[2] + row / s.ny;
   size_t base = ((size_t)cz * P.dim[1] + cy) * P.dim[0];
@@ -65,8 +98,8 @@ __device__ __forceinline__ void seg_row(const DevParams &P, const int *cell_star
 
 // Ball scan, one warp per grid row: lanes stride over the row's contiguous point segment (coalesced float4 loads).
 // body(in_range, point) is called by all 32 lanes together, so it may use warp collectives.
-template <int NT, class F>
-__device__ __forceinline__ void scan_rows(const DevParams &P, const DevCloud &cl, const SegRange &sr, F &&body) {
+template <int NT, class G, class F>
+__device__ __forceinline__ void scan_rows(const G &P, const DevCloud &cl, const SegRange &sr, F &&body) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int NW = NT / 32;
   // this warp owns rows warp, warp + NW, ...; the bounds of 32 of them are fetched at once (one lane each) so that

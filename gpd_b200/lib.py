@@ -24,6 +24,7 @@ EXPORTS = [
     "gpdb_get_cloud", "gpdb_get_cloud_source_index", "gpdb_preprocess_timings", "gpdb_detect_select", "gpdb_load_weights_file", "gpdb_read_weights_file", "gpdb_set_samples",
     "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
+    "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select",
 ]
 
 
@@ -84,6 +85,9 @@ def lib():
     L.gpdb_find_clusters.argtypes = [vp, vp, C.c_int32, C.c_int32, vp]
     L.gpdb_reevaluate.argtypes = [vp, vp, C.c_int32, vp]
     L.gpdb_set_overlap.argtypes = [vp, C.c_int32]
+    L.gpdb_set_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
+    L.gpdb_detect_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
+    L.gpdb_detect_batch_select.argtypes = [vp, vp, vp, C.c_int32, C.POINTER(abi.Result), vp]
     _LIB = L
     return L
 
@@ -142,6 +146,52 @@ def read_weights_file(weights_file, channels, model_file=None):
     return arrs, relu.value
 
 
+def pack_clouds(clouds):
+    """The CSR arrays of gpdb_set_clouds for a list of cloud dicts (xyz [N, 3], normals [N, 3], optional cam_source
+    [N, K], optional view_points [K, 3]): point offsets [B+1], xyz, normals, cam_source (None when no cloud has one; a
+    cloud without one is seen by all its cameras), camera counts [B] and view points, each concatenated in cloud order."""
+    if not clouds:
+        raise ValueError("pack_clouds: need at least one cloud")
+    xyz = [np.asarray(c["xyz"], dtype=np.float32).reshape(-1, 3) for c in clouds]
+    nrm = [np.asarray(c["normals"], dtype=np.float64).reshape(-1, 3) for c in clouds]
+    vps = [np.asarray(c.get("view_points") if c.get("view_points") is not None else np.zeros((1, 3)), dtype=np.float64).reshape(-1, 3)
+           for c in clouds]
+    ks = np.array([len(v) for v in vps], dtype=np.int32)
+    offsets = np.zeros(len(clouds) + 1, np.int32)
+    offsets[1:] = np.cumsum([len(x) for x in xyz])
+    cam = None
+    if any(c.get("cam_source") is not None for c in clouds):
+        blocks = []
+        for c, x, k in zip(clouds, xyz, ks):
+            cs = c.get("cam_source")
+            blocks.append(np.ones((len(x), k), np.int32) if cs is None else np.asarray(cs, dtype=np.int32).reshape(len(x), k))
+        cam = np.ascontiguousarray(np.concatenate([b.ravel() for b in blocks]))
+    return {"offsets": offsets, "xyz": np.ascontiguousarray(np.concatenate(xyz)), "normals": np.ascontiguousarray(np.concatenate(nrm)),
+            "cam_source": cam, "n_cameras": ks, "view_points": np.ascontiguousarray(np.concatenate(vps))}
+
+
+def pack_samples(sample_lists):
+    """The CSR arrays of gpdb_detect_batch for one list of cloud-local sample indices per cloud: (offsets [B+1], indices)."""
+    arrs = [np.asarray(s, dtype=np.int32).ravel() for s in sample_lists]
+    offsets = np.zeros(len(arrs) + 1, np.int32)
+    offsets[1:] = np.cumsum([len(a) for a in arrs])
+    return offsets, np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros(0, np.int32))
+
+
+def split_batch_result(out, sample_offsets, cand_offsets):
+    """Per-cloud views of one batch result (abi.result_to_numpy dict): the slices of every per-sample / per-pose array at
+    sample_offsets and of the candidates (and images) at cand_offsets."""
+    views = []
+    for b in range(len(sample_offsets) - 1):
+        s0, s1, c0, c1 = sample_offsets[b], sample_offsets[b + 1], cand_offsets[b], cand_offsets[b + 1]
+        v = {"n_samples": s1 - s0, "poses_per_sample": out["poses_per_sample"], "n_candidates": c1 - c0,
+             "candidates": out["candidates"][c0:c1], "images": None if out["images"] is None else out["images"][c0:c1]}
+        for k in ("frame_valid", "frames", "pose_flags", "pose_scores"):
+            v[k] = None if out[k] is None else out[k][s0:s1]
+        views.append(v)
+    return views
+
+
 class Context:
     """One gpdb_ctx: one CUDA device + stream (gpdb_create ... gpdb_destroy)."""
 
@@ -153,6 +203,7 @@ class Context:
             self.h = None
             raise GpdbError(rc, lib().gpdb_last_error(None).decode())
         self._keep = []
+        self._n_clouds = 0  # clouds of the installed batch (gpdb_detect_batch reads that many + 1 sample offsets)
 
     def close(self):
         if getattr(self, "h", None):
@@ -263,6 +314,48 @@ class Context:
         out = np.zeros(len(hands), dtype=abi.POSE_DTYPE)
         n = self._check(lib().gpdb_find_clusters(self.h, _p(hands), len(hands), int(min_inliers), _p(out)))
         return out[:n].copy()
+
+    def set_clouds(self, clouds):
+        """gpdb_set_clouds: installs a batch of processed clouds (list of dicts as set_cloud takes) beside the single cloud."""
+        pk = pack_clouds(clouds)
+        self._n_clouds = 0  # a failed gpdb_set_clouds leaves no batch
+        self._check(lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
+                                          _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])))
+        self._n_clouds = len(clouds)
+
+    def _pack_batch_samples(self, sample_lists):
+        # the C-ABI takes no cloud count: it reads and writes B + 1 offsets for the B installed clouds
+        if len(sample_lists) != self._n_clouds:
+            raise ValueError(f"{len(sample_lists)} sample lists for a batch of {self._n_clouds} clouds (one list per cloud)")
+        return pack_samples(sample_lists)
+
+    def detect_batch(self, sample_lists):
+        """gpdb_detect_batch: one list of cloud-local sample indices per installed cloud; returns one result dict per
+        cloud (views of the single batch result), each as detect() would return for that cloud alone."""
+        offsets, sidx = self._pack_batch_samples(sample_lists)
+        res = abi.Result()
+        coff = np.zeros(len(offsets), np.int32)
+        self._check(lib().gpdb_detect_batch(self.h, _p(offsets), _p(sidx), C.byref(res), _p(coff)))
+        S, Cc = self.params.image_size, self.params.image_num_channels
+        out = abi.result_to_numpy(res, S * S * Cc)
+        lib().gpdb_free_result(C.byref(res))
+        return split_batch_result(out, offsets, coff)
+
+    def detect_batch_select(self, sample_lists, num_selected):
+        """gpdb_detect_batch_select: the num_selected best candidates of every cloud; returns one record array per cloud."""
+        offsets, sidx = self._pack_batch_samples(sample_lists)
+        res = abi.Result()
+        soff = np.zeros(len(offsets), np.int32)
+        self._check(lib().gpdb_detect_batch_select(self.h, _p(offsets), _p(sidx), int(num_selected), C.byref(res), _p(soff)))
+        out = abi.result_to_numpy(res, 0)
+        lib().gpdb_free_result(C.byref(res))
+        return [out["candidates"][soff[b]:soff[b + 1]] for b in range(len(offsets) - 1)]
+
+    def detect_batch_raw(self, offsets_i32, sidx_i32, res, cand_offsets_i32):
+        """Timed path for tools/bench_batch.py: no numpy conversion; caller frees `res`."""
+        if len(offsets_i32) != self._n_clouds + 1 or len(cand_offsets_i32) != self._n_clouds + 1:
+            raise ValueError(f"offsets need {self._n_clouds + 1} entries for a batch of {self._n_clouds} clouds")
+        return self._check(lib().gpdb_detect_batch(self.h, _p(offsets_i32), _p(sidx_i32), C.byref(res), _p(cand_offsets_i32)))
 
     def set_samples(self, samples):
         """Cloud::setSamples: arbitrary float64 positions [n, 3]; returns the sample indices that address them."""

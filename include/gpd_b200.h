@@ -216,6 +216,37 @@ int gpdb_detect_select(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n_sampl
 int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n_samples, uint8_t *d_flags_out,
                          float *d_scores_out, gpdb_result *stats);
 
+/* --- batches of clouds: many small scenes (views of objects, dataset evaluation, multi-camera cells) in one call -------
+ * gpdb_set_clouds installs B processed clouds, concatenated: cloud b owns the points point_offsets[b] ..
+ * point_offsets[b+1] - 1 of xyz (3 floats per point) and normals (3 doubles per point), its own n_cameras[b] = K_b <= 8
+ * cameras (view_points: the 3 x K_b blocks of the clouds one after the other) and camera sources (cam_source: the
+ * N_b x K_b int32 blocks one after the other, entries > 0 = seen, as gpdb_set_cloud; NULL = every camera sees every point).
+ * Every cloud gets its own neighbour grid on the device; the batch is held beside the single cloud, and gpdb_set_cloud,
+ * gpdb_preprocess, gpdb_detect and every other entry point behave as before whatever batch is installed. Empty clouds,
+ * K_b outside 1..8, non-finite coordinates and malformed offsets are GPDB_ERR_INVALID; a failed call leaves no batch.
+ * Returns B. Sample positions (gpdb_set_samples) do not apply to a batch: called while only a batch is installed,
+ * gpdb_set_samples is GPDB_ERR_INVALID. Preprocessing stays per cloud (gpdb_preprocess + gpdb_get_cloud). */
+int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
+                    const int32_t *cam_source, const int32_t *n_cameras, const double *view_points);
+
+/* gpdb_detect over every cloud of the batch in ONE call: sample_idx holds indices LOCAL to each cloud in CSR form (cloud b:
+ * sample_idx[sample_offsets[b] .. sample_offsets[b+1]), an empty range is allowed). The result is one gpdb_result in
+ * concatenated sample order: frames, flags and scores per sample of the whole stream; candidates (and images with
+ * keep_images) grouped by cloud, cloud b's at cand_offsets_out[b] .. cand_offsets_out[b+1] - 1. Pose records carry the
+ * cloud-local sample_index and sample_slot, so each cloud's slice equals gpdb_detect on that cloud alone, bit for bit.
+ * sample_offsets and cand_offsets_out hold B + 1 entries for the B clouds of the installed batch (the call takes no
+ * count: the caller keeps it from gpdb_set_clouds). A local index outside its cloud or malformed offsets:
+ * GPDB_ERR_INVALID; a neighbourhood beyond the last tier anywhere: GPDB_ERR_CAPACITY for the whole call. The image limits of gpdb_detect apply to the largest K_b of the batch. */
+int gpdb_detect_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out,
+                      int32_t *cand_offsets_out);
+
+/* gpdb_detect_select applied to every cloud of the batch: the num_selected best candidates of each cloud (descending score,
+ * ties in (sample slot, pose slot) order), chosen by one stable sort on the device; only they cross PCIe. Cloud b's
+ * records are out->candidates[sel_offsets_out[b] .. sel_offsets_out[b+1]); out->n_total_candidates counts the classified
+ * candidates of all clouds. */
+int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, int32_t num_selected,
+                             gpdb_result *out, int32_t *sel_offsets_out);
+
 /* Run all work of this context on an existing CUDA stream (cudaStream_t passed as void*), e.g. the
  * host framework's current stream, instead of the context's own stream. */
 int gpdb_set_stream(gpdb_ctx *ctx, void *cuda_stream);
