@@ -342,6 +342,7 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->d_bxyz);
   cudaFree(ctx->d_bnrm);
   cudaFree(ctx->d_bcam);
+  cudaFree(ctx->d_bsrc);
   cudaFree(ctx->d_bcell_start);
   cudaFree(ctx->d_bdesc);
   cudaFree(ctx->d_bsoff);
@@ -1098,6 +1099,44 @@ static int run_pipeline(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpd
 }
 static int check_state(gpdb_ctx *ctx, bool need_cloud, bool need_weights) { return gpdb_check_state(ctx, need_cloud, need_weights); }
 
+// Batch arenas, grow-only like the cloud arrays: points (pts4 / xyz / nrm / cam / src) and per-cloud tables.
+int gpdb_batch_reserve(gpdb_ctx *ctx, size_t N, int n_clouds) {
+  if (N > ctx->bcloud_cap) {
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(ctx->d_bpts4); ctx->d_bpts4 = nullptr;
+    cudaFree(ctx->d_bxyz); ctx->d_bxyz = nullptr;
+    cudaFree(ctx->d_bnrm); ctx->d_bnrm = nullptr;
+    cudaFree(ctx->d_bcam); ctx->d_bcam = nullptr;
+    cudaFree(ctx->d_bsrc); ctx->d_bsrc = nullptr;
+    ctx->bcloud_cap = 0;
+    const size_t cap = N + N / 8 + 1024;
+    CUDA_TRY(cudaMalloc(&ctx->d_bpts4, sizeof(float4) * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bxyz, sizeof(float) * 3 * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bnrm, sizeof(double) * 3 * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bcam, cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bsrc, sizeof(int) * cap));
+    ctx->bcloud_cap = cap;
+  }
+  if ((size_t)n_clouds + 1 > ctx->bdesc_cap) {
+    cudaFree(ctx->d_bdesc); ctx->d_bdesc = nullptr;
+    cudaFree(ctx->d_bsoff); ctx->d_bsoff = nullptr;
+    free(ctx->b_off); ctx->b_off = nullptr;
+    free(ctx->b_sel); ctx->b_sel = nullptr;
+    ctx->bdesc_cap = 0;
+    const size_t cap = (size_t)n_clouds + 1 + n_clouds / 4;
+    CUDA_TRY(cudaMalloc(&ctx->d_bdesc, sizeof(CloudDesc) * cap));
+    CUDA_TRY(cudaMalloc(&ctx->d_bsoff, sizeof(int) * cap));
+    ctx->b_off = (int *)malloc(sizeof(int) * cap);
+    ctx->b_sel = (int *)malloc(sizeof(int) * cap);
+    if (!ctx->b_off || !ctx->b_sel) {
+      gpdb_set_error(ctx, GPDB_ERR_CUDA, "batch of clouds: host allocation failed");
+      return GPDB_ERR_CUDA;
+    }
+    ctx->bdesc_cap = cap;
+  }
+  return GPDB_OK;
+}
+
 extern "C" {
 
 int gpdb_detect(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_result *out) {
@@ -1191,37 +1230,11 @@ int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offset
     cs += (size_t)D.N * D.K;
     D.all_seen = all_seen ? 1 : 0;
   }
-  // grow-only arenas
-  if ((size_t)N > ctx->bcloud_cap) {
-    cudaFree(ctx->d_bpts4); ctx->d_bpts4 = nullptr;
-    cudaFree(ctx->d_bxyz); ctx->d_bxyz = nullptr;
-    cudaFree(ctx->d_bnrm); ctx->d_bnrm = nullptr;
-    cudaFree(ctx->d_bcam); ctx->d_bcam = nullptr;
-    ctx->bcloud_cap = 0;
-    const size_t cap = (size_t)N + N / 8 + 1024;
-    CUDA_TRY(cudaMalloc(&ctx->d_bpts4, sizeof(float4) * cap));
-    CUDA_TRY(cudaMalloc(&ctx->d_bxyz, sizeof(float) * 3 * cap));
-    CUDA_TRY(cudaMalloc(&ctx->d_bnrm, sizeof(double) * 3 * cap));
-    CUDA_TRY(cudaMalloc(&ctx->d_bcam, cap));
-    ctx->bcloud_cap = cap;
+  {
+    int rc = gpdb_batch_reserve(ctx, (size_t)N, n_clouds);
+    if (rc != GPDB_OK) return rc;
   }
-  if ((size_t)n_clouds + 1 > ctx->bdesc_cap) {
-    cudaFree(ctx->d_bdesc); ctx->d_bdesc = nullptr;
-    cudaFree(ctx->d_bsoff); ctx->d_bsoff = nullptr;
-    free(ctx->b_off); ctx->b_off = nullptr;
-    free(ctx->b_sel); ctx->b_sel = nullptr;
-    ctx->bdesc_cap = 0;
-    const size_t cap = (size_t)n_clouds + 1 + n_clouds / 4;
-    CUDA_TRY(cudaMalloc(&ctx->d_bdesc, sizeof(CloudDesc) * cap));
-    CUDA_TRY(cudaMalloc(&ctx->d_bsoff, sizeof(int) * cap));
-    ctx->b_off = (int *)malloc(sizeof(int) * cap);
-    ctx->b_sel = (int *)malloc(sizeof(int) * cap);
-    if (!ctx->b_off || !ctx->b_sel) {
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "gpdb_set_clouds: host allocation failed");
-      return GPDB_ERR_CUDA;
-    }
-    ctx->bdesc_cap = cap;
-  }
+  ctx->b_has_src = false;
   CUDA_TRY(cudaMemcpyAsync(ctx->d_bxyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(ctx->d_bnrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(ctx->d_bcam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
@@ -1241,6 +1254,180 @@ int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offset
   memcpy(ctx->b_off, point_offsets, sizeof(int) * ((size_t)n_clouds + 1));
   ctx->b_maxk = maxk;
   return n_clouds;
+}
+
+}  // extern "C"
+
+// gpdb_preprocess_clouds after the argument checks; the caller drops the batch when this fails
+static int preprocess_clouds(gpdb_ctx *ctx, int32_t B, const int32_t *roff, const float *xyz, const double *normals,
+                             const int32_t *cam_source, const int32_t *n_cameras, const double *view_points,
+                             const gpdb_preprocess_params *pp, int32_t *poff, cudaEvent_t ev[6]) {
+  const int M = roff[B];
+  // ---- camera masks, packed per cloud with its own K_b (gpdb_preprocess: a camera sees a point when its entry is 1)
+  std::vector<uint8_t> cam((size_t)M);
+  std::vector<CloudDesc> desc((size_t)B);
+  size_t cs = 0, vs = 0;  // running offsets into cam_source (N_b x K_b blocks) and view_points (3 x K_b blocks)
+  int maxk = 0;
+  for (int b = 0; b < B; b++) {
+    CloudDesc &D = desc[b];
+    memset(&D, 0, sizeof(D));
+    D.K = n_cameras[b];
+    maxk = std::max(maxk, D.K);
+    for (int k = 0; k < D.K; k++)
+      for (int r = 0; r < 3; r++) D.vp[k][r] = view_points[vs + 3 * k + r];
+    vs += 3 * (size_t)D.K;
+    D.all_seen = cam_source ? 0 : 1;  // as gpdb_preprocess
+    const int nb = roff[b + 1] - roff[b];
+    for (int i = 0; i < nb; i++) {
+      uint8_t m = (uint8_t)((1u << D.K) - 1);
+      if (cam_source) {
+        m = 0;
+        for (int k = 0; k < D.K; k++) {
+          const int32_t v = cam_source[cs + (size_t)i * D.K + k];
+          if (!pp->voxelize && v != 0 && v != 1) {
+            gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: cloud %d: cam_source[%d][%d] = %d; without "
+                           "voxelisation entries must be 0 or 1", b, i, k, (int)v);
+            return GPDB_ERR_INVALID;
+          }
+          if (v == 1) m |= (uint8_t)(1u << k);
+        }
+      }
+      cam[(size_t)roff[b] + i] = m;
+    }
+    cs += (size_t)nb * D.K;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  // ---- one upload of the concatenated raw arrays
+  const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
+  unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, 7, raw_bytes);
+  if (!raw) return GPDB_ERR_CUDA;
+  double *d_nrm_raw = normals ? (double *)raw : nullptr;
+  float *d_xyz_raw = (float *)(raw + (normals ? sizeof(double) * 3 * (size_t)M : 0));
+  uint8_t *d_cam_raw = (uint8_t *)(d_xyz_raw + 3 * (size_t)M);
+  cudaEventRecord(ev[0], ctx->stream);
+  CUDA_TRY(cudaMemcpyAsync(d_xyz_raw, xyz, sizeof(float) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_cam_raw, cam.data(), (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+  if (normals) CUDA_TRY(cudaMemcpyAsync(d_nrm_raw, normals, sizeof(double) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+  cudaEventRecord(ev[1], ctx->stream);
+  // ---- removeNans + filterWorkspace + voxelizeCloud of every cloud, into the batch arenas
+  int rc = pre_filter_voxelize_batch(ctx, d_xyz_raw, d_cam_raw, d_nrm_raw, M, B, roff, *pp, poff, ev[2]);
+  if (rc != GPDB_OK) return rc;
+  cudaEventRecord(ev[3], ctx->stream);
+  // ---- install as the batch (as gpdb_set_clouds), one grid per cloud
+  const int N = poff[B];
+  for (int b = 0; b < B; b++) {
+    desc[b].off = poff[b];
+    desc[b].N = poff[b + 1] - poff[b];
+  }
+  CUDA_TRY(cudaMemcpyAsync(ctx->d_bdesc, desc.data(), sizeof(CloudDesc) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+  ctx->bcloud.pts4 = ctx->d_bpts4;
+  ctx->bcloud.xyz = ctx->d_bxyz;
+  ctx->bcloud.nrm = ctx->d_bnrm;
+  ctx->bcloud.cam = ctx->d_bcam;
+  ctx->bcloud.samples = nullptr;
+  ctx->bcloud.n_points = N;
+  ctx->b_n = B;
+  memcpy(ctx->b_off, poff, sizeof(int) * ((size_t)B + 1));
+  ctx->b_maxk = maxk;
+  rc = geo_build_grid_batch(ctx, N);
+  if (rc != GPDB_OK) return rc;
+  cudaEventRecord(ev[4], ctx->stream);
+  // ---- calculateNormalsOMP + reverseNormals, every cloud against its own grid; then the per-cloud nonunit flags (the
+  // grid build derived them from normals that did not exist yet)
+  if (pp->estimate_normals) {
+    rc = pre_normals_batch(ctx, pp->normals_radius);
+    if (rc != GPDB_OK) return rc;
+  }
+  rc = pre_nonunit_batch(ctx);
+  if (rc != GPDB_OK) return rc;
+  cudaEventRecord(ev[5], ctx->stream);
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  memset(ctx->pre_ms, 0, sizeof(ctx->pre_ms));
+  float t;
+  for (int i = 0; i < 5; i++)
+    if (cudaEventElapsedTime(&t, ev[i], ev[i + 1]) == cudaSuccess) ctx->pre_ms[i] = t;
+  if (cudaEventElapsedTime(&t, ev[0], ev[5]) == cudaSuccess) ctx->pre_ms[5] = t;
+  ctx->b_has_src = true;
+  return B;
+}
+
+extern "C" {
+
+int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
+                           const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
+                           const double *view_points, const gpdb_preprocess_params *pp, int32_t *processed_offsets_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  ctx->b_n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
+  ctx->b_has_src = false;
+  if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || !pp || !processed_offsets_out ||
+      point_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, "
+                   "xyz, view_points, params, processed_offsets_out");
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < n_clouds; b++) {
+    if (point_offsets[b + 1] <= point_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: raw cloud %d has %d points (offsets must increase)", b,
+                     point_offsets[b + 1] - point_offsets[b]);
+      return GPDB_ERR_INVALID;
+    }
+    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: cloud %d has %d cameras (1 <= cameras <= %d)", b,
+                     n_cameras[b], GPDB_MAX_CAMERAS);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  if (!pp->estimate_normals && !normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: estimate_normals = 0 needs the caller's normals");
+    return GPDB_ERR_INVALID;
+  }
+  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: voxel_size and normals_radius must be positive");
+    return GPDB_ERR_INVALID;
+  }
+  cudaEvent_t ev[6] = {};
+  for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
+  const int rc = preprocess_clouds(ctx, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
+                                   processed_offsets_out, ev);
+  for (auto &e : ev) cudaEventDestroy(e);
+  if (rc < 0) {
+    ctx->b_n = 0;
+    ctx->b_has_src = false;
+  }
+  return rc;
+}
+
+int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out, int32_t *src_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (ctx->b_n == 0) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_get_clouds: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first");
+    return GPDB_ERR_STATE;
+  }
+  if (src_out && !ctx->b_has_src) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_get_clouds: source indices exist after gpdb_preprocess_clouds only");
+    return GPDB_ERR_STATE;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const int B = ctx->b_n;
+  const size_t N = (size_t)ctx->b_off[B];
+  if (xyz_out) CUDA_TRY(cudaMemcpyAsync(xyz_out, ctx->d_bxyz, sizeof(float) * 3 * N, cudaMemcpyDeviceToHost, ctx->stream));
+  if (normals_out) CUDA_TRY(cudaMemcpyAsync(normals_out, ctx->d_bnrm, sizeof(double) * 3 * N, cudaMemcpyDeviceToHost, ctx->stream));
+  if (src_out) CUDA_TRY(cudaMemcpyAsync(src_out, ctx->d_bsrc, sizeof(int) * N, cudaMemcpyDeviceToHost, ctx->stream));
+  std::vector<uint8_t> cam(cam_source_out ? N : 0);
+  std::vector<CloudDesc> desc(cam_source_out ? (size_t)B : 0);
+  if (cam_source_out) {  // the masks expanded on the host: each cloud has its own camera count
+    CUDA_TRY(cudaMemcpyAsync(cam.data(), ctx->d_bcam, N, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(desc.data(), ctx->d_bdesc, sizeof(CloudDesc) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (cam_source_out) {
+    size_t o = 0;
+    for (int b = 0; b < B; b++)
+      for (int i = ctx->b_off[b]; i < ctx->b_off[b + 1]; i++)
+        for (int k = 0; k < desc[b].K; k++) cam_source_out[o++] = (cam[i] >> k) & 1;
+  }
+  return (int)N;
 }
 
 }  // extern "C"

@@ -197,6 +197,8 @@ struct gpdb_ctx {
   int b_n, b_maxk;    // clouds installed (0: none), largest camera count
   int *b_off;         // host copy of the point offsets [b_n + 1]
   int *b_sel;         // host: per-cloud offsets of the last batch selection [b_n + 1]
+  int *d_bsrc;        // cloud-local raw index of each point (valid after gpdb_preprocess_clouds: b_has_src)
+  bool b_has_src;
   CloudTable run;     // n > 0 while a batch call runs: the geometry launchers use the batch instantiations
 };
 
@@ -256,6 +258,13 @@ int pre_filter_voxelize(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_
 int pre_normals(gpdb_ctx *ctx, double radius);
 int pre_nonunit(gpdb_ctx *ctx);
 int pre_cam_expand(gpdb_ctx *ctx, int *d_out);
+// (re)allocates the batch arenas for at least n points and n_clouds clouds (api.cu)
+int gpdb_batch_reserve(gpdb_ctx *ctx, size_t n, int n_clouds);
+// filters + voxelises a raw batch into the batch arenas (reserved inside); poff[B+1] (host) = processed offsets
+int pre_filter_voxelize_batch(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_cam_raw, const double *d_nrm_raw, int M,
+                              int B, const int *roff, const gpdb_preprocess_params &pp, int *poff, cudaEvent_t ev_filter_done);
+int pre_normals_batch(gpdb_ctx *ctx, double radius);  // normals of the installed batch (grids built)
+int pre_nonunit_batch(gpdb_ctx *ctx);                 // per-cloud nonunit flags of the installed batch, in the descriptors
 
 // lenet_simt.cu
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);

@@ -2872,17 +2872,10 @@ __device__ __forceinline__ int b_f2ord(float f) {  // order-preserving int image
   int i = __float_as_int(f);
   return i >= 0 ? i : i ^ 0x7fffffff;
 }
-// the cloud holding concatenated point g: largest b with d[b].off <= g (clouds are not empty)
-__device__ __forceinline__ int b_cloud_of_point(const CloudDesc *d, int B, int g) {
-  int lo = 0, hi = B;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (d[mid].off <= g) lo = mid; else hi = mid;
-  }
-  return lo;
-}
 // one CTA per cloud: bounds, then the grid geo_build_grid derives from them (same float32 steps), and whether any normal
-// is off unit length (pre_nonunit). ncell[b] = cells of cloud b.
+// is off unit length (pre_nonunit). ncell[b] = cells of cloud b. A cloud without points (gpdb_preprocess_clouds keeps a
+// view the filter emptied) gets the grid of bounds 0..0: 2 x 2 x 2 cells that no search reads, since no sample and no
+// point belongs to it (b_cloud_of_point passes over it).
 __global__ void __launch_bounds__(256) k_batch_desc(const float *xyz, const double *nrm, CloudDesc *d, long long *ncell) {
   __shared__ int s_mn[3], s_mx[3], s_nonunit;
   CloudDesc &D = d[blockIdx.x];
@@ -2917,8 +2910,8 @@ __global__ void __launch_bounds__(256) k_batch_desc(const float *xyz, const doub
   if (threadIdx.x != 0) return;
   float lo[3], hi[3];
   for (int a = 0; a < 3; a++) {
-    lo[a] = __int_as_float(s_mn[a] >= 0 ? s_mn[a] : s_mn[a] ^ 0x7fffffff);
-    hi[a] = __int_as_float(s_mx[a] >= 0 ? s_mx[a] : s_mx[a] ^ 0x7fffffff);
+    lo[a] = D.N > 0 ? __int_as_float(s_mn[a] >= 0 ? s_mn[a] : s_mn[a] ^ 0x7fffffff) : 0.0f;
+    hi[a] = D.N > 0 ? __int_as_float(s_mx[a] >= 0 ? s_mx[a] : s_mx[a] ^ 0x7fffffff) : 0.0f;
   }
   float cell = 0.02f;
   double nc;
@@ -3336,18 +3329,20 @@ int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
   if (!cid) return GPDB_ERR_CUDA;
   int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
   const int tb = 256, gb = (N + tb - 1) / tb;
-  k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bdesc, B, N, cid, idx, ctx->d_bcell_start);
-  LAUNCH_CHECK();
   size_t tmp2 = 0;
   tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream);
   cub::DeviceScan::InclusiveSum(nullptr, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream);
   tmp = gpdb_scratch(ctx, 1, std::max(tmp_bytes, tmp2));
   if (!tmp) return GPDB_ERR_CUDA;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream));
-  ctx->launches += 4;
-  k_batch_fill_sorted<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, idx2, ctx->d_bdesc, B, N, ctx->d_bpts4);
-  LAUNCH_CHECK();
+  if (N > 0) {  // a preprocessed batch may hold no point at all (every view filtered out)
+    k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bdesc, B, N, cid, idx, ctx->d_bcell_start);
+    LAUNCH_CHECK();
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream));
+    ctx->launches += 4;
+    k_batch_fill_sorted<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, idx2, ctx->d_bdesc, B, N, ctx->d_bpts4);
+    LAUNCH_CHECK();
+  }
   CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream));
   ctx->launches += 2;
   ctx->bcloud.cell_start = ctx->d_bcell_start;

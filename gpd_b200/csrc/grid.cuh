@@ -46,6 +46,29 @@ struct CloudSel<true> {
     return t.d[lo];
   }
 };
+// the cloud holding concatenated point g: largest b with d[b].off <= g. A cloud without points shares its offset with the
+// next cloud, so the search passes over it to the cloud that holds g.
+__device__ __forceinline__ int b_cloud_of_point(const CloudDesc *d, int B, int g) {
+  int lo = 0, hi = B;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (d[mid].off <= g) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+// The cloud of a concatenated point (kernels with one thread or warp per point). Single cloud: DevParams, offset 0.
+template <bool BATCH>
+struct PointSel {
+  static __device__ __forceinline__ const DevParams &get(const DevParams &P, const CloudTable &, int) { return P; }
+};
+template <>
+struct PointSel<true> {
+  static __device__ __forceinline__ const CloudDesc &get(const DevParams &, const CloudTable &t, int g) {
+    return t.d[b_cloud_of_point(t.d, t.n, g)];
+  }
+};
+__device__ __forceinline__ int cloud_off(const DevParams &) { return 0; }
+__device__ __forceinline__ int cloud_off(const CloudDesc &D) { return D.off; }
 // The arrays of that cloud: indices (sample indices, pts4 w bits) are local to it; pts4 positions and cell_start values
 // stay batch-wide.
 __device__ __forceinline__ DevCloud local_cloud(const DevParams &, const DevCloud &cl) { return cl; }

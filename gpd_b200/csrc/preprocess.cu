@@ -255,10 +255,14 @@ __device__ void pcl_eigen33_smallest(const float cov[3][3], float *evec) {
 // (arrival positions grouped by bucket) + 2 B pad, rk u16[cap] (rank of each arrival position). Once the ranks are
 // known, keys / grp / pad are dead and receive the coordinates IN SORTED ORDER (sx, sy over the keys, sz over grp + pad),
 // so that the ordered accumulation reads three plain arrays sequentially (16-byte loads, no index chain).
-template <int WARPS, int NB>
-__global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, DevCloud cl, int N, float r2, float rf,
-                                                        int cap, double *nrm_out, int *ovf, int *ovf_count, int tier,
-                                                        int *err) {
+// BATCH: one warp per point of the concatenated batch (N = all points); the warp resolves its cloud and works on that
+// cloud's arrays, grid, view points and cameras only. The batch pts4 carries cloud-local indices in its w bits, so the
+// (dist, index) keys, their order and the float32 sums are those of a single-cloud run. `ovf` and `nrm_out` are indexed
+// by concatenated point.
+template <int WARPS, int NB, bool BATCH>
+__global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, DevCloud cl0, CloudTable tab, int N, float r2,
+                                                        float rf, int cap, double *nrm_out, int *ovf, int *ovf_count,
+                                                        int tier, int *err) {
   const DevParams &P = *Pp;
   extern __shared__ __align__(16) unsigned char nrm_dyn[];
   __shared__ int s_hist[WARPS][2 * NB + 1];
@@ -272,16 +276,19 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
   float *sz = reinterpret_cast<float *>(grp);                       // sorted z [cap] (over grp + pad)
   int *hist = s_hist[warp];      // [0..NB]: bucket starts after the scan
   int *fill = hist + NB + 1;     // [0..NB): per-bucket cursor of the grouping pass
-  int i;
+  int g;  // concatenated point
   if (tier == 0) {
-    i = blockIdx.x * WARPS + warp;
-    if (i >= N) return;
+    g = blockIdx.x * WARPS + warp;
+    if (g >= N) return;
   } else {
     if ((int)blockIdx.x >= *ovf_count) return;
-    i = ovf[blockIdx.x];
+    g = ovf[blockIdx.x];
   }
+  const auto &G = PointSel<BATCH>::get(P, tab, g);
+  const DevCloud cl = local_cloud(G, cl0);
+  const int i = g - cloud_off(G);  // index in its cloud
   const uint8_t camm = cl.cam[i];
-  double *out = nrm_out + 3 * (size_t)i;
+  double *out = nrm_out + 3 * (size_t)g;
   if (camm == 0) {  // seen by no camera: the reference leaves the column uninitialised; specified as 0
     if (lane < 3) out[lane] = 0.0;
     return;
@@ -290,11 +297,11 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
   __syncwarp();
   const float q[3] = {cl.xyz[3 * (size_t)i], cl.xyz[3 * (size_t)i + 1], cl.xyz[3 * (size_t)i + 2]};
   const float bscale = (float)NB / r2;
-  const SegRange sr = seg_range(P, q, rf);
+  const SegRange sr = seg_range(G, q, rf);
   int cnt = 0;
   for (int j0 = 0; j0 < sr.nrows; j0 += 32) {
     int st = 0, len = 0;
-    if (j0 + lane < sr.nrows) seg_row(P, cl.cell_start, sr, j0 + lane, st, len);
+    if (j0 + lane < sr.nrows) seg_row(G, cl.cell_start, sr, j0 + lane, st, len);
     unsigned nonempty = __ballot_sync(0xffffffffu, len > 0);
     while (nonempty) {
       const int j = __ffs(nonempty) - 1;
@@ -330,7 +337,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
   }
   if (cnt > cap) {
     if (lane == 0) {
-      if (tier == 0) ovf[atomicAdd(ovf_count, 1)] = i;
+      if (tier == 0) ovf[atomicAdd(ovf_count, 1)] = g;
       else atomicAdd(err + 4, 1);
     }
     if (tier == 0) return;
@@ -421,7 +428,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
     pcl_eigen33_smallest(cov, n);
     // flipNormalTowardsViewpoint, float32, view point of the first camera that sees the point
     const int camera = __ffs((unsigned)camm) - 1;
-    const float vx = (float)P.vp[camera][0] - q[0], vy = (float)P.vp[camera][1] - q[1], vz = (float)P.vp[camera][2] - q[2];
+    const float vx = (float)G.vp[camera][0] - q[0], vy = (float)G.vp[camera][1] - q[1], vz = (float)G.vp[camera][2] - q[2];
     const float cos_theta = vx * n[0] + vy * n[1] + vz * n[2];
     if (cos_theta < 0) {
       n[0] *= -1;
@@ -432,9 +439,9 @@ __global__ void __launch_bounds__(WARPS * 32) k_normals(const DevParams *Pp, Dev
   if (lane != 0) return;
   double nd[3] = {(double)n[0], (double)n[1], (double)n[2]};
   bool needs_reverse = true;
-  for (int j = 0; j < P.K; j++)
+  for (int j = 0; j < G.K; j++)
     if ((camm >> j) & 1) {
-      const double d0 = (double)q[0] - P.vp[j][0], d1 = (double)q[1] - P.vp[j][1], d2 = (double)q[2] - P.vp[j][2];
+      const double d0 = (double)q[0] - G.vp[j][0], d1 = (double)q[1] - G.vp[j][1], d2 = (double)q[2] - G.vp[j][2];
       if (nd[0] * d0 + nd[1] * d1 + nd[2] * d2 < 0) {
         needs_reverse = false;
         break;
@@ -460,6 +467,164 @@ __global__ void k_cam_expand(const uint8_t *cam, int N, int K, int *out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   for (int k = 0; k < K; k++) out[(size_t)i * K + k] = (cam[i] >> k) & 1;
+}
+
+// ---- batches of raw clouds (gpdb_preprocess_clouds) --------------------------------------------------------
+// Every cloud goes through the steps above on its own: the filter keeps the clouds contiguous (the compaction preserves
+// order), the voxel sort orders by (cloud, voxel key, index), each cloud's voxels are emitted with its own minimum, and
+// src is an index into the cloud's own raw points.
+
+// largest b < B with off[b] <= k: the cloud of point k of a concatenation (an emptied cloud repeats its successor's offset)
+__device__ __forceinline__ int seg_of(const int *off, int B, int k) {
+  int lo = 0, hi = B;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= k) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+// filtered offsets: the exclusive scan of the filter flags (M + 1 entries) read at the raw offsets; bounds reset
+__global__ void k_bpre_offsets(const int *pos, const int *roff, int B, int *foff, int *bounds) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > B) return;
+  foff[b] = pos[roff[b]];
+  if (b < B)
+    for (int a = 0; a < 3; a++) {
+      bounds[6 * b + a] = INT_MAX;
+      bounds[6 * b + 3 + a] = INT_MIN;
+    }
+}
+// pcl::getMinMax3D of every cloud, bounds[6b .. 6b+5] as k_bounds: blockIdx.x = cloud, the gridDim.y CTAs of a cloud
+// share its points, so that one large view among small ones is reduced by many SMs, not one
+__global__ void __launch_bounds__(256) k_bpre_bounds(const float *xyz1, const int *foff, int *bounds) {
+  __shared__ int s_b[6];
+  const int b = blockIdx.x;
+  if (threadIdx.x < 6) s_b[threadIdx.x] = threadIdx.x < 3 ? INT_MAX : INT_MIN;
+  __syncthreads();
+  int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
+  const int end = foff[b + 1];
+  for (int i = foff[b] + blockIdx.y * blockDim.x + threadIdx.x; i < end; i += gridDim.y * blockDim.x)
+    for (int a = 0; a < 3; a++) {
+      const int o = f2ord(xyz1[3 * (size_t)i + a]);
+      mn[a] = min(mn[a], o);
+      mx[a] = max(mx[a], o);
+    }
+  for (int a = 0; a < 3; a++) {
+    mn[a] = __reduce_min_sync(0xffffffffu, mn[a]);
+    mx[a] = __reduce_max_sync(0xffffffffu, mx[a]);
+  }
+  if ((threadIdx.x & 31) == 0)
+    for (int a = 0; a < 3; a++) {
+      atomicMin(s_b + a, mn[a]);
+      atomicMax(s_b + 3 + a, mx[a]);
+    }
+  __syncthreads();
+  if (threadIdx.x < 3) atomicMin(bounds + 6 * b + threadIdx.x, s_b[threadIdx.x]);
+  else if (threadIdx.x < 6) atomicMax(bounds + 6 * b + threadIdx.x, s_b[threadIdx.x]);
+}
+// k_vox_keys with the cloud's own minimum; cl_of[k] = cloud of filtered point k; err[0] counts out-of-range voxel
+// indices, err[1] = the first cloud that has one
+__global__ void k_bvox_keys(const float *xyz1, int n, const int *foff, int B, const int *bounds, float cell,
+                            unsigned long long *keys, int *vals, int *cl_of, int *err) {
+  int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int b = seg_of(foff, B, k);
+  unsigned long long key = 0;
+  for (int a = 0; a < 3; a++) {
+    int c = voxel_of(xyz1[3 * (size_t)k + a], ord2f(bounds[6 * b + a]), cell);
+    if (c < 0 || c >= (1 << 21)) {
+      atomicAdd(err, 1);
+      atomicMin(err + 1, b);
+      c = max(0, min(c, (1 << 21) - 1));
+    }
+    key = (key << 21) | (unsigned long long)c;
+  }
+  keys[k] = key;
+  vals[k] = k;
+  cl_of[k] = b;
+}
+// the cloud of each entry after the (stable) key sort: the key of the second sort
+__global__ void k_bvox_cloud_keys(const int *vals, const int *cl_of, int n, unsigned *ck) {
+  int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < n) ck[s] = (unsigned)cl_of[vals[s]];
+}
+// run heads in (cloud, key, index) order: a new voxel where the cloud OR the key changes (two clouds may share a key)
+__global__ void k_bvox_heads(const unsigned long long *keys, const int *vals, const unsigned *ck, int n, int *head) {
+  int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  head[s] = (s == 0 || ck[s] != ck[s - 1] || keys[vals[s]] != keys[vals[s - 1]]) ? 1 : 0;
+}
+// k_vox_groups with the cloud above the descending-first-index key
+__global__ void k_bvox_groups(const int *head, const int *gid_incl, const int *vals, const unsigned *ck, int n, int *gfirst,
+                              int *gbegin, unsigned long long *gorder_key, int *gorder_val) {
+  int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || !head[s]) return;
+  int g = gid_incl[s] - 1;
+  gfirst[g] = vals[s];
+  gbegin[g] = s;
+  gorder_key[g] = ((unsigned long long)ck[s] << 32) | (0x7fffffffu - (unsigned)vals[s]);
+  gorder_val[g] = g;
+}
+// processed offsets: cloud b's sorted entries are foff[b] .. foff[b+1]-1, so its voxels start after the heads before foff[b]
+__global__ void k_bvox_offsets(const int *gid_incl, const int *foff, int B, int *poff) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b <= B) poff[b] = foff[b] == 0 ? 0 : gid_incl[foff[b] - 1];
+}
+// k_vox_emit per cloud: the corner from the cloud's minimum, src local to the cloud's raw points, and the normal run walk
+// bounded by the cloud's sorted range
+__global__ void k_bvox_emit(const int *gsorted, const unsigned long long *gkeys, int U, const int *gfirst, const int *gbegin,
+                            const int *vals, const unsigned long long *keys, const int *foff, const int *roff, const int *keep,
+                            const float *xyz1, const int *bounds, float cell, const uint8_t *cam_in, const double *nrm_in,
+                            float *xyz_out, uint8_t *cam_out, double *nrm_out, int *src_out) {
+  int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= U) return;
+  const int g = gsorted[o], b = (int)(gkeys[o] >> 32), k = gfirst[g], i = keep[k];
+  for (int a = 0; a < 3; a++) {
+    const float mn = ord2f(bounds[6 * b + a]);
+    const int c = voxel_of(xyz1[3 * (size_t)k + a], mn, cell);
+    const float t = cell * (float)c;
+    xyz_out[3 * (size_t)o + a] = mn + t;
+  }
+  cam_out[o] = cam_in[i];
+  src_out[o] = i - roff[b];
+  if (nrm_in) {
+    double acc[3] = {0.0, 0.0, 0.0};
+    const unsigned long long key = keys[vals[gbegin[g]]];
+    const int end = foff[b + 1];
+    int s = gbegin[g];
+    for (; s < end && keys[vals[s]] == key; s++) {
+      const double *nn = nrm_in + 3 * (size_t)keep[vals[s]];
+      acc[0] += nn[0];
+      acc[1] += nn[1];
+      acc[2] += nn[2];
+    }
+    const double cnt = (double)(s - gbegin[g]);
+    nrm_out[3 * (size_t)o] = acc[0] / cnt;
+    nrm_out[3 * (size_t)o + 1] = acc[1] / cnt;
+    nrm_out[3 * (size_t)o + 2] = acc[2] / cnt;
+  }
+}
+// voxelize = 0: the filtered points themselves (k_gather_plain, src local to the cloud)
+__global__ void k_bgather_plain(const int *keep, int n1, const int *foff, const int *roff, int B, const float *xyz1,
+                                const uint8_t *cam_in, const double *nrm_in, float *xyz_out, uint8_t *cam_out, double *nrm_out,
+                                int *src_out) {
+  int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n1) return;
+  const int i = keep[k];
+  for (int a = 0; a < 3; a++) xyz_out[3 * (size_t)k + a] = xyz1[3 * (size_t)k + a];
+  cam_out[k] = cam_in[i];
+  src_out[k] = i - roff[seg_of(foff, B, k)];
+  if (nrm_in)
+    for (int a = 0; a < 3; a++) nrm_out[3 * (size_t)k + a] = nrm_in[3 * (size_t)i + a];
+}
+// per-cloud k_nonunit: the descriptors' flags, cleared first
+__global__ void k_bnonunit_clear(CloudDesc *d, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) d[b].nonunit = 0;
+}
+__global__ void k_bnonunit(const double *nrm, CloudDesc *d, int B, int N) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < N && !unit_normal(nrm + 3 * (size_t)g)) d[b_cloud_of_point(d, B, g)].nonunit = 1;
 }
 
 }  // namespace
@@ -505,9 +670,10 @@ int pre_bounds(gpdb_ctx *ctx, const float *d_xyz, int n, int *d_bounds, float lo
   return GPDB_OK;
 }
 
-// Normal estimation over the installed cloud (ctx->cloud, grid built): writes ctx->d_nrm.
-int pre_normals(gpdb_ctx *ctx, double radius) {
-  const int N = ctx->N;
+// Normal estimation over N points of the cloud cl (grid built; tab.n > 0: a batch whose descriptors hold the grids):
+// writes nrm_out.
+template <bool BATCH>
+static int run_normals(gpdb_ctx *ctx, const DevCloud &cl, const CloudTable &tab, int N, double *nrm_out, double radius) {
   const float r2 = (float)(radius * radius);
   const float rf = (float)radius * 1.0001f + 1e-6f;
   int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * ((size_t)N + 1));
@@ -515,17 +681,17 @@ int pre_normals(gpdb_ctx *ctx, double radius) {
   int *ovf_count = ovf + N;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   const size_t sm1 = (size_t)NRM_WARPS * NRM_CAP1 * NRM_BYTES_PER, sm2 = (size_t)NRM_CAP2 * NRM_BYTES_PER;
-  CUDA_TRY(cudaFuncSetAttribute(k_normals<NRM_WARPS, NRM_NB1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
-  CUDA_TRY(cudaFuncSetAttribute(k_normals<1, NRM_NB2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
-  k_normals<NRM_WARPS, NRM_NB1><<<(N + NRM_WARPS - 1) / NRM_WARPS, NRM_WARPS * 32, sm1, ctx->stream>>>(
-      ctx->dp, ctx->cloud, N, r2, rf, NRM_CAP1, ctx->d_nrm, ovf, ovf_count, 0, ctx->d_err);
+  CUDA_TRY(cudaFuncSetAttribute(k_normals<NRM_WARPS, NRM_NB1, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
+  CUDA_TRY(cudaFuncSetAttribute(k_normals<1, NRM_NB2, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+  k_normals<NRM_WARPS, NRM_NB1, BATCH><<<(N + NRM_WARPS - 1) / NRM_WARPS, NRM_WARPS * 32, sm1, ctx->stream>>>(
+      ctx->dp, cl, tab, N, r2, rf, NRM_CAP1, nrm_out, ovf, ovf_count, 0, ctx->d_err);
   LAUNCH_CHECK();
   int h_ovf = 0;
   CUDA_TRY(cudaMemcpyAsync(&h_ovf, ovf_count, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   if (h_ovf > 0) {
-    k_normals<1, NRM_NB2><<<h_ovf, 32, sm2, ctx->stream>>>(ctx->dp, ctx->cloud, N, r2, rf, NRM_CAP2, ctx->d_nrm, ovf, ovf_count, 1,
-                                                  ctx->d_err);
+    k_normals<1, NRM_NB2, BATCH><<<h_ovf, 32, sm2, ctx->stream>>>(ctx->dp, cl, tab, N, r2, rf, NRM_CAP2, nrm_out, ovf,
+                                                                  ovf_count, 1, ctx->d_err);
     LAUNCH_CHECK();
     int e4 = 0;
     CUDA_TRY(cudaMemcpyAsync(&e4, ctx->d_err + 4, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -538,6 +704,11 @@ int pre_normals(gpdb_ctx *ctx, double radius) {
     }
   }
   return GPDB_OK;
+}
+
+// Normal estimation over the installed cloud (ctx->cloud, grid built): writes ctx->d_nrm.
+int pre_normals(gpdb_ctx *ctx, double radius) {
+  return run_normals<false>(ctx, ctx->cloud, CloudTable{nullptr, nullptr, 0}, ctx->N, ctx->d_nrm, radius);
 }
 
 // Filter + voxelise the raw device arrays into the context's cloud arrays (ctx->d_xyz / d_cam / d_nrm / d_src,
@@ -658,5 +829,142 @@ int pre_nonunit(gpdb_ctx *ctx) {
 int pre_cam_expand(gpdb_ctx *ctx, int *d_out) {
   k_cam_expand<<<(ctx->N + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_cam, ctx->N, ctx->K, d_out);
   LAUNCH_CHECK();
+  return GPDB_OK;
+}
+
+// ---- gpdb_preprocess_clouds --------------------------------------------------------------------------------------------
+// Filter + voxelise the raw batch (M points; cloud b owns raw points roff[b] .. roff[b+1]-1, host offsets) into the batch
+// arenas ctx->d_bxyz / d_bcam / d_bnrm / d_bsrc (reserved here once the output size is known). poff[B+1] (host)
+// receives the processed offsets; a cloud the filter empties keeps its place with no points. d_nrm_raw may be null.
+int pre_filter_voxelize_batch(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_cam_raw, const double *d_nrm_raw, int M,
+                              int B, const int *roff, const gpdb_preprocess_params &pp, int *poff, cudaEvent_t ev_filter_done) {
+  const int tb = 256;
+  // ---- removeNans + filterWorkspace, one scan for all clouds
+  // slot 4: workspace [6 doubles], raw / filtered / processed offsets [B+1 each], bounds [6B], voxel error [2]
+  double *d_ws = (double *)gpdb_scratch(ctx, 4, sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2));
+  if (!d_ws) return GPDB_ERR_CUDA;
+  int *d_roff = (int *)(d_ws + 6), *d_foff = d_roff + B + 1, *d_poff = d_foff + B + 1, *d_bounds = d_poff + B + 1;
+  int *d_verr = d_bounds + 6 * B;
+  const int verr0[2] = {0, INT_MAX};
+  CUDA_TRY(cudaMemcpyAsync(d_ws, pp.workspace, sizeof(double) * 6, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_roff, roff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_verr, verr0, sizeof(verr0), cudaMemcpyHostToDevice, ctx->stream));
+  int *flag = (int *)gpdb_scratch(ctx, 5, sizeof(int) * (3 * (size_t)M + 2) + sizeof(float) * 3 * (size_t)M);
+  if (!flag) return GPDB_ERR_CUDA;
+  int *pos = flag + M + 1, *keep = pos + M + 1;
+  float *xyz1 = (float *)(keep + M);
+  k_pre_flag<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, M, d_ws, flag);
+  LAUNCH_CHECK();
+  CUDA_TRY(cudaMemsetAsync(flag + M, 0, sizeof(int), ctx->stream));  // pos[M] = number of filtered points
+  size_t tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, M + 1, ctx->stream);
+  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  if (!tmp) return GPDB_ERR_CUDA;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, M + 1, ctx->stream));
+  ctx->launches += 2;
+  k_pre_compact<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, flag, pos, M, keep, xyz1);
+  LAUNCH_CHECK();
+  k_bpre_offsets<<<(B + 1 + tb - 1) / tb, tb, 0, ctx->stream>>>(pos, d_roff, B, d_foff, d_bounds);
+  LAUNCH_CHECK();
+  std::vector<int> foff((size_t)B + 1);
+  CUDA_TRY(cudaMemcpyAsync(foff.data(), d_foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  cudaEventRecord(ev_filter_done, ctx->stream);
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  const int M1 = foff[B];
+
+  if (!pp.voxelize || M1 == 0) {
+    memcpy(poff, foff.data(), sizeof(int) * ((size_t)B + 1));
+    int rc = gpdb_batch_reserve(ctx, (size_t)M1, B);
+    if (rc != GPDB_OK || M1 == 0) return rc;
+    k_bgather_plain<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(keep, M1, d_foff, d_roff, B, xyz1, d_cam_raw, d_nrm_raw,
+                                                                ctx->d_bxyz, ctx->d_bcam, ctx->d_bnrm, ctx->d_bsrc);
+    LAUNCH_CHECK();
+    return GPDB_OK;
+  }
+  // ---- voxelizeCloud of every cloud
+  const float cell = (float)pp.voxel_size;
+  int largest = 0;
+  for (int b = 0; b < B; b++) largest = std::max(largest, foff[b + 1] - foff[b]);
+  const int ysplit = std::min(64, std::max(1, (largest + 8191) / 8192));  // ~8 K points per CTA in the largest cloud
+  k_bpre_bounds<<<dim3(B, ysplit), 256, 0, ctx->stream>>>(xyz1, d_foff, d_bounds);
+  LAUNCH_CHECK();
+  // sort buffers: keys x2 (8 B), vals x3, cloud of point, cloud keys x2, head, gid, gfirst, gbegin, group order vals x2
+  // (4 B each), group order keys x2 (8 B)
+  unsigned long long *keys = (unsigned long long *)gpdb_scratch(ctx, 6, (size_t)M1 * (16 + 48 + 16));
+  if (!keys) return GPDB_ERR_CUDA;
+  unsigned long long *keys2 = keys + M1, *gord_k = keys2 + M1, *gord_k2 = gord_k + M1;
+  int *vals = (int *)(gord_k2 + M1), *vals2 = vals + M1, *vals3 = vals2 + M1, *cl_of = vals3 + M1;
+  unsigned *ck = (unsigned *)(cl_of + M1), *ck2 = ck + M1;
+  int *head = (int *)(ck2 + M1), *gid = head + M1, *gfirst = gid + M1, *gbegin = gfirst + M1, *gord_v = gbegin + M1;
+  int *gord_v2 = gord_v + M1;
+  int cloud_bits = 0;
+  while ((1 << cloud_bits) < B) cloud_bits++;
+  k_bvox_keys<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(xyz1, M1, d_foff, B, d_bounds, cell, keys, vals, cl_of, d_verr);
+  LAUNCH_CHECK();
+  size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, t1, keys, keys2, vals, vals2, M1, 0, 63, ctx->stream);
+  if (cloud_bits) cub::DeviceRadixSort::SortPairs(nullptr, t2, ck, ck2, vals2, vals3, M1, 0, cloud_bits, ctx->stream);
+  cub::DeviceScan::InclusiveSum(nullptr, t3, head, gid, M1, ctx->stream);
+  cub::DeviceRadixSort::SortPairs(nullptr, t4, gord_k, gord_k2, gord_v, gord_v2, M1, 0, 32 + cloud_bits, ctx->stream);
+  tmp = gpdb_scratch(ctx, 1, std::max(std::max(t1, t2), std::max(t3, t4)));
+  if (!tmp) return GPDB_ERR_CUDA;
+  // (cloud, key, index) order: the key sort keeps index order among equal keys, the cloud sort keeps key order
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t1, keys, keys2, vals, vals2, M1, 0, 63, ctx->stream));
+  ctx->launches += 9;
+  if (cloud_bits) {
+    k_bvox_cloud_keys<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(vals2, cl_of, M1, ck);
+    LAUNCH_CHECK();
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t2, ck, ck2, vals2, vals3, M1, 0, cloud_bits, ctx->stream));
+    ctx->launches += 5;
+  } else {
+    vals3 = vals2;
+    CUDA_TRY(cudaMemsetAsync(ck2, 0, sizeof(unsigned) * (size_t)M1, ctx->stream));
+  }
+  k_bvox_heads<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(keys, vals3, ck2, M1, head);
+  LAUNCH_CHECK();
+  CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, t3, head, gid, M1, ctx->stream));
+  ctx->launches += 2;
+  k_bvox_groups<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(head, gid, vals3, ck2, M1, gfirst, gbegin, gord_k, gord_v);
+  LAUNCH_CHECK();
+  k_bvox_offsets<<<(B + 1 + tb - 1) / tb, tb, 0, ctx->stream>>>(gid, d_foff, B, d_poff);
+  LAUNCH_CHECK();
+  int verr[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(poff, d_poff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(verr, d_verr, sizeof(verr), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (verr[0]) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "voxelisation: %d points fall outside the 2^21-voxel range, the first in cloud %d "
+                   "(voxel_size %g too small for the cloud extent)", verr[0], verr[1], (double)cell);
+    return GPDB_ERR_INVALID;
+  }
+  const int U = poff[B];
+  // output order: cloud, then descending index of each voxel's first point
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, t4, gord_k, gord_k2, gord_v, gord_v2, U, 0, 32 + cloud_bits, ctx->stream));
+  ctx->launches += 8;
+  int rc = gpdb_batch_reserve(ctx, (size_t)U, B);
+  if (rc != GPDB_OK) return rc;
+  k_bvox_emit<<<(U + tb - 1) / tb, tb, 0, ctx->stream>>>(gord_v2, gord_k2, U, gfirst, gbegin, vals3, keys, d_foff, d_roff, keep,
+                                                         xyz1, d_bounds, cell, d_cam_raw, d_nrm_raw, ctx->d_bxyz, ctx->d_bcam,
+                                                         ctx->d_bnrm, ctx->d_bsrc);
+  LAUNCH_CHECK();
+  return GPDB_OK;
+}
+
+// Normal estimation over the installed batch (ctx->bcloud, grids built): writes ctx->d_bnrm.
+int pre_normals_batch(gpdb_ctx *ctx, double radius) {
+  const int N = ctx->b_off[ctx->b_n];
+  if (N == 0) return GPDB_OK;
+  return run_normals<true>(ctx, ctx->bcloud, CloudTable{ctx->d_bdesc, nullptr, ctx->b_n}, N, ctx->d_bnrm, radius);
+}
+
+// the nonunit flag of every cloud of the installed batch (as pre_nonunit, per cloud), in its descriptor
+int pre_nonunit_batch(gpdb_ctx *ctx) {
+  const int B = ctx->b_n, N = ctx->b_off[B];
+  k_bnonunit_clear<<<(B + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_bdesc, B);
+  LAUNCH_CHECK();
+  if (N > 0) {
+    k_bnonunit<<<(N + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_bnrm, ctx->d_bdesc, B, N);
+    LAUNCH_CHECK();
+  }
   return GPDB_OK;
 }

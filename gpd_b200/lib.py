@@ -24,7 +24,7 @@ EXPORTS = [
     "gpdb_get_cloud", "gpdb_get_cloud_source_index", "gpdb_preprocess_timings", "gpdb_detect_select", "gpdb_load_weights_file", "gpdb_read_weights_file", "gpdb_set_samples",
     "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
-    "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select",
+    "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
 ]
 
 
@@ -88,6 +88,8 @@ def lib():
     L.gpdb_set_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     L.gpdb_detect_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_detect_batch_select.argtypes = [vp, vp, vp, C.c_int32, C.POINTER(abi.Result), vp]
+    L.gpdb_preprocess_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, C.POINTER(abi.PreprocessParams), vp]
+    L.gpdb_get_clouds.argtypes = [vp, vp, vp, vp, vp]
     _LIB = L
     return L
 
@@ -147,13 +149,19 @@ def read_weights_file(weights_file, channels, model_file=None):
 
 
 def pack_clouds(clouds):
-    """The CSR arrays of gpdb_set_clouds for a list of cloud dicts (xyz [N, 3], normals [N, 3], optional cam_source
-    [N, K], optional view_points [K, 3]): point offsets [B+1], xyz, normals, cam_source (None when no cloud has one; a
-    cloud without one is seen by all its cameras), camera counts [B] and view points, each concatenated in cloud order."""
+    """The CSR arrays of gpdb_set_clouds / gpdb_preprocess_clouds for a list of cloud dicts (xyz [N, 3], normals [N, 3],
+    optional cam_source [N, K], optional view_points [K, 3]): point offsets [B+1], xyz, normals (None when no cloud has
+    them, as raw clouds whose normals are estimated; ValueError when only some have them), cam_source (None when no
+    cloud has one; a cloud without one is seen by all its cameras), camera counts [B] and view points, each concatenated
+    in cloud order."""
     if not clouds:
         raise ValueError("pack_clouds: need at least one cloud")
     xyz = [np.asarray(c["xyz"], dtype=np.float32).reshape(-1, 3) for c in clouds]
-    nrm = [np.asarray(c["normals"], dtype=np.float64).reshape(-1, 3) for c in clouds]
+    has_nrm = [c.get("normals") is not None for c in clouds]
+    if any(has_nrm) and not all(has_nrm):
+        raise ValueError(f"pack_clouds: clouds {[i for i, h in enumerate(has_nrm) if not h]} have no normals; either every "
+                         "cloud has normals or none has")
+    nrm = [np.asarray(c["normals"], dtype=np.float64).reshape(-1, 3) for c in clouds] if all(has_nrm) else None
     vps = [np.asarray(c.get("view_points") if c.get("view_points") is not None else np.zeros((1, 3)), dtype=np.float64).reshape(-1, 3)
            for c in clouds]
     ks = np.array([len(v) for v in vps], dtype=np.int32)
@@ -166,7 +174,8 @@ def pack_clouds(clouds):
             cs = c.get("cam_source")
             blocks.append(np.ones((len(x), k), np.int32) if cs is None else np.asarray(cs, dtype=np.int32).reshape(len(x), k))
         cam = np.ascontiguousarray(np.concatenate([b.ravel() for b in blocks]))
-    return {"offsets": offsets, "xyz": np.ascontiguousarray(np.concatenate(xyz)), "normals": np.ascontiguousarray(np.concatenate(nrm)),
+    return {"offsets": offsets, "xyz": np.ascontiguousarray(np.concatenate(xyz)),
+            "normals": None if nrm is None else np.ascontiguousarray(np.concatenate(nrm)),
             "cam_source": cam, "n_cameras": ks, "view_points": np.ascontiguousarray(np.concatenate(vps))}
 
 
@@ -204,6 +213,7 @@ class Context:
             raise GpdbError(rc, lib().gpdb_last_error(None).decode())
         self._keep = []
         self._n_clouds = 0  # clouds of the installed batch (gpdb_detect_batch reads that many + 1 sample offsets)
+        self._batch = None  # (point offsets, camera counts, view point blocks, has source indices) of the installed batch
 
     def close(self):
         if getattr(self, "h", None):
@@ -318,10 +328,52 @@ class Context:
     def set_clouds(self, clouds):
         """gpdb_set_clouds: installs a batch of processed clouds (list of dicts as set_cloud takes) beside the single cloud."""
         pk = pack_clouds(clouds)
-        self._n_clouds = 0  # a failed gpdb_set_clouds leaves no batch
+        self._n_clouds, self._batch = 0, None  # a failed gpdb_set_clouds leaves no batch
         self._check(lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
                                           _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])))
         self._n_clouds = len(clouds)
+        self._batch = (pk["offsets"], pk["n_cameras"], pk["view_points"], False)
+
+    def preprocess_clouds(self, raw_clouds, pp=None, read_back=True):
+        """gpdb_preprocess_clouds: preprocess() of every raw cloud (list of dicts: xyz, optional normals, optional
+        cam_source, view_points) in one call, the processed clouds installed as the batch (detect_batch works straight
+        after it). Returns one dict per cloud as preprocess() returns (xyz, normals, cam_source, view_points, src), or the
+        processed point offsets [B+1] when read_back is False. A cloud the filter empties stays, with no points."""
+        pk = pack_clouds(raw_clouds)
+        if pp is None:
+            pp = preprocess_params()
+        B = len(raw_clouds)
+        poff = np.zeros(B + 1, np.int32)
+        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._check(lib().gpdb_preprocess_clouds(self.h, B, _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
+                                                 _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"]), C.byref(pp),
+                                                 _p(poff)))
+        self._n_clouds = B
+        self._batch = (poff, pk["n_cameras"], pk["view_points"], True)
+        return self.get_clouds() if read_back else poff
+
+    def get_clouds(self):
+        """gpdb_get_clouds: the installed batch as one dict per cloud (xyz, normals, cam_source [N_b, K_b], view_points,
+        and src, the index into the cloud's raw points, after preprocess_clouds)."""
+        if self._batch is None:
+            self._check(lib().gpdb_get_clouds(self.h, None, None, None, None))  # raises: no batch installed
+        offsets, ks, vps, has_src = self._batch
+        n = int(offsets[-1])
+        xyz = np.zeros((n, 3), np.float32)
+        nrm = np.zeros((n, 3), np.float64)
+        cam = np.zeros(int(np.sum(np.diff(offsets) * ks)), np.int32)
+        src = np.zeros(n, np.int32) if has_src else None
+        self._check(lib().gpdb_get_clouds(self.h, _p(xyz), _p(nrm), _p(cam), _p(src)))
+        out, c0, v0 = [], 0, 0
+        for b in range(len(ks)):
+            o0, o1, k = int(offsets[b]), int(offsets[b + 1]), int(ks[b])
+            d = {"xyz": xyz[o0:o1].copy(), "normals": nrm[o0:o1].copy(), "cam_source": cam[c0:c0 + (o1 - o0) * k].reshape(o1 - o0, k).copy(),
+                 "view_points": vps[v0:v0 + k].copy()}
+            if has_src:
+                d["src"] = src[o0:o1].copy()
+            out.append(d)
+            c0, v0 = c0 + (o1 - o0) * k, v0 + k
+        return out
 
     def _pack_batch_samples(self, sample_lists):
         # the C-ABI takes no cloud count: it reads and writes B + 1 offsets for the B installed clouds

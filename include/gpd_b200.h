@@ -225,7 +225,7 @@ int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n_s
  * gpdb_preprocess, gpdb_detect and every other entry point behave as before whatever batch is installed. Empty clouds,
  * K_b outside 1..8, non-finite coordinates and malformed offsets are GPDB_ERR_INVALID; a failed call leaves no batch.
  * Returns B. Sample positions (gpdb_set_samples) do not apply to a batch: called while only a batch is installed,
- * gpdb_set_samples is GPDB_ERR_INVALID. Preprocessing stays per cloud (gpdb_preprocess + gpdb_get_cloud). */
+ * gpdb_set_samples is GPDB_ERR_INVALID. Raw views are preprocessed into a batch by gpdb_preprocess_clouds. */
 int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points);
 
@@ -325,8 +325,33 @@ int gpdb_get_cloud(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *
  * (the first point of its voxel, cloud.cpp:304-310 `(*res.first)(3)`). Returns N. */
 int gpdb_get_cloud_source_index(gpdb_ctx *ctx, int32_t *src_out);
 
-/* Device time (ms, CUDA events) of the stages of the last gpdb_preprocess call:
- * ms[0] upload, ms[1] NaN/workspace filter, ms[2] voxelise, ms[3] grid build, ms[4] normals, ms[5] whole call. */
+/* CandidatesGenerator::preprocessPointCloud for every cloud of a batch in ONE call (the gpdb_preprocess steps, each cloud
+ * on its own), leaving the processed clouds installed as the batch, exactly as gpdb_set_clouds would install them.
+ * Raw cloud b: points point_offsets[b] .. point_offsets[b+1]-1 of xyz (normals likewise, may be NULL when
+ * estimate_normals = 1), n_cameras[b] cameras, view points and cam_source blocks as gpdb_set_clouds (cam_source NULL:
+ * every camera sees every point). One gpdb_preprocess_params for all clouds. processed_offsets_out[B+1] receives the
+ * processed point offsets. Returns B or a negative error; a failed call leaves no batch, the single cloud is never touched.
+ * Every processed cloud is bit-equal to gpdb_preprocess on that raw cloud alone (points, camera sources, source indices,
+ * normals). Camera sources follow gpdb_preprocess: an entry counts as seen when it is exactly 1, and with voxelize = 0
+ * an entry other than 0 or 1 is GPDB_ERR_INVALID. A raw cloud must hold at least one point; a cloud the filter empties
+ * stays in the batch with no points (equal processed offsets: it takes only an empty sample range in
+ * gpdb_detect_batch). Malformed offsets, K_b outside 1..8, missing normals with estimate_normals = 0 and a
+ * non-positive voxel_size or normals_radius are GPDB_ERR_INVALID before any device work; a voxel index of 2^21 or more
+ * in any cloud is GPDB_ERR_INVALID (the message names the cloud); more than 8 192 neighbours within normals_radius at
+ * one point is GPDB_ERR_CAPACITY. */
+int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
+                           const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
+                           const double *view_points, const gpdb_preprocess_params *pp, int32_t *processed_offsets_out);
+
+/* Reads back the installed batch (after gpdb_preprocess_clouds or gpdb_set_clouds), concatenated in cloud order:
+ * xyz_out [3*N], normals_out [3*N], cam_source_out (the N_b x K_b int32 blocks one after the other), src_out [N] =
+ * index into cloud b's RAW points of the point that represents each processed point (gpdb_preprocess_clouds only;
+ * GPDB_ERR_STATE after gpdb_set_clouds). Any output may be NULL. Returns N; GPDB_ERR_STATE when no batch is installed. */
+int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out, int32_t *src_out);
+
+/* Device time (ms, CUDA events) of the stages of the last gpdb_preprocess or gpdb_preprocess_clouds call (for a batch:
+ * all clouds together): ms[0] upload, ms[1] NaN/workspace filter, ms[2] voxelise, ms[3] grid build, ms[4] normals,
+ * ms[5] whole call. */
 int gpdb_preprocess_timings(const gpdb_ctx *ctx, double ms_out[6]);
 
 /* Replaces: HandSearch::reevaluateHypotheses (hand_search.cpp:66-134; GraspDetector::evalGroundTruth,
