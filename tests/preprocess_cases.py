@@ -14,7 +14,7 @@ from oracle import oracle
 # cameras in front of the table (z = 0.9), looking along +z (test_gpu_geometry_params.py uses the same set)
 CAMS = [[0.0, 0.0, 0.0], [0.6, 0.0, 0.0], [-0.5, 0.1, 0.05], [0.0, 0.5, 0.0], [0.1, -0.5, 0.1], [0.45, 0.45, 0.0],
         [-0.4, -0.4, 0.0], [0.3, -0.2, -0.2]]
-GRID_CELL = 0.02      # cell of the neighbour grid (geometry.cu geo_build_grid) for clouds of a few metres
+GRID_CELL = 0.02      # first cell of the neighbour grid (geometry.cu geo_build_grid); grid_of grows it for large clouds
 TIER0_CAP = 1024      # neighbours per point held by k_normals' first tier
 TIER1_CAP = 8192      # ... by its second tier; beyond it gpdb_preprocess reports GPDB_ERR_CAPACITY
 TABLE_WS = [-0.6, 0.6, -0.5, 0.5, 0.2, 1.0]
@@ -80,15 +80,27 @@ def voxel_reference(xyz, ws, cell):
     return keep[first[order]], (mn + c * uniq[order].astype(np.float32)).astype(np.float32)
 
 
-def grid_rows(xyz, r):
-    """Grid rows (y, z cell pairs) the ball scan of k_normals visits for each point: the 2 cm cells from the cloud's
-    minimum, the ball widened as preprocess.cu's pre_normals does."""
+def grid_of(xyz):
+    """(lo, dim, cell, cells, growth steps) of the neighbour grid of a cloud, in the float32 steps of geo_build_grid and
+    k_batch_desc: 2 cm cells from the cloud's minimum, grown by 1.5x while the grid would need more than 48e6 cells."""
     p = np.asarray(xyz, np.float32)
     lo, hi = p.min(0), p.max(0)
-    dim = np.floor((hi - lo) / np.float32(GRID_CELL)).astype(np.int64) + 2
-    assert np.prod(dim.astype(np.float64)) <= 48e6  # the grid keeps its 2 cm cell
+    cell, steps = np.float32(GRID_CELL), 0
+    while True:
+        dim = np.floor((hi - lo) / cell).astype(np.int64) + 2
+        cells = float(np.prod(dim.astype(np.float64)))
+        if cells <= 48e6:
+            return lo, dim, cell, cells, steps
+        cell, steps = np.float32(cell * np.float32(1.5)), steps + 1
+
+
+def grid_rows(xyz, r):
+    """Grid rows (y, z cell pairs) the ball scan of k_normals visits for each point: the cells of grid_of from the
+    cloud's minimum, the ball widened as preprocess.cu's pre_normals does."""
+    p = np.asarray(xyz, np.float32)
+    lo, dim, cell, _, _ = grid_of(p)
     rf = np.float32(r) * np.float32(1.0001) + np.float32(1e-6)
-    inv = np.float32(1.0) / np.float32(GRID_CELL)
+    inv = np.float32(1.0) / cell
     rows = np.ones(len(p), np.int64)
     for a in (1, 2):
         c0 = np.clip(np.floor((p[:, a] - rf - lo[a]) * inv).astype(np.int64), 0, dim[a] - 1)
