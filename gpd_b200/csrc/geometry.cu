@@ -1235,6 +1235,29 @@ __device__ __forceinline__ double cell_mean(unsigned long long acc, const double
   const double sum = (double)(acc & 0xffffffffffffull);
   return c < (unsigned)RCP_N ? sum * rcp[c] : sum / ((double)c * 4294967296.0);
 }
+// The image tiles hold 64-bit cells (low word at the lower address) but are updated with 32-bit shared-memory atomics:
+// sm_90 has no native 64-bit shared atomic add or max, and the compare-and-swap loop the compiler emits instead
+// serialises lanes that hit the same cell (common for shadow voxels, which collapse along each projection axis).
+//
+// cell_add: one entry into a cell accumulator (count << 48 | fixed-point sum). Each adder carries its own overflow of the
+// low word into the high word, so the final 64-bit value is the exact sum whatever order the adders run in. Returns
+// whether this entry carried.
+__device__ __forceinline__ bool cell_add(unsigned long long *cell, unsigned q) {
+  unsigned *w = reinterpret_cast<unsigned *>(cell);
+  const unsigned lo_old = atomicAdd(w, q);
+  const bool carry = lo_old + q < lo_old;
+  atomicAdd(w + 1, (1u << 16) + (carry ? 1u : 0u));
+  return carry;
+}
+// key_max_dist, barrier, key_max_index: the cell ends up holding the largest key (distance bits << 32 | index), as one
+// 64-bit atomicMax would leave it. The index word is only raised by keys whose distance equals the cell's maximum.
+__device__ __forceinline__ void key_max_dist(unsigned long long *cell, unsigned long long key) {
+  atomicMax(reinterpret_cast<unsigned *>(cell) + 1, (unsigned)(key >> 32));
+}
+__device__ __forceinline__ void key_max_index(unsigned long long *cell, unsigned long long key) {
+  unsigned *w = reinterpret_cast<unsigned *>(cell);
+  if (w[1] == (unsigned)(key >> 32)) atomicMax(w, (unsigned)key);
+}
 
 __device__ __forceinline__ bool fully_covered(const unsigned *occf, int S);
 // block-wide reduction of up to eight floats with max (use negated values for min). Contains two barriers. With `occf`
@@ -1544,9 +1567,15 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         const unsigned cc = bcell[k];
         const int row = S - 1 - (int)((cc >> (8 * a0)) & 255), col = (cc >> (8 * a1)) & 255;
         const int pix = row * S + col;
-        atomicMax(tileA + pix, bkeys[k]);
-        atomicAdd(tileB + pix, (1ull << 48) + (unsigned long long)bq[a2 * BC + k]);
+        key_max_dist(tileA + pix, bkeys[k]);
         atomicOr(&sm.occf[pix >> 5], 1u << (pix & 31));
+      }
+      __syncthreads();
+      for (int k = tid; k < bn; k += NT_IMG) {
+        const unsigned cc = bcell[k];
+        const int pix = (S - 1 - (int)((cc >> (8 * a0)) & 255)) * S + (int)((cc >> (8 * a1)) & 255);
+        key_max_index(tileA + pix, bkeys[k]);
+        cell_add(tileB + pix, bq[a2 * BC + k]);
       }
       __syncthreads();
       // the winner of a cell (its point with the largest key) carries the cell's values: |n| of that point, 1 - mean depth
@@ -2023,7 +2052,7 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         for (int pj = 0; pj < 3; pj++) {
           const int a0 = (pj == 0) ? 0 : 2, a1 = (pj == 2) ? 0 : 1, a2 = (pj == 0) ? 2 : (pj == 1 ? 0 : 1);
           const int row = S - 1 - cellv[a0], col = cellv[a1];
-          atomicAdd(tileA + (size_t)pj * SS + row * S + col, (1ull << 48) + (unsigned long long)unit_q32(u[a2]));
+          cell_add(tileA + (size_t)pj * SS + row * S + col, unit_q32(u[a2]));
         }
       };
       if (tid == 0) sm.wl_n = 0;
@@ -2184,7 +2213,41 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
 // (see geo_images; otherwise k_images does all the work). Results are bit-identical to
 // k_images (tests/test_gpu_parity.py::test_image_kernels_agree).
 // ------------------------------------------------------------------------------------------------
+// Balanced expansion of the set bits of one bitmap word per lane (shadow voxels are spatially clustered, so a loop over
+// each lane's own word would hold the warp for the densest word's popcount): the warp's set bits, in lane then bit order,
+// are handed out 32 at a time. Each lane finds its slot's word by a binary search over the inclusive popcount scan, and
+// the bit with __fns. reserve(total) is called once by all lanes and returns the warp's first output position;
+// emit(position, code | bit) runs once per set bit. Called by all 32 lanes together.
+template <class R, class E>
+__device__ __forceinline__ void warp_expand_bits(unsigned bits, unsigned code, R &&reserve, E &&emit) {
+  const int lane = threadIdx.x & 31;
+  const int cnt = __popc(bits);
+  int incl = cnt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  const int total = __shfl_sync(0xffffffffu, incl, 31);
+  const int base = reserve(total);
+  for (int j0 = 0; j0 < total; j0 += 32) {
+    const int j = j0 + lane;
+    int w = 0;  // first lane whose inclusive count exceeds j
+#pragma unroll
+    for (int s = 16; s; s >>= 1) {
+      const int v = __shfl_sync(0xffffffffu, incl, w + s - 1);
+      if (v <= j) w += s;
+    }
+    const unsigned wbits = __shfl_sync(0xffffffffu, bits, w), wcode = __shfl_sync(0xffffffffu, code, w);
+    const int wexcl = __shfl_sync(0xffffffffu, incl - cnt, w);
+    if (j < total) emit(base + j, wcode | __fns(wbits, 0, j - wexcl + 1));
+  }
+}
+
 constexpr int BOX_CAP2 = 1024;
+// the in-ball list of the shadow casting fills the image's 57.6 KB slot behind the 43.2 KB of point planes
+constexpr int IMG2_S = 60;  // the only image size of the fast path
+constexpr int BALL_CAP2 = (IMG2_S * IMG2_S * 16 - 12 * IMG2_S * IMG2_S) / 4;
 struct Img2Smem {
   SegScan<NT_IMG> seg;
   gpdb_pose h;
@@ -2195,10 +2258,19 @@ struct Img2Smem {
   unsigned occf[MAXPIX / 32 + 2];
   unsigned lcgA[GPDB_MAX_NSP], lcgC[GPDB_MAX_NSP];
   int cam_or, n_img, box_n, wl_n, dl_n, st_n;
+  int ball_n;   // in-ball points recorded by scan 1 (positions in the cell-sorted array)
   int nonunit;  // a box point has a normal of other than unit length: the image is redone by k_images (exact fold)
   int bm_org[3], bm_dims[3];
   float fred[NT_IMG / 32][8];
+  // shadow phase invariants of the image, read from here rather than held in registers (k_images2 runs at 64 registers):
+  // the float frame and sample, the box widened by the jitter (voxel test) and by the margin (slab cull), and per camera
+  // the slab reciprocals of the shadow vector (0: the vector is parallel to that slab)
+  float fR[9], fs[3], fbx_lo[3], fbx_hi[3], cull_lo[3], cull_hi[3];
+  float cull_inv[2][3];
 };
+// two CTAs per SM: 2 x (dynamic + static + the 1 KB the hardware reserves per CTA) within Hopper's 228 KB per SM
+constexpr size_t IMG2_DYN_SMEM = (size_t)2 * 8 * IMG2_S * IMG2_S + (size_t)3 * IMG2_S * IMG2_S + (size_t)BOX_CAP2 * 36;
+static_assert(2 * (IMG2_DYN_SMEM + sizeof(Img2Smem) + 1024) <= 228 * 1024, "k_images2 no longer fits two CTAs per SM");
 
 template <bool BATCH>
 __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevCloud cl0, CloudTable tab, const gpdb_pose *cand, int nc,
@@ -2208,7 +2280,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
   const DevParams &P = *Pp;
   extern __shared__ __align__(16) unsigned char dyn[];
   __shared__ Img2Smem sm;
-  constexpr int S = 60, SS = S * S, RW = S / 4, PLB = SS;  // 15 words per row, 3600-byte planes
+  constexpr int S = IMG2_S, SS = S * S, RW = S / 4, PLB = SS;  // 15 words per row, 3600-byte planes
   constexpr int PIXT = (SS + NT_IMG - 1) / NT_IMG;
   constexpr int JW = (BOX_CAP2 + NT_IMG - 1) / NT_IMG;  // box points per thread
   const int C = P.C;
@@ -2243,9 +2315,12 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       sm.cam_or = 0;
       sm.n_img = 0;
       sm.box_n = 0;
+      sm.ball_n = 0;
       sm.nonunit = 0;
     }
     uint8_t *gimg = p16 + (size_t)b * SS * 16;  // the image's own memory: first the point planes, finally the pixels
+    // ... and behind the twelve point planes, the list of in-ball points that the shadow casting walks once per camera
+    int *ball = reinterpret_cast<int *>(gimg + 12 * PLB);
     for (int k = tid; k < (npp * PLB) >> 4; k += NT_IMG) reinterpret_cast<uint4 *>(gimg)[k] = make_uint4(0, 0, 0, 0);
     for (int k = tid; k < SS; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);  // tiles A, B
     for (int k = tid; k < (3 * PLB) >> 4; k += NT_IMG) reinterpret_cast<uint4 *>(splanes)[k] = make_uint4(0, 0, 0, 0);
@@ -2261,12 +2336,13 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
     // ---- ball scan 1: neighbourhood centre, camera set, raw box points
     double sx = 0, sy = 0, sz = 0;
     int cnt = 0, cam_or = 0;
-    scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
-      bool inb = false;
+    scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int where) {
+      bool inb = false, inball = false;
       unsigned long long key = 0;
       if (in) {
         float d = l2_simple(q, p.x, p.y, p.z);
         if (d < P.r2_img) {
+          inball = true;
           const int idx = __float_as_int(p.w);
           sx += (double)p.x;
           sy += (double)p.y;
@@ -2280,6 +2356,17 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
             key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)idx;
             if (G.nonunit && !unit_normal(cl.nrm + 3 * (size_t)idx)) sm.nonunit = 1;
           }
+        }
+      }
+      if (C == 15) {
+        const unsigned mb = __ballot_sync(0xffffffffu, inball);
+        if (mb) {
+          const int leader = __ffs(mb) - 1;
+          int base = 0;
+          if (lane == leader) base = atomicAdd(&sm.ball_n, __popc(mb));
+          base = __shfl_sync(0xffffffffu, base, leader);
+          const int pos = base + __popc(mb & ((1u << lane) - 1));
+          if (inball && pos < BALL_CAP2) ball[pos] = where;
         }
       }
       unsigned mk = __ballot_sync(0xffffffffu, inb);
@@ -2355,9 +2442,15 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       for (int k = tid; k < bn; k += NT_IMG) {
         const unsigned cc = bcell[k];
         const int pix = (S - 1 - (int)((cc >> (8 * a0)) & 255)) * S + (int)((cc >> (8 * a1)) & 255);
-        atomicMax(tileA + pix, bkeys[k]);
-        atomicAdd(tileB + pix, (1ull << 48) + (unsigned long long)bq[a2 * BOX_CAP2 + k]);
+        key_max_dist(tileA + pix, bkeys[k]);
         atomicOr(&sm.occf[pix >> 5], 1u << (pix & 31));
+      }
+      __syncthreads();
+      for (int k = tid; k < bn; k += NT_IMG) {
+        const unsigned cc = bcell[k];
+        const int pix = (S - 1 - (int)((cc >> (8 * a0)) & 255)) * S + (int)((cc >> (8 * a1)) & 255);
+        key_max_index(tileA + pix, bkeys[k]);
+        cell_add(tileB + pix, bq[a2 * BOX_CAP2 + k]);
       }
       __syncthreads();
       // winners (largest key of their cell) carry the cell's values; each thread owns <= JW box points
@@ -2475,6 +2568,22 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           sm.bm_org[r] = lo;
           sm.bm_dims[r] = min(hi - lo + 1, bmd);
         }
+        for (int e = 0; e < 9; e++) sm.fR[e] = (float)h.frame[e];
+        for (int r = 0; r < 3; r++) sm.fs[r] = (float)h.sample[r];
+        const float jm = (float)(gmax * voxel * 0.3 * 1.7320508075688772 + 2e-5);
+        sm.fbx_lo[0] = (float)h.bottom - jm;
+        sm.fbx_lo[1] = (float)(h.center - P.vol_w / 2.0) - jm;
+        sm.fbx_lo[2] = (float)(-P.vol_h) - jm;
+        sm.fbx_hi[0] = (float)(h.bottom + P.vol_d) + jm;
+        sm.fbx_hi[1] = (float)(h.center + P.vol_w / 2.0) + jm;
+        sm.fbx_hi[2] = (float)P.vol_h + jm;
+        const double wm = 0.0105;
+        const double bx_lo[3] = {h.bottom - wm, h.center - P.vol_w / 2.0 - wm, -P.vol_h - wm};
+        const double bx_hi[3] = {h.bottom + P.vol_d + wm, h.center + P.vol_w / 2.0 + wm, P.vol_h + wm};
+        for (int a = 0; a < 3; a++) {
+          sm.cull_lo[a] = (float)bx_lo[a] - 1e-5f;
+          sm.cull_hi[a] = (float)bx_hi[a] + 1e-5f;
+        }
       }
       if (tid < K) {
         double s0 = sm.center[0] - G.vp[tid][0], s1 = sm.center[1] - G.vp[tid][1], s2 = sm.center[2] - G.vp[tid][2];
@@ -2483,6 +2592,10 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         sm.sv[tid][1] = P.shadow_length * s1 / nn;
         sm.sv[tid][2] = P.shadow_length * s2 / nn;
         to_frame(h.frame, sm.sv[tid][0], sm.sv[tid][1], sm.sv[tid][2], sm.svh[tid][0], sm.svh[tid][1], sm.svh[tid][2]);
+        for (int a = 0; a < 3; a++) {
+          const float dv = (float)sm.svh[tid][a];
+          sm.cull_inv[tid][a] = fabsf(dv) < 1e-6f ? 0.0f : 1.0f / dv;
+        }
       }
       for (int k = tid; k < bm_words * K; k += NT_IMG) bitmap[k] = 0u;
       __syncthreads();
@@ -2497,22 +2610,13 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         to_frame(h.frame, w0 - h.sample[0], w1 - h.sample[1], w2 - h.sample[2], x, y, z);
         return in_image_box(P, h, x, y, z);
       };
-      const int cam_set = sm.cam_or;
+      const int cam_set = sm.cam_or, nball = sm.ball_n;
       float4 *wl = reinterpret_cast<float4 *>(tileA);       // work list over tile A ...
       constexpr int WL_CAP = (SS * 8) / 20;
       unsigned *wrange = reinterpret_cast<unsigned *>(wl + WL_CAP);
       unsigned *dlist = reinterpret_cast<unsigned *>(tileB);  // ... draw list over tile B
       constexpr int DL_CAP = 2 * SS;
-      const double wm = 0.0105;
-      const double bx_lo[3] = {h.bottom - wm, h.center - P.vol_w / 2.0 - wm, -P.vol_h - wm};
-      const double bx_hi[3] = {h.bottom + P.vol_d + wm, h.center + P.vol_w / 2.0 + wm, P.vol_h + wm};
-      float fR[9];
-#pragma unroll
-      for (int e = 0; e < 9; e++) fR[e] = (float)h.frame[e];
-      const float fsx = (float)h.sample[0], fsy = (float)h.sample[1], fsz = (float)h.sample[2];
-      const float jm = (float)(gmax * voxel * 0.3 * 1.7320508075688772 + 2e-5);
-      const float fbx_lo[3] = {(float)h.bottom - jm, (float)(h.center - P.vol_w / 2.0) - jm, (float)(-P.vol_h) - jm};
-      const float fbx_hi[3] = {(float)(h.bottom + P.vol_d) + jm, (float)(h.center + P.vol_w / 2.0) + jm, (float)P.vol_h + jm};
+      const float *fR = sm.fR, *fs = sm.fs, *fbx_lo = sm.fbx_lo, *fbx_hi = sm.fbx_hi, *cull_lo = sm.cull_lo, *cull_hi = sm.cull_hi;
       auto draw_bit = [&](double px, double py, double pz, unsigned seed, int k) -> int {
         const double s0 = sm.sv[k][0], s1 = sm.sv[k][1], s2 = sm.sv[k][2];
         double u = (double)((seed >> 16) & 0x7FFFu) * mxu;
@@ -2521,7 +2625,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         int v2 = (int)((pz + u * s2) * P.vox_mult);
         int b0 = v0 - o0, b1 = v1 - o1, b2 = v2 - o2;
         if ((unsigned)b0 >= (unsigned)d0 || (unsigned)b1 >= (unsigned)d1 || (unsigned)b2 >= (unsigned)d2) return -1;
-        const float wx = fmaf((float)v0, 0.003f, -fsx), wy = fmaf((float)v1, 0.003f, -fsy), wz = fmaf((float)v2, 0.003f, -fsz);
+        const float wx = fmaf((float)v0, 0.003f, -fs[0]), wy = fmaf((float)v1, 0.003f, -fs[1]), wz = fmaf((float)v2, 0.003f, -fs[2]);
         const float hx = fmaf(fR[0], wx, fmaf(fR[1], wy, fR[2] * wz));
         const float hy = fmaf(fR[3], wx, fmaf(fR[4], wy, fR[5] * wz));
         const float hz = fmaf(fR[6], wx, fmaf(fR[7], wy, fR[8] * wz));
@@ -2531,16 +2635,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       for (int k = 0; k < K; k++) {
         if (!((cam_set >> k) & 1)) continue;
         unsigned *bm = bitmap + (size_t)k * bm_words;
-        float cull_lo[3], cull_hi[3], cull_inv[3];
-        bool cull_par[3];
-#pragma unroll
-        for (int a = 0; a < 3; a++) {
-          const float dv = (float)sm.svh[k][a];
-          cull_par[a] = fabsf(dv) < 1e-6f;
-          cull_inv[a] = cull_par[a] ? 0.0f : 1.0f / dv;
-          cull_lo[a] = (float)bx_lo[a] - 1e-5f;
-          cull_hi[a] = (float)bx_hi[a] + 1e-5f;
-        }
+        const float *cull_inv = sm.cull_inv[k];
         __syncthreads();
         if (tid == 0) {
           sm.wl_n = 0;
@@ -2548,14 +2643,14 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         }
         __syncthreads();
         auto cull = [&](const float4 &p, unsigned &rg) -> bool {
-          const float wx = p.x - fsx, wy = p.y - fsy, wz = p.z - fsz;
+          const float wx = p.x - fs[0], wy = p.y - fs[1], wz = p.z - fs[2];
           const float o3[3] = {fmaf(fR[0], wx, fmaf(fR[1], wy, fR[2] * wz)), fmaf(fR[3], wx, fmaf(fR[4], wy, fR[5] * wz)),
                                fmaf(fR[6], wx, fmaf(fR[7], wy, fR[8] * wz))};
           float tmin = 0.0f, tmax = 1.0f;
           bool hit = true;
 #pragma unroll
           for (int a = 0; a < 3; a++) {
-            if (cull_par[a]) {
+            if (cull_inv[a] == 0.0f) {
               hit = hit && o3[a] >= cull_lo[a] && o3[a] <= cull_hi[a];
             } else {
               const float t1 = (cull_lo[a] - o3[a]) * cull_inv[a], t2 = (cull_hi[a] - o3[a]) * cull_inv[a];
@@ -2568,9 +2663,8 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           rg = (unsigned)r0 | ((unsigned)r1 << 16);
           return true;
         };
-        scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
-          unsigned rg = 0;
-          const bool ok = in && l2_simple(q, p.x, p.y, p.z) < P.r2_img && cull(p, rg);
+        // appends the point to the work list (one shared-memory atomic per warp); called by all 32 lanes together
+        auto append = [&](bool ok, const float4 &p, unsigned rg) {
           const unsigned mk = __ballot_sync(0xffffffffu, ok);
           if (!mk) return;
           const int leader = __ffs(mk) - 1;
@@ -2594,7 +2688,27 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
               }
             }
           }
-        });
+        };
+        if (nball <= BALL_CAP2) {  // the neighbourhood recorded by scan 1: independent loads, all lanes busy (uniform)
+          for (int i0 = 0; i0 < nball; i0 += NT_IMG) {
+            const int i = i0 + tid;
+            float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+            unsigned rg = 0;
+            bool ok = false;
+            if (i < nball) {
+              p = __ldg(cl.pts4 + __ldcg(ball + i));  // the list was written by this CTA: L2, not L1
+              ok = cull(p, rg);
+            }
+            append(ok, p, rg);
+          }
+        } else {  // more in-ball points than the list holds: walk the grid again
+          scan_balanced<NT_IMG>(G, cl, sr, sm.seg, [&](bool in, const float4 &p, int) {
+            unsigned rg = 0;
+            const bool ok = in && l2_simple(q, p.x, p.y, p.z) < P.r2_img && cull(p, rg);
+            append(ok, p, rg);
+          });
+          if (prof && tid == 0) atomicAdd(prof + 14, 1ull);
+        }
         __syncthreads();
         const int nw = min(sm.wl_n, WL_CAP);
         if (prof && tid == 0) atomicAdd(prof + 9, (unsigned long long)nw);
@@ -2681,34 +2795,30 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
           const int a0 = (pj == 0) ? 0 : 2, a1 = (pj == 2) ? 0 : 1, a2 = (pj == 0) ? 2 : (pj == 1 ? 0 : 1);
           const int pix = (S - 1 - cellv[a0]) * S + cellv[a1];
           const unsigned qv = unit_q32(u[a2]);
-          if (pj >= pj_lo && pj < pj_hi) atomicAdd(tileA + (size_t)(pj - pj_lo) * SS + pix, (1ull << 48) + (unsigned long long)qv);
+          if (pj >= pj_lo && pj < pj_hi) cell_add(tileA + (size_t)(pj - pj_lo) * SS + pix, qv);
           if (pj == 2) st = make_uint2((unsigned)pix | 0x80000000u, qv);
         }
         return st;
       };
+      // voxel code b0 | b1 << 8 | b2 << 16 of bit 0 of bitmap word wd (0 past the bitmap's end: such words are empty)
+      auto word_code = [&](int wd) -> unsigned {
+        const int rowi = wd >> 1;
+        return ((unsigned)(rowi % d1) << 8) | ((unsigned)(rowi / d1) << 16) | ((unsigned)(wd & 1) << 5);
+      };
       for (int wd0 = 0; wd0 * 32 < nbits; wd0 += NT_IMG) {
         const int wd = wd0 + tid;
-        unsigned bits = (wd * 32 < nbits) ? bitmap[wd] : 0u;
-        int cntb = __popc(bits);
-        int incl = cntb;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          int v = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += v;
-        }
-        int total = __shfl_sync(0xffffffffu, incl, 31), base = 0;
-        if (lane == 31 && total) base = atomicAdd(&sm.st_n, total);
-        base = __shfl_sync(0xffffffffu, base, 31);
-        int pos = base + incl - cntb;
-        const int rowi = wd >> 1;
-        const unsigned hi = ((unsigned)(rowi % d1) << 8) | ((unsigned)(rowi / d1) << 16) | ((unsigned)(wd & 1) << 5);
-        while (bits) {
-          int bi = __ffs(bits) - 1;
-          bits &= bits - 1;
-          if (pos < ST_CAP) stash[pos].x = hi | (unsigned)bi;
-          else eval_voxel(hi | (unsigned)bi, 0, 2);  // list full: projections 0 and 1 in place (2: second walk below)
-          pos++;
-        }
+        const unsigned bits = (wd * 32 < nbits) ? bitmap[wd] : 0u;
+        warp_expand_bits(
+            bits, word_code(wd),
+            [&](int total) {
+              int base = 0;
+              if (lane == 0 && total) base = atomicAdd(&sm.st_n, total);
+              return __shfl_sync(0xffffffffu, base, 0);
+            },
+            [&](int pos, unsigned code) {
+              if (pos < ST_CAP) stash[pos].x = code;
+              else eval_voxel(code, 0, 2);  // list full: projections 0 and 1 in place (2: second walk below)
+            });
       }
       __syncthreads();
       const int nset_all = sm.st_n, nset = min(nset_all, ST_CAP);
@@ -2783,21 +2893,25 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       if (nset_all <= ST_CAP) {
         for (int i = tid; i < nset; i += NT_IMG) {
           const uint2 st = stash[i];
-          if (st.x & 0x80000000u) atomicAdd(tileA + (st.x & 0x7fffffffu), (1ull << 48) + (unsigned long long)st.y);
+          if (st.x & 0x80000000u) {
+            const bool carry = cell_add(tileA + (st.x & 0x7fffffffu), st.y);
+            if (prof && carry) atomicAdd(prof + 0, 1ull);
+          }
         }
       } else {
-        for (int wd = tid; wd * 32 < nbits; wd += NT_IMG) {
-          unsigned bits = bitmap[wd];
-          const int rowi = wd >> 1;
-          const unsigned hi = ((unsigned)(rowi % d1) << 8) | ((unsigned)(rowi / d1) << 16) | ((unsigned)(wd & 1) << 5);
-          while (bits) {
-            int bi = __ffs(bits) - 1;
-            bits &= bits - 1;
-            eval_voxel(hi | (unsigned)bi, 2, 3);
-          }
+        for (int wd0 = 0; wd0 * 32 < nbits; wd0 += NT_IMG) {
+          const int wd = wd0 + tid;
+          const unsigned bits = (wd * 32 < nbits) ? bitmap[wd] : 0u;
+          warp_expand_bits(bits, word_code(wd), [](int) { return 0; }, [&](int, unsigned code) { eval_voxel(code, 2, 3); });
         }
       }
       __syncthreads();
+      if (prof) {  // the most shadow voxels summed into one cell of projection 2
+        unsigned most = 0;
+        for (int k = tid; k < SS; k += NT_IMG) most = max(most, (unsigned)(tileA[k] >> 48));
+        most = __reduce_max_sync(0xffffffffu, most);
+        if (lane == 0 && most) atomicMax(prof + 1, (unsigned long long)most);
+      }
       shadow_channel(2, tileA);
       __syncthreads();
       for (int k = tid; k < MAXPIX / 32; k += NT_IMG) sm.occf[k] = 0u;
@@ -3183,7 +3297,7 @@ static int launch_images(gpdb_ctx *ctx, const DevCloud &cl, const gpdb_pose *d_c
     if (!ovf) return GPDB_ERR_CUDA;                                            // may run concurrently on its own stream
     int *ovf_count = ovf + nc;
     CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
-    const size_t smem2 = (size_t)2 * 8 * S * S + (size_t)3 * S * S + (size_t)BOX_CAP2 * 36;
+    const size_t smem2 = IMG2_DYN_SMEM;
     CUDA_TRY(cudaFuncSetAttribute(k_images2<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
     k_images2<BATCH><<<std::min(nc, ctx->sm_count * 64), NT_IMG, smem2, ctx->stream>>>(ctx->dp, cl, tab, d_cand, nc, d_p16, ctx->d_qtab, ovf,
                                                                                ovf_count, ctx->d_prof);

@@ -411,7 +411,9 @@ int gpdb_last_timings(const gpdb_ctx *ctx, double ms_out[8]);
 /* Development aid: per-phase SM-cycle counters of the image kernel (thread 0 of every CTA, summed over CTAs).
  * enable != 0 allocates / clears the counters, enable == 0 frees them; cycles_out (may be NULL) receives the
  * counters accumulated so far: [2] ball scan, [3] point channels, [4] shadow setup, [5] shadow casting,
- * [6] shadow bitmap pass, [7] shadow channels, [8] output flush. */
+ * [6] shadow bitmap pass, [7] shadow channels, [8] output flush. Event counts of the fast image kernel: [0] shadow
+ * cell-sum entries of projection 2 whose low word carried, [1] the most shadow voxels summed into one cell of
+ * projection 2, [14] shadow casts that walked the grid because the in-ball list was full. */
 int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]);
 
 /* Version / build info string (arch, lenet implementation). */
