@@ -1688,12 +1688,24 @@ int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]) 
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   if (ctx->d_prof && cycles_out)
     CUDA_TRY(cudaMemcpy(cycles_out, ctx->d_prof, sizeof(uint64_t) * 16, cudaMemcpyDeviceToHost));
-  if (enable && !ctx->d_prof) CUDA_TRY(cudaMalloc(&ctx->d_prof, sizeof(uint64_t) * 16));
-  if (enable) CUDA_TRY(cudaMemset(ctx->d_prof, 0, sizeof(uint64_t) * 16));
+  // slots 0..15: phase cycles and image events; 16..31: the path counters of gpdb_debug_path_counts (GPDB_PROF_PATH)
+  if (enable && !ctx->d_prof) CUDA_TRY(cudaMalloc(&ctx->d_prof, sizeof(uint64_t) * 32));
+  if (enable) CUDA_TRY(cudaMemset(ctx->d_prof, 0, sizeof(uint64_t) * 32));
   if (!enable && ctx->d_prof) {
     cudaFree(ctx->d_prof);
     ctx->d_prof = nullptr;
   }
+  return GPDB_OK;
+}
+
+int gpdb_debug_path_counts(gpdb_ctx *ctx, uint64_t counts_out[16]) {
+  if (!ctx || !counts_out) return GPDB_ERR_INVALID;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (ctx->d_prof)
+    CUDA_TRY(cudaMemcpy(counts_out, ctx->d_prof + GPDB_PROF_PATH, sizeof(uint64_t) * 16, cudaMemcpyDeviceToHost));
+  else
+    memset(counts_out, 0, sizeof(uint64_t) * 16);
   return GPDB_OK;
 }
 

@@ -110,6 +110,14 @@ struct CloudTable {
 // [3] hand-search tier-1 overflow count (informational), [4] normal-estimation capacity (final tier)
 #define GPDB_NERR 8
 
+// path counters (gpdb_debug_path_counts): d_prof[GPDB_PROF_PATH + e], counted only while the counters are on; the events
+// are listed in include/gpd_b200.h
+#define GPDB_PROF_PATH 16
+enum PathEvent {
+  PATH_FRAMES_T1, PATH_FRAMES_T2, PATH_HANDS_T2, PATH_HANDS_T3, PATH_HANDS_SLAB, PATH_IMG2_BOX, PATH_IMG2_NONUNIT, PATH_IMG_GL,
+  PATH_IMG2_CAST, PATH_IMG2_DRAW, PATH_IMG2_STASH, PATH_IMG_CAST, PATH_IMG_DRAW, PATH_IMG_STASH, PATH_IMG_BALL
+};
+
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
     cudaError_t e__ = (expr);                                                                 \
@@ -173,7 +181,7 @@ struct gpdb_ctx {
   void *scratch[24];
   size_t scratch_sz[24];
   int *d_err;
-  unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles), nullptr = off
+  unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles, 32 slots: PATH_* below), nullptr = off
   int64_t launches;
   double last_ms[8];
   double pre_ms[6];   // gpdb_preprocess stage timings

@@ -506,7 +506,8 @@ template <bool BATCH>
 __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevCloud cl0, CloudTable tab, const int *sidx, int n, int slot0,
                                                     const double *frames, const uint8_t *fvalid, gpdb_pose *poses,
                                                     uint8_t *flags, int cap, const int *in_list, const int *in_count,
-                                                    int *out_list, int *out_count, float4 *glist, int *err) {
+                                                    int *out_list, int *out_count, float4 *glist, int *err,
+                                                    unsigned long long *prof) {
   const DevParams &P = *Pp;
   extern __shared__ __align__(16) unsigned char dyn[];
   float4 *list = glist ? glist + (size_t)blockIdx.x * cap : reinterpret_cast<float4 *>(dyn);
@@ -774,6 +775,7 @@ __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevC
                 visitD(x, y, z, __float_as_int(p.w), 1);
               }
             } else {
+              if (prof && lane == 0) atomicAdd(prof + GPDB_PROF_PATH + PATH_HANDS_SLAB, 1ull);
               for (int a = lane; a < m; a += 32) {
                 float4 p = list[a];
                 double x, y, z;
@@ -1956,7 +1958,10 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         }
         __syncthreads();
         const int nw = min(sm.wl_n, WL_CAP);
-        if (prof && tid == 0) atomicAdd(prof + 9, (unsigned long long)nw);
+        if (prof && tid == 0) {
+          atomicAdd(prof + 9, (unsigned long long)nw);
+          if (sm.wl_n > WL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG_CAST, (unsigned long long)(sm.wl_n - WL_CAP));
+        }
         const int nsp = P.nsp;
         const unsigned nsp_magic = nsp > 1 ? (unsigned)((0x100000000ull + (unsigned)nsp - 1) / (unsigned)nsp) : 0u;  // ceil(2^32 / nsp)
         // Draws in two dense steps. (1) the cheap part of every (point, draw) pair — LCG skip-ahead + the window test of
@@ -2002,7 +2007,10 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         }
         __syncthreads();
         const int ndl = min(sm.dl_n, DL_CAP);
-        if (prof && tid == 0) atomicAdd(prof + 10, (unsigned long long)sm.dl_n);
+        if (prof && tid == 0) {
+          atomicAdd(prof + 10, (unsigned long long)sm.dl_n);
+          if (sm.dl_n > DL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG_DRAW, (unsigned long long)(sm.dl_n - DL_CAP));
+        }
         auto list_bit = [&](int i) -> int {
           if (i >= ndl) return -1;
           const unsigned code = dlist[i];
@@ -2087,6 +2095,8 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
         atomicAdd(prof + 11, (unsigned long long)sm.wl_n);
         atomicAdd(prof + 12, (unsigned long long)bn);
         atomicAdd(prof + 13, (unsigned long long)sm.n_img);
+        if (sm.wl_n > BL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG_STASH, 1ull);
+        if (sm.ball_n > BALL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG_BALL, 1ull);
       }
       for (int i = tid; i < nset; i += NT_IMG) eval_voxel(blist[i]);
       __syncthreads();
@@ -2412,7 +2422,10 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       sm.center[0] = a0 / nn;
       sm.center[1] = a1 / nn;
       sm.center[2] = a2 / nn;
-      if (sm.box_n > BOX_CAP2 || sm.nonunit) ovf[atomicAdd(ovf_count, 1)] = b;  // redone by k_images (larger list / exact fold)
+      if (sm.box_n > BOX_CAP2 || sm.nonunit) {
+        ovf[atomicAdd(ovf_count, 1)] = b;  // redone by k_images (larger list / exact fold)
+        if (prof) atomicAdd(prof + GPDB_PROF_PATH + (sm.box_n > BOX_CAP2 ? PATH_IMG2_BOX : PATH_IMG2_NONUNIT), 1ull);
+      }
     }
     __syncthreads();
     PHASE(2);
@@ -2711,7 +2724,10 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         }
         __syncthreads();
         const int nw = min(sm.wl_n, WL_CAP);
-        if (prof && tid == 0) atomicAdd(prof + 9, (unsigned long long)nw);
+        if (prof && tid == 0) {
+          atomicAdd(prof + 9, (unsigned long long)nw);
+          if (sm.wl_n > WL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG2_CAST, (unsigned long long)(sm.wl_n - WL_CAP));
+        }
         const int nsp = P.nsp;
         const unsigned nsp_magic = nsp > 1 ? (unsigned)((0x100000000ull + (unsigned)nsp - 1) / (unsigned)nsp) : 0u;
         const int nd = nw * nsp;
@@ -2746,7 +2762,10 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         }
         __syncthreads();
         const int ndl = min(sm.dl_n, DL_CAP);
-        if (prof && tid == 0) atomicAdd(prof + 10, (unsigned long long)sm.dl_n);
+        if (prof && tid == 0) {
+          atomicAdd(prof + 10, (unsigned long long)sm.dl_n);
+          if (sm.dl_n > DL_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG2_DRAW, (unsigned long long)(sm.dl_n - DL_CAP));
+        }
         auto list_bit = [&](int i) -> int {
           if (i >= ndl) return -1;
           const unsigned code = dlist[i];
@@ -2826,6 +2845,7 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         atomicAdd(prof + 11, (unsigned long long)nset_all);
         atomicAdd(prof + 12, (unsigned long long)bn);
         atomicAdd(prof + 13, (unsigned long long)sm.n_img);
+        if (nset_all > ST_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG2_STASH, 1ull);
       }
       for (int i = tid; i < nset; i += NT_IMG) stash[i] = eval_voxel(stash[i].x, 0, 2);
       __syncthreads();
@@ -3169,6 +3189,21 @@ int geo_build_grid(gpdb_ctx *ctx, const float lo[3], const float hi[3], int N) {
   return GPDB_OK;
 }
 
+__global__ void k_path_add(unsigned long long *prof, int e0, const int *n0, int e1, const int *n1) {
+  // atomic: the hand search of the next chunk may run on its own stream beside the image kernels of this one
+  atomicAdd(prof + GPDB_PROF_PATH + e0, (unsigned long long)(unsigned)*n0);
+  if (n1) atomicAdd(prof + GPDB_PROF_PATH + e1, (unsigned long long)(unsigned)*n1);
+}
+
+// path counters on: adds the lengths of the overflow lists of a tiered launch (n1 may be null) to the path counters. A
+// development aid, so not counted in ctx->launches (the launch count of a call is the same with the counters on or off).
+static int path_add(gpdb_ctx *ctx, int e0, const int *n0, int e1, const int *n1) {
+  if (!ctx->d_prof) return GPDB_OK;
+  k_path_add<<<1, 1, 0, ctx->stream>>>(ctx->d_prof, e0, n0, e1, n1);
+  CUDA_TRY(cudaGetLastError());
+  return GPDB_OK;
+}
+
 template <bool BATCH>
 static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
   const int cap0 = 128;  // ~44 points at the default nn_radius on a 3 mm cloud
@@ -3196,7 +3231,7 @@ static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, i
   k_frames<BATCH><<<g2, LRF_WARPS * 32, 0, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, d_frames, d_valid, ctx->d_err,
                                                           LRF_CAP_GLOBAL, ovf, ovf_count, ovf2, ovf2_count, gkeys, 2);
   LAUNCH_CHECK();
-  return GPDB_OK;
+  return path_add(ctx, PATH_FRAMES_T1, ovf_count, PATH_FRAMES_T2, ovf2_count);
 }
 
 int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
@@ -3222,19 +3257,20 @@ static int launch_hands(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, in
   const CloudTable tab = ctx->run;
   k_hands<BATCH><<<n, NT_HANDS, HANDS_CAP1 * 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames, d_valid, d_poses,
                                                                 d_flags, HANDS_CAP1, nullptr, nullptr, ovf, ovf_count, nullptr,
-                                                                ctx->d_err);
+                                                                ctx->d_err, ctx->d_prof);
   LAUNCH_CHECK();
   // large-tile pass over the samples whose neighbourhood did not fit tier 1 (persistent CTAs) ...
   k_hands<BATCH><<<ctx->sm_count, NT_HANDS, HANDS_CAP2 * 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames,
                                                                             d_valid, d_poses, d_flags, HANDS_CAP2, ovf,
-                                                                            ovf_count, ovf2, ovf2_count, nullptr, ctx->d_err);
+                                                                            ovf_count, ovf2, ovf2_count, nullptr, ctx->d_err,
+                                                                            ctx->d_prof);
   LAUNCH_CHECK();
   // ... and the last tier over what did not fit that either: neighbourhood in global memory (usually an empty list)
   k_hands<BATCH><<<ctx->sm_count, NT_HANDS, 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames, d_valid, d_poses,
                                                                d_flags, HANDS_CAP3, ovf2, ovf2_count, nullptr, nullptr, glist,
-                                                               ctx->d_err);
+                                                               ctx->d_err, ctx->d_prof);
   LAUNCH_CHECK();
-  return GPDB_OK;
+  return path_add(ctx, PATH_HANDS_T2, ovf_count, PATH_HANDS_T3, ovf2_count);
 }
 
 int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
@@ -3338,7 +3374,7 @@ static int launch_images(gpdb_ctx *ctx, const DevCloud &cl, const gpdb_pose *d_c
                                                                     gl, gl_cap, nullptr, nullptr);
   }
   LAUNCH_CHECK();
-  return GPDB_OK;
+  return path_add(ctx, PATH_IMG_GL, ovf2_count, 0, nullptr);
 }
 
 int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {

@@ -25,7 +25,13 @@ EXPORTS = [
     "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
     "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
+    "gpdb_debug_path_counts",
 ]
+
+# gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
+PATH_EVENTS = ["frames_tier1", "frames_tier2", "hands_tile", "hands_global", "hands_full_slab", "images2_box",
+               "images2_nonunit", "images_global", "images2_cast_in_place", "images2_draw_in_place", "images2_stash_full",
+               "images_cast_in_place", "images_draw_in_place", "images_voxel_list_full", "images_ball_record_full"]
 
 
 class GpdbError(RuntimeError):
@@ -66,6 +72,7 @@ def lib():
     L.gpdb_detect_resident.argtypes = [vp, vp, C.c_int32, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_set_stream.argtypes = [vp, vp]
     L.gpdb_debug_phase_cycles.argtypes = [vp, C.c_int, vp]
+    L.gpdb_debug_path_counts.argtypes = [vp, vp]
     L.gpdb_preprocess_params_default.argtypes = [C.POINTER(abi.PreprocessParams)]
     L.gpdb_preprocess.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, C.POINTER(abi.PreprocessParams)]
     L.gpdb_get_cloud.argtypes = [vp, vp, vp, vp]
@@ -507,6 +514,13 @@ class Context:
         out = np.zeros(16, np.uint64)
         self._check(lib().gpdb_debug_phase_cycles(self.h, enable, _p(out)))
         return out
+
+    def path_counts(self):
+        """gpdb_debug_path_counts as a dict (PATH_EVENTS): how often each tier or in-place fallback of the geometry kernels
+        ran since phase_cycles(1) enabled the counters (all zero while they are off)."""
+        out = np.zeros(16, np.uint64)
+        self._check(lib().gpdb_debug_path_counts(self.h, _p(out)))
+        return {name: int(out[i]) for i, name in enumerate(PATH_EVENTS)}
 
     def last_timings(self):
         ms = np.zeros(8)

@@ -415,6 +415,21 @@ int gpdb_last_timings(const gpdb_ctx *ctx, double ms_out[8]);
  * cell-sum entries of projection 2 whose low word carried, [1] the most shadow voxels summed into one cell of
  * projection 2, [14] shadow casts that walked the grid because the in-ball list was full. */
 int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]);
+/* Development aid: how often the geometry kernels left their first choice of list for a larger tier or an in-place
+ * fallback, counted while gpdb_debug_phase_cycles(ctx, 1, ...) has the counters enabled (summed since then; all zero when
+ * they are off). counts_out receives:
+ *  [0] k_frames samples re-run by tier 1 (ball over 128 keys)  [1] ... by tier 2 (over 1 024 keys)
+ *  [2] k_hands samples moved to the 12 800-point tile (staged list over 2 176 points)  [3] ... to the global-memory tier
+ *      (over 12 800)  [4] k_hands poses whose Antipodal passes walked the whole staged list (closing region over 1 024
+ *      points, or a staged list over 65 535)
+ *  [5] k_images2 images handed to k_images because the box holds over 1 024 points  [6] ... because a box point has a
+ *      normal of other than unit length  [7] k_images images redone by the global-memory box list (over 2 048 points)
+ *  [8] k_images2 shadow points cast in place (work list full)  [9] ... draws evaluated in place (draw list full)
+ *  [10] ... images whose shadow voxel stash overflowed
+ *  [11] k_images shadow points cast in place  [12] ... draws evaluated in place  [13] ... images whose shadow voxel
+ *       list overflowed  [14] ... shadow casts that walked the grid because the in-ball record (tile C) was full
+ *  [15] unused, zero. */
+int gpdb_debug_path_counts(gpdb_ctx *ctx, uint64_t counts_out[16]);
 
 /* Version / build info string (arch, lenet implementation). */
 const char *gpdb_build_info(void);
