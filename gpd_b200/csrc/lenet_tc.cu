@@ -15,13 +15,14 @@
 //          ONE instruction stream reads A once; the int32 dot products are exact and the epilogue recombines the three
 //          digits in float32 (see k_conv1_i8 below).
 //   conv2: activations a and weights w are scaled by powers of two (exact) and split in two fp16 terms each;
-//          D[:, 0:56] += a_hi w_hi + a_lo w_hi, D[:, 56:112] += a_hi w_lo  (error ~2^-22), summed in the epilogue.
-// Output pixels with x beyond the valid width are computed and discarded (7 % / 14 % of the rows).
+//          D += w_hi a_hi + w_lo a_hi + w_hi a_lo  (error ~2^-22), with the filters as M and the pixels as N.
+// Output pixels with x beyond the valid width are computed and discarded (7 % / 14 % of the rows / columns).
 //
 // conv1 computes a tile of 128 GEMM rows with two warpgroups (rows 0..63 | 64..127); conv2 is warp-specialised: a converter
-// warpgroup feeds two consumer warpgroups that each own whole 128-row tiles and alternate on the tensor cores. The
-// weights stay resident in shared memory (26.6 KB / 115.5 KB). The 2x2 max-pool + bias (+ReLU for the 12-channel net) is
-// fused into the epilogue: registers -> x-pair max by shuffle -> small smem stage -> y-pair max -> global.
+// warpgroup feeds two consumer warpgroups that each own whole 224-column tiles and alternate on the tensor cores. The
+// weights stay resident in shared memory (26.6 KB / 132 KB). The 2x2 max-pool + bias (+ReLU for the 12-channel net) is
+// fused into the epilogue: conv1: registers -> x-pair max by shuffle -> small smem stage -> y-pair max -> global;
+// conv2: x-pair max in registers -> y-pair max by shuffle -> small smem stage -> global.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -154,27 +155,39 @@ __global__ void __launch_bounds__(C1_NT, C1_CTAS_PER_SM) k_conv1_i8(const uint8_
 
 // ---------------------------------------------------------------------------------------------------------
 // conv2: P1 [784 px][20] f32 -> ip1's fp16 hi/lo operand xc (k = c + 50 j, j = 12x12 pooled pixel), max-pooled.
-// Tile T (6 per image) = output rows 4T .. 4T+3 = GEMM rows m = y*28 + x (112 of 128) over the EIGHT input rows
-// 4T .. 4T+7 (224 consecutive P1 pixels, 17.5 KB), held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two
-// pixels, see c2_off) of 232 pixels. The 4 halo rows of a tile are converted twice. One CTA per SM, three warpgroups:
-//   warpgroup 0, converter: one bulk copy per tile brings its float32 pixels into a raw buffer (two, filled two tiles
-//     ahead); the warpgroup converts them to the scaled fp16 hi/lo planes of a plane stage and arrives on its `full` barrier.
+// Transposed implicit GEMM: M = the 50 filters (padded to 64) = the weights as the A operand, N = 224 output pixels, K = taps x
+// channels. Tile T (3 per image) = output rows 8T .. 8T+7 = GEMM columns n = y*28 + x over the TWELVE input rows 8T .. 8T+11
+// (336 consecutive P1 pixels, 26.25 KB), held as six fp16 channel planes (hi p0..2, lo p0..2; plane 2 pairs two pixels, see
+// c2_off) of 344 pixels. The 4 halo rows of a tile are converted twice. One CTA per SM, three warpgroups:
+//   warpgroup 0, converter: loads a tile's float32 pixels from global memory (L2: a bulk prefetch pulls each tile in two
+//     tiles ahead) straight into registers, converts them to the scaled fp16 hi/lo planes of a plane stage and arrives on
+//     its `full` barrier.
 //   warpgroups 1, 2, consumers: consumer c owns the tiles g = c, c + 2, ... of the CTA's sequence (and plane stage c) and
-//     issues both m64 halves of each. Named barriers order the two consumers' instruction batches (ping-pong), so the
-//     tensor cores run one consumer's tile while the other runs its epilogue (x-pair max by shuffle -> own stage ->
-//     y-pair max + bias -> 16-byte stores of 8 consecutive k of xc).
-// N = 112 + 56: D[:, 0:56] += a_hi w_hi + a_lo w_hi, D[:, 56:112] += a_hi w_lo (w rows 50..55 / 106..111 are zero).
+//     issues 33 x 3 m64n224k16 per tile. Named barriers order the two consumers' instruction batches (ping-pong), so the
+//     tensor cores run one consumer's tile while the other runs its epilogue (x-pair max in registers, y-pair max by
+//     shuffle -> own stage -> bias -> 16-byte stores of 8 consecutive k of xc).
+// The three products w_hi a_hi, w_lo a_hi, w_hi a_lo land on the same output element at the same scale: ONE accumulator.
+// An instruction reads 2 KB of weights + 7 KB of pixels per 112 tensor clocks (~82 B / clock of shared memory), and a
+// tile's batch runs 11 088 tensor clocks, so the consumers hand the tensor cores over half as often per pixel as with
+// 128-pixel tiles.
 // ---------------------------------------------------------------------------------------------------------
-constexpr int C2_W = 28, C2_NPIX = 232, C2_PLANE = C2_NPIX * 16, C2_NCH = 65, C2_NMMA = 33;
-constexpr int C2_N = 112, C2_BCHUNK = C2_N * 16;  // B rows per K-chunk: 0..55 w_hi, 56..111 w_lo
-constexpr int C2_B_BYTES = 2 * C2_NMMA * C2_BCHUNK;
-constexpr int C2_TILES = 6, C2_TILE_PIX = 8 * C2_W;  // 224 input pixels per tile
-constexpr int C2_STAGE = 6 * C2_PLANE;               // one plane stage: hi p0..2, lo p0..2
-constexpr int C2_RAW_BYTES = C2_TILE_PIX * 20 * 4;   // a tile's float32 input pixels
-constexpr int C2_STG_FLOATS = 56 * 50;               // x-pooled rows of a tile [dy 0..3][x/2 0..13][50]
+constexpr int C2_W = 28, C2_NCH = 65, C2_NMMA = 33;
+constexpr int C2_TILES = 3, C2_N = 8 * C2_W, C2_TILE_PIX = 12 * C2_W;  // 224 GEMM columns over 336 input pixels per tile
+constexpr int C2_NPIX = C2_TILE_PIX + 8, C2_PLANE = C2_NPIX * 16;      // + an 8-pixel zero tail
+constexpr int C2_ACHUNK = 2 * 64 * 16;                                  // one K-chunk of A: w_hi rows 0..63, w_lo rows 0..63
+constexpr int C2_A_BYTES = 2 * C2_NMMA * C2_ACHUNK;                    // 66 chunks (the last one zero)
+constexpr int C2_STAGE = 6 * C2_PLANE;                                  // one plane stage: hi p0..2, lo p0..2
+constexpr int C2_STG_FLOATS = 4 * 12 * 50;                              // a tile's pooled outputs [py 0..3][px 0..11][50]
 constexpr int C2_NT = 384;
+// Shared memory: [A: 66 chunks x (hi, lo) x 64 rows x 16 B = 135 168 B][2 plane stages x 6 x 344 px x 16 B = 66 048 B]
+// [2 pooled stages x 2 400 floats = 19 200 B] = 220 416 B dynamic. GEMM column n of chunk c reads pixel n + c2_off(c) / 16
+// (+1 for the zero chunk 65, LBO 16), at most 223 + 4 * 28 + 4 + 1 = 340 of its plane: pixels 336..343 are the zero tail,
+// written once, and only columns with x >= 24 (discarded) reach them, except as a right neighbour of plane 2 whose
+// weights (tap kw = 5) are zero. The valid tap reads of a column stay in its own row, so nothing else crosses planes.
+constexpr int C2_SMEM = C2_A_BYTES + 2 * C2_STAGE + 2 * C2_STG_FLOATS * 4;
+static_assert(C2_SMEM + 64 * 4 + 4 * 8 <= 227 * 1024, "conv2: dynamic + static shared memory above the opt-in limit");
 constexpr int IP_K = 7200, IP_KCH = IP_K / 8;  // ip1 reduction length, in 8-element chunks
-// K-chunks (8 fp16 = 16 B per GEMM row): c < 50: plane p = c / 25 (channels 8p .. 8p+7), tap (kh, kw) = c % 25.
+// K-chunks (8 fp16 = 16 B per GEMM column): c < 50: plane p = c / 25 (channels 8p .. 8p+7), tap (kh, kw) = c % 25.
 // c >= 50: plane 2 holds, per pixel, channels 16..19 of that pixel AND of its right neighbour, so one chunk covers the two
 // taps (kh, 2j) and (kh, 2j+1) of the last four channels, j = (c - 50) % 3, kh = (c - 50) / 3 (the tap kw = 5 of j = 2 has
 // zero weights): 65 chunks instead of 75 with a zero-padded third plane (-13 % tensor-core work).
@@ -189,61 +202,52 @@ __global__ void __launch_bounds__(C2_NT, 1) k_conv2_tc(const float *__restrict__
                                                        __half *__restrict__ xc, float x_scale) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ float sbias[64];
-  __shared__ uint64_t raw_full[2], full[2], empty[2];
-  uint8_t *sB = smem;                    // 66 chunks x 112 rows x 16 B
-  uint8_t *sPl = sB + C2_B_BYTES;        // 2 plane stages
-  // the x-pooled stages of the two consumers follow the planes: the unused GEMM rows 112..127 of the last plane read up to
-  // 192 B past the plane stages, and those bytes must exist (the values only reach discarded rows)
-  float *stg = reinterpret_cast<float *>(sPl + 2 * C2_STAGE);
-  float *raw = stg + 2 * C2_STG_FLOATS;  // 2 x [224 px][20] float32
+  __shared__ uint64_t full[2], empty[2];
+  uint8_t *sA = smem;                   // 66 chunks x (w_hi | w_lo) x 64 rows x 16 B
+  uint8_t *sPl = sA + C2_A_BYTES;       // 2 plane stages
+  float *stg = reinterpret_cast<float *>(sPl + 2 * C2_STAGE);  // the pooled stages of the two consumers
   const int tid = threadIdx.x, wg_id = tid >> 7, wt = tid & 127, warp = wt >> 5, lane = tid & 31, q = lane & 3;
 
-  for (int i = tid; i < C2_B_BYTES / 16; i += C2_NT) reinterpret_cast<uint4 *>(sB)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
-  // the 8-pixel tail of every plane is read by valid rows (as zero A elements) and never written again
+  for (int i = tid; i < C2_A_BYTES / 16; i += C2_NT) reinterpret_cast<uint4 *>(sA)[i] = reinterpret_cast<const uint4 *>(wblob)[i];
   for (int i = tid; i < 2 * 6 * 8; i += C2_NT)
     reinterpret_cast<uint4 *>(sPl + (i >> 3) * C2_PLANE + (C2_TILE_PIX + (i & 7)) * 16)[0] = make_uint4(0, 0, 0, 0);
   if (tid < 64) sbias[tid] = tid < NF2 ? bias[tid] : 0.0f;
   if (tid == 0) {
     for (int s = 0; s < 2; s++) {
-      wg::mbar_init(&raw_full[s], 1);  // the expect_tx arrival + the bulk copy's bytes
-      wg::mbar_init(&full[s], 128);    // every converter thread, after its own proxy fence
-      wg::mbar_init(&empty[s], 4);     // one arrival per consumer warp
+      wg::mbar_init(&full[s], 128);  // every converter thread, after its own proxy fence
+      wg::mbar_init(&empty[s], 4);   // one arrival per consumer warp
     }
     wg::fence_mbar_init();
   }
   wg::fence_async_smem();  // weights and zero tails (generic proxy) before the tensor-core reads (async proxy)
   __syncthreads();
 
-  // the CTA's tiles g = 0 .. G-1: image blockIdx.x + (g / 6) * gridDim.x, tile g % 6
+  // the CTA's tiles g = 0 .. G-1: image blockIdx.x + (g / 3) * gridDim.x, tile g % 3
   const int G = C2_TILES * ((n - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x);
-  auto tile_image = [&](int g) { return (int)blockIdx.x + (g / C2_TILES) * (int)gridDim.x; };
+  auto tile_src = [&](int g) {
+    return p1 + ((size_t)blockIdx.x + (size_t)(g / C2_TILES) * gridDim.x) * 784 * NF1 + (size_t)(g % C2_TILES) * 8 * C2_W * NF1;
+  };
 
   if (wg_id == 0) {
     // ===== converter
     wg::setmaxnreg_dec<40>();
-    auto fetch = [&](int g) {
-      const int s = g & 1;
-      wg::mbar_expect_tx(&raw_full[s], C2_RAW_BYTES);
-      wg::bulk_g2s(raw + s * (C2_RAW_BYTES / 4),
-                   p1 + (size_t)tile_image(g) * 784 * NF1 + (size_t)(g % C2_TILES) * 4 * C2_W * NF1, C2_RAW_BYTES,
-                   &raw_full[s]);
-    };
     if (wt == 0)
-      for (int g = 0; g < 2 && g < G; g++) fetch(g);
+      for (int g = 0; g < 2 && g < G; g++) wg::bulk_prefetch_l2(tile_src(g), C2_TILE_PIX * NF1 * 4);
     for (int g = 0; g < G; g++) {
       const int s = g & 1;
-      const float *rs = raw + s * (C2_RAW_BYTES / 4);
+      const float *rs = tile_src(g);
       uint8_t *pl = sPl + s * C2_STAGE;
-      wg::mbar_wait(&raw_full[s], (g >> 1) & 1);
+      if (wt == 0 && g + 2 < G) wg::bulk_prefetch_l2(tile_src(g + 2), C2_TILE_PIX * NF1 * 4);
       wg::mbar_wait(&empty[s], ((g >> 1) & 1) ^ 1);
-      // (pixel, plane) items: 224 x 3; plane 2 takes channels 16..19 of the pixel and of its right neighbour
+      // (pixel, plane) items: 336 x 3; plane 2 takes channels 16..19 of the pixel and of its right neighbour
+#pragma unroll 2
       for (int i = wt; i < C2_TILE_PIX * 3; i += 128) {
         const int lp = i / 3, p = i - lp * 3;
         const float *src = rs + lp * NF1 + p * 8;
-        const float4 x0 = *reinterpret_cast<const float4 *>(src);
+        const float4 x0 = __ldg(reinterpret_cast<const float4 *>(src));
         float4 x1 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p < 2) x1 = *reinterpret_cast<const float4 *>(src + 4);
-        else if (lp + 1 < C2_TILE_PIX) x1 = *reinterpret_cast<const float4 *>(src + NF1);
+        if (p < 2) x1 = __ldg(reinterpret_cast<const float4 *>(src + 4));
+        else if (lp + 1 < C2_TILE_PIX) x1 = __ldg(reinterpret_cast<const float4 *>(src + NF1));
         const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
         __half hi[8], lo[8];
 #pragma unroll
@@ -257,10 +261,6 @@ __global__ void __launch_bounds__(C2_NT, 1) k_conv2_tc(const float *__restrict__
       }
       wg::fence_async_smem();  // this thread's plane writes -> the tensor-core reads
       wg::mbar_arrive(&full[s]);
-      if (g + 2 < G) {
-        wg::bar_sync(5, 128);  // every converter thread has read raw buffer s before the copy overwrites it
-        if (wt == 0) fetch(g + 2);
-      }
     }
     return;
   }
@@ -268,72 +268,64 @@ __global__ void __launch_bounds__(C2_NT, 1) k_conv2_tc(const float *__restrict__
   // ===== consumers
   wg::setmaxnreg_inc<232>();
   const int c = wg_id - 1;
-  const uint32_t arow = wg::smem_u32(sPl) + (uint32_t)c * C2_STAGE, sB_u = wg::smem_u32(sB);
+  const uint32_t bpl = wg::smem_u32(sPl) + (uint32_t)c * C2_STAGE, sA_u = wg::smem_u32(sA);
   float *st = stg + c * C2_STG_FLOATS;
   for (int g = c; g < G; g += 2) {
-    const int im = tile_image(g), T = g % C2_TILES;
+    const int im = (int)blockIdx.x + (g / C2_TILES) * (int)gridDim.x, T = g % C2_TILES;
     // this consumer's batch goes after the other's previous one; the barrier also orders the previous epilogue's stage
     // reads (all 128 threads) before this tile's stage writes
     if (g > 0) wg::bar_sync(1 + c, 256);
     wg::mbar_wait(&full[c], (g >> 1) & 1);
-    float d[2][56];
+    float d[C2_N / 2];
     wg::fence();
 #pragma unroll
-    for (int i = 0; i < C2_NMMA; i++) {  // a_hi x [w_hi | w_lo]
+    for (int i = 0; i < C2_NMMA; i++) {  // w_hi a_hi + w_lo a_hi + w_hi a_lo
       const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
       const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-      const uint64_t db = wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128);
-#pragma unroll
-      for (int hh = 0; hh < 2; hh++) wg::mma_f16_n112(d[hh], wg::desc(arow + hh * 64 * 16 + a0, lbo, 128), db, i > 0);
-    }
-#pragma unroll
-    for (int i = 0; i < C2_NMMA; i++) {  // a_lo x w_hi
-      const uint32_t a0 = c2_off(2 * i), a1 = c2_off(2 * i + 1);
-      const uint32_t lbo = (2 * i + 1 >= C2_NCH) ? 16u : (a1 - a0);
-      const uint64_t db = wg::desc(sB_u + (uint32_t)(2 * i) * C2_BCHUNK, C2_BCHUNK, 128);
-#pragma unroll
-      for (int hh = 0; hh < 2; hh++)
-        wg::mma_f16_n56(d[hh], wg::desc(arow + 3 * C2_PLANE + hh * 64 * 16 + a0, lbo, 128), db, true);
+      const uint64_t whi = wg::desc(sA_u + (uint32_t)(2 * i) * C2_ACHUNK, C2_ACHUNK, 128);
+      const uint64_t wlo = wg::desc(sA_u + (uint32_t)(2 * i) * C2_ACHUNK + 64 * 16, C2_ACHUNK, 128);
+      const uint64_t ahi = wg::desc(bpl + a0, lbo, 128), alo = wg::desc(bpl + 3 * C2_PLANE + a0, lbo, 128);
+      wg::mma_f16_n224(d, whi, ahi, i > 0);
+      wg::mma_f16_n224(d, wlo, ahi, true);
+      wg::mma_f16_n224(d, whi, alo, true);
     }
     wg::commit();
     if (g + 1 < G) wg::bar_arrive(2 - c, 256);  // the other consumer may issue its next batch
     wg::wait<0>();
-    wg::reg_fence(d[0]);
-    wg::reg_fence(d[1]);
+    wg::reg_fence(d);
     if (lane == 0) wg::mbar_arrive(&empty[c]);
-    // columns c and 56 + c are values i and i + 28 of the same thread; rows r, r + 1 are lanes l, l ^ 4
+    // value 4 j + 2 h + e of this thread: filter 16 warp + lane / 4 + 8 h, column 8 j + 2 q + e, so the x-pair
+    // (e = 0, 1) is in the thread: column pair cp = 4 j + q = 14 y + x / 2. Its y-partner cp + 14 = 4 (j + 3) + q + 2
+    // (q < 2) or 4 (j + 4) + q - 2 (q >= 2) is in lane l ^ 2, which sends the pair the receiver needs.
 #pragma unroll
-    for (int hh = 0; hh < 2; hh++)
+    for (int h = 0; h < 2; h++) {
+      const int ch = 16 * warp + (lane >> 2) + 8 * h;
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int r = hh * 64 + warp * 16 + (lane >> 2) + 8 * h, rr = r >> 1;  // rr = [dy 0..3][x/2 0..13]
-        const bool wr = (r & 1) == 0 && r < 112 && (rr % 14) < 12;
-#pragma unroll
-        for (int j = 0; j < 7; j++)
-#pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int i = 4 * j + 2 * h + e, ch = 8 * j + 2 * q + e;
-            float v = (d[hh][i] + d[hh][i + 28]) * out_scale;
-            v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
-            if (wr && ch < NF2) st[rr * NF2 + ch] = v;
-          }
+      for (int j = 0; j < C2_N / 8; j++) {
+        const int j3 = j + 3 < C2_N / 8 ? j + 3 : C2_N / 8 - 1, j4 = j + 4 < C2_N / 8 ? j + 4 : C2_N / 8 - 1;
+        const float mine = fmaxf(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+        const float send = q >= 2 ? fmaxf(d[4 * j3 + 2 * h], d[4 * j3 + 2 * h + 1]) : fmaxf(d[4 * j4 + 2 * h], d[4 * j4 + 2 * h + 1]);
+        const float v = fmaxf(mine, __shfl_xor_sync(0xffffffffu, send, 2)) * out_scale;
+        const int cp = 4 * j + q, y = cp / 14, px = cp - 14 * y;
+        if ((y & 1) == 0 && px < 12 && ch < NF2) st[((y >> 1) * 12 + px) * NF2 + ch] = v;
       }
+    }
     wg::bar_sync(3 + c, 128);
-    // the tile's 2 x 12 x 50 = 1200 consecutive k (from 1200 T) are 150 whole 8-element chunks of ip1's A operand:
+    // the tile's 4 x 12 x 50 = 2400 consecutive k (from 2400 T) are 300 whole 8-element chunks of ip1's A operand:
     // [tile im/128][hi|lo][k/8][row im%128][k%8] fp16, scaled by x_scale
     __half *xrow = xc + (size_t)(im >> 7) * 2 * IP_KCH * 128 * 8 + (size_t)(im & 127) * 8;
-    for (int ci = wt; ci < 150; ci += 128) {
+    for (int ci = wt; ci < C2_STG_FLOATS / 8; ci += 128) {
       __half hi[8], lo[8];
 #pragma unroll
       for (int e = 0; e < 8; e++) {
-        const int kk = 8 * ci + e, qq = kk / 600, px = (kk % 600) / NF2, ch = kk % NF2;  // kk = 600 qq + 50 px + ch
-        float m = fmaxf(st[((2 * qq) * 14 + px) * NF2 + ch], st[((2 * qq + 1) * 14 + px) * NF2 + ch]) + sbias[ch];
+        const int kk = 8 * ci + e;
+        float m = st[kk] + sbias[kk % NF2];
         if (relu) m = fmaxf(m, 0.0f);
         const float a = m * x_scale;
         hi[e] = __float2half_rn(a);
         lo[e] = __float2half_rn(a - __half2float(hi[e]));
       }
-      __half *dst = xrow + (size_t)(150 * T + ci) * 128 * 8;
+      __half *dst = xrow + (size_t)(C2_STG_FLOATS / 8 * T + ci) * 128 * 8;
       *reinterpret_cast<uint4 *>(dst) = *reinterpret_cast<uint4 *>(hi);
       *reinterpret_cast<uint4 *>(dst + (size_t)IP_KCH * 128 * 8) = *reinterpret_cast<uint4 *>(lo);
     }
@@ -477,7 +469,8 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
           }
     }
   }
-  // conv2 blob: [chunk c][row n: 0..55 = w_hi (50 used), 56..111 = w_lo][8 x fp16], weights scaled by 2^k
+  // conv2 blob (the A operand): [chunk c (66, last zero)][w_hi | w_lo][filter row 0..63 (50 used)][8 x fp16], weights
+  // scaled by 2^k
   float mx = 0.0f;
   for (size_t i = 0; i < (size_t)NF2 * NF1 * 25; i++) mx = std::fmax(mx, std::fabs(w[2][i]));
   t.w2_scale = pow2_scale(mx, 16.0f);
@@ -510,7 +503,7 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
     return std::ldexp(1.0f, std::max(lo, std::min(hi, j)));
   };
   t.a2_scale = safe_scale(a1_bound, t.w2_scale);
-  std::vector<__half> b2((size_t)(2 * C2_NMMA) * C2_N * 8, __float2half(0.0f));
+  std::vector<__half> b2((size_t)C2_A_BYTES / 2, __float2half(0.0f));
   for (int c = 0; c < C2_NCH; c++) {
     for (int o = 0; o < NF2; o++)
       for (int e = 0; e < 8; e++) {
@@ -524,8 +517,8 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
         float wv = w[2][(((size_t)o * NF1 + ch) * 5 + kh) * 5 + kw] * t.w2_scale;
         __half hi = __float2half_rn(wv);
         __half lo = __float2half_rn(wv - __half2float(hi));
-        b2[((size_t)c * C2_N + o) * 8 + e] = hi;
-        b2[((size_t)c * C2_N + C2_N / 2 + o) * 8 + e] = lo;
+        b2[((size_t)(2 * c) * 64 + o) * 8 + e] = hi;
+        b2[((size_t)(2 * c + 1) * 64 + o) * 8 + e] = lo;
       }
   }
   // ip1 blob: [o-block 4][K-block 150][chunk 6][row 256: 0..127 w_hi(o), 128..255 w_lo(o)][8 x fp16], W(o,k) = w[4][o + 500 k]
@@ -572,7 +565,7 @@ int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, _
   const LenetTc &t = ctx->tc;
   const int relu = ctx->prm.relu_after_conv;
   size_t sm1 = (size_t)C1_B_BYTES + C1_PLANE + 2 * C1_STAGE_FLOATS * sizeof(float);
-  size_t sm2 = (size_t)C2_B_BYTES + 2 * C2_STAGE + 2 * C2_STG_FLOATS * sizeof(float) + 2 * C2_RAW_BYTES;
+  size_t sm2 = (size_t)C2_SMEM;
   size_t sm3 = (size_t)IP_STAGES * IP_STAGE_BYTES;
   CUDA_TRY(cudaFuncSetAttribute(k_conv1_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
   CUDA_TRY(cudaFuncSetAttribute(k_conv2_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
