@@ -181,21 +181,29 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
   const bool is_root = cs.rank == root;
   // header: N, K, validity of the root's arguments, the view points
   double hdr[4 + 3 * GPDB_MAX_CAMERAS] = {0};
+  std::vector<uint8_t> cam;  // the root's camera masks (a camera sees a point when its entry is > 0, as gpdb_set_cloud)
+  CloudDesc desc;
   if (is_root) {
     bool ok = xyz && normals && view_points && N > 0 && K > 0 && K <= GPDB_MAX_CAMERAS;
     if (ok)
       for (size_t i = 0; i < 3 * (size_t)N && ok; i++) ok = std::isfinite(xyz[i]);
+    if (ok) {  // a failure here is reported through the header too: every rank waits in its broadcast
+      const int32_t off[2] = {0, N};
+      cam.resize((size_t)N);
+      ok = gpdb_pack_cameras(ctx, "gpdb_set_cloud_bcast", 1, off, cam_source, &K, view_points, false, false, cam.data(),
+                             &desc) == GPDB_OK;
+    }
     hdr[0] = ok ? N : -1;
     hdr[1] = K;
-    bool all_seen = true;
-    if (ok && cam_source)
-      for (size_t i = 0; i < (size_t)N * K && all_seen; i++) all_seen = cam_source[i] > 0;
-    hdr[2] = all_seen ? 1 : 0;
-    if (ok) memcpy(hdr + 4, view_points, sizeof(double) * 3 * (size_t)K);
+    if (ok) {
+      hdr[2] = desc.all_seen;
+      memcpy(hdr + 4, view_points, sizeof(double) * 3 * (size_t)K);
+    }
   }
   double *d_hdr = (double *)gpdb_scratch(ctx, 4, sizeof(hdr));
   if (!d_hdr) return GPDB_ERR_CUDA;
-  ctx->cloud_set = false;
+  CloudSet &s = ctx->one;
+  s.n = 0;
   if (is_root) CUDA_TRY(cudaMemcpyAsync(d_hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, ctx->stream));
   NCCL_TRY(g_nccl.Broadcast(d_hdr, d_hdr, sizeof(hdr), ncclUint8, root, cs.comm, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(hdr, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, ctx->stream));
@@ -207,27 +215,24 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
   }
   N = (int32_t)hdr[0];
   K = (int32_t)hdr[1];
-  if ((rc = gpdb_cloud_reserve(ctx, (size_t)N)) != GPDB_OK) return rc;
+  if ((rc = gpdb_cloud_reserve(ctx, s, (size_t)N, 1)) != GPDB_OK) return rc;
   if (is_root) {
-    std::vector<uint8_t> cam((size_t)N, (uint8_t)((1u << K) - 1));
-    if (cam_source)
-      for (int i = 0; i < N; i++) {
-        uint8_t m = 0;
-        for (int k = 0; k < K; k++)
-          if (cam_source[(size_t)i * K + k] > 0) m |= (uint8_t)(1u << k);
-        cam[i] = m;
-      }
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_xyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_nrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_cam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // `cam` goes out of scope
+    CUDA_TRY(cudaMemcpyAsync(s.xyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.nrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.cam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
   }
   NCCL_TRY(g_nccl.GroupStart());
-  NCCL_TRY(g_nccl.Broadcast(ctx->d_xyz, ctx->d_xyz, sizeof(float) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
-  NCCL_TRY(g_nccl.Broadcast(ctx->d_nrm, ctx->d_nrm, sizeof(double) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
-  NCCL_TRY(g_nccl.Broadcast(ctx->d_cam, ctx->d_cam, (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
+  NCCL_TRY(g_nccl.Broadcast(s.xyz, s.xyz, sizeof(float) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
+  NCCL_TRY(g_nccl.Broadcast(s.nrm, s.nrm, sizeof(double) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
+  NCCL_TRY(g_nccl.Broadcast(s.cam, s.cam, (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
   NCCL_TRY(g_nccl.GroupEnd());
-  if ((rc = gpdb_install_device_cloud(ctx, N, K, hdr + 4, (int)hdr[2])) != GPDB_OK) return rc;
+  memset(&desc, 0, sizeof(desc));
+  desc.K = K;
+  desc.all_seen = (int)hdr[2];
+  for (int k = 0; k < K; k++)
+    for (int r = 0; r < 3; r++) desc.vp[k][r] = hdr[4 + 3 * k + r];
+  const int off[2] = {0, N};
+  if ((rc = gpdb_install_clouds(ctx, s, &desc, off, 1, true)) != GPDB_OK) return rc;
   return N;
 }
 
@@ -251,7 +256,7 @@ int gpdb_detect_sharded_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx_loca
     CUDA_TRY(cudaMemsetAsync(d_scores + a, 0xFF, sizeof(float) * (b - a), ctx->stream));
     CUDA_TRY(cudaMemsetAsync(d_flags + a, 0, b - a, ctx->stream));
   }
-  int nc = gpdb_run_pipeline(ctx, d_sample_idx_local, n_local, stats, true, true, d_flags, d_scores, -1, 0);
+  int nc = gpdb_run_pipeline(ctx, ctx->one, d_sample_idx_local, n_local, stats, true, true, d_flags, d_scores, -1, 0);
   if (nc < 0) return nc;
   cs.count = nc;
   CUDA_TRY(cudaMemcpyAsync(mine + slot - 16, &cs.count, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -274,7 +279,7 @@ int gpdb_detect_sharded(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpd
   int32_t lo, hi, slot_samples;
   gpdb_shard_bounds(n, cs.rank, cs.nranks, &lo, &hi, &slot_samples);
   // this rank's slice through the host-buffer pipeline (pose records of the slice -> pinned arena, sample_slot global)
-  int nc = gpdb_run_pipeline(ctx, sample_idx + lo, hi - lo, out, true, false, nullptr, nullptr, -1, lo);
+  int nc = gpdb_run_pipeline(ctx, ctx->one, sample_idx + lo, hi - lo, out, true, false, nullptr, nullptr, -1, lo);
   if (nc < 0) return nc;
   // the pipeline left the slice's dense flags / scores in its device scratch (slots 10 / 11): pack them into this
   // rank's slot and all-gather

@@ -1,12 +1,14 @@
 // common.cuh — shared declarations of libgpd_b200.so (sm_90a only).
 //
-// HBM layout of one context (see DESIGN.md "data layout"):
-//   cloud   pts4   float4[N]  points SORTED BY GRID CELL: x,y,z + original index bits  (4.8 MB @300k)
-//           xyz    float[3N]  points by original index (nb0 lookups)
-//           nrm    double[3N] normals by original index, 3xN column-major as the ABI gives them
-//           cam    uint8[N]   bit k set when camera k sees the point
-//           cell_start int[ncell+1]   uniform grid, x fastest: a run of cells along x is ONE
+// HBM layout of one context (see DESIGN.md "data layout"): two cloud stores (CloudSet), `one` for the single cloud and
+// `many` for a batch, each holding the concatenated points of its clouds:
+//   store   pts4   float4[N]  points SORTED BY (CLOUD, GRID CELL): x,y,z + cloud-local index bits  (4.8 MB @300k)
+//           xyz    float[3N]  points by concatenated index (nb0 lookups)
+//           nrm    double[3N] normals by concatenated index, 3xN column-major as the ABI gives them
+//           cam    uint8[N]   bit k set when camera k of the point's cloud sees the point
+//           cell_start int[ncell+1]   one uniform grid per cloud, x fastest: a run of cells along x is ONE
 //                                     contiguous segment of pts4
+//           desc   CloudDesc[n]       per cloud: grid, point range, cameras
 //   per chunk of samples: frames double[9n], dense pose records gpdb_pose[n*P], flags uint8[n*P],
 //           compact candidate list gpdb_pose[nc], images uint8[nc*S*S*C] (HWC, the cv::Mat layout),
 //           LeNet activations.
@@ -54,14 +56,6 @@ struct DevParams {
   // radii: float32 predicates (dist < r2) and search extents
   float r2_lrf, r2_hs, r2_img;
   float rf_lrf, rf_hs, rf_img;
-  // grid
-  float lo[3], inv_cell;
-  int dim[3];
-  // cloud
-  int N, K;
-  int all_seen;                // every point is seen by every camera (cam mask complete): the per-point masks need not be read
-  int nonunit;                 // some normal is not of unit length (unit_normal): images holding one fold their cells exactly
-  double vp[GPDB_MAX_CAMERAS][3];
   // LeNet
   int relu_after_conv;
 };
@@ -87,23 +81,47 @@ struct DevCloud {
   int n_points;
 };
 
-// One cloud of a batch (gpdb_set_clouds): the fields of DevParams that are per cloud, under the same names, so that the
-// grid helpers (grid.cuh) and the kernels read either. The clouds' arrays are concatenated; pts4 is sorted by
-// (cloud, cell) and its w bits hold the CLOUD-LOCAL index, so keys, shadow seeds and pose records match a single-cloud run.
+// One cloud of a store: its grid, its range of the concatenated arrays and its cameras. pts4 is sorted by (cloud, cell)
+// and its w bits hold the CLOUD-LOCAL index, so keys, shadow seeds and pose records of a cloud do not depend on the
+// clouds stored beside it.
 struct CloudDesc {
   float lo[3], inv_cell;
   int dim[3];
-  int cell_base;              // first entry of this cloud's cells in the batch's cell_start
+  int cell_base;              // first entry of this cloud's cells in the store's cell_start
   int off, N, K;              // first point in the concatenated arrays, points, cameras
-  int all_seen, nonunit;
+  int all_seen;               // every point is seen by every camera (cam mask complete): the per-point masks need not be read
+  int nonunit;                // some normal is not of unit length (unit_normal): images holding one fold their cells exactly
   double vp[GPDB_MAX_CAMERAS][3];
 };
-// The clouds of the current batch call: d[n] descriptors, soff[n+1] the CSR offsets of the call's samples per cloud
-// (a sample's position in the call = its sample slot). n == 0: the single cloud of the context.
+// The clouds of a store as the kernels see them: d[n] descriptors, soff[n+1] the CSR offsets of the running batch call's
+// samples per cloud (a sample's position in the call = its sample slot).
 struct CloudTable {
   const CloudDesc *d;
   const int *soff;
   int n;
+};
+
+// A store of clouds. Its arrays are grow-only arenas (repeated installs, one per camera frame, do not pay cudaMalloc /
+// cudaFree); n == 0: nothing installed. The context keeps two, `one` and `many`, and a call on one never touches the other.
+struct CloudSet {
+  float4 *pts4;
+  float *xyz;
+  double *nrm;
+  uint8_t *cam;
+  int *src;             // cloud-local raw index of each point (valid after preprocessing: has_src)
+  int *cell_start;
+  CloudDesc *desc;      // [n] on the device
+  int *soff;            // [n + 1] sample offsets of the running batch call (device)
+  int *off;             // [n + 1] point offsets (host)
+  int *sel;             // [n + 1] per-cloud offsets of the last batch selection (host)
+  size_t point_cap, cell_cap, desc_cap;
+  int n, maxk;          // clouds installed, largest camera count
+  bool has_src;
+  double *samples;      // gpdb_set_samples positions (3 x n_samples) of the single cloud, or nullptr
+  int n_samples;
+  DevCloud view;        // the concatenated arrays as the kernels read them
+  int points() const { return n ? off[n] : 0; }
+  CloudTable table() const { return CloudTable{desc, soff, n}; }
 };
 
 // device error counters: [0] LRF capacity, [1] hand-search capacity (final tier), [2] image box list,
@@ -162,17 +180,8 @@ struct gpdb_ctx {
   CommState *comm;
   int sm_count;
   char err[512];
-  // cloud
-  DevCloud cloud;
-  float4 *d_pts4;
-  float *d_xyz;
-  double *d_nrm;
-  uint8_t *d_cam;
-  int *d_cell_start;
-  size_t cloud_cap;       // capacity (points) of pts4 / xyz / nrm / cam / src: grown, never shrunk
-  size_t cell_cap;        // capacity (ints) of cell_start
-  int N, K;
-  bool cloud_set;
+  CloudSet one;       // the single cloud (gpdb_set_cloud / gpdb_preprocess): a store of one cloud
+  CloudSet many;      // the batch of clouds (gpdb_set_clouds / gpdb_preprocess_clouds)
   double *d_qtab;
   // weights
   LenetWeights w;
@@ -187,27 +196,7 @@ struct gpdb_ctx {
   double pre_ms[6];   // gpdb_preprocess stage timings
   gpdb_pose *d_sel;   // gpdb_detect_select: all classified candidates of a call (grown on demand)
   size_t sel_cap;
-  double *d_samples;  // gpdb_set_samples positions (3 x n_samples), or nullptr
-  int n_samples;
-  int *d_src;         // raw index of each processed point (valid after gpdb_preprocess: has_src)
-  bool has_src;
   cudaEvent_t ev[8];
-  // batch of clouds (gpdb_set_clouds), held beside the single cloud; grow-only arenas as the cloud arrays
-  DevCloud bcloud;    // the concatenated arrays (xyz / nrm / cam by concatenated index, pts4 sorted by (cloud, cell))
-  float4 *d_bpts4;
-  float *d_bxyz;
-  double *d_bnrm;
-  uint8_t *d_bcam;
-  int *d_bcell_start;
-  CloudDesc *d_bdesc;
-  int *d_bsoff;       // [B+1] sample offsets of the running batch call
-  size_t bcloud_cap, bcell_cap, bdesc_cap;
-  int b_n, b_maxk;    // clouds installed (0: none), largest camera count
-  int *b_off;         // host copy of the point offsets [b_n + 1]
-  int *b_sel;         // host: per-cloud offsets of the last batch selection [b_n + 1]
-  int *d_bsrc;        // cloud-local raw index of each point (valid after gpdb_preprocess_clouds: b_has_src)
-  bool b_has_src;
-  CloudTable run;     // n > 0 while a batch call runs: the geometry launchers use the batch instantiations
 };
 
 void gpdb_set_error(gpdb_ctx *ctx, int code, const char *fmt, ...);
@@ -222,34 +211,45 @@ int gpdb_pipe_create(gpdb_ctx *ctx);
 void gpdb_pipe_destroy(gpdb_ctx *ctx);
 int gpdb_check_state(gpdb_ctx *ctx, bool need_cloud, bool need_weights);
 void *gpdb_result_extra(gpdb_result *r, size_t bytes);  // pinned host memory owned by the result (freed with it)
-// the chunked device pipeline (see api.cu); slot_base is added to every sample_slot (rank offset of a sharded call)
-int gpdb_run_pipeline(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_result *out, bool with_images_and_scores,
-                      bool resident, uint8_t *flags_ext, float *scores_ext, int select_k, int slot_base);
-// installs the cloud whose device arrays d_xyz / d_nrm / d_cam already hold N points (grid bounds by device reduction)
-int gpdb_install_device_cloud(gpdb_ctx *ctx, int N, int K, const double *view_points, int all_seen);
+// the chunked device pipeline (see api.cu) over the clouds of store s (ctx->many: a batch call whose sample offsets are
+// in s.soff); slot_base is added to every sample_slot (rank offset of a sharded call)
+int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int32_t n, gpdb_result *out,
+                      bool with_images_and_scores, bool resident, uint8_t *flags_ext, float *scores_ext, int select_k,
+                      int slot_base);
+// (re)allocates the arenas of store s for at least n points and n_clouds clouds
+int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds);
+// Installs the B clouds whose points the arrays of s already hold (cloud b: off[b] .. off[b+1]-1, host offsets): desc[b]
+// (host) carries K / vp / all_seen and receives the point range; uploads the descriptors and builds the grids. nonunit:
+// also set the descriptors' nonunit flags from the stored normals (false: the caller sets them once the normals exist).
+int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *off, int B, bool nonunit);
+// Packs the camera-source matrices of B clouds (cloud b: off[b+1] - off[b] rows of n_cameras[b] entries, concatenated,
+// or null: every camera sees every point) into cam (one bit per camera) and fills desc[b].K / vp / all_seen. A camera
+// sees a point when its entry is > 0 (eq1 false) or == 1 (eq1 true); strict01 refuses entries other than 0 and 1.
+int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
+                      const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
+                      CloudDesc *desc);
 
 // geometry.cu
-// builds the neighbour grid over ctx->d_xyz (N points) whose per-axis bounds are lo / hi
-int geo_build_grid(gpdb_ctx *ctx, const float lo[3], const float hi[3], int N);
-// builds the per-cloud grids of the installed batch (N concatenated points, ctx->b_n clouds) and its descriptor table
-int geo_build_grid_batch(gpdb_ctx *ctx, int N);
-// the top k of every cloud of the running batch among the n candidate records (sample-slot order, scores filled) ->
-// *d_out (device scratch); sel_off[b_n + 1] (host) receives the per-cloud output offsets. Returns the total or an error.
-int geo_select_batch(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, int *sel_off, gpdb_pose **d_out);
-int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid);
-int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
-              gpdb_pose *d_poses, uint8_t *d_flags);
+// builds the per-cloud grids of store s (its s.n descriptors hold off / N) and fills the descriptors' grid fields
+int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s);
+// the top k of every cloud of the running batch (store s) among the n candidate records (sample-slot order, scores
+// filled) -> *d_out (device scratch); s.sel[s.n + 1] (host) receives the per-cloud output offsets. Returns the total or
+// an error.
+int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n, int k, gpdb_pose **d_out);
+int geo_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid);
+int geo_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, int slot0, const double *d_frames,
+              const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags);
 // compacts poses with VALID|FILTERED into d_cand (in (sample,pose) order); *d_count receives the count
 int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags, int n_poses, gpdb_pose *d_cand,
                 int *d_count);
 // grasp images in the P16 layout: S*S pixels of 16 bytes (channels 0..C-1, zero padded) per image = conv1's operand
-int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16);
+int geo_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_cand, int nc, uint8_t *d_p16);
 int geo_p16_to_hwc(gpdb_ctx *ctx, const uint8_t *d_p16, int n, uint8_t *d_hwc);  // -> cv::Mat layout (C bytes per pixel)
 int geo_hwc_to_p16(gpdb_ctx *ctx, const uint8_t *d_hwc, int n, uint8_t *d_p16);
 int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_scores, int nc, int slot0, int P,
                        float *d_pose_scores, gpdb_pose *d_cand_out);
 
-// HandSearch::reevaluateHypotheses: labels + half / full flags of the given hands against the installed cloud
+// HandSearch::reevaluateHypotheses: labels + half / full flags of the given hands against the single cloud
 int geo_reeval(gpdb_ctx *ctx, gpdb_pose *d_hands, int n, int *d_labels);
 // Clustering::findClusters (remove_inliers = false): dense per-hand cluster records + keep flags (3 = cluster), for geo_compact
 int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, int min_inliers, gpdb_pose *d_dense, uint8_t *d_keep);
@@ -257,22 +257,15 @@ int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, int min_inliers
 int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *d_out);
 
 // preprocess.cu (cloud preprocessing, SURVEY.md 8(f).1)
-// (re)allocates the context's cloud arrays for at least n points (api.cu)
-int gpdb_cloud_reserve(gpdb_ctx *ctx, size_t n);
-int pre_bounds(gpdb_ctx *ctx, const float *d_xyz, int n, int *d_bounds, float lo[3], float hi[3]);
-// filters + voxelises the raw arrays into the context's cloud arrays (reserved inside); *n_out = processed points
-int pre_filter_voxelize(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_cam_raw, const double *d_nrm_raw, int M,
-                        const gpdb_preprocess_params &pp, int *n_out, cudaEvent_t ev_filter_done);
-int pre_normals(gpdb_ctx *ctx, double radius);
-int pre_nonunit(gpdb_ctx *ctx);
-int pre_cam_expand(gpdb_ctx *ctx, int *d_out);
-// (re)allocates the batch arenas for at least n points and n_clouds clouds (api.cu)
-int gpdb_batch_reserve(gpdb_ctx *ctx, size_t n, int n_clouds);
-// filters + voxelises a raw batch into the batch arenas (reserved inside); poff[B+1] (host) = processed offsets
-int pre_filter_voxelize_batch(gpdb_ctx *ctx, const float *d_xyz_raw, const uint8_t *d_cam_raw, const double *d_nrm_raw, int M,
-                              int B, const int *roff, const gpdb_preprocess_params &pp, int *poff, cudaEvent_t ev_filter_done);
-int pre_normals_batch(gpdb_ctx *ctx, double radius);  // normals of the installed batch (grids built)
-int pre_nonunit_batch(gpdb_ctx *ctx);                 // per-cloud nonunit flags of the installed batch, in the descriptors
+// per-cloud bounds of xyz (cloud b: points d_off[b] .. d_off[b+1]-1, device offsets; `largest` points in the largest
+// cloud) -> bounds[6b .. 6b+5] (min x y z, max x y z as order-preserving ints; an empty cloud keeps INT_MAX / INT_MIN)
+int pre_bounds_batch(gpdb_ctx *ctx, const float *xyz, const int *d_off, int B, int largest, int *bounds);
+// filters + voxelises a raw batch into the arenas of store s (reserved inside); poff[B+1] (host) = processed offsets
+int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw, const uint8_t *d_cam_raw,
+                              const double *d_nrm_raw, int M, int B, const int *roff, const gpdb_preprocess_params &pp,
+                              int *poff, cudaEvent_t ev_filter_done);
+int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
+int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 
 // lenet_simt.cu
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);

@@ -162,25 +162,6 @@ __device__ __forceinline__ int seg_lookup(const SegScan<NT> &seg, int c) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// grid build
-// ------------------------------------------------------------------------------------------------
-__global__ void k_cell_ids(const DevParams *Pp, const float *xyz, int N, int *cid, int *idx, int *counts) {
-  const DevParams &P = *Pp;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  int c = (cell_of(P, xyz[3 * i + 2], 2) * P.dim[1] + cell_of(P, xyz[3 * i + 1], 1)) * P.dim[0] + cell_of(P, xyz[3 * i], 0);
-  cid[i] = c;
-  idx[i] = i;
-  atomicAdd(counts + c + 1, 1);
-}
-__global__ void k_fill_sorted(const float *xyz, const int *idx_sorted, int N, float4 *pts4) {
-  int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= N) return;
-  int i = idx_sorted[k];
-  pts4[k] = make_float4(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], __int_as_float(i));
-}
-
-// ------------------------------------------------------------------------------------------------
 // 3x3 symmetric eigen-solver: Eigen::SelfAdjointEigenSolver<Matrix3d>::compute restated
 // (same sequence of operations as oracle/gpd_oracle.cpp eigen3 -> identical bits).
 // ------------------------------------------------------------------------------------------------
@@ -364,8 +345,8 @@ __device__ __forceinline__ bool lrf_sample(const DevParams &P, const DevCloud &c
                                            uint8_t *valid, int *err, double *s_acc_w) {
   const int lane = threadIdx.x & 31;
   const int si = sidx[i];
-  const auto &G = CloudSel<BATCH>::get(P, tab, i);  // geo_frames runs over the whole call: slot = i
-  const DevCloud cl = local_cloud(G, cl0);
+  const auto &G = CloudSel<BATCH>::get(tab, i);  // geo_frames runs over the whole call: slot = i
+  const DevCloud cl = CloudSel<BATCH>::local(G, cl0);
   double sp[3];
   sample_position(cl, si, sp);
   float q[3] = {(float)sp[0], (float)sp[1], (float)sp[2]};
@@ -521,8 +502,8 @@ __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevC
   for (int w = blockIdx.x; w < work_n; w += gridDim.x) {
     const int i = in_list ? in_list[w] : w;
     const int si = sidx[i];
-    const auto &G = CloudSel<BATCH>::get(P, tab, slot0 + i);
-    const DevCloud cl = local_cloud(G, cl0);
+    const auto &G = CloudSel<BATCH>::get(tab, slot0 + i);
+    const DevCloud cl = CloudSel<BATCH>::local(G, cl0);
     __syncthreads();
     if (tid == 0) {
       S.count = 0;
@@ -925,13 +906,13 @@ __global__ void k_gather_poses(const gpdb_pose *cand, const int *order, int k, g
 // k_hands. A labelling path, not a throughput path: no shared-memory staging.
 // ------------------------------------------------------------------------------------------------
 template <class F>
-__device__ __forceinline__ void warp_scan_ball(const DevParams &P, const DevCloud &cl, const SegRange &sr, const float q[3], float r2,
+__device__ __forceinline__ void warp_scan_ball(const CloudDesc &G, const DevCloud &cl, const SegRange &sr, const float q[3], float r2,
                                                F &&body) {  // body(point) for every in-ball point, lanes in lockstep
   const int lane = threadIdx.x & 31;
   for (int j0 = 0; j0 < sr.nrows; j0 += 32) {
     const int myrow = j0 + lane;
     int st = 0, len = 0;
-    if (myrow < sr.nrows) seg_row(P, cl.cell_start, sr, myrow, st, len);
+    if (myrow < sr.nrows) seg_row(G, cl.cell_start, sr, myrow, st, len);
     unsigned nonempty = __ballot_sync(0xffffffffu, len > 0);
     while (nonempty) {
       const int j = __ffs(nonempty) - 1;
@@ -948,8 +929,10 @@ __device__ __forceinline__ void warp_scan_ball(const DevParams &P, const DevClou
   }
 }
 
-__global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl, gpdb_pose *hands, int n, int *labels) {
+__global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl, CloudTable tab, gpdb_pose *hands, int n,
+                                                int *labels) {
   const DevParams &P = *Pp;
+  const CloudDesc &G = CloudSel<false>::get(tab, 0);
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= n) return;
   gpdb_pose &h = hands[i];
@@ -961,7 +944,7 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
   const int idx = h.finger_idx;
   const double top = h.top, bottom = top - P.hand_depth, hh = P.hand_height;  // evaluateFingers(points, hand.getTop(), idx)
   const float q[3] = {(float)smp[0], (float)smp[1], (float)smp[2]};            // eigenVectorToPcl (:136-142)
-  const SegRange sr = seg_range(P, q, P.rf_hs);
+  const SegRange sr = seg_range(G, q, P.rf_hs);
   int label = 0;
   bool half = false, full = false;
   if (idx >= 0 && idx < P.nfp) {
@@ -977,7 +960,7 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
         if ((y > s0 && y < s0w) || (y > s1 && y < s1w)) blocked = 1;
       }
     };
-    warp_scan_ball(P, cl, sr, q, P.r2_hs, [&](const float4 &p) {
+    warp_scan_ball(G, cl, sr, q, P.r2_hs, [&](const float4 &p) {
       nball++;
       const unsigned long long key = ((unsigned long long)__float_as_uint(l2_simple(q, p.x, p.y, p.z)) << 32) | (unsigned)__float_as_int(p.w);
       best = key < best ? key : best;
@@ -1011,7 +994,7 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
       int cnt = 0;
       double mny = DBL_MAX, mxy = -DBL_MAX;
       auto in_region = [&](double x, double y) { return x > bottom && x < top && y > left && y < right; };
-      warp_scan_ball(P, cl, sr, q, P.r2_hs, [&](const float4 &p) {
+      warp_scan_ball(G, cl, sr, q, P.r2_hs, [&](const float4 &p) {
         double x, y, z;
         to_frame(R, (double)p.x - smp[0], (double)p.y - smp[1], (double)p.z - smp[2], x, y, z);
         if (z > -1.0 * hh && z < hh && in_region(x, y)) {
@@ -1053,7 +1036,7 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
             rmaxx = fmax(rmaxx, x); rminx = fmin(rminx, x); rmaxz = fmax(rmaxz, z); rminz = fmin(rminz, z);
           }
         };
-        warp_scan_ball(P, cl, sr, q, P.r2_hs, [&](const float4 &p) {
+        warp_scan_ball(G, cl, sr, q, P.r2_hs, [&](const float4 &p) {
           double x, y, z;
           to_frame(R, (double)p.x - smp[0], (double)p.y - smp[1], (double)p.z - smp[2], x, y, z);
           if (z > -1.0 * hh && z < hh && in_region(x, y)) visitD(x, y, z, __float_as_int(p.w), 1);
@@ -1075,7 +1058,7 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
             if (ldot > P.cosf && y < min_x && inw) nl += wgt;
             if (rdot > P.cosf && y > max_x && inw) nr += wgt;
           };
-          warp_scan_ball(P, cl, sr, q, P.r2_hs, [&](const float4 &p) {
+          warp_scan_ball(G, cl, sr, q, P.r2_hs, [&](const float4 &p) {
             double x, y, z;
             to_frame(R, (double)p.x - smp[0], (double)p.y - smp[1], (double)p.z - smp[2], x, y, z);
             if (z > -1.0 * hh && z < hh && in_region(x, y)) visitE(x, y, z, __float_as_int(p.w), 1);
@@ -1429,8 +1412,8 @@ __global__ void __launch_bounds__(NT_IMG, 1) k_images(const DevParams *Pp, DevCl
     for (int k = tid; k < SS; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);  // tiles A, B: clean
     __syncthreads();
     PHASE(1);   // image start
-    const auto &G = CloudSel<BATCH>::get(P, tab, sm.h.sample_slot);
-    const DevCloud cl = local_cloud(G, cl0);
+    const auto &G = CloudSel<BATCH>::get(tab, sm.h.sample_slot);
+    const DevCloud cl = CloudSel<BATCH>::local(G, cl0);
     const bool need_cam = (C == 15) && !G.all_seen;  // the camera set of the neighbourhood is only read by the shadow
     const gpdb_pose &h = sm.h;
     const double inv_d = 1.0 / P.vol_d, inv_w = 1.0 / P.vol_w, inv_h = 1.0 / (2.0 * P.vol_h);
@@ -2337,8 +2320,8 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
     __syncthreads();
     PHASE(1);
     const gpdb_pose &h = sm.h;
-    const auto &G = CloudSel<BATCH>::get(P, tab, h.sample_slot);
-    const DevCloud cl = local_cloud(G, cl0);
+    const auto &G = CloudSel<BATCH>::get(tab, h.sample_slot);
+    const DevCloud cl = CloudSel<BATCH>::local(G, cl0);
     const bool need_cam = (C == 15) && !G.all_seen;
     const double inv_d = 1.0 / P.vol_d, inv_w = 1.0 / P.vol_w, inv_h = 1.0 / (2.0 * P.vol_h);
     float q[3] = {(float)h.sample[0], (float)h.sample[1], (float)h.sample[2]};
@@ -3002,50 +2985,19 @@ __global__ void k_hwc_to_p16(const uint8_t *__restrict__ hwc, size_t npix, int C
 // ------------------------------------------------------------------------------------------------
 // batch of clouds (gpdb_set_clouds): one grid per cloud, built for all clouds in one segmented pass
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int b_f2ord(float f) {  // order-preserving int image of a float (as pre_bounds)
-  int i = __float_as_int(f);
-  return i >= 0 ? i : i ^ 0x7fffffff;
-}
-// one CTA per cloud: bounds, then the grid geo_build_grid derives from them (same float32 steps), and whether any normal
-// is off unit length (pre_nonunit). ncell[b] = cells of cloud b. A cloud without points (gpdb_preprocess_clouds keeps a
-// view the filter emptied) gets the grid of bounds 0..0: 2 x 2 x 2 cells that no search reads, since no sample and no
-// point belongs to it (b_cloud_of_point passes over it).
-__global__ void __launch_bounds__(256) k_batch_desc(const float *xyz, const double *nrm, CloudDesc *d, long long *ncell) {
-  __shared__ int s_mn[3], s_mx[3], s_nonunit;
-  CloudDesc &D = d[blockIdx.x];
-  if (threadIdx.x < 3) {
-    s_mn[threadIdx.x] = INT_MAX;
-    s_mx[threadIdx.x] = INT_MIN;
-  }
-  if (threadIdx.x == 0) s_nonunit = 0;
-  __syncthreads();
-  int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
-  bool nonunit = false;
-  for (int i = D.off + threadIdx.x; i < D.off + D.N; i += blockDim.x) {
-    for (int a = 0; a < 3; a++) {
-      const int o = b_f2ord(xyz[3 * (size_t)i + a]);
-      mn[a] = min(mn[a], o);
-      mx[a] = max(mx[a], o);
-    }
-    if (!unit_normal(nrm + 3 * (size_t)i)) nonunit = true;
-  }
-  for (int a = 0; a < 3; a++) {
-    mn[a] = __reduce_min_sync(0xffffffffu, mn[a]);
-    mx[a] = __reduce_max_sync(0xffffffffu, mx[a]);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    for (int a = 0; a < 3; a++) {
-      atomicMin(s_mn + a, mn[a]);
-      atomicMax(s_mx + a, mx[a]);
-    }
-  }
-  if (nonunit) s_nonunit = 1;
-  __syncthreads();
-  if (threadIdx.x != 0) return;
+// per cloud: the grid over its bounds (pre_bounds_batch; float32 steps: 2 cm cells, grown x1.5 while the grid has more than
+// 48e6 cells). ncell[b] = cells of cloud b. A cloud without points (gpdb_preprocess_clouds keeps a view the filter
+// emptied) gets the grid of bounds 0..0: 2 x 2 x 2 cells that no search reads, since no sample and no point belongs to it
+// (b_cloud_of_point passes over it).
+__global__ void k_batch_desc(const int *bounds, CloudDesc *d, int B, long long *ncell) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  CloudDesc &D = d[b];
   float lo[3], hi[3];
   for (int a = 0; a < 3; a++) {
-    lo[a] = D.N > 0 ? __int_as_float(s_mn[a] >= 0 ? s_mn[a] : s_mn[a] ^ 0x7fffffff) : 0.0f;
-    hi[a] = D.N > 0 ? __int_as_float(s_mx[a] >= 0 ? s_mx[a] : s_mx[a] ^ 0x7fffffff) : 0.0f;
+    const int mn = bounds[6 * b + a], mx = bounds[6 * b + 3 + a];  // order-preserving ints
+    lo[a] = D.N > 0 ? __int_as_float(mn >= 0 ? mn : mn ^ 0x7fffffff) : 0.0f;
+    hi[a] = D.N > 0 ? __int_as_float(mx >= 0 ? mx : mx ^ 0x7fffffff) : 0.0f;
   }
   float cell = 0.02f;
   double nc;
@@ -3060,14 +3012,13 @@ __global__ void __launch_bounds__(256) k_batch_desc(const float *xyz, const doub
   }
   for (int a = 0; a < 3; a++) D.lo[a] = lo[a];
   D.inv_cell = 1.0f / cell;
-  D.nonunit = s_nonunit;
-  ncell[blockIdx.x] = (long long)nc;
+  ncell[b] = (long long)nc;
 }
 __global__ void k_batch_base(CloudDesc *d, const long long *base, int B) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b < B) d[b].cell_base = (int)base[b];
 }
-// cell id of every point in the batch-wide numbering (cloud b's cells start at its cell_base): sorting by it orders the
+// cell id of every point in the store-wide numbering (cloud b's cells start at its cell_base): sorting by it orders the
 // points by (cloud, cell), stable in point order
 __global__ void k_batch_cell_ids(const float *xyz, const CloudDesc *d, int B, int N, int *cid, int *idx, int *counts) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -3141,54 +3092,6 @@ __global__ void k_batch_sel_order(const int *sorted_vals, const int *cand_off, c
     }                                                    \
   } while (0)
 
-int geo_build_grid(gpdb_ctx *ctx, const float lo[3], const float hi[3], int N) {
-  DevParams &hp = ctx->hp;
-  float cell = 0.02f;
-  size_t ncell;
-  for (;;) {
-    double nc = 1;
-    for (int a = 0; a < 3; a++) {
-      hp.dim[a] = (int)floorf((hi[a] - lo[a]) / cell) + 2;
-      nc *= hp.dim[a];
-    }
-    if (nc <= 48e6) { ncell = (size_t)nc; break; }
-    cell *= 1.5f;
-  }
-  for (int a = 0; a < 3; a++) hp.lo[a] = lo[a];
-  hp.inv_cell = 1.0f / cell;
-  hp.N = N;
-  CUDA_TRY(cudaMemcpyAsync(ctx->dp, &hp, sizeof(DevParams), cudaMemcpyHostToDevice, ctx->stream));
-  if (ncell + 1 > ctx->cell_cap) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->d_cell_start);
-    ctx->d_cell_start = nullptr;
-    ctx->cell_cap = 0;
-    CUDA_TRY(cudaMalloc(&ctx->d_cell_start, sizeof(int) * (ncell + 1 + ncell / 4)));
-    ctx->cell_cap = ncell + 1 + ncell / 4;
-  }
-  CUDA_TRY(cudaMemsetAsync(ctx->d_cell_start, 0, sizeof(int) * (ncell + 1), ctx->stream));
-  int *cid = (int *)gpdb_scratch(ctx, 0, sizeof(int) * (size_t)N * 4);
-  if (!cid) return GPDB_ERR_CUDA;
-  int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
-  const int tb = 256, gb = (N + tb - 1) / tb;
-  k_cell_ids<<<gb, tb, 0, ctx->stream>>>(ctx->dp, ctx->d_xyz, N, cid, idx, ctx->d_cell_start);
-  LAUNCH_CHECK();
-  size_t tmp_bytes = 0, tmp2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream);
-  cub::DeviceScan::InclusiveSum(nullptr, tmp2, ctx->d_cell_start, ctx->d_cell_start, (int)(ncell + 1), ctx->stream);
-  void *tmp = gpdb_scratch(ctx, 1, std::max(tmp_bytes, tmp2));
-  if (!tmp) return GPDB_ERR_CUDA;
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream));
-  ctx->launches += 4;
-  k_fill_sorted<<<gb, tb, 0, ctx->stream>>>(ctx->d_xyz, idx2, N, ctx->d_pts4);
-  LAUNCH_CHECK();
-  CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, tmp2, ctx->d_cell_start, ctx->d_cell_start, (int)(ncell + 1), ctx->stream));
-  ctx->launches += 2;
-  ctx->cloud.cell_start = ctx->d_cell_start;
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return GPDB_OK;
-}
-
 __global__ void k_path_add(unsigned long long *prof, int e0, const int *n0, int e1, const int *n1) {
   // atomic: the hand search of the next chunk may run on its own stream beside the image kernels of this one
   atomicAdd(prof + GPDB_PROF_PATH + e0, (unsigned long long)(unsigned)*n0);
@@ -3205,7 +3108,7 @@ static int path_add(gpdb_ctx *ctx, int e0, const int *n0, int e1, const int *n1)
 }
 
 template <bool BATCH>
-static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
+static int launch_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
   const int cap0 = 128;  // ~44 points at the default nn_radius on a 3 mm cloud
   const size_t smem0 = (size_t)2 * LRF_WARPS * cap0 * sizeof(unsigned long long);
   const size_t smem1 = (size_t)2 * LRF_WARPS * LRF_CAP * sizeof(unsigned long long);
@@ -3218,7 +3121,8 @@ static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, i
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
-  const CloudTable tab = ctx->run;
+  const DevCloud &cl = s.view;
+  const CloudTable tab = s.table();
   const int grid = (n + LRF_WARPS - 1) / LRF_WARPS;
   k_frames<BATCH><<<grid, LRF_WARPS * 32, smem0, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, d_frames, d_valid, ctx->d_err, cap0,
                                                                 ovf, ovf_count, ovf2, ovf2_count, nullptr, 0);
@@ -3234,17 +3138,19 @@ static int launch_frames(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, i
   return path_add(ctx, PATH_FRAMES_T1, ovf_count, PATH_FRAMES_T2, ovf2_count);
 }
 
-int geo_frames(gpdb_ctx *ctx, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
+// The geometry launchers run the one-cloud instantiations (BATCH = false) when the store holds one cloud: they carry no
+// per-sample cloud search and spill less.
+int geo_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
   if (n <= 0) return GPDB_OK;
-  return ctx->run.n ? launch_frames<true>(ctx, ctx->bcloud, d_sidx, n, d_frames, d_valid)
-                    : launch_frames<false>(ctx, ctx->cloud, d_sidx, n, d_frames, d_valid);
+  return s.n > 1 ? launch_frames<true>(ctx, s, d_sidx, n, d_frames, d_valid)
+                 : launch_frames<false>(ctx, s, d_sidx, n, d_frames, d_valid);
 }
 
 static const int HANDS_CAP1 = 2176, HANDS_CAP2 = 12800;  // tier 1: 4 CTAs per SM (34 KB + 20 KB static each, <= 64 registers)
 static const int HANDS_CAP3 = 131072;                    // last tier: neighbourhood staged in global memory (2 MB per CTA)
 
 template <bool BATCH>
-static int launch_hands(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, int n, int slot0, const double *d_frames,
+static int launch_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, int slot0, const double *d_frames,
                         const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags) {
   // per call, not once per process: function attributes belong to the current device's context (one context per GPU)
   CUDA_TRY(cudaFuncSetAttribute(k_hands<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, HANDS_CAP2 * 16));
@@ -3254,7 +3160,8 @@ static int launch_hands(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, in
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
-  const CloudTable tab = ctx->run;
+  const DevCloud &cl = s.view;
+  const CloudTable tab = s.table();
   k_hands<BATCH><<<n, NT_HANDS, HANDS_CAP1 * 16, ctx->stream>>>(ctx->dp, cl, tab, d_sidx, n, slot0, d_frames, d_valid, d_poses,
                                                                 d_flags, HANDS_CAP1, nullptr, nullptr, ovf, ovf_count, nullptr,
                                                                 ctx->d_err, ctx->d_prof);
@@ -3273,11 +3180,11 @@ static int launch_hands(gpdb_ctx *ctx, const DevCloud &cl, const int *d_sidx, in
   return path_add(ctx, PATH_HANDS_T2, ovf_count, PATH_HANDS_T3, ovf2_count);
 }
 
-int geo_hands(gpdb_ctx *ctx, const int *d_sidx, int n, int slot0, const double *d_frames, const uint8_t *d_valid,
-              gpdb_pose *d_poses, uint8_t *d_flags) {
+int geo_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, int slot0, const double *d_frames,
+              const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags) {
   if (n <= 0) return GPDB_OK;
-  return ctx->run.n ? launch_hands<true>(ctx, ctx->bcloud, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags)
-                    : launch_hands<false>(ctx, ctx->cloud, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags);
+  return s.n > 1 ? launch_hands<true>(ctx, s, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags)
+                 : launch_hands<false>(ctx, s, d_sidx, n, slot0, d_frames, d_valid, d_poses, d_flags);
 }
 
 int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags, int n_poses, gpdb_pose *d_cand,
@@ -3310,10 +3217,11 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
 // cameras, or shadow bitmaps that leave less than 2 KB of the box list: two cameras at the default image volume) or when
 // GPD_B200_IMAGES_KERNEL=1 forces it (tests compare the kernels).
 template <bool BATCH>
-static int launch_images(gpdb_ctx *ctx, const DevCloud &cl, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
+static int launch_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
   const DevParams &hp = ctx->hp;
-  const int K = BATCH ? ctx->b_maxk : hp.K;  // a batch is sized for its largest camera count
-  const CloudTable tab = ctx->run;
+  const int K = s.maxk;  // a batch is sized for its largest camera count
+  const DevCloud &cl = s.view;
+  const CloudTable tab = s.table();
   const int S = hp.S, RS = (S + 3) & ~3;
   const size_t plane_bytes = ((size_t)hp.C * S * RS + 15) / 16 * 16;
   const size_t tiles = (size_t)3 * 8 * S * S;
@@ -3377,10 +3285,9 @@ static int launch_images(gpdb_ctx *ctx, const DevCloud &cl, const gpdb_pose *d_c
   return path_add(ctx, PATH_IMG_GL, ovf2_count, 0, nullptr);
 }
 
-int geo_images(gpdb_ctx *ctx, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
+int geo_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_cand, int nc, uint8_t *d_p16) {
   if (nc <= 0) return GPDB_OK;
-  return ctx->run.n ? launch_images<true>(ctx, ctx->bcloud, d_cand, nc, d_p16)
-                    : launch_images<false>(ctx, ctx->cloud, d_cand, nc, d_p16);
+  return s.n > 1 ? launch_images<true>(ctx, s, d_cand, nc, d_p16) : launch_images<false>(ctx, s, d_cand, nc, d_p16);
 }
 
 int geo_p16_to_hwc(gpdb_ctx *ctx, const uint8_t *d_p16, int n, uint8_t *d_hwc) {
@@ -3400,7 +3307,7 @@ int geo_hwc_to_p16(gpdb_ctx *ctx, const uint8_t *d_hwc, int n, uint8_t *d_p16) {
 
 int geo_reeval(gpdb_ctx *ctx, gpdb_pose *d_hands, int n, int *d_labels) {
   if (n <= 0) return GPDB_OK;
-  k_reeval<<<(n * 32 + 127) / 128, 128, 0, ctx->stream>>>(ctx->dp, ctx->cloud, d_hands, n, d_labels);
+  k_reeval<<<(n * 32 + 127) / 128, 128, 0, ctx->stream>>>(ctx->dp, ctx->one.view, ctx->one.table(), d_hands, n, d_labels);
   LAUNCH_CHECK();
   return GPDB_OK;
 }
@@ -3440,15 +3347,22 @@ int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_sc
   return GPDB_OK;
 }
 
-// The grids of the batch installed in ctx->d_bxyz / d_bnrm (N points, ctx->b_n clouds whose descriptors hold off / N / K /
-// all_seen / vp): bounds, dims, cell bases and non-unit flags on the device, one sort over (cloud, cell) for all clouds.
-int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
-  const int B = ctx->b_n;
-  long long *ncell = (long long *)gpdb_scratch(ctx, 5, sizeof(long long) * 2 * ((size_t)B + 1));
+// The grids of store s (s.n clouds whose descriptors hold off / N): per-cloud bounds with many CTAs per cloud, dims and
+// cell bases on the device, one sort over (cloud, cell) for all clouds.
+int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
+  const int B = s.n, N = s.points();
+  long long *ncell =
+      (long long *)gpdb_scratch(ctx, 5, sizeof(long long) * 2 * ((size_t)B + 1) + sizeof(int) * (7 * (size_t)B + 1));
   if (!ncell) return GPDB_ERR_CUDA;
   long long *base = ncell + B + 1;
+  int *d_off = (int *)(base + B + 1), *bounds = d_off + B + 1;
+  CUDA_TRY(cudaMemcpyAsync(d_off, s.off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  int largest = 0;
+  for (int b = 0; b < B; b++) largest = std::max(largest, s.off[b + 1] - s.off[b]);
+  int rc = pre_bounds_batch(ctx, s.xyz, d_off, B, largest, bounds);
+  if (rc != GPDB_OK) return rc;
   CUDA_TRY(cudaMemsetAsync(ncell + B, 0, sizeof(long long), ctx->stream));
-  k_batch_desc<<<B, 256, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bnrm, ctx->d_bdesc, ncell);
+  k_batch_desc<<<(B + 255) / 256, 256, 0, ctx->stream>>>(bounds, s.desc, B, ncell);
   LAUNCH_CHECK();
   size_t tmp_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ncell, base, B + 1, ctx->stream);
@@ -3463,18 +3377,18 @@ int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
     gpdb_set_error(ctx, GPDB_ERR_CAPACITY, "gpdb_set_clouds: the grids of the batch need %lld cells (max %d)", total, INT_MAX - 1);
     return GPDB_ERR_CAPACITY;
   }
-  k_batch_base<<<(B + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_bdesc, base, B);
+  k_batch_base<<<(B + 255) / 256, 256, 0, ctx->stream>>>(s.desc, base, B);
   LAUNCH_CHECK();
   const size_t ncells = (size_t)total;
-  if (ncells + 1 > ctx->bcell_cap) {
+  if (ncells + 1 > s.cell_cap) {
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(ctx->d_bcell_start);
-    ctx->d_bcell_start = nullptr;
-    ctx->bcell_cap = 0;
-    CUDA_TRY(cudaMalloc(&ctx->d_bcell_start, sizeof(int) * (ncells + 1 + ncells / 4)));
-    ctx->bcell_cap = ncells + 1 + ncells / 4;
+    cudaFree(s.cell_start);
+    s.cell_start = nullptr;
+    s.cell_cap = 0;
+    CUDA_TRY(cudaMalloc(&s.cell_start, sizeof(int) * (ncells + 1 + ncells / 4)));
+    s.cell_cap = ncells + 1 + ncells / 4;
   }
-  CUDA_TRY(cudaMemsetAsync(ctx->d_bcell_start, 0, sizeof(int) * (ncells + 1), ctx->stream));
+  CUDA_TRY(cudaMemsetAsync(s.cell_start, 0, sizeof(int) * (ncells + 1), ctx->stream));
   int *cid = (int *)gpdb_scratch(ctx, 0, sizeof(int) * (size_t)N * 4);
   if (!cid) return GPDB_ERR_CUDA;
   int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
@@ -3482,20 +3396,20 @@ int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
   size_t tmp2 = 0;
   tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream);
-  cub::DeviceScan::InclusiveSum(nullptr, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream);
+  cub::DeviceScan::InclusiveSum(nullptr, tmp2, s.cell_start, s.cell_start, (int)(ncells + 1), ctx->stream);
   tmp = gpdb_scratch(ctx, 1, std::max(tmp_bytes, tmp2));
   if (!tmp) return GPDB_ERR_CUDA;
   if (N > 0) {  // a preprocessed batch may hold no point at all (every view filtered out)
-    k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, ctx->d_bdesc, B, N, cid, idx, ctx->d_bcell_start);
+    k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(s.xyz, s.desc, B, N, cid, idx, s.cell_start);
     LAUNCH_CHECK();
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream));
     ctx->launches += 4;
-    k_batch_fill_sorted<<<gb, tb, 0, ctx->stream>>>(ctx->d_bxyz, idx2, ctx->d_bdesc, B, N, ctx->d_bpts4);
+    k_batch_fill_sorted<<<gb, tb, 0, ctx->stream>>>(s.xyz, idx2, s.desc, B, N, s.pts4);
     LAUNCH_CHECK();
   }
-  CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, tmp2, ctx->d_bcell_start, ctx->d_bcell_start, (int)(ncells + 1), ctx->stream));
+  CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, tmp2, s.cell_start, s.cell_start, (int)(ncells + 1), ctx->stream));
   ctx->launches += 2;
-  ctx->bcloud.cell_start = ctx->d_bcell_start;
+  s.view.cell_start = s.cell_start;
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return GPDB_OK;
 }
@@ -3504,20 +3418,21 @@ int geo_build_grid_batch(gpdb_ctx *ctx, int N) {
 // (cloud, descending score) with one stable device-wide radix sort, so ties keep candidate order and one large cloud is
 // sorted by the whole device; the first min(k, count) of every cloud are gathered to d_out in cloud order.
 // sel_off[B+1] (host) receives the output offsets; returns the total.
-int geo_select_batch(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, int *sel_off, gpdb_pose **d_out) {
-  const int B = ctx->run.n;
+int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n, int k, gpdb_pose **d_out) {
+  const int B = s.n;
+  int *sel_off = s.sel;
   *d_out = nullptr;
   unsigned long long *keys = (unsigned long long *)gpdb_scratch(
       ctx, 3, sizeof(unsigned long long) * 2 * (size_t)n + sizeof(int) * (3 * (size_t)n + 2 * ((size_t)B + 1)));
   if (!keys) return GPDB_ERR_CUDA;
   unsigned long long *keys2 = keys + n;
   int *vals = (int *)(keys2 + n), *vals2 = vals + n, *order = vals2 + n, *cand_off = order + n, *d_sel_off = cand_off + B + 1;
-  k_batch_cand_off<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, ctx->run.soff, B, cand_off);
+  k_batch_cand_off<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, s.soff, B, cand_off);
   LAUNCH_CHECK();
   std::vector<int> coff((size_t)B + 1);
   CUDA_TRY(cudaMemcpyAsync(coff.data(), cand_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
   if (n > 0) {
-    k_batch_select_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, ctx->run.soff, B, keys, vals);
+    k_batch_select_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, s.soff, B, keys, vals);
     LAUNCH_CHECK();
     int cloud_bits = 0;
     while ((1ll << cloud_bits) < B) cloud_bits++;

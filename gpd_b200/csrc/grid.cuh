@@ -7,7 +7,7 @@
 
 namespace {
 
-// G: DevParams (the single cloud) or CloudDesc (one cloud of a batch): both carry lo / inv_cell / dim
+// G: a CloudDesc
 template <class G>
 __device__ __forceinline__ int cell_of(const G &P, float v, int a) {
   int c = (int)floorf((v - P.lo[a]) * P.inv_cell);
@@ -29,15 +29,29 @@ __device__ __forceinline__ void sample_position(const DevCloud &cl, int si, doub
   }
 }
 
-// The cloud of a sample slot. Single cloud (BATCH = false): DevParams itself, so that instantiation compiles to the code
-// it always was. Batch: the descriptor of the cloud whose CSR sample range holds the slot (binary search over soff).
+// The arrays of a cloud: indices (sample indices, pts4 w bits) are local to it; pts4 positions and cell_start values
+// stay store-wide.
+__device__ __forceinline__ DevCloud local_cloud(const CloudDesc &D, DevCloud cl) {
+  cl.xyz += 3 * (size_t)D.off;
+  cl.nrm += 3 * (size_t)D.off;
+  cl.cam += D.off;
+  cl.cell_start += D.cell_base;
+  cl.n_points = D.N;
+  return cl;
+}
+
+// The cloud of a sample slot (get) and its arrays (local). A store of one cloud (BATCH = false): descriptor 0, whose offset
+// and cell_base are 0, so its arrays are the store's own and `local` is the identity; the one-cloud instantiations carry
+// no slot search and no offset arithmetic (k_hands spills more with them). Batch: the descriptor of the cloud whose CSR
+// sample range holds the slot (binary search over soff), its arrays offset to that cloud.
 template <bool BATCH>
 struct CloudSel {
-  static __device__ __forceinline__ const DevParams &get(const DevParams &P, const CloudTable &, int) { return P; }
+  static __device__ __forceinline__ const CloudDesc &get(const CloudTable &t, int) { return t.d[0]; }
+  static __device__ __forceinline__ DevCloud local(const CloudDesc &, const DevCloud &cl) { return cl; }
 };
 template <>
 struct CloudSel<true> {
-  static __device__ __forceinline__ const CloudDesc &get(const DevParams &, const CloudTable &t, int slot) {
+  static __device__ __forceinline__ const CloudDesc &get(const CloudTable &t, int slot) {
     int lo = 0, hi = t.n;  // largest b with soff[b] <= slot
     while (hi - lo > 1) {
       const int mid = (lo + hi) >> 1;
@@ -45,6 +59,7 @@ struct CloudSel<true> {
     }
     return t.d[lo];
   }
+  static __device__ __forceinline__ DevCloud local(const CloudDesc &D, const DevCloud &cl) { return local_cloud(D, cl); }
 };
 // the cloud holding concatenated point g: largest b with d[b].off <= g. A cloud without points shares its offset with the
 // next cloud, so the search passes over it to the cloud that holds g.
@@ -56,29 +71,9 @@ __device__ __forceinline__ int b_cloud_of_point(const CloudDesc *d, int B, int g
   }
   return lo;
 }
-// The cloud of a concatenated point (kernels with one thread or warp per point). Single cloud: DevParams, offset 0.
-template <bool BATCH>
-struct PointSel {
-  static __device__ __forceinline__ const DevParams &get(const DevParams &P, const CloudTable &, int) { return P; }
-};
-template <>
-struct PointSel<true> {
-  static __device__ __forceinline__ const CloudDesc &get(const DevParams &, const CloudTable &t, int g) {
-    return t.d[b_cloud_of_point(t.d, t.n, g)];
-  }
-};
-__device__ __forceinline__ int cloud_off(const DevParams &) { return 0; }
-__device__ __forceinline__ int cloud_off(const CloudDesc &D) { return D.off; }
-// The arrays of that cloud: indices (sample indices, pts4 w bits) are local to it; pts4 positions and cell_start values
-// stay batch-wide.
-__device__ __forceinline__ DevCloud local_cloud(const DevParams &, const DevCloud &cl) { return cl; }
-__device__ __forceinline__ DevCloud local_cloud(const CloudDesc &D, DevCloud cl) {
-  cl.xyz += 3 * (size_t)D.off;
-  cl.nrm += 3 * (size_t)D.off;
-  cl.cam += D.off;
-  cl.cell_start += D.cell_base;
-  cl.n_points = D.N;
-  return cl;
+// The cloud of a concatenated point (kernels with one thread or warp per point).
+__device__ __forceinline__ const CloudDesc &point_cloud(const CloudTable &t, int g) {
+  return t.d[b_cloud_of_point(t.d, t.n, g)];
 }
 
 // FLANN L2_Simple<float> (float32, accumulated x,y,z in order)

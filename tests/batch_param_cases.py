@@ -2,7 +2,7 @@
 test_batch_param_cases.py proves on the CPU that each reaches the path it names).
 
 - Grown grid cells: a cloud whose bounding box would need more than 48e6 cells of 2 cm gets cells of 3 cm, then 4.5 cm
-  (geo_build_grid, k_batch_desc). A few outlier points 8 m (one growth step) or 12 m (two steps) away on each axis do
+  (k_batch_desc). A few outlier points 8 m (one growth step) or 12 m (two steps) away on each axis do
   that to any table scene.
 - The batch-wide cell guard: two-point clouds spanning 7.2 m on each axis need just under 48e6 cells each (no growth);
   46 of them need more than INT_MAX - 1 together, so gpdb_set_clouds refuses them with GPDB_ERR_CAPACITY.

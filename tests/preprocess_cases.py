@@ -14,7 +14,7 @@ from oracle import oracle
 # cameras in front of the table (z = 0.9), looking along +z (test_gpu_geometry_params.py uses the same set)
 CAMS = [[0.0, 0.0, 0.0], [0.6, 0.0, 0.0], [-0.5, 0.1, 0.05], [0.0, 0.5, 0.0], [0.1, -0.5, 0.1], [0.45, 0.45, 0.0],
         [-0.4, -0.4, 0.0], [0.3, -0.2, -0.2]]
-GRID_CELL = 0.02      # first cell of the neighbour grid (geometry.cu geo_build_grid); grid_of grows it for large clouds
+GRID_CELL = 0.02      # first cell of the neighbour grid (geometry.cu k_batch_desc); grid_of grows it for large clouds
 TIER0_CAP = 1024      # neighbours per point held by k_normals' first tier
 TIER1_CAP = 8192      # ... by its second tier; beyond it gpdb_preprocess reports GPDB_ERR_CAPACITY
 TABLE_WS = [-0.6, 0.6, -0.5, 0.5, 0.2, 1.0]
@@ -81,8 +81,8 @@ def voxel_reference(xyz, ws, cell):
 
 
 def grid_of(xyz):
-    """(lo, dim, cell, cells, growth steps) of the neighbour grid of a cloud, in the float32 steps of geo_build_grid and
-    k_batch_desc: 2 cm cells from the cloud's minimum, grown by 1.5x while the grid would need more than 48e6 cells."""
+    """(lo, dim, cell, cells, growth steps) of the neighbour grid of a cloud, in the float32 steps of k_batch_desc:
+    2 cm cells from the cloud's minimum, grown by 1.5x while the grid would need more than 48e6 cells."""
     p = np.asarray(xyz, np.float32)
     lo, hi = p.min(0), p.max(0)
     cell, steps = np.float32(GRID_CELL), 0

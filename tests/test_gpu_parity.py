@@ -6,6 +6,8 @@ follow the oracle's operation order with FMA contraction off, so in practice bit
 <= 1 LSB on <= 0.1 % of pixels (the per-cell means are exact fixed-point sums on the GPU, a float32 running mean in
 the reference); scores within 1e-4 relative to the largest |score| (float32 accumulation order).
 """
+import ctypes
+
 import numpy as np
 import pytest
 
@@ -431,8 +433,15 @@ def test_sharded_entry_points_on_one_rank_equal_detect():
     p, ctx, oc, w = make(s, 15)
     ref = ctx.detect(sidx)
     ctx.comm_init(lib.comm_unique_id(), 0, 1)
+    # a preprocessed cloud has source indices; the broadcast cloud that replaces it has none
+    wide = lib.preprocess_params(workspace=(-1e3, 1e3, -1e3, 1e3, -1e3, 1e3), voxelize=0, estimate_normals=0)
+    assert ctx.preprocess(s["xyz"], s["cam_source"], s["view_points"], wide, normals=s["normals"])["src"].size > 0
     n = ctx.set_cloud_bcast(0, s["xyz"], s["normals"], s["cam_source"], s["view_points"])
     assert n == len(s["xyz"])
+    src = np.zeros(n, np.int32)
+    assert lib.lib().gpdb_get_cloud_source_index(ctx.h, src.ctypes.data_as(ctypes.c_void_p)) == -3  # GPDB_ERR_STATE
+    with pytest.raises(lib.GpdbError):  # refused arguments leave the installed cloud in place
+        ctx.preprocess(s["xyz"], s["cam_source"], s["view_points"], lib.preprocess_params(voxel_size=0.0))
     sh = ctx.detect_sharded(sidx)
     assert np.array_equal(sh["pose_flags"], ref["pose_flags"])
     assert np.array_equal(sh["pose_scores"].view(np.uint32), ref["pose_scores"].view(np.uint32))
