@@ -1431,13 +1431,13 @@ int gpdb_images(gpdb_ctx *ctx, const gpdb_pose *poses, int32_t n, uint8_t *image
   return n;
 }
 
-int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *scores_out, float *logits_out) {
-  int rc = check_state(ctx, false, true);
-  if (rc != GPDB_OK) return rc;
-  if (n < 0 || (n > 0 && (!images_hwc || !scores_out))) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_classify: bad arguments");
-    return GPDB_ERR_INVALID;
-  }
+namespace {
+
+// The classify loop of gpdb_classify and gpdb_debug_lenet_layers: HWC -> P16 and lenet_forward in batches of batch_size.
+// scores_out / logits_out may be null; layers (null for gpdb_classify) receives every layer's output at offset b0.
+int classify_batches(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *scores_out, float *logits_out,
+                     const LenetLayers *layers) {
+  int rc;
   const size_t isz = (size_t)ctx->hp.S * ctx->hp.S * ctx->hp.C, psz = (size_t)ctx->hp.S * ctx->hp.S * 16;
   const int batch = ctx->prm.batch_size > 0 ? ctx->prm.batch_size : 8192;
   for (int b0 = 0; b0 < n; b0 += batch) {
@@ -1449,14 +1449,43 @@ int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *sc
     float *d_logits = d_scores + bn;
     CUDA_TRY(cudaMemcpyAsync(d_img, images_hwc + isz * (size_t)b0, isz * (size_t)bn, cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = geo_hwc_to_p16(ctx, d_img, bn, d_p16)) != GPDB_OK) return rc;  // cv::Mat bytes -> 16-byte pixels
-    if ((rc = lenet_forward(ctx, d_p16, bn, d_scores, d_logits)) != GPDB_OK) return rc;
-    CUDA_TRY(cudaMemcpyAsync(scores_out + b0, d_scores, sizeof(float) * (size_t)bn, cudaMemcpyDeviceToHost, ctx->stream));
+    LenetLayers at = {};
+    if (layers)
+      at = {layers->pool1 ? layers->pool1 + (size_t)b0 * 20 * 28 * 28 : nullptr,
+            layers->pool2 ? layers->pool2 + (size_t)b0 * 7200 : nullptr, layers->ip1 ? layers->ip1 + (size_t)b0 * 500 : nullptr};
+    if ((rc = lenet_forward(ctx, d_p16, bn, d_scores, d_logits, layers ? &at : nullptr)) != GPDB_OK) return rc;
+    if (scores_out)
+      CUDA_TRY(cudaMemcpyAsync(scores_out + b0, d_scores, sizeof(float) * (size_t)bn, cudaMemcpyDeviceToHost, ctx->stream));
     if (logits_out)
       CUDA_TRY(cudaMemcpyAsync(logits_out + 2 * (size_t)b0, d_logits, sizeof(float) * 2 * (size_t)bn,
                                cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   }
   return n;
+}
+
+}  // namespace
+
+int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *scores_out, float *logits_out) {
+  int rc = check_state(ctx, false, true);
+  if (rc != GPDB_OK) return rc;
+  if (n < 0 || (n > 0 && (!images_hwc || !scores_out))) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_classify: bad arguments");
+    return GPDB_ERR_INVALID;
+  }
+  return classify_batches(ctx, images_hwc, n, scores_out, logits_out, nullptr);
+}
+
+int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *pool1_out, double *pool2_out,
+                            float *ip1_out, float *logits_out) {
+  int rc = check_state(ctx, false, true);
+  if (rc != GPDB_OK) return rc;
+  if (n < 0 || (n > 0 && !images_hwc)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_debug_lenet_layers: bad arguments");
+    return GPDB_ERR_INVALID;
+  }
+  const LenetLayers layers = {pool1_out, pool2_out, ip1_out};
+  return classify_batches(ctx, images_hwc, n, nullptr, logits_out, &layers);
 }
 
 int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_out) {

@@ -269,10 +269,21 @@ int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud 
 
 // lenet_simt.cu
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);
-int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits);
+// Host buffers that receive the layer outputs of a forward pass (gpdb_debug_lenet_layers), any of them null:
+// pool1 [n][20][28][28], pool2 [n][7200] (k = c + 50 j, the values ip1 multiplies), ip1 [n][500]
+struct LenetLayers {
+  float *pool1;
+  double *pool2;
+  float *ip1;
+};
+// layers == nullptr (every production call): the kernels alone, nothing is read back
+int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits,
+                  const LenetLayers *layers = nullptr);
 
 // lenet_tc.cu (wgmma conv1 / conv2 / ip1)
 int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]);
 struct __half;
 int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, __half *xc, float *h3);
 size_t lenet_tc_xc_bytes(int n);
+// pool1 and pool2 of the last lenet_tc_forward (device p1 / xc, stream synchronised) in the LenetLayers layout
+int lenet_tc_read_layers(gpdb_ctx *ctx, int n, const float *p1, const __half *xc, const LenetLayers &out);

@@ -12,6 +12,8 @@
 // scaling (imageToArray, eigen_classifier.cpp:130-149).
 #include <cuda_fp16.h>
 
+#include <vector>
+
 #include "common.cuh"
 
 namespace {
@@ -279,7 +281,28 @@ int lenet_upload(gpdb_ctx *ctx, const float *const w[8]) {
   return rc;
 }
 
-int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits) {
+// Copies the layer outputs of the forward pass that just ran (p2: the tensor-core xc operand or SIMT float32 [n][7200]).
+static int read_layers(gpdb_ctx *ctx, int n, bool use_tc, const float *p1, const void *p2, const float *h3,
+                       const LenetLayers &out) {
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (use_tc) {
+    int rc = lenet_tc_read_layers(ctx, n, p1, reinterpret_cast<const __half *>(p2), out);
+    if (rc != GPDB_OK) return rc;
+  } else {
+    const size_t np1 = (size_t)n * NF1 * 28 * 28, np2 = (size_t)n * 7200;
+    if (out.pool1) CUDA_TRY(cudaMemcpy(out.pool1, p1, sizeof(float) * np1, cudaMemcpyDeviceToHost));
+    if (out.pool2) {
+      std::vector<float> t(np2);
+      CUDA_TRY(cudaMemcpy(t.data(), p2, sizeof(float) * np2, cudaMemcpyDeviceToHost));
+      for (size_t i = 0; i < np2; i++) out.pool2[i] = t[i];
+    }
+  }
+  if (out.ip1) CUDA_TRY(cudaMemcpy(out.ip1, h3, sizeof(float) * (size_t)n * NH, cudaMemcpyDeviceToHost));
+  return GPDB_OK;
+}
+
+int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits,
+                  const LenetLayers *layers) {
   if (n <= 0) return GPDB_OK;
   const int S = ctx->prm.image_size, C = ctx->prm.image_num_channels;
   const int P1 = (S - 4) / 2, P2 = (P1 - 4) / 2, K = NF2 * P2 * P2;
@@ -305,7 +328,7 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
     k_ip2<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(h3, n, w.i2w, w.i2b, d_scores, d_logits);
     LAUNCH_CHECK();
     gpdb_st_end(ctx, 7, e4);
-    return GPDB_OK;
+    return layers ? read_layers(ctx, n, true, p1, p2, h3, *layers) : GPDB_OK;
   } else {
   cudaEvent_t e1 = gpdb_st_begin(ctx);
   k_conv1_pool<<<std::min(n, ctx->sm_count * 2), 224, sm1, ctx->stream>>>(d_images, n, S, C, w.c1w, w.c1b, relu, p1);
@@ -323,5 +346,5 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
   k_ip2<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(h3, n, w.i2w, w.i2b, d_scores, d_logits);
   LAUNCH_CHECK();
   gpdb_st_end(ctx, 7, e3);
-  return GPDB_OK;
+  return layers ? read_layers(ctx, n, false, p1, p2, h3, *layers) : GPDB_OK;
 }

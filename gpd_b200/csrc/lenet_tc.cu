@@ -57,6 +57,7 @@ constexpr int C1_NT = 256, C1_CTAS_PER_SM = 2;
 constexpr int C1_IMG_BYTES = C1_W * C1_W * 16;  // one P16 image
 constexpr int C1_B_BYTES = 2 * C1_NMMA * C1_BCHUNK;
 constexpr int C1_STAGE_FLOATS = 28 * NF1;       // x-pooled upper output row of a tile
+constexpr double C1_W_MAX = 127.0 * 65536 + 127.0 * 257;  // largest |W| of three balanced int8 digits (top digit <= 127)
 
 // chunk c -> byte offset of row 0 inside the plane (monotonic in c)
 __host__ __device__ constexpr uint32_t c1_off(int c) {
@@ -432,7 +433,9 @@ __global__ void __launch_bounds__(IP_NT, 1) k_ip1_tc(const __half *__restrict__ 
 
 static float pow2_scale(float maxabs, float target) {
   if (!(maxabs > 0.0f)) return 1.0f;
-  return std::exp2(std::floor(std::log2(target / maxabs)));
+  const float q = target / maxabs;
+  if (std::isinf(q)) return std::ldexp(1.0f, 127);  // maxabs below ~5e-38: the largest float32 power of two, not inf
+  return std::exp2(std::floor(std::log2(q)));
 }
 
 // Build the tensor-core weight blobs from the reference's .bin layout (conv OIHW row-major).
@@ -448,9 +451,13 @@ int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]) {
     for (int o = 0; o < NF1; o++) {
       float mxo = 0.0f;
       for (size_t i = 0; i < (size_t)C * 25; i++) mxo = std::fmax(mxo, std::fabs(w[0][(size_t)o * C * 25 + i]));
-      const double so = mxo > 0.0f ? (double)mxo / 8300000.0 : 1.0;
-      scales[o] = (float)so;
-      t.c1_aff.scale[o] = (float)so;
+      // Below max|w_o| ~ 1e-36 the scale is a float32 subnormal (or 0) with a few bits: rounded down, it would put
+      // |W| past the largest value the digits hold, 127 * 65536 + 127 * 257 (the top digit clamped, that weight wrong by
+      // up to ~7 %). Step it up to the next float until max|w_o| / s_o fits; a normal scale never moves.
+      float so = mxo > 0.0f ? (float)((double)mxo / 8300000.0) : 1.0f;
+      while ((double)mxo / (double)so > C1_W_MAX) so = std::nextafter(so, INFINITY);
+      scales[o] = so;
+      t.c1_aff.scale[o] = so;
       t.c1_aff.bias[o] = w[1][o];
       for (int ch = 0; ch < C && ch < 16; ch++)
         for (int kh = 0; kh < 5; kh++)
@@ -588,3 +595,27 @@ int lenet_tc_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *p1, _
 }
 
 size_t lenet_tc_xc_bytes(int n) { return (size_t)((n + 127) / 128) * 2 * IP_KCH * 128 * 16; }
+
+// p1 [n][784 px][20] -> [n][20][784]; xc [im/128][hi|lo][k/8][im%128][8] fp16 (scaled by x3_scale) -> (hi + lo) / x3_scale
+// [n][7200] in float64: exactly the operand ip1 multiplies
+int lenet_tc_read_layers(gpdb_ctx *ctx, int n, const float *p1, const __half *xc, const LenetLayers &out) {
+  if (out.pool1) {
+    std::vector<float> t((size_t)n * 784 * NF1);
+    CUDA_TRY(cudaMemcpy(t.data(), p1, sizeof(float) * t.size(), cudaMemcpyDeviceToHost));
+    for (size_t im = 0; im < (size_t)n; im++)
+      for (int px = 0; px < 784; px++)
+        for (int c = 0; c < NF1; c++) out.pool1[(im * NF1 + c) * 784 + px] = t[(im * 784 + px) * NF1 + c];
+  }
+  if (out.pool2) {
+    std::vector<__half> t(lenet_tc_xc_bytes(n) / sizeof(__half));
+    CUDA_TRY(cudaMemcpy(t.data(), xc, lenet_tc_xc_bytes(n), cudaMemcpyDeviceToHost));
+    const double inv = 1.0 / (double)ctx->tc.x3_scale;  // a power of two: exact
+    for (size_t im = 0; im < (size_t)n; im++)
+      for (int k = 0; k < IP_K; k++) {
+        const size_t hi = (((im >> 7) * 2 * IP_KCH + (size_t)(k >> 3)) * 128 + (im & 127)) * 8 + (k & 7);
+        const size_t lo = hi + (size_t)IP_KCH * 128 * 8;
+        out.pool2[im * IP_K + k] = ((double)__half2float(t[hi]) + (double)__half2float(t[lo])) * inv;
+      }
+  }
+  return GPDB_OK;
+}

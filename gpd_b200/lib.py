@@ -25,7 +25,7 @@ EXPORTS = [
     "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
     "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
-    "gpdb_debug_path_counts",
+    "gpdb_debug_path_counts", "gpdb_debug_lenet_layers",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -73,6 +73,7 @@ def lib():
     L.gpdb_set_stream.argtypes = [vp, vp]
     L.gpdb_debug_phase_cycles.argtypes = [vp, C.c_int, vp]
     L.gpdb_debug_path_counts.argtypes = [vp, vp]
+    L.gpdb_debug_lenet_layers.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp]
     L.gpdb_preprocess_params_default.argtypes = [C.POINTER(abi.PreprocessParams)]
     L.gpdb_preprocess.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, C.POINTER(abi.PreprocessParams)]
     L.gpdb_get_cloud.argtypes = [vp, vp, vp, vp]
@@ -509,6 +510,18 @@ class Context:
         logits = np.zeros((n, 2), np.float32)
         self._check(lib().gpdb_classify(self.h, _p(images), n, _p(scores), _p(logits)))
         return scores, logits
+
+    def lenet_layers(self, images):
+        """gpdb_debug_lenet_layers: classify() that also returns every layer the selected implementation computed, as a
+        dict: pool1 [n, 20, 28, 28] float32, pool2 [n, 7200] float64 (k = c + 50 j, the values ip1 multiplies), ip1
+        [n, 500] float32, logits [n, 2] float32."""
+        images = np.ascontiguousarray(images, dtype=np.uint8)
+        n = images.shape[0]
+        out = {"pool1": np.zeros((n, 20, 28, 28), np.float32), "pool2": np.zeros((n, 7200), np.float64),
+               "ip1": np.zeros((n, 500), np.float32), "logits": np.zeros((n, 2), np.float32)}
+        self._check(lib().gpdb_debug_lenet_layers(self.h, _p(images), n, _p(out["pool1"]), _p(out["pool2"]), _p(out["ip1"]),
+                                                  _p(out["logits"])))
+        return out
 
     def phase_cycles(self, enable=1):
         out = np.zeros(16, np.uint64)

@@ -171,7 +171,13 @@ int gpdb_read_weights_file(const char *model_file, const char *weights_file, int
                            int32_t *relu_layers_out, char *err_out, int32_t err_len);
 
 /* Same, from memory, in the layout of the .bin files (A14): conv = OIHW row-major,
- * ip = column-major (out, in). Sizes: conv1 20*C*25, conv2 50*20*25, ip1 500*7200, ip2 2*500. */
+ * ip = column-major (out, in). Sizes: conv1 20*C*25, conv2 50*20*25, ip1 500*7200, ip2 2*500.
+ * Any finite float32 weights are accepted. The tensor-core conv1 holds each filter as 24-bit integers times a float32
+ * scale s_o ~ max|w_o| / 8.3e6; for max|w_o| below ~1e-36 that scale is subnormal, so s_o is rounded up until
+ * max|w_o| / s_o <= 127 * 65536 + 127 * 257 (no digit overflows) and such a filter keeps fewer than 24 bits, down to its
+ * weights' own subnormal resolution (s_o >= 2^-149). The power-of-two fp16 scale of the conv2 / ip1 weights is
+ * held to 2^127 when their max|w| is below ~5e-38. The per-layer error bounds of both implementations are in
+ * tests/lenet_layer_bounds.py. */
 int gpdb_set_weights(gpdb_ctx *ctx, const float *conv1_w, const float *conv1_b,
                      const float *conv2_w, const float *conv2_b, const float *ip1_w,
                      const float *ip1_b, const float *ip2_w, const float *ip2_b);
@@ -430,6 +436,16 @@ int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]);
  *       list overflowed  [14] ... shadow casts that walked the grid because the in-ball record (tile C) was full
  *  [15] unused, zero. */
 int gpdb_debug_path_counts(gpdb_ctx *ctx, uint64_t counts_out[16]);
+/* Development aid: gpdb_classify (same batching, same kernels of the implementation lenet_impl selects) that also returns
+ * what each LeNet layer computed, in one layout for both implementations. images_hwc as gpdb_classify; outputs:
+ *  pool1_out [n][20][28][28]  conv1 + bias (+ReLU) + 2x2 max-pool, NCHW
+ *  pool2_out [n][7200]        k = c + 50 j: exactly the values ip1 multiplies (the tensor cores' fp16 hi + lo operand,
+ *                             unscaled, hence float64)
+ *  ip1_out   [n][500]         ip1 + bias + ReLU
+ *  logits_out [n][2]
+ * Any output may be NULL. Returns n. */
+int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *pool1_out, double *pool2_out,
+                            float *ip1_out, float *logits_out);
 
 /* Version / build info string (arch, lenet implementation). */
 const char *gpdb_build_info(void);

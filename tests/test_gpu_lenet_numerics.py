@@ -110,16 +110,23 @@ def test_weight_scale_sweep_against_float64(ch):
                 assert np.array_equal(lg, np.ldexp(base[0], k).astype(np.float32)), k
 
 
+def activations_at_the_bound():
+    """The shipped 15-channel net with all-positive conv1 / conv2 weights and biases, and images of which 7 are all-255:
+    (weights, images). test_gpu_lenet_layers.py checks the same case layer by layer."""
+    w, _ = load_weights(15)
+    w = [np.abs(a) if i < 4 else np.array(a) for i, a in enumerate(w)]
+    imgs = _images(15, n=64, seed=3)
+    imgs[2:8] = 255
+    return w, imgs
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("relu", [0, 1])
 def test_activations_at_the_bound(impl, relu):
     """All-positive conv1 / conv2 weights and biases with an all-255 image drive pool1 to exactly the bound the fp16
     activation scales are derived from (and pool2 close to its bound): the logits stay finite and match float64."""
-    w, _ = load_weights(15)
-    w = [np.abs(a) if i < 4 else np.array(a) for i, a in enumerate(w)]
-    imgs = _images(15, n=64, seed=3)
-    imgs[2:8] = 255
+    w, imgs = activations_at_the_bound()
     lo = lenet_reference(w, imgs, relu)
     lg = _classify(w, imgs, 15, relu, impl)
     assert _rel_err(lg, lo) <= REL_BOUND[impl]
