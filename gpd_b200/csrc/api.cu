@@ -293,6 +293,7 @@ int gpdb_create(const gpdb_params *params, gpdb_ctx **ctx_out) {
   ctx->prm = *params;
   ctx->device = params->device;
   ctx->sm_count = prop.multiProcessorCount;
+  ctx->smem_optin = (int)prop.sharedMemPerBlockOptin;
   int rc = fill_dev_params(ctx);
   if (rc != GPDB_OK) {
     strncpy(g_create_err, ctx->err, sizeof(g_create_err) - 1);

@@ -179,6 +179,7 @@ struct gpdb_ctx {
   PipeState *pipe;
   CommState *comm;
   int sm_count;
+  int smem_optin;  // largest shared memory (dynamic + static) one block may opt in to, in bytes
   char err[512];
   CloudSet one;       // the single cloud (gpdb_set_cloud / gpdb_preprocess): a store of one cloud
   CloudSet many;      // the batch of clouds (gpdb_set_clouds / gpdb_preprocess_clouds)

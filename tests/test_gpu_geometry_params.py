@@ -94,6 +94,31 @@ def test_four_cameras_15ch_is_a_clean_error():
     ctx.close()
 
 
+@pytest.mark.parametrize("width,bm_dim", [(0.116, 52), (0.12, 53)])
+def test_general_tier_shared_memory_bound(width, bm_dim):
+    """Three 15-channel shadow bitmaps at the edge of k_images' shared memory: dynamic + static may not pass the device's
+    opt-in maximum per block (232 448 B on H100, of which the static part takes 9 520 B). bm_dim 52 needs 221 680 B of
+    dynamic memory and runs; bm_dim 53 needs 224 208 B and is refused with GPDB_ERR_INVALID, after which the same
+    context still makes images."""
+    s = scene(3)
+    sidx = scenes.sample_indices(5, 60000, 100)
+    p, ctx, oc, _ = make(s, 15, volume_width=width)
+    cand = ctx.hand_search(sidx)["candidates"]
+    assert len(cand) > 20
+    if bm_dim == 53:
+        with pytest.raises(lib.GpdbError) as e:
+            ctx.images(cand)
+        assert e.value.code == -1 and "shared memory" in str(e.value), str(e.value)
+        s = scene(2)
+        ctx.set_cloud(s["xyz"], s["normals"], s["cam_source"], s["view_points"])
+        oc = oracle.OracleCloud(s["xyz"], s["normals"], s["cam_source"], s["view_points"])
+        cand = ctx.hand_search(sidx)["candidates"]
+    io, ig = oc.images(p, cand), ctx.images(cand)
+    d = np.abs(io.astype(np.int32).reshape(ig.shape) - ig.astype(np.int32))
+    assert io.max() > 0 and d.max() <= 1 and np.count_nonzero(d) <= 1e-3 * d.size
+    ctx.close()
+
+
 @pytest.mark.parametrize("k,fast", [(2, True), (3, False)])
 def test_multi_camera_and_unseen_points_15ch(k, fast, monkeypatch):
     """cam_source rows with several cameras (every camera that sees the point) and with none: the shadow's camera set."""
