@@ -104,6 +104,49 @@ static double linspaced(int size, double low, double high, int i) {
   return (i == size1) ? high : (low + (double)i * step);
 }
 
+// doubles <-> integers in the same order (-0 and +0 share key 0), so that bisection can walk adjacent doubles
+static long long ordered_key(double x) {
+  long long b;
+  memcpy(&b, &x, sizeof(b));
+  return b < 0 ? -(b & 0x7fffffffffffffffLL) : b;
+}
+static double from_ordered_key(long long k) {
+  long long b = k < 0 ? (-k) | (long long)0x8000000000000000ULL : k;
+  double x;
+  memcpy(&x, &b, sizeof(x));
+  return x;
+}
+
+// filterGraspsDirection (grasp_detector.cpp:437-438) erases a grasp when std::acos(dot) > thresh_rad. CUDA's acos is not
+// correctly rounded (2 ulp), so the kernel must not evaluate it: acos is non-increasing on [-1, 1], and the predicate
+// becomes dot < d*, with d* the smallest double in [-1, 1] that the host's acos keeps (2 when it keeps none, -1 when it
+// keeps all, as for a NaN or >= pi threshold). |dot| > 1 and NaN give acos = NaN, which the reference keeps.
+static int direction_keep_edge(gpdb_ctx *ctx, double thresh, double *d_star) {
+  auto rejects = [thresh](long long k) { return std::acos(from_ordered_key(k)) > thresh; };
+  long long lo = ordered_key(-1.0), hi = ordered_key(1.0);
+  if (!rejects(lo)) {
+    *d_star = -1.0;
+    return GPDB_OK;
+  }
+  if (rejects(hi)) {
+    *d_star = 2.0;
+    return GPDB_OK;
+  }
+  while (hi - lo > 1) {  // rejects(lo), !rejects(hi)
+    long long mid = lo + (hi - lo) / 2;
+    (rejects(mid) ? lo : hi) = mid;
+  }
+  // the bisection is right only if the host acos is non-increasing over all of [-1, 1], which libm's acos is; this
+  // check is local: it confirms one switch across the 256 doubles either side of it and catches a libm that is not
+  for (long long k = 1; k <= 256; k++)
+    if ((hi - k >= ordered_key(-1.0) && !rejects(hi - k)) || (hi + k <= ordered_key(1.0) && rejects(hi + k))) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "the host acos is not monotone near thresh_rad = %.17g", thresh);
+      return GPDB_ERR_INVALID;
+    }
+  *d_star = from_ordered_key(hi);
+  return GPDB_OK;
+}
+
 static int fill_dev_params(gpdb_ctx *ctx) {
   const gpdb_params &p = ctx->prm;
   DevParams &d = ctx->hp;
@@ -166,6 +209,7 @@ static int fill_dev_params(gpdb_ctx *ctx) {
   d.filt_dir = p.filter_approach_direction;
   for (int i = 0; i < 3; i++) d.dir[i] = p.direction[i];
   d.thresh = p.thresh_rad;
+  if (direction_keep_edge(ctx, p.thresh_rad, &d.dir_keep) != GPDB_OK) return GPDB_ERR_INVALID;
   const double uy[3] = {0, 1, 0};
   angle_axis_matrix(M_PI, uy, d.rotb);
   static const double AXES[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};

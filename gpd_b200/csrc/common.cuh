@@ -42,6 +42,7 @@ struct DevParams {
   double min_ap, max_ap, ws[6];
   int filt_dir;
   double dir[3], thresh;
+  double dir_keep;             // smallest dot in [-1, 1] the direction filter keeps (host acos(dot) <= thresh); 2: none
   // rotations (hand_set.cpp:52-53,68-69): rotb = AngleAxis(pi, UnitY); rot[a*n_orient+i]
   double rotb[9];
   double rot[GPDB_MAX_HAND_AXES * GPDB_MAX_ORIENT][9];

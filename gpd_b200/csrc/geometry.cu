@@ -845,9 +845,9 @@ __global__ void __launch_bounds__(NT_HANDS, 4) k_hands(const DevParams *Pp, DevC
             double mx = fmax(fmax(fmax(lb, rb), fmax(lt, rt)), ap);
             ok = ok && mn >= P.ws[2 * r] && mx <= P.ws[2 * r + 1];
           }
-          if (ok && P.filt_dir) {  // filterGraspsDirection (:422-456)
+          if (ok && P.filt_dir) {  // filterGraspsDirection (:422-456): acos(dot) > thresh as the host evaluates it
             double dot = (P.dir[0] * R[0] + P.dir[1] * R[1]) + P.dir[2] * R[2];
-            if (acos(dot) > P.thresh) ok = false;
+            if (dot >= -1.0 && dot <= 1.0 && dot < P.dir_keep) ok = false;
           }
           if (ok) fl |= GPDB_POSE_FILTERED;
         }
