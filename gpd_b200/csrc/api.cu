@@ -266,6 +266,7 @@ static void cloud_free(CloudSet &s) {
   for (void *p : dev) cudaFree(p);
   free(s.off);
   free(s.sel);
+  free(s.pos);
 }
 
 extern "C" {
@@ -463,13 +464,15 @@ int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds) {
     cudaFree(s.soff); s.soff = nullptr;
     free(s.off); s.off = nullptr;
     free(s.sel); s.sel = nullptr;
+    free(s.pos); s.pos = nullptr;
     s.desc_cap = 0;
     const size_t cap = (size_t)n_clouds + 1 + n_clouds / 4;
     CUDA_TRY(cudaMalloc(&s.desc, sizeof(CloudDesc) * cap));
     CUDA_TRY(cudaMalloc(&s.soff, sizeof(int) * cap));
     s.off = (int *)malloc(sizeof(int) * cap);
     s.sel = (int *)malloc(sizeof(int) * cap);
-    if (!s.off || !s.sel) {
+    s.pos = (int *)malloc(sizeof(int) * cap);
+    if (!s.off || !s.sel || !s.pos) {
       gpdb_set_error(ctx, GPDB_ERR_CUDA, "cloud store: host allocation failed");
       return GPDB_ERR_CUDA;
     }
@@ -676,6 +679,24 @@ static int get_clouds(gpdb_ctx *ctx, CloudSet &s, float *xyz_out, double *normal
   return (int)N;
 }
 
+// replaces the sample positions of store s by n positions (3 x n, column-major; n == 0: none)
+static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int n) {
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  cudaFree(s.samples);
+  s.samples = nullptr;
+  s.n_samples = 0;
+  s.view.samples = nullptr;
+  if (n > 0) {
+    CUDA_TRY(cudaMalloc(&s.samples, sizeof(double) * 3 * (size_t)n));
+    CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    s.view.samples = s.samples;
+    s.n_samples = n;
+  }
+  return GPDB_OK;
+}
+
 extern "C" {
 
 int gpdb_set_cloud(gpdb_ctx *ctx, const float *xyz, const double *normals, const int32_t *cam_source, int32_t N,
@@ -742,20 +763,41 @@ int gpdb_set_samples(gpdb_ctx *ctx, const double *samples, int32_t n) {
     gpdb_set_error(ctx, GPDB_ERR_STATE, "no point cloud: call gpdb_set_cloud / gpdb_preprocess first");
     return GPDB_ERR_STATE;
   }
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  cudaFree(s.samples);
-  s.samples = nullptr;
-  s.n_samples = 0;
-  s.view.samples = nullptr;
-  if (n > 0) {
-    CUDA_TRY(cudaMalloc(&s.samples, sizeof(double) * 3 * (size_t)n));
-    CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    s.view.samples = s.samples;
-    s.n_samples = n;
+  const int rc = upload_samples(ctx, s, samples, n);
+  return rc < 0 ? rc : s.points();  // the first sample index that addresses samples[0]
+}
+
+int gpdb_set_clouds_samples(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *samples) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = ctx->many;
+  s.n_samples = 0;  // past this point, a failed call leaves no positions behind
+  if (!s.n) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_set_clouds_samples: no batch of clouds: call gpdb_set_clouds / "
+                   "gpdb_preprocess_clouds first");
+    return GPDB_ERR_STATE;
   }
-  return s.points();  // the first sample index that addresses samples[0]
+  const int B = s.n;
+  if (!pos_offsets || pos_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: need pos_offsets[%d] starting at 0", B + 1);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++)
+    if (pos_offsets[b + 1] < pos_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: pos_offsets decrease at cloud %d", b);
+      return GPDB_ERR_INVALID;
+    }
+  const int M = pos_offsets[B];
+  if (M > 0 && !samples) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: null samples_xyz for %d positions", M);
+    return GPDB_ERR_INVALID;
+  }
+  memcpy(s.pos, pos_offsets, sizeof(int) * ((size_t)B + 1));
+  // each descriptor's first position: one strided copy into the pos field of the B device descriptors
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaMemcpy2DAsync(&s.desc[0].pos, sizeof(CloudDesc), s.pos, sizeof(int), sizeof(int), (size_t)B,
+                             cudaMemcpyHostToDevice, ctx->stream));
+  const int rc = upload_samples(ctx, s, samples, M);
+  return rc < 0 ? rc : M;
 }
 
 int gpdb_get_cloud(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out) {
@@ -1246,6 +1288,7 @@ int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offset
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is untouched either way
+  ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
   if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !normals || !view_points || point_offsets[0] != 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, "
                    "normals, view_points");
@@ -1273,6 +1316,7 @@ int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
   ctx->many.has_src = false;
+  ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
   if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || !pp || !processed_offsets_out ||
       point_offsets[0] != 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, "
@@ -1320,12 +1364,13 @@ int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t 
 
 namespace {
 
-// gpdb_detect_batch / gpdb_detect_batch_select: checks the CSR sample lists against the installed batch and runs them as
-// ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back with cloud-local
-// sample slots, grouped by cloud (offsets_out).
+// gpdb_detect_batch / gpdb_detect_batch_select / gpdb_hand_search_batch: checks the CSR sample lists against the installed
+// batch and runs them as ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back
+// with cloud-local sample slots, grouped by cloud (offsets_out). Only the classifying calls (with_images_and_scores) need
+// weights.
 int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out, int32_t *offsets_out,
-              int select_k, const char *name) {
-  int rc = gpdb_check_state(ctx, false, true);
+              bool with_images_and_scores, int select_k, const char *name) {
+  int rc = gpdb_check_state(ctx, false, with_images_and_scores);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
   if (s.n == 0) {
@@ -1348,16 +1393,16 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
     return GPDB_ERR_INVALID;
   }
   for (int b = 0; b < B; b++) {
-    const int nb = s.off[b + 1] - s.off[b];
+    const int nb = s.off[b + 1] - s.off[b], mb = s.positions(b);  // N_b points, then M_b positions
     for (int i = sample_offsets[b]; i < sample_offsets[b + 1]; i++)
-      if (sample_idx[i] < 0 || sample_idx[i] >= nb) {
-        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d)", name, sample_idx[i],
-                       i, b, nb);
+      if (sample_idx[i] < 0 || sample_idx[i] >= nb + mb) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
+                       "positions)", name, sample_idx[i], i, b, nb, mb);
         return GPDB_ERR_INVALID;
       }
   }
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  rc = gpdb_run_pipeline(ctx, s, sample_idx, n, out, true, false, nullptr, nullptr, select_k, 0);
+  rc = gpdb_run_pipeline(ctx, s, sample_idx, n, out, with_images_and_scores, false, nullptr, nullptr, select_k, 0);
   if (rc < 0) return rc;
   // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
   if (select_k >= 0) {
@@ -1388,7 +1433,16 @@ int gpdb_detect_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch: null cand_offsets_out");
     return GPDB_ERR_INVALID;
   }
-  return run_batch(ctx, sample_offsets, sample_idx, out, cand_offsets_out, -1, "gpdb_detect_batch");
+  return run_batch(ctx, sample_offsets, sample_idx, out, cand_offsets_out, true, -1, "gpdb_detect_batch");
+}
+
+int gpdb_hand_search_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out,
+                           int32_t *cand_offsets_out) {
+  if (ctx && !cand_offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_hand_search_batch: null cand_offsets_out");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, sample_idx, out, cand_offsets_out, false, -1, "gpdb_hand_search_batch");
 }
 
 int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, int32_t num_selected,
@@ -1397,7 +1451,7 @@ int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch_select: need sel_offsets_out and num_selected >= 0");
     return GPDB_ERR_INVALID;
   }
-  return run_batch(ctx, sample_offsets, sample_idx, out, sel_offsets_out, num_selected, "gpdb_detect_batch_select");
+  return run_batch(ctx, sample_offsets, sample_idx, out, sel_offsets_out, true, num_selected, "gpdb_detect_batch_select");
 }
 
 int gpdb_set_overlap(gpdb_ctx *ctx, int32_t enable) {
@@ -1552,31 +1606,72 @@ int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_
   return n;
 }
 
+}  // extern "C"
+
+// gpdb_find_clusters_batch after the argument checks (gpdb_find_clusters: one group): the clusters of all G groups in one
+// k_clusters launch, compacted in hand order, so group g's are clusters_out[cluster_offsets_out[g] ..
+// cluster_offsets_out[g+1]); returns their total
+static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
+                         gpdb_pose *clusters_out, int32_t *cluster_offsets_out) {
+  const int n = hand_offsets[G];
+  for (int g = 0; g <= G; g++) cluster_offsets_out[g] = 0;
+  if (n == 0) return 0;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  gpdb_pose *d_in = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n * 3);
+  int *d_goff = (int *)gpdb_scratch(ctx, 18, sizeof(int) * (2 * (size_t)G + 1) + (size_t)n);
+  int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
+  if (!d_in || !d_goff || !d_count) return GPDB_ERR_CUDA;
+  gpdb_pose *d_dense = d_in + n, *d_out = d_dense + n;
+  int *d_gcount = d_goff + G + 1;
+  uint8_t *d_keep = (uint8_t *)(d_gcount + G);
+  CUDA_TRY(cudaMemcpyAsync(d_in, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_goff, hand_offsets, sizeof(int) * ((size_t)G + 1), cudaMemcpyHostToDevice, ctx->stream));
+  int rc;
+  if ((rc = geo_clusters(ctx, d_in, n, d_goff, G, min_inliers, d_dense, d_keep, d_gcount)) != GPDB_OK) return rc;
+  if ((rc = geo_compact(ctx, d_dense, d_keep, n, d_out, d_count + 2)) != GPDB_OK) return rc;  // order of i kept
+  // per-group counts -> exclusive scan: the groups' slices of the compacted list
+  CUDA_TRY(cudaMemcpyAsync(cluster_offsets_out + 1, d_gcount, sizeof(int) * (size_t)G, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  for (int g = 0; g < G; g++) cluster_offsets_out[g + 1] += cluster_offsets_out[g];
+  const int nc = cluster_offsets_out[G];
+  if (nc > 0) {
+    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  return nc;
+}
+
+extern "C" {
+
 int gpdb_find_clusters(gpdb_ctx *ctx, const gpdb_pose *hands, int32_t n, int32_t min_inliers, gpdb_pose *clusters_out) {
   if (!ctx) return GPDB_ERR_INVALID;
   if (n < 0 || (n > 0 && (!hands || !clusters_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  if (n == 0) return 0;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  gpdb_pose *d_in = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n * 3);
-  uint8_t *d_keep = (uint8_t *)gpdb_scratch(ctx, 18, (size_t)n);
-  int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
-  if (!d_in || !d_keep || !d_count) return GPDB_ERR_CUDA;
-  gpdb_pose *d_dense = d_in + n, *d_out = d_dense + n;
-  CUDA_TRY(cudaMemcpyAsync(d_in, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  int rc;
-  if ((rc = geo_clusters(ctx, d_in, n, min_inliers, d_dense, d_keep)) != GPDB_OK) return rc;
-  if ((rc = geo_compact(ctx, d_dense, d_keep, n, d_out, d_count + 2)) != GPDB_OK) return rc;  // order of i kept
-  int nc = 0;
-  CUDA_TRY(cudaMemcpyAsync(&nc, d_count + 2, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  if (nc > 0) {
-    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  const int32_t hand_offsets[2] = {0, n};
+  int32_t cluster_offsets[2];
+  return find_clusters(ctx, 1, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets);
+}
+
+int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *hands,
+                             int32_t min_inliers, gpdb_pose *clusters_out, int32_t *cluster_offsets_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (n_groups < 0 || !hand_offsets || !cluster_offsets_out || hand_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: need n_groups >= 0, hand_offsets[n_groups + 1] starting "
+                   "at 0 and cluster_offsets_out");
+    return GPDB_ERR_INVALID;
   }
-  return nc;
+  for (int g = 0; g < n_groups; g++)
+    if (hand_offsets[g + 1] < hand_offsets[g]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: hand_offsets decrease at group %d", g);
+      return GPDB_ERR_INVALID;
+    }
+  if (hand_offsets[n_groups] > 0 && (!hands || !clusters_out)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: null hands or clusters_out");
+    return GPDB_ERR_INVALID;
+  }
+  return find_clusters(ctx, n_groups, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets_out);
 }
 
 void gpdb_free_result(gpdb_result *r) {

@@ -92,6 +92,7 @@ struct CloudDesc {
   int off, N, K;              // first point in the concatenated arrays, points, cameras
   int all_seen;               // every point is seen by every camera (cam mask complete): the per-point masks need not be read
   int nonunit;                // some normal is not of unit length (unit_normal): images holding one fold their cells exactly
+  int pos;                    // first of this cloud's sample positions in the store's samples (gpdb_set_clouds_samples)
   double vp[GPDB_MAX_CAMERAS][3];
 };
 // The clouds of a store as the kernels see them: d[n] descriptors, soff[n+1] the CSR offsets of the running batch call's
@@ -115,11 +116,13 @@ struct CloudSet {
   int *soff;            // [n + 1] sample offsets of the running batch call (device)
   int *off;             // [n + 1] point offsets (host)
   int *sel;             // [n + 1] per-cloud offsets of the last batch selection (host)
+  int *pos;             // [n + 1] per-cloud offsets of the sample positions while n_samples > 0 (host; the batch only)
   size_t point_cap, cell_cap, desc_cap;
   int n, maxk;          // clouds installed, largest camera count
   bool has_src;
-  double *samples;      // gpdb_set_samples positions (3 x n_samples) of the single cloud, or nullptr
-  int n_samples;
+  double *samples;      // sample positions (3 x n_samples): gpdb_set_samples (single cloud) / gpdb_set_clouds_samples (batch,
+  int n_samples;        // cloud b's at pos[b] .. pos[b+1]-1), or nullptr
+  int positions(int b) const { return n_samples ? pos[b + 1] - pos[b] : 0; }  // sample positions of cloud b
   DevCloud view;        // the concatenated arrays as the kernels read them
   int points() const { return n ? off[n] : 0; }
   CloudTable table() const { return CloudTable{desc, soff, n}; }
@@ -253,8 +256,11 @@ int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_sc
 
 // HandSearch::reevaluateHypotheses: labels + half / full flags of the given hands against the single cloud
 int geo_reeval(gpdb_ctx *ctx, gpdb_pose *d_hands, int n, int *d_labels);
-// Clustering::findClusters (remove_inliers = false): dense per-hand cluster records + keep flags (3 = cluster), for geo_compact
-int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, int min_inliers, gpdb_pose *d_dense, uint8_t *d_keep);
+// Clustering::findClusters (remove_inliers = false) on each of G groups of hands (group g: d_goff[g] .. d_goff[g+1]-1,
+// device offsets): dense per-hand cluster records + keep flags (3 = cluster), for geo_compact; d_gcount[G] (zeroed here)
+// receives the clusters per group
+int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, const int *d_goff, int G, int min_inliers, gpdb_pose *d_dense,
+                 uint8_t *d_keep, int *d_gcount);
 // the k highest-scoring of the n candidate records (scores filled), descending, stable -> d_out[k]
 int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *d_out);
 

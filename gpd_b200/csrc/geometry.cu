@@ -1085,11 +1085,19 @@ __global__ void __launch_bounds__(128) k_reeval(const DevParams *Pp, DevCloud cl
 // 5 mm; cluster position = mean inlier position, score = lower bound of the 99 % confidence interval of the inlier
 // scores (Welford update in index order, :62-70). One warp per hand: the lanes test 32 hands j at a time, lane 0 folds
 // the inliers of the ballot IN INDEX ORDER, so the float64 running mean / variance are the reference's sequential ones.
+// Groups (goff[G+1]): hand i is clustered against the hands of its own group only, as findClusters on that group alone;
+// gcount[g] counts the group's clusters.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_clusters(const gpdb_pose *__restrict__ hands, int n, int min_inliers, double cos_thresh,
-                           gpdb_pose *__restrict__ out, uint8_t *__restrict__ keep) {
+__global__ void k_clusters(const gpdb_pose *__restrict__ hands, int n, const int *__restrict__ goff, int G, int min_inliers,
+                           double cos_thresh, gpdb_pose *__restrict__ out, uint8_t *__restrict__ keep, int *gcount) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (i >= n) return;
+  int g = 0, gh = G;  // largest g with goff[g] <= i: empty groups share their offset with the next group
+  while (gh - g > 1) {
+    const int mid = (g + gh) >> 1;
+    if (__ldg(goff + mid) <= i) g = mid; else gh = mid;
+  }
+  const int lo = __ldg(goff + g), hi = __ldg(goff + g + 1);
   const double AXIS_ALIGN_DIST_THRESH = 0.005, MAX_DIST_THRESH = 0.05;
   const double ai[3] = {hands[i].frame[6], hands[i].frame[7], hands[i].frame[8]};
   const double pi[3] = {hands[i].position[0], hands[i].position[1], hands[i].position[2]};
@@ -1100,10 +1108,10 @@ __global__ void k_clusters(const gpdb_pose *__restrict__ hands, int n, int min_i
     for (int c = 0; c < 3; c++) outer[r][c] = ai[r] * ai[c];
   int num_inliers = 0;
   double pd[3] = {0.0, 0.0, 0.0}, mean = 0.0, sd = 0.0;
-  for (int j0 = 0; j0 < n; j0 += 32) {
+  for (int j0 = lo; j0 < hi; j0 += 32) {
     const int j = j0 + lane;
     bool inl = false;
-    if (j < n && j != i) {
+    if (j < hi && j != i) {
       const double aj[3] = {hands[j].frame[6], hands[j].frame[7], hands[j].frame[8]};
       const double axis_aligned = ai[0] * aj[0] + ai[1] * aj[1] + ai[2] * aj[2];
       const double d[3] = {pi[0] - hands[j].position[0], pi[1] - hands[j].position[1], pi[2] - hands[j].position[2]};
@@ -1142,6 +1150,7 @@ __global__ void k_clusters(const gpdb_pose *__restrict__ hands, int n, int min_i
       for (int r = 0; r < 3; r++) o.position[r] = pi[r] + pd[r];
       o.score = (float)conf_lb;
       k = 3;  // VALID | FILTERED: geo_compact keeps it
+      atomicAdd(gcount + g, 1);
     }
     out[i] = o;
     keep[i] = k;
@@ -2909,10 +2918,13 @@ int geo_reeval(gpdb_ctx *ctx, gpdb_pose *d_hands, int n, int *d_labels) {
   return GPDB_OK;
 }
 
-int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, int min_inliers, gpdb_pose *d_dense, uint8_t *d_keep) {
+int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, const int *d_goff, int G, int min_inliers, gpdb_pose *d_dense,
+                 uint8_t *d_keep, int *d_gcount) {
+  CUDA_TRY(cudaMemsetAsync(d_gcount, 0, sizeof(int) * (size_t)G, ctx->stream));
   if (n <= 0) return GPDB_OK;
   const double cos_thresh = std::cos(12.0 * M_PI / 180.0);  // AXIS_ALIGN_ANGLE_THRESH (clustering.cpp:9)
-  k_clusters<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(d_hands, n, min_inliers, cos_thresh, d_dense, d_keep);
+  k_clusters<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(d_hands, n, d_goff, G, min_inliers, cos_thresh, d_dense, d_keep,
+                                                            d_gcount);
   LAUNCH_CHECK();
   return GPDB_OK;
 }

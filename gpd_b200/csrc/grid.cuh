@@ -15,7 +15,7 @@ __device__ __forceinline__ int cell_of(const G &P, float v, int a) {
 }
 
 // position of a sample: a cloud point (index < n_points: Cloud::getSampleIndices) or an arbitrary float64 position
-// (index >= n_points: Cloud::setSamples / gpdb_set_samples)
+// (index >= n_points: Cloud::setSamples / gpdb_set_samples / gpdb_set_clouds_samples)
 __device__ __forceinline__ void sample_position(const DevCloud &cl, int si, double out[3]) {
   if (si < cl.n_points) {
     out[0] = (double)cl.xyz[3 * (size_t)si];
@@ -36,6 +36,7 @@ __device__ __forceinline__ DevCloud local_cloud(const CloudDesc &D, DevCloud cl)
   cl.nrm += 3 * (size_t)D.off;
   cl.cam += D.off;
   cl.cell_start += D.cell_base;
+  cl.samples += 3 * (size_t)D.pos;
   cl.n_points = D.N;
   return cl;
 }

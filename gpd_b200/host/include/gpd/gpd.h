@@ -20,8 +20,10 @@
 #include <iostream>
 #include <map>
 #include <memory>
+#include <random>
 #include <sstream>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "gpd_b200.h"
@@ -246,9 +248,26 @@ class GraspDetector {
   ~GraspDetector();
   // grasp_detector.cpp:192-328: candidates -> filter -> images -> classify (one gpdb_detect) -> select -> sort
   std::vector<std::unique_ptr<candidate::Hand>> detectGrasps(const util::Cloud &cloud);
+  // detectGrasps of every cloud of a batch of views in one device pass per step: the processed clouds (installed by
+  // preprocessPointClouds, else by gpdb_set_clouds) -> gpdb_detect_batch_select at each cloud's sample indices ->
+  // gpdb_find_clusters_batch (with the per-cloud "3 clusters or fewer: add all grasps" rule) -> sort. Result b equals
+  // detectGrasps(clouds[b]).
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> detectGrasps(const std::vector<util::Cloud> &clouds);
   // CandidatesGenerator::preprocessPointCloud (candidates_generator.cpp:14-37) on the device: removeNans,
   // filterWorkspace, voxelizeCloud, calculateNormals (skipped when the cloud brings normals), then subsample
   void preprocessPointCloud(util::Cloud &cloud);
+  // preprocessPointCloud of every cloud in one call (gpdb_preprocess_clouds), the processed clouds left installed as the
+  // batch; either every cloud brings normals or none does. Returns false (and prints the error) when the call fails.
+  bool preprocessPointClouds(std::vector<util::Cloud> &clouds);
+  // the batch counterparts of candidateSamplePositions / classifyAtPositions / findClustersOnDevice over the installed
+  // batch (one entry per cloud; positions: 3 x m_b column-major, installed with gpdb_set_clouds_samples; empty
+  // positions: the clouds' sample indices)
+  std::vector<std::vector<double>> candidateSamplePositions(const std::vector<util::Cloud> &clouds,
+                                                            const std::vector<std::vector<double>> *positions);
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> classifyAtPositions(
+      const std::vector<util::Cloud> &clouds, const std::vector<std::vector<double>> &positions, double min_score);
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> findClustersOnDevice(
+      const std::vector<std::vector<std::unique_ptr<candidate::Hand>>> &hands, int min_inliers);
   const gpdb_preprocess_params &getPreprocessParams() const { return pre_params_; }
   std::vector<std::unique_ptr<candidate::Hand>> selectGrasps(std::vector<std::unique_ptr<candidate::Hand>> &hands) const;
   // GraspDetector::generateGraspCandidates + filterGraspsWorkspace / filterGraspsDirection (grasp_detector.cpp:330-398,
@@ -295,7 +314,13 @@ class GraspDetector {
   int min_inliers_{1};
   bool has_classifier_{false};
   std::string model_file_, weights_file_;
+  // clouds whose processed arrays are resident as the batch, with their revisions
+  std::vector<std::pair<const util::Cloud *, unsigned>> installed_batch_;
   bool ensureCloud(const util::Cloud &cloud);
+  bool ensureBatch(const std::vector<util::Cloud> &clouds);
+  // gpdb_set_clouds_samples (positions given) or the sample indices of every cloud, in CSR form
+  bool batchSamples(const std::vector<util::Cloud> &clouds, const std::vector<std::vector<double>> *positions,
+                    std::vector<int32_t> &offsets, std::vector<int32_t> &idx);
 };
 
 // SequentialImportanceSampling (include/gpd/sequential_importance_sampling.h, src/gpd/sequential_importance_sampling.cpp:
@@ -309,13 +334,26 @@ class SequentialImportanceSampling {
  public:
   explicit SequentialImportanceSampling(const std::string &config_filename);
   std::vector<std::unique_ptr<candidate::Hand>> detectGrasps(util::Cloud &cloud);
+  // detectGrasps of every cloud of a batch (processed by detector().preprocessPointClouds), each round one
+  // gpdb_set_clouds_samples + one gpdb_hand_search_batch for all clouds, the final classification one gpdb_detect_batch
+  // and one gpdb_find_clusters_batch. Cloud b draws from its own generator seeded seed + b, so result b equals
+  // detectGrasps(clouds[b]) with setSeed(seed + b). A cloud without initial candidates returns no grasps.
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> detectGrasps(std::vector<util::Cloud> &clouds);
   void setSeed(unsigned seed) { seed_ = seed; }
-  // 3 x m positions of every sample that was evaluated / that carried a hand set, over all rounds (for the parity tests)
+  // 3 x m positions of every sample that was evaluated / that carried a hand set, over all rounds (for the parity tests);
+  // after a batch run, those of cloud b (batchEvaluatedPositions()[b], batchHandSetPositions()[b])
   const std::vector<double> &evaluatedPositions() const { return evaluated_; }
   const std::vector<double> &handSetPositions() const { return kept_; }
+  const std::vector<std::vector<double>> &batchEvaluatedPositions() const { return evaluated_batch_; }
+  const std::vector<std::vector<double>> &batchHandSetPositions() const { return kept_batch_; }
   GraspDetector &detector() { return *grasp_detector_; }
 
  private:
+  // the positions of one round (:109-128): Gaussians around the kept hand-set positions, then uniform draws of the cloud's
+  // initial sample points inside the workspace. gen and distr (normal, sigma = standard_deviation) carry over between rounds.
+  std::vector<double> drawRound(std::mt19937 &gen, std::normal_distribution<double> &distr, const util::Cloud &cloud,
+                                const std::vector<double> &kept, const std::vector<int> &init_indices) const;
+  std::vector<std::vector<double>> evaluated_batch_, kept_batch_;
   int num_init_samples_{50}, num_iterations_{5}, num_samples_{50}, sampling_method_{0};
   double prob_rand_samples_{0.3}, radius_{0.02}, min_score_{0};
   std::vector<double> workspace_;

@@ -7,6 +7,9 @@
 //               (src/cem_detect_grasps.cpp:14-66 -> SequentialImportanceSampling::detectGrasps), and prints the evaluated
 //               sample positions (SIS_SAMPLE lines) so that a test can recompute the result independently.
 // --gpus N      shards the samples over N GPUs inside libgpd_b200 (GraspDetector::detectGraspsMultiGpu).
+// --batch PCD_FILE...  runs every PCD file as one cloud of a batch (one device pass per step for all of them, with or
+//               without --sis; cloud b seeds its sampler with SEED + b) and prints, per file, a line `CLOUD b PCD_FILE`
+//               followed by the result lines a run on that file alone prints.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -26,13 +29,71 @@ static bool checkFileExists(const std::string &file_name) {
   return true;
 }
 
+static void print_grasps(const std::vector<std::unique_ptr<candidate::Hand>> &grasps) {
+  for (size_t i = 0; i < grasps.size() && i < 5; i++) {
+    printf("--- grasp %zu ---\n", i);
+    grasps[i]->print();
+  }
+  printf("RESULT n_grasps=%zu best_score=%.6f\n", grasps.size(), grasps.empty() ? 0.0 : grasps[0]->getScore());
+}
+
+static void print_sis(const std::vector<std::unique_ptr<candidate::Hand>> &grasps, const std::vector<double> &kept,
+                      const std::vector<double> &evaluated) {
+  for (size_t i = 0; i + 2 < kept.size(); i += 3) printf("SIS_SAMPLE %.17g %.17g %.17g\n", kept[i], kept[i + 1], kept[i + 2]);
+  for (size_t i = 0; i < grasps.size(); i++)
+    printf("SIS_GRASP %.9g %.17g %.17g %.17g\n", grasps[i]->getScore(), grasps[i]->getPosition()[0], grasps[i]->getPosition()[1],
+           grasps[i]->getPosition()[2]);
+  printf("RESULT n_grasps=%zu evaluated=%zu hand_sets=%zu\n", grasps.size(), evaluated.size() / 3, kept.size() / 3);
+}
+
+// --batch: every PCD file one cloud of a batch
+static int run_batch(const std::string &config_filename, const std::vector<std::string> &files, bool sis, unsigned sis_seed) {
+  for (const std::string &f : files)
+    if (!checkFileExists(f)) return -1;
+  util::ConfigFile config_file(config_filename);
+  config_file.ExtractKeys();
+  if (config_file.getValueOfKey<bool>("centered_at_origin", false)) {
+    std::cout << "Error: --batch does not support centered_at_origin\n";
+    return -1;
+  }
+  std::vector<double> camera_position = config_file.getValueOfKeyAsStdVectorDouble("camera_position", "0.0 0.0 0.0");
+  std::vector<util::Cloud> clouds;
+  for (const std::string &f : files) {
+    clouds.emplace_back(f, camera_position);
+    if (clouds.back().size() == 0) {
+      std::cout << "Error: Input point cloud " << f << " is empty or does not exist!\n";
+      return -1;
+    }
+  }
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> grasps;
+  std::unique_ptr<SequentialImportanceSampling> sampler;
+  std::unique_ptr<GraspDetector> detector;
+  if (sis) {
+    sampler = std::make_unique<SequentialImportanceSampling>(config_filename);
+    sampler->setSeed(sis_seed);
+    if (!sampler->detector().preprocessPointClouds(clouds)) return -1;
+    grasps = sampler->detectGrasps(clouds);
+  } else {
+    detector = std::make_unique<GraspDetector>(config_filename);
+    if (!detector->preprocessPointClouds(clouds)) return -1;
+    grasps = detector->detectGrasps(clouds);
+  }
+  for (size_t b = 0; b < files.size(); b++) {
+    printf("CLOUD %zu %s\n", b, files[b].c_str());
+    if (sis) print_sis(grasps[b], sampler->batchHandSetPositions()[b], sampler->batchEvaluatedPositions()[b]);
+    else print_grasps(grasps[b]);
+  }
+  return 0;
+}
+
 int main(int argc, char *argv[]) {
-  bool dump = false, sis = false;
+  bool dump = false, sis = false, batch = false;
   unsigned sis_seed = 1;
   int gpus = 1;
   std::vector<std::string> args;
   for (int i = 1; i < argc; i++) {
     if (std::strcmp(argv[i], "--dump-config") == 0) dump = true;
+    else if (std::strcmp(argv[i], "--batch") == 0) batch = true;
     else if (std::strcmp(argv[i], "--sis") == 0) {
       sis = true;
       if (i + 1 < argc && argv[i + 1][0] >= '0' && argv[i + 1][0] <= '9') sis_seed = (unsigned)std::atoi(argv[++i]);
@@ -80,6 +141,7 @@ int main(int argc, char *argv[]) {
     printf("}\n");
     return 0;
   }
+  if (batch) return run_batch(config_filename, std::vector<std::string>(args.begin() + 1, args.end()), sis, sis_seed);
   const std::string pcd_filename = args[1];
   if (!checkFileExists(pcd_filename)) return -1;
   util::ConfigFile config_file(config_filename);
@@ -99,12 +161,7 @@ int main(int argc, char *argv[]) {
     sampler.setSeed(sis_seed);
     sampler.detector().preprocessPointCloud(cloud);
     std::vector<std::unique_ptr<candidate::Hand>> grasps = sampler.detectGrasps(cloud);
-    const std::vector<double> &kept = sampler.handSetPositions();
-    for (size_t i = 0; i + 2 < kept.size(); i += 3) printf("SIS_SAMPLE %.17g %.17g %.17g\n", kept[i], kept[i + 1], kept[i + 2]);
-    for (size_t i = 0; i < grasps.size(); i++)
-      printf("SIS_GRASP %.9g %.17g %.17g %.17g\n", grasps[i]->getScore(), grasps[i]->getPosition()[0], grasps[i]->getPosition()[1],
-             grasps[i]->getPosition()[2]);
-    printf("RESULT n_grasps=%zu evaluated=%zu hand_sets=%zu\n", grasps.size(), sampler.evaluatedPositions().size() / 3, kept.size() / 3);
+    print_sis(grasps, sampler.handSetPositions(), sampler.evaluatedPositions());
     return 0;
   }
   GraspDetector detector(config_filename);
@@ -117,10 +174,6 @@ int main(int argc, char *argv[]) {
     printf("Reversing normal directions ...\n");
   }
   std::vector<std::unique_ptr<candidate::Hand>> grasps = gpus > 1 ? detector.detectGraspsMultiGpu(cloud, gpus) : detector.detectGrasps(cloud);
-  for (size_t i = 0; i < grasps.size() && i < 5; i++) {
-    printf("--- grasp %zu ---\n", i);
-    grasps[i]->print();
-  }
-  printf("RESULT n_grasps=%zu best_score=%.6f\n", grasps.size(), grasps.empty() ? 0.0 : grasps[0]->getScore());
+  print_grasps(grasps);
   return 0;
 }

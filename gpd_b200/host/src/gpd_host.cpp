@@ -1104,6 +1104,232 @@ std::vector<std::unique_ptr<candidate::Hand>> GraspDetector::detectGrasps(const 
   return hands;
 }
 
+// ---- batches of clouds ------------------------------------------------------------------------------------------------
+bool GraspDetector::preprocessPointClouds(std::vector<util::Cloud> &clouds) {
+  installed_batch_.clear();
+  if (!ctx_ || clouds.empty()) return false;
+  const int B = (int)clouds.size();
+  const bool with_normals = clouds[0].hasNormals();
+  std::vector<int32_t> roff(B + 1, 0), ks(B);
+  std::vector<float> xyz;
+  std::vector<double> nrm, vps;
+  std::vector<int32_t> cam;
+  bool any_cam = false;
+  for (const util::Cloud &c : clouds) any_cam |= !c.getCameraSource().empty();
+  for (int b = 0; b < B; b++) {
+    const util::Cloud &c = clouds[b];
+    printf("Processing cloud with %zu points.\n", c.size());
+    if (c.hasNormals() != with_normals) {
+      printf("ERROR: preprocessPointClouds: either every cloud brings normals or none does\n");
+      return false;
+    }
+    roff[b + 1] = roff[b] + (int)c.size();
+    ks[b] = c.numCameras();
+    xyz.insert(xyz.end(), c.getPoints().begin(), c.getPoints().end());
+    if (with_normals) nrm.insert(nrm.end(), c.getNormals().begin(), c.getNormals().end());
+    vps.insert(vps.end(), c.getViewPoints().begin(), c.getViewPoints().end());
+    // camera sources: k x N column-major = the N x k row blocks the C-ABI takes; a cloud without one: seen by every camera
+    if (any_cam) {
+      if (c.getCameraSource().empty()) cam.insert(cam.end(), c.size() * (size_t)ks[b], 1);
+      else cam.insert(cam.end(), c.getCameraSource().begin(), c.getCameraSource().end());
+    }
+  }
+  gpdb_preprocess_params pp = pre_params_;
+  pp.estimate_normals = with_normals ? 0 : 1;  // supplied normals are kept, as preprocessPointCloud does
+  std::vector<int32_t> poff(B + 1, 0);
+  if (gpdb_preprocess_clouds(ctx_, B, roff.data(), xyz.data(), with_normals ? nrm.data() : nullptr, any_cam ? cam.data() : nullptr,
+                             ks.data(), vps.data(), &pp, poff.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return false;
+  }
+  const int N = poff[B];
+  std::vector<float> pxyz(3 * (size_t)N);
+  std::vector<double> pnrm(3 * (size_t)N);
+  size_t ncam = 0;
+  for (int b = 0; b < B; b++) ncam += (size_t)(poff[b + 1] - poff[b]) * ks[b];
+  std::vector<int32_t> pcam(ncam);
+  if (N > 0 && gpdb_get_clouds(ctx_, pxyz.data(), pnrm.data(), pcam.data(), nullptr) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return false;
+  }
+  size_t c0 = 0;
+  for (int b = 0; b < B; b++) {
+    const size_t o0 = poff[b], o1 = poff[b + 1], k = ks[b];
+    if (pp.voxelize) printf("Voxelized cloud: %d\n", (int)(o1 - o0));
+    clouds[b].setProcessed(std::vector<float>(pxyz.begin() + 3 * o0, pxyz.begin() + 3 * o1),
+                           std::vector<double>(pnrm.begin() + 3 * o0, pnrm.begin() + 3 * o1),
+                           std::vector<int>(pcam.begin() + c0, pcam.begin() + c0 + (o1 - o0) * k));
+    c0 += (o1 - o0) * k;
+    clouds[b].subsample(num_samples_);
+    installed_batch_.emplace_back(&clouds[b], clouds[b].revision());
+  }
+  return true;
+}
+
+bool GraspDetector::ensureBatch(const std::vector<util::Cloud> &clouds) {
+  bool same = installed_batch_.size() == clouds.size();
+  for (size_t b = 0; same && b < clouds.size(); b++)
+    same = installed_batch_[b].first == &clouds[b] && installed_batch_[b].second == clouds[b].revision();
+  if (same) return true;
+  installed_batch_.clear();
+  const int B = (int)clouds.size();
+  std::vector<int32_t> off(B + 1, 0), ks(B);
+  std::vector<float> xyz;
+  std::vector<double> nrm, vps;
+  std::vector<int32_t> cam;
+  bool any_cam = false;
+  for (const util::Cloud &c : clouds) any_cam |= !c.getCameraSource().empty();
+  for (int b = 0; b < B; b++) {
+    const util::Cloud &c = clouds[b];
+    if (c.getNormals().size() != 3 * c.size()) {
+      printf("ERROR: cloud %d has no surface normals: call GraspDetector::preprocessPointClouds first\n", b);
+      return false;
+    }
+    off[b + 1] = off[b] + (int)c.size();
+    ks[b] = c.numCameras();
+    xyz.insert(xyz.end(), c.getPoints().begin(), c.getPoints().end());
+    nrm.insert(nrm.end(), c.getNormals().begin(), c.getNormals().end());
+    vps.insert(vps.end(), c.getViewPoints().begin(), c.getViewPoints().end());
+    if (any_cam) {
+      if (c.getCameraSource().empty()) cam.insert(cam.end(), c.size() * (size_t)ks[b], 1);
+      else cam.insert(cam.end(), c.getCameraSource().begin(), c.getCameraSource().end());
+    }
+  }
+  if (gpdb_set_clouds(ctx_, B, off.data(), xyz.data(), nrm.data(), any_cam ? cam.data() : nullptr, ks.data(), vps.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return false;
+  }
+  for (int b = 0; b < B; b++) installed_batch_.emplace_back(&clouds[b], clouds[b].revision());
+  return true;
+}
+
+bool GraspDetector::batchSamples(const std::vector<util::Cloud> &clouds, const std::vector<std::vector<double>> *positions,
+                                 std::vector<int32_t> &offsets, std::vector<int32_t> &idx) {
+  const size_t B = clouds.size();
+  offsets.assign(B + 1, 0);
+  idx.clear();
+  if (!positions) {
+    for (size_t b = 0; b < B; b++) {
+      idx.insert(idx.end(), clouds[b].getSampleIndices().begin(), clouds[b].getSampleIndices().end());
+      offsets[b + 1] = (int32_t)idx.size();
+    }
+    return true;
+  }
+  std::vector<int32_t> poff(B + 1, 0);
+  std::vector<double> all;
+  for (size_t b = 0; b < B; b++) {
+    const std::vector<double> &p = (*positions)[b];
+    all.insert(all.end(), p.begin(), p.end());
+    poff[b + 1] = poff[b] + (int32_t)(p.size() / 3);
+    for (int32_t j = 0; j < poff[b + 1] - poff[b]; j++) idx.push_back((int32_t)clouds[b].size() + j);  // N_b + j
+    offsets[b + 1] = (int32_t)idx.size();
+  }
+  if (gpdb_set_clouds_samples(ctx_, poff.data(), all.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return false;
+  }
+  return true;
+}
+
+std::vector<std::vector<double>> GraspDetector::candidateSamplePositions(const std::vector<util::Cloud> &clouds,
+                                                                         const std::vector<std::vector<double>> *positions) {
+  std::vector<std::vector<double>> out;
+  std::vector<int32_t> offsets, idx;
+  if (!ctx_ || clouds.empty() || !ensureBatch(clouds) || !batchSamples(clouds, positions, offsets, idx)) return out;
+  gpdb_result r;
+  std::vector<int32_t> coff(clouds.size() + 1);
+  if (gpdb_hand_search_batch(ctx_, offsets.data(), idx.data(), &r, coff.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return out;
+  }
+  out.resize(clouds.size());
+  for (size_t b = 0; b < clouds.size(); b++) {
+    int last_slot = -1;
+    for (int i = coff[b]; i < coff[b + 1]; i++) {  // a cloud's candidates are in (sample slot, pose slot) order
+      if (r.candidates[i].sample_slot == last_slot) continue;
+      last_slot = r.candidates[i].sample_slot;
+      for (int k = 0; k < 3; k++) out[b].push_back(r.candidates[i].sample[k]);
+    }
+  }
+  gpdb_free_result(&r);
+  return out;
+}
+
+std::vector<std::vector<std::unique_ptr<candidate::Hand>>> GraspDetector::classifyAtPositions(
+    const std::vector<util::Cloud> &clouds, const std::vector<std::vector<double>> &positions, double min_score) {
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> out(clouds.size());
+  std::vector<int32_t> offsets, idx;
+  if (!ctx_ || !has_classifier_ || clouds.empty() || !ensureBatch(clouds) || !batchSamples(clouds, &positions, offsets, idx))
+    return out;
+  gpdb_result r;
+  std::vector<int32_t> coff(clouds.size() + 1);
+  if (gpdb_detect_batch(ctx_, offsets.data(), idx.data(), &r, coff.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return out;
+  }
+  for (size_t b = 0; b < clouds.size(); b++)
+    for (int i = coff[b]; i < coff[b + 1]; i++)
+      if ((double)r.candidates[i].score > min_score) out[b].push_back(std::make_unique<candidate::Hand>(r.candidates[i]));
+  gpdb_free_result(&r);
+  return out;
+}
+
+std::vector<std::vector<std::unique_ptr<candidate::Hand>>> GraspDetector::findClustersOnDevice(
+    const std::vector<std::vector<std::unique_ptr<candidate::Hand>>> &hands, int min_inliers) {
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> out(hands.size());
+  if (!ctx_) return out;
+  std::vector<int32_t> hoff(hands.size() + 1, 0), coff(hands.size() + 1);
+  std::vector<gpdb_pose> in;
+  for (size_t g = 0; g < hands.size(); g++) {
+    for (const auto &h : hands[g]) in.push_back(h->raw());
+    hoff[g + 1] = (int32_t)in.size();
+  }
+  std::vector<gpdb_pose> res(in.size());
+  if (gpdb_find_clusters_batch(ctx_, (int)hands.size(), hoff.data(), in.data(), min_inliers, res.data(), coff.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return out;
+  }
+  for (size_t g = 0; g < hands.size(); g++)
+    for (int i = coff[g]; i < coff[g + 1]; i++) out[g].push_back(std::make_unique<candidate::Hand>(res[i]));
+  return out;
+}
+
+std::vector<std::vector<std::unique_ptr<candidate::Hand>>> GraspDetector::detectGrasps(const std::vector<util::Cloud> &clouds) {
+  const size_t B = clouds.size();
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> hands(B);
+  if (!ctx_ || !has_classifier_) {
+    printf("ERROR: detector not initialised (%s)\n", ctx_ ? "no classifier weights" : gpdb_last_error(nullptr));
+    return hands;
+  }
+  std::vector<int32_t> offsets, idx;
+  if (B == 0 || !ensureBatch(clouds) || !batchSamples(clouds, nullptr, offsets, idx)) return hands;
+  // steps 1-4 + selectGrasps of every cloud in one call (grasp_detector.cpp:222-283,405-420)
+  gpdb_result r;
+  std::vector<int32_t> soff(B + 1);
+  if (gpdb_detect_batch_select(ctx_, offsets.data(), idx.data(), num_selected_, &r, soff.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx_));
+    return hands;
+  }
+  printf("Generated %d hand sets in %zu clouds.\n", r.n_samples, B);
+  printf("Number of grasp candidates within workspace and gripper width: %d\n", r.n_total_candidates);
+  for (size_t b = 0; b < B; b++)
+    for (int i = soff[b]; i < soff[b + 1]; i++) hands[b].push_back(std::make_unique<candidate::Hand>(r.candidates[i]));
+  gpdb_free_result(&r);
+  if (cluster_grasps_) {  // 6. Cluster the grasps of every cloud in one call (grasp_detector.cpp:283-301)
+    std::vector<std::vector<std::unique_ptr<candidate::Hand>>> clusters = findClustersOnDevice(hands, min_inliers_);
+    for (size_t b = 0; b < B; b++) {
+      if (clusters[b].size() <= 3)  // not enough clusters: add all grasps of that cloud
+        for (auto &h : hands[b]) clusters[b].push_back(std::move(h));
+      hands[b] = std::move(clusters[b]);
+    }
+  }
+  for (auto &hb : hands)
+    std::sort(hb.begin(), hb.end(), [](const std::unique_ptr<candidate::Hand> &a, const std::unique_ptr<candidate::Hand> &b) {
+      return a->getScore() > b->getScore();
+    });
+  return hands;
+}
+
 // ---- SequentialImportanceSampling (sequential_importance_sampling.cpp) -------------------------------------------------
 SequentialImportanceSampling::SequentialImportanceSampling(const std::string &config_filename) {
   util::ConfigFile config_file(config_filename);
@@ -1121,6 +1347,104 @@ SequentialImportanceSampling::SequentialImportanceSampling(const std::string &co
   clustering_ = std::make_unique<Clustering>(config_file.getValueOfKey<int>("min_inliers", 1));
 }
 
+std::vector<double> SequentialImportanceSampling::drawRound(std::mt19937 &gen, std::normal_distribution<double> &distr,
+                                                           const util::Cloud &cloud, const std::vector<double> &kept,
+                                                           const std::vector<int> &init_indices) const {
+  auto uniform_index = [&](size_t n) { return (size_t)(gen() % (unsigned long)n); };  // rand() % n upstream
+  const int num_rand_samples = (int)(prob_rand_samples_ * num_samples_);  // :100-101
+  const int num_gauss_samples = num_samples_ - num_rand_samples;
+  const double sigma = radius_;
+  const double term = 1.0 / std::sqrt(std::pow(2.0 * M_PI, 3.0) * std::pow(sigma, 3.0));
+  std::vector<double> samples(3 * (size_t)num_samples_, 0.0);
+  const size_t m = kept.size() / 3;
+  int j = 0;
+  while (j < num_gauss_samples) {  // 2.1 samples close to existing affordances (:187-236)
+    const size_t idx = uniform_index(m);
+    double x[3];
+    for (int k = 0; k < 3; k++) x[k] = kept[3 * idx + k] + distr(gen);
+    if (sampling_method_ == 1) {  // MAX_OF_GAUSSIANS: rejection sampling (:213-234)
+      auto dens = [&](size_t h) {
+        double d2 = 0;
+        for (int k = 0; k < 3; k++) d2 += (x[k] - kept[3 * h + k]) * (x[k] - kept[3 * h + k]);
+        return term * std::exp((-1.0 / (2.0 * sigma)) * d2);
+      };
+      double maxp = 0;
+      for (size_t h = 0; h < m; h++) maxp = std::max(maxp, dens(h));
+      if (!(dens(idx) >= maxp)) continue;
+    }
+    for (int k = 0; k < 3; k++) samples[3 * (size_t)j + k] = x[k];
+    j++;
+  }
+  int i = 0, guard = 0;
+  while (i < num_rand_samples && guard++ < 1000000) {  // 2.2 uniform samples inside the workspace (:239-270)
+    const int pi = init_indices.empty() ? (int)uniform_index(cloud.size()) : init_indices[uniform_index(init_indices.size())];
+    const double sx = cloud.getPoints()[3 * (size_t)pi], sy = cloud.getPoints()[3 * (size_t)pi + 1], sz = cloud.getPoints()[3 * (size_t)pi + 2];
+    if (sx >= workspace_[0] && sx <= workspace_[1] && sy >= workspace_[2] && sy <= workspace_[3] && sz >= workspace_[4] &&
+        sz <= workspace_[5]) {
+      samples[3 * (size_t)(num_gauss_samples + i)] = sx;
+      samples[3 * (size_t)(num_gauss_samples + i) + 1] = sy;
+      samples[3 * (size_t)(num_gauss_samples + i) + 2] = sz;
+      i++;
+    }
+  }
+  return samples;
+}
+
+std::vector<std::vector<std::unique_ptr<candidate::Hand>>> SequentialImportanceSampling::detectGrasps(
+    std::vector<util::Cloud> &clouds) {
+  const size_t B = clouds.size();
+  std::vector<std::vector<std::unique_ptr<candidate::Hand>>> out(B);
+  evaluated_batch_.assign(B, {});
+  kept_batch_.assign(B, {});
+  if (B == 0) return out;
+  // 1. initial grasp hypotheses of every cloud in one hand search (:68-79)
+  std::vector<std::vector<int>> init_indices(B);
+  for (size_t b = 0; b < B; b++) {
+    clouds[b].setSamples({});
+    clouds[b].subsample(num_init_samples_);
+    init_indices[b] = clouds[b].getSampleIndices();
+    for (int i : init_indices[b])
+      for (int k = 0; k < 3; k++) evaluated_batch_[b].push_back((double)clouds[b].getPoints()[3 * (size_t)i + k]);
+  }
+  kept_batch_ = grasp_detector_->candidateSamplePositions(clouds, nullptr);
+  if (kept_batch_.size() != B) {
+    kept_batch_.assign(B, {});
+    return out;
+  }
+  std::vector<std::mt19937> gen;
+  std::vector<std::normal_distribution<double>> distr;
+  std::vector<char> active(B);
+  for (size_t b = 0; b < B; b++) {
+    gen.emplace_back(seed_ + (unsigned)b);
+    distr.emplace_back(0.0, radius_);
+    active[b] = !kept_batch_[b].empty();  // a cloud without initial candidates stops here, the others go on
+    printf("Cloud %zu: initially detected grasp candidates: %zu\n", b, kept_batch_[b].size() / 3);
+  }
+  // 2. importance sampling (:109-160): every round draws each active cloud's positions on the host, then one
+  // gpdb_set_clouds_samples + one gpdb_hand_search_batch evaluate them for all clouds
+  for (int it = 0; it < num_iterations_; it++) {
+    std::vector<std::vector<double>> samples(B);
+    for (size_t b = 0; b < B; b++) {
+      if (!active[b]) continue;
+      samples[b] = drawRound(gen[b], distr[b], clouds[b], kept_batch_[b], init_indices[b]);
+      evaluated_batch_[b].insert(evaluated_batch_[b].end(), samples[b].begin(), samples[b].end());
+    }
+    std::vector<std::vector<double>> fresh = grasp_detector_->candidateSamplePositions(clouds, &samples);
+    if (fresh.size() != B) return out;
+    for (size_t b = 0; b < B; b++) kept_batch_[b].insert(kept_batch_[b].end(), fresh[b].begin(), fresh[b].end());
+  }
+  // 3. classify the grasps of all clouds (:168-170), 4. cluster them (:177-179)
+  std::vector<std::vector<double>> final_positions(B);
+  for (size_t b = 0; b < B; b++)
+    if (active[b]) final_positions[b] = kept_batch_[b];
+  out = grasp_detector_->classifyAtPositions(clouds, final_positions, min_score_);
+  if (out.size() != B) out.resize(B);
+  if (clustering_->getMinInliers() > 0) out = grasp_detector_->findClustersOnDevice(out, clustering_->getMinInliers());
+  if (out.size() != B) out.resize(B);
+  for (size_t b = 0; b < B; b++) printf("Cloud %zu: found %zu grasps.\n", b, out[b].size());
+  return out;
+}
+
 std::vector<std::unique_ptr<candidate::Hand>> SequentialImportanceSampling::detectGrasps(util::Cloud &cloud) {
   std::vector<std::unique_ptr<candidate::Hand>> none;
   evaluated_.clear();
@@ -1130,7 +1454,6 @@ std::vector<std::unique_ptr<candidate::Hand>> SequentialImportanceSampling::dete
     return none;
   }
   std::mt19937 gen(seed_);
-  auto uniform_index = [&](size_t n) { return (size_t)(gen() % (unsigned long)n); };  // rand() % n upstream
   // 1. Find initial grasp hypotheses (:68-79)
   cloud.setSamples({});
   cloud.subsample(num_init_samples_);
@@ -1139,46 +1462,11 @@ std::vector<std::unique_ptr<candidate::Hand>> SequentialImportanceSampling::dete
   kept_ = grasp_detector_->candidateSamplePositions(cloud);
   printf("Initially detected grasp candidates: %zu\n", kept_.size() / 3);
   if (kept_.empty()) return none;
-  const int num_rand_samples = (int)(prob_rand_samples_ * num_samples_);  // :100-101
-  const int num_gauss_samples = num_samples_ - num_rand_samples;
-  const double sigma = radius_;
-  const double term = 1.0 / std::sqrt(std::pow(2.0 * M_PI, 3.0) * std::pow(sigma, 3.0));
-  std::normal_distribution<double> distr{0.0, sigma};
+  std::normal_distribution<double> distr{0.0, radius_};
   const std::vector<int> init_indices = cloud.getSampleIndices();
   // 2. Find grasp hypotheses using importance sampling (:109-160)
   for (int it = 0; it < num_iterations_; it++) {
-    std::vector<double> samples(3 * (size_t)num_samples_, 0.0);
-    const size_t m = kept_.size() / 3;
-    int j = 0;
-    while (j < num_gauss_samples) {  // 2.1 samples close to existing affordances (:187-236)
-      const size_t idx = uniform_index(m);
-      double x[3];
-      for (int k = 0; k < 3; k++) x[k] = kept_[3 * idx + k] + distr(gen);
-      if (sampling_method_ == 1) {  // MAX_OF_GAUSSIANS: rejection sampling (:213-234)
-        auto dens = [&](size_t h) {
-          double d2 = 0;
-          for (int k = 0; k < 3; k++) d2 += (x[k] - kept_[3 * h + k]) * (x[k] - kept_[3 * h + k]);
-          return term * std::exp((-1.0 / (2.0 * sigma)) * d2);
-        };
-        double maxp = 0;
-        for (size_t h = 0; h < m; h++) maxp = std::max(maxp, dens(h));
-        if (!(dens(idx) >= maxp)) continue;
-      }
-      for (int k = 0; k < 3; k++) samples[3 * (size_t)j + k] = x[k];
-      j++;
-    }
-    int i = 0, guard = 0;
-    while (i < num_rand_samples && guard++ < 1000000) {  // 2.2 uniform samples inside the workspace (:239-270)
-      const int pi = init_indices.empty() ? (int)uniform_index(cloud.size()) : init_indices[uniform_index(init_indices.size())];
-      const double sx = cloud.getPoints()[3 * (size_t)pi], sy = cloud.getPoints()[3 * (size_t)pi + 1], sz = cloud.getPoints()[3 * (size_t)pi + 2];
-      if (sx >= workspace_[0] && sx <= workspace_[1] && sy >= workspace_[2] && sy <= workspace_[3] && sz >= workspace_[4] &&
-          sz <= workspace_[5]) {
-        samples[3 * (size_t)(num_gauss_samples + i)] = sx;
-        samples[3 * (size_t)(num_gauss_samples + i) + 1] = sy;
-        samples[3 * (size_t)(num_gauss_samples + i) + 2] = sz;
-        i++;
-      }
-    }
+    std::vector<double> samples = drawRound(gen, distr, cloud, kept_, init_indices);
     // 2.3 evaluate grasp hypotheses at <samples> (:129-144)
     cloud.setSamples(samples);
     evaluated_.insert(evaluated_.end(), samples.begin(), samples.end());

@@ -25,7 +25,8 @@ EXPORTS = [
     "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
     "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
-    "gpdb_debug_path_counts", "gpdb_debug_lenet_layers",
+    "gpdb_debug_path_counts", "gpdb_debug_lenet_layers", "gpdb_set_clouds_samples", "gpdb_hand_search_batch",
+    "gpdb_find_clusters_batch",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -98,6 +99,9 @@ def lib():
     L.gpdb_detect_batch_select.argtypes = [vp, vp, vp, C.c_int32, C.POINTER(abi.Result), vp]
     L.gpdb_preprocess_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, C.POINTER(abi.PreprocessParams), vp]
     L.gpdb_get_clouds.argtypes = [vp, vp, vp, vp, vp]
+    L.gpdb_set_clouds_samples.argtypes = [vp, vp, vp]
+    L.gpdb_hand_search_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
+    L.gpdb_find_clusters_batch.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
     _LIB = L
     return L
 
@@ -389,17 +393,50 @@ class Context:
             raise ValueError(f"{len(sample_lists)} sample lists for a batch of {self._n_clouds} clouds (one list per cloud)")
         return pack_samples(sample_lists)
 
-    def detect_batch(self, sample_lists):
-        """gpdb_detect_batch: one list of cloud-local sample indices per installed cloud; returns one result dict per
-        cloud (views of the single batch result), each as detect() would return for that cloud alone."""
+    def _batch_result(self, fn, sample_lists):
         offsets, sidx = self._pack_batch_samples(sample_lists)
         res = abi.Result()
         coff = np.zeros(len(offsets), np.int32)
-        self._check(lib().gpdb_detect_batch(self.h, _p(offsets), _p(sidx), C.byref(res), _p(coff)))
+        self._check(fn(self.h, _p(offsets), _p(sidx), C.byref(res), _p(coff)))
         S, Cc = self.params.image_size, self.params.image_num_channels
         out = abi.result_to_numpy(res, S * S * Cc)
         lib().gpdb_free_result(C.byref(res))
         return split_batch_result(out, offsets, coff)
+
+    def detect_batch(self, sample_lists):
+        """gpdb_detect_batch: one list of cloud-local sample indices per installed cloud; returns one result dict per
+        cloud (views of the single batch result), each as detect() would return for that cloud alone."""
+        return self._batch_result(lib().gpdb_detect_batch, sample_lists)
+
+    def hand_search_batch(self, sample_lists):
+        """gpdb_hand_search_batch: hand_search() of every installed cloud in one call (no images, NaN scores, no weights
+        needed); returns one result dict per cloud, as detect_batch does."""
+        return self._batch_result(lib().gpdb_hand_search_batch, sample_lists)
+
+    def set_clouds_samples(self, positions):
+        """gpdb_set_clouds_samples: Cloud::setSamples for every installed cloud (one [m_b, 3] float64 array per cloud,
+        m_b may be 0); returns per cloud the cloud-local sample indices N_b .. N_b + m_b - 1 that address them."""
+        if len(positions) != self._n_clouds:
+            raise ValueError(f"{len(positions)} position arrays for a batch of {self._n_clouds} clouds (one per cloud)")
+        arrs = [np.asarray(p, dtype=np.float64).reshape(-1, 3) for p in positions]
+        poff = np.zeros(len(arrs) + 1, np.int32)
+        poff[1:] = np.cumsum([len(a) for a in arrs])
+        sm = np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros((0, 3)))
+        self._check(lib().gpdb_set_clouds_samples(self.h, _p(poff), _p(sm)))
+        npts = np.diff(self._batch[0])
+        return [np.arange(npts[b], npts[b] + len(a), dtype=np.int32) for b, a in enumerate(arrs)]
+
+    def find_clusters_batch(self, groups, min_inliers):
+        """gpdb_find_clusters_batch: find_clusters() on every group of hands (list of abi.POSE_DTYPE arrays) in one call;
+        returns one cluster array per group."""
+        arrs = [np.asarray(g, dtype=abi.POSE_DTYPE).ravel() for g in groups]
+        hoff = np.zeros(len(arrs) + 1, np.int32)
+        hoff[1:] = np.cumsum([len(a) for a in arrs])
+        hands = np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros(0, abi.POSE_DTYPE))
+        out = np.zeros(len(hands), dtype=abi.POSE_DTYPE)
+        coff = np.zeros(len(arrs) + 1, np.int32)
+        self._check(lib().gpdb_find_clusters_batch(self.h, len(arrs), _p(hoff), _p(hands), int(min_inliers), _p(out), _p(coff)))
+        return [out[coff[g]:coff[g + 1]].copy() for g in range(len(arrs))]
 
     def detect_batch_select(self, sample_lists, num_selected):
         """gpdb_detect_batch_select: the num_selected best candidates of every cloud; returns one record array per cloud."""

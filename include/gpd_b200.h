@@ -230,8 +230,9 @@ int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n_s
  * Every cloud gets its own neighbour grid on the device; the batch is held beside the single cloud, and gpdb_set_cloud,
  * gpdb_preprocess, gpdb_detect and every other entry point behave as before whatever batch is installed. Empty clouds,
  * K_b outside 1..8, non-finite coordinates and malformed offsets are GPDB_ERR_INVALID; a failed call leaves no batch.
- * Returns B. Sample positions (gpdb_set_samples) do not apply to a batch: called while only a batch is installed,
- * gpdb_set_samples is GPDB_ERR_INVALID. Raw views are preprocessed into a batch by gpdb_preprocess_clouds. */
+ * Returns B. gpdb_set_samples addresses the single cloud only: called while only a batch is installed, it is
+ * GPDB_ERR_INVALID (a batch takes its positions from gpdb_set_clouds_samples). Raw views are preprocessed into a batch by
+ * gpdb_preprocess_clouds. */
 int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points);
 
@@ -252,6 +253,22 @@ int gpdb_detect_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_
  * candidates of all clouds. */
 int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, int32_t num_selected,
                              gpdb_result *out, int32_t *sel_offsets_out);
+
+/* Cloud::setSamples for every cloud of the installed batch (SequentialImportanceSampling over many views): cloud b owns
+ * the columns pos_offsets[b] .. pos_offsets[b+1]-1 of samples_xyz (3 x M float64, column-major, as gpdb_set_samples;
+ * pos_offsets has B + 1 entries, starts at 0 and never decreases; an empty range is allowed). In gpdb_detect_batch,
+ * gpdb_detect_batch_select and gpdb_hand_search_batch the local index N_b + j then addresses position j of cloud b
+ * (indices below N_b keep addressing points), and each cloud's results equal gpdb_set_cloud + gpdb_set_samples + the
+ * single-cloud call on that cloud, bit for bit (shadow draws are seeded by the cloud-local index). Each call replaces all
+ * positions; a failed call, and any gpdb_set_clouds / gpdb_preprocess_clouds, successful or not, leaves none. The single
+ * cloud's positions (gpdb_set_samples) and these never touch each other. Returns M; GPDB_ERR_STATE when no batch is
+ * installed, GPDB_ERR_INVALID for malformed offsets. */
+int gpdb_set_clouds_samples(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *samples_xyz);
+
+/* gpdb_hand_search over every cloud of the batch in ONE call: inputs and output layout of gpdb_detect_batch (cloud b's
+ * candidates at cand_offsets_out[b] .. cand_offsets_out[b+1] - 1), no images, pose_scores NaN. Needs no weights. */
+int gpdb_hand_search_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out,
+                           int32_t *cand_offsets_out);
 
 /* Run all work of this context on an existing CUDA stream (cudaStream_t passed as void*), e.g. the
  * host framework's current stream, instead of the context's own stream. */
@@ -374,6 +391,15 @@ int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n_hands, int32_t *l
  * the clusters in the order of their seed hands (position = mean inlier position, score = lower 99 % confidence bound).
  * Returns the number of clusters. */
 int gpdb_find_clusters(gpdb_ctx *ctx, const gpdb_pose *hands, int32_t n_hands, int32_t min_inliers, gpdb_pose *clusters_out);
+
+/* gpdb_find_clusters on each of n_groups groups of hands independently, in one call (step 6 of detectGrasps over a batch
+ * of clouds): group g is hands[hand_offsets[g] .. hand_offsets[g+1]) (hand_offsets: n_groups + 1 entries starting at 0,
+ * never decreasing; an empty group is allowed). Group g's clusters are clusters_out[cluster_offsets_out[g] ..
+ * cluster_offsets_out[g+1]) (cluster_offsets_out: n_groups + 1 entries), in seed-hand order, bit-equal to
+ * gpdb_find_clusters on that group alone; clusters_out has room for hand_offsets[n_groups] records. Needs no cloud.
+ * Returns the number of clusters of all groups. */
+int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *hands,
+                             int32_t min_inliers, gpdb_pose *clusters_out, int32_t *cluster_offsets_out);
 
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory

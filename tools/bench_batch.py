@@ -15,7 +15,21 @@ parameters, 500 samples per view (fewer when a view keeps fewer points), and tim
 with the preprocessing alone of (a) and (c) and the device stage times of (c)'s gpdb_preprocess_clouds
 (gpdb_preprocess_timings). It checks once, outside the timed region, that (a) and (c) give identical flags and scores.
 
-    python tools/bench_batch.py [--sizes 1 16 64 256] [--reps 3] [--raw]
+--sis times cem_detect_grasps' device steps over B processed views (synthetic_raw_scene(1000 + i, n_points=20000) after
+default preprocessing) with the default SIS parameters: 50 initial samples, 5 rounds of 50 positions, the final
+classification at every position that carried a hand and the clustering (min_inliers 1). The per-view loop of
+single-cloud calls (gpdb_set_cloud, gpdb_hand_search, gpdb_set_samples + gpdb_hand_search per round, gpdb_set_samples +
+gpdb_detect, gpdb_find_clusters) runs against one batch call per step (gpdb_set_clouds, gpdb_hand_search_batch,
+gpdb_set_clouds_samples + gpdb_hand_search_batch per round, gpdb_set_clouds_samples + gpdb_detect_batch,
+gpdb_find_clusters_batch), both through lib.py. The round positions come from one seeded numpy generator (Gaussians around
+the initial hand-set positions and uniform cloud points) and are shared by both routes, so the timing measures the device
+path and not a host RNG. --detect-full times detectGrasps from raw views: preprocessing, the selection of the 100 best
+candidates at 500 samples per view and their clustering, looped (gpdb_preprocess, gpdb_detect_select, gpdb_find_clusters)
+against batched (gpdb_preprocess_clouds, gpdb_detect_batch_select, gpdb_find_clusters_batch). Both modes check once,
+outside the timed region, that the two routes return identical records, and print per step the median wall time of each
+route and the samples/s of the whole route.
+
+    python tools/bench_batch.py [--sizes 1 16 64 256] [--reps 3] [--raw | --sis | --detect-full]
 """
 import argparse
 import ctypes as C
@@ -172,13 +186,163 @@ def main_raw(a, ctx, gpu):
                           "gpu": gpu}), flush=True)
 
 
+SIS_INIT, SIS_ROUNDS, SIS_PER_ROUND, SIS_SIGMA, MIN_INLIERS, NUM_SELECTED = 50, 5, 50, 0.02, 1, 100
+
+
+class Steps:
+    """Wall time per named step (each step ends in a call that returns host results, i.e. after a device synchronise)."""
+
+    def __init__(self):
+        self.t = {}
+        self.t0 = time.perf_counter()
+
+    def __call__(self, name):
+        now = time.perf_counter()
+        self.t[name] = self.t.get(name, 0.0) + now - self.t0
+        self.t0 = now
+
+
+def hand_set_positions(view):
+    """Positions of the samples that carried at least one hand (candidates are in sample-slot order)."""
+    c = view["candidates"]
+    _, first = np.unique(c["sample_slot"], return_index=True)
+    return c["sample"][first].astype(np.float64)
+
+
+def sis_loop(ctx, clouds, init, rounds):
+    st, kept, out = Steps(), [], []
+    for b, c in enumerate(clouds):
+        ctx.set_cloud(c["xyz"], c["normals"], c["cam_source"], c["view_points"])
+        st("install")
+        k = [hand_set_positions(ctx.hand_search(init[b]))]
+        st("init_search")
+        for r in rounds:
+            k.append(hand_set_positions(ctx.hand_search(ctx.set_samples(r[b]))))
+            st("rounds")
+        kept.append(np.concatenate(k))
+        det = ctx.detect(ctx.set_samples(kept[-1]))["candidates"]
+        st("classify")
+        out.append((det, ctx.find_clusters(det, MIN_INLIERS)))
+        st("cluster")
+    return st.t, sum(len(k) for k in kept), out
+
+
+def sis_batch(ctx, clouds, init, rounds):
+    st = Steps()
+    ctx.set_clouds(clouds)
+    st("install")
+    kept = [[hand_set_positions(v)] for v in ctx.hand_search_batch(init)]
+    st("init_search")
+    for r in rounds:
+        for k, v in zip(kept, ctx.hand_search_batch(ctx.set_clouds_samples(r))):
+            k.append(hand_set_positions(v))
+        st("rounds")
+    kept = [np.concatenate(k) for k in kept]
+    det = [v["candidates"] for v in ctx.detect_batch(ctx.set_clouds_samples(kept))]
+    st("classify")
+    clusters = ctx.find_clusters_batch(det, MIN_INLIERS)
+    st("cluster")
+    return st.t, sum(len(k) for k in kept), list(zip(det, clusters))
+
+
+def full_loop(ctx, views, pp, samples):
+    st, out = Steps(), []
+    for v, s in zip(views, samples):
+        ctx.preprocess(v["xyz"], v["cam_source"], v["view_points"], pp, read_back=False)
+        st("preprocess")
+        sel = ctx.detect_select(s, NUM_SELECTED)["candidates"]
+        st("select")
+        out.append((sel, ctx.find_clusters(sel, MIN_INLIERS)))
+        st("cluster")
+    return st.t, 0, out
+
+
+def full_batch(ctx, views, pp, samples):
+    st = Steps()
+    ctx.preprocess_clouds(views, pp, read_back=False)
+    st("preprocess")
+    sel = ctx.detect_batch_select(samples, NUM_SELECTED)
+    st("select")
+    clusters = ctx.find_clusters_batch(sel, MIN_INLIERS)
+    st("cluster")
+    return st.t, 0, list(zip(sel, clusters))
+
+
+def same_records(ra, rb):
+    return len(ra) == len(rb) and all(x.tobytes() == y.tobytes() for a, b in zip(ra, rb) for x, y in zip(a, b))
+
+
+def main_steps(a, ctx, gpu):
+    """--sis / --detect-full: the per-view loop against one batch call per step."""
+    pp = lib.preprocess_params()
+    pool = []
+    for i in range(max(a.sizes)):
+        s = scenes.synthetic_raw_scene(1000 + i, n_points=N_POINTS)
+        pool.append({"xyz": s["xyz"], "cam_source": s["cam_source"], "view_points": s["view_points"]})
+    med = lambda v: float(np.median(v))  # noqa: E731
+    for B in a.sizes:
+        views = pool[:B]
+        clouds = ctx.preprocess_clouds(views, pp)
+        n = [len(c["xyz"]) for c in clouds]
+        rng = np.random.default_rng(B)
+        if a.sis:
+            init = [rng.choice(nb, min(SIS_INIT, nb), replace=False).astype(np.int32) for nb in n]
+            # round positions of every view from one generator, shared by both routes: Gaussians around the initial
+            # hand-set positions (70 %) and cloud points (30 %), as the default prob_rand_samples = 0.3 mixes them
+            ctx.set_clouds(clouds)
+            start = [hand_set_positions(v) for v in ctx.hand_search_batch(init)]
+            rounds = []
+            for _ in range(SIS_ROUNDS):
+                r = []
+                for c, s0 in zip(clouds, start):
+                    ng = SIS_PER_ROUND - int(0.3 * SIS_PER_ROUND)
+                    centre = s0[rng.integers(0, len(s0), ng)] if len(s0) else c["xyz"][rng.integers(0, len(c["xyz"]), ng)]
+                    pts = c["xyz"][rng.integers(0, len(c["xyz"]), SIS_PER_ROUND - ng)].astype(np.float64)
+                    r.append(np.vstack([centre + rng.normal(0.0, SIS_SIGMA, centre.shape), pts]))
+                rounds.append(r)
+            loop, batch, args = sis_loop, sis_batch, (clouds, init, rounds)
+            n_search = sum(len(i) for i in init) + SIS_ROUNDS * SIS_PER_ROUND * B
+        else:
+            samples = [rng.choice(nb, min(N_SAMPLES, nb), replace=False).astype(np.int32) for nb in n]
+            loop, batch, args = full_loop, full_batch, (views, pp, samples)
+            n_search = sum(len(s) for s in samples)
+        # warm-up of every shape, and the one check that both routes return the same records
+        _, kl, rl = loop(ctx, *args)
+        _, kb, rb = batch(ctx, *args)
+        assert kl == kb and same_records(rl, rb), "the loop and the batch route differ"
+        tl, tb = [], []
+        for _ in range(a.reps):
+            tl.append(loop(ctx, *args)[0])
+            tb.append(batch(ctx, *args)[0])
+        n_total = n_search + kl  # hand-search samples + classified positions (--sis)
+        steps = list(tl[0])
+        line = {"mode": "sis" if a.sis else "detect_full", "B": B, "processed_points": int(sum(n)), "samples": n_total,
+                "loop_ms": round(1e3 * med([sum(t.values()) for t in tl]), 2),
+                "batch_ms": round(1e3 * med([sum(t.values()) for t in tb]), 2),
+                "loop_sps": round(n_total / med([sum(t.values()) for t in tl])),
+                "batch_sps": round(n_total / med([sum(t.values()) for t in tb])),
+                "loop_steps_ms": {s: round(1e3 * med([t[s] for t in tl]), 2) for s in steps},
+                "batch_steps_ms": {s: round(1e3 * med([t[s] for t in tb]), 2) for s in steps},
+                "clusters": int(sum(len(c) for _, c in rb)), "gpu": gpu}
+        print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--sizes", type=int, nargs="+", default=[1, 16, 64, 256])
     ap.add_argument("--reps", type=int, default=3)
-    ap.add_argument("--raw", action="store_true", help="start from raw views: three preprocessing + detection routes")
+    mode = ap.add_mutually_exclusive_group()
+    mode.add_argument("--raw", action="store_true", help="start from raw views: three preprocessing + detection routes")
+    mode.add_argument("--sis", action="store_true", help="cem_detect_grasps' steps: per-view loop against batch calls")
+    mode.add_argument("--detect-full", action="store_true", help="detectGrasps from raw views: loop against batch calls")
     a = ap.parse_args()
     w, relu = weights()
+    if a.sis or a.detect_full:
+        ctx = lib.Context(lib.default_params(channels=15, relu_after_conv=relu))
+        ctx.set_weights(w)
+        main_steps(a, ctx, gpu_info())
+        ctx.close()
+        return
     if a.raw:
         ctx = lib.Context(lib.default_params(channels=15, relu_after_conv=relu))
         ctx.set_weights(w)
