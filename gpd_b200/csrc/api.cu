@@ -388,7 +388,7 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->tc.b1);
   cudaFree(ctx->tc.b2);
   cudaFree(ctx->tc.b3);
-  for (int i = 0; i < 24; i++) cudaFree(ctx->scratch[i]);
+  for (int i = 0; i < 25; i++) cudaFree(ctx->scratch[i]);
   for (int i = 0; i < 8; i++)
     if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
   if (ctx->stream && ctx->own_stream) cudaStreamDestroy(ctx->stream);
@@ -515,19 +515,27 @@ static unsigned pack_rows(const int32_t *rows, int nb, int K, uint8_t *dst, Seen
   return seen_by_all;
 }
 
-int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
-                      const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
-                      CloudDesc *desc) {
-  const int32_t *rows = cam_source;  // cloud b's N_b x K_b block
-  size_t vs = 0;                     // running offset into view_points (3 x K_b blocks)
+// the camera fields of B descriptors: K_b and the 3 x K_b view point blocks, one after the other; the rest zeroed
+static void camera_descs(int B, const int32_t *n_cameras, const double *view_points, CloudDesc *desc) {
+  size_t vs = 0;  // running offset into view_points
   for (int b = 0; b < B; b++) {
     CloudDesc &D = desc[b];
     memset(&D, 0, sizeof(D));
-    const int K = n_cameras[b];  // locals, not D's fields: the byte stores to cam below may alias anything
-    D.K = K;
-    for (int k = 0; k < K; k++)
+    D.K = n_cameras[b];
+    for (int k = 0; k < D.K; k++)
       for (int r = 0; r < 3; r++) D.vp[k][r] = view_points[vs + 3 * k + r];
-    vs += 3 * (size_t)K;
+    vs += 3 * (size_t)D.K;
+  }
+}
+
+int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
+                      const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
+                      CloudDesc *desc) {
+  camera_descs(B, n_cameras, view_points, desc);
+  const int32_t *rows = cam_source;  // cloud b's N_b x K_b block
+  for (int b = 0; b < B; b++) {
+    CloudDesc &D = desc[b];
+    const int K = n_cameras[b];  // a local, not D's field: the byte stores to cam below may alias anything
     const unsigned all = (1u << K) - 1;
     const int nb = off[b + 1] - off[b];
     uint8_t *dst = cam + off[b];
@@ -548,6 +556,78 @@ int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off
     if (rows) rows += (size_t)nb * K;
     D.all_seen = (seen_by_all & all) == all ? 1 : 0;
   }
+  return GPDB_OK;
+}
+
+// ---- the device-resident entry points (gpdb_*_device): bulk arrays in device memory, sizes and offsets on the host ----
+
+static const unsigned long long NO_BAD = ~0ull;  // the check word of scratch slot 24 when no position offends
+
+// every non-null pointer must be device (or managed) memory of the context's device; runs before any device work
+static int check_device_ptrs(gpdb_ctx *ctx, const char *name, int n, const char *const *names, const void *const *ptrs) {
+  for (int i = 0; i < n; i++) {
+    if (!ptrs[i]) continue;
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, ptrs[i]);
+    if (e != cudaSuccess) cudaGetLastError();
+    if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ctx->device) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s is not device memory of device %d", name, names[i], ctx->device);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  return GPDB_OK;
+}
+
+// reads the check word *d_bad after the work queued before it (stream synchronised)
+static int read_check(gpdb_ctx *ctx, const unsigned long long *d_bad, unsigned long long *bad) {
+  CUDA_TRY(cudaMemcpyAsync(bad, d_bad, sizeof(*bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return GPDB_OK;
+}
+
+// gpdb_pack_cameras with cam_source (d_rows) and cam (d_cam) in device memory: the masks and each cloud's all_seen are
+// computed by batch_pack_cameras, the descriptors' camera fields on the host; same rules, same error
+static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *d_rows,
+                               const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01,
+                               uint8_t *d_cam, CloudDesc *desc) {
+  camera_descs(B, n_cameras, view_points, desc);
+  // slot 24: check word, element offsets of the cam_source blocks [B+1], point offsets [B+1], K_b [B], all_seen [B]
+  const size_t bytes = sizeof(long long) * ((size_t)B + 2) + sizeof(int) * (3 * (size_t)B + 1);
+  std::vector<unsigned char> h(bytes);
+  unsigned long long *h_bad = (unsigned long long *)h.data();
+  long long *h_roff = (long long *)(h_bad + 1);
+  int *h_off = (int *)(h_roff + B + 1), *h_k = h_off + B + 1, *h_all = h_k + B;
+  *h_bad = NO_BAD;
+  h_roff[0] = 0;
+  for (int b = 0; b < B; b++) {
+    h_roff[b + 1] = h_roff[b] + (long long)(off[b + 1] - off[b]) * n_cameras[b];
+    h_k[b] = n_cameras[b];
+    h_all[b] = 1;
+  }
+  memcpy(h_off, off, sizeof(int) * ((size_t)B + 1));
+  unsigned char *d = (unsigned char *)gpdb_scratch(ctx, 24, bytes);
+  if (!d) return GPDB_ERR_CUDA;
+  unsigned long long *d_bad = (unsigned long long *)d;
+  long long *d_roff = (long long *)(d_bad + 1);
+  int *d_off = (int *)(d_roff + B + 1), *d_k = d_off + B + 1, *d_all = d_k + B;
+  CUDA_TRY(cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+  int rc = batch_pack_cameras(ctx, d_rows, d_off, d_roff, d_k, B, off[B], eq1, strict01, d_cam, d_all, d_bad);
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaMemcpyAsync(h_all, d_all, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  unsigned long long e;
+  if ((rc = read_check(ctx, d_bad, &e)) != GPDB_OK) return rc;
+  if (e != NO_BAD) {
+    int b = 0;
+    while ((unsigned long long)h_roff[b + 1] <= e) b++;
+    int32_t v = 0;
+    CUDA_TRY(cudaMemcpyAsync(&v, d_rows + e, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    const long long r = (long long)e - h_roff[b];
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must be 0 or "
+                   "1", name, b, (int)(r / n_cameras[b]), (int)(r % n_cameras[b]), (int)v);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++) desc[b].all_seen = h_all[b];
   return GPDB_OK;
 }
 
@@ -578,36 +658,83 @@ static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t n_cl
   return rc == GPDB_OK ? n_clouds : rc;
 }
 
+// set_clouds from the caller's device arrays: the finiteness check and the camera masks run on the device, the points and
+// normals are copied device to device into the store
+static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *point_offsets,
+                             const float *d_xyz, const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
+                             const double *view_points) {
+  const int N = point_offsets[B];
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  unsigned long long *d_bad = (unsigned long long *)gpdb_scratch(ctx, 24, sizeof(unsigned long long));
+  if (!d_bad) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
+  int rc = batch_first_nonfinite(ctx, d_xyz, 3 * (long long)N, d_bad);
+  unsigned long long bad = NO_BAD;
+  if (rc == GPDB_OK) rc = read_check(ctx, d_bad, &bad);
+  if (rc != GPDB_OK) return rc;
+  if (bad != NO_BAD) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess "
+                   "first)", name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  std::vector<CloudDesc> desc((size_t)B);
+  rc = gpdb_cloud_reserve(ctx, s, (size_t)N, B);
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.xyz, d_xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.nrm, d_normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyDeviceToDevice, ctx->stream));
+  rc = pack_cameras_device(ctx, name, B, point_offsets, d_cam_source, n_cameras, view_points, false, false, s.cam, desc.data());
+  if (rc == GPDB_OK) rc = gpdb_install_clouds(ctx, s, desc.data(), point_offsets, B, true);
+  return rc == GPDB_OK ? B : rc;
+}
+
 // gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); the caller drops
-// the store when this fails
+// the store when this fails. device: xyz, normals and cam_source are the caller's device arrays (read in place, the
+// camera masks packed on the device), else host arrays uploaded here.
 static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *roff, const float *xyz,
                              const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
                              const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff,
-                             cudaEvent_t ev[6]) {
+                             cudaEvent_t ev[6], bool device) {
   const int M = roff[B];
   // ---- camera masks, packed per cloud with its own K_b. A camera sees a point when its entry is exactly 1: the
   // reference's voxelisation keeps only those entries (cloud.cpp:327) and its normal estimation and reverseNormals test
   // == 1 (cloud.cpp:581,611). Without voxelisation the reference keeps the raw values, which its normals read as == 1 and
   // the grasp path as >= 1; one bit cannot hold both, so other values are rejected there.
-  std::vector<uint8_t> cam((size_t)M);
   std::vector<CloudDesc> desc((size_t)B);
-  int rc = gpdb_pack_cameras(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, cam.data(),
+  const float *d_xyz_raw = xyz;
+  const double *d_nrm_raw = normals;
+  uint8_t *d_cam_raw = nullptr;
+  std::vector<uint8_t> cam;
+  int rc;
+  if (device) {
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    d_cam_raw = (uint8_t *)gpdb_scratch(ctx, 7, (size_t)M + 16);
+    if (!d_cam_raw) return GPDB_ERR_CUDA;
+    cudaEventRecord(ev[0], ctx->stream);
+    rc = pack_cameras_device(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, d_cam_raw,
                              desc.data());
-  if (rc != GPDB_OK) return rc;
+    if (rc != GPDB_OK) return rc;
+  } else {
+    cam.resize((size_t)M);
+    rc = gpdb_pack_cameras(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, cam.data(),
+                           desc.data());
+    if (rc != GPDB_OK) return rc;
+    CUDA_TRY(cudaSetDevice(ctx->device));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    // ---- one upload of the concatenated raw arrays
+    const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
+    unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, 7, raw_bytes);
+    if (!raw) return GPDB_ERR_CUDA;
+    double *nrm_up = normals ? (double *)raw : nullptr;
+    float *xyz_up = (float *)(raw + (normals ? sizeof(double) * 3 * (size_t)M : 0));
+    d_cam_raw = (uint8_t *)(xyz_up + 3 * (size_t)M);
+    cudaEventRecord(ev[0], ctx->stream);
+    CUDA_TRY(cudaMemcpyAsync(xyz_up, xyz, sizeof(float) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(d_cam_raw, cam.data(), (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+    if (normals) CUDA_TRY(cudaMemcpyAsync(nrm_up, normals, sizeof(double) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
+    d_xyz_raw = xyz_up;
+    d_nrm_raw = nrm_up;
+  }
   for (CloudDesc &D : desc) D.all_seen = cam_source ? 0 : 1;  // without a camera-source matrix every camera sees every point
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  // ---- one upload of the concatenated raw arrays
-  const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
-  unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, 7, raw_bytes);
-  if (!raw) return GPDB_ERR_CUDA;
-  double *d_nrm_raw = normals ? (double *)raw : nullptr;
-  float *d_xyz_raw = (float *)(raw + (normals ? sizeof(double) * 3 * (size_t)M : 0));
-  uint8_t *d_cam_raw = (uint8_t *)(d_xyz_raw + 3 * (size_t)M);
-  cudaEventRecord(ev[0], ctx->stream);
-  CUDA_TRY(cudaMemcpyAsync(d_xyz_raw, xyz, sizeof(float) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(d_cam_raw, cam.data(), (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
-  if (normals) CUDA_TRY(cudaMemcpyAsync(d_nrm_raw, normals, sizeof(double) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
   cudaEventRecord(ev[1], ctx->stream);
   // ---- removeNans + filterWorkspace + voxelizeCloud of every cloud, into the store's arenas
   rc = pre_filter_voxelize_batch(ctx, s, d_xyz_raw, d_cam_raw, d_nrm_raw, M, B, roff, *pp, poff, ev[2]);
@@ -640,12 +767,14 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
 // preprocess_clouds, and a failed call leaves no cloud in s
 static int preprocess_into(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *roff, const float *xyz,
                            const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
-                           const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff) {
+                           const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff,
+                           bool device = false) {
   s.n = 0;
   s.has_src = false;
   cudaEvent_t ev[6] = {};
   for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
-  const int rc = preprocess_clouds(ctx, s, name, B, roff, xyz, normals, cam_source, n_cameras, view_points, pp, poff, ev);
+  const int rc =
+      preprocess_clouds(ctx, s, name, B, roff, xyz, normals, cam_source, n_cameras, view_points, pp, poff, ev, device);
   for (auto &e : ev) cudaEventDestroy(e);
   if (rc < 0) {
     s.n = 0;
@@ -970,7 +1099,9 @@ int check_device_errors(gpdb_ctx *ctx) {
 // The chunked device pipeline behind gpdb_detect / gpdb_hand_search / gpdb_detect_resident / gpdb_detect_sharded.
 //   resident == false: sample_idx is a HOST array, every result is copied back to the host (out)
 //   resident == true : sample_idx, flags_ext, scores_ext are DEVICE arrays; nothing but the per-chunk
-//                      candidate count crosses PCIe (out receives counts and timings only)
+//                      candidate count crosses PCIe (out receives counts and timings only). A resident batch call
+//                      (gpdb_detect_batch_select_device) keeps flags and scores in scratch and writes its selection
+//                      to sel_out.
 // select_k >= 0 (gpdb_detect_select): the classified candidates of all chunks stay on the device, the select_k best are
 // sorted out there and only they are copied back; no per-sample / per-pose array is returned.
 //
@@ -981,9 +1112,10 @@ int check_device_errors(gpdb_ctx *ctx) {
 // chunk i go to the pinned arena while chunk i+1 computes.
 int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int32_t n, gpdb_result *out,
                       bool with_images_and_scores, bool resident, uint8_t *flags_ext, float *scores_ext, int select_k,
-                      int slot_base) {
+                      int slot_base, gpdb_pose *sel_out) {
   const bool selecting = select_k >= 0;
   const bool batch = &s == &ctx->many;  // run_batch has checked the samples against the clouds
+  const bool ext = resident && !batch;  // per-pose flags and scores in the caller's device arrays
   memset(out, 0, sizeof(*out));
   PipeState &ps = *ctx->pipe;
   const int P = ctx->hp.P, S = ctx->hp.S, C = ctx->hp.C;
@@ -1006,11 +1138,11 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
   const bool to_host = !resident && !selecting;  // per-sample / per-pose arrays + all candidate records go to the host
   const size_t nP = (size_t)n * P;
   const int cmax = std::min(chunk, std::max(n, 1));
-  int *d_sidx = resident ? const_cast<int *>(sample_idx) : (int *)gpdb_scratch(ctx, 7, sizeof(int) * (size_t)n);
+  int *d_sidx = resident && sample_idx ? const_cast<int *>(sample_idx) : (int *)gpdb_scratch(ctx, 7, sizeof(int) * (size_t)n);
   double *d_frames = (double *)gpdb_scratch(ctx, 8, sizeof(double) * 9 * (size_t)n);
   uint8_t *d_valid = (uint8_t *)gpdb_scratch(ctx, 9, (size_t)n);
-  uint8_t *d_flags = resident ? flags_ext : (uint8_t *)gpdb_scratch(ctx, 10, nP);
-  float *d_pscores = resident ? scores_ext : (float *)gpdb_scratch(ctx, 11, sizeof(float) * nP);
+  uint8_t *d_flags = ext ? flags_ext : (uint8_t *)gpdb_scratch(ctx, 10, nP);
+  float *d_pscores = ext ? scores_ext : (float *)gpdb_scratch(ctx, 11, sizeof(float) * nP);
   gpdb_pose *d_poses = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)cmax * P);
   gpdb_pose *d_cand2 = (gpdb_pose *)gpdb_scratch(ctx, 13, 2 * sizeof(gpdb_pose) * (size_t)cmax * P);  // double-buffered
   int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
@@ -1202,7 +1334,9 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
     rc = geo_select_batch(ctx, s, ctx->d_sel, total_nc, select_k, &d_top);
     if (rc < 0) return finish(rc);
     n_sel = rc;
-    if (n_sel > 0) {
+    // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
+    PIPE_TRY(batch_local_slots(ctx, d_top, n_sel, s.soff, s.n, resident ? sel_out : d_top));
+    if (n_sel > 0 && !resident) {
       PIPE_CUDA(cudaStreamSynchronize(ps.copy));
       if (!arena_reserve(ar, 1, sizeof(gpdb_pose) * (size_t)n_sel, 0)) {
         gpdb_set_error(ctx, GPDB_ERR_CUDA, "cudaHostAlloc of the candidate arena failed");
@@ -1284,30 +1418,77 @@ int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n, 
   return run_pipeline(ctx, d_sample_idx, n, stats, true, true, d_flags_out, d_scores_out);
 }
 
+}  // extern "C"
+
+// the argument checks of gpdb_set_clouds[_device] after ctx (the caller has dropped the batch); `raw`: those of
+// gpdb_preprocess_clouds[_device]
+static int check_clouds_args(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
+                             const double *normals, const int32_t *n_cameras, const double *view_points,
+                             const gpdb_preprocess_params *pp, const int32_t *processed_offsets_out, bool raw) {
+  if (raw ? (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || !pp || !processed_offsets_out ||
+             point_offsets[0] != 0)
+          : (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !normals || !view_points || point_offsets[0] != 0)) {
+    if (raw)
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, "
+                     "view_points, params, processed_offsets_out", name);
+    else
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, normals, "
+                     "view_points", name);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < n_clouds; b++) {
+    if (point_offsets[b + 1] <= point_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d has %d points (offsets must increase)", name, raw ? "raw cloud" : "cloud",
+                     b, point_offsets[b + 1] - point_offsets[b]);
+      return GPDB_ERR_INVALID;
+    }
+    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d has %d cameras (1 <= cameras <= %d)", name, b, n_cameras[b],
+                     GPDB_MAX_CAMERAS);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  if (!raw) return GPDB_OK;
+  if (!pp->estimate_normals && !normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals = 0 needs the caller's normals", name);
+    return GPDB_ERR_INVALID;
+  }
+  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: voxel_size and normals_radius must be positive", name);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+extern "C" {
+
 int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is untouched either way
   ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
-  if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !normals || !view_points || point_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, "
-                   "normals, view_points");
-    return GPDB_ERR_INVALID;
-  }
-  for (int b = 0; b < n_clouds; b++) {
-    if (point_offsets[b + 1] <= point_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: cloud %d has %d points (offsets must increase)", b,
-                     point_offsets[b + 1] - point_offsets[b]);
-      return GPDB_ERR_INVALID;
-    }
-    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds: cloud %d has %d cameras (1 <= cameras <= %d)", b, n_cameras[b],
-                     GPDB_MAX_CAMERAS);
-      return GPDB_ERR_INVALID;
-    }
-  }
-  return set_clouds(ctx, ctx->many, "gpdb_set_clouds", n_clouds, point_offsets, xyz, normals, cam_source, n_cameras,
-                    view_points);
+  const char *name = "gpdb_set_clouds";
+  const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, nullptr, nullptr,
+                                   false);
+  if (rc != GPDB_OK) return rc;
+  return set_clouds(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
+}
+
+int gpdb_set_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
+                           const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
+                           const double *view_points) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  ctx->many.n = 0;
+  ctx->many.n_samples = 0;
+  const char *name = "gpdb_set_clouds_device";
+  int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, d_xyz, d_normals, n_cameras, view_points, nullptr, nullptr,
+                             false);
+  const char *names[3] = {"d_xyz", "d_normals", "d_cam_source"};
+  const void *ptrs[3] = {d_xyz, d_normals, d_cam_source};
+  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 3, names, ptrs);
+  if (rc != GPDB_OK) return rc;
+  return set_clouds_device(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
+                           view_points);
 }
 
 int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
@@ -1317,34 +1498,31 @@ int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
   ctx->many.has_src = false;
   ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
-  if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || !pp || !processed_offsets_out ||
-      point_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: need n_clouds > 0, point_offsets (starting at 0), n_cameras, "
-                   "xyz, view_points, params, processed_offsets_out");
-    return GPDB_ERR_INVALID;
-  }
-  for (int b = 0; b < n_clouds; b++) {
-    if (point_offsets[b + 1] <= point_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: raw cloud %d has %d points (offsets must increase)", b,
-                     point_offsets[b + 1] - point_offsets[b]);
-      return GPDB_ERR_INVALID;
-    }
-    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: cloud %d has %d cameras (1 <= cameras <= %d)", b,
-                     n_cameras[b], GPDB_MAX_CAMERAS);
-      return GPDB_ERR_INVALID;
-    }
-  }
-  if (!pp->estimate_normals && !normals) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: estimate_normals = 0 needs the caller's normals");
-    return GPDB_ERR_INVALID;
-  }
-  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess_clouds: voxel_size and normals_radius must be positive");
-    return GPDB_ERR_INVALID;
-  }
-  return preprocess_into(ctx, ctx->many, "gpdb_preprocess_clouds", n_clouds, point_offsets, xyz, normals, cam_source,
-                         n_cameras, view_points, pp, processed_offsets_out);
+  const char *name = "gpdb_preprocess_clouds";
+  const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, pp,
+                                   processed_offsets_out, true);
+  if (rc != GPDB_OK) return rc;
+  return preprocess_into(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
+                         processed_offsets_out);
+}
+
+int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
+                                  const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
+                                  const double *view_points, const gpdb_preprocess_params *pp,
+                                  int32_t *processed_offsets_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  ctx->many.n = 0;
+  ctx->many.has_src = false;
+  ctx->many.n_samples = 0;
+  const char *name = "gpdb_preprocess_clouds_device";
+  int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, d_xyz, d_normals, n_cameras, view_points, pp,
+                             processed_offsets_out, true);
+  const char *names[3] = {"d_xyz", "d_normals", "d_cam_source"};
+  const void *ptrs[3] = {d_xyz, d_normals, d_cam_source};
+  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 3, names, ptrs);
+  if (rc != GPDB_OK) return rc;
+  return preprocess_into(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
+                         view_points, pp, processed_offsets_out, true);
 }
 
 int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out, int32_t *src_out) {
@@ -1367,9 +1545,10 @@ namespace {
 // gpdb_detect_batch / gpdb_detect_batch_select / gpdb_hand_search_batch: checks the CSR sample lists against the installed
 // batch and runs them as ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back
 // with cloud-local sample slots, grouped by cloud (offsets_out). Only the classifying calls (with_images_and_scores) need
-// weights.
+// weights. device (gpdb_detect_batch_select_device): sample_idx and sel_out are device arrays, the sample lists are checked
+// on the device and the selection stays there.
 int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out, int32_t *offsets_out,
-              bool with_images_and_scores, int select_k, const char *name) {
+              bool with_images_and_scores, int select_k, const char *name, bool device = false, gpdb_pose *sel_out = nullptr) {
   int rc = gpdb_check_state(ctx, false, with_images_and_scores);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
@@ -1392,26 +1571,55 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null sample_idx", name);
     return GPDB_ERR_INVALID;
   }
-  for (int b = 0; b < B; b++) {
-    const int nb = s.off[b + 1] - s.off[b], mb = s.positions(b);  // N_b points, then M_b positions
-    for (int i = sample_offsets[b]; i < sample_offsets[b + 1]; i++)
-      if (sample_idx[i] < 0 || sample_idx[i] >= nb + mb) {
-        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
-                       "positions)", name, sample_idx[i], i, b, nb, mb);
-        return GPDB_ERR_INVALID;
-      }
+  if (device) {
+    if (n > 0 && select_k > 0 && !sel_out) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_selected_out", name);
+      return GPDB_ERR_INVALID;
+    }
+    const char *names[2] = {"d_sample_idx", "d_selected_out"};
+    const void *ptrs[2] = {sample_idx, sel_out};
+    if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+  } else {
+    for (int b = 0; b < B; b++) {
+      const int nb = s.off[b + 1] - s.off[b], mb = s.positions(b);  // N_b points, then M_b positions
+      for (int i = sample_offsets[b]; i < sample_offsets[b + 1]; i++)
+        if (sample_idx[i] < 0 || sample_idx[i] >= nb + mb) {
+          gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
+                         "positions)", name, sample_idx[i], i, b, nb, mb);
+          return GPDB_ERR_INVALID;
+        }
+    }
   }
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  rc = gpdb_run_pipeline(ctx, s, sample_idx, n, out, with_images_and_scores, false, nullptr, nullptr, select_k, 0);
-  if (rc < 0) return rc;
-  // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
-  if (select_k >= 0) {
-    for (int b = 0; b < B; b++) {
-      offsets_out[b] = s.sel[b];
-      for (int j = s.sel[b]; j < s.sel[b + 1]; j++) out->candidates[j].sample_slot -= sample_offsets[b];
+  if (device && n > 0) {  // the same check on the device: the first offending position, then its cloud and value
+    unsigned char *d = (unsigned char *)gpdb_scratch(ctx, 24, sizeof(unsigned long long) + sizeof(int) * (size_t)B);
+    if (!d) return GPDB_ERR_CUDA;
+    unsigned long long *d_bad = (unsigned long long *)d;
+    int *d_lim = (int *)(d_bad + 1);
+    std::vector<int> lim((size_t)B);
+    for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b] + s.positions(b);
+    CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+    unsigned long long bad = NO_BAD;
+    rc = batch_check_samples(ctx, sample_idx, n, s.soff, B, d_lim, d_bad);
+    if (rc == GPDB_OK) rc = read_check(ctx, d_bad, &bad);
+    if (rc != GPDB_OK) return rc;
+    if (bad != NO_BAD) {
+      const int i = (int)bad;
+      int b = 0, v = 0;
+      while (sample_offsets[b + 1] <= i) b++;
+      CUDA_TRY(cudaMemcpyAsync(&v, sample_idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
+                     "positions)", name, v, i, b, s.off[b + 1] - s.off[b], s.positions(b));
+      return GPDB_ERR_INVALID;
     }
-    offsets_out[B] = s.sel[B];
-  } else {
+  }
+  rc = gpdb_run_pipeline(ctx, s, sample_idx, n, out, with_images_and_scores, device, nullptr, nullptr, select_k, 0, sel_out);
+  if (rc < 0) return rc;
+  if (select_k >= 0) {  // the pipeline has made the selected records' sample slots cloud-local
+    memcpy(offsets_out, s.sel, sizeof(int) * ((size_t)B + 1));
+  } else {  // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
     int b = 0;
     offsets_out[0] = 0;
     for (int j = 0; j < out->n_candidates; j++) {
@@ -1452,6 +1660,17 @@ int gpdb_detect_batch_select(gpdb_ctx *ctx, const int32_t *sample_offsets, const
     return GPDB_ERR_INVALID;
   }
   return run_batch(ctx, sample_offsets, sample_idx, out, sel_offsets_out, true, num_selected, "gpdb_detect_batch_select");
+}
+
+int gpdb_detect_batch_select_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx,
+                                    int32_t num_selected, gpdb_pose *d_selected_out, int32_t *sel_offsets_out,
+                                    gpdb_result *stats) {
+  if (ctx && (!sel_offsets_out || num_selected < 0)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch_select_device: need sel_offsets_out and num_selected >= 0");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, d_sample_idx, stats, sel_offsets_out, true, num_selected,
+                   "gpdb_detect_batch_select_device", true, d_selected_out);
 }
 
 int gpdb_set_overlap(gpdb_ctx *ctx, int32_t enable) {
@@ -1610,21 +1829,25 @@ int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_
 
 // gpdb_find_clusters_batch after the argument checks (gpdb_find_clusters: one group): the clusters of all G groups in one
 // k_clusters launch, compacted in hand order, so group g's are clusters_out[cluster_offsets_out[g] ..
-// cluster_offsets_out[g+1]); returns their total
+// cluster_offsets_out[g+1]); returns their total. device: hands and clusters_out are device arrays (no copy of the hands)
 static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
-                         gpdb_pose *clusters_out, int32_t *cluster_offsets_out) {
+                         gpdb_pose *clusters_out, int32_t *cluster_offsets_out, bool device = false) {
   const int n = hand_offsets[G];
   for (int g = 0; g <= G; g++) cluster_offsets_out[g] = 0;
   if (n == 0) return 0;
   CUDA_TRY(cudaSetDevice(ctx->device));
-  gpdb_pose *d_in = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n * 3);
+  gpdb_pose *d_dense = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n * (device ? 2 : 3));
   int *d_goff = (int *)gpdb_scratch(ctx, 18, sizeof(int) * (2 * (size_t)G + 1) + (size_t)n);
   int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
-  if (!d_in || !d_goff || !d_count) return GPDB_ERR_CUDA;
-  gpdb_pose *d_dense = d_in + n, *d_out = d_dense + n;
+  if (!d_dense || !d_goff || !d_count) return GPDB_ERR_CUDA;
+  gpdb_pose *d_out = d_dense + n;
   int *d_gcount = d_goff + G + 1;
   uint8_t *d_keep = (uint8_t *)(d_gcount + G);
-  CUDA_TRY(cudaMemcpyAsync(d_in, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  const gpdb_pose *d_in = hands;
+  if (!device) {
+    d_in = d_out + n;
+    CUDA_TRY(cudaMemcpyAsync(d_out + n, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  }
   CUDA_TRY(cudaMemcpyAsync(d_goff, hand_offsets, sizeof(int) * ((size_t)G + 1), cudaMemcpyHostToDevice, ctx->stream));
   int rc;
   if ((rc = geo_clusters(ctx, d_in, n, d_goff, G, min_inliers, d_dense, d_keep, d_gcount)) != GPDB_OK) return rc;
@@ -1635,7 +1858,8 @@ static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, cons
   for (int g = 0; g < G; g++) cluster_offsets_out[g + 1] += cluster_offsets_out[g];
   const int nc = cluster_offsets_out[G];
   if (nc > 0) {
-    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc,
+                             device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   }
   return nc;
@@ -1654,24 +1878,49 @@ int gpdb_find_clusters(gpdb_ctx *ctx, const gpdb_pose *hands, int32_t n, int32_t
   return find_clusters(ctx, 1, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets);
 }
 
-int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *hands,
-                             int32_t min_inliers, gpdb_pose *clusters_out, int32_t *cluster_offsets_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
+}  // extern "C"
+
+// the argument checks of gpdb_find_clusters_batch[_device]
+static int check_groups_args(gpdb_ctx *ctx, const char *name, int32_t n_groups, const int32_t *hand_offsets,
+                             const gpdb_pose *hands, const gpdb_pose *clusters_out, const int32_t *cluster_offsets_out) {
   if (n_groups < 0 || !hand_offsets || !cluster_offsets_out || hand_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: need n_groups >= 0, hand_offsets[n_groups + 1] starting "
-                   "at 0 and cluster_offsets_out");
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_groups >= 0, hand_offsets[n_groups + 1] starting at 0 and "
+                   "cluster_offsets_out", name);
     return GPDB_ERR_INVALID;
   }
   for (int g = 0; g < n_groups; g++)
     if (hand_offsets[g + 1] < hand_offsets[g]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: hand_offsets decrease at group %d", g);
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: hand_offsets decrease at group %d", name, g);
       return GPDB_ERR_INVALID;
     }
   if (hand_offsets[n_groups] > 0 && (!hands || !clusters_out)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_find_clusters_batch: null hands or clusters_out");
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null hands or clusters_out", name);
     return GPDB_ERR_INVALID;
   }
+  return GPDB_OK;
+}
+
+extern "C" {
+
+int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *hands,
+                             int32_t min_inliers, gpdb_pose *clusters_out, int32_t *cluster_offsets_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  const int rc = check_groups_args(ctx, "gpdb_find_clusters_batch", n_groups, hand_offsets, hands, clusters_out,
+                                   cluster_offsets_out);
+  if (rc != GPDB_OK) return rc;
   return find_clusters(ctx, n_groups, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets_out);
+}
+
+int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *d_hands,
+                                    int32_t min_inliers, gpdb_pose *d_clusters_out, int32_t *cluster_offsets_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  const char *name = "gpdb_find_clusters_batch_device";
+  int rc = check_groups_args(ctx, name, n_groups, hand_offsets, d_hands, d_clusters_out, cluster_offsets_out);
+  const char *names[2] = {"d_hands", "d_clusters_out"};
+  const void *ptrs[2] = {d_hands, d_clusters_out};
+  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 2, names, ptrs);
+  if (rc != GPDB_OK) return rc;
+  return find_clusters(ctx, n_groups, hand_offsets, d_hands, min_inliers, d_clusters_out, cluster_offsets_out, true);
 }
 
 void gpdb_free_result(gpdb_result *r) {

@@ -191,9 +191,9 @@ struct gpdb_ctx {
   // weights
   LenetWeights w;
   LenetTc tc;
-  // scratch (grown on demand)
-  void *scratch[24];
-  size_t scratch_sz[24];
+  // scratch (grown on demand); slot 24: the check word and per-cloud arrays of the device-resident entry points
+  void *scratch[25];
+  size_t scratch_sz[25];
   int *d_err;
   unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles, 32 slots: PATH_* below), nullptr = off
   int64_t launches;
@@ -217,10 +217,11 @@ void gpdb_pipe_destroy(gpdb_ctx *ctx);
 int gpdb_check_state(gpdb_ctx *ctx, bool need_cloud, bool need_weights);
 void *gpdb_result_extra(gpdb_result *r, size_t bytes);  // pinned host memory owned by the result (freed with it)
 // the chunked device pipeline (see api.cu) over the clouds of store s (ctx->many: a batch call whose sample offsets are
-// in s.soff); slot_base is added to every sample_slot (rank offset of a sharded call)
+// in s.soff); slot_base is added to every sample_slot (rank offset of a sharded call). A batch selection (ctx->many,
+// select_k >= 0) gets cloud-local sample slots; resident, it is written to sel_out (device) instead of the host arena.
 int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int32_t n, gpdb_result *out,
                       bool with_images_and_scores, bool resident, uint8_t *flags_ext, float *scores_ext, int select_k,
-                      int slot_base);
+                      int slot_base, gpdb_pose *sel_out = nullptr);
 // (re)allocates the arenas of store s for at least n points and n_clouds clouds
 int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds);
 // Installs the B clouds whose points the arrays of s already hold (cloud b: off[b] .. off[b+1]-1, host offsets): desc[b]
@@ -233,6 +234,22 @@ int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *
 int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
                       const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
                       CloudDesc *desc);
+
+// batch_device.cu (the device-resident batch entry points). The checks lower *d_first_bad (set to all ones by the caller)
+// to the first offending position.
+// camera masks of N points in B clouds (point offsets d_off[B+1]; cloud b's N_b x K_b int32 block starts at entry
+// d_row_off[b] of d_rows, K_b = d_k[b]; d_rows null: every camera sees every point), as gpdb_pack_cameras packs them;
+// d_all_seen[b] (1 on entry) drops to 0 when a point of cloud b misses a camera; strict01: first entry other than 0 / 1
+int batch_pack_cameras(gpdb_ctx *ctx, const int32_t *d_rows, const int *d_off, const long long *d_row_off, const int *d_k,
+                       int B, int N, bool eq1, bool strict01, uint8_t *d_cam, int *d_all_seen,
+                       unsigned long long *d_first_bad);
+// first point (float index / 3) of d_v[n] with a non-finite coordinate
+int batch_first_nonfinite(gpdb_ctx *ctx, const float *d_v, long long n, unsigned long long *d_first_bad);
+// first position i of the CSR sample list (cloud b: d_soff[b] .. d_soff[b+1]-1) with d_sidx[i] outside [0, d_lim[b])
+int batch_check_samples(gpdb_ctx *ctx, const int *d_sidx, int n, const int *d_soff, int B, const int *d_lim,
+                        unsigned long long *d_first_bad);
+// d_out[j] = d_in[j] with its sample slot made local to the cloud whose slots d_soff assigns it (d_in may equal d_out)
+int batch_local_slots(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, const int *d_soff, int B, gpdb_pose *d_out);
 
 // geometry.cu
 // builds the per-cloud grids of store s (its s.n descriptors hold off / N) and fills the descriptors' grid fields

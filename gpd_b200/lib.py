@@ -26,7 +26,8 @@ EXPORTS = [
     "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
     "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
     "gpdb_debug_path_counts", "gpdb_debug_lenet_layers", "gpdb_set_clouds_samples", "gpdb_hand_search_batch",
-    "gpdb_find_clusters_batch",
+    "gpdb_find_clusters_batch", "gpdb_preprocess_clouds_device", "gpdb_set_clouds_device", "gpdb_detect_batch_select_device",
+    "gpdb_find_clusters_batch_device",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -102,6 +103,10 @@ def lib():
     L.gpdb_set_clouds_samples.argtypes = [vp, vp, vp]
     L.gpdb_hand_search_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_find_clusters_batch.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
+    L.gpdb_preprocess_clouds_device.argtypes = L.gpdb_preprocess_clouds.argtypes
+    L.gpdb_set_clouds_device.argtypes = L.gpdb_set_clouds.argtypes
+    L.gpdb_detect_batch_select_device.argtypes = [vp, vp, vp, C.c_int32, vp, vp, C.POINTER(abi.Result)]
+    L.gpdb_find_clusters_batch_device.argtypes = L.gpdb_find_clusters_batch.argtypes
     _LIB = L
     return L
 
@@ -213,6 +218,42 @@ def split_batch_result(out, sample_offsets, cand_offsets):
     return views
 
 
+POSE_BYTES = C.sizeof(abi.Pose)
+
+
+def poses_from_tensor(t):
+    """The gpdb_pose records of a uint8 tensor [n, POSE_BYTES] (as the *_tensors methods return them) as a host
+    abi.POSE_DTYPE array."""
+    return t.detach().cpu().numpy().reshape(-1).view(abi.POSE_DTYPE).copy()
+
+
+def _host_i32(name, a, n=None):
+    a = np.ascontiguousarray(a, dtype=np.int32).ravel()
+    if n is not None and len(a) != n:
+        raise ValueError(f"{name}: {len(a)} entries, need {n}")
+    return a
+
+
+def _device_arg(name, t, dtype, device, numel, optional=False):
+    """The device pointer of a tensor argument of the gpdb_*_device calls, after the checks the library cannot make
+    (dtype, contiguity, size); ValueError / TypeError before any library call. An empty tensor passes NULL."""
+    import torch
+    if t is None:
+        if optional:
+            return None
+        raise ValueError(f"{name}: a CUDA tensor is required")
+    if not isinstance(t, torch.Tensor) or t.device.type != "cuda" or t.device.index != device:
+        where = t.device if isinstance(t, torch.Tensor) else type(t).__name__
+        raise ValueError(f"{name}: need a tensor on cuda:{device}, got {where}")
+    if t.dtype != dtype:
+        raise TypeError(f"{name}: need {dtype}, got {t.dtype}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name}: need a contiguous tensor")
+    if t.numel() != numel:
+        raise ValueError(f"{name}: {t.numel()} elements, need {numel}")
+    return C.c_void_p(t.data_ptr()) if numel else None
+
+
 class Context:
     """One gpdb_ctx: one CUDA device + stream (gpdb_create ... gpdb_destroy)."""
 
@@ -226,6 +267,7 @@ class Context:
         self._keep = []
         self._n_clouds = 0  # clouds of the installed batch (gpdb_detect_batch reads that many + 1 sample offsets)
         self._batch = None  # (point offsets, camera counts, view point blocks, has source indices) of the installed batch
+        self._stream = None  # the torch stream the *_tensors methods last moved the context to
 
     def close(self):
         if getattr(self, "h", None):
@@ -447,6 +489,95 @@ class Context:
         out = abi.result_to_numpy(res, 0)
         lib().gpdb_free_result(C.byref(res))
         return [out["candidates"][soff[b]:soff[b + 1]] for b in range(len(offsets) - 1)]
+
+    # ---- device-resident batches (gpdb_*_device): CUDA tensors in, CUDA tensors out -----------------------------------
+    # Every method checks device, dtype, contiguity and size of its tensors before the library call, moves the context
+    # to torch.cuda.current_stream() (inputs made ready on it need no synchronisation; later calls of this context run
+    # there too) and allocates its outputs with torch. Sizes and offsets are host arrays.
+
+    def _torch_stream(self):
+        import torch
+        s = torch.cuda.current_stream(self.params.device).cuda_stream
+        if s != self._stream:
+            self.set_stream(s)
+            self._stream = s
+
+    def _cloud_tensors(self, point_offsets, xyz, normals, cam_source, n_cameras, view_points, normals_optional):
+        off = _host_i32("point_offsets", point_offsets)
+        B = len(off) - 1
+        if B < 1:
+            raise ValueError("point_offsets: need at least two entries (one cloud)")
+        ks = _host_i32("n_cameras", n_cameras, B)
+        vp = np.ascontiguousarray(view_points, dtype=np.float64).reshape(-1, 3)
+        if len(vp) != int(ks.sum()):
+            raise ValueError(f"view_points: {len(vp)} rows, need sum(n_cameras) = {int(ks.sum())}")
+        import torch
+        dev = self.params.device
+        M = int(off[-1])
+        ptrs = (_device_arg("xyz", xyz, torch.float32, dev, 3 * M),
+                _device_arg("normals", normals, torch.float64, dev, 3 * M, optional=normals_optional),
+                _device_arg("cam_source", cam_source, torch.int32, dev, int(np.sum(np.diff(off).astype(np.int64) * ks)),
+                            optional=True))
+        self._torch_stream()
+        return off, ks, vp, ptrs
+
+    def preprocess_clouds_tensors(self, point_offsets, xyz, n_cameras, view_points, cam_source=None, normals=None, pp=None):
+        """gpdb_preprocess_clouds_device: preprocess_clouds() of raw clouds held in CUDA tensors, concatenated (cloud b:
+        rows point_offsets[b] .. point_offsets[b+1]-1 of xyz [M, 3] float32 and normals [M, 3] float64 or None; cam_source
+        int32 holding the N_b x K_b blocks one after the other, or None). point_offsets [B+1], n_cameras [B] and
+        view_points [sum K_b, 3] are host arrays. Installs the processed batch; returns its point offsets [B+1]."""
+        off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, True)
+        if pp is None:
+            pp = preprocess_params()
+        B = len(ks)
+        poff = np.zeros(B + 1, np.int32)
+        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._check(lib().gpdb_preprocess_clouds_device(self.h, B, _p(off), px, pn, pc, _p(ks), _p(vp), C.byref(pp), _p(poff)))
+        self._n_clouds = B
+        self._batch = (poff, ks, vp, True)
+        return poff
+
+    def set_clouds_tensors(self, point_offsets, xyz, normals, n_cameras, view_points, cam_source=None):
+        """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them
+        (normals required)."""
+        off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, False)
+        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._check(lib().gpdb_set_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp)))
+        self._n_clouds = len(ks)
+        self._batch = (off, ks, vp, False)
+
+    def detect_batch_select_tensors(self, sample_offsets, d_sample_idx, k):
+        """gpdb_detect_batch_select_device: the k best candidates of every installed cloud, for cloud-local sample indices
+        in an int32 CUDA tensor (CSR: cloud b's at sample_offsets[b] .. sample_offsets[b+1]-1, sample_offsets a host array
+        of B+1 entries). Returns (records, offsets): a uint8 CUDA tensor [n, POSE_BYTES] of gpdb_pose records (cloud b's
+        rows offsets[b] .. offsets[b+1]-1, as detect_batch_select returns them; poses_from_tensor reads them) and the host
+        offsets [B+1]."""
+        import torch
+        off = _host_i32("sample_offsets", sample_offsets, self._n_clouds + 1)
+        ps = _device_arg("d_sample_idx", d_sample_idx, torch.int32, self.params.device, int(off[-1]))
+        self._torch_stream()
+        out = torch.empty((self._n_clouds * max(int(k), 0), POSE_BYTES), dtype=torch.uint8, device=f"cuda:{self.params.device}")
+        soff = np.zeros(len(off), np.int32)
+        stats = abi.Result()
+        n = self._check(lib().gpdb_detect_batch_select_device(self.h, _p(off), ps, int(k),
+                                                               C.c_void_p(out.data_ptr()) if out.numel() else None, _p(soff),
+                                                               C.byref(stats)))
+        return out[:n], soff
+
+    def find_clusters_batch_tensors(self, hand_offsets, hands, min_inliers):
+        """gpdb_find_clusters_batch_device: find_clusters_batch() on groups of gpdb_pose records held in a uint8 CUDA tensor
+        [n, POSE_BYTES] (group g: rows hand_offsets[g] .. hand_offsets[g+1]-1, hand_offsets a host array). Returns
+        (clusters, offsets): a uint8 CUDA tensor [nc, POSE_BYTES] and the host offsets [G+1]."""
+        import torch
+        hoff = _host_i32("hand_offsets", hand_offsets)
+        n = int(hoff[-1]) if len(hoff) else 0
+        ph = _device_arg("hands", hands, torch.uint8, self.params.device, n * POSE_BYTES)
+        self._torch_stream()
+        out = torch.empty((n, POSE_BYTES), dtype=torch.uint8, device=f"cuda:{self.params.device}")
+        coff = np.zeros(max(len(hoff), 1), np.int32)
+        nc = self._check(lib().gpdb_find_clusters_batch_device(self.h, len(hoff) - 1, _p(hoff), ph, int(min_inliers),
+                                                               C.c_void_p(out.data_ptr()) if n else None, _p(coff)))
+        return out[:nc], coff
 
     def detect_batch_raw(self, offsets_i32, sidx_i32, res, cand_offsets_i32):
         """Timed path for tools/bench_batch.py: no numpy conversion; caller frees `res`."""

@@ -401,6 +401,47 @@ int gpdb_find_clusters(gpdb_ctx *ctx, const gpdb_pose *hands, int32_t n_hands, i
 int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *hands,
                              int32_t min_inliers, gpdb_pose *clusters_out, int32_t *cluster_offsets_out);
 
+/* --- device-resident batches: clouds, samples and results that live in GPU memory ------------------------------------
+ * The batch calls above from device memory, with no bulk PCIe traffic: preprocess (or install), detect + select and
+ * cluster a batch whose arrays a framework produced on the GPU (simulated depth cameras, device depth-to-cloud).
+ * Sizes and offsets stay on the host (B, point / sample / hand offsets, n_cameras, view_points, the preprocessing
+ * parameters; the library sizes its launches from them). Arguments named d_* are device pointers on the context's device:
+ * any non-NULL d_* argument that cudaPointerGetAttributes does not report as device or managed memory of that device is
+ * GPDB_ERR_INVALID, before any device work. The library reads and writes them in order on the context's stream
+ * (gpdb_set_stream: e.g. the framework's current stream, so that inputs made ready on it need no synchronisation) and, as
+ * every entry point, returns once its outputs are complete: they may then be used on any stream.
+ * Each call has the semantics, error codes, messages and failure rules of its host twin (a failed install leaves no batch,
+ * the single cloud is never touched); its checks run on the device (non-finite coordinates, cam_source entries, sample
+ * indices) and report the first offending point / entry / position, as the host loops do. */
+
+/* gpdb_preprocess_clouds from device arrays: d_xyz [3M] float32, d_normals [3M] float64 or NULL, d_cam_source (the
+ * N_b x K_b int32 blocks) or NULL; the raw arrays are read in place and the camera masks packed on the device. */
+int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
+                                  const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
+                                  const double *view_points, const gpdb_preprocess_params *pp,
+                                  int32_t *processed_offsets_out);
+
+/* gpdb_set_clouds from device arrays (d_xyz [3N], d_normals [3N], d_cam_source or NULL): copied device to device into
+ * the batch; the finiteness check and the camera masks run on the device. Returns B. */
+int gpdb_set_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
+                           const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
+                           const double *view_points);
+
+/* gpdb_detect_batch_select with device sample indices (d_sample_idx [sample_offsets[B]], cloud-local, checked on the
+ * device) and a device result: d_selected_out has room for B * num_selected records and receives them exactly as
+ * gpdb_detect_batch_select returns them (cloud-local sample_slot; cloud b's at sel_offsets_out[b] ..
+ * sel_offsets_out[b+1]); sel_offsets_out [B + 1] is a host array. stats receives the counts (n_candidates = records
+ * written, n_total_candidates), the stage timings and the launch count; its array members stay NULL and it needs no
+ * gpdb_free_result. Returns the number of records. */
+int gpdb_detect_batch_select_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx,
+                                    int32_t num_selected, gpdb_pose *d_selected_out, int32_t *sel_offsets_out,
+                                    gpdb_result *stats);
+
+/* gpdb_find_clusters_batch with device hands (d_hands [hand_offsets[G]]) and clusters (d_clusters_out, room for
+ * hand_offsets[G] records); hand_offsets and cluster_offsets_out [G + 1] are host arrays. */
+int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *d_hands,
+                                    int32_t min_inliers, gpdb_pose *d_clusters_out, int32_t *cluster_offsets_out);
+
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
  * back for the next call. A result may outlive its context. */
