@@ -62,7 +62,7 @@ void gpdb_set_error(gpdb_ctx *ctx, int code, const char *fmt, ...) {
   fprintf(stderr, "%s\n", dst);  // reference convention: errors are also printed
 }
 
-void *gpdb_scratch(gpdb_ctx *ctx, int slot, size_t bytes) {
+void *gpdb_scratch(gpdb_ctx *ctx, ScratchSlot slot, size_t bytes) {
   if (bytes == 0) bytes = 16;
   if (ctx->scratch_sz[slot] >= bytes) return ctx->scratch[slot];
   if (ctx->scratch[slot]) {
@@ -358,7 +358,7 @@ int gpdb_create(const gpdb_params *params, gpdb_ctx **ctx_out) {
          cudaMemcpy(ctx->dp, &ctx->hp, sizeof(DevParams), cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemset(ctx->d_err, 0, sizeof(int) * GPDB_NERR) == cudaSuccess;
   }
-  for (int i = 0; ok && i < 8; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
+  for (cudaEvent_t &e : ctx->ev) ok = ok && cudaEventCreate(&e) == cudaSuccess;
   ok = ok && gpdb_pipe_create(ctx) == GPDB_OK;
   ctx->overlap_hands = !(getenv("GPD_B200_OVERLAP") && getenv("GPD_B200_OVERLAP")[0] == '0');
   if (!ok) {
@@ -388,9 +388,9 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->tc.b1);
   cudaFree(ctx->tc.b2);
   cudaFree(ctx->tc.b3);
-  for (int i = 0; i < 25; i++) cudaFree(ctx->scratch[i]);
-  for (int i = 0; i < 8; i++)
-    if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+  for (int i = 0; i < SCR_N; i++) cudaFree(ctx->scratch[i]);
+  for (cudaEvent_t e : ctx->ev)
+    if (e) cudaEventDestroy(e);
   if (ctx->stream && ctx->own_stream) cudaStreamDestroy(ctx->stream);
   delete ctx->st;
   delete ctx;
@@ -561,7 +561,7 @@ int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off
 
 // ---- the device-resident entry points (gpdb_*_device): bulk arrays in device memory, sizes and offsets on the host ----
 
-static const unsigned long long NO_BAD = ~0ull;  // the check word of scratch slot 24 when no position offends
+static const unsigned long long NO_BAD = ~0ull;  // the check word when no position offends
 
 // every non-null pointer must be device (or managed) memory of the context's device; runs before any device work
 static int check_device_ptrs(gpdb_ctx *ctx, const char *name, int n, const char *const *names, const void *const *ptrs) {
@@ -578,8 +578,16 @@ static int check_device_ptrs(gpdb_ctx *ctx, const char *name, int n, const char 
   return GPDB_OK;
 }
 
-// reads the check word *d_bad after the work queued before it (stream synchronised)
-static int read_check(gpdb_ctx *ctx, const unsigned long long *d_bad, unsigned long long *bad) {
+// The check-word protocol of the device-side checks. The word, at the head of SCR_CHECK, is set to all ones;
+// enqueue(d_bad, d_extra) queues the kernel that lowers it to the first offending position, with `extra` bytes behind the
+// word for the check's own arrays; *bad receives the word (NO_BAD: nothing offends) once the stream has drained.
+template <class Enqueue>
+static int first_bad(gpdb_ctx *ctx, size_t extra, unsigned long long *bad, Enqueue enqueue) {
+  unsigned long long *d_bad = (unsigned long long *)gpdb_scratch(ctx, SCR_CHECK, sizeof(*d_bad) + extra);
+  if (!d_bad) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
+  const int rc = enqueue(d_bad, d_bad + 1);
+  if (rc != GPDB_OK) return rc;
   CUDA_TRY(cudaMemcpyAsync(bad, d_bad, sizeof(*bad), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return GPDB_OK;
@@ -591,13 +599,11 @@ static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int
                                const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01,
                                uint8_t *d_cam, CloudDesc *desc) {
   camera_descs(B, n_cameras, view_points, desc);
-  // slot 24: check word, element offsets of the cam_source blocks [B+1], point offsets [B+1], K_b [B], all_seen [B]
-  const size_t bytes = sizeof(long long) * ((size_t)B + 2) + sizeof(int) * (3 * (size_t)B + 1);
+  // behind the check word: element offsets of the cam_source blocks [B+1], point offsets [B+1], K_b [B], all_seen [B]
+  const size_t bytes = sizeof(long long) * ((size_t)B + 1) + sizeof(int) * (3 * (size_t)B + 1);
   std::vector<unsigned char> h(bytes);
-  unsigned long long *h_bad = (unsigned long long *)h.data();
-  long long *h_roff = (long long *)(h_bad + 1);
+  long long *h_roff = (long long *)h.data();
   int *h_off = (int *)(h_roff + B + 1), *h_k = h_off + B + 1, *h_all = h_k + B;
-  *h_bad = NO_BAD;
   h_roff[0] = 0;
   for (int b = 0; b < B; b++) {
     h_roff[b + 1] = h_roff[b] + (long long)(off[b + 1] - off[b]) * n_cameras[b];
@@ -605,17 +611,16 @@ static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int
     h_all[b] = 1;
   }
   memcpy(h_off, off, sizeof(int) * ((size_t)B + 1));
-  unsigned char *d = (unsigned char *)gpdb_scratch(ctx, 24, bytes);
-  if (!d) return GPDB_ERR_CUDA;
-  unsigned long long *d_bad = (unsigned long long *)d;
-  long long *d_roff = (long long *)(d_bad + 1);
-  int *d_off = (int *)(d_roff + B + 1), *d_k = d_off + B + 1, *d_all = d_k + B;
-  CUDA_TRY(cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = batch_pack_cameras(ctx, d_rows, d_off, d_roff, d_k, B, off[B], eq1, strict01, d_cam, d_all, d_bad);
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(h_all, d_all, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
   unsigned long long e;
-  if ((rc = read_check(ctx, d_bad, &e)) != GPDB_OK) return rc;
+  const int rc = first_bad(ctx, bytes, &e, [&](unsigned long long *d_bad, void *d) -> int {
+    long long *d_roff = (long long *)d;
+    int *d_off = (int *)(d_roff + B + 1), *d_k = d_off + B + 1, *d_all = d_k + B;
+    CUDA_TRY(cudaMemcpyAsync(d, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+    const int r = batch_pack_cameras(ctx, d_rows, d_off, d_roff, d_k, B, off[B], eq1, strict01, d_cam, d_all, d_bad);
+    if (r == GPDB_OK) CUDA_TRY(cudaMemcpyAsync(h_all, d_all, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+    return r;
+  });
+  if (rc != GPDB_OK) return rc;
   if (e != NO_BAD) {
     int b = 0;
     while ((unsigned long long)h_roff[b + 1] <= e) b++;
@@ -665,12 +670,10 @@ static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
                              const double *view_points) {
   const int N = point_offsets[B];
   CUDA_TRY(cudaSetDevice(ctx->device));
-  unsigned long long *d_bad = (unsigned long long *)gpdb_scratch(ctx, 24, sizeof(unsigned long long));
-  if (!d_bad) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
-  int rc = batch_first_nonfinite(ctx, d_xyz, 3 * (long long)N, d_bad);
-  unsigned long long bad = NO_BAD;
-  if (rc == GPDB_OK) rc = read_check(ctx, d_bad, &bad);
+  unsigned long long bad;
+  int rc = first_bad(ctx, 0, &bad, [&](unsigned long long *d_bad, void *) {
+    return batch_first_nonfinite(ctx, d_xyz, 3 * (long long)N, d_bad);
+  });
   if (rc != GPDB_OK) return rc;
   if (bad != NO_BAD) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess "
@@ -687,13 +690,18 @@ static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   return rc == GPDB_OK ? B : rc;
 }
 
-// gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); the caller drops
-// the store when this fails. device: xyz, normals and cam_source are the caller's device arrays (read in place, the
-// camera masks packed on the device), else host arrays uploaded here.
+// gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); a failed call
+// leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays (read in place, the camera
+// masks packed on the device), else host arrays uploaded here.
 static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *roff, const float *xyz,
                              const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
                              const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff,
-                             cudaEvent_t ev[6], bool device) {
+                             bool device = false) {
+  s.n = 0;
+  s.has_src = false;
+  // the stage boundaries are recorded in the context's events: preprocessing calls on one context are serialised by the
+  // stream synchronisation that ends this function, and a call that fails before it reads no event
+  cudaEvent_t *ev = ctx->ev;
   const int M = roff[B];
   // ---- camera masks, packed per cloud with its own K_b. A camera sees a point when its entry is exactly 1: the
   // reference's voxelisation keeps only those entries (cloud.cpp:327) and its normal estimation and reverseNormals test
@@ -707,7 +715,7 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   int rc;
   if (device) {
     CUDA_TRY(cudaSetDevice(ctx->device));
-    d_cam_raw = (uint8_t *)gpdb_scratch(ctx, 7, (size_t)M + 16);
+    d_cam_raw = (uint8_t *)gpdb_scratch(ctx, SCR_SIDX, (size_t)M + 16);
     if (!d_cam_raw) return GPDB_ERR_CUDA;
     cudaEventRecord(ev[0], ctx->stream);
     rc = pack_cameras_device(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, d_cam_raw,
@@ -722,7 +730,7 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     // ---- one upload of the concatenated raw arrays
     const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
-    unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, 7, raw_bytes);
+    unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, SCR_SIDX, raw_bytes);
     if (!raw) return GPDB_ERR_CUDA;
     double *nrm_up = normals ? (double *)raw : nullptr;
     float *xyz_up = (float *)(raw + (normals ? sizeof(double) * 3 * (size_t)M : 0));
@@ -745,15 +753,23 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   if (rc != GPDB_OK) return rc;
   cudaEventRecord(ev[4], ctx->stream);
   // ---- calculateNormalsOMP + reverseNormals, every cloud against its own grid; then the per-cloud nonunit flags: zero
-  // normals (points no camera sees) and voxel averages of supplied normals are not of unit length
-  if (pp->estimate_normals) {
-    rc = pre_normals_batch(ctx, s, pp->normals_radius);
-    if (rc != GPDB_OK) return rc;
+  // normals (points no camera sees) and voxel averages of supplied normals are not of unit length. The store holds the
+  // clouds by now: a failure drops them again.
+  auto tail = [&]() -> int {
+    if (pp->estimate_normals) {
+      const int r = pre_normals_batch(ctx, s, pp->normals_radius);
+      if (r != GPDB_OK) return r;
+    }
+    const int r = pre_nonunit_batch(ctx, s);
+    if (r != GPDB_OK) return r;
+    cudaEventRecord(ev[5], ctx->stream);
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return GPDB_OK;
+  };
+  if ((rc = tail()) != GPDB_OK) {
+    s.n = 0;
+    return rc;
   }
-  rc = pre_nonunit_batch(ctx, s);
-  if (rc != GPDB_OK) return rc;
-  cudaEventRecord(ev[5], ctx->stream);
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   memset(ctx->pre_ms, 0, sizeof(ctx->pre_ms));
   float t;
   for (int i = 0; i < 5; i++)
@@ -761,26 +777,6 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   if (cudaEventElapsedTime(&t, ev[0], ev[5]) == cudaSuccess) ctx->pre_ms[5] = t;
   s.has_src = true;
   return B;
-}
-
-// gpdb_preprocess_clouds / gpdb_preprocess after the argument checks: the events of the stage timings around
-// preprocess_clouds, and a failed call leaves no cloud in s
-static int preprocess_into(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *roff, const float *xyz,
-                           const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
-                           const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff,
-                           bool device = false) {
-  s.n = 0;
-  s.has_src = false;
-  cudaEvent_t ev[6] = {};
-  for (auto &e : ev) CUDA_TRY(cudaEventCreate(&e));
-  const int rc =
-      preprocess_clouds(ctx, s, name, B, roff, xyz, normals, cam_source, n_cameras, view_points, pp, poff, ev, device);
-  for (auto &e : ev) cudaEventDestroy(e);
-  if (rc < 0) {
-    s.n = 0;
-    s.has_src = false;
-  }
-  return rc;
 }
 
 // the arrays of store s to the host; the camera masks are expanded on the host, each cloud with its own camera count
@@ -870,7 +866,7 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
   }
   const int32_t roff[2] = {0, M};
   int32_t poff[2] = {0, 0};
-  const int rc = preprocess_into(ctx, ctx->one, "gpdb_preprocess", 1, roff, xyz, normals, cam_source, &K, view_points, pp,
+  const int rc = preprocess_clouds(ctx, ctx->one, "gpdb_preprocess", 1, roff, xyz, normals, cam_source, &K, view_points, pp,
                                  poff);
   if (rc < 0) return rc;
   if (poff[1] == 0) {  // the filter kept no point: no cloud
@@ -1096,26 +1092,22 @@ int check_device_errors(gpdb_ctx *ctx) {
 
 }  // namespace
 
-// The chunked device pipeline behind gpdb_detect / gpdb_hand_search / gpdb_detect_resident / gpdb_detect_sharded.
-//   resident == false: sample_idx is a HOST array, every result is copied back to the host (out)
-//   resident == true : sample_idx, flags_ext, scores_ext are DEVICE arrays; nothing but the per-chunk
-//                      candidate count crosses PCIe (out receives counts and timings only). A resident batch call
-//                      (gpdb_detect_batch_select_device) keeps flags and scores in scratch and writes its selection
-//                      to sel_out.
-// select_k >= 0 (gpdb_detect_select): the classified candidates of all chunks stay on the device, the select_k best are
-// sorted out there and only they are copied back; no per-sample / per-pose array is returned.
+// The chunked device pipeline behind the detect and hand-search entry points, single cloud, batch and sharded; the request
+// (PipeRequest, common.cuh) says where the samples are and where the results go. With device samples and a destination on
+// the device nothing but the per-chunk candidate count crosses PCIe. A selecting call (PIPE_TOP_*) keeps the classified
+// candidates of all chunks on the device, sorts the select_k best out there and delivers only them; no per-sample /
+// per-pose array is returned.
 //
 // Stream schedule (H = hand search + compaction of a chunk, I/L/S = images, LeNet, score scatter):
 //   compute: F  H0  H1  I0 L0 S0  H2  I1 L1 S1  ...      copy:  frames | n0 | n1 | cand0 flags0 scores0 | n2 | cand1 ...
 // The candidate count of chunk i is read back on the copy stream while H(i+1) runs, so the device never waits for the
 // host; every chunk is ONE k_images / LeNet launch sized to its candidate count (no tail launches), and the results of
 // chunk i go to the pinned arena while chunk i+1 computes.
-int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int32_t n, gpdb_result *out,
-                      bool with_images_and_scores, bool resident, uint8_t *flags_ext, float *scores_ext, int select_k,
-                      int slot_base, gpdb_pose *sel_out) {
-  const bool selecting = select_k >= 0;
-  const bool batch = &s == &ctx->many;  // run_batch has checked the samples against the clouds
-  const bool ext = resident && !batch;  // per-pose flags and scores in the caller's device arrays
+int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out) {
+  CloudSet &s = *rq.store;
+  const int n = rq.n;
+  const bool to_host = rq.dest == PIPE_TO_HOST;  // per-sample / per-pose arrays + all candidate records go to the host
+  const bool selecting = rq.dest == PIPE_TOP_HOST || rq.dest == PIPE_TOP_DEVICE;
   memset(out, 0, sizeof(*out));
   PipeState &ps = *ctx->pipe;
   const int P = ctx->hp.P, S = ctx->hp.S, C = ctx->hp.C;
@@ -1123,31 +1115,33 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
   const size_t psz = (size_t)S * S * 16;   // one image in the device layout (16-byte pixels, see k_images)
   out->n_samples = n;
   out->poses_per_sample = P;
-  if (!resident && !batch)
+  if (!rq.samples_on_device && !rq.per_cloud)
     for (int i = 0; i < n; i++)
-      if (sample_idx[i] < 0 || sample_idx[i] >= s.points() + s.n_samples) {
+      if (rq.sample_idx[i] < 0 || rq.sample_idx[i] >= s.points() + s.n_samples) {
         gpdb_set_error(ctx, GPDB_ERR_INVALID, "sample index %d at position %d outside the cloud (N = %d, + %d sample positions)",
-                       sample_idx[i], i, s.points(), s.n_samples);
+                       rq.sample_idx[i], i, s.points(), s.n_samples);
         return GPDB_ERR_INVALID;
       }
   const int64_t launches0 = ctx->launches;
   double ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   const int chunk = ctx->prm.chunk_samples > 0 ? ctx->prm.chunk_samples : 16384;
   const int batch_cap = ctx->prm.batch_size > 0 ? ctx->prm.batch_size : 32768;  // images per k_images / LeNet launch
-  const bool keep = with_images_and_scores && ctx->prm.keep_images && !resident && !selecting;
-  const bool to_host = !resident && !selecting;  // per-sample / per-pose arrays + all candidate records go to the host
+  const bool keep = rq.classify && ctx->prm.keep_images && to_host;
   const size_t nP = (size_t)n * P;
   const int cmax = std::min(chunk, std::max(n, 1));
-  int *d_sidx = resident && sample_idx ? const_cast<int *>(sample_idx) : (int *)gpdb_scratch(ctx, 7, sizeof(int) * (size_t)n);
-  double *d_frames = (double *)gpdb_scratch(ctx, 8, sizeof(double) * 9 * (size_t)n);
-  uint8_t *d_valid = (uint8_t *)gpdb_scratch(ctx, 9, (size_t)n);
-  uint8_t *d_flags = ext ? flags_ext : (uint8_t *)gpdb_scratch(ctx, 10, nP);
-  float *d_pscores = ext ? scores_ext : (float *)gpdb_scratch(ctx, 11, sizeof(float) * nP);
-  gpdb_pose *d_poses = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)cmax * P);
-  gpdb_pose *d_cand2 = (gpdb_pose *)gpdb_scratch(ctx, 13, 2 * sizeof(gpdb_pose) * (size_t)cmax * P);  // double-buffered
-  int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
+  int *d_sidx = rq.samples_on_device && rq.sample_idx ? const_cast<int *>(rq.sample_idx)
+                                                      : (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)n);
+  double *d_frames = (double *)gpdb_scratch(ctx, SCR_FRAMES, sizeof(double) * 9 * (size_t)n);
+  uint8_t *d_valid = (uint8_t *)gpdb_scratch(ctx, SCR_VALID, (size_t)n);
+  uint8_t *d_flags = rq.d_flags ? rq.d_flags : (uint8_t *)gpdb_scratch(ctx, SCR_FLAGS, nP);
+  float *d_pscores = rq.d_scores ? rq.d_scores : (float *)gpdb_scratch(ctx, SCR_PSCORES, sizeof(float) * nP);
+  gpdb_pose *d_poses = (gpdb_pose *)gpdb_scratch(ctx, SCR_POSES, sizeof(gpdb_pose) * (size_t)cmax * P);
+  gpdb_pose *d_cand2 = (gpdb_pose *)gpdb_scratch(ctx, SCR_CAND, 2 * sizeof(gpdb_pose) * (size_t)cmax * P);  // double-buffered
+  int *d_count = (int *)gpdb_scratch(ctx, SCR_COUNT, 64);
   if (!d_sidx || !d_frames || !d_valid || !d_flags || !d_pscores || !d_poses || !d_cand2 || !d_count) return GPDB_ERR_CUDA;
   gpdb_pose *d_cand[2] = {d_cand2, d_cand2 + (size_t)cmax * P};
+  rq.d_flags = d_flags;
+  rq.d_scores = d_pscores;
 
   HostArena *ar = nullptr;
   int rc = GPDB_OK;
@@ -1191,12 +1185,12 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
   // host-side layout of the fixed-size arrays inside arena buffer 0
   const size_t off_valid = 0, off_frames = ((size_t)n + 63) / 64 * 64, off_flags = off_frames + sizeof(double) * 9 * (size_t)n,
                off_scores = (off_flags + nP + 63) / 64 * 64, fixed_bytes = off_scores + sizeof(float) * nP + 64;
-  if (!resident) {
+  if (to_host || rq.dest == PIPE_TOP_HOST) {
     ar = arena_acquire(ctx);
     if (!ar) return GPDB_ERR_STATE;
     const size_t guess = std::max((size_t)1024, nP / 8);  // grown on demand
     if (!arena_reserve(ar, 0, to_host ? fixed_bytes : 64, 0) ||
-        !arena_reserve(ar, 1, sizeof(gpdb_pose) * (selecting ? (size_t)std::max(select_k, 1) : guess), 0)) {
+        !arena_reserve(ar, 1, sizeof(gpdb_pose) * (selecting ? (size_t)std::max(rq.select_k, 1) : guess), 0)) {
       gpdb_set_error(ctx, GPDB_ERR_CUDA, "cudaHostAlloc of the result arena failed");
       return finish(GPDB_ERR_CUDA);
     }
@@ -1207,8 +1201,8 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
   ctx->st->used = 0;
   cudaEvent_t t_all = gpdb_st_begin(ctx);
   if (n > 0) {
-    if (!resident)
-      PIPE_CUDA(cudaMemcpyAsync(d_sidx, sample_idx, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    if (!rq.samples_on_device)
+      PIPE_CUDA(cudaMemcpyAsync(d_sidx, rq.sample_idx, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
     PIPE_CUDA(cudaMemsetAsync(d_pscores, 0xFF, sizeof(float) * nP, ctx->stream));  // 0xFFFFFFFF = NaN
   }
   cudaEvent_t t0 = gpdb_st_begin(ctx);
@@ -1237,7 +1231,7 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
     if (overlap && cand_consumed[b]) CUDA_TRY(cudaStreamWaitEvent(hs, ps.ev_consumed[b], 0));  // ... and images / scatter read it
     ctx->stream = hs;  // the launchers (and the stage timers) use the context's current stream
     cudaEvent_t t1 = gpdb_st_begin(ctx);
-    int r = geo_hands(ctx, s, d_sidx + c0, nn, c0 + slot_base, d_frames + 9 * (size_t)c0, d_valid + c0, d_poses,
+    int r = geo_hands(ctx, s, d_sidx + c0, nn, c0 + rq.slot_base, d_frames + 9 * (size_t)c0, d_valid + c0, d_poses,
                       d_flags + (size_t)c0 * P);
     if (r == GPDB_OK) r = geo_compact(ctx, d_poses, d_flags + (size_t)c0 * P, nn * P, d_cand[b], d_count + b);
     if (r == GPDB_OK) gpdb_st_end(ctx, 1, t1);
@@ -1258,11 +1252,11 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
     if (overlap) PIPE_CUDA(cudaStreamWaitEvent(main_stream, ps.ev_compact[b], 0));  // d_cand[b], flags of chunk ci are ready
     total_nc += nc;
     uint8_t *d_img = nullptr;  // keep_images: the chunk's images in the cv::Mat layout
-    if (with_images_and_scores && nc > 0) {
-      float *d_scores = (float *)gpdb_scratch(ctx, 15, sizeof(float) * (size_t)nc);
+    if (rq.classify && nc > 0) {
+      float *d_scores = (float *)gpdb_scratch(ctx, SCR_SCORES, sizeof(float) * (size_t)nc);
       const int ib = std::min(nc, batch_cap);
-      uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, 0, psz * (size_t)ib);
-      if (keep) d_img = (uint8_t *)gpdb_scratch(ctx, 16, isz * (size_t)nc);
+      uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, SCR_P16, psz * (size_t)ib);
+      if (keep) d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz * (size_t)nc);
       if (!d_scores || !d_p16 || (keep && !d_img)) return finish(GPDB_ERR_CUDA);
       if (keep && ci > 0) PIPE_CUDA(cudaStreamWaitEvent(ctx->stream, ps.ev_copied[b ^ 1], 0));  // d_img is being read
       for (int b0 = 0; b0 < nc; b0 += batch_cap) {
@@ -1275,7 +1269,7 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
         PIPE_TRY(lenet_forward(ctx, d_p16, bn, d_scores + b0, nullptr));
         gpdb_st_end(ctx, 3, t3);
       }
-      PIPE_TRY(geo_scatter_scores(ctx, d_cand[b], d_scores, nc, c0 + slot_base, P, d_pscores + (size_t)c0 * P, d_cand[b]));
+      PIPE_TRY(geo_scatter_scores(ctx, d_cand[b], d_scores, nc, c0 + rq.slot_base, P, d_pscores + (size_t)c0 * P, d_cand[b]));
       if (keep) {
         PIPE_CUDA(cudaStreamSynchronize(ps.copy));  // growing moves the buffer: earlier image copies must have landed
         if (!arena_reserve(ar, 2, img_host + isz * (size_t)nc, img_host)) {
@@ -1329,14 +1323,14 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
     }
   }
   int n_sel = 0;
-  if (selecting && batch) {  // the top select_k of every cloud
+  if (selecting && rq.per_cloud) {  // the top select_k of every cloud
     gpdb_pose *d_top = nullptr;
-    rc = geo_select_batch(ctx, s, ctx->d_sel, total_nc, select_k, &d_top);
+    rc = geo_select_batch(ctx, s, ctx->d_sel, total_nc, rq.select_k, &d_top);
     if (rc < 0) return finish(rc);
     n_sel = rc;
     // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
-    PIPE_TRY(batch_local_slots(ctx, d_top, n_sel, s.soff, s.n, resident ? sel_out : d_top));
-    if (n_sel > 0 && !resident) {
+    PIPE_TRY(batch_local_slots(ctx, d_top, n_sel, s.soff, s.n, rq.dest == PIPE_TOP_DEVICE ? rq.d_selected : d_top));
+    if (n_sel > 0 && rq.dest == PIPE_TOP_HOST) {
       PIPE_CUDA(cudaStreamSynchronize(ps.copy));
       if (!arena_reserve(ar, 1, sizeof(gpdb_pose) * (size_t)n_sel, 0)) {
         gpdb_set_error(ctx, GPDB_ERR_CUDA, "cudaHostAlloc of the candidate arena failed");
@@ -1345,9 +1339,9 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
       PIPE_CUDA(cudaMemcpyAsync(ar->buf[1], d_top, sizeof(gpdb_pose) * (size_t)n_sel, cudaMemcpyDeviceToHost, ctx->stream));
     }
   } else if (selecting) {
-    n_sel = std::min(select_k, total_nc);
+    n_sel = std::min(rq.select_k, total_nc);
     if (n_sel > 0) {
-      gpdb_pose *d_top = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)std::max(n_sel, cmax * P));
+      gpdb_pose *d_top = (gpdb_pose *)gpdb_scratch(ctx, SCR_POSES, sizeof(gpdb_pose) * (size_t)std::max(n_sel, cmax * P));
       if (!d_top) return finish(GPDB_ERR_CUDA);
       PIPE_TRY(geo_select(ctx, ctx->d_sel, total_nc, n_sel, d_top));
       PIPE_CUDA(cudaMemcpyAsync(ar->buf[1], d_top, sizeof(gpdb_pose) * (size_t)n_sel, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1378,44 +1372,42 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int
   return out->n_candidates;
 }
 
-static int run_pipeline(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_result *out, bool with_images_and_scores,
-                        bool resident, uint8_t *flags_ext, float *scores_ext, int select_k = -1) {
-  return gpdb_run_pipeline(ctx, ctx->one, sample_idx, n, out, with_images_and_scores, resident, flags_ext, scores_ext, select_k,
-                           0);
-}
-static int check_state(gpdb_ctx *ctx, bool need_cloud, bool need_weights) { return gpdb_check_state(ctx, need_cloud, need_weights); }
-
 extern "C" {
 
 int gpdb_detect(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_result *out) {
-  int rc = check_state(ctx, true, true);
+  int rc = gpdb_check_state(ctx, true, true);
   if (rc != GPDB_OK) return rc;
   if (!out || (n > 0 && !sample_idx) || n < 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  return run_pipeline(ctx, sample_idx, n, out, true, false, nullptr, nullptr);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = sample_idx, .n = n, .classify = true, .dest = PIPE_TO_HOST};
+  return gpdb_run_pipeline(ctx, rq, out);
 }
 
 int gpdb_detect_select(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, int32_t num_selected, gpdb_result *out) {
-  int rc = check_state(ctx, true, true);
+  int rc = gpdb_check_state(ctx, true, true);
   if (rc != GPDB_OK) return rc;
   if (!out || (n > 0 && !sample_idx) || n < 0 || num_selected < 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_select: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  return run_pipeline(ctx, sample_idx, n, out, true, false, nullptr, nullptr, num_selected);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = sample_idx, .n = n, .classify = true, .dest = PIPE_TOP_HOST,
+                    .select_k = num_selected};
+  return gpdb_run_pipeline(ctx, rq, out);
 }
 
 int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n, uint8_t *d_flags_out,
                          float *d_scores_out, gpdb_result *stats) {
-  int rc = check_state(ctx, true, true);
+  int rc = gpdb_check_state(ctx, true, true);
   if (rc != GPDB_OK) return rc;
   if (!stats || n < 0 || (n > 0 && (!d_sample_idx || !d_flags_out || !d_scores_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_resident: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  return run_pipeline(ctx, d_sample_idx, n, stats, true, true, d_flags_out, d_scores_out);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = d_sample_idx, .n = n, .samples_on_device = true, .classify = true,
+                    .d_flags = d_flags_out, .d_scores = d_scores_out, .dest = PIPE_STAY};
+  return gpdb_run_pipeline(ctx, rq, stats);
 }
 
 }  // extern "C"
@@ -1502,7 +1494,7 @@ int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point
   const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, pp,
                                    processed_offsets_out, true);
   if (rc != GPDB_OK) return rc;
-  return preprocess_into(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
+  return preprocess_clouds(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
                          processed_offsets_out);
 }
 
@@ -1521,7 +1513,7 @@ int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t
   const void *ptrs[3] = {d_xyz, d_normals, d_cam_source};
   if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 3, names, ptrs);
   if (rc != GPDB_OK) return rc;
-  return preprocess_into(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
+  return preprocess_clouds(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
                          view_points, pp, processed_offsets_out, true);
 }
 
@@ -1592,17 +1584,13 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
   }
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   if (device && n > 0) {  // the same check on the device: the first offending position, then its cloud and value
-    unsigned char *d = (unsigned char *)gpdb_scratch(ctx, 24, sizeof(unsigned long long) + sizeof(int) * (size_t)B);
-    if (!d) return GPDB_ERR_CUDA;
-    unsigned long long *d_bad = (unsigned long long *)d;
-    int *d_lim = (int *)(d_bad + 1);
     std::vector<int> lim((size_t)B);
     for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b] + s.positions(b);
-    CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
-    unsigned long long bad = NO_BAD;
-    rc = batch_check_samples(ctx, sample_idx, n, s.soff, B, d_lim, d_bad);
-    if (rc == GPDB_OK) rc = read_check(ctx, d_bad, &bad);
+    unsigned long long bad;
+    rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
+      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+      return batch_check_samples(ctx, sample_idx, n, s.soff, B, (const int *)d_lim, d_bad);
+    });
     if (rc != GPDB_OK) return rc;
     if (bad != NO_BAD) {
       const int i = (int)bad;
@@ -1615,7 +1603,11 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
       return GPDB_ERR_INVALID;
     }
   }
-  rc = gpdb_run_pipeline(ctx, s, sample_idx, n, out, with_images_and_scores, device, nullptr, nullptr, select_k, 0, sel_out);
+  PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = device, .per_cloud = true,
+                    .classify = with_images_and_scores,
+                    .dest = select_k < 0 ? PIPE_TO_HOST : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
+                    .select_k = select_k, .d_selected = sel_out};
+  rc = gpdb_run_pipeline(ctx, rq, out);
   if (rc < 0) return rc;
   if (select_k >= 0) {  // the pipeline has made the selected records' sample slots cloud-local
     memcpy(offsets_out, s.sel, sizeof(int) * ((size_t)B + 1));
@@ -1690,17 +1682,18 @@ int gpdb_set_stream(gpdb_ctx *ctx, void *cuda_stream) {
 }
 
 int gpdb_hand_search(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpdb_result *out) {
-  int rc = check_state(ctx, true, false);
+  int rc = gpdb_check_state(ctx, true, false);
   if (rc != GPDB_OK) return rc;
   if (!out || (n > 0 && !sample_idx) || n < 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_hand_search: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  return run_pipeline(ctx, sample_idx, n, out, false, false, nullptr, nullptr);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = sample_idx, .n = n, .classify = false, .dest = PIPE_TO_HOST};
+  return gpdb_run_pipeline(ctx, rq, out);
 }
 
 int gpdb_frames(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, double *frames_out, uint8_t *valid_out) {
-  int rc = check_state(ctx, true, false);
+  int rc = gpdb_check_state(ctx, true, false);
   if (rc != GPDB_OK) return rc;
   if (n < 0 || (n > 0 && (!sample_idx || !frames_out || !valid_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_frames: bad arguments");
@@ -1712,9 +1705,9 @@ int gpdb_frames(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, double *fra
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "sample index %d outside the cloud (N = %d)", sample_idx[i], ctx->one.points());
       return GPDB_ERR_INVALID;
     }
-  int *d_sidx = (int *)gpdb_scratch(ctx, 7, sizeof(int) * (size_t)n);
-  double *d_frames = (double *)gpdb_scratch(ctx, 8, sizeof(double) * 9 * (size_t)n);
-  uint8_t *d_valid = (uint8_t *)gpdb_scratch(ctx, 9, (size_t)n);
+  int *d_sidx = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)n);
+  double *d_frames = (double *)gpdb_scratch(ctx, SCR_FRAMES, sizeof(double) * 9 * (size_t)n);
+  uint8_t *d_valid = (uint8_t *)gpdb_scratch(ctx, SCR_VALID, (size_t)n);
   if (!d_sidx || !d_frames || !d_valid) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(d_sidx, sample_idx, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = geo_frames(ctx, ctx->one, d_sidx, n, d_frames, d_valid)) != GPDB_OK) return rc;
@@ -1725,7 +1718,7 @@ int gpdb_frames(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, double *fra
 }
 
 int gpdb_images(gpdb_ctx *ctx, const gpdb_pose *poses, int32_t n, uint8_t *images_out) {
-  int rc = check_state(ctx, true, false);
+  int rc = gpdb_check_state(ctx, true, false);
   if (rc != GPDB_OK) return rc;
   if (n < 0 || (n > 0 && (!poses || !images_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_images: bad arguments");
@@ -1735,9 +1728,9 @@ int gpdb_images(gpdb_ctx *ctx, const gpdb_pose *poses, int32_t n, uint8_t *image
   const int batch = 8192;
   for (int b0 = 0; b0 < n; b0 += batch) {
     const int bn = std::min(batch, n - b0);
-    gpdb_pose *d_cand = (gpdb_pose *)gpdb_scratch(ctx, 13, sizeof(gpdb_pose) * (size_t)bn);
-    uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, 0, psz * (size_t)bn);
-    uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, 16, isz * (size_t)bn);
+    gpdb_pose *d_cand = (gpdb_pose *)gpdb_scratch(ctx, SCR_CAND, sizeof(gpdb_pose) * (size_t)bn);
+    uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, SCR_P16, psz * (size_t)bn);
+    uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz * (size_t)bn);
     if (!d_cand || !d_p16 || !d_img) return GPDB_ERR_CUDA;
     CUDA_TRY(cudaMemcpyAsync(d_cand, poses + b0, sizeof(gpdb_pose) * (size_t)bn, cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = geo_images(ctx, ctx->one, d_cand, bn, d_p16)) != GPDB_OK) return rc;
@@ -1760,9 +1753,9 @@ int classify_batches(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float 
   const int batch = ctx->prm.batch_size > 0 ? ctx->prm.batch_size : 8192;
   for (int b0 = 0; b0 < n; b0 += batch) {
     const int bn = std::min(batch, n - b0);
-    uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, 16, isz * (size_t)bn);
-    uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, 0, psz * (size_t)bn);
-    float *d_scores = (float *)gpdb_scratch(ctx, 15, sizeof(float) * (size_t)bn * 3);
+    uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz * (size_t)bn);
+    uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, SCR_P16, psz * (size_t)bn);
+    float *d_scores = (float *)gpdb_scratch(ctx, SCR_SCORES, sizeof(float) * (size_t)bn * 3);
     if (!d_img || !d_p16 || !d_scores) return GPDB_ERR_CUDA;
     float *d_logits = d_scores + bn;
     CUDA_TRY(cudaMemcpyAsync(d_img, images_hwc + isz * (size_t)b0, isz * (size_t)bn, cudaMemcpyHostToDevice, ctx->stream));
@@ -1785,7 +1778,7 @@ int classify_batches(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float 
 }  // namespace
 
 int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *scores_out, float *logits_out) {
-  int rc = check_state(ctx, false, true);
+  int rc = gpdb_check_state(ctx, false, true);
   if (rc != GPDB_OK) return rc;
   if (n < 0 || (n > 0 && (!images_hwc || !scores_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_classify: bad arguments");
@@ -1796,7 +1789,7 @@ int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *sc
 
 int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *pool1_out, double *pool2_out,
                             float *ip1_out, float *logits_out) {
-  int rc = check_state(ctx, false, true);
+  int rc = gpdb_check_state(ctx, false, true);
   if (rc != GPDB_OK) return rc;
   if (n < 0 || (n > 0 && !images_hwc)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_debug_lenet_layers: bad arguments");
@@ -1807,15 +1800,15 @@ int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n,
 }
 
 int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_out) {
-  int rc = check_state(ctx, true, false);
+  int rc = gpdb_check_state(ctx, true, false);
   if (rc != GPDB_OK) return rc;
   if (n < 0 || (n > 0 && (!hands || !labels_out))) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_reevaluate: bad arguments");
     return GPDB_ERR_INVALID;
   }
   if (n == 0) return 0;
-  gpdb_pose *d_h = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n);
-  int *d_l = (int *)gpdb_scratch(ctx, 18, sizeof(int) * (size_t)n);
+  gpdb_pose *d_h = (gpdb_pose *)gpdb_scratch(ctx, SCR_HANDS, sizeof(gpdb_pose) * (size_t)n);
+  int *d_l = (int *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int) * (size_t)n);
   if (!d_h || !d_l) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(d_h, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = geo_reeval(ctx, d_h, n, d_l)) != GPDB_OK) return rc;
@@ -1836,9 +1829,9 @@ static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, cons
   for (int g = 0; g <= G; g++) cluster_offsets_out[g] = 0;
   if (n == 0) return 0;
   CUDA_TRY(cudaSetDevice(ctx->device));
-  gpdb_pose *d_dense = (gpdb_pose *)gpdb_scratch(ctx, 17, sizeof(gpdb_pose) * (size_t)n * (device ? 2 : 3));
-  int *d_goff = (int *)gpdb_scratch(ctx, 18, sizeof(int) * (2 * (size_t)G + 1) + (size_t)n);
-  int *d_count = (int *)gpdb_scratch(ctx, 14, 64);
+  gpdb_pose *d_dense = (gpdb_pose *)gpdb_scratch(ctx, SCR_HANDS, sizeof(gpdb_pose) * (size_t)n * (device ? 2 : 3));
+  int *d_goff = (int *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int) * (2 * (size_t)G + 1) + (size_t)n);
+  int *d_count = (int *)gpdb_scratch(ctx, SCR_COUNT, 64);
   if (!d_dense || !d_goff || !d_count) return GPDB_ERR_CUDA;
   gpdb_pose *d_out = d_dense + n;
   int *d_gcount = d_goff + G + 1;

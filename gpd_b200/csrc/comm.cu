@@ -200,7 +200,7 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
       memcpy(hdr + 4, view_points, sizeof(double) * 3 * (size_t)K);
     }
   }
-  double *d_hdr = (double *)gpdb_scratch(ctx, 4, sizeof(hdr));
+  double *d_hdr = (double *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(hdr));
   if (!d_hdr) return GPDB_ERR_CUDA;
   CloudSet &s = ctx->one;
   s.n = 0;
@@ -256,7 +256,9 @@ int gpdb_detect_sharded_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx_loca
     CUDA_TRY(cudaMemsetAsync(d_scores + a, 0xFF, sizeof(float) * (b - a), ctx->stream));
     CUDA_TRY(cudaMemsetAsync(d_flags + a, 0, b - a, ctx->stream));
   }
-  int nc = gpdb_run_pipeline(ctx, ctx->one, d_sample_idx_local, n_local, stats, true, true, d_flags, d_scores, -1, 0);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = d_sample_idx_local, .n = n_local, .samples_on_device = true,
+                    .classify = true, .d_flags = d_flags, .d_scores = d_scores, .dest = PIPE_STAY};
+  int nc = gpdb_run_pipeline(ctx, rq, stats);
   if (nc < 0) return nc;
   cs.count = nc;
   CUDA_TRY(cudaMemcpyAsync(mine + slot - 16, &cs.count, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
@@ -279,13 +281,15 @@ int gpdb_detect_sharded(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpd
   int32_t lo, hi, slot_samples;
   gpdb_shard_bounds(n, cs.rank, cs.nranks, &lo, &hi, &slot_samples);
   // this rank's slice through the host-buffer pipeline (pose records of the slice -> pinned arena, sample_slot global)
-  int nc = gpdb_run_pipeline(ctx, ctx->one, sample_idx + lo, hi - lo, out, true, false, nullptr, nullptr, -1, lo);
+  PipeRequest rq = {.store = &ctx->one, .sample_idx = sample_idx + lo, .n = hi - lo, .classify = true, .dest = PIPE_TO_HOST,
+                    .slot_base = lo};
+  int nc = gpdb_run_pipeline(ctx, rq, out);
   if (nc < 0) return nc;
-  // the pipeline left the slice's dense flags / scores in its device scratch (slots 10 / 11): pack them into this
-  // rank's slot and all-gather
+  // the request now names the device arrays holding the slice's dense flags / scores: pack them into this rank's slot
+  // and all-gather
   const size_t slot = (size_t)gpdb_slot_bytes(slot_samples, P);
   const size_t np_l = (size_t)(hi - lo) * P, np_s = (size_t)slot_samples * P;
-  uint8_t *d_gath = (uint8_t *)gpdb_scratch(ctx, 5, slot * (size_t)cs.nranks);
+  uint8_t *d_gath = (uint8_t *)gpdb_scratch(ctx, SCR_WORK_B, slot * (size_t)cs.nranks);
   if (!d_gath) { gpdb_free_result(out); return GPDB_ERR_CUDA; }
   uint8_t *mine = d_gath + slot * (size_t)cs.rank;
   int err = GPDB_OK;
@@ -293,8 +297,8 @@ int gpdb_detect_sharded(gpdb_ctx *ctx, const int32_t *sample_idx, int32_t n, gpd
   cu(cudaMemsetAsync(mine, 0xFF, sizeof(float) * np_s, ctx->stream));
   cu(cudaMemsetAsync(mine + sizeof(float) * np_s, 0, slot - sizeof(float) * np_s, ctx->stream));
   if (np_l) {
-    cu(cudaMemcpyAsync(mine, ctx->scratch[11], sizeof(float) * np_l, cudaMemcpyDeviceToDevice, ctx->stream));
-    cu(cudaMemcpyAsync(mine + sizeof(float) * np_s, ctx->scratch[10], np_l, cudaMemcpyDeviceToDevice, ctx->stream));
+    cu(cudaMemcpyAsync(mine, rq.d_scores, sizeof(float) * np_l, cudaMemcpyDeviceToDevice, ctx->stream));
+    cu(cudaMemcpyAsync(mine + sizeof(float) * np_s, rq.d_flags, np_l, cudaMemcpyDeviceToDevice, ctx->stream));
   }
   cs.count = nc;
   cu(cudaMemcpyAsync(mine + slot - 16, &cs.count, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));

@@ -171,6 +171,60 @@ struct StageTimes;  // api.cu
 struct PipeState;   // api.cu: copy stream, events and the pinned result arenas of the chunk pipeline
 struct CommState;   // comm.cu: NCCL communicator (multi-GPU sharding)
 
+// The scratch buffers of a context (gpdb_scratch), each grown on demand and never shrunk. This enum is the whole slot
+// map: a buffer is addressed by its enumerator only, and a buffer several stages share is named for what it is, not for
+// one of its users. Two users of one buffer must never run at the same time. Outside the chunk pipeline all work of a
+// context is ordered on its one stream; the pipeline (gpdb_run_pipeline) drains its streams before it returns, and while
+// it runs it is the only place with two users live at once. Its rule is:
+//
+//   while the main stream is inside images / LeNet / score scatter of chunk i, the hand-search stream runs the hand
+//   search and compaction of chunk i + 1. The two sets of buffers must stay disjoint:
+//     hand-search stream writes  SCR_CUB, SCR_OVF, SCR_KEYS, SCR_POSES, SCR_CAND (its half), SCR_COUNT, SCR_HANDS_GL,
+//                                and chunk i + 1's range of SCR_FLAGS
+//     main stream writes         SCR_P16, SCR_WORK_A / B / C, SCR_SCORES, SCR_HWC, SCR_IMG_GL, SCR_IMG_OVF2, SCR_IMG_OVF,
+//                                chunk i's range of SCR_PSCORES and (ordered by events) chunk i's half of SCR_CAND
+//   both read SCR_SIDX, SCR_FRAMES and SCR_VALID, complete before the hand-search stream starts. The frames stage, the
+//   selection after the last chunk and every other entry point run on the main stream alone and may use either set.
+//   A stage that joins one of the two concurrent phases takes its buffers from that phase's set or gets a new one.
+enum ScratchSlot {
+  // main stream: images in the P16 layout (pipeline, gpdb_images, gpdb_classify); cell ids of the grid build
+  SCR_P16,
+  // cub temporary storage: the compaction on the hand-search stream; select, grid build and preprocessing otherwise
+  SCR_CUB,
+  // overflow lists of k_frames / k_hands (frames finish before the hand-search stream starts); of the normal estimation
+  SCR_OVF,
+  // compaction flags and positions (hand-search stream); sort keys and values of the selection
+  SCR_KEYS,
+  // stage workspaces. LeNet: pool1 / pool2 / ip1 (main stream). Preprocessing: header, filter flags + filtered points,
+  // voxel sort buffers. B is also the cell counts of the grid build; in the sharded calls A is the broadcast header and
+  // B the all-gather buffer
+  SCR_WORK_A, SCR_WORK_B, SCR_WORK_C,
+  // sample indices of a call; the raw upload / the device camera masks of preprocessing
+  SCR_SIDX,
+  // per call: frames, frame validity, dense per-pose flags, dense per-pose scores
+  SCR_FRAMES, SCR_VALID, SCR_FLAGS, SCR_PSCORES,
+  // dense pose records of one chunk (hand-search stream); the selection output after the last chunk
+  SCR_POSES,
+  // double-buffered candidate lists (gpdb_images: the uploaded poses); candidate counts [2] + the cluster count
+  SCR_CAND, SCR_COUNT,
+  // main stream: candidate scores (+ logits in gpdb_classify); images in the cv::Mat layout
+  SCR_SCORES, SCR_HWC,
+  // gpdb_reevaluate: hands, labels. Clustering: dense + compacted records (+ uploaded hands); group offsets, counts, keep flags
+  SCR_HANDS, SCR_LABELS,
+  // global-memory fallbacks of the capacity tiers. Image stage (main stream): the box lists of k_images' last tier and
+  // the overflow list of its shared-memory tier
+  SCR_IMG_GL, SCR_IMG_OVF2,
+  // k_hands last tier: the staged neighbourhoods (hand-search stream)
+  SCR_HANDS_GL,
+  // overflow list of k_images2 (main stream; not SCR_OVF, which the hand search of the next chunk is writing)
+  SCR_IMG_OVF,
+  // k_frames last tier: the staged neighbourhood keys
+  SCR_FRAMES_GL,
+  // device-resident entry points: the check word, then the per-cloud arrays of the check
+  SCR_CHECK,
+  SCR_N
+};
+
 struct gpdb_ctx {
   gpdb_params prm;
   DevParams hp;       // host copy
@@ -191,9 +245,9 @@ struct gpdb_ctx {
   // weights
   LenetWeights w;
   LenetTc tc;
-  // scratch (grown on demand); slot 24: the check word and per-cloud arrays of the device-resident entry points
-  void *scratch[25];
-  size_t scratch_sz[25];
+  // scratch (grown on demand), addressed through gpdb_scratch only
+  void *scratch[SCR_N];
+  size_t scratch_sz[SCR_N];
   int *d_err;
   unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles, 32 slots: PATH_* below), nullptr = off
   int64_t launches;
@@ -201,7 +255,7 @@ struct gpdb_ctx {
   double pre_ms[6];   // gpdb_preprocess stage timings
   gpdb_pose *d_sel;   // gpdb_detect_select: all classified candidates of a call (grown on demand)
   size_t sel_cap;
-  cudaEvent_t ev[8];
+  cudaEvent_t ev[6];  // stage boundaries of a preprocessing call (pre_ms)
 };
 
 void gpdb_set_error(gpdb_ctx *ctx, int code, const char *fmt, ...);
@@ -209,19 +263,37 @@ void gpdb_set_error(gpdb_ctx *ctx, int code, const char *fmt, ...);
 // compaction, 2 images, 3 LeNet, 4 whole call, 5 conv1, 6 conv2, 7 ip1+ip2
 cudaEvent_t gpdb_st_begin(gpdb_ctx *ctx);
 void gpdb_st_end(gpdb_ctx *ctx, int stage, cudaEvent_t begin);
-void *gpdb_scratch(gpdb_ctx *ctx, int slot, size_t bytes);  // returns nullptr on failure (error set)
+void *gpdb_scratch(gpdb_ctx *ctx, ScratchSlot slot, size_t bytes);  // returns nullptr on failure (error set)
 
 // api.cu
 int gpdb_pipe_create(gpdb_ctx *ctx);
 void gpdb_pipe_destroy(gpdb_ctx *ctx);
 int gpdb_check_state(gpdb_ctx *ctx, bool need_cloud, bool need_weights);
 void *gpdb_result_extra(gpdb_result *r, size_t bytes);  // pinned host memory owned by the result (freed with it)
-// the chunked device pipeline (see api.cu) over the clouds of store s (ctx->many: a batch call whose sample offsets are
-// in s.soff); slot_base is added to every sample_slot (rank offset of a sharded call). A batch selection (ctx->many,
-// select_k >= 0) gets cloud-local sample slots; resident, it is written to sel_out (device) instead of the host arena.
-int gpdb_run_pipeline(gpdb_ctx *ctx, CloudSet &s, const int32_t *sample_idx, int32_t n, gpdb_result *out,
-                      bool with_images_and_scores, bool resident, uint8_t *flags_ext, float *scores_ext, int select_k,
-                      int slot_base, gpdb_pose *sel_out = nullptr);
+// Where the results of a pipeline call go. The result struct always receives the counts and timings.
+enum PipeDest {
+  PIPE_TO_HOST,      // the per-sample / per-pose arrays and every candidate record (+ images if kept) to the host arena
+  PIPE_TOP_HOST,     // the select_k best records (per_cloud: of every cloud, sample slots cloud-local) to the host arena
+  PIPE_TOP_DEVICE,   // the same selection of a per_cloud call to d_selected on the device; nothing to the host
+  PIPE_STAY          // nothing leaves the device: the caller reads the dense flags and scores there
+};
+// One call of the chunked device pipeline (see api.cu): where its inputs are and where its outputs go.
+struct PipeRequest {
+  CloudSet *store;            // the clouds the samples address
+  const int32_t *sample_idx;  // n sample indices, in host or device memory
+  int32_t n;
+  bool samples_on_device;
+  bool per_cloud;             // the samples are the CSR stream of a batch call (offsets in store->soff, checked by the
+                              // caller); else they address the one cloud of the store and host samples are checked here
+  bool classify;              // images + LeNet scores; false: the hand search alone
+  uint8_t *d_flags;           // dense per-pose flags and scores [n * P] on the device. In: the caller's arrays, or null for
+  float *d_scores;            // the pipeline's scratch. Out: the arrays that were used, valid until the next call
+  PipeDest dest;
+  int select_k;               // PIPE_TOP_*: records to keep (per cloud when per_cloud)
+  gpdb_pose *d_selected;      // PIPE_TOP_DEVICE: receives them
+  int slot_base;              // added to every sample_slot (rank offset of a sharded call)
+};
+int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out);
 // (re)allocates the arenas of store s for at least n points and n_clouds clouds
 int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds);
 // Installs the B clouds whose points the arrays of s already hold (cloud b: off[b] .. off[b+1]-1, host offsets): desc[b]

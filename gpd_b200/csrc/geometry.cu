@@ -2713,10 +2713,10 @@ static int launch_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, in
   const size_t smem0 = (size_t)2 * LRF_WARPS * cap0 * sizeof(unsigned long long);
   const size_t smem1 = (size_t)2 * LRF_WARPS * LRF_CAP * sizeof(unsigned long long);
   CUDA_TRY(cudaFuncSetAttribute(k_frames<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-  int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * 2 * ((size_t)n + 1));
+  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * 2 * ((size_t)n + 1));
   const int g2 = 37;  // tier 2: 148 warps, 2 x 8 B x LRF_CAP_GLOBAL each (38 MB of scratch)
   unsigned long long *gkeys =
-      (unsigned long long *)gpdb_scratch(ctx, 23, sizeof(unsigned long long) * 2 * LRF_CAP_GLOBAL * (size_t)g2 * LRF_WARPS);
+      (unsigned long long *)gpdb_scratch(ctx, SCR_FRAMES_GL, sizeof(unsigned long long) * 2 * LRF_CAP_GLOBAL * (size_t)g2 * LRF_WARPS);
   if (!ovf || !gkeys) return GPDB_ERR_CUDA;
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
@@ -2754,8 +2754,8 @@ static int launch_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int
                         const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags) {
   // per call, not once per process: function attributes belong to the current device's context (one context per GPU)
   CUDA_TRY(cudaFuncSetAttribute(k_hands<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, HANDS_CAP2 * 16));
-  int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * 2 * ((size_t)n + 1));
-  float4 *glist = (float4 *)gpdb_scratch(ctx, 21, sizeof(float4) * (size_t)HANDS_CAP3 * ctx->sm_count);
+  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * 2 * ((size_t)n + 1));
+  float4 *glist = (float4 *)gpdb_scratch(ctx, SCR_HANDS_GL, sizeof(float4) * (size_t)HANDS_CAP3 * ctx->sm_count);
   if (!ovf || !glist) return GPDB_ERR_CUDA;
   int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
@@ -2793,7 +2793,7 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
     CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int), ctx->stream));
     return GPDB_OK;
   }
-  int *f01 = (int *)gpdb_scratch(ctx, 3, sizeof(int) * (size_t)n_poses * 2);
+  int *f01 = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * (size_t)n_poses * 2);
   if (!f01) return GPDB_ERR_CUDA;
   int *pos = f01 + n_poses;
   const int tb = 256, gb = (n_poses + tb - 1) / tb;
@@ -2801,7 +2801,7 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
   LAUNCH_CHECK();
   size_t tmp_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, f01, pos, n_poses, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
   if (!tmp) return GPDB_ERR_CUDA;
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, f01, pos, n_poses, ctx->stream));
   ctx->launches += 2;
@@ -2861,8 +2861,8 @@ static int launch_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_ca
   const bool fast = S == 60 && (hp.C != 15 || (K <= 2 && bm + 2048 <= (size_t)BOX_CAP2 * 36)) && !(force && force[0] == '1');
   const int *d_work = nullptr, *d_work_n = nullptr;
   if (fast) {
-    int *ovf = (int *)gpdb_scratch(ctx, 22, sizeof(int) * ((size_t)nc + 1));  // not slot 2: the hand search of the next chunk
-    if (!ovf) return GPDB_ERR_CUDA;                                            // may run concurrently on its own stream
+    int *ovf = (int *)gpdb_scratch(ctx, SCR_IMG_OVF, sizeof(int) * ((size_t)nc + 1));  // not SCR_OVF: the hand search of
+    if (!ovf) return GPDB_ERR_CUDA;                                                    // the next chunk may be writing it
     int *ovf_count = ovf + nc;
     CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
     const size_t smem2 = IMG2_DYN_SMEM;
@@ -2875,10 +2875,10 @@ static int launch_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_ca
   }
   // general tier (2 048-point box list in shared memory): everything, or the overflow list of the fast path; its own
   // overflow goes to a second list ...
-  int *ovf2 = (int *)gpdb_scratch(ctx, 20, sizeof(int) * ((size_t)nc + 1));
+  int *ovf2 = (int *)gpdb_scratch(ctx, SCR_IMG_OVF2, sizeof(int) * ((size_t)nc + 1));
   const int gl_cap = 32768;
   const size_t gl_slice = (size_t)gl_cap * 36 + (size_t)16 * S * S;
-  unsigned char *gl = (unsigned char *)gpdb_scratch(ctx, 19, gl_slice * (size_t)ctx->sm_count);
+  unsigned char *gl = (unsigned char *)gpdb_scratch(ctx, SCR_IMG_GL, gl_slice * (size_t)ctx->sm_count);
   if (!ovf2 || !gl) return GPDB_ERR_CUDA;
   int *ovf2_count = ovf2 + nc;
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
@@ -2931,7 +2931,7 @@ int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, const int *d_go
 
 int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *d_out) {
   if (n <= 0 || k <= 0) return GPDB_OK;
-  unsigned *keys = (unsigned *)gpdb_scratch(ctx, 3, sizeof(unsigned) * (size_t)n * 4);
+  unsigned *keys = (unsigned *)gpdb_scratch(ctx, SCR_KEYS, sizeof(unsigned) * (size_t)n * 4);
   if (!keys) return GPDB_ERR_CUDA;
   unsigned *keys2 = keys + n;
   int *vals = (int *)(keys2 + n), *vals2 = vals + n;
@@ -2939,7 +2939,7 @@ int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *
   LAUNCH_CHECK();
   size_t tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
   if (!tmp) return GPDB_ERR_CUDA;
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32, ctx->stream));
   ctx->launches += 4;
@@ -2961,7 +2961,7 @@ int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_sc
 int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
   const int B = s.n, N = s.points();
   long long *ncell =
-      (long long *)gpdb_scratch(ctx, 5, sizeof(long long) * 2 * ((size_t)B + 1) + sizeof(int) * (7 * (size_t)B + 1));
+      (long long *)gpdb_scratch(ctx, SCR_WORK_B, sizeof(long long) * 2 * ((size_t)B + 1) + sizeof(int) * (7 * (size_t)B + 1));
   if (!ncell) return GPDB_ERR_CUDA;
   long long *base = ncell + B + 1;
   int *d_off = (int *)(base + B + 1), *bounds = d_off + B + 1;
@@ -2975,7 +2975,7 @@ int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
   LAUNCH_CHECK();
   size_t tmp_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, ncell, base, B + 1, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
   if (!tmp) return GPDB_ERR_CUDA;
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, ncell, base, B + 1, ctx->stream));
   ctx->launches += 1;
@@ -2998,7 +2998,7 @@ int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
     s.cell_cap = ncells + 1 + ncells / 4;
   }
   CUDA_TRY(cudaMemsetAsync(s.cell_start, 0, sizeof(int) * (ncells + 1), ctx->stream));
-  int *cid = (int *)gpdb_scratch(ctx, 0, sizeof(int) * (size_t)N * 4);
+  int *cid = (int *)gpdb_scratch(ctx, SCR_P16, sizeof(int) * (size_t)N * 4);
   if (!cid) return GPDB_ERR_CUDA;
   int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
   const int tb = 256, gb = (N + tb - 1) / tb;
@@ -3006,7 +3006,7 @@ int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
   tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, cid, cid2, idx, idx2, N, 0, 32, ctx->stream);
   cub::DeviceScan::InclusiveSum(nullptr, tmp2, s.cell_start, s.cell_start, (int)(ncells + 1), ctx->stream);
-  tmp = gpdb_scratch(ctx, 1, std::max(tmp_bytes, tmp2));
+  tmp = gpdb_scratch(ctx, SCR_CUB, std::max(tmp_bytes, tmp2));
   if (!tmp) return GPDB_ERR_CUDA;
   if (N > 0) {  // a preprocessed batch may hold no point at all (every view filtered out)
     k_batch_cell_ids<<<gb, tb, 0, ctx->stream>>>(s.xyz, s.desc, B, N, cid, idx, s.cell_start);
@@ -3032,7 +3032,7 @@ int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n,
   int *sel_off = s.sel;
   *d_out = nullptr;
   unsigned long long *keys = (unsigned long long *)gpdb_scratch(
-      ctx, 3, sizeof(unsigned long long) * 2 * (size_t)n + sizeof(int) * (3 * (size_t)n + 2 * ((size_t)B + 1)));
+      ctx, SCR_KEYS, sizeof(unsigned long long) * 2 * (size_t)n + sizeof(int) * (3 * (size_t)n + 2 * ((size_t)B + 1)));
   if (!keys) return GPDB_ERR_CUDA;
   unsigned long long *keys2 = keys + n;
   int *vals = (int *)(keys2 + n), *vals2 = vals + n, *order = vals2 + n, *cand_off = order + n, *d_sel_off = cand_off + B + 1;
@@ -3047,7 +3047,7 @@ int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n,
     while ((1ll << cloud_bits) < B) cloud_bits++;
     size_t tmp_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32 + cloud_bits, ctx->stream);
-    void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+    void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
     if (!tmp) return GPDB_ERR_CUDA;
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, vals2, n, 0, 32 + cloud_bits, ctx->stream));
     ctx->launches += 4;
@@ -3060,7 +3060,7 @@ int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n,
   CUDA_TRY(cudaMemcpyAsync(d_sel_off, sel_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   k_batch_sel_order<<<(total + 255) / 256, 256, 0, ctx->stream>>>(vals2, cand_off, d_sel_off, B, total, order);
   LAUNCH_CHECK();
-  gpdb_pose *out = (gpdb_pose *)gpdb_scratch(ctx, 12, sizeof(gpdb_pose) * (size_t)total);
+  gpdb_pose *out = (gpdb_pose *)gpdb_scratch(ctx, SCR_POSES, sizeof(gpdb_pose) * (size_t)total);
   if (!out) return GPDB_ERR_CUDA;
   k_gather_poses<<<(total * 32 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, order, total, out);
   LAUNCH_CHECK();

@@ -312,9 +312,9 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
   }
   const LenetWeights &w = ctx->w;
   const bool use_tc = ctx->tc.ready && ctx->prm.lenet_impl != 1;
-  float *p1 = (float *)gpdb_scratch(ctx, 4, sizeof(float) * (size_t)n * NF1 * P1 * P1);
-  float *p2 = (float *)gpdb_scratch(ctx, 5, use_tc ? lenet_tc_xc_bytes(n) : sizeof(float) * (size_t)n * K);
-  float *h3 = (float *)gpdb_scratch(ctx, 6, sizeof(float) * (size_t)n * NH);
+  float *p1 = (float *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(float) * (size_t)n * NF1 * P1 * P1);
+  float *p2 = (float *)gpdb_scratch(ctx, SCR_WORK_B, use_tc ? lenet_tc_xc_bytes(n) : sizeof(float) * (size_t)n * K);
+  float *h3 = (float *)gpdb_scratch(ctx, SCR_WORK_C, sizeof(float) * (size_t)n * NH);
   if (!p1 || !p2 || !h3) return GPDB_ERR_CUDA;
   const int relu = ctx->prm.relu_after_conv;
   size_t sm1 = sizeof(float) * C * 25 * NF1 + (size_t)C * S * S;

@@ -535,7 +535,7 @@ int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius) {
   const CloudTable tab = s.table();
   const float r2 = (float)(radius * radius);
   const float rf = (float)radius * 1.0001f + 1e-6f;
-  int *ovf = (int *)gpdb_scratch(ctx, 2, sizeof(int) * ((size_t)N + 1));
+  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * ((size_t)N + 1));
   if (!ovf) return GPDB_ERR_CUDA;
   int *ovf_count = ovf + N;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
@@ -589,8 +589,8 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
                               int *poff, cudaEvent_t ev_filter_done) {
   const int tb = 256;
   // ---- removeNans + filterWorkspace, one scan for all clouds
-  // slot 4: workspace [6 doubles], raw / filtered / processed offsets [B+1 each], bounds [6B], voxel error [2]
-  double *d_ws = (double *)gpdb_scratch(ctx, 4, sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2));
+  // header: workspace [6 doubles], raw / filtered / processed offsets [B+1 each], bounds [6B], voxel error [2]
+  double *d_ws = (double *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2));
   if (!d_ws) return GPDB_ERR_CUDA;
   int *d_roff = (int *)(d_ws + 6), *d_foff = d_roff + B + 1, *d_poff = d_foff + B + 1, *d_bounds = d_poff + B + 1;
   int *d_verr = d_bounds + 6 * B;
@@ -598,7 +598,7 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   CUDA_TRY(cudaMemcpyAsync(d_ws, pp.workspace, sizeof(double) * 6, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(d_roff, roff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(d_verr, verr0, sizeof(verr0), cudaMemcpyHostToDevice, ctx->stream));
-  int *flag = (int *)gpdb_scratch(ctx, 5, sizeof(int) * (3 * (size_t)M + 2) + sizeof(float) * 3 * (size_t)M);
+  int *flag = (int *)gpdb_scratch(ctx, SCR_WORK_B, sizeof(int) * (3 * (size_t)M + 2) + sizeof(float) * 3 * (size_t)M);
   if (!flag) return GPDB_ERR_CUDA;
   int *pos = flag + M + 1, *keep = pos + M + 1;
   float *xyz1 = (float *)(keep + M);
@@ -607,7 +607,7 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   CUDA_TRY(cudaMemsetAsync(flag + M, 0, sizeof(int), ctx->stream));  // pos[M] = number of filtered points
   size_t tmp_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, M + 1, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, 1, tmp_bytes);
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
   if (!tmp) return GPDB_ERR_CUDA;
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, M + 1, ctx->stream));
   ctx->launches += 2;
@@ -638,7 +638,7 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   if (rc != GPDB_OK) return rc;
   // sort buffers: keys x2 (8 B), vals x3, cloud of point, cloud keys x2, head, gid, gfirst, gbegin, group order vals x2
   // (4 B each), group order keys x2 (8 B)
-  unsigned long long *keys = (unsigned long long *)gpdb_scratch(ctx, 6, (size_t)M1 * (16 + 48 + 16));
+  unsigned long long *keys = (unsigned long long *)gpdb_scratch(ctx, SCR_WORK_C, (size_t)M1 * (16 + 48 + 16));
   if (!keys) return GPDB_ERR_CUDA;
   unsigned long long *keys2 = keys + M1, *gord_k = keys2 + M1, *gord_k2 = gord_k + M1;
   int *vals = (int *)(gord_k2 + M1), *vals2 = vals + M1, *vals3 = vals2 + M1, *cl_of = vals3 + M1;
@@ -654,7 +654,7 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   if (cloud_bits) cub::DeviceRadixSort::SortPairs(nullptr, t2, ck, ck2, vals2, vals3, M1, 0, cloud_bits, ctx->stream);
   cub::DeviceScan::InclusiveSum(nullptr, t3, head, gid, M1, ctx->stream);
   cub::DeviceRadixSort::SortPairs(nullptr, t4, gord_k, gord_k2, gord_v, gord_v2, M1, 0, 32 + cloud_bits, ctx->stream);
-  tmp = gpdb_scratch(ctx, 1, std::max(std::max(t1, t2), std::max(t3, t4)));
+  tmp = gpdb_scratch(ctx, SCR_CUB, std::max(std::max(t1, t2), std::max(t3, t4)));
   if (!tmp) return GPDB_ERR_CUDA;
   // (cloud, key, index) order: the key sort keeps index order among equal keys, the cloud sort keeps key order. keys2
   // holds the keys in the final order: the key sort leaves them so, and after a cloud sort they are gathered into its order.
