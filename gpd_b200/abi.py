@@ -129,6 +129,22 @@ class PreprocessParams(C.Structure):
     ]
 
 
+class SisParams(C.Structure):
+    """gpdb_sis_params — cfg keys of SequentialImportanceSampling (sequential_importance_sampling.cpp:19-31)."""
+
+    _fields_ = [
+        ("num_iterations", C.c_int32),
+        ("num_samples_per_iteration", C.c_int32),
+        ("prob_rand_samples", C.c_double),
+        ("standard_deviation", C.c_double),
+        ("sampling_method", C.c_int32),
+        ("workspace", C.c_double * 6),
+        ("min_score", C.c_double),
+        ("min_inliers", C.c_int32),
+        ("seed", C.c_uint64),
+    ]
+
+
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""
     p = PreprocessParams()

@@ -40,6 +40,20 @@ void gpdb_st_end(gpdb_ctx *ctx, int stage, cudaEvent_t begin) {
   cudaEventRecord(e, ctx->stream);
   ctx->st->spans.push_back({stage, begin, e});
 }
+// What the last SIS call evaluated and kept, for gpdb_sis_positions (gpdb_sis_batch): the counts on
+// the host, the positions in SCR_SIS
+struct SisState {
+  bool valid = false;
+  int B = 0, R = 0, S = 0;
+  std::vector<int> init_off;  // [B + 1] initial samples per cloud (they size the kept arena)
+  std::vector<int> ecount;    // [R * B] round-major, as the device holds them
+  std::vector<int> koff;      // [B + 1] kept positions per cloud
+};
+// a new batch, or a SIS call that fails, leaves nothing for gpdb_sis_positions to read
+static void gpdb_sis_forget(gpdb_ctx *ctx) {
+  if (ctx->sis) ctx->sis->valid = false;
+}
+
 static void st_collect(gpdb_ctx *ctx, double *ms) {
   for (auto &sp : ctx->st->spans) {
     float t = 0;
@@ -381,6 +395,7 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->d_prof);
   cudaFree(ctx->d_qtab);
   cudaFree(ctx->d_sel);
+  delete ctx->sis;
   cloud_free(ctx->one);
   cloud_free(ctx->many);
   float *w[8] = {ctx->w.c1w, ctx->w.c1b, ctx->w.c2w, ctx->w.c2b, ctx->w.i1w, ctx->w.i1b, ctx->w.i2w, ctx->w.i2b};
@@ -804,21 +819,30 @@ static int get_clouds(gpdb_ctx *ctx, CloudSet &s, float *xyz_out, double *normal
   return (int)N;
 }
 
-// replaces the sample positions of store s by n positions (3 x n, column-major; n == 0: none)
-static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int n) {
+// drops the sample positions of store s and makes its arena hold n positions (grown, never shrunk)
+static int reserve_samples(gpdb_ctx *ctx, CloudSet &s, int n) {
   CUDA_TRY(cudaSetDevice(ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  cudaFree(s.samples);
-  s.samples = nullptr;
   s.n_samples = 0;
-  s.view.samples = nullptr;
-  if (n > 0) {
-    CUDA_TRY(cudaMalloc(&s.samples, sizeof(double) * 3 * (size_t)n));
-    CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  if ((size_t)n > s.samples_cap) {
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    s.view.samples = s.samples;
-    s.n_samples = n;
+    cudaFree(s.samples);
+    s.samples = nullptr;
+    s.samples_cap = 0;
+    s.view.samples = nullptr;
+    CUDA_TRY(cudaMalloc(&s.samples, sizeof(double) * 3 * (size_t)n));
+    s.samples_cap = (size_t)n;
   }
+  s.view.samples = s.samples;  // an install (gpdb_install_clouds) resets the kernels' view of the arena
+  return GPDB_OK;
+}
+
+// replaces the sample positions of store s by n host positions (3 x n, column-major; n == 0: none)
+static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int n) {
+  const int rc = reserve_samples(ctx, s, n);
+  if (rc != GPDB_OK || n == 0) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  s.n_samples = n;
   return GPDB_OK;
 }
 
@@ -1278,7 +1302,7 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out) {
         }
       }
     }
-    if (nc > 0 && selecting) {  // keep the chunk's scored candidates on the device
+    if (nc > 0 && (selecting || rq.dest == PIPE_ALL_DEVICE)) {  // keep the chunk's scored candidates on the device
       if ((size_t)total_nc > ctx->sel_cap) {
         const size_t cap = std::max((size_t)total_nc * 2, (size_t)65536);
         gpdb_pose *grown = nullptr;
@@ -1458,6 +1482,7 @@ int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offset
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is untouched either way
+  gpdb_sis_forget(ctx);  // the SIS positions describe clouds that are gone
   ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
   const char *name = "gpdb_set_clouds";
   const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, nullptr, nullptr,
@@ -1471,6 +1496,7 @@ int gpdb_set_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point
                            const double *view_points) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;
+  gpdb_sis_forget(ctx);
   ctx->many.n_samples = 0;
   const char *name = "gpdb_set_clouds_device";
   int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, d_xyz, d_normals, n_cameras, view_points, nullptr, nullptr,
@@ -1488,6 +1514,7 @@ int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point
                            const double *view_points, const gpdb_preprocess_params *pp, int32_t *processed_offsets_out) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
+  gpdb_sis_forget(ctx);
   ctx->many.has_src = false;
   ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
   const char *name = "gpdb_preprocess_clouds";
@@ -1504,6 +1531,7 @@ int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t
                                   int32_t *processed_offsets_out) {
   if (!ctx) return GPDB_ERR_INVALID;
   ctx->many.n = 0;
+  gpdb_sis_forget(ctx);
   ctx->many.has_src = false;
   ctx->many.n_samples = 0;
   const char *name = "gpdb_preprocess_clouds_device";
@@ -1822,7 +1850,8 @@ int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_
 
 // gpdb_find_clusters_batch after the argument checks (gpdb_find_clusters: one group): the clusters of all G groups in one
 // k_clusters launch, compacted in hand order, so group g's are clusters_out[cluster_offsets_out[g] ..
-// cluster_offsets_out[g+1]); returns their total. device: hands and clusters_out are device arrays (no copy of the hands)
+// cluster_offsets_out[g+1]); returns their total. device: hands are device arrays (no copy of the hands); clusters_out
+// may be host or device memory
 static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
                          gpdb_pose *clusters_out, int32_t *cluster_offsets_out, bool device = false) {
   const int n = hand_offsets[G];
@@ -1851,8 +1880,7 @@ static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, cons
   for (int g = 0; g < G; g++) cluster_offsets_out[g + 1] += cluster_offsets_out[g];
   const int nc = cluster_offsets_out[G];
   if (nc > 0) {
-    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc,
-                             device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(clusters_out, d_out, sizeof(gpdb_pose) * (size_t)nc, cudaMemcpyDefault, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   }
   return nc;
@@ -1914,6 +1942,327 @@ int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32
   if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 2, names, ptrs);
   if (rc != GPDB_OK) return rc;
   return find_clusters(ctx, n_groups, hand_offsets, d_hands, min_inliers, d_clusters_out, cluster_offsets_out, true);
+}
+
+}  // extern "C"
+
+// ---- sequential importance sampling (gpdb_sis_batch) ----------------------------------------------------------------
+
+// The arrays of SCR_SIS (doubles first): kept [3 * KC] with KC = n_init + B*R*S, evaluated [3 * B*R*S]; then the ints:
+// init offsets [B+1] and indices [n_init], kept counts [B], round counts [R*B], hand counts [B], the installed sample
+// list [KC]
+struct SisArena {
+  double *kept, *eval;
+  int *init_off, *init_idx, *kcount, *ecount, *hcount, *sidx;
+};
+static size_t sis_arena(int B, int R, int S, int n_init, void *base, SisArena *a) {
+  const size_t RS = (size_t)R * S, KC = (size_t)n_init + (size_t)B * RS;
+  double *d = (double *)base;
+  int *i = (int *)(d + 3 * (KC + (size_t)B * RS));
+  if (a) *a = {d, d + 3 * KC, i, i + B + 1, i + B + 1 + n_init, i + 2 * B + 1 + n_init,
+               i + 2 * B + 1 + n_init + R * (size_t)B, i + 3 * B + 1 + n_init + R * (size_t)B};
+  return sizeof(double) * 3 * (KC + (size_t)B * RS) + sizeof(int) * (3 * (size_t)B + 1 + n_init + (size_t)R * B + KC);
+}
+
+// The argument checks of gpdb_sis_batch[_device] after the state checks: parameters and offsets
+static int check_sis_args(gpdb_ctx *ctx, const char *name, int B, const gpdb_sis_params *sp, const int32_t *init_offsets,
+                          const void *init_idx, const void *out, const int32_t *hand_offsets_out) {
+  if (!sp || !init_offsets || init_offsets[0] != 0 || !out || !hand_offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need params, init_offsets[%d] starting at 0, a result and hand_offsets_out",
+                   name, B + 1);
+    return GPDB_ERR_INVALID;
+  }
+  if (sp->num_iterations < 0 || sp->num_samples_per_iteration < 0 || sp->min_inliers < 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: num_iterations, num_samples_per_iteration and min_inliers must not be negative",
+                   name);
+    return GPDB_ERR_INVALID;
+  }
+  if (!(sp->prob_rand_samples >= 0.0 && sp->prob_rand_samples <= 1.0)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: prob_rand_samples = %g outside [0, 1]", name, sp->prob_rand_samples);
+    return GPDB_ERR_INVALID;
+  }
+  if (!(std::isfinite(sp->standard_deviation) && sp->standard_deviation > 0.0)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: standard_deviation = %g must be finite and positive", name,
+                   sp->standard_deviation);
+    return GPDB_ERR_INVALID;
+  }
+  if (sp->sampling_method != 0 && sp->sampling_method != 1) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sampling_method = %d (0 sum of Gaussians, 1 max of Gaussians)", name,
+                   sp->sampling_method);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++)
+    if (init_offsets[b + 1] < init_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init_offsets decrease at cloud %d", name, b);
+      return GPDB_ERR_INVALID;
+    }
+  if (init_offsets[B] > 0 && !init_idx) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null init_idx", name);
+    return GPDB_ERR_INVALID;
+  }
+  const long long kc = (long long)init_offsets[B] + (long long)B * sp->num_iterations * sp->num_samples_per_iteration;
+  if (kc * ctx->hp.P > INT32_MAX) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %lld positions of %d poses exceed the 2^31 records of one call", name, kc,
+                   ctx->hp.P);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// The hand search of the CSR list d_sidx (offsets in s.soff, n samples) and the kept-set update it implies
+static int sis_search(gpdb_ctx *ctx, CloudSet &s, const int *d_sidx, int n, const SisArena &a, int RS) {
+  gpdb_result r;
+  PipeRequest rq = {.store = &s, .sample_idx = d_sidx, .n = n, .samples_on_device = true, .per_cloud = true,
+                    .classify = false, .dest = PIPE_STAY};
+  const int rc = gpdb_run_pipeline(ctx, rq, &r);
+  if (rc < 0) return rc;
+  return sis_keep(ctx, s, rq.d_flags, d_sidx, a.init_off, RS, a.kept, a.kcount);
+}
+
+// Installs, as gpdb_set_clouds_samples would, cloud b's cnt[b] positions of src (see sis_install) straight into the
+// store's sample arena, with the sample list N_b + j; h_cnt (host) gives the offsets. Returns the number of positions.
+static int sis_install_positions(gpdb_ctx *ctx, CloudSet &s, const SisArena &a, const int *h_cnt, const double *src,
+                                 int stride, int add, const int *init_off, const int *d_cnt) {
+  const int B = s.n;
+  s.pos[0] = 0;
+  for (int b = 0; b < B; b++) s.pos[b + 1] = s.pos[b] + h_cnt[b];
+  int rc = reserve_samples(ctx, s, s.pos[B]);
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.soff, s.pos, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = sis_install(ctx, s, src, stride, add, init_off, d_cnt, s.soff, s.samples, a.sidx)) != GPDB_OK) return rc;
+  s.n_samples = s.pos[B];
+  return s.n_samples;
+}
+
+// gpdb_sis_batch[_device] after the checks: d_init_idx already in the arena. dest (host or device) receives the records,
+// out the counts and timings.
+static int sis_run(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const SisArena &a, gpdb_pose *dest,
+                   bool dest_on_host, int32_t *hand_offsets_out, gpdb_result *out) {
+  CloudSet &s = ctx->many;
+  SisState &st = *ctx->sis;
+  const int B = s.n, R = sp->num_iterations, S = sp->num_samples_per_iteration, RS = R * S, P = ctx->hp.P;
+  const int64_t launches0 = ctx->launches;
+  // 1. the initial hand sets (:68-79)
+  CUDA_TRY(cudaMemcpyAsync(s.soff, init_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  int rc = sis_search(ctx, s, a.init_idx, init_offsets[B], a, RS);
+  if (rc != GPDB_OK) return rc;
+  std::vector<int> h_cnt((size_t)B);
+  CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.kcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  bool any_active = false;
+  for (int c : h_cnt) any_active |= c > 0;
+  // 2. the rounds (:109-160): draws, then the hand search at the drawn positions
+  SisDraw q = {R, S, 0, 0, sp->sampling_method, 0, sp->standard_deviation, {}, sp->seed};
+  q.n_rand = (int)(sp->prob_rand_samples * S);
+  q.n_gauss = S - q.n_rand;
+  for (int k = 0; k < 6; k++) q.ws[k] = sp->workspace[k];
+  int max_init = 0;
+  for (int b = 0; b < B; b++) max_init = std::max(max_init, init_offsets[b + 1] - init_offsets[b]);
+  for (int r = 0; r < R && any_active; r++) {
+    q.round = r;
+    const int stage_cap = std::min(max_init + r * S, 1920);  // 45 KB: with the scan storage inside the 48 KB default
+    if ((rc = sis_draw(ctx, q, B, s, a.init_off, a.init_idx, a.kept, a.kcount, stage_cap, a.eval, a.ecount)) != GPDB_OK)
+      return rc;
+    CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.ecount + (size_t)r * B, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost,
+                             ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    const int n = sis_install_positions(ctx, s, a, h_cnt.data(), a.eval, RS, r * S, nullptr, a.ecount + (size_t)r * B);
+    if (n < 0) return n;
+    if (n > 0 && (rc = sis_search(ctx, s, a.sidx, n, a, RS)) != GPDB_OK) return rc;
+  }
+  // 3. classify at every kept position (:168-170), keep score > min_score
+  st.ecount.resize((size_t)R * B);
+  CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.kcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(st.ecount.data(), a.ecount, sizeof(int) * st.ecount.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  const int M = sis_install_positions(ctx, s, a, h_cnt.data(), a.kept, RS, 0, a.init_off, a.kcount);
+  if (M < 0) return M;
+  st.koff.assign(s.pos, s.pos + B + 1);
+  PipeRequest rq = {.store = &s, .sample_idx = a.sidx, .n = M, .samples_on_device = true, .per_cloud = true, .classify = true,
+                    .dest = PIPE_ALL_DEVICE};
+  if ((rc = gpdb_run_pipeline(ctx, rq, out)) < 0) return rc;
+  const int total = out->n_total_candidates;
+  uint8_t *d_keep = (uint8_t *)gpdb_scratch(ctx, SCR_FLAGS, (size_t)total);
+  gpdb_pose *d_filt = (gpdb_pose *)gpdb_scratch(ctx, SCR_POSES, sizeof(gpdb_pose) * (size_t)total);
+  int *d_count = (int *)gpdb_scratch(ctx, SCR_COUNT, 64);
+  if (!d_keep || !d_filt || !d_count) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemsetAsync(a.hcount, 0, sizeof(int) * (size_t)B, ctx->stream));
+  if ((rc = sis_filter(ctx, ctx->d_sel, total, s.soff, B, sp->min_score, d_keep, a.hcount)) != GPDB_OK) return rc;
+  if ((rc = geo_compact(ctx, ctx->d_sel, d_keep, total, d_filt, d_count)) != GPDB_OK) return rc;
+  std::vector<int32_t> hoff((size_t)B + 1, 0);
+  CUDA_TRY(cudaMemcpyAsync(hoff.data() + 1, a.hcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  for (int b = 0; b < B; b++) hoff[b + 1] += hoff[b];
+  int n_out = hoff[B];
+  if (dest_on_host) dest = n_out ? (gpdb_pose *)malloc(sizeof(gpdb_pose) * (size_t)n_out) : nullptr;
+  if (n_out && !dest) {
+    gpdb_set_error(ctx, GPDB_ERR_CUDA, "out of host memory for %d records", n_out);
+    return GPDB_ERR_CUDA;
+  }
+  // 4. cluster (:177-179)
+  if (sp->min_inliers > 0) {
+    n_out = find_clusters(ctx, B, hoff.data(), d_filt, sp->min_inliers, dest, hand_offsets_out, true);
+  } else {
+    memcpy(hand_offsets_out, hoff.data(), sizeof(int32_t) * ((size_t)B + 1));
+    if (n_out) {
+      cudaError_t e = cudaMemcpyAsync(dest, d_filt, sizeof(gpdb_pose) * (size_t)n_out, cudaMemcpyDefault, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+      if (e != cudaSuccess) {
+        gpdb_set_error(ctx, GPDB_ERR_CUDA, "copy of the %d records: %s", n_out, cudaGetErrorString(e));
+        n_out = GPDB_ERR_CUDA;
+      }
+    }
+  }
+  if (n_out < 0) {
+    if (dest_on_host) free(dest);
+    return n_out;
+  }
+  st.valid = true;
+  out->n_samples = M;
+  out->poses_per_sample = P;
+  out->n_candidates = n_out;
+  out->candidates = dest_on_host ? dest : nullptr;
+  out->kernel_launches = ctx->launches - launches0;
+  return n_out;
+}
+
+// gpdb_sis_batch[_device]: checks, the initial indices into the arena (checked on the host, or on the device), sis_run
+static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp, const int32_t *init_offsets,
+                     const int32_t *init_idx, bool device, gpdb_pose *d_hands_out, int32_t *hand_offsets_out,
+                     gpdb_result *out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = ctx->many;
+  s.n_samples = 0;  // a failed call leaves no positions behind, and no SIS positions to read back
+  gpdb_sis_forget(ctx);
+  int rc = gpdb_check_state(ctx, false, true);
+  if (rc != GPDB_OK) return rc;
+  if (!ctx->sis) ctx->sis = new SisState();
+  if (s.n == 0) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first", name);
+    return GPDB_ERR_STATE;
+  }
+  const int B = s.n;
+  if ((rc = check_sis_args(ctx, name, B, sp, init_offsets, init_idx, out, hand_offsets_out)) != GPDB_OK) return rc;
+  const int n0 = init_offsets[B];
+  if (device) {
+    const char *names[2] = {"d_init_idx", "d_hands_out"};
+    const void *ptrs[2] = {init_idx, d_hands_out};
+    if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+    const long long kc = (long long)n0 + (long long)B * sp->num_iterations * sp->num_samples_per_iteration;
+    if (kc > 0 && !d_hands_out) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands_out", name);
+      return GPDB_ERR_INVALID;
+    }
+  } else {
+    for (int b = 0; b < B; b++)
+      for (int i = init_offsets[b]; i < init_offsets[b + 1]; i++)
+        if (init_idx[i] < 0 || init_idx[i] >= s.off[b + 1] - s.off[b]) {
+          gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name,
+                         init_idx[i], i, b, s.off[b + 1] - s.off[b]);
+          return GPDB_ERR_INVALID;
+        }
+  }
+  SisState &st = *ctx->sis;
+  const int R = sp->num_iterations, S = sp->num_samples_per_iteration;
+  void *base = gpdb_scratch(ctx, SCR_SIS, sis_arena(B, R, S, n0, nullptr, nullptr));
+  if (!base) return GPDB_ERR_CUDA;
+  SisArena a;
+  sis_arena(B, R, S, n0, base, &a);
+  CUDA_TRY(cudaMemcpyAsync(a.init_off, init_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  if (n0 > 0)
+    CUDA_TRY(cudaMemcpyAsync(a.init_idx, init_idx, sizeof(int) * (size_t)n0,
+                             device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemsetAsync(a.kcount, 0, sizeof(int) * (size_t)B * (R + 1), ctx->stream));  // kept and round counts
+  if (device && n0 > 0) {  // the init indices on the device: the first offending position, then its cloud and value
+    std::vector<int> lim((size_t)B);
+    for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b];
+    unsigned long long bad;
+    rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
+      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+      return batch_check_samples(ctx, a.init_idx, n0, a.init_off, B, (const int *)d_lim, d_bad);
+    });
+    if (rc != GPDB_OK) return rc;
+    if (bad != NO_BAD) {
+      const int i = (int)bad;
+      int b = 0, v = 0;
+      while (init_offsets[b + 1] <= i) b++;
+      CUDA_TRY(cudaMemcpyAsync(&v, a.init_idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name, v, i, b, lim[b]);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  st.B = B;
+  st.R = R;
+  st.S = S;
+  st.init_off.assign(init_offsets, init_offsets + B + 1);
+  rc = sis_run(ctx, sp, init_offsets, a, d_hands_out, !device, hand_offsets_out, out);
+  if (rc < 0) {
+    s.n_samples = 0;
+    st.valid = false;
+  }
+  return rc;
+}
+
+extern "C" {
+
+void gpdb_sis_params_default(gpdb_sis_params *p) {
+  memset(p, 0, sizeof(*p));
+  p->num_iterations = 5;
+  p->num_samples_per_iteration = 50;
+  p->prob_rand_samples = 0.3;
+  p->standard_deviation = 0.02;
+  const double ws[6] = {-1, 1, -1, 1, -1, 1};
+  for (int i = 0; i < 6; i++) p->workspace[i] = ws[i];
+  p->min_inliers = 1;
+}
+
+int gpdb_sis_batch(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *init_idx,
+                   gpdb_result *out, int32_t *hand_offsets_out) {
+  return sis_batch(ctx, "gpdb_sis_batch", sp, init_offsets, init_idx, false, nullptr, hand_offsets_out, out);
+}
+
+int gpdb_sis_batch_device(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *d_init_idx,
+                          gpdb_pose *d_hands_out, int32_t *hand_offsets_out, gpdb_result *stats) {
+  return sis_batch(ctx, "gpdb_sis_batch_device", sp, init_offsets, d_init_idx, true, d_hands_out, hand_offsets_out, stats);
+}
+
+int gpdb_sis_positions(gpdb_ctx *ctx, int32_t *eval_offsets_out, int32_t *eval_round_counts_out, double *eval_xyz_out,
+                       int32_t *kept_offsets_out, double *kept_xyz_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (!ctx->sis || !ctx->sis->valid) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_sis_positions: no successful gpdb_sis_batch call on this context");
+    return GPDB_ERR_STATE;
+  }
+  const SisState &st = *ctx->sis;
+  const int B = st.B, R = st.R, S = st.S, RS = R * S;
+  SisArena a;
+  sis_arena(B, R, S, st.init_off[B], ctx->scratch[SCR_SIS], &a);
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  // the evaluated and kept arenas, read once on the context's stream and unpacked on the host
+  std::vector<double> ev(eval_xyz_out ? 3 * (size_t)B * RS : 0), kp(kept_xyz_out ? 3 * ((size_t)st.init_off[B] + (size_t)B * RS) : 0);
+  if (!ev.empty()) CUDA_TRY(cudaMemcpyAsync(ev.data(), a.eval, sizeof(double) * ev.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  if (!kp.empty()) CUDA_TRY(cudaMemcpyAsync(kp.data(), a.kept, sizeof(double) * kp.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (eval_offsets_out || eval_round_counts_out || eval_xyz_out) {
+    size_t o = 0;
+    if (eval_offsets_out) eval_offsets_out[0] = 0;
+    for (int b = 0; b < B; b++) {
+      for (int r = 0; r < R; r++) {
+        const int c = st.ecount[(size_t)r * B + b];
+        if (eval_round_counts_out) eval_round_counts_out[(size_t)b * R + r] = c;
+        if (eval_xyz_out) memcpy(eval_xyz_out + 3 * o, ev.data() + 3 * ((size_t)b * R + r) * S, sizeof(double) * 3 * c);
+        o += c;
+      }
+      if (eval_offsets_out) eval_offsets_out[b + 1] = (int32_t)o;
+    }
+  }
+  if (kept_offsets_out) memcpy(kept_offsets_out, st.koff.data(), sizeof(int32_t) * ((size_t)B + 1));
+  if (kept_xyz_out)  // cloud b's kept positions start at position init_off[b] + b*R*S of the arena
+    for (int b = 0; b < B; b++)
+      memcpy(kept_xyz_out + 3 * (size_t)st.koff[b], kp.data() + 3 * ((size_t)st.init_off[b] + (size_t)b * RS),
+             sizeof(double) * 3 * (size_t)(st.koff[b + 1] - st.koff[b]));
+  return B;
 }
 
 void gpdb_free_result(gpdb_result *r) {

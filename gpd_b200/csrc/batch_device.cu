@@ -8,16 +8,6 @@
 
 namespace {
 
-// largest b in [0, n) with a[b] <= x, for a non-decreasing a with a[0] <= x: the cloud that owns position x of a CSR array
-__device__ __forceinline__ int owner(const int *a, int n, long long x) {
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] <= x) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 // one thread per point: bit k of cam[g] set when entry k of the point's row counts as seen (== 1 with eq1, else > 0); a
 // null rows means every camera sees every point. all_seen[b] (set to 1 by the caller) drops to 0 when a point of cloud b
 // misses a camera; with strict01, entries other than 0 / 1 report their index in the concatenated blocks.
@@ -25,7 +15,7 @@ __global__ void k_pack_cameras(const int32_t *rows, const int *off, const long l
                                int eq1, int strict01, uint8_t *cam, int *all_seen, unsigned long long *first_bad) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= N) return;
-  const int b = owner(off, B, g);
+  const int b = csr_owner(off, B, g);
   const int K = ks[b];
   const unsigned all = (1u << K) - 1;
   unsigned m = all;
@@ -53,7 +43,7 @@ __global__ void k_check_samples(const int *sidx, int n, const int *soff, int B, 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int v = sidx[i];
-  if (v < 0 || v >= lim[owner(soff, B, i)]) atomicMin(first_bad, (unsigned long long)i);
+  if (v < 0 || v >= lim[csr_owner(soff, B, i)]) atomicMin(first_bad, (unsigned long long)i);
 }
 
 // sample slots are positions in the whole sample stream: subtract the first slot of the record's cloud (in may equal out)
@@ -61,7 +51,7 @@ __global__ void k_local_slots(const gpdb_pose *in, int n, const int *soff, int B
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   gpdb_pose p = in[j];
-  p.sample_slot -= soff[owner(soff, B, p.sample_slot)];
+  p.sample_slot -= soff[csr_owner(soff, B, p.sample_slot)];
   out[j] = p;
 }
 

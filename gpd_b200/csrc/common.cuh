@@ -121,7 +121,8 @@ struct CloudSet {
   int n, maxk;          // clouds installed, largest camera count
   bool has_src;
   double *samples;      // sample positions (3 x n_samples): gpdb_set_samples (single cloud) / gpdb_set_clouds_samples (batch,
-  int n_samples;        // cloud b's at pos[b] .. pos[b+1]-1), or nullptr
+  int n_samples;        // cloud b's at pos[b] .. pos[b+1]-1), or nullptr; a grow-only arena of samples_cap positions
+  size_t samples_cap;
   int positions(int b) const { return n_samples ? pos[b + 1] - pos[b] : 0; }  // sample positions of cloud b
   DevCloud view;        // the concatenated arrays as the kernels read them
   int points() const { return n ? off[n] : 0; }
@@ -170,6 +171,7 @@ struct LenetTc {  // tensor-core (wgmma) weight blobs, lenet_tc.cu
 struct StageTimes;  // api.cu
 struct PipeState;   // api.cu: copy stream, events and the pinned result arenas of the chunk pipeline
 struct CommState;   // comm.cu: NCCL communicator (multi-GPU sharding)
+struct SisState;    // api.cu: host-side record of the last gpdb_sis_batch call (gpdb_sis_positions)
 
 // The scratch buffers of a context (gpdb_scratch), each grown on demand and never shrunk. This enum is the whole slot
 // map: a buffer is addressed by its enumerator only, and a buffer several stages share is named for what it is, not for
@@ -222,6 +224,9 @@ enum ScratchSlot {
   SCR_FRAMES_GL,
   // device-resident entry points: the check word, then the per-cloud arrays of the check
   SCR_CHECK,
+  // gpdb_sis_batch: kept / evaluated positions, the round's sample lists and counts (main stream, between pipeline calls;
+  // read again by gpdb_sis_positions)
+  SCR_SIS,
   SCR_N
 };
 
@@ -236,6 +241,7 @@ struct gpdb_ctx {
   StageTimes *st;
   PipeState *pipe;
   CommState *comm;
+  SisState *sis;
   int sm_count;
   int smem_optin;  // largest shared memory (dynamic + static) one block may opt in to, in bytes
   char err[512];
@@ -275,7 +281,8 @@ enum PipeDest {
   PIPE_TO_HOST,      // the per-sample / per-pose arrays and every candidate record (+ images if kept) to the host arena
   PIPE_TOP_HOST,     // the select_k best records (per_cloud: of every cloud, sample slots cloud-local) to the host arena
   PIPE_TOP_DEVICE,   // the same selection of a per_cloud call to d_selected on the device; nothing to the host
-  PIPE_STAY          // nothing leaves the device: the caller reads the dense flags and scores there
+  PIPE_STAY,         // nothing leaves the device: the caller reads the dense flags and scores there
+  PIPE_ALL_DEVICE    // PIPE_STAY, and every scored candidate record stays in ctx->d_sel (sample-slot order, stream slots)
 };
 // One call of the chunked device pipeline (see api.cu): where its inputs are and where its outputs go.
 struct PipeRequest {
@@ -307,6 +314,16 @@ int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off
                       const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
                       CloudDesc *desc);
 
+// largest b in [0, n) with a[b] <= x, for a non-decreasing a with a[0] <= x: the cloud that owns position x of a CSR array
+__device__ __forceinline__ int csr_owner(const int *a, int n, long long x) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (a[mid] <= x) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // batch_device.cu (the device-resident batch entry points). The checks lower *d_first_bad (set to all ones by the caller)
 // to the first offending position.
 // camera masks of N points in B clouds (point offsets d_off[B+1]; cloud b's N_b x K_b int32 block starts at entry
@@ -322,6 +339,33 @@ int batch_check_samples(gpdb_ctx *ctx, const int *d_sidx, int n, const int *d_so
                         unsigned long long *d_first_bad);
 // d_out[j] = d_in[j] with its sample slot made local to the cloud whose slots d_soff assigns it (d_in may equal d_out)
 int batch_local_slots(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, const int *d_soff, int B, gpdb_pose *d_out);
+
+// sis.cu (gpdb_sis_batch, include/gpd_b200_sis.h). Per cloud b of a batch with R rounds of S positions and initial
+// offsets init_off[B+1] (device), the kept arena holds room for init_off[b+1] - init_off[b] + R*S positions from position
+// init_off[b] + b*R*S, the evaluated arena S positions per (cloud, round) from (b*R + r)*S; kcount[b] counts the kept
+// positions, ecount[r*B + b] the positions of round r.
+struct SisDraw {
+  int R, S, n_gauss, n_rand, method, round;
+  double sigma, ws[6];
+  unsigned long long seed;
+};
+// the draws of round q.round for every cloud with a kept position (one CTA per cloud); stage_cap: kept positions a CTA may
+// stage in shared memory
+int sis_draw(gpdb_ctx *ctx, const SisDraw &q, int B, const CloudSet &s, const int *d_init_off, const int *d_init_idx,
+             const double *d_kept, const int *d_kcount, int stage_cap, double *d_eval, int *d_ecount);
+// appends, per cloud and in sample order, the position of every sample of the CSR list d_sidx (offsets s.soff) with a
+// VALID|FILTERED pose in the dense flags [n * P] to the cloud's kept positions
+int sis_keep(gpdb_ctx *ctx, const CloudSet &s, const uint8_t *d_flags, const int *d_sidx, const int *d_init_off, int RS,
+             double *d_kept, int *d_kcount);
+// the positions to install, as gpdb_set_clouds_samples would lay them out: cloud b's d_cnt[b] positions from position
+// b*stride + add (+ d_init_off[b] when given) of d_src go to d_dst (the store's sample arena) at d_soff[b],
+// d_sidx[d_soff[b] + j] = N_b + j, and the descriptors' first position becomes d_soff[b]
+int sis_install(gpdb_ctx *ctx, CloudSet &s, const double *d_src, int stride, int add, const int *d_init_off,
+                const int *d_cnt, const int *d_soff, double *d_dst, int *d_sidx);
+// the final score filter over n records of a batch call (stream sample slots, offsets d_soff): keep flag 3 where
+// score > min_score, sample slots made cloud-local, d_hcount[b] (zeroed by the caller) counts cloud b's kept records
+int sis_filter(gpdb_ctx *ctx, gpdb_pose *d_rec, int n, const int *d_soff, int B, double min_score, uint8_t *d_keep,
+               int *d_hcount);
 
 // geometry.cu
 // builds the per-cloud grids of store s (its s.n descriptors hold off / N) and fills the descriptors' grid fields

@@ -27,7 +27,8 @@ EXPORTS = [
     "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
     "gpdb_debug_path_counts", "gpdb_debug_lenet_layers", "gpdb_set_clouds_samples", "gpdb_hand_search_batch",
     "gpdb_find_clusters_batch", "gpdb_preprocess_clouds_device", "gpdb_set_clouds_device", "gpdb_detect_batch_select_device",
-    "gpdb_find_clusters_batch_device",
+    "gpdb_find_clusters_batch_device", "gpdb_sis_params_default", "gpdb_sis_batch", "gpdb_sis_batch_device",
+    "gpdb_sis_positions",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -107,6 +108,11 @@ def lib():
     L.gpdb_set_clouds_device.argtypes = L.gpdb_set_clouds.argtypes
     L.gpdb_detect_batch_select_device.argtypes = [vp, vp, vp, C.c_int32, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_find_clusters_batch_device.argtypes = L.gpdb_find_clusters_batch.argtypes
+    L.gpdb_sis_params_default.argtypes = [C.POINTER(abi.SisParams)]
+    L.gpdb_sis_params_default.restype = None
+    L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
+    L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
+    L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
     _LIB = L
     return L
 
@@ -142,6 +148,18 @@ def preprocess_params(**over):
     """gpdb_preprocess_params with the reference defaults (cfg/eigen_params.cfg:16-21), overridden by keyword."""
     p = abi.PreprocessParams()
     lib().gpdb_preprocess_params_default(C.byref(p))
+    for k, v in over.items():
+        if k == "workspace":
+            p.workspace[:] = list(v)
+        else:
+            setattr(p, k, v)
+    return p
+
+
+def sis_params(**over):
+    """gpdb_sis_params with the reference defaults (gpdb_sis_params_default), overridden by keyword (cfg key names)."""
+    p = abi.SisParams()
+    lib().gpdb_sis_params_default(C.byref(p))
     for k, v in over.items():
         if k == "workspace":
             p.workspace[:] = list(v)
@@ -268,6 +286,7 @@ class Context:
         self._n_clouds = 0  # clouds of the installed batch (gpdb_detect_batch reads that many + 1 sample offsets)
         self._batch = None  # (point offsets, camera counts, view point blocks, has source indices) of the installed batch
         self._stream = None  # the torch stream the *_tensors methods last moved the context to
+        self._sis_shape = None  # (B, num_iterations) of the last successful SIS call: sizes sis_positions' arrays
 
     def close(self):
         if getattr(self, "h", None):
@@ -382,7 +401,7 @@ class Context:
     def set_clouds(self, clouds):
         """gpdb_set_clouds: installs a batch of processed clouds (list of dicts as set_cloud takes) beside the single cloud."""
         pk = pack_clouds(clouds)
-        self._n_clouds, self._batch = 0, None  # a failed gpdb_set_clouds leaves no batch
+        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed gpdb_set_clouds leaves no batch
         self._check(lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
                                           _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])))
         self._n_clouds = len(clouds)
@@ -398,7 +417,7 @@ class Context:
             pp = preprocess_params()
         B = len(raw_clouds)
         poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_preprocess_clouds(self.h, B, _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
                                                  _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"]), C.byref(pp),
                                                  _p(poff)))
@@ -490,6 +509,39 @@ class Context:
         lib().gpdb_free_result(C.byref(res))
         return [out["candidates"][soff[b]:soff[b + 1]] for b in range(len(offsets) - 1)]
 
+    def sis_batch(self, init_lists, **sis):
+        """gpdb_sis_batch: SequentialImportanceSampling::detectGrasps on every installed cloud in one call, from one list of
+        cloud-local initial point indices per cloud; keywords are gpdb_sis_params fields (sis_params). Returns a dict:
+        "hands" one record array per cloud (hands with score > min_score, or their clusters when min_inliers > 0),
+        "n_samples" the kept positions, "n_total_candidates" the classified candidates, and the positions of
+        sis_positions()."""
+        offsets, idx = self._pack_batch_samples(init_lists)
+        sp = sis_params(**sis)
+        res = abi.Result()
+        hoff = np.zeros(len(offsets), np.int32)
+        self._sis_shape = None  # a failed call leaves nothing to read back
+        self._check(lib().gpdb_sis_batch(self.h, C.byref(sp), _p(offsets), _p(idx), C.byref(res), _p(hoff)))
+        self._sis_shape = (len(hoff) - 1, sp.num_iterations)
+        out = abi.result_to_numpy(res, 0)
+        lib().gpdb_free_result(C.byref(res))
+        return {"hands": [out["candidates"][hoff[b]:hoff[b + 1]] for b in range(len(hoff) - 1)], "n_samples": out["n_samples"],
+                "n_total_candidates": out["n_total_candidates"], **self.sis_positions()}
+
+    def sis_positions(self):
+        """gpdb_sis_positions: per cloud, "evaluated" the positions of every round [n, 3] in round order, "round_counts"
+        [B, num_iterations], and "kept" the positions that carried a hand [k, 3], initial samples first. The arrays are
+        sized by the batch of that call; after a new batch is installed there is nothing to read (GpdbError)."""
+        if self._sis_shape is None:  # the library holds no record either: let it name the error
+            self._check(lib().gpdb_sis_positions(self.h, None, None, None, None, None))
+            raise GpdbError(-3, "sis_positions: no successful SIS call on the installed batch")
+        B, R = self._sis_shape
+        eoff, koff, rcount = np.zeros(B + 1, np.int32), np.zeros(B + 1, np.int32), np.zeros(B * R, np.int32)
+        self._check(lib().gpdb_sis_positions(self.h, _p(eoff), _p(rcount), None, _p(koff), None))
+        ev, kept = np.zeros((int(eoff[-1]), 3)), np.zeros((int(koff[-1]), 3))
+        self._check(lib().gpdb_sis_positions(self.h, None, None, _p(ev), None, _p(kept)))
+        return {"evaluated": [ev[eoff[b]:eoff[b + 1]] for b in range(B)], "round_counts": rcount.reshape(B, R),
+                "kept": [kept[koff[b]:koff[b + 1]] for b in range(B)]}
+
     # ---- device-resident batches (gpdb_*_device): CUDA tensors in, CUDA tensors out -----------------------------------
     # Every method checks device, dtype, contiguity and size of its tensors before the library call, moves the context
     # to torch.cuda.current_stream() (inputs made ready on it need no synchronisation; later calls of this context run
@@ -531,7 +583,7 @@ class Context:
             pp = preprocess_params()
         B = len(ks)
         poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_preprocess_clouds_device(self.h, B, _p(off), px, pn, pc, _p(ks), _p(vp), C.byref(pp), _p(poff)))
         self._n_clouds = B
         self._batch = (poff, ks, vp, True)
@@ -541,7 +593,7 @@ class Context:
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them
         (normals required)."""
         off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, False)
-        self._n_clouds, self._batch = 0, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_set_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp)))
         self._n_clouds = len(ks)
         self._batch = (off, ks, vp, False)
@@ -563,6 +615,29 @@ class Context:
                                                                C.c_void_p(out.data_ptr()) if out.numel() else None, _p(soff),
                                                                C.byref(stats)))
         return out[:n], soff
+
+    def sis_batch_tensors(self, init_offsets, d_init_idx, **sis):
+        """gpdb_sis_batch_device: sis_batch() from cloud-local initial indices in an int32 CUDA tensor (CSR: cloud b's at
+        init_offsets[b] .. init_offsets[b+1]-1, init_offsets a host array of B+1 entries). Returns (records, offsets, stats):
+        a uint8 CUDA tensor [n, POSE_BYTES] of gpdb_pose records (cloud b's rows offsets[b] .. offsets[b+1]-1, as sis_batch
+        returns them; poses_from_tensor reads them), the host offsets [B+1] and a dict of n_samples, n_total_candidates
+        and kernel_launches."""
+        import torch
+        off = _host_i32("init_offsets", init_offsets, self._n_clouds + 1)
+        pi = _device_arg("d_init_idx", d_init_idx, torch.int32, self.params.device, int(off[-1]))
+        sp = sis_params(**sis)
+        self._torch_stream()
+        P = self.params.num_hand_axes * self.params.num_orientations
+        cap = (int(off[-1]) + self._n_clouds * max(sp.num_iterations, 0) * max(sp.num_samples_per_iteration, 0)) * P
+        out = torch.empty((cap, POSE_BYTES), dtype=torch.uint8, device=f"cuda:{self.params.device}")
+        hoff = np.zeros(len(off), np.int32)
+        stats = abi.Result()
+        self._sis_shape = None
+        n = self._check(lib().gpdb_sis_batch_device(self.h, C.byref(sp), _p(off), pi,
+                                                     C.c_void_p(out.data_ptr()) if cap else None, _p(hoff), C.byref(stats)))
+        self._sis_shape = (len(hoff) - 1, sp.num_iterations)
+        return out[:n], hoff, {"n_samples": stats.n_samples, "n_total_candidates": stats.n_total_candidates,
+                               "kernel_launches": stats.kernel_launches}
 
     def find_clusters_batch_tensors(self, hand_offsets, hands, min_inliers):
         """gpdb_find_clusters_batch_device: find_clusters_batch() on groups of gpdb_pose records held in a uint8 CUDA tensor

@@ -442,6 +442,53 @@ int gpdb_detect_batch_select_device(gpdb_ctx *ctx, const int32_t *sample_offsets
 int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *d_hands,
                                     int32_t min_inliers, gpdb_pose *d_clusters_out, int32_t *cluster_offsets_out);
 
+/* --- sequential importance sampling: SequentialImportanceSampling::detectGrasps on the device ----------------------------
+ * (sequential_importance_sampling.cpp:54-270) over every cloud of the installed batch (gpdb_set_clouds[_device] /
+ * gpdb_preprocess_clouds[_device]; a single cloud is a batch of one) in ONE call: the initial hand search, every round's
+ * draws (include/gpd_b200_sis.h), hand search and kept-set bookkeeping, the final classification at all kept positions, the
+ * score filter and the clustering run on the device; a round reads back B counts. Field names are the reference's SIS cfg
+ * keys (:19-31). */
+typedef struct gpdb_sis_params {
+  int32_t num_iterations;            /* rounds (5)                                                            */
+  int32_t num_samples_per_iteration; /* positions drawn per round and cloud (50)                              */
+  double prob_rand_samples;          /* share of uniform positions (0.3): num_rand = (int)(prob * S)          */
+  double standard_deviation;         /* sigma of the Gaussian proposals (0.02)                                */
+  int32_t sampling_method;           /* 0 sum of Gaussians, 1 max of Gaussians (rejection)                    */
+  double workspace[6];               /* uniform positions: inclusive bounds min_x max_x min_y max_y min_z max_z */
+  double min_score;                  /* keep hands with score > min_score (pruneGraspCandidates)              */
+  int32_t min_inliers;               /* > 0: return the clusters (findClusters); 0: the kept hands            */
+  uint64_t seed;                     /* cloud b draws with key seed + b                                       */
+} gpdb_sis_params;
+
+/* The reference defaults above, workspace -1..1, min_score 0, min_inliers 1, seed 0. */
+void gpdb_sis_params_default(gpdb_sis_params *p);
+
+/* init_idx: cloud-local point indices in CSR form (cloud b: init_idx[init_offsets[b] .. init_offsets[b+1]), B + 1
+ * offsets), drawn by the caller (Cloud::subsample). A cloud whose initial search finds no hand is inactive: no rounds, no
+ * output. The result holds per cloud the hands with score > min_score at the kept positions, in the order
+ * gpdb_detect_batch returns them there (cloud-local sample slots), or their clusters in seed order when min_inliers > 0;
+ * cloud b's records are out->candidates[hand_offsets_out[b] .. hand_offsets_out[b+1]). The per-sample arrays are NULL,
+ * n_samples counts the kept positions and n_total_candidates the classified candidates. Afterwards the batch holds the
+ * kept positions as gpdb_set_clouds_samples would install them; a failed call leaves none, the single cloud is never
+ * touched. Needs weights (GPDB_ERR_STATE). Negative counts, prob_rand_samples outside [0, 1], a sigma that is not finite
+ * and positive, a sampling_method other than 0 / 1, malformed offsets and an init index outside its cloud are
+ * GPDB_ERR_INVALID before any device work. Returns the number of records. */
+int gpdb_sis_batch(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *init_idx,
+                   gpdb_result *out, int32_t *hand_offsets_out);
+/* The same from device memory (the rules of the device-resident family above): d_init_idx is checked on the device,
+ * d_hands_out has room for (init_offsets[B] + B * num_iterations * num_samples_per_iteration) * P records and receives
+ * them; stats receives the counts, timings and launches, its array members stay NULL. Bit-equal to gpdb_sis_batch. */
+int gpdb_sis_batch_device(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *d_init_idx,
+                          gpdb_pose *d_hands_out, int32_t *hand_offsets_out, gpdb_result *stats);
+/* What the last successful SIS call evaluated and kept (host arrays, any may be NULL): eval_offsets_out [B+1] and
+ * eval_xyz_out [3 x total] the positions of every round, per cloud in round order, eval_round_counts_out [B * iterations]
+ * (cloud-major) the positions of each round (fewer than drawn when a proposal loop ran out); kept_offsets_out [B+1] and
+ * kept_xyz_out the positions of every sample that carried a VALID|FILTERED pose, the initial samples first, then the
+ * rounds, in sample order. The arrays are sized by the batch of that call. Returns B; GPDB_ERR_STATE when none ran, the
+ * last one failed, or a batch was installed since (gpdb_set_clouds[_device], gpdb_preprocess_clouds[_device]). */
+int gpdb_sis_positions(gpdb_ctx *ctx, int32_t *eval_offsets_out, int32_t *eval_round_counts_out, double *eval_xyz_out,
+                       int32_t *kept_offsets_out, double *kept_xyz_out);
+
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
  * back for the next call. A result may outlive its context. */

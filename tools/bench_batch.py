@@ -29,7 +29,13 @@ against batched (gpdb_preprocess_clouds, gpdb_detect_batch_select, gpdb_find_clu
 outside the timed region, that the two routes return identical records, and print per step the median wall time of each
 route and the samples/s of the whole route.
 
-    python tools/bench_batch.py [--sizes 1 16 64 256] [--reps 3] [--raw | --sis | --detect-full]
+--sis-device adds, in the same command and on the same views and initial samples, one gpdb_sis_batch_device call per step
+(the whole of cem_detect_grasps with its draws on the device, default SIS parameters, initial indices in a CUDA tensor) and
+prints its median wall time and samples/s (initial samples + evaluated round positions + classified kept positions) next
+to the --sis batch route. The two routes draw different round positions, so their records are not compared; the device
+call is checked once to equal gpdb_sis_batch bit for bit.
+
+    python tools/bench_batch.py [--sizes 1 16 64 256] [--reps 3] [--raw | --sis | --sis-device | --detect-full]
 """
 import argparse
 import ctypes as C
@@ -245,6 +251,31 @@ def sis_batch(ctx, clouds, init, rounds):
     return st.t, sum(len(k) for k in kept), list(zip(det, clusters))
 
 
+def sis_device(ctx, clouds, offsets, d_init):
+    """gpdb_set_clouds + one gpdb_sis_batch_device call: (wall time, samples evaluated, records on the device)."""
+    import torch
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()  # the install is timed, as the batch route's install step is
+    ctx.set_clouds(clouds)
+    rec, hoff, stats = ctx.sis_batch_tensors(offsets, d_init, min_inliers=MIN_INLIERS)
+    t = time.perf_counter() - t0
+    rounds = ctx.sis_positions()["round_counts"]
+    return t, int(offsets[-1]) + int(rounds.sum()) + stats["n_samples"], (rec, hoff)
+
+
+def sis_device_check(ctx, clouds, init):
+    """The device call's arguments, after the one check that it equals gpdb_sis_batch on the same views."""
+    import torch
+    offsets, idx = lib.pack_samples(init)
+    d_init = torch.from_numpy(idx).cuda()
+    ctx.set_clouds(clouds)
+    host = ctx.sis_batch(init, min_inliers=MIN_INLIERS)["hands"]
+    _, _, (rec, hoff) = sis_device(ctx, clouds, offsets, d_init)
+    recs = lib.poses_from_tensor(rec)
+    assert all(recs[hoff[b]:hoff[b + 1]].tobytes() == h.tobytes() for b, h in enumerate(host)), "device SIS != host SIS"
+    return offsets, d_init
+
+
 def full_loop(ctx, views, pp, samples):
     st, out = Steps(), []
     for v, s in zip(views, samples):
@@ -285,7 +316,7 @@ def main_steps(a, ctx, gpu):
         clouds = ctx.preprocess_clouds(views, pp)
         n = [len(c["xyz"]) for c in clouds]
         rng = np.random.default_rng(B)
-        if a.sis:
+        if a.sis or a.sis_device:
             init = [rng.choice(nb, min(SIS_INIT, nb), replace=False).astype(np.int32) for nb in n]
             # round positions of every view from one generator, shared by both routes: Gaussians around the initial
             # hand-set positions (70 %) and cloud points (30 %), as the default prob_rand_samples = 0.3 mixes them
@@ -310,13 +341,16 @@ def main_steps(a, ctx, gpu):
         _, kl, rl = loop(ctx, *args)
         _, kb, rb = batch(ctx, *args)
         assert kl == kb and same_records(rl, rb), "the loop and the batch route differ"
-        tl, tb = [], []
+        dev = sis_device_check(ctx, clouds, init) if a.sis_device else None
+        tl, tb, td = [], [], []
         for _ in range(a.reps):
             tl.append(loop(ctx, *args)[0])
             tb.append(batch(ctx, *args)[0])
+            if dev:
+                td.append(sis_device(ctx, clouds, *dev)[0])
         n_total = n_search + kl  # hand-search samples + classified positions (--sis)
         steps = list(tl[0])
-        line = {"mode": "sis" if a.sis else "detect_full", "B": B, "processed_points": int(sum(n)), "samples": n_total,
+        line = {"mode": "sis_device" if a.sis_device else "sis" if a.sis else "detect_full", "B": B, "processed_points": int(sum(n)), "samples": n_total,
                 "loop_ms": round(1e3 * med([sum(t.values()) for t in tl]), 2),
                 "batch_ms": round(1e3 * med([sum(t.values()) for t in tb]), 2),
                 "loop_sps": round(n_total / med([sum(t.values()) for t in tl])),
@@ -324,6 +358,9 @@ def main_steps(a, ctx, gpu):
                 "loop_steps_ms": {s: round(1e3 * med([t[s] for t in tl]), 2) for s in steps},
                 "batch_steps_ms": {s: round(1e3 * med([t[s] for t in tb]), 2) for s in steps},
                 "clusters": int(sum(len(c) for _, c in rb)), "gpu": gpu}
+        if dev:
+            n_dev = sis_device(ctx, clouds, *dev)[1]
+            line.update({"device_ms": round(1e3 * med(td), 2), "device_samples": n_dev, "device_sps": round(n_dev / med(td))})
         print(json.dumps(line), flush=True)
 
 
@@ -334,10 +371,11 @@ def main():
     mode = ap.add_mutually_exclusive_group()
     mode.add_argument("--raw", action="store_true", help="start from raw views: three preprocessing + detection routes")
     mode.add_argument("--sis", action="store_true", help="cem_detect_grasps' steps: per-view loop against batch calls")
+    mode.add_argument("--sis-device", action="store_true", help="--sis plus one gpdb_sis_batch_device call per step")
     mode.add_argument("--detect-full", action="store_true", help="detectGrasps from raw views: loop against batch calls")
     a = ap.parse_args()
     w, relu = weights()
-    if a.sis or a.detect_full:
+    if a.sis or a.sis_device or a.detect_full:
         ctx = lib.Context(lib.default_params(channels=15, relu_after_conv=relu))
         ctx.set_weights(w)
         main_steps(a, ctx, gpu_info())
