@@ -2282,15 +2282,18 @@ void gpdb_free_result(gpdb_result *r) {
   memset(r, 0, sizeof(*r));
 }
 
-int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]) {
+int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[32]) {
   if (!ctx) return GPDB_ERR_INVALID;
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  if (ctx->d_prof && cycles_out)
+  // slots 0..15: phase cycles and image events; 16..31: the path counters of gpdb_debug_path_counts (GPDB_PROF_PATH);
+  // 32..47: the shadow sub-phases and their events (GPDB_PROF_SUB), returned as cycles_out[16..31]
+  if (ctx->d_prof && cycles_out) {
     CUDA_TRY(cudaMemcpy(cycles_out, ctx->d_prof, sizeof(uint64_t) * 16, cudaMemcpyDeviceToHost));
-  // slots 0..15: phase cycles and image events; 16..31: the path counters of gpdb_debug_path_counts (GPDB_PROF_PATH)
-  if (enable && !ctx->d_prof) CUDA_TRY(cudaMalloc(&ctx->d_prof, sizeof(uint64_t) * 32));
-  if (enable) CUDA_TRY(cudaMemset(ctx->d_prof, 0, sizeof(uint64_t) * 32));
+    CUDA_TRY(cudaMemcpy(cycles_out + 16, ctx->d_prof + GPDB_PROF_SUB, sizeof(uint64_t) * 16, cudaMemcpyDeviceToHost));
+  }
+  if (enable && !ctx->d_prof) CUDA_TRY(cudaMalloc(&ctx->d_prof, sizeof(uint64_t) * GPDB_PROF_SLOTS));
+  if (enable) CUDA_TRY(cudaMemset(ctx->d_prof, 0, sizeof(uint64_t) * GPDB_PROF_SLOTS));
   if (!enable && ctx->d_prof) {
     cudaFree(ctx->d_prof);
     ctx->d_prof = nullptr;

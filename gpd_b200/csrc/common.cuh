@@ -136,6 +136,10 @@ struct CloudSet {
 // path counters (gpdb_debug_path_counts): d_prof[GPDB_PROF_PATH + e], counted only while the counters are on; the events
 // are listed in include/gpd_b200.h
 #define GPDB_PROF_PATH 16
+// sub-phase cycles and events of the shadow half of the image kernels: d_prof[GPDB_PROF_SUB + i], returned by
+// gpdb_debug_phase_cycles as cycles_out[16 + i] (the slots are listed in include/gpd_b200.h)
+#define GPDB_PROF_SUB 32
+#define GPDB_PROF_SLOTS 48
 enum PathEvent {
   PATH_FRAMES_T1, PATH_FRAMES_T2, PATH_HANDS_T2, PATH_HANDS_T3, PATH_HANDS_SLAB, PATH_IMG2_BOX, PATH_IMG2_NONUNIT, PATH_IMG_GL,
   PATH_IMG2_CAST, PATH_IMG2_DRAW, PATH_IMG2_STASH, PATH_IMG_CAST, PATH_IMG_DRAW, PATH_IMG_STASH, PATH_IMG_BALL
@@ -255,7 +259,7 @@ struct gpdb_ctx {
   void *scratch[SCR_N];
   size_t scratch_sz[SCR_N];
   int *d_err;
-  unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles, 32 slots: PATH_* below), nullptr = off
+  unsigned long long *d_prof;  // optional phase counters (gpdb_debug_phase_cycles, GPDB_PROF_SLOTS slots), nullptr = off
   int64_t launches;
   double last_ms[8];
   double pre_ms[6];   // gpdb_preprocess stage timings

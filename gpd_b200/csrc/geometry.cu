@@ -1360,6 +1360,15 @@ __device__ __noinline__ float dilated_min(const float *F, int S) {
       t_phase = now__;                                                  \
     }                                                                   \
   } while (0)
+// sub-phase timing of the shadow half (gpdb_debug_phase_cycles [16 + i]): thread 0 adds the cycles since t, restarts t
+__device__ __forceinline__ void sub_phase(unsigned long long *prof, int i, long long &t) {
+  if (prof && threadIdx.x == 0) {
+    const long long now = clock64();
+    atomicAdd(prof + GPDB_PROF_SUB + i, (unsigned long long)(now - t));
+    t = now;
+  }
+}
+enum SubPhase { SUB_CULL, SUB_WINDOW, SUB_EXPAND, SUB_CHANNELS, SUB_STASH, SUB_CLEARS, SUB_PROBE, SUB_EVT_SHARED };
 
 // ---- phases shared by the two image kernels (k_images, k_images2). Every function is called by all threads of the CTA
 // together unless it says otherwise.
@@ -1384,6 +1393,7 @@ __device__ __forceinline__ int warp_append(bool pred, int *counter) {
 template <class R, class E>
 __device__ __forceinline__ void warp_expand_bits(unsigned bits, unsigned code, R &&reserve, E &&emit) {
   const int lane = threadIdx.x & 31;
+  if (!__any_sync(0xffffffffu, bits != 0u)) return;  // most words of a bitmap are empty
   const int cnt = __popc(bits);
   int incl = cnt;
 #pragma unroll
@@ -1673,45 +1683,47 @@ __device__ __noinline__ void shadow_setup(const DevParams &P, const G &Gd, Sm &s
   const gpdb_pose &h = sm.h;
   const int tid = threadIdx.x;
   const double voxel = GPDB_SHADOW_VOXEL;
-  if (tid == 0) {
-    const double jmax = gmax * voxel * 0.3 + 1e-9;
+  if (tid < 32) {
     const double half_od = P.vol_w / 2.0;
-    double mn[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, mx[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
-    for (int cr = 0; cr < 8; cr++) {
+    // lane 3 cr + r (< 24): world coordinate r of box corner cr; lanes r < 3 then take the min / max over the corners in
+    // corner order
+    double wv = 0.0;
+    if (tid < 24) {
+      const int cr = tid / 3, r = tid - 3 * cr;
       double cx = (cr & 1) ? h.bottom + P.vol_d : h.bottom;
       double cy = (cr & 2) ? h.center + half_od : h.center - half_od;
       double cz = (cr & 4) ? P.vol_h : -P.vol_h;
-      for (int r = 0; r < 3; r++) {
-        double wv = h.frame[r] * cx + h.frame[3 + r] * cy + h.frame[6 + r] * cz + h.sample[r];
-        mn[r] = fmin(mn[r], wv);
-        mx[r] = fmax(mx[r], wv);
-      }
+      wv = h.frame[r] * cx + h.frame[3 + r] * cy + h.frame[6 + r] * cz + h.sample[r];
     }
-    for (int r = 0; r < 3; r++) {
-      int lo = (int)floor((mn[r] - jmax) * P.vox_mult) - 1;
-      int hi = (int)floor((mx[r] + jmax) * P.vox_mult) + 1;
-      sm.bm_org[r] = lo;
-      sm.bm_dims[r] = min(hi - lo + 1, P.bm_dim);
+    double mn = DBL_MAX, mx = -DBL_MAX;
+#pragma unroll
+    for (int cr = 0; cr < 8; cr++) {
+      const double v = __shfl_sync(0xffffffffu, wv, 3 * cr + tid % 3);
+      mn = fmin(mn, v);
+      mx = fmax(mx, v);
     }
-    // pre-test: float32 frame and sample, box widened by the jitter (gmax 0.0009 sqrt 3) + 2e-5 slack
-    for (int e = 0; e < 9; e++) sm.fR[e] = (float)h.frame[e];
-    for (int r = 0; r < 3; r++) sm.fs[r] = (float)h.sample[r];
-    const float jm = (float)(gmax * voxel * 0.3 * 1.7320508075688772 + 2e-5);
-    sm.fbx_lo[0] = (float)h.bottom - jm;
-    sm.fbx_lo[1] = (float)(h.center - P.vol_w / 2.0) - jm;
-    sm.fbx_lo[2] = (float)(-P.vol_h) - jm;
-    sm.fbx_hi[0] = (float)(h.bottom + P.vol_d) + jm;
-    sm.fbx_hi[1] = (float)(h.center + P.vol_w / 2.0) + jm;
-    sm.fbx_hi[2] = (float)P.vol_h + jm;
-    // slab cull: the image box in the hand frame, widened by voxel truncation (<= 0.003 sqrt 3) + jitter (<= gmax 0.0009
-    // sqrt 3), + 1e-5 for the float32 rounding of the cull
-    const double wm = 0.0105;
-    const double bx_lo[3] = {h.bottom - wm, h.center - P.vol_w / 2.0 - wm, -P.vol_h - wm};
-    const double bx_hi[3] = {h.bottom + P.vol_d + wm, h.center + P.vol_w / 2.0 + wm, P.vol_h + wm};
-    for (int a = 0; a < 3; a++) {
-      sm.cull_lo[a] = (float)bx_lo[a] - 1e-5f;
-      sm.cull_hi[a] = (float)bx_hi[a] + 1e-5f;
+    if (tid < 3) {
+      const int a = tid;
+      const double jmax = gmax * voxel * 0.3 + 1e-9;
+      int lo = (int)floor((mn - jmax) * P.vox_mult) - 1;
+      int hi = (int)floor((mx + jmax) * P.vox_mult) + 1;
+      sm.bm_org[a] = lo;
+      sm.bm_dims[a] = min(hi - lo + 1, P.bm_dim);
+      // pre-test: float32 frame and sample, box widened by the jitter (gmax 0.0009 sqrt 3) + 2e-5 slack
+      sm.fs[a] = (float)h.sample[a];
+      const float jm = (float)(gmax * voxel * 0.3 * 1.7320508075688772 + 2e-5);
+      sm.fbx_lo[a] = (a == 0 ? (float)h.bottom : a == 1 ? (float)(h.center - P.vol_w / 2.0) : (float)(-P.vol_h)) - jm;
+      sm.fbx_hi[a] = (a == 0 ? (float)(h.bottom + P.vol_d) : a == 1 ? (float)(h.center + P.vol_w / 2.0) : (float)P.vol_h) + jm;
+      // slab cull: the image box in the hand frame, widened by voxel truncation (<= 0.003 sqrt 3) + jitter (<= gmax
+      // 0.0009 sqrt 3), + 1e-5 for the float32 rounding of the cull
+      const double wm = 0.0105;
+      const double bx_lo = a == 0 ? h.bottom - wm : a == 1 ? h.center - P.vol_w / 2.0 - wm : -P.vol_h - wm;
+      const double bx_hi = a == 0 ? h.bottom + P.vol_d + wm : a == 1 ? h.center + P.vol_w / 2.0 + wm : P.vol_h + wm;
+      sm.cull_lo[a] = (float)bx_lo - 1e-5f;
+      sm.cull_hi[a] = (float)bx_hi + 1e-5f;
     }
+    if (tid < 9) sm.fR[tid] = (float)h.frame[tid];
+    if (tid == 0) sm.wl_n = 0;  // the work-list count of the first camera's casting
   }
   if (tid < Gd.K) {
     double s0 = sm.center[0] - Gd.vp[tid][0], s1 = sm.center[1] - Gd.vp[tid][1], s2 = sm.center[2] - Gd.vp[tid][2];
@@ -1831,12 +1843,12 @@ __device__ __forceinline__ void cast_camera(const DevParams &P, const G &Gd, con
                                             const CastLists &L, bool use_ball, int nball, BallAt &&ball_at,
                                             unsigned long long *prof, bool count_walks) {
   const int tid = threadIdx.x;
-  __syncthreads();
-  if (tid == 0) {
-    sm.wl_n = 0;
-    sm.dl_n = 0;
-  }
-  __syncthreads();
+  long long t_sub = 0;
+  if (prof && tid == 0) t_sub = clock64();
+  __syncthreads();  // the previous camera's lists have been read
+  // sm.wl_n is 0 on entry (shadow_setup, or the previous camera behind its window-test barrier); sm.dl_n, read by the
+  // previous camera before the barrier above, is first counted behind the append's barrier
+  if (tid == 0) sm.dl_n = 0;
   // appends the point to the work list; called by all 32 lanes together
   auto append = [&](bool ok, const float4 &p, unsigned rg) {
     const int pos = warp_append(ok, &sm.wl_n);
@@ -1875,6 +1887,7 @@ __device__ __forceinline__ void cast_camera(const DevParams &P, const G &Gd, con
     if (count_walks && prof && tid == 0) atomicAdd(prof + 14, 1ull);
   }
   __syncthreads();
+  sub_phase(prof, SUB_CULL, t_sub);
   const int nw = min(sm.wl_n, L.wl_cap);
   if (prof && tid == 0) {
     atomicAdd(prof + 9, (unsigned long long)nw);
@@ -1883,30 +1896,53 @@ __device__ __forceinline__ void cast_camera(const DevParams &P, const G &Gd, con
   const int nsp = P.nsp;
   const unsigned nsp_magic = nsp > 1 ? (unsigned)((0x100000000ull + (unsigned)nsp - 1) / (unsigned)nsp) : 0u;  // ceil(2^32 / nsp)
   const int nd = nw * nsp;
-  for (int w0 = 0; w0 < nd; w0 += NT_IMG) {  // window test of every draw, survivors compacted
-    const int w = w0 + tid;
-    bool pass = false;
-    unsigned code = 0, seed = 0;
-    if (w < nd) {
-      // w / nsp by multiply-high: exact for w < 2^32 / nsp (w < WL_CAP * nsp < 2^20)
-      const int item = nsp > 1 ? (int)__umulhi((unsigned)w, nsp_magic) : w, t = w - item * nsp;
-      seed = sm.lcgA[t] * __float_as_uint(L.wl[item].w) + sm.lcgC[t];
-      const unsigned rg = L.wrange[item];
-      const int r = (int)((seed >> 16) & 0x7FFFu);
-      pass = r >= (int)(rg & 0xFFFFu) && r <= (int)(rg >> 16);
-      code = ((unsigned)item << 7) | (unsigned)t;
+  // window test of every draw, survivors compacted: WT draws per thread between two slot reservations, so that a warp
+  // takes one scan and one shared-memory atomic per 32 WT draws (the loop was bound by that chain, not by the test)
+  constexpr int WT = 4;
+  const int lane = tid & 31;
+  for (int w0 = 0; w0 < nd; w0 += WT * NT_IMG) {
+    unsigned code[WT], pm = 0;
+#pragma unroll
+    for (int j = 0; j < WT; j++) {
+      const int w = w0 + j * NT_IMG + tid;
+      code[j] = 0;
+      if (w < nd) {
+        // w / nsp by multiply-high: exact for w < 2^32 / nsp (w < WL_CAP * nsp < 2^20)
+        const int item = nsp > 1 ? (int)__umulhi((unsigned)w, nsp_magic) : w, t = w - item * nsp;
+        const unsigned seed = sm.lcgA[t] * __float_as_uint(L.wl[item].w) + sm.lcgC[t];
+        const unsigned rg = L.wrange[item];
+        const int r = (int)((seed >> 16) & 0x7FFFu);
+        if (r >= (int)(rg & 0xFFFFu) && r <= (int)(rg >> 16)) pm |= 1u << j;
+        code[j] = ((unsigned)item << 7) | (unsigned)t;
+      }
     }
-    const int pos = warp_append(pass, &sm.dl_n);
-    if (pass) {
-      if (pos < L.dl_cap) L.dlist[pos] = code;
+    const int cnt = __popc(pm);
+    int incl = cnt;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    int pos = 0;
+    if (lane == 31 && incl) pos = atomicAdd(&sm.dl_n, incl);
+    pos = __shfl_sync(0xffffffffu, pos, 31) + incl - cnt;
+#pragma unroll
+    for (int j = 0; j < WT; j++) {
+      if (!((pm >> j) & 1u)) continue;
+      if (pos < L.dl_cap) L.dlist[pos] = code[j];
       else {  // list full: evaluate in place
-        const float4 e = L.wl[code >> 7];
+        const float4 e = L.wl[code[j] >> 7];
+        const int t = (int)(code[j] & 127u);
+        const unsigned seed = sm.lcgA[t] * __float_as_uint(e.w) + sm.lcgC[t];
         set_bit(bm, draw_bit(P, sm, vb, (double)e.x, (double)e.y, (double)e.z, seed, k));
       }
+      pos++;
     }
   }
   __syncthreads();
+  sub_phase(prof, SUB_WINDOW, t_sub);
   const int ndl = min(sm.dl_n, L.dl_cap);
+  if (tid == 0) sm.wl_n = 0;  // for the next camera: every read of this camera's count lies before the barrier above
   if (prof && tid == 0) {
     atomicAdd(prof + 10, (unsigned long long)sm.dl_n);
     if (sm.dl_n > L.dl_cap) atomicAdd(prof + GPDB_PROF_PATH + L.path_draw, (unsigned long long)(sm.dl_n - L.dl_cap));
@@ -1940,10 +1976,11 @@ __device__ __forceinline__ void intersect_bitmaps(unsigned *bitmap, int bm_words
 
 // One shadow voxel (code b0 | b1 << 8 | b2 << 16 in the bitmap AABB): the exact float64 box test of its jittered point,
 // then its entry into the sum tiles of projections [pj_lo, pj_hi) (tile pj - pj_lo, S S cells each). Returns projection
-// 2's entry (cell | 1 << 31, fixed-point coordinate), zero when the point lies outside the box.
+// 2's entry (cell | 1 << 31, fixed-point coordinate), zero when the point lies outside the box. evt (may be null) counts
+// the entries whose cell another active lane of the warp hits in the same update.
 __device__ __forceinline__ uint2 eval_voxel(const DevParams &P, const gpdb_pose &h, const double *qtab, const double (&inv)[3],
                                             int S, const VoxelBox &vb, unsigned long long *tiles, unsigned code, int pj_lo,
-                                            int pj_hi) {
+                                            int pj_hi, unsigned long long *evt = nullptr) {
   int b0 = code & 255, b1 = (code >> 8) & 255, b2 = code >> 16;
   double x, y, z;
   if (!voxel_point_in_box(P, h, qtab, b0 + vb.o0, b1 + vb.o1, b2 + vb.o2, x, y, z)) return make_uint2(0u, 0u);
@@ -1956,7 +1993,10 @@ __device__ __forceinline__ uint2 eval_voxel(const DevParams &P, const gpdb_pose 
     const Proj pr(pj);
     const int pix = (S - 1 - cellv[pr.a0]) * S + cellv[pr.a1];
     const unsigned qv = unit_q32(u[pr.a2]);
-    if (pj >= pj_lo && pj < pj_hi) cell_add(tiles + (size_t)(pj - pj_lo) * S * S + pix, qv);
+    if (pj >= pj_lo && pj < pj_hi) {
+      if (evt && __popc(__match_any_sync(__activemask(), pj * S * S + pix)) > 1) atomicAdd(evt, 1ull);
+      cell_add(tiles + (size_t)(pj - pj_lo) * S * S + pix, qv);
+    }
     if (pj == 2) st = make_uint2((unsigned)pix | 0x80000000u, qv);
   }
   return st;
@@ -2364,7 +2404,7 @@ template <bool BATCH>
 __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevCloud cl0, CloudTable tab, const gpdb_pose *cand, int nc,
                                                        uint8_t *p16, const double *qtab, int *ovf, int *ovf_count,
                                                        unsigned long long *prof) {
-  long long t_phase = 0;
+  long long t_phase = 0, t_sub = 0;
   const DevParams &P = *Pp;
   extern __shared__ __align__(16) unsigned char dyn[];
   __shared__ Img2Smem sm;
@@ -2501,19 +2541,29 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
       }
       __syncthreads();
       PHASE(5);
+      t_sub = t_phase;
       intersect_bitmaps(bitmap, bm_words, K, cam_set);
       for (int k = tid; k < SS; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);  // tiles A, B
       if (tid == 0) sm.wl_n = 0;
       __syncthreads();
       // voxel list (8 B per voxel behind the bitmaps): .x = voxel code, later the stash for projection 2
       const int nbits = 64 * vb.d1 * vb.d2;
+      // continued past the shared memory in the image's HBM slot, over the in-ball list (dead once the casting is done)
       uint2 *stash = reinterpret_cast<uint2 *>(bitmap + (((size_t)bm_words * (K > 1 ? K : 1) + 1) & ~(size_t)1));
-      const int ST_CAP = (LIST_BYTES - (int)((reinterpret_cast<unsigned char *>(stash)) - lbase)) / 8;
+      const int ST_SM = (LIST_BYTES - (int)((reinterpret_cast<unsigned char *>(stash)) - lbase)) / 8;
+      uint2 *gstash = reinterpret_cast<uint2 *>(ball);
+      const int ST_CAP = ST_SM + BALL_CAP2 / 2;
+      auto st_put = [&](int i, uint2 v) {
+        if (i < ST_SM) stash[i] = v;
+        else __stcg(gstash + (i - ST_SM), v);
+      };
+      auto st_get = [&](int i) -> uint2 { return i < ST_SM ? stash[i] : __ldcg(gstash + (i - ST_SM)); };  // L2, not L1
       expand_bitmap(bitmap, nbits, vb.d1, &sm.wl_n, [&](int pos, unsigned code) {
-        if (pos < ST_CAP) stash[pos].x = code;
+        if (pos < ST_CAP) st_put(pos, make_uint2(code, 0u));
         else eval_voxel(P, h, qtab, inv, S, vb, tileA, code, 0, 2);  // list full: projections 0 and 1 in place (2: second walk below)
       });
       __syncthreads();
+      sub_phase(prof, SUB_EXPAND, t_sub);
       const int nset_all = sm.wl_n, nset = min(nset_all, ST_CAP);
       if (prof && tid == 0) {
         atomicAdd(prof + 11, (unsigned long long)nset_all);
@@ -2521,19 +2571,24 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         atomicAdd(prof + 13, (unsigned long long)sm.n_img);
         if (nset_all > ST_CAP) atomicAdd(prof + GPDB_PROF_PATH + PATH_IMG2_STASH, 1ull);
       }
-      for (int i = tid; i < nset; i += NT_IMG) stash[i] = eval_voxel(P, h, qtab, inv, S, vb, tileA, stash[i].x, 0, 2);
+      unsigned long long *evt = prof ? prof + GPDB_PROF_SUB + SUB_EVT_SHARED : nullptr;
+      for (int i = tid; i < nset; i += NT_IMG) st_put(i, eval_voxel(P, h, qtab, inv, S, vb, tileA, st_get(i).x, 0, 2, evt));
       __syncthreads();
       PHASE(6);
+      t_sub = t_phase;
       shadow_channel(sm, rcp, S, tileA, splanes, S);
       shadow_channel(sm, rcp, S, tileB, splanes + PLB, S);
       __syncthreads();
+      sub_phase(prof, SUB_CHANNELS, t_sub);
       for (int k = tid; k < SS / 2; k += NT_IMG) reinterpret_cast<uint4 *>(tileA)[k] = make_uint4(0, 0, 0, 0);  // tile A
       __syncthreads();
+      sub_phase(prof, SUB_CLEARS, t_sub);
       // projection 2: from the stash, or — when the voxel list overflowed — by a second walk over the whole bitmap
       if (nset_all <= ST_CAP) {
         for (int i = tid; i < nset; i += NT_IMG) {
-          const uint2 st = stash[i];
+          const uint2 st = st_get(i);
           if (st.x & 0x80000000u) {
+            if (evt && __popc(__match_any_sync(__activemask(), st.x)) > 1) atomicAdd(evt, 1ull);
             const bool carry = cell_add(tileA + (st.x & 0x7fffffffu), st.y);
             if (prof && carry) atomicAdd(prof + 0, 1ull);
           }
@@ -2542,17 +2597,21 @@ __global__ void __launch_bounds__(NT_IMG, 2) k_images2(const DevParams *Pp, DevC
         expand_bitmap(bitmap, nbits, vb.d1, nullptr, [&](int, unsigned code) { eval_voxel(P, h, qtab, inv, S, vb, tileA, code, 2, 3); });
       }
       __syncthreads();
+      sub_phase(prof, SUB_STASH, t_sub);
       if (prof) {  // the most shadow voxels summed into one cell of projection 2
         unsigned most = 0;
         for (int k = tid; k < SS; k += NT_IMG) most = max(most, (unsigned)(tileA[k] >> 48));
         most = __reduce_max_sync(0xffffffffu, most);
         if ((tid & 31) == 0 && most) atomicMax(prof + 1, (unsigned long long)most);
       }
+      sub_phase(prof, SUB_PROBE, t_sub);
       shadow_channel(sm, rcp, S, tileA, splanes + 2 * PLB, S);
       __syncthreads();
+      sub_phase(prof, SUB_CHANNELS, t_sub);
       for (int k = tid; k < MAXPIX / 32; k += NT_IMG) sm.occf[k] = 0u;
     }
     __syncthreads();
+    if (C == 15) sub_phase(prof, SUB_CLEARS, t_sub);
     PHASE(7);
     // ---- the point planes come back from the image's memory into the dead tiles, then dilation + pixel assembly
     for (int k = tid; k < (npp * PLB) >> 4; k += NT_IMG)

@@ -767,7 +767,7 @@ class Context:
         return out
 
     def phase_cycles(self, enable=1):
-        out = np.zeros(16, np.uint64)
+        out = np.zeros(32, np.uint64)
         self._check(lib().gpdb_debug_phase_cycles(self.h, enable, _p(out)))
         return out
 

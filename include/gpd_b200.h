@@ -533,8 +533,13 @@ int gpdb_last_timings(const gpdb_ctx *ctx, double ms_out[8]);
  * counters accumulated so far: [2] ball scan, [3] point channels, [4] shadow setup, [5] shadow casting,
  * [6] shadow bitmap pass, [7] shadow channels, [8] output flush. Event counts of the fast image kernel: [0] shadow
  * cell-sum entries of projection 2 whose low word carried, [1] the most shadow voxels summed into one cell of
- * projection 2, [14] shadow casts that walked the grid because the in-ball list was full. */
-int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[16]);
+ * projection 2, [14] shadow casts that walked the grid because the in-ball list was full. Sub-phases of the shadow
+ * (cycles as above; the draw evaluation is [5] - [16] - [17], the voxel evaluation [6] - [18]): [16] casting: cull +
+ * work-list append (both image kernels), [17] casting: window test (both); k_images2: [18] voxel pass: bitmap
+ * intersection + expansion, [19] the shadow_channel passes, [20] the projection-2 stash sum, [21] the tile clears,
+ * [22] the scan behind [1] (only while the counters are on); [23] event: shadow cell-sum entries whose cell another
+ * active lane of the same warp hits in the same update. */
+int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[32]);
 /* Development aid: how often the geometry kernels left their first choice of list for a larger tier or an in-place
  * fallback, counted while gpdb_debug_phase_cycles(ctx, 1, ...) has the counters enabled (summed since then; all zero when
  * they are off). counts_out receives:
