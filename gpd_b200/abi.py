@@ -145,6 +145,18 @@ class SisParams(C.Structure):
     ]
 
 
+# Argument types of the device-resident calls that take sample positions, return every hand and make and classify grasp
+# images from device memory (include/gpd_b200.h, "device-resident batches"); every one returns int. Pointers are
+# c_void_p (host or device addresses), the result is a gpdb_result *.
+RESIDENT_PROTOTYPES = {
+    "gpdb_set_clouds_samples_device": [C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_hand_search_batch_device": [C.c_void_p] * 6 + [C.POINTER(Result)],
+    "gpdb_detect_batch_device": [C.c_void_p] * 7 + [C.POINTER(Result)],
+    "gpdb_images_batch_device": [C.c_void_p] * 4,
+    "gpdb_classify_device": [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
+}
+
+
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""
     p = PreprocessParams()

@@ -916,37 +916,66 @@ int gpdb_set_samples(gpdb_ctx *ctx, const double *samples, int32_t n) {
   return rc < 0 ? rc : s.points();  // the first sample index that addresses samples[0]
 }
 
-int gpdb_set_clouds_samples(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *samples) {
+}  // extern "C"
+
+// gpdb_set_clouds_samples[_device]: `name` is the entry point the errors name; device: samples is a device array, copied
+// device to device into the store's sample arena
+static int set_clouds_samples(gpdb_ctx *ctx, const char *name, const int32_t *pos_offsets, const double *samples,
+                              bool device) {
   if (!ctx) return GPDB_ERR_INVALID;
   CloudSet &s = ctx->many;
   s.n_samples = 0;  // past this point, a failed call leaves no positions behind
   if (!s.n) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_set_clouds_samples: no batch of clouds: call gpdb_set_clouds / "
-                   "gpdb_preprocess_clouds first");
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first", name);
     return GPDB_ERR_STATE;
   }
   const int B = s.n;
   if (!pos_offsets || pos_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: need pos_offsets[%d] starting at 0", B + 1);
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need pos_offsets[%d] starting at 0", name, B + 1);
     return GPDB_ERR_INVALID;
   }
   for (int b = 0; b < B; b++)
     if (pos_offsets[b + 1] < pos_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: pos_offsets decrease at cloud %d", b);
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: pos_offsets decrease at cloud %d", name, b);
       return GPDB_ERR_INVALID;
     }
   const int M = pos_offsets[B];
   if (M > 0 && !samples) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_set_clouds_samples: null samples_xyz for %d positions", M);
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null samples_xyz for %d positions", name, M);
     return GPDB_ERR_INVALID;
+  }
+  if (device) {
+    const char *names[1] = {"d_samples_xyz"};
+    const void *ptrs[1] = {samples};
+    const int rc = check_device_ptrs(ctx, name, 1, names, ptrs);
+    if (rc != GPDB_OK) return rc;
   }
   memcpy(s.pos, pos_offsets, sizeof(int) * ((size_t)B + 1));
   // each descriptor's first position: one strided copy into the pos field of the B device descriptors
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaMemcpy2DAsync(&s.desc[0].pos, sizeof(CloudDesc), s.pos, sizeof(int), sizeof(int), (size_t)B,
                              cudaMemcpyHostToDevice, ctx->stream));
-  const int rc = upload_samples(ctx, s, samples, M);
-  return rc < 0 ? rc : M;
+  if (!device) {
+    const int rc = upload_samples(ctx, s, samples, M);
+    return rc < 0 ? rc : M;
+  }
+  const int rc = reserve_samples(ctx, s, M);
+  if (rc != GPDB_OK) return rc;
+  if (M > 0)
+    CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)M, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  s.n_samples = M;
+  return M;
+}
+
+extern "C" {
+
+int gpdb_set_clouds_samples(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *samples) {
+  return set_clouds_samples(ctx, "gpdb_set_clouds_samples", pos_offsets, samples, false);
+}
+
+int gpdb_set_clouds_samples_device(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *d_samples_xyz) {
+  return set_clouds_samples(ctx, "gpdb_set_clouds_samples_device", pos_offsets, d_samples_xyz, true);
 }
 
 int gpdb_get_cloud(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out) {
@@ -1118,7 +1147,8 @@ int check_device_errors(gpdb_ctx *ctx) {
 
 // The chunked device pipeline behind the detect and hand-search entry points, single cloud, batch and sharded; the request
 // (PipeRequest, common.cuh) says where the samples are and where the results go. With device samples and a destination on
-// the device nothing but the per-chunk candidate count crosses PCIe. A selecting call (PIPE_TOP_*) keeps the classified
+// the device nothing but the per-chunk candidate count (and for PIPE_ALL_CALLER the per-cloud offsets) crosses PCIe. A
+// selecting call (PIPE_TOP_*) keeps the classified
 // candidates of all chunks on the device, sorts the select_k best out there and delivers only them; no per-sample /
 // per-pose array is returned.
 //
@@ -1316,6 +1346,9 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out) {
       }
       PIPE_CUDA(cudaMemcpyAsync(ctx->d_sel + (total_nc - nc), d_cand[b], sizeof(gpdb_pose) * (size_t)nc, cudaMemcpyDeviceToDevice, ctx->stream));
     }
+    if (nc > 0 && rq.dest == PIPE_ALL_CALLER)  // the caller's buffer holds n * P records: no growth, ordered as above
+      PIPE_CUDA(cudaMemcpyAsync(rq.d_selected + (total_nc - nc), d_cand[b], sizeof(gpdb_pose) * (size_t)nc,
+                                cudaMemcpyDeviceToDevice, ctx->stream));
     if (overlap) {
       PIPE_CUDA(cudaEventRecord(ps.ev_consumed[b], main_stream));
       cand_consumed[b] = true;
@@ -1370,6 +1403,10 @@ int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out) {
       PIPE_TRY(geo_select(ctx, ctx->d_sel, total_nc, n_sel, d_top));
       PIPE_CUDA(cudaMemcpyAsync(ar->buf[1], d_top, sizeof(gpdb_pose) * (size_t)n_sel, cudaMemcpyDeviceToHost, ctx->stream));
     }
+  } else if (rq.dest == PIPE_ALL_CALLER) {
+    // the per-cloud offsets are found on the stream slots; then the slots are made cloud-local in place
+    PIPE_TRY(geo_batch_cand_off(ctx, s, rq.d_selected, total_nc, s.sel));
+    PIPE_TRY(batch_local_slots(ctx, rq.d_selected, total_nc, s.soff, s.n, rq.d_selected));
   }
   gpdb_st_end(ctx, 4, t_all);
   rc = finish(total_nc);
@@ -1565,10 +1602,12 @@ namespace {
 // gpdb_detect_batch / gpdb_detect_batch_select / gpdb_hand_search_batch: checks the CSR sample lists against the installed
 // batch and runs them as ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back
 // with cloud-local sample slots, grouped by cloud (offsets_out). Only the classifying calls (with_images_and_scores) need
-// weights. device (gpdb_detect_batch_select_device): sample_idx and sel_out are device arrays, the sample lists are checked
-// on the device and the selection stays there.
+// weights. device (gpdb_*_batch*_device): sample_idx and sel_out are device arrays, the sample lists are checked on the
+// device and the records stay there: the selection (select_k >= 0), or every record (select_k < 0, PIPE_ALL_CALLER) with the
+// dense flags / scores in the caller's d_flags / d_scores when those are given. sel_name names sel_out in the messages.
 int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out, int32_t *offsets_out,
-              bool with_images_and_scores, int select_k, const char *name, bool device = false, gpdb_pose *sel_out = nullptr) {
+              bool with_images_and_scores, int select_k, const char *name, bool device = false, gpdb_pose *sel_out = nullptr,
+              const char *sel_name = "d_selected_out", uint8_t *d_flags = nullptr, float *d_scores = nullptr) {
   int rc = gpdb_check_state(ctx, false, with_images_and_scores);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
@@ -1592,13 +1631,13 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
     return GPDB_ERR_INVALID;
   }
   if (device) {
-    if (n > 0 && select_k > 0 && !sel_out) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_selected_out", name);
+    if (n > 0 && select_k != 0 && !sel_out) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, sel_name);
       return GPDB_ERR_INVALID;
     }
-    const char *names[2] = {"d_sample_idx", "d_selected_out"};
-    const void *ptrs[2] = {sample_idx, sel_out};
-    if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+    const char *names[4] = {"d_sample_idx", sel_name, "d_flags_out", "d_scores_out"};
+    const void *ptrs[4] = {sample_idx, sel_out, d_flags, d_scores};
+    if ((rc = check_device_ptrs(ctx, name, 4, names, ptrs)) != GPDB_OK) return rc;
   } else {
     for (int b = 0; b < B; b++) {
       const int nb = s.off[b + 1] - s.off[b], mb = s.positions(b);  // N_b points, then M_b positions
@@ -1632,12 +1671,12 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
     }
   }
   PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = device, .per_cloud = true,
-                    .classify = with_images_and_scores,
-                    .dest = select_k < 0 ? PIPE_TO_HOST : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
+                    .classify = with_images_and_scores, .d_flags = d_flags, .d_scores = d_scores,
+                    .dest = select_k < 0 ? (device ? PIPE_ALL_CALLER : PIPE_TO_HOST) : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
                     .select_k = select_k, .d_selected = sel_out};
   rc = gpdb_run_pipeline(ctx, rq, out);
   if (rc < 0) return rc;
-  if (select_k >= 0) {  // the pipeline has made the selected records' sample slots cloud-local
+  if (rq.dest != PIPE_TO_HOST) {  // the pipeline has made the records' sample slots cloud-local
     memcpy(offsets_out, s.sel, sizeof(int) * ((size_t)B + 1));
   } else {  // sample slots are positions in the whole stream on the device: make them cloud-local, as a single-cloud call has them
     int b = 0;
@@ -1691,6 +1730,77 @@ int gpdb_detect_batch_select_device(gpdb_ctx *ctx, const int32_t *sample_offsets
   }
   return run_batch(ctx, sample_offsets, d_sample_idx, stats, sel_offsets_out, true, num_selected,
                    "gpdb_detect_batch_select_device", true, d_selected_out);
+}
+
+int gpdb_hand_search_batch_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx,
+                                  uint8_t *d_flags_out, gpdb_pose *d_hands_out, int32_t *cand_offsets_out, gpdb_result *stats) {
+  if (ctx && !cand_offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_hand_search_batch_device: null cand_offsets_out");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, d_sample_idx, stats, cand_offsets_out, false, -1, "gpdb_hand_search_batch_device",
+                   true, d_hands_out, "d_hands_out", d_flags_out);
+}
+
+int gpdb_detect_batch_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx, uint8_t *d_flags_out,
+                             float *d_scores_out, gpdb_pose *d_candidates_out, int32_t *cand_offsets_out, gpdb_result *stats) {
+  if (ctx && !cand_offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_detect_batch_device: null cand_offsets_out");
+    return GPDB_ERR_INVALID;
+  }
+  return run_batch(ctx, sample_offsets, d_sample_idx, stats, cand_offsets_out, true, -1, "gpdb_detect_batch_device", true,
+                   d_candidates_out, "d_candidates_out", d_flags_out, d_scores_out);
+}
+
+// ImageGenerator::createImages for given hands of the installed batch. The image kernels find a record's cloud from its
+// sample slot through the store's soff (CloudSel<true>); here soff holds the hand offsets and every hand is copied into
+// the candidate scratch with its position in d_hands as its slot (batch_image_hands), so hand j is imaged against the cloud
+// whose group holds it. That slot is the only record field the image kernels index memory with; sample, frame and box only
+// feed arithmetic, and sample_index seeds the shadow draws as in gpdb_detect_batch. Every batch call uploads its own
+// offsets to soff before it reads them, so borrowing soff here leaves nothing behind. A batch of one runs the one-cloud
+// kernels, as gpdb_detect_batch does.
+int gpdb_images_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, const gpdb_pose *d_hands, uint8_t *d_images_out) {
+  const char *name = "gpdb_images_batch_device";
+  int rc = gpdb_check_state(ctx, false, false);
+  if (rc != GPDB_OK) return rc;
+  CloudSet &s = ctx->many;
+  if (s.n == 0) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds first", name);
+    return GPDB_ERR_STATE;
+  }
+  const int B = s.n;
+  if (!hand_offsets || hand_offsets[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need hand_offsets[%d] starting at 0", name, B + 1);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++)
+    if (hand_offsets[b + 1] < hand_offsets[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: hand_offsets decrease at cloud %d", name, b);
+      return GPDB_ERR_INVALID;
+    }
+  const int n = hand_offsets[B];
+  if (n > 0 && (!d_hands || !d_images_out)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands or d_images_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  const char *names[2] = {"d_hands", "d_images_out"};
+  const void *ptrs[2] = {d_hands, d_images_out};
+  if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+  if (n == 0) return 0;
+  CUDA_TRY(cudaMemcpyAsync(s.soff, hand_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  const size_t isz = (size_t)ctx->hp.S * ctx->hp.S * ctx->hp.C, psz = (size_t)ctx->hp.S * ctx->hp.S * 16;
+  const int batch = ctx->prm.batch_size > 0 ? ctx->prm.batch_size : 8192;
+  for (int b0 = 0; b0 < n; b0 += batch) {
+    const int bn = std::min(batch, n - b0);
+    gpdb_pose *d_cand = (gpdb_pose *)gpdb_scratch(ctx, SCR_CAND, sizeof(gpdb_pose) * (size_t)bn);
+    uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, SCR_P16, psz * (size_t)bn);
+    if (!d_cand || !d_p16) return GPDB_ERR_CUDA;
+    if ((rc = batch_image_hands(ctx, d_hands + b0, bn, b0, d_cand)) != GPDB_OK) return rc;
+    if ((rc = geo_images(ctx, s, d_cand, bn, d_p16)) != GPDB_OK) return rc;
+    if ((rc = geo_p16_to_hwc(ctx, d_p16, bn, d_images_out + isz * (size_t)b0)) != GPDB_OK) return rc;
+  }
+  if ((rc = check_device_errors(ctx)) != GPDB_OK) return rc;  // drains the stream
+  return n;
 }
 
 int gpdb_set_overlap(gpdb_ctx *ctx, int32_t enable) {
@@ -1774,11 +1884,25 @@ namespace {
 
 // The classify loop of gpdb_classify and gpdb_debug_lenet_layers: HWC -> P16 and lenet_forward in batches of batch_size.
 // scores_out / logits_out may be null; layers (null for gpdb_classify) receives every layer's output at offset b0.
+// device (gpdb_classify_device): images and outputs are device arrays; the images are converted in place and LeNet writes
+// the outputs directly, with one synchronisation at the end.
 int classify_batches(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *scores_out, float *logits_out,
-                     const LenetLayers *layers) {
+                     const LenetLayers *layers, bool device = false) {
   int rc;
   const size_t isz = (size_t)ctx->hp.S * ctx->hp.S * ctx->hp.C, psz = (size_t)ctx->hp.S * ctx->hp.S * 16;
   const int batch = ctx->prm.batch_size > 0 ? ctx->prm.batch_size : 8192;
+  if (device) {
+    for (int b0 = 0; b0 < n; b0 += batch) {
+      const int bn = std::min(batch, n - b0);
+      uint8_t *d_p16 = (uint8_t *)gpdb_scratch(ctx, SCR_P16, psz * (size_t)bn);
+      if (!d_p16) return GPDB_ERR_CUDA;
+      if ((rc = geo_hwc_to_p16(ctx, images_hwc + isz * (size_t)b0, bn, d_p16)) != GPDB_OK) return rc;
+      if ((rc = lenet_forward(ctx, d_p16, bn, scores_out + b0, logits_out ? logits_out + 2 * (size_t)b0 : nullptr)) != GPDB_OK)
+        return rc;
+    }
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return n;
+  }
   for (int b0 = 0; b0 < n; b0 += batch) {
     const int bn = std::min(batch, n - b0);
     uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz * (size_t)bn);
@@ -1813,6 +1937,20 @@ int gpdb_classify(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *sc
     return GPDB_ERR_INVALID;
   }
   return classify_batches(ctx, images_hwc, n, scores_out, logits_out, nullptr);
+}
+
+int gpdb_classify_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, int32_t n, float *d_scores_out, float *d_logits_out) {
+  const char *name = "gpdb_classify_device";
+  int rc = gpdb_check_state(ctx, false, true);
+  if (rc != GPDB_OK) return rc;
+  if (n < 0 || (n > 0 && (!d_images_hwc || !d_scores_out))) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: bad arguments", name);
+    return GPDB_ERR_INVALID;
+  }
+  const char *names[3] = {"d_images_hwc", "d_scores_out", "d_logits_out"};
+  const void *ptrs[3] = {d_images_hwc, d_scores_out, d_logits_out};
+  if ((rc = check_device_ptrs(ctx, name, 3, names, ptrs)) != GPDB_OK) return rc;
+  return classify_batches(ctx, d_images_hwc, n, d_scores_out, d_logits_out, nullptr, true);
 }
 
 int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *pool1_out, double *pool2_out,

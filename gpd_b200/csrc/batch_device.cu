@@ -1,5 +1,6 @@
 // batch_device.cu — kernels of the device-resident batch entry points (gpdb_*_device, api.cu): camera-mask packing, the
-// finiteness and sample-index checks, and cloud-local sample slots of selected records. The checks write the lowest
+// finiteness and sample-index checks, cloud-local sample slots of records, and the caller's hands made addressable by the
+// image kernels. The checks write the lowest
 // offending position (atomicMin into a word the caller set to all ones), so that their error messages name what the
 // host loops of the host entry points name.
 #include <algorithm>
@@ -55,6 +56,16 @@ __global__ void k_local_slots(const gpdb_pose *in, int n, const int *soff, int B
   out[j] = p;
 }
 
+// the caller's hands as the image kernels address them: sample slot = the hand's position in the caller's array, which
+// the hand offsets (uploaded as the store's soff) assign to its cloud. No other field of a record indexes memory there.
+__global__ void k_image_hands(const gpdb_pose *in, int n, int base, gpdb_pose *out) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  gpdb_pose p = in[j];
+  p.sample_slot = base + j;
+  out[j] = p;
+}
+
 }  // namespace
 
 #define LAUNCH_CHECK()                                                                                    \
@@ -96,6 +107,13 @@ int batch_check_samples(gpdb_ctx *ctx, const int *d_sidx, int n, const int *d_so
 int batch_local_slots(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, const int *d_soff, int B, gpdb_pose *d_out) {
   if (n == 0) return GPDB_OK;
   k_local_slots<<<(n + 127) / 128, 128, 0, ctx->stream>>>(d_in, n, d_soff, B, d_out);
+  LAUNCH_CHECK();
+  return GPDB_OK;
+}
+
+int batch_image_hands(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, int base, gpdb_pose *d_out) {
+  if (n == 0) return GPDB_OK;
+  k_image_hands<<<(n + 127) / 128, 128, 0, ctx->stream>>>(d_in, n, base, d_out);
   LAUNCH_CHECK();
   return GPDB_OK;
 }

@@ -113,9 +113,10 @@ struct CloudSet {
   int *src;             // cloud-local raw index of each point (valid after preprocessing: has_src)
   int *cell_start;
   CloudDesc *desc;      // [n] on the device
-  int *soff;            // [n + 1] sample offsets of the running batch call (device)
+  int *soff;            // [n + 1] sample offsets of the running batch call (device; the hand offsets of
+                        // gpdb_images_batch_device)
   int *off;             // [n + 1] point offsets (host)
-  int *sel;             // [n + 1] per-cloud offsets of the last batch selection (host)
+  int *sel;             // [n + 1] per-cloud offsets of the records the last batch call left on the device (host)
   int *pos;             // [n + 1] per-cloud offsets of the sample positions while n_samples > 0 (host; the batch only)
   size_t point_cap, cell_cap, desc_cap;
   int n, maxk;          // clouds installed, largest camera count
@@ -286,7 +287,9 @@ enum PipeDest {
   PIPE_TOP_HOST,     // the select_k best records (per_cloud: of every cloud, sample slots cloud-local) to the host arena
   PIPE_TOP_DEVICE,   // the same selection of a per_cloud call to d_selected on the device; nothing to the host
   PIPE_STAY,         // nothing leaves the device: the caller reads the dense flags and scores there
-  PIPE_ALL_DEVICE    // PIPE_STAY, and every scored candidate record stays in ctx->d_sel (sample-slot order, stream slots)
+  PIPE_ALL_DEVICE,   // PIPE_STAY, and every scored candidate record stays in ctx->d_sel (sample-slot order, stream slots)
+  PIPE_ALL_CALLER    // every candidate record of a per_cloud call to d_selected (room for n * P), grouped by cloud with
+                     // cloud-local sample slots; store->sel (host) receives the per-cloud offsets
 };
 // One call of the chunked device pipeline (see api.cu): where its inputs are and where its outputs go.
 struct PipeRequest {
@@ -301,7 +304,7 @@ struct PipeRequest {
   float *d_scores;            // the pipeline's scratch. Out: the arrays that were used, valid until the next call
   PipeDest dest;
   int select_k;               // PIPE_TOP_*: records to keep (per cloud when per_cloud)
-  gpdb_pose *d_selected;      // PIPE_TOP_DEVICE: receives them
+  gpdb_pose *d_selected;      // PIPE_TOP_DEVICE, PIPE_ALL_CALLER: receives them
   int slot_base;              // added to every sample_slot (rank offset of a sharded call)
 };
 int gpdb_run_pipeline(gpdb_ctx *ctx, PipeRequest &rq, gpdb_result *out);
@@ -343,6 +346,9 @@ int batch_check_samples(gpdb_ctx *ctx, const int *d_sidx, int n, const int *d_so
                         unsigned long long *d_first_bad);
 // d_out[j] = d_in[j] with its sample slot made local to the cloud whose slots d_soff assigns it (d_in may equal d_out)
 int batch_local_slots(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, const int *d_soff, int B, gpdb_pose *d_out);
+// d_out[j] = d_in[j] with sample slot base + j: the image kernels then find hand j's cloud from the hand offsets held in
+// the store's soff (gpdb_images_batch_device)
+int batch_image_hands(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, int base, gpdb_pose *d_out);
 
 // sis.cu (gpdb_sis_batch, include/gpd_b200_sis.h). Per cloud b of a batch with R rounds of S positions and initial
 // offsets init_off[B+1] (device), the kept arena holds room for init_off[b+1] - init_off[b] + R*S positions from position
@@ -378,6 +384,9 @@ int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s);
 // filled) -> *d_out (device scratch); s.sel[s.n + 1] (host) receives the per-cloud output offsets. Returns the total or
 // an error.
 int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n, int k, gpdb_pose **d_out);
+// the per-cloud offsets of the n candidate records of the running batch (store s; sample-slot order, stream slots) ->
+// cand_off[s.n + 1] (host), once the stream has drained
+int geo_batch_cand_off(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_cand, int n, int *cand_off);
 int geo_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid);
 int geo_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, int slot0, const double *d_frames,
               const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags);

@@ -3126,3 +3126,14 @@ int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n,
   *d_out = out;
   return total;
 }
+
+int geo_batch_cand_off(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_cand, int n, int *cand_off) {
+  const int B = s.n;
+  int *d_off = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * ((size_t)B + 1));
+  if (!d_off) return GPDB_ERR_CUDA;
+  k_batch_cand_off<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, s.soff, B, d_off);
+  LAUNCH_CHECK();
+  CUDA_TRY(cudaMemcpyAsync(cand_off, d_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return GPDB_OK;
+}

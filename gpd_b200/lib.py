@@ -28,7 +28,8 @@ EXPORTS = [
     "gpdb_debug_path_counts", "gpdb_debug_lenet_layers", "gpdb_set_clouds_samples", "gpdb_hand_search_batch",
     "gpdb_find_clusters_batch", "gpdb_preprocess_clouds_device", "gpdb_set_clouds_device", "gpdb_detect_batch_select_device",
     "gpdb_find_clusters_batch_device", "gpdb_sis_params_default", "gpdb_sis_batch", "gpdb_sis_batch_device",
-    "gpdb_sis_positions",
+    "gpdb_sis_positions", "gpdb_set_clouds_samples_device", "gpdb_hand_search_batch_device", "gpdb_detect_batch_device",
+    "gpdb_images_batch_device", "gpdb_classify_device",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -113,6 +114,8 @@ def lib():
     L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
+    for name, argtypes in abi.RESIDENT_PROTOTYPES.items():
+        getattr(L, name).argtypes = argtypes
     _LIB = L
     return L
 
@@ -653,6 +656,77 @@ class Context:
         nc = self._check(lib().gpdb_find_clusters_batch_device(self.h, len(hoff) - 1, _p(hoff), ph, int(min_inliers),
                                                                C.c_void_p(out.data_ptr()) if n else None, _p(coff)))
         return out[:nc], coff
+
+    def set_clouds_samples_tensors(self, pos_offsets, xyz):
+        """gpdb_set_clouds_samples_device: set_clouds_samples() from a float64 CUDA tensor xyz [M, 3] (cloud b's positions
+        at rows pos_offsets[b] .. pos_offsets[b+1]-1, pos_offsets a host array of B+1 entries), e.g. drawn by a model on the
+        GPU. Returns each cloud's first position index N_b (int32 [B]): cloud-local index N_b + j addresses its position j."""
+        import torch
+        off = _host_i32("pos_offsets", pos_offsets, self._n_clouds + 1)
+        px = _device_arg("xyz", xyz, torch.float64, self.params.device, 3 * int(off[-1]))
+        self._torch_stream()
+        self._check(lib().gpdb_set_clouds_samples_device(self.h, _p(off), px))
+        return np.diff(self._batch[0]).astype(np.int32)
+
+    def _all_records(self, fn, sample_offsets, d_sample_idx, scores):
+        import torch
+        off = _host_i32("sample_offsets", sample_offsets, self._n_clouds + 1)
+        dev = self.params.device
+        n, P = int(off[-1]), self.params.num_hand_axes * self.params.num_orientations
+        ps = _device_arg("d_sample_idx", d_sample_idx, torch.int32, dev, n)
+        self._torch_stream()
+        rec = torch.empty((n * P, POSE_BYTES), dtype=torch.uint8, device=f"cuda:{dev}")
+        flags = torch.empty((n, P), dtype=torch.uint8, device=f"cuda:{dev}")
+        dense = [flags] + ([torch.empty((n, P), dtype=torch.float32, device=f"cuda:{dev}")] if scores else [])
+        coff = np.zeros(len(off), np.int32)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t.numel() else None  # noqa: E731
+        stats = abi.Result()
+        nc = self._check(fn(self.h, _p(off), ps, *[ptr(t) for t in dense], ptr(rec), _p(coff), C.byref(stats)))
+        return (rec[:nc], *dense, coff)
+
+    def hand_search_batch_tensors(self, sample_offsets, d_sample_idx):
+        """gpdb_hand_search_batch_device: hand_search_batch() for cloud-local sample indices in an int32 CUDA tensor (CSR,
+        sample_offsets a host array of B+1 entries). Returns (records, flags, offsets): every VALID|FILTERED record as a uint8
+        CUDA tensor [nc, POSE_BYTES] (cloud b's rows offsets[b] .. offsets[b+1]-1, cloud-local sample slots, as
+        hand_search_batch returns them; poses_from_tensor reads them), the pose flags [n, P] uint8 on the device and the host
+        offsets [B+1]."""
+        return self._all_records(lib().gpdb_hand_search_batch_device, sample_offsets, d_sample_idx, False)
+
+    def detect_batch_tensors(self, sample_offsets, d_sample_idx):
+        """gpdb_detect_batch_device: detect_batch() on the device, as hand_search_batch_tensors. Returns (records, flags,
+        scores, offsets): the scored records, the pose flags [n, P] uint8 and scores [n, P] float32 (NaN where no image was
+        classified) on the device, and the host offsets [B+1]. No images: images_batch_tensors makes them."""
+        return self._all_records(lib().gpdb_detect_batch_device, sample_offsets, d_sample_idx, True)
+
+    def images_batch_tensors(self, hand_offsets, hands):
+        """gpdb_images_batch_device: the grasp images of gpdb_pose records in a uint8 CUDA tensor [n, POSE_BYTES] (cloud b's
+        at rows hand_offsets[b] .. hand_offsets[b+1]-1, hand_offsets a host array of B+1 entries), as a uint8 CUDA tensor
+        [n, S, S, C] in the cv::Mat layout, byte-equal to detect_batch's images of the same records."""
+        import torch
+        hoff = _host_i32("hand_offsets", hand_offsets, self._n_clouds + 1)
+        dev = self.params.device
+        n = int(hoff[-1])
+        ph = _device_arg("hands", hands, torch.uint8, dev, n * POSE_BYTES)
+        self._torch_stream()
+        S, Cc = self.params.image_size, self.params.image_num_channels
+        out = torch.empty((n, S, S, Cc), dtype=torch.uint8, device=f"cuda:{dev}")
+        self._check(lib().gpdb_images_batch_device(self.h, _p(hoff), ph, C.c_void_p(out.data_ptr()) if n else None))
+        return out
+
+    def classify_tensors(self, images):
+        """gpdb_classify_device: classify() of uint8 CUDA images [n, S, S, C] (cv::Mat layout). Returns (scores [n], logits
+        [n, 2]), float32 CUDA tensors, bit-equal to classify() of the same images."""
+        import torch
+        dev = self.params.device
+        S, Cc = self.params.image_size, self.params.image_num_channels
+        n = images.shape[0] if isinstance(images, torch.Tensor) and images.dim() > 0 else 0
+        pi = _device_arg("images", images, torch.uint8, dev, n * S * S * Cc)
+        self._torch_stream()
+        scores = torch.empty(n, dtype=torch.float32, device=f"cuda:{dev}")
+        logits = torch.empty((n, 2), dtype=torch.float32, device=f"cuda:{dev}")
+        self._check(lib().gpdb_classify_device(self.h, pi, n, C.c_void_p(scores.data_ptr()) if n else None,
+                                               C.c_void_p(logits.data_ptr()) if n else None))
+        return scores, logits
 
     def detect_batch_raw(self, offsets_i32, sidx_i32, res, cand_offsets_i32):
         """Timed path for tools/bench_batch.py: no numpy conversion; caller frees `res`."""

@@ -403,7 +403,9 @@ int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *han
 
 /* --- device-resident batches: clouds, samples and results that live in GPU memory ------------------------------------
  * The batch calls above from device memory, with no bulk PCIe traffic: preprocess (or install), detect + select and
- * cluster a batch whose arrays a framework produced on the GPU (simulated depth cameras, device depth-to-cloud).
+ * cluster a batch whose arrays a framework produced on the GPU (simulated depth cameras, device depth-to-cloud); install
+ * sample positions a model drew on the GPU, return every hand with its pose flags and scores, and make and classify
+ * grasp images for a classifier of the caller's.
  * Sizes and offsets stay on the host (B, point / sample / hand offsets, n_cameras, view_points, the preprocessing
  * parameters; the library sizes its launches from them). Arguments named d_* are device pointers on the context's device:
  * any non-NULL d_* argument that cudaPointerGetAttributes does not report as device or managed memory of that device is
@@ -441,6 +443,37 @@ int gpdb_detect_batch_select_device(gpdb_ctx *ctx, const int32_t *sample_offsets
  * hand_offsets[G] records); hand_offsets and cluster_offsets_out [G + 1] are host arrays. */
 int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *d_hands,
                                     int32_t min_inliers, gpdb_pose *d_clusters_out, int32_t *cluster_offsets_out);
+
+/* gpdb_set_clouds_samples with the positions in device memory: d_samples_xyz (3 x M float64, column-major, M =
+ * pos_offsets[B]) is copied device to device into the batch's sample arena. Same rules: the values are not checked, each
+ * call replaces all positions, a failed call and any new batch leave none, GPDB_ERR_STATE without a batch. Returns M. */
+int gpdb_set_clouds_samples_device(gpdb_ctx *ctx, const int32_t *pos_offsets, const double *d_samples_xyz);
+
+/* gpdb_hand_search_batch with device sample indices (d_sample_idx [n = sample_offsets[B]], checked on the device) and
+ * device results: d_hands_out has room for n * P records and receives every VALID|FILTERED record exactly as
+ * gpdb_hand_search_batch returns them (grouped by cloud, cloud-local sample_slot; cloud b's at cand_offsets_out[b] ..
+ * cand_offsets_out[b+1], a host array of B + 1 entries); d_flags_out [n * P] receives the pose flags (may be NULL).
+ * stats receives the counts, timings and launch count; its array members stay NULL. Needs no weights. Returns the number
+ * of records. */
+int gpdb_hand_search_batch_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx,
+                                  uint8_t *d_flags_out, gpdb_pose *d_hands_out, int32_t *cand_offsets_out, gpdb_result *stats);
+
+/* gpdb_detect_batch the same way: d_candidates_out (room for n * P records) receives the scored records as
+ * gpdb_detect_batch returns them, d_flags_out / d_scores_out [n * P] the pose flags and scores (NaN where no image was
+ * classified; either may be NULL). No images: size d_images_out of gpdb_images_batch_device from cand_offsets_out. */
+int gpdb_detect_batch_device(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *d_sample_idx, uint8_t *d_flags_out,
+                             float *d_scores_out, gpdb_pose *d_candidates_out, int32_t *cand_offsets_out, gpdb_result *stats);
+
+/* ImageGenerator::createImages (gpdb_images) for given hands of the installed batch: group b, d_hands[hand_offsets[b] ..
+ * hand_offsets[b+1]), belongs to cloud b (hand_offsets: B + 1 host entries starting at 0, never decreasing). d_images_out
+ * receives hand_offsets[B] images of S*S*C bytes, HWC uint8 (the cv::Mat layout of gpdb_images), byte-identical to
+ * gpdb_detect_batch with keep_images = 1 for the same records. The records' sample_slot is ignored; sample_index seeds the
+ * shadow draws. Returns the number of images. */
+int gpdb_images_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, const gpdb_pose *d_hands, uint8_t *d_images_out);
+
+/* gpdb_classify on n images in device memory (d_images_hwc [n * S*S*C], HWC uint8): d_scores_out [n] and d_logits_out
+ * [n * 2] (may be NULL) are written by the classifier directly. Bit-equal to gpdb_classify, for both lenet_impl values. */
+int gpdb_classify_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, int32_t n, float *d_scores_out, float *d_logits_out);
 
 /* --- sequential importance sampling: SequentialImportanceSampling::detectGrasps on the device ----------------------------
  * (sequential_importance_sampling.cpp:54-270) over every cloud of the installed batch (gpdb_set_clouds[_device] /

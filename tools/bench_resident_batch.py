@@ -12,7 +12,16 @@ For each B it checks once, outside the timed region, that both routes return ide
 then prints one JSON line with the median wall time per step and of the whole route over --reps repetitions, the
 samples/s of each route, and the GPU name and power limit. Needs a GPU.
 
-    python tools/bench_resident_batch.py [--sizes 16 64 256] [--reps 5]
+--search: a learned sampler's loop instead. The B views are installed once (default preprocessing); every view gets 500
+positions drawn by torch on the device (Gaussian offsets, sigma 2 mm, around random points of the processed view), and
+the samples are exactly those positions (local indices N_b .. N_b + 499):
+  host route:   .cpu() of the positions, gpdb_set_clouds_samples, gpdb_detect_batch (records, flags and scores to the host);
+  device route: gpdb_set_clouds_samples_device, gpdb_detect_batch_device (records, flags and scores stay in CUDA tensors).
+It checks once, outside the timed region, that both routes return the same records, offsets, flags and score bits, and
+also times gpdb_hand_search_batch_device + gpdb_images_batch_device (the grasp images of every hand, for a classifier of
+the caller's) on their own. Each JSON line gives the median and the min / max over --reps repetitions.
+
+    python tools/bench_resident_batch.py [--sizes 16 64 256] [--reps 5] [--search]
 """
 import argparse
 import json
@@ -95,10 +104,95 @@ def device_route(ctx, views, samples, vps, pp):
     return st.t, (lib.poses_from_tensor(rec).tobytes(), lib.poses_from_tensor(cl).tobytes())
 
 
+SIGMA = 0.002
+
+
+def draw_positions(xyz, poff, gen):
+    """N_SAMPLES positions per view on the device: Gaussian offsets around uniformly drawn points of the view."""
+    counts = torch.from_numpy(np.diff(poff)).cuda().repeat_interleave(N_SAMPLES)
+    first = torch.from_numpy(poff[:-1]).cuda().repeat_interleave(N_SAMPLES)
+    pick = first + (torch.rand(len(counts), device="cuda", generator=gen, dtype=torch.float64) * counts).long()
+    return xyz[pick].double() + SIGMA * torch.randn((len(counts), 3), device="cuda", generator=gen, dtype=torch.float64)
+
+
+def search_host(ctx, pos, B):
+    st = Steps()
+    p = pos.cpu().numpy()
+    st("to_host")
+    first = ctx.set_clouds_samples([p[b * N_SAMPLES:(b + 1) * N_SAMPLES] for b in range(B)])
+    st("install")
+    res = ctx.detect_batch(first)
+    st("detect")
+    out = (b"".join(r["candidates"].tobytes() for r in res), [r["n_candidates"] for r in res],
+           np.concatenate([r["pose_flags"] for r in res]).tobytes(), np.concatenate([r["pose_scores"] for r in res]).tobytes())
+    return st.t, out
+
+
+def search_device(ctx, pos, soff, sidx):
+    st = Steps()
+    ctx.set_clouds_samples_tensors(soff, pos)
+    st("install")
+    rec, flags, scores, coff = ctx.detect_batch_tensors(soff, sidx)
+    st("detect")
+    return st.t, (rec, flags, scores, coff)
+
+
+def search_images(ctx, soff, sidx):
+    st = Steps()
+    rec, _, coff = ctx.hand_search_batch_tensors(soff, sidx)
+    st("hand_search")
+    img = ctx.images_batch_tensors(coff, rec)
+    st("images")
+    return st.t, len(img)
+
+
+def main_search(ctx, a, pool, pp, gpu):
+    spread = lambda v: [round(1e3 * min(v), 2), round(1e3 * max(v), 2)]  # noqa: E731
+    med = lambda v: float(np.median(v))  # noqa: E731
+    for B in a.sizes:
+        poff = ctx.preprocess_clouds([{"xyz": r["xyz"], "cam_source": r["cam_source"], "view_points": r["view_points"]}
+                                      for r in pool[:B]], pp, read_back=False)
+        xyz = torch.from_numpy(np.concatenate([c["xyz"] for c in ctx.get_clouds()])).cuda()
+        gen = torch.Generator(device="cuda").manual_seed(B)
+        pos = draw_positions(xyz, poff, gen)
+        soff = np.arange(B + 1, dtype=np.int32) * N_SAMPLES
+        sidx = (torch.from_numpy(np.diff(poff)).cuda().int().repeat_interleave(N_SAMPLES)
+                + torch.arange(N_SAMPLES, device="cuda", dtype=torch.int32).repeat(B)).contiguous()
+        n = B * N_SAMPLES
+        torch.cuda.synchronize()
+        # warm-up of every shape, and the one check that both routes agree bit for bit
+        _, h = search_host(ctx, pos, B)
+        _, (rec, flags, scores, coff) = search_device(ctx, pos, soff, sidx)
+        assert h[0] == lib.poses_from_tensor(rec).tobytes(), "records differ"
+        assert list(np.diff(coff)) == h[1], "offsets differ"
+        assert h[2] == flags.cpu().numpy().tobytes() and h[3] == scores.cpu().numpy().tobytes(), "flags or scores differ"
+        del rec, flags, scores
+        _, n_img = search_images(ctx, soff, sidx)
+        th, td, ti = [], [], []
+        for _ in range(a.reps):
+            th.append(search_host(ctx, pos, B)[0])
+            td.append(search_device(ctx, pos, soff, sidx)[0])
+            ti.append(search_images(ctx, soff, sidx)[0])
+        tot = lambda ts: [sum(t.values()) for t in ts]  # noqa: E731
+        host_ms, dev_ms, img_ms = med(tot(th)), med(tot(td)), med(tot(ti))
+        print(json.dumps({"mode": "search", "B": B, "processed_points": int(poff[-1]), "samples": n,
+                          "candidates": int(coff[-1]), "images": n_img,
+                          "host_ms": round(1e3 * host_ms, 2), "device_ms": round(1e3 * dev_ms, 2),
+                          "host_ms_min_max": spread(tot(th)), "device_ms_min_max": spread(tot(td)),
+                          "host_sps": round(n / host_ms), "device_sps": round(n / dev_ms),
+                          "host_steps_ms": {s: round(1e3 * med([t[s] for t in th]), 2) for s in th[0]},
+                          "device_steps_ms": {s: round(1e3 * med([t[s] for t in td]), 2) for s in td[0]},
+                          "search_images_ms": round(1e3 * img_ms, 2), "search_images_ms_min_max": spread(tot(ti)),
+                          "search_images_sps": round(n / img_ms), "images_per_s": round(n_img / img_ms),
+                          "search_images_steps_ms": {s: round(1e3 * med([t[s] for t in ti]), 2) for s in ti[0]},
+                          "gpu": gpu}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--sizes", type=int, nargs="+", default=[16, 64, 256])
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--search", action="store_true", help="positions drawn on the device: the host against the device route")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_resident_batch.py needs a CUDA device")
@@ -108,6 +202,10 @@ def main():
     pp = lib.preprocess_params()
     gpu = gpu_info()
     pool = [scenes.synthetic_raw_scene(1000 + i, n_points=N_POINTS) for i in range(max(a.sizes))]
+    if a.search:
+        main_search(ctx, a, pool, pp, gpu)
+        ctx.close()
+        return
     med = lambda v: float(np.median(v))  # noqa: E731
     for B in a.sizes:
         raw = pool[:B]
