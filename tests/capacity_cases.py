@@ -30,12 +30,45 @@ WL_CAP = (2 * IMG2_S * IMG2_S * 8) // 20  # k_images: WL_CAP, the shadow work li
 DL_CAP = 2 * IMG2_S * IMG2_S            # CastLists::dl_cap, the draw list of either kernel (7 200)
 
 
-def st_cap2(bm_dim, n_cameras):
-    """k_images2's voxel stash (ST_CAP): what LIST_BYTES (BOX_CAP2 x 36 B) leaves behind the cameras' shadow
-    bitmaps (2 bm_dim^2 words each) and one word of alignment, in 8-byte entries."""
+def st_sm2(bm_dim, n_cameras):
+    """The shared-memory part of k_images2's voxel stash (ST_SM): what LIST_BYTES (BOX_CAP2 x 36 B) leaves behind the
+    cameras' shadow bitmaps (2 bm_dim^2 words each) and one word of alignment, in 8-byte entries."""
     bm_words = 2 * bm_dim * bm_dim
     used = ((bm_words * max(n_cameras, 1) + 1) & ~1) * 4
     return (BOX_CAP2 * 36 - used) // 8
+
+
+def st_cap2(bm_dim, n_cameras):
+    """k_images2's voxel stash (ST_CAP): ST_SM entries in shared memory, then BALL_CAP2 / 2 more in the image's own
+    HBM slot over the in-ball list; past it the voxels of projection 2 take a second walk over the bitmap."""
+    return st_sm2(bm_dim, n_cameras) + BALL_CAP2 // 2
+
+
+BOX_CAP2_BYTES = BOX_CAP2 * 36   # k_images2's LIST_BYTES
+
+
+def list_bytes(bm_dim, n_cameras):
+    """launch_images: k_images' box-list region at 15 channels, which the shadow bitmaps and the voxel list alias."""
+    bm = n_cameras * (2 * bm_dim * bm_dim) * 4
+    return (max(BOX_CAP * 36, bm + 4096 * 4) + 15) // 16 * 16
+
+
+def bl_cap(bm_dim, n_cameras):
+    """k_images' voxel list (BL_CAP): the 4-byte entries of list_bytes behind bitmap 0."""
+    return list_bytes(bm_dim, n_cameras) // 4 - 2 * bm_dim * bm_dim
+
+
+def fast_path_15(bm_dim, n_cameras):
+    """launch_images: whether a 15-channel image of size 60 goes to k_images2, whose shadow bitmaps must leave 2 KB of
+    its list free."""
+    return n_cameras <= 2 and n_cameras * (2 * bm_dim * bm_dim) * 4 + 2048 <= BOX_CAP2_BYTES
+
+
+def bm_dim(volume_width=0.10, volume_depth=0.06, volume_height=0.02):
+    """api.cu fill_dev_params: the shadow bitmap's extent in voxels."""
+    import math
+    diag = math.sqrt(volume_depth * volume_depth + volume_width * volume_width + 4.0 * volume_height * volume_height)
+    return int(math.ceil((diag + 2.0 * 3.2 * 0.003 * 0.3) / 0.003)) + 4
 
 
 # search radii at the default hand and image geometry (api.cu fill_dev_params)

@@ -15,8 +15,15 @@ BOX_EDGES = [cc.BOX_CAP2, cc.BOX_CAP2 + 1, cc.BOX_CAP, cc.BOX_CAP + 1]
 
 def test_caps_mirror_the_kernels():
     assert cc.BALL_CAP2 == 3600 and cc.WL_CAP2 == 1440 and cc.WL_CAP == 2880 and cc.DL_CAP == 7200
-    # the default 15-channel bitmap (48^2 x 2 words) at one camera, and 46^2 at two (volume_depth 0.05)
-    assert cc.st_cap2(48, 1) == 2304 and cc.st_cap2(46, 2) == 376
+    # k_images2's voxel stash: the default 15-channel bitmap (48^2 x 2 words) at one camera, and 46^2 at two
+    # (volume_depth 0.05); shared memory first (ST_SM), then 1 800 entries in the image's HBM slot (ST_CAP)
+    assert cc.st_sm2(48, 1) == 2304 and cc.st_cap2(48, 1) == 4104
+    assert cc.st_sm2(46, 2) == 376 and cc.st_cap2(46, 2) == 2176
+    # k_images' voxel list behind bitmap 0 (BL_CAP): 13 824 at the default geometry, 12 600 at volume_height 0.04
+    assert cc.bl_cap(cc.bm_dim(), 1) == 13824 and cc.bl_cap(cc.bm_dim(volume_height=0.04), 1) == 12600
+    # k_images2 takes two cameras up to bm_dim 46 (volume_depth 0.05); 47 (volume_depth 0.055) goes to k_images
+    assert cc.fast_path_15(cc.bm_dim(volume_depth=0.05), 2) and not cc.fast_path_15(cc.bm_dim(volume_depth=0.055), 2)
+    assert cc.bm_dim(volume_depth=0.05) == 46 and cc.bm_dim(volume_depth=0.055) == 47
 
 
 @pytest.mark.parametrize("n,at_position", [(n, False) for n in FRAME_EDGES] +

@@ -9,6 +9,9 @@ import numpy as np
 import pytest
 
 import capacity_cases as cc
+import image_reference as ir
+import shadow_cast_reference as scr
+import shadow_counters as gsc
 from gpd_b200 import lib
 from conftest import load_weights
 from oracle import oracle
@@ -215,41 +218,39 @@ def test_hands_closing_region_capacity(n):
     ctx.close()
 
 
-# ---- shadow phase of the 15-channel images: in-place fallbacks of the work list, the draw list and the voxel stash
+# ---- shadow phase of the 15-channel images: in-place fallbacks of the work list, the draw list and the voxel stash,
+# counted exactly against tests/shadow_cast_reference.py (test_gpu_shadow_cast.py pins each list at its edge)
 
 SHADOW = {
-    # name: (box points, out-of-box points, cameras, overrides, counters that must be zero, counters that must be >= 1)
-    "small": (40, 0, 1, {}, ["images2_cast_in_place", "images2_draw_in_place", "images2_stash_full",
-                             "images_cast_in_place", "images_draw_in_place", "images_voxel_list_full"], []),
-    "work_list": (1000, 900, 1, {}, ["images_cast_in_place", "images_voxel_list_full"], ["images2_cast_in_place"]),
-    "draw_list": (1000, 100, 1, {}, ["images2_cast_in_place"], ["images2_draw_in_place", "images_draw_in_place"]),
-    "stash_1cam": (1000, 100, 1, {}, ["images_voxel_list_full"], ["images2_stash_full"]),
-    "stash_2cam": (1000, 100, 2, {"volume_depth": 0.05}, [], ["images2_stash_full"]),
+    # name: (box points, out-of-box points, cameras, overrides)
+    "small": (40, 0, 1, {}),
+    "work_list": (1000, 900, 1, {}),
+    "draw_list": (1000, 100, 1, {}),
+    "stash_1cam": (1000, 100, 1, {}),
+    "stash_2cam": (1000, 100, 2, {"volume_depth": 0.05}),
 }
 
 
 @pytest.mark.parametrize("name", list(SHADOW))
 def test_images2_shadow_fallbacks(name, monkeypatch):
-    n_box, n_out, k, over, zero, hit = SHADOW[name]
+    n_box, n_out, k, over = SHADOW[name]
     cloud, pose = cc.image_box(n_box, n_outside=n_out)
     if k == 2:
         cloud["view_points"] = np.array([[0.0, 0.0, 0.0], [0.3, 0.0, 0.0]])
         cloud["cam_source"] = np.ones((len(cloud["xyz"]), 2), np.int32)
     p, ctx, oc = context(cloud, channels=15, **over)
-    ig, counts = counted(ctx, ctx.images, pose)
-    monkeypatch.setenv("GPD_B200_IMAGES_KERNEL", "1")
-    ig1, forced = counted(ctx, ctx.images, pose)
-    monkeypatch.delenv("GPD_B200_IMAGES_KERNEL")
+    g = ir.Geometry(C=15, d=over.get("volume_depth", 0.06))
+    r = scr.cast(cloud, pose[0], g)
+    ig, counts, slots = gsc.counted_images(ctx, pose, False, monkeypatch)
+    ig1, forced, slots1 = gsc.counted_images(ctx, pose, True, monkeypatch)
     assert counts["images2_box"] == 0  # the fast kernel made this image itself
     assert np.array_equal(ig, ig1)
     io = oc.images(p, pose)
     d = np.abs(io.astype(np.int32).reshape(ig.shape) - ig.astype(np.int32))
     assert io[..., 14].max() > 0 and d.max() <= 1 and np.count_nonzero(d) <= 1e-3 * d.size
-    both = {**{f"fast:{e}": v for e, v in counts.items()}, **{f"forced:{e}": v for e, v in forced.items()}}
-    for e in zero:
-        assert (counts if e.startswith("images2") else forced)[e] == 0, both
-    for e in hit:
-        assert (counts if e.startswith("images2") else forced)[e] >= 1, both
+    box_n = cc.box_count(cloud, pose, g.w, g.d, g.h, g.radius)
+    gsc.assert_counters(gsc.expected(r, g, box_n, False), counts, slots)
+    gsc.assert_counters(gsc.expected(r, g, box_n, True), forced, slots1)
     ctx.close()
 
 
