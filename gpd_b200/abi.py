@@ -157,6 +157,37 @@ RESIDENT_PROTOTYPES = {
 }
 
 
+DEPTH_U16, DEPTH_F32 = 0, 1  # GPDB_DEPTH_U16 / GPDB_DEPTH_F32
+
+
+class DepthCamera(C.Structure):
+    """gpdb_depth_camera (include/gpd_b200_depth.h): one pinhole depth camera of a view."""
+
+    _fields_ = [
+        ("width", C.c_int32),
+        ("height", C.c_int32),
+        ("fx", C.c_double),
+        ("fy", C.c_double),
+        ("cx", C.c_double),
+        ("cy", C.c_double),
+        ("pose", C.c_double * 12),  # camera-to-world [R | t], row-major 3 x 4
+        ("depth_scale", C.c_double),
+        ("min_depth", C.c_double),
+        ("max_depth", C.c_double),
+    ]
+
+
+# gpdb_preprocess_depth[_device], gpdb_subsample_clouds[_device] (include/gpd_b200.h)
+DEPTH_PROTOTYPES = {
+    "gpdb_preprocess_depth": [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                              C.POINTER(PreprocessParams), C.c_void_p],
+    "gpdb_preprocess_depth_device": [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.POINTER(PreprocessParams), C.c_void_p],
+    "gpdb_subsample_clouds": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_subsample_clouds_device": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
+}
+
+
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""
     p = PreprocessParams()

@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "../../include/gpd_b200_depth.h"
 #include "common.cuh"
 
 static char g_create_err[512] = "";
@@ -281,6 +282,7 @@ static void cloud_free(CloudSet &s) {
   free(s.off);
   free(s.sel);
   free(s.pos);
+  free(s.raw_off);
 }
 
 extern "C" {
@@ -480,6 +482,7 @@ int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds) {
     free(s.off); s.off = nullptr;
     free(s.sel); s.sel = nullptr;
     free(s.pos); s.pos = nullptr;
+    free(s.raw_off); s.raw_off = nullptr;
     s.desc_cap = 0;
     const size_t cap = (size_t)n_clouds + 1 + n_clouds / 4;
     CUDA_TRY(cudaMalloc(&s.desc, sizeof(CloudDesc) * cap));
@@ -487,7 +490,8 @@ int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds) {
     s.off = (int *)malloc(sizeof(int) * cap);
     s.sel = (int *)malloc(sizeof(int) * cap);
     s.pos = (int *)malloc(sizeof(int) * cap);
-    if (!s.off || !s.sel || !s.pos) {
+    s.raw_off = (int *)malloc(sizeof(int) * cap);
+    if (!s.off || !s.sel || !s.pos || !s.raw_off) {
       gpdb_set_error(ctx, GPDB_ERR_CUDA, "cloud store: host allocation failed");
       return GPDB_ERR_CUDA;
     }
@@ -705,6 +709,9 @@ static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   return rc == GPDB_OK ? B : rc;
 }
 
+static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
+                              const gpdb_preprocess_params *pp, int32_t *poff);
+
 // gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); a failed call
 // leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays (read in place, the camera
 // masks packed on the device), else host arrays uploaded here.
@@ -762,9 +769,18 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   // ---- removeNans + filterWorkspace + voxelizeCloud of every cloud, into the store's arenas
   rc = pre_filter_voxelize_batch(ctx, s, d_xyz_raw, d_cam_raw, d_nrm_raw, M, B, roff, *pp, poff, ev[2]);
   if (rc != GPDB_OK) return rc;
+  return preprocess_install(ctx, s, desc.data(), B, roff, pp, poff);
+}
+
+// The steps of a preprocessing call after the filter and voxelisation (store s holds the processed points, poff[B+1] their
+// offsets, desc[B] the camera fields): install with one grid per cloud, normals, nonunit flags, stage timings, and the
+// raw offsets roff[B+1] the source indices refer to. A failure leaves no cloud in s.
+static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
+                              const gpdb_preprocess_params *pp, int32_t *poff) {
+  cudaEvent_t *ev = ctx->ev;
   cudaEventRecord(ev[3], ctx->stream);
   // ---- install, one grid per cloud
-  rc = gpdb_install_clouds(ctx, s, desc.data(), poff, B, false);
+  int rc = gpdb_install_clouds(ctx, s, desc, poff, B, false);
   if (rc != GPDB_OK) return rc;
   cudaEventRecord(ev[4], ctx->stream);
   // ---- calculateNormalsOMP + reverseNormals, every cloud against its own grid; then the per-cloud nonunit flags: zero
@@ -790,6 +806,7 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   for (int i = 0; i < 5; i++)
     if (cudaEventElapsedTime(&t, ev[i], ev[i + 1]) == cudaSuccess) ctx->pre_ms[i] = t;
   if (cudaEventElapsedTime(&t, ev[0], ev[5]) == cudaSuccess) ctx->pre_ms[5] = t;
+  memcpy(s.raw_off, roff, sizeof(int) * ((size_t)B + 1));
   s.has_src = true;
   return B;
 }
@@ -1593,6 +1610,204 @@ int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t 
     return GPDB_ERR_STATE;
   }
   return get_clouds(ctx, ctx->many, xyz_out, normals_out, cam_source_out, src_out);
+}
+
+}  // extern "C"
+
+// ---- depth images and Cloud::subsample (include/gpd_b200_depth.h) ------------------------------------------------------
+
+// the argument checks of gpdb_preprocess_depth[_device]; roff[B+1] receives the raw offsets (cumulative pixels per view)
+static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                            int32_t format, const void *depth, const gpdb_preprocess_params *pp, const int32_t *poff,
+                            std::vector<int> &roff) {
+  if (B <= 0 || !n_cameras || !cams || !depth || !pp || !poff) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth, params, processed_offsets_out",
+                   name);
+    return GPDB_ERR_INVALID;
+  }
+  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
+    return GPDB_ERR_INVALID;
+  }
+  if (!pp->estimate_normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
+    return GPDB_ERR_INVALID;
+  }
+  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || !(pp->normals_radius > 0.0)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: voxel_size and normals_radius must be positive", name);
+    return GPDB_ERR_INVALID;
+  }
+  roff.assign((size_t)B + 1, 0);
+  long long total = 0;
+  for (int b = 0, c = 0; b < B; b++) {
+    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d has %d cameras (1 <= cameras <= %d)", name, b, n_cameras[b],
+                     GPDB_MAX_CAMERAS);
+      return GPDB_ERR_INVALID;
+    }
+    for (int k = 0; k < n_cameras[b]; k++, c++) {
+      const gpdb_depth_camera &D = cams[c];
+      const char *bad = nullptr;
+      bool finite = std::isfinite(D.fx) && std::isfinite(D.fy) && std::isfinite(D.cx) && std::isfinite(D.cy);
+      for (int e = 0; e < 12; e++) finite = finite && std::isfinite(D.pose[e]);
+      if (D.width < 1 || D.height < 1) bad = "width and height must be at least 1";
+      else if (!finite) bad = "non-finite intrinsics or pose";
+      else if (!(D.fx > 0.0) || !(D.fy > 0.0)) bad = "fx and fy must be positive";
+      else if (!(D.depth_scale > 0.0) || !std::isfinite(D.depth_scale)) bad = "depth_scale must be finite and positive";
+      else if (!(D.min_depth >= 0.0)) bad = "min_depth must be >= 0";
+      else if (!(D.max_depth > D.min_depth)) bad = "max_depth must exceed min_depth";
+      if (bad) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d (camera %d of the call): %s", name, b, k, c, bad);
+        return GPDB_ERR_INVALID;
+      }
+      total += (long long)D.width * D.height;
+      if (total >= (1ll << 31)) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d: the call holds 2^31 or more pixels", name, b, k);
+        return GPDB_ERR_INVALID;
+      }
+    }
+    roff[b + 1] = (int)total;
+  }
+  return GPDB_OK;
+}
+
+// gpdb_preprocess_depth[_device] after the argument checks: d_depth in device memory (the host twin has uploaded it)
+static int preprocess_depth(gpdb_ctx *ctx, CloudSet &s, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                            int32_t format, const void *depth, bool device, const gpdb_preprocess_params *pp,
+                            const std::vector<int> &roff, int32_t *poff) {
+  cudaEvent_t *ev = ctx->ev;
+  const int M = roff[B];
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaEventRecord(ev[0], ctx->stream);
+  const void *d_depth = depth;
+  if (!device) {
+    const size_t bytes = (size_t)M * (format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float));
+    void *up = gpdb_scratch(ctx, SCR_UPLOAD, bytes);
+    if (!up) return GPDB_ERR_CUDA;
+    CUDA_TRY(cudaMemcpyAsync(up, depth, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    d_depth = up;
+  }
+  // the camera fields of the descriptors: view point k = t of camera k; one-hot camera sources, as a cam_source matrix
+  std::vector<CloudDesc> desc((size_t)B);
+  for (int b = 0, c = 0; b < B; b++) {
+    CloudDesc &D = desc[b];
+    memset(&D, 0, sizeof(D));
+    D.K = n_cameras[b];
+    for (int k = 0; k < D.K; k++, c++)
+      for (int r = 0; r < 3; r++) D.vp[k][r] = cams[c].pose[4 * r + 3];
+  }
+  cudaEventRecord(ev[1], ctx->stream);
+  int rc = pre_depth_batch(ctx, s, d_depth, format, cams, n_cameras, B, roff.data(), *pp, poff, ev[2]);
+  if (rc != GPDB_OK) return rc;
+  return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff);
+}
+
+static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const int32_t *n_cameras,
+                       const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
+                       const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
+  gpdb_sis_forget(ctx);
+  ctx->many.has_src = false;
+  ctx->many.n_samples = 0;
+  std::vector<int> roff;
+  int rc = check_depth_args(ctx, name, n_views, n_cameras, cameras, depth_format, depth, pp, processed_offsets_out, roff);
+  if (rc == GPDB_OK && device) {
+    const char *names[1] = {"d_depth"};
+    const void *ptrs[1] = {depth};
+    rc = check_device_ptrs(ctx, name, 1, names, ptrs);
+  }
+  if (rc != GPDB_OK) return rc;
+  return preprocess_depth(ctx, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
+                          processed_offsets_out);
+}
+
+// gpdb_subsample_clouds[_device]: the state and argument checks, then the device draw (the host twin uploads the mask and
+// copies the indices back)
+static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples, uint64_t seed, const uint8_t *mask,
+                           int32_t *idx_out, int32_t *offsets_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = ctx->many;
+  if (s.n == 0) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_preprocess_depth / gpdb_preprocess_clouds first",
+                   name);
+    return GPDB_ERR_STATE;
+  }
+  if (num_samples < 0 || !offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need num_samples >= 0 (got %d) and sample_offsets_out", name, num_samples);
+    return GPDB_ERR_INVALID;
+  }
+  if (mask && !s.has_src) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: a mask needs the source indices of a preprocessing call (gpdb_preprocess_depth "
+                   "/ gpdb_preprocess_clouds); the batch was installed by gpdb_set_clouds", name);
+    return GPDB_ERR_STATE;
+  }
+  const int B = s.n;
+  long long room = 0;
+  for (int b = 0; b < B; b++) {
+    const int nb = s.off[b + 1] - s.off[b];
+    room += num_samples == 0 ? nb : std::min(num_samples, nb);
+  }
+  if (room > 0 && !idx_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, device ? "d_sample_idx_out" : "sample_idx_out");
+    return GPDB_ERR_INVALID;
+  }
+  if (device) {
+    const char *names[2] = {"d_mask", "d_sample_idx_out"};
+    const void *ptrs[2] = {mask, idx_out};
+    const int rc = check_device_ptrs(ctx, name, 2, names, ptrs);
+    if (rc != GPDB_OK) return rc;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const uint8_t *d_mask = mask;
+  int *d_out = idx_out;
+  if (!device) {
+    if (mask) {
+      const size_t M = (size_t)s.raw_off[B];
+      uint8_t *up = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, M);
+      if (!up) return GPDB_ERR_CUDA;
+      CUDA_TRY(cudaMemcpyAsync(up, mask, M, cudaMemcpyHostToDevice, ctx->stream));
+      d_mask = up;
+    }
+    d_out = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)room);
+    if (!d_out) return GPDB_ERR_CUDA;
+  }
+  std::vector<int> soff((size_t)B + 1);
+  const int n = sub_draw_batch(ctx, s, num_samples, seed, d_mask, d_out, soff.data());
+  if (n < 0) return n;
+  if (!device && n > 0) {
+    CUDA_TRY(cudaMemcpyAsync(idx_out, d_out, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  memcpy(offsets_out, soff.data(), sizeof(int) * ((size_t)B + 1));
+  return n;
+}
+
+extern "C" {
+
+int gpdb_preprocess_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                          int32_t depth_format, const void *depth, const gpdb_preprocess_params *pp,
+                          int32_t *processed_offsets_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth", n_views, n_cameras, cameras, depth_format, depth, pp,
+                     processed_offsets_out, false);
+}
+
+int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                                 int32_t depth_format, const void *d_depth, const gpdb_preprocess_params *pp,
+                                 int32_t *processed_offsets_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
+                     processed_offsets_out, true);
+}
+
+int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *mask, int32_t *sample_idx_out,
+                          int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds", num_samples, seed, mask, sample_idx_out, sample_offsets_out, false);
+}
+
+int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_mask,
+                                 int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_device", num_samples, seed, d_mask, d_sample_idx_out,
+                         sample_offsets_out, true);
 }
 
 }  // extern "C"

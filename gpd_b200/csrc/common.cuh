@@ -118,6 +118,7 @@ struct CloudSet {
   int *off;             // [n + 1] point offsets (host)
   int *sel;             // [n + 1] per-cloud offsets of the records the last batch call left on the device (host)
   int *pos;             // [n + 1] per-cloud offsets of the sample positions while n_samples > 0 (host; the batch only)
+  int *raw_off;         // [n + 1] raw point offsets of the preprocessing call that installed the clouds (host, with src)
   size_t point_cap, cell_cap, desc_cap;
   int n, maxk;          // clouds installed, largest camera count
   bool has_src;
@@ -200,13 +201,14 @@ enum ScratchSlot {
   SCR_CUB,
   // overflow lists of k_frames / k_hands (frames finish before the hand-search stream starts); of the normal estimation
   SCR_OVF,
-  // compaction flags and positions (hand-search stream); sort keys and values of the selection
+  // compaction flags and positions (hand-search stream; the pixel filter of gpdb_preprocess_depth and the eligible points of
+  // gpdb_subsample_clouds); sort keys and values of the selection
   SCR_KEYS,
   // stage workspaces. LeNet: pool1 / pool2 / ip1 (main stream). Preprocessing: header, filter flags + filtered points,
   // voxel sort buffers. B is also the cell counts of the grid build; in the sharded calls A is the broadcast header and
   // B the all-gather buffer
   SCR_WORK_A, SCR_WORK_B, SCR_WORK_C,
-  // sample indices of a call; the raw upload / the device camera masks of preprocessing
+  // sample indices of a call (gpdb_subsample_clouds: its output); the raw upload / the device camera masks of preprocessing
   SCR_SIDX,
   // per call: frames, frame validity, dense per-pose flags, dense per-pose scores
   SCR_FRAMES, SCR_VALID, SCR_FLAGS, SCR_PSCORES,
@@ -232,6 +234,8 @@ enum ScratchSlot {
   // gpdb_sis_batch: kept / evaluated positions, the round's sample lists and counts (main stream, between pipeline calls;
   // read again by gpdb_sis_positions)
   SCR_SIS,
+  // host twins of gpdb_preprocess_depth / gpdb_subsample_clouds: the uploaded depth images, the uploaded mask
+  SCR_UPLOAD,
   SCR_N
 };
 
@@ -418,6 +422,32 @@ int pre_bounds_batch(gpdb_ctx *ctx, const float *xyz, const int *d_off, int B, i
 int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw, const uint8_t *d_cam_raw,
                               const double *d_nrm_raw, int M, int B, const int *roff, const gpdb_preprocess_params &pp,
                               int *poff, cudaEvent_t ev_filter_done);
+// the two halves of pre_filter_voxelize_batch, for a front that filters its own way (depth.cu). PreBatch: the device
+// header of one call (SCR_WORK_A): workspace, raw / filtered / processed offsets, bounds, voxel error words, and `extra`
+// bytes for the front
+struct PreBatch {
+  double *ws;
+  int *roff, *foff, *poff, *bounds, *verr;
+  unsigned char *extra;
+};
+int pre_batch_header(gpdb_ctx *ctx, int B, const int *roff, const gpdb_preprocess_params &pp, size_t extra, PreBatch &h);
+// h.foff from the exclusive scan pos of the filter flags (M + 1 entries): foff[b] = pos[roff[b]]
+int pre_filter_offsets(gpdb_ctx *ctx, const int *pos, const PreBatch &h, int B);
+// the filtered points (host offsets foff[B+1]; keep = raw index in the call's numbering, xyz1 the coordinates) voxelised
+// (or gathered) into store s; poff[B+1] (host) = processed offsets
+int pre_voxelize_back(gpdb_ctx *ctx, CloudSet &s, const PreBatch &h, const int *foff, const int *keep, const float *xyz1,
+                      const uint8_t *d_cam_raw, const double *d_nrm_raw, int B, const gpdb_preprocess_params &pp, int *poff);
+
+// depth.cu (include/gpd_b200_depth.h). The depth front of preprocessing: back-projection fused into the NaN / workspace
+// filter, then pre_voxelize_back. C cameras (d_cams, a device table written by depth_camera_table), cam_off[C+1] their
+// pixel offsets in the call (host), B views with raw offsets roff[B+1] (host, cumulative pixels per view).
+int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format, const gpdb_depth_camera *cams,
+                    const int *n_cameras, int B, const int *roff, const gpdb_preprocess_params &pp, int *poff,
+                    cudaEvent_t ev_filter_done);
+// Cloud::subsample of every cloud of store s (has_src when d_mask is given; mask indexed by the store's raw_off): cloud
+// b's draw to d_out at soff[b] (host, B + 1); returns the total or an error
+int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned long long seed, const uint8_t *d_mask,
+                   int *d_out, int *soff);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 

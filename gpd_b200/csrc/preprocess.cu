@@ -579,6 +579,32 @@ int pre_bounds_batch(gpdb_ctx *ctx, const float *xyz, const int *d_off, int B, i
   return GPDB_OK;
 }
 
+// The header of a preprocessing call in SCR_WORK_A: workspace [6 doubles], raw / filtered / processed offsets [B+1 each],
+// bounds [6B], voxel error [2], then `extra` bytes for the caller (h.extra, 8-byte aligned). Uploads the workspace, the
+// raw offsets and the voxel error words.
+int pre_batch_header(gpdb_ctx *ctx, int B, const int *roff, const gpdb_preprocess_params &pp, size_t extra, PreBatch &h) {
+  const size_t head = sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2);
+  const size_t head8 = (head + 7) / 8 * 8;
+  h.ws = (double *)gpdb_scratch(ctx, SCR_WORK_A, head8 + extra);
+  if (!h.ws) return GPDB_ERR_CUDA;
+  h.roff = (int *)(h.ws + 6), h.foff = h.roff + B + 1, h.poff = h.foff + B + 1, h.bounds = h.poff + B + 1;
+  h.verr = h.bounds + 6 * B;
+  h.extra = (unsigned char *)h.ws + head8;
+  const int verr0[2] = {0, INT_MAX};
+  CUDA_TRY(cudaMemcpyAsync(h.ws, pp.workspace, sizeof(double) * 6, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(h.roff, roff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(h.verr, verr0, sizeof(verr0), cudaMemcpyHostToDevice, ctx->stream));
+  return GPDB_OK;
+}
+
+// filtered offsets h.foff[b] = pos[roff[b]] from the exclusive scan pos (M + 1 entries) of the filter flags
+int pre_filter_offsets(gpdb_ctx *ctx, const int *pos, const PreBatch &h, int B) {
+  const int tb = 256;
+  k_bpre_offsets<<<(B + 1 + tb - 1) / tb, tb, 0, ctx->stream>>>(pos, h.roff, B, h.foff);
+  LAUNCH_CHECK();
+  return GPDB_OK;
+}
+
 // Filter + voxelise the raw batch (M points; cloud b owns raw points roff[b] .. roff[b+1]-1, host offsets) into the arenas
 // of store s (reserved here once the output size is known). poff[B+1] (host) receives the processed offsets; a cloud the
 // filter empties keeps its place with no points. d_nrm_raw may be null. Every cloud goes through the steps on its own:
@@ -589,20 +615,14 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
                               int *poff, cudaEvent_t ev_filter_done) {
   const int tb = 256;
   // ---- removeNans + filterWorkspace, one scan for all clouds
-  // header: workspace [6 doubles], raw / filtered / processed offsets [B+1 each], bounds [6B], voxel error [2]
-  double *d_ws = (double *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2));
-  if (!d_ws) return GPDB_ERR_CUDA;
-  int *d_roff = (int *)(d_ws + 6), *d_foff = d_roff + B + 1, *d_poff = d_foff + B + 1, *d_bounds = d_poff + B + 1;
-  int *d_verr = d_bounds + 6 * B;
-  const int verr0[2] = {0, INT_MAX};
-  CUDA_TRY(cudaMemcpyAsync(d_ws, pp.workspace, sizeof(double) * 6, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(d_roff, roff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(d_verr, verr0, sizeof(verr0), cudaMemcpyHostToDevice, ctx->stream));
+  PreBatch h;
+  int rc = pre_batch_header(ctx, B, roff, pp, 0, h);
+  if (rc != GPDB_OK) return rc;
   int *flag = (int *)gpdb_scratch(ctx, SCR_WORK_B, sizeof(int) * (3 * (size_t)M + 2) + sizeof(float) * 3 * (size_t)M);
   if (!flag) return GPDB_ERR_CUDA;
   int *pos = flag + M + 1, *keep = pos + M + 1;
   float *xyz1 = (float *)(keep + M);
-  k_pre_flag<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, M, d_ws, flag);
+  k_pre_flag<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, M, h.ws, flag);
   LAUNCH_CHECK();
   CUDA_TRY(cudaMemsetAsync(flag + M, 0, sizeof(int), ctx->stream));  // pos[M] = number of filtered points
   size_t tmp_bytes = 0;
@@ -613,16 +633,27 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   ctx->launches += 2;
   k_pre_compact<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, flag, pos, M, keep, xyz1);
   LAUNCH_CHECK();
-  k_bpre_offsets<<<(B + 1 + tb - 1) / tb, tb, 0, ctx->stream>>>(pos, d_roff, B, d_foff);
-  LAUNCH_CHECK();
+  if ((rc = pre_filter_offsets(ctx, pos, h, B)) != GPDB_OK) return rc;
   std::vector<int> foff((size_t)B + 1);
-  CUDA_TRY(cudaMemcpyAsync(foff.data(), d_foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(foff.data(), h.foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
   cudaEventRecord(ev_filter_done, ctx->stream);
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return pre_voxelize_back(ctx, s, h, foff.data(), keep, xyz1, d_cam_raw, d_nrm_raw, B, pp, poff);
+}
+
+// The back of pre_filter_voxelize_batch, after the filter: voxelise (or, with voxelize = 0, gather) the filtered points
+// into the arenas of store s. foff[B+1] (host) = filtered offsets (also in h.foff), keep[k] = the raw index of filtered
+// point k in the call's numbering (made cloud-local with h.roff), xyz1 [3 * foff[B]] its coordinates; d_cam_raw /
+// d_nrm_raw are indexed by raw index.
+int pre_voxelize_back(gpdb_ctx *ctx, CloudSet &s, const PreBatch &h, const int *foff, const int *keep, const float *xyz1,
+                      const uint8_t *d_cam_raw, const double *d_nrm_raw, int B, const gpdb_preprocess_params &pp, int *poff) {
+  const int tb = 256;
+  const int *d_roff = h.roff, *d_foff = h.foff;
+  int *d_poff = h.poff, *d_bounds = h.bounds, *d_verr = h.verr;
   const int M1 = foff[B];
 
   if (!pp.voxelize || M1 == 0) {
-    memcpy(poff, foff.data(), sizeof(int) * ((size_t)B + 1));
+    memcpy(poff, foff, sizeof(int) * ((size_t)B + 1));
     int rc = gpdb_cloud_reserve(ctx, s, (size_t)M1, B);
     if (rc != GPDB_OK || M1 == 0) return rc;
     k_bgather_plain<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(keep, M1, d_foff, d_roff, B, xyz1, d_cam_raw, d_nrm_raw,
@@ -654,7 +685,7 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   if (cloud_bits) cub::DeviceRadixSort::SortPairs(nullptr, t2, ck, ck2, vals2, vals3, M1, 0, cloud_bits, ctx->stream);
   cub::DeviceScan::InclusiveSum(nullptr, t3, head, gid, M1, ctx->stream);
   cub::DeviceRadixSort::SortPairs(nullptr, t4, gord_k, gord_k2, gord_v, gord_v2, M1, 0, 32 + cloud_bits, ctx->stream);
-  tmp = gpdb_scratch(ctx, SCR_CUB, std::max(std::max(t1, t2), std::max(t3, t4)));
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, std::max(std::max(t1, t2), std::max(t3, t4)));
   if (!tmp) return GPDB_ERR_CUDA;
   // (cloud, key, index) order: the key sort keeps index order among equal keys, the cloud sort keeps key order. keys2
   // holds the keys in the final order: the key sort leaves them so, and after a cloud sort they are gathered into its order.

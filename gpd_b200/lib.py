@@ -29,7 +29,8 @@ EXPORTS = [
     "gpdb_find_clusters_batch", "gpdb_preprocess_clouds_device", "gpdb_set_clouds_device", "gpdb_detect_batch_select_device",
     "gpdb_find_clusters_batch_device", "gpdb_sis_params_default", "gpdb_sis_batch", "gpdb_sis_batch_device",
     "gpdb_sis_positions", "gpdb_set_clouds_samples_device", "gpdb_hand_search_batch_device", "gpdb_detect_batch_device",
-    "gpdb_images_batch_device", "gpdb_classify_device",
+    "gpdb_images_batch_device", "gpdb_classify_device", "gpdb_preprocess_depth", "gpdb_preprocess_depth_device",
+    "gpdb_subsample_clouds", "gpdb_subsample_clouds_device",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -114,7 +115,7 @@ def lib():
     L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
-    for name, argtypes in abi.RESIDENT_PROTOTYPES.items():
+    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES}.items():
         getattr(L, name).argtypes = argtypes
     _LIB = L
     return L
@@ -217,6 +218,29 @@ def pack_clouds(clouds):
             "cam_source": cam, "n_cameras": ks, "view_points": np.ascontiguousarray(np.concatenate(vps))}
 
 
+def depth_camera(width, height, fx, fy, cx, cy, pose=None, depth_scale=0.001, min_depth=0.0, max_depth=float("inf")):
+    """A gpdb_depth_camera (include/gpd_b200_depth.h): pinhole intrinsics in pixels, pose = camera-to-world [R | t] as a
+    3 x 4 (or 4 x 4) array, identity when None; depth_scale in metres per stored unit (0.001 for uint16 millimetres, 1.0
+    for float32 metres); a pixel is valid iff min_depth <= z <= max_depth."""
+    c = abi.DepthCamera()
+    c.width, c.height = int(width), int(height)
+    c.fx, c.fy, c.cx, c.cy = float(fx), float(fy), float(cx), float(cy)
+    P = np.eye(4)[:3] if pose is None else np.asarray(pose, dtype=np.float64)[:3, :4]
+    c.pose[:] = [float(v) for v in P.ravel()]
+    c.depth_scale, c.min_depth, c.max_depth = float(depth_scale), float(min_depth), float(max_depth)
+    return c
+
+
+def _depth_cameras(n_cameras, cameras):
+    ks = _host_i32("n_cameras", n_cameras)
+    cams = list(cameras)
+    if len(cams) != int(ks.sum()):
+        raise ValueError(f"cameras: {len(cams)} descriptions, need sum(n_cameras) = {int(ks.sum())}")
+    arr = (abi.DepthCamera * max(len(cams), 1))(*cams)
+    vps = np.array([[c.pose[3], c.pose[7], c.pose[11]] for c in cams], dtype=np.float64).reshape(-1, 3)
+    return ks, arr, vps
+
+
 def pack_samples(sample_lists):
     """The CSR arrays of gpdb_detect_batch for one list of cloud-local sample indices per cloud: (offsets [B+1], indices)."""
     arrs = [np.asarray(s, dtype=np.int32).ravel() for s in sample_lists]
@@ -290,6 +314,7 @@ class Context:
         self._batch = None  # (point offsets, camera counts, view point blocks, has source indices) of the installed batch
         self._stream = None  # the torch stream the *_tensors methods last moved the context to
         self._sis_shape = None  # (B, num_iterations) of the last successful SIS call: sizes sis_positions' arrays
+        self._n_raw = None  # raw points (pixels) of the preprocessing call that installed the batch: the length of a mask
 
     def close(self):
         if getattr(self, "h", None):
@@ -404,7 +429,7 @@ class Context:
     def set_clouds(self, clouds):
         """gpdb_set_clouds: installs a batch of processed clouds (list of dicts as set_cloud takes) beside the single cloud."""
         pk = pack_clouds(clouds)
-        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed gpdb_set_clouds leaves no batch
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed gpdb_set_clouds leaves no batch
         self._check(lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
                                           _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])))
         self._n_clouds = len(clouds)
@@ -420,12 +445,13 @@ class Context:
             pp = preprocess_params()
         B = len(raw_clouds)
         poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_preprocess_clouds(self.h, B, _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
                                                  _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"]), C.byref(pp),
                                                  _p(poff)))
         self._n_clouds = B
         self._batch = (poff, pk["n_cameras"], pk["view_points"], True)
+        self._n_raw = int(pk["offsets"][-1])
         return self.get_clouds() if read_back else poff
 
     def get_clouds(self):
@@ -586,17 +612,114 @@ class Context:
             pp = preprocess_params()
         B = len(ks)
         poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_preprocess_clouds_device(self.h, B, _p(off), px, pn, pc, _p(ks), _p(vp), C.byref(pp), _p(poff)))
         self._n_clouds = B
         self._batch = (poff, ks, vp, True)
+        self._n_raw = int(off[-1])
         return poff
+
+    def _install_depth(self, fn, n_cameras, cameras, fmt, ptr, pp):
+        ks, arr, vps = _depth_cameras(n_cameras, cameras)
+        if pp is None:
+            pp = preprocess_params()
+        B = len(ks)
+        poff = np.zeros(B + 1, np.int32)
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
+        self._check(fn(self.h, B, _p(ks), C.cast(arr, C.c_void_p), int(fmt), ptr, C.byref(pp), _p(poff)))
+        self._n_clouds = B
+        self._batch = (poff, ks, vps, True)
+        self._n_raw = sum(int(c.width) * int(c.height) for c in arr[:len(cameras)])
+        return poff
+
+    def preprocess_depth(self, views, pp=None, read_back=True):
+        """gpdb_preprocess_depth: preprocess_clouds() of views given as depth images. views: one list per view of
+        (image, camera) pairs, image a [height, width] uint16 or float32 array (one dtype for the whole call, which selects
+        GPDB_DEPTH_U16 / GPDB_DEPTH_F32), camera a depth_camera(). View b's raw cloud is its cameras' pixels concatenated
+        (include/gpd_b200_depth.h), so src indexes those pixels. Installs the processed batch; returns one dict per view as
+        preprocess_clouds() does, or the processed point offsets [B+1] when read_back is False."""
+        imgs, cams, ks = [], [], []
+        for view in views:
+            ks.append(len(view))
+            for img, cam in view:
+                imgs.append(np.asarray(img))
+                cams.append(cam)
+        dts = {a.dtype for a in imgs}
+        if len(dts) != 1 or next(iter(dts)) not in (np.dtype(np.uint16), np.dtype(np.float32)):
+            raise TypeError(f"preprocess_depth: need every image uint16 or every image float32, got {sorted(map(str, dts))}")
+        fmt = abi.DEPTH_U16 if next(iter(dts)) == np.uint16 else abi.DEPTH_F32
+        for i, (a, c) in enumerate(zip(imgs, cams)):
+            if a.shape != (c.height, c.width):
+                raise ValueError(f"preprocess_depth: image {i} has shape {a.shape}, its camera is {c.height} x {c.width}")
+        depth = np.ascontiguousarray(np.concatenate([a.ravel() for a in imgs]))
+        poff = self._install_depth(lib().gpdb_preprocess_depth, ks, cams, fmt, _p(depth), pp)
+        return self.get_clouds() if read_back else poff
+
+    def preprocess_depth_tensors(self, n_cameras, cameras, d_depth, pp=None):
+        """gpdb_preprocess_depth_device: preprocess_depth() of depth images held in ONE CUDA tensor, every camera's image
+        back to back in camera order (n_cameras [B] per view, cameras the sum(n_cameras) depth_camera()s, view by view).
+        The tensor's dtype selects the format: torch.uint16 (or int16 holding the same bits) or torch.float32. Installs the
+        processed batch; returns its point offsets [B+1]."""
+        import torch
+        cams = list(cameras)
+        n = sum(int(c.width) * int(c.height) for c in cams)
+        if not isinstance(d_depth, torch.Tensor):
+            raise ValueError(f"d_depth: need a tensor on cuda:{self.params.device}, got {type(d_depth).__name__}")
+        u16 = [d for d in (getattr(torch, "uint16", None), torch.int16) if d is not None]
+        if d_depth.dtype in u16:
+            fmt, dt = abi.DEPTH_U16, d_depth.dtype
+        elif d_depth.dtype == torch.float32:
+            fmt, dt = abi.DEPTH_F32, torch.float32
+        else:
+            raise TypeError(f"d_depth: need torch.uint16 or torch.float32, got {d_depth.dtype}")
+        ptr = _device_arg("d_depth", d_depth, dt, self.params.device, n)
+        self._torch_stream()
+        return self._install_depth(lib().gpdb_preprocess_depth_device, n_cameras, cams, fmt, ptr, pp)
+
+    def _subsample_room(self, num_samples):
+        npts = np.diff(self._batch[0]).astype(np.int64) if self._batch is not None else np.zeros(0, np.int64)
+        return int(npts.sum()) if num_samples == 0 else int(np.minimum(npts, max(int(num_samples), 0)).sum())
+
+    def subsample_clouds(self, num_samples, seed, mask=None):
+        """gpdb_subsample_clouds: Cloud::subsample of every installed cloud (include/gpd_b200_depth.h 5): num_samples
+        cloud-local point indices per cloud without replacement, ascending (0: every eligible point), drawn with key
+        seed + b. mask: one uint8 per raw point (pixel) of the preprocessing call that installed the batch, concatenated
+        by view, or None; only points whose source raw point has a nonzero byte are eligible. Returns one int32 array per
+        cloud, as detect_batch takes them."""
+        room = self._subsample_room(num_samples)
+        idx = np.zeros(max(room, 1), np.int32)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8).ravel()
+        if m is not None and self._n_raw is not None and len(m) != self._n_raw:
+            raise ValueError(f"mask: {len(m)} bytes, need one per raw point ({self._n_raw})")
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        self._check(lib().gpdb_subsample_clouds(self.h, int(num_samples), C.c_uint64(int(seed)), _p(m), _p(idx), _p(soff)))
+        return [idx[soff[b]:soff[b + 1]].copy() for b in range(self._n_clouds)]
+
+    def subsample_clouds_tensors(self, num_samples, seed, d_mask=None):
+        """gpdb_subsample_clouds_device: subsample_clouds() with the mask (uint8 CUDA tensor, one byte per raw point, or
+        None) on the device. Returns (offsets, indices): the host offsets [B+1] and an int32 CUDA tensor of the cloud-local
+        indices (cloud b's at offsets[b] .. offsets[b+1]-1), the CSR pair detect_batch_select_tensors / sis_batch_tensors
+        take."""
+        import torch
+        dev = self.params.device
+        if d_mask is not None:
+            n_raw = self._n_raw if self._n_raw is not None else (d_mask.numel() if isinstance(d_mask, torch.Tensor) else 0)
+            pm = _device_arg("d_mask", d_mask, torch.uint8, dev, int(n_raw))
+        else:
+            pm = None
+        self._torch_stream()
+        room = self._subsample_room(num_samples)
+        out = torch.empty(room, dtype=torch.int32, device=f"cuda:{dev}")
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        n = self._check(lib().gpdb_subsample_clouds_device(self.h, int(num_samples), C.c_uint64(int(seed)), pm,
+                                                           C.c_void_p(out.data_ptr()) if room else None, _p(soff)))
+        return soff, out[:n]
 
     def set_clouds_tensors(self, point_offsets, xyz, normals, n_cameras, view_points, cam_source=None):
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them
         (normals required)."""
         off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, False)
-        self._n_clouds, self._batch, self._sis_shape = 0, None, None  # a failed call leaves no batch
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
         self._check(lib().gpdb_set_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp)))
         self._n_clouds = len(ks)
         self._batch = (off, ks, vp, False)

@@ -330,7 +330,8 @@ void gpdb_preprocess_params_default(gpdb_preprocess_params *p);
  * (cloud extent / voxel_size) is GPDB_ERR_INVALID. After either error, or a rejected cam_source, the context holds
  * no cloud until the next successful gpdb_set_cloud / gpdb_preprocess.
  * Not covered: refine_normals_k, remove_outliers, sample_above_plane (PCL filters outside the default cfg) and
- * Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect).
+ * Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch draws them on the device with
+ * gpdb_subsample_clouds).
  * Semantics that differ from the reference by specification (DESIGN.md "preprocessing"): the voxel set is an
  * exact set (the reference's std::set comparator is not a strict weak order), output order = descending index
  * of each voxel's first point (the reference's iteration order whenever its de-duplication succeeds). */
@@ -521,6 +522,47 @@ int gpdb_sis_batch_device(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_
  * last one failed, or a batch was installed since (gpdb_set_clouds[_device], gpdb_preprocess_clouds[_device]). */
 int gpdb_sis_positions(gpdb_ctx *ctx, int32_t *eval_offsets_out, int32_t *eval_round_counts_out, double *eval_xyz_out,
                        int32_t *kept_offsets_out, double *kept_xyz_out);
+
+/* --- depth images and Cloud::subsample on the device (include/gpd_b200_depth.h) -----------------------------------------
+ * The two steps in front of and behind preprocessing that a depth-camera or simulator user would otherwise write: depth
+ * images -> gpdb_preprocess_depth[_device] -> gpdb_subsample_clouds[_device] -> gpdb_detect_batch_select[_device] ->
+ * gpdb_find_clusters_batch[_device], without leaving the GPU. The camera struct, the arithmetic, the raw-cloud numbering
+ * and the sampling rule are specified in gpd_b200_depth.h. */
+typedef struct gpdb_depth_camera gpdb_depth_camera;
+
+/* gpdb_preprocess_clouds of n_views views given as depth images: view b has n_cameras[b] cameras (1..8); cameras holds
+ * the sum of n_cameras host descriptions, view by view, and depth every camera's image back to back in the same order,
+ * all of one format (GPDB_DEPTH_U16 / GPDB_DEPTH_F32). View b's raw cloud is the concatenation of its cameras' pixels
+ * (gpd_b200_depth.h 3), and the call installs exactly what gpdb_preprocess_clouds installs from it (processed offsets
+ * to processed_offsets_out [B+1]; gpdb_get_clouds' src_out = pixel index into the view's concatenated images). The raw
+ * cloud is never built: back-projection runs inside the NaN / workspace filter. Failure rules of gpdb_preprocess_clouds
+ * (a failed call leaves no batch, drops the SIS record and the sample positions, never touches the single cloud). These
+ * are GPDB_ERR_INVALID before any device work, the message naming the view and camera: K_b outside 1..8, a width or
+ * height < 1, non-finite intrinsics or pose, fx or fy <= 0, depth_scale <= 0, min_depth < 0, max_depth <= min_depth, an
+ * unknown format, estimate_normals = 0, 2^31 or more pixels in the call, and the gpdb_preprocess_clouds parameter
+ * checks. The rotation of a pose is not checked for orthonormality. Returns B. */
+int gpdb_preprocess_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                          int32_t depth_format, const void *depth, const gpdb_preprocess_params *pp,
+                          int32_t *processed_offsets_out);
+/* The same with the images in device memory (d_depth on the context's device, read in place on the context's stream). */
+int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                                 int32_t depth_format, const void *d_depth, const gpdb_preprocess_params *pp,
+                                 int32_t *processed_offsets_out);
+
+/* Replaces: Cloud::subsample (cloud.cpp:350-370) for every cloud of the installed batch, by the rule of gpd_b200_depth.h
+ * 5: cloud b draws min(num_samples, eligible points) cloud-local point indices without replacement, in ascending order
+ * (num_samples = 0: every eligible point). mask (may be NULL) holds one byte per raw point of the preprocessing call that
+ * installed the batch (gpdb_preprocess_clouds[_device] / gpdb_preprocess_depth[_device]), concatenated by view; a point
+ * is eligible when the byte of its source raw point is nonzero. sample_idx_out has room for sum over b of min(num_samples,
+ * N_b) entries (N_b when num_samples = 0) and receives cloud b's draw at sample_offsets_out[b] .. sample_offsets_out[b+1]
+ * (B + 1 host entries): the CSR lists gpdb_detect_batch[_select][_device], gpdb_hand_search_batch[_device] and
+ * gpdb_sis_batch[_device] take. The batch is not changed. No batch, or a mask after gpdb_set_clouds[_device] (no source
+ * indices), is GPDB_ERR_STATE; a negative num_samples is GPDB_ERR_INVALID. Returns the number of indices. */
+int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *mask, int32_t *sample_idx_out,
+                          int32_t *sample_offsets_out);
+/* The same with the mask and the indices in device memory (sample_offsets_out stays a host array). */
+int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_mask,
+                                 int32_t *d_sample_idx_out, int32_t *sample_offsets_out);
 
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
