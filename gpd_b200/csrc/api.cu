@@ -8,7 +8,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/gpd_b200_depth.h"
@@ -547,6 +549,13 @@ static void camera_descs(int B, const int32_t *n_cameras, const double *view_poi
   }
 }
 
+// entry (row, k) of cloud b's cam_source block is neither 0 nor 1, which only voxelisation accepts
+static int cam_source_error(gpdb_ctx *ctx, const char *name, int b, long long row, long long k, int v) {
+  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must be 0 or 1",
+                 name, b, (int)row, (int)k, v);
+  return GPDB_ERR_INVALID;
+}
+
 int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
                       const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
                       CloudDesc *desc) {
@@ -567,11 +576,7 @@ int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off
       seen_by_all = pack_rows(rows, nb, K, dst, [](int32_t v) { return v > 0; });
     if (rows && strict01)
       for (size_t e = 0; e < (size_t)nb * K; e++)
-        if (rows[e] != 0 && rows[e] != 1) {
-          gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must "
-                         "be 0 or 1", name, b, (int)(e / K), (int)(e % K), (int)rows[e]);
-          return GPDB_ERR_INVALID;
-        }
+        if (rows[e] != 0 && rows[e] != 1) return cam_source_error(ctx, name, b, e / K, e % K, rows[e]);
     if (rows) rows += (size_t)nb * K;
     D.all_seen = (seen_by_all & all) == all ? 1 : 0;
   }
@@ -583,14 +588,15 @@ int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off
 static const unsigned long long NO_BAD = ~0ull;  // the check word when no position offends
 
 // every non-null pointer must be device (or managed) memory of the context's device; runs before any device work
-static int check_device_ptrs(gpdb_ctx *ctx, const char *name, int n, const char *const *names, const void *const *ptrs) {
-  for (int i = 0; i < n; i++) {
-    if (!ptrs[i]) continue;
+static int check_device_ptrs(gpdb_ctx *ctx, const char *name,
+                             std::initializer_list<std::pair<const char *, const void *>> ptrs) {
+  for (const auto &p : ptrs) {
+    if (!p.second) continue;
     cudaPointerAttributes a;
-    const cudaError_t e = cudaPointerGetAttributes(&a, ptrs[i]);
+    const cudaError_t e = cudaPointerGetAttributes(&a, p.second);
     if (e != cudaSuccess) cudaGetLastError();
     if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ctx->device) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s is not device memory of device %d", name, names[i], ctx->device);
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s is not device memory of device %d", name, p.first, ctx->device);
       return GPDB_ERR_INVALID;
     }
   }
@@ -610,6 +616,83 @@ static int first_bad(gpdb_ctx *ctx, size_t extra, unsigned long long *bad, Enque
   CUDA_TRY(cudaMemcpyAsync(bad, d_bad, sizeof(*bad), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return GPDB_OK;
+}
+
+// ---- the checks shared by the batch entry points and their _device twins ----------------------------------------------
+
+// what every call that installs a batch does first: a failed call leaves no batch, no sample positions and no SIS record
+// behind (the SIS positions describe clouds that are gone); the single cloud is never touched
+static void drop_batch(gpdb_ctx *ctx) {
+  ctx->many.n = 0;
+  ctx->many.has_src = false;
+  ctx->many.n_samples = 0;
+  gpdb_sis_forget(ctx);
+}
+
+// GPDB_ERR_STATE unless a batch is installed; hint names the calls that install one
+static int need_batch(gpdb_ctx *ctx, const char *name, const char *hint) {
+  if (ctx->many.n) return GPDB_OK;
+  gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call %s first", name, hint);
+  return GPDB_ERR_STATE;
+}
+
+// CSR offsets off[B+1] (the array `label`) from the host: they start at 0 and never decrease; entry b belongs to the b-th
+// `unit` (cloud or group). A call whose start message lists other arguments too checks the start itself first.
+static int check_offsets(gpdb_ctx *ctx, const char *name, const char *label, const int32_t *off, int B, const char *unit) {
+  if (!off || off[0] != 0) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need %s[%d] starting at 0", name, label, B + 1);
+    return GPDB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; b++)
+    if (off[b + 1] < off[b]) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s decrease at %s %d", name, label, unit, b);
+      return GPDB_ERR_INVALID;
+    }
+  return GPDB_OK;
+}
+
+// The cloud-local indices idx[off[b] .. off[b+1]) of cloud b of the installed batch must lie in [0, N_b + M_b), M_b its
+// sample positions. A host list (d_off null) is checked here; a device list by batch_check_samples, with d_off the offsets
+// on the device. Either way the first offending position is named. init: the initial indices of gpdb_sis_batch, which
+// has dropped the positions (M_b = 0) and names the indices so.
+static int check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *idx,
+                               const int *d_off) {
+  const CloudSet &s = ctx->many;
+  const int B = s.n, n = off[B];
+  std::vector<int> lim((size_t)B);
+  for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b] + s.positions(b);
+  unsigned long long bad = NO_BAD;
+  if (!d_off) {
+    for (int b = 0; b < B && bad == NO_BAD; b++)
+      for (int i = off[b]; i < off[b + 1]; i++)
+        if (idx[i] < 0 || idx[i] >= lim[b]) {
+          bad = i;
+          break;
+        }
+  } else if (n > 0) {
+    const int rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
+      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+      return batch_check_samples(ctx, idx, n, d_off, B, (const int *)d_lim, d_bad);
+    });
+    if (rc != GPDB_OK) return rc;
+  }
+  if (bad == NO_BAD) return GPDB_OK;
+  const int i = (int)bad;
+  int b = 0, v = 0;
+  while (off[b + 1] <= i) b++;
+  if (d_off) {
+    CUDA_TRY(cudaMemcpyAsync(&v, idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  } else {
+    v = idx[i];
+  }
+  const int nb = s.off[b + 1] - s.off[b];
+  if (init)
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name, v, i, b, nb);
+  else
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
+                   "positions)", name, v, i, b, nb, s.positions(b));
+  return GPDB_ERR_INVALID;
 }
 
 // gpdb_pack_cameras with cam_source (d_rows) and cam (d_cam) in device memory: the masks and each cloud's all_seen are
@@ -647,12 +730,17 @@ static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int
     CUDA_TRY(cudaMemcpyAsync(&v, d_rows + e, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     const long long r = (long long)e - h_roff[b];
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must be 0 or "
-                   "1", name, b, (int)(r / n_cameras[b]), (int)(r % n_cameras[b]), (int)v);
-    return GPDB_ERR_INVALID;
+    return cam_source_error(ctx, name, b, r / n_cameras[b], r % n_cameras[b], v);
   }
   for (int b = 0; b < B; b++) desc[b].all_seen = h_all[b];
   return GPDB_OK;
+}
+
+// point `point` of an install has a NaN or infinite coordinate
+static int nonfinite_error(gpdb_ctx *ctx, const char *name, unsigned long long point) {
+  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess first)",
+                 name, point);
+  return GPDB_ERR_INVALID;
 }
 
 // gpdb_set_clouds into store s after the argument checks (gpdb_set_cloud: `one`, a batch of one); `name` is the entry
@@ -662,11 +750,7 @@ static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t n_cl
                       const double *view_points) {
   const int N = point_offsets[n_clouds];
   for (size_t i = 0; i < 3 * (size_t)N; i++)
-    if (!std::isfinite(xyz[i])) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %zu has a non-finite coordinate (run removeNans / gpdb_preprocess "
-                     "first)", name, i / 3);
-      return GPDB_ERR_INVALID;
-    }
+    if (!std::isfinite(xyz[i])) return nonfinite_error(ctx, name, i / 3);
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   std::vector<uint8_t> cam((size_t)N);
@@ -694,11 +778,7 @@ static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
     return batch_first_nonfinite(ctx, d_xyz, 3 * (long long)N, d_bad);
   });
   if (rc != GPDB_OK) return rc;
-  if (bad != NO_BAD) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess "
-                   "first)", name, bad);
-    return GPDB_ERR_INVALID;
-  }
+  if (bad != NO_BAD) return nonfinite_error(ctx, name, bad);
   std::vector<CloudDesc> desc((size_t)B);
   rc = gpdb_cloud_reserve(ctx, s, (size_t)N, B);
   if (rc != GPDB_OK) return rc;
@@ -863,6 +943,19 @@ static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int
   return GPDB_OK;
 }
 
+// the preprocessing parameters, against the caller's normals (null: none)
+static int check_preprocess_params(gpdb_ctx *ctx, const char *name, const gpdb_preprocess_params *pp, const double *normals) {
+  if (!pp->estimate_normals && !normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals = 0 needs the caller's normals", name);
+    return GPDB_ERR_INVALID;
+  }
+  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: voxel_size and normals_radius must be positive", name);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
 extern "C" {
 
 int gpdb_set_cloud(gpdb_ctx *ctx, const float *xyz, const double *normals, const int32_t *cam_source, int32_t N,
@@ -897,18 +990,11 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
                    GPDB_MAX_CAMERAS);
     return GPDB_ERR_INVALID;
   }
-  if (!pp->estimate_normals && !normals) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess: estimate_normals = 0 needs the caller's normals");
-    return GPDB_ERR_INVALID;
-  }
-  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_preprocess: voxel_size and normals_radius must be positive");
-    return GPDB_ERR_INVALID;
-  }
+  int rc = check_preprocess_params(ctx, "gpdb_preprocess", pp, normals);
+  if (rc != GPDB_OK) return rc;
   const int32_t roff[2] = {0, M};
   int32_t poff[2] = {0, 0};
-  const int rc = preprocess_clouds(ctx, ctx->one, "gpdb_preprocess", 1, roff, xyz, normals, cam_source, &K, view_points, pp,
-                                 poff);
+  rc = preprocess_clouds(ctx, ctx->one, "gpdb_preprocess", 1, roff, xyz, normals, cam_source, &K, view_points, pp, poff);
   if (rc < 0) return rc;
   if (poff[1] == 0) {  // the filter kept no point: no cloud
     ctx->one.n = 0;
@@ -942,42 +1028,26 @@ static int set_clouds_samples(gpdb_ctx *ctx, const char *name, const int32_t *po
   if (!ctx) return GPDB_ERR_INVALID;
   CloudSet &s = ctx->many;
   s.n_samples = 0;  // past this point, a failed call leaves no positions behind
-  if (!s.n) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first", name);
-    return GPDB_ERR_STATE;
-  }
+  int rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds");
+  if (rc != GPDB_OK) return rc;
   const int B = s.n;
-  if (!pos_offsets || pos_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need pos_offsets[%d] starting at 0", name, B + 1);
-    return GPDB_ERR_INVALID;
-  }
-  for (int b = 0; b < B; b++)
-    if (pos_offsets[b + 1] < pos_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: pos_offsets decrease at cloud %d", name, b);
-      return GPDB_ERR_INVALID;
-    }
+  if ((rc = check_offsets(ctx, name, "pos_offsets", pos_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int M = pos_offsets[B];
   if (M > 0 && !samples) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null samples_xyz for %d positions", name, M);
     return GPDB_ERR_INVALID;
   }
-  if (device) {
-    const char *names[1] = {"d_samples_xyz"};
-    const void *ptrs[1] = {samples};
-    const int rc = check_device_ptrs(ctx, name, 1, names, ptrs);
-    if (rc != GPDB_OK) return rc;
-  }
+  if (device && (rc = check_device_ptrs(ctx, name, {{"d_samples_xyz", samples}})) != GPDB_OK) return rc;
   memcpy(s.pos, pos_offsets, sizeof(int) * ((size_t)B + 1));
   // each descriptor's first position: one strided copy into the pos field of the B device descriptors
   CUDA_TRY(cudaSetDevice(ctx->device));
   CUDA_TRY(cudaMemcpy2DAsync(&s.desc[0].pos, sizeof(CloudDesc), s.pos, sizeof(int), sizeof(int), (size_t)B,
                              cudaMemcpyHostToDevice, ctx->stream));
   if (!device) {
-    const int rc = upload_samples(ctx, s, samples, M);
+    rc = upload_samples(ctx, s, samples, M);
     return rc < 0 ? rc : M;
   }
-  const int rc = reserve_samples(ctx, s, M);
-  if (rc != GPDB_OK) return rc;
+  if ((rc = reserve_samples(ctx, s, M)) != GPDB_OK) return rc;
   if (M > 0)
     CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)M, cudaMemcpyDeviceToDevice, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
@@ -1490,20 +1560,17 @@ int gpdb_detect_resident(gpdb_ctx *ctx, const int32_t *d_sample_idx, int32_t n, 
 
 }  // extern "C"
 
-// the argument checks of gpdb_set_clouds[_device] after ctx (the caller has dropped the batch); `raw`: those of
-// gpdb_preprocess_clouds[_device]
-static int check_clouds_args(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
-                             const double *normals, const int32_t *n_cameras, const double *view_points,
-                             const gpdb_preprocess_params *pp, const int32_t *processed_offsets_out, bool raw) {
-  if (raw ? (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || !pp || !processed_offsets_out ||
-             point_offsets[0] != 0)
-          : (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !normals || !view_points || point_offsets[0] != 0)) {
-    if (raw)
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, "
-                     "view_points, params, processed_offsets_out", name);
-    else
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, normals, "
-                     "view_points", name);
+// gpdb_set_clouds[_device] and, raw, gpdb_preprocess_clouds[_device]: drop the batch, check the arguments (device: the d_*
+// pointers too), then install or preprocess into the batch store
+static int clouds_entry(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
+                        const double *normals, const int32_t *cam_source, const int32_t *n_cameras, const double *view_points,
+                        const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool raw, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  drop_batch(ctx);
+  if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || point_offsets[0] != 0 ||
+      (raw ? !pp || !processed_offsets_out : !normals)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, %s", name,
+                   raw ? "view_points, params, processed_offsets_out" : "normals, view_points");
     return GPDB_ERR_INVALID;
   }
   for (int b = 0; b < n_clouds; b++) {
@@ -1518,93 +1585,53 @@ static int check_clouds_args(gpdb_ctx *ctx, const char *name, int32_t n_clouds, 
       return GPDB_ERR_INVALID;
     }
   }
-  if (!raw) return GPDB_OK;
-  if (!pp->estimate_normals && !normals) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals = 0 needs the caller's normals", name);
-    return GPDB_ERR_INVALID;
-  }
-  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || (pp->estimate_normals && !(pp->normals_radius > 0.0))) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: voxel_size and normals_radius must be positive", name);
-    return GPDB_ERR_INVALID;
-  }
-  return GPDB_OK;
+  int rc = raw ? check_preprocess_params(ctx, name, pp, normals) : GPDB_OK;
+  if (rc == GPDB_OK && device)
+    rc = check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals", normals}, {"d_cam_source", cam_source}});
+  if (rc != GPDB_OK) return rc;
+  CloudSet &s = ctx->many;
+  if (raw)
+    return preprocess_clouds(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
+                             processed_offsets_out, device);
+  if (device)
+    return set_clouds_device(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
+  return set_clouds(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
 }
 
 extern "C" {
 
 int gpdb_set_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz, const double *normals,
                     const int32_t *cam_source, const int32_t *n_cameras, const double *view_points) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is untouched either way
-  gpdb_sis_forget(ctx);  // the SIS positions describe clouds that are gone
-  ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
-  const char *name = "gpdb_set_clouds";
-  const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, nullptr, nullptr,
-                                   false);
-  if (rc != GPDB_OK) return rc;
-  return set_clouds(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
+  return clouds_entry(ctx, "gpdb_set_clouds", n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points,
+                      nullptr, nullptr, false, false);
 }
 
 int gpdb_set_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
                            const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
                            const double *view_points) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  ctx->many.n = 0;
-  gpdb_sis_forget(ctx);
-  ctx->many.n_samples = 0;
-  const char *name = "gpdb_set_clouds_device";
-  int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, d_xyz, d_normals, n_cameras, view_points, nullptr, nullptr,
-                             false);
-  const char *names[3] = {"d_xyz", "d_normals", "d_cam_source"};
-  const void *ptrs[3] = {d_xyz, d_normals, d_cam_source};
-  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 3, names, ptrs);
-  if (rc != GPDB_OK) return rc;
-  return set_clouds_device(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
-                           view_points);
+  return clouds_entry(ctx, "gpdb_set_clouds_device", n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
+                      view_points, nullptr, nullptr, false, true);
 }
 
 int gpdb_preprocess_clouds(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *xyz,
                            const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
                            const double *view_points, const gpdb_preprocess_params *pp, int32_t *processed_offsets_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
-  gpdb_sis_forget(ctx);
-  ctx->many.has_src = false;
-  ctx->many.n_samples = 0;  // a new batch, or none, drops the positions
-  const char *name = "gpdb_preprocess_clouds";
-  const int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, xyz, normals, n_cameras, view_points, pp,
-                                   processed_offsets_out, true);
-  if (rc != GPDB_OK) return rc;
-  return preprocess_clouds(ctx, ctx->many, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
-                         processed_offsets_out);
+  return clouds_entry(ctx, "gpdb_preprocess_clouds", n_clouds, point_offsets, xyz, normals, cam_source, n_cameras,
+                      view_points, pp, processed_offsets_out, true, false);
 }
 
 int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *point_offsets, const float *d_xyz,
                                   const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
                                   const double *view_points, const gpdb_preprocess_params *pp,
                                   int32_t *processed_offsets_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  ctx->many.n = 0;
-  gpdb_sis_forget(ctx);
-  ctx->many.has_src = false;
-  ctx->many.n_samples = 0;
-  const char *name = "gpdb_preprocess_clouds_device";
-  int rc = check_clouds_args(ctx, name, n_clouds, point_offsets, d_xyz, d_normals, n_cameras, view_points, pp,
-                             processed_offsets_out, true);
-  const char *names[3] = {"d_xyz", "d_normals", "d_cam_source"};
-  const void *ptrs[3] = {d_xyz, d_normals, d_cam_source};
-  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 3, names, ptrs);
-  if (rc != GPDB_OK) return rc;
-  return preprocess_clouds(ctx, ctx->many, name, n_clouds, point_offsets, d_xyz, d_normals, d_cam_source, n_cameras,
-                         view_points, pp, processed_offsets_out, true);
+  return clouds_entry(ctx, "gpdb_preprocess_clouds_device", n_clouds, point_offsets, d_xyz, d_normals, d_cam_source,
+                      n_cameras, view_points, pp, processed_offsets_out, true, true);
 }
 
 int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out, int32_t *src_out) {
   if (!ctx) return GPDB_ERR_INVALID;
-  if (ctx->many.n == 0) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_get_clouds: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first");
-    return GPDB_ERR_STATE;
-  }
+  const int rc = need_batch(ctx, "gpdb_get_clouds", "gpdb_set_clouds / gpdb_preprocess_clouds");
+  if (rc != GPDB_OK) return rc;
   if (src_out && !ctx->many.has_src) {
     gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_get_clouds: source indices exist after gpdb_preprocess_clouds only");
     return GPDB_ERR_STATE;
@@ -1633,10 +1660,8 @@ static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const in
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
     return GPDB_ERR_INVALID;
   }
-  if ((pp->voxelize && !(pp->voxel_size > 0.0)) || !(pp->normals_radius > 0.0)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: voxel_size and normals_radius must be positive", name);
-    return GPDB_ERR_INVALID;
-  }
+  const int rc = check_preprocess_params(ctx, name, pp, nullptr);
+  if (rc != GPDB_OK) return rc;
   roff.assign((size_t)B + 1, 0);
   long long total = 0;
   for (int b = 0, c = 0; b < B; b++) {
@@ -1706,17 +1731,10 @@ static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const i
                        const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
                        const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device) {
   if (!ctx) return GPDB_ERR_INVALID;
-  ctx->many.n = 0;  // a failed call leaves no batch behind; the single cloud is never touched
-  gpdb_sis_forget(ctx);
-  ctx->many.has_src = false;
-  ctx->many.n_samples = 0;
+  drop_batch(ctx);
   std::vector<int> roff;
   int rc = check_depth_args(ctx, name, n_views, n_cameras, cameras, depth_format, depth, pp, processed_offsets_out, roff);
-  if (rc == GPDB_OK && device) {
-    const char *names[1] = {"d_depth"};
-    const void *ptrs[1] = {depth};
-    rc = check_device_ptrs(ctx, name, 1, names, ptrs);
-  }
+  if (rc == GPDB_OK && device) rc = check_device_ptrs(ctx, name, {{"d_depth", depth}});
   if (rc != GPDB_OK) return rc;
   return preprocess_depth(ctx, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
                           processed_offsets_out);
@@ -1728,11 +1746,8 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
                            int32_t *idx_out, int32_t *offsets_out, bool device) {
   if (!ctx) return GPDB_ERR_INVALID;
   CloudSet &s = ctx->many;
-  if (s.n == 0) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_preprocess_depth / gpdb_preprocess_clouds first",
-                   name);
-    return GPDB_ERR_STATE;
-  }
+  int rc = need_batch(ctx, name, "gpdb_preprocess_depth / gpdb_preprocess_clouds");
+  if (rc != GPDB_OK) return rc;
   if (num_samples < 0 || !offsets_out) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need num_samples >= 0 (got %d) and sample_offsets_out", name, num_samples);
     return GPDB_ERR_INVALID;
@@ -1752,12 +1767,7 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, device ? "d_sample_idx_out" : "sample_idx_out");
     return GPDB_ERR_INVALID;
   }
-  if (device) {
-    const char *names[2] = {"d_mask", "d_sample_idx_out"};
-    const void *ptrs[2] = {mask, idx_out};
-    const int rc = check_device_ptrs(ctx, name, 2, names, ptrs);
-    if (rc != GPDB_OK) return rc;
-  }
+  if (device && (rc = check_device_ptrs(ctx, name, {{"d_mask", mask}, {"d_sample_idx_out", idx_out}})) != GPDB_OK) return rc;
   CUDA_TRY(cudaSetDevice(ctx->device));
   const uint8_t *d_mask = mask;
   int *d_out = idx_out;
@@ -1826,20 +1836,13 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
   int rc = gpdb_check_state(ctx, false, with_images_and_scores);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
-  if (s.n == 0) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds first", name);
-    return GPDB_ERR_STATE;
-  }
+  if ((rc = need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
   const int B = s.n;
   if (!out || !sample_offsets || sample_offsets[0] != 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need out and sample_offsets[%d] starting at 0", name, B + 1);
     return GPDB_ERR_INVALID;
   }
-  for (int b = 0; b < B; b++)
-    if (sample_offsets[b + 1] < sample_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample_offsets decrease at cloud %d", name, b);
-      return GPDB_ERR_INVALID;
-    }
+  if ((rc = check_offsets(ctx, name, "sample_offsets", sample_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int n = sample_offsets[B];
   if (n > 0 && !sample_idx) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null sample_idx", name);
@@ -1850,41 +1853,14 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, sel_name);
       return GPDB_ERR_INVALID;
     }
-    const char *names[4] = {"d_sample_idx", sel_name, "d_flags_out", "d_scores_out"};
-    const void *ptrs[4] = {sample_idx, sel_out, d_flags, d_scores};
-    if ((rc = check_device_ptrs(ctx, name, 4, names, ptrs)) != GPDB_OK) return rc;
+    rc = check_device_ptrs(ctx, name, {{"d_sample_idx", sample_idx}, {sel_name, sel_out}, {"d_flags_out", d_flags},
+                                       {"d_scores_out", d_scores}});
   } else {
-    for (int b = 0; b < B; b++) {
-      const int nb = s.off[b + 1] - s.off[b], mb = s.positions(b);  // N_b points, then M_b positions
-      for (int i = sample_offsets[b]; i < sample_offsets[b + 1]; i++)
-        if (sample_idx[i] < 0 || sample_idx[i] >= nb + mb) {
-          gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
-                         "positions)", name, sample_idx[i], i, b, nb, mb);
-          return GPDB_ERR_INVALID;
-        }
-    }
+    rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, nullptr);
   }
+  if (rc != GPDB_OK) return rc;
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if (device && n > 0) {  // the same check on the device: the first offending position, then its cloud and value
-    std::vector<int> lim((size_t)B);
-    for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b] + s.positions(b);
-    unsigned long long bad;
-    rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
-      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
-      return batch_check_samples(ctx, sample_idx, n, s.soff, B, (const int *)d_lim, d_bad);
-    });
-    if (rc != GPDB_OK) return rc;
-    if (bad != NO_BAD) {
-      const int i = (int)bad;
-      int b = 0, v = 0;
-      while (sample_offsets[b + 1] <= i) b++;
-      CUDA_TRY(cudaMemcpyAsync(&v, sample_idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
-      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sample index %d at position %d outside cloud %d (N = %d, + %d sample "
-                     "positions)", name, v, i, b, s.off[b + 1] - s.off[b], s.positions(b));
-      return GPDB_ERR_INVALID;
-    }
-  }
+  if (device && (rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, s.soff)) != GPDB_OK) return rc;
   PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = device, .per_cloud = true,
                     .classify = with_images_and_scores, .d_flags = d_flags, .d_scores = d_scores,
                     .dest = select_k < 0 ? (device ? PIPE_ALL_CALLER : PIPE_TO_HOST) : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
@@ -1979,28 +1955,15 @@ int gpdb_images_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, const g
   int rc = gpdb_check_state(ctx, false, false);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
-  if (s.n == 0) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds first", name);
-    return GPDB_ERR_STATE;
-  }
+  if ((rc = need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
   const int B = s.n;
-  if (!hand_offsets || hand_offsets[0] != 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need hand_offsets[%d] starting at 0", name, B + 1);
-    return GPDB_ERR_INVALID;
-  }
-  for (int b = 0; b < B; b++)
-    if (hand_offsets[b + 1] < hand_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: hand_offsets decrease at cloud %d", name, b);
-      return GPDB_ERR_INVALID;
-    }
+  if ((rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int n = hand_offsets[B];
   if (n > 0 && (!d_hands || !d_images_out)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands or d_images_out", name);
     return GPDB_ERR_INVALID;
   }
-  const char *names[2] = {"d_hands", "d_images_out"};
-  const void *ptrs[2] = {d_hands, d_images_out};
-  if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+  if ((rc = check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_images_out", d_images_out}})) != GPDB_OK) return rc;
   if (n == 0) return 0;
   CUDA_TRY(cudaMemcpyAsync(s.soff, hand_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   const size_t isz = (size_t)ctx->hp.S * ctx->hp.S * ctx->hp.C, psz = (size_t)ctx->hp.S * ctx->hp.S * 16;
@@ -2162,9 +2125,9 @@ int gpdb_classify_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, int32_t n, 
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: bad arguments", name);
     return GPDB_ERR_INVALID;
   }
-  const char *names[3] = {"d_images_hwc", "d_scores_out", "d_logits_out"};
-  const void *ptrs[3] = {d_images_hwc, d_scores_out, d_logits_out};
-  if ((rc = check_device_ptrs(ctx, name, 3, names, ptrs)) != GPDB_OK) return rc;
+  rc = check_device_ptrs(ctx, name, {{"d_images_hwc", d_images_hwc}, {"d_scores_out", d_scores_out},
+                                     {"d_logits_out", d_logits_out}});
+  if (rc != GPDB_OK) return rc;
   return classify_batches(ctx, d_images_hwc, n, d_scores_out, d_logits_out, nullptr, true);
 }
 
@@ -2262,11 +2225,8 @@ static int check_groups_args(gpdb_ctx *ctx, const char *name, int32_t n_groups, 
                    "cluster_offsets_out", name);
     return GPDB_ERR_INVALID;
   }
-  for (int g = 0; g < n_groups; g++)
-    if (hand_offsets[g + 1] < hand_offsets[g]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: hand_offsets decrease at group %d", name, g);
-      return GPDB_ERR_INVALID;
-    }
+  const int rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, n_groups, "group");
+  if (rc != GPDB_OK) return rc;
   if (hand_offsets[n_groups] > 0 && (!hands || !clusters_out)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null hands or clusters_out", name);
     return GPDB_ERR_INVALID;
@@ -2290,9 +2250,7 @@ int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32
   if (!ctx) return GPDB_ERR_INVALID;
   const char *name = "gpdb_find_clusters_batch_device";
   int rc = check_groups_args(ctx, name, n_groups, hand_offsets, d_hands, d_clusters_out, cluster_offsets_out);
-  const char *names[2] = {"d_hands", "d_clusters_out"};
-  const void *ptrs[2] = {d_hands, d_clusters_out};
-  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, 2, names, ptrs);
+  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_clusters_out", d_clusters_out}});
   if (rc != GPDB_OK) return rc;
   return find_clusters(ctx, n_groups, hand_offsets, d_hands, min_inliers, d_clusters_out, cluster_offsets_out, true);
 }
@@ -2344,11 +2302,8 @@ static int check_sis_args(gpdb_ctx *ctx, const char *name, int B, const gpdb_sis
                    sp->sampling_method);
     return GPDB_ERR_INVALID;
   }
-  for (int b = 0; b < B; b++)
-    if (init_offsets[b + 1] < init_offsets[b]) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init_offsets decrease at cloud %d", name, b);
-      return GPDB_ERR_INVALID;
-    }
+  const int rc = check_offsets(ctx, name, "init_offsets", init_offsets, B, "cloud");
+  if (rc != GPDB_OK) return rc;
   if (init_offsets[B] > 0 && !init_idx) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null init_idx", name);
     return GPDB_ERR_INVALID;
@@ -2490,30 +2445,19 @@ static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp,
   int rc = gpdb_check_state(ctx, false, true);
   if (rc != GPDB_OK) return rc;
   if (!ctx->sis) ctx->sis = new SisState();
-  if (s.n == 0) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call gpdb_set_clouds / gpdb_preprocess_clouds first", name);
-    return GPDB_ERR_STATE;
-  }
+  if ((rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds")) != GPDB_OK) return rc;
   const int B = s.n;
   if ((rc = check_sis_args(ctx, name, B, sp, init_offsets, init_idx, out, hand_offsets_out)) != GPDB_OK) return rc;
   const int n0 = init_offsets[B];
   if (device) {
-    const char *names[2] = {"d_init_idx", "d_hands_out"};
-    const void *ptrs[2] = {init_idx, d_hands_out};
-    if ((rc = check_device_ptrs(ctx, name, 2, names, ptrs)) != GPDB_OK) return rc;
+    if ((rc = check_device_ptrs(ctx, name, {{"d_init_idx", init_idx}, {"d_hands_out", d_hands_out}})) != GPDB_OK) return rc;
     const long long kc = (long long)n0 + (long long)B * sp->num_iterations * sp->num_samples_per_iteration;
     if (kc > 0 && !d_hands_out) {
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands_out", name);
       return GPDB_ERR_INVALID;
     }
-  } else {
-    for (int b = 0; b < B; b++)
-      for (int i = init_offsets[b]; i < init_offsets[b + 1]; i++)
-        if (init_idx[i] < 0 || init_idx[i] >= s.off[b + 1] - s.off[b]) {
-          gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name,
-                         init_idx[i], i, b, s.off[b + 1] - s.off[b]);
-          return GPDB_ERR_INVALID;
-        }
+  } else if ((rc = check_cloud_indices(ctx, name, true, init_offsets, init_idx, nullptr)) != GPDB_OK) {
+    return rc;
   }
   SisState &st = *ctx->sis;
   const int R = sp->num_iterations, S = sp->num_samples_per_iteration;
@@ -2526,25 +2470,7 @@ static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp,
     CUDA_TRY(cudaMemcpyAsync(a.init_idx, init_idx, sizeof(int) * (size_t)n0,
                              device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemsetAsync(a.kcount, 0, sizeof(int) * (size_t)B * (R + 1), ctx->stream));  // kept and round counts
-  if (device && n0 > 0) {  // the init indices on the device: the first offending position, then its cloud and value
-    std::vector<int> lim((size_t)B);
-    for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b];
-    unsigned long long bad;
-    rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
-      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
-      return batch_check_samples(ctx, a.init_idx, n0, a.init_off, B, (const int *)d_lim, d_bad);
-    });
-    if (rc != GPDB_OK) return rc;
-    if (bad != NO_BAD) {
-      const int i = (int)bad;
-      int b = 0, v = 0;
-      while (init_offsets[b + 1] <= i) b++;
-      CUDA_TRY(cudaMemcpyAsync(&v, a.init_idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
-      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name, v, i, b, lim[b]);
-      return GPDB_ERR_INVALID;
-    }
-  }
+  if (device && (rc = check_cloud_indices(ctx, name, true, init_offsets, a.init_idx, a.init_off)) != GPDB_OK) return rc;
   st.B = B;
   st.R = R;
   st.S = S;
