@@ -188,6 +188,28 @@ DEPTH_PROTOTYPES = {
 }
 
 
+class PlaneParams(C.Structure):
+    """gpdb_plane_params (include/gpd_b200.h, rules in include/gpd_b200_plane.h)."""
+
+    _fields_ = [
+        ("distance_threshold", C.c_double),
+        ("max_iterations", C.c_int32),
+        ("probability", C.c_double),
+        ("seed", C.c_uint64),
+    ]
+
+
+# gpdb_segment_plane[s][_device], gpdb_subsample_clouds_points[_device] (include/gpd_b200.h)
+PLANE_PROTOTYPES = {
+    "gpdb_plane_params_default": [C.POINTER(PlaneParams)],
+    "gpdb_segment_plane": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_segment_planes": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_segment_planes_device": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_subsample_clouds_points": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
+    "gpdb_subsample_clouds_points_device": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
+}
+
+
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""
     p = PreprocessParams()

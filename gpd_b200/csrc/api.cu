@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/gpd_b200_depth.h"
+#include "../../include/gpd_b200_plane.h"
 #include "common.cuh"
 
 static char g_create_err[512] = "";
@@ -1743,7 +1744,7 @@ static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const i
 // gpdb_subsample_clouds[_device]: the state and argument checks, then the device draw (the host twin uploads the mask and
 // copies the indices back)
 static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples, uint64_t seed, const uint8_t *mask,
-                           int32_t *idx_out, int32_t *offsets_out, bool device) {
+                           int32_t *idx_out, int32_t *offsets_out, bool device, bool per_point = false) {
   if (!ctx) return GPDB_ERR_INVALID;
   CloudSet &s = ctx->many;
   int rc = need_batch(ctx, name, "gpdb_preprocess_depth / gpdb_preprocess_clouds");
@@ -1752,7 +1753,7 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need num_samples >= 0 (got %d) and sample_offsets_out", name, num_samples);
     return GPDB_ERR_INVALID;
   }
-  if (mask && !s.has_src) {
+  if (mask && !per_point && !s.has_src) {
     gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: a mask needs the source indices of a preprocessing call (gpdb_preprocess_depth "
                    "/ gpdb_preprocess_clouds); the batch was installed by gpdb_set_clouds", name);
     return GPDB_ERR_STATE;
@@ -1773,7 +1774,7 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
   int *d_out = idx_out;
   if (!device) {
     if (mask) {
-      const size_t M = (size_t)s.raw_off[B];
+      const size_t M = per_point ? (size_t)s.points() : (size_t)s.raw_off[B];
       uint8_t *up = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, M);
       if (!up) return GPDB_ERR_CUDA;
       CUDA_TRY(cudaMemcpyAsync(up, mask, M, cudaMemcpyHostToDevice, ctx->stream));
@@ -1783,7 +1784,7 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
     if (!d_out) return GPDB_ERR_CUDA;
   }
   std::vector<int> soff((size_t)B + 1);
-  const int n = sub_draw_batch(ctx, s, num_samples, seed, d_mask, d_out, soff.data());
+  const int n = sub_draw_batch(ctx, s, num_samples, seed, d_mask, per_point, d_out, soff.data());
   if (n < 0) return n;
   if (!device && n > 0) {
     CUDA_TRY(cudaMemcpyAsync(idx_out, d_out, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1818,6 +1819,90 @@ int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t se
                                  int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
   return subsample_entry(ctx, "gpdb_subsample_clouds_device", num_samples, seed, d_mask, d_sample_idx_out,
                          sample_offsets_out, true);
+}
+
+int gpdb_subsample_clouds_points(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *point_mask,
+                                 int32_t *sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_points", num_samples, seed, point_mask, sample_idx_out,
+                         sample_offsets_out, false, true);
+}
+
+int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_point_mask,
+                                        int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_points_device", num_samples, seed, d_point_mask, d_sample_idx_out,
+                         sample_offsets_out, true, true);
+}
+
+}  // extern "C"
+
+// ---- the support plane (include/gpd_b200_plane.h) ----------------------------------------------------------------------
+
+// gpdb_segment_plane / gpdb_segment_planes[_device]: the state and argument checks, then plane_segment_batch on the
+// single cloud (single) or the batch. The host twins let the eligible bytes come back through SCR_UPLOAD.
+static int segment_entry(gpdb_ctx *ctx, const char *name, bool single, const gpdb_plane_params *pl, float *planes_out,
+                         int32_t *n_inliers_out, int32_t *n_hyp_out, uint8_t *eligible_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (!pl || !planes_out || !n_inliers_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need params, %s and n_inliers_out", name, single ? "plane_out" : "planes_out");
+    return GPDB_ERR_INVALID;
+  }
+  const char *bad = nullptr;
+  if (!std::isfinite(pl->distance_threshold) || !(pl->distance_threshold > 0.0))
+    bad = "distance_threshold must be finite and positive";
+  else if (pl->max_iterations < 1 || pl->max_iterations > GPDB_PLANE_MAX_ITERATIONS)
+    bad = "max_iterations must lie in 1..1024";
+  else if (!(pl->probability > 0.0 && pl->probability < 1.0))
+    bad = "probability must lie in (0, 1)";
+  if (bad) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s", name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  if (device && (rc = check_device_ptrs(ctx, name, {{"d_eligible_out", eligible_out}})) != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const int N = s.points();
+  uint8_t *d_elig = eligible_out;
+  if (!device && eligible_out) {
+    d_elig = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, (size_t)N + 16);
+    if (!d_elig) return GPDB_ERR_CUDA;
+  }
+  rc = plane_segment_batch(ctx, s, *pl, planes_out, n_inliers_out, n_hyp_out, d_elig);
+  if (rc < 0) return rc;
+  if (!device && eligible_out && N > 0) {
+    CUDA_TRY(cudaMemcpyAsync(eligible_out, d_elig, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  return rc;
+}
+
+extern "C" {
+
+void gpdb_plane_params_default(gpdb_plane_params *p) {
+  if (!p) return;
+  p->distance_threshold = 0.01;
+  p->max_iterations = 50;
+  p->probability = 0.99;
+  p->seed = 0;
+}
+
+int gpdb_segment_plane(gpdb_ctx *ctx, const gpdb_plane_params *pl, float plane_out[4], int32_t *n_inliers_out,
+                       uint8_t *eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_plane", true, pl, plane_out, n_inliers_out, nullptr, eligible_out, false);
+}
+
+int gpdb_segment_planes(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                        int32_t *n_hypotheses_out, uint8_t *eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_planes", false, pl, planes_out, n_inliers_out, n_hypotheses_out, eligible_out,
+                       false);
+}
+
+int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                               int32_t *n_hypotheses_out, uint8_t *d_eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_planes_device", false, pl, planes_out, n_inliers_out, n_hypotheses_out,
+                       d_eligible_out, true);
 }
 
 }  // extern "C"

@@ -234,8 +234,11 @@ enum ScratchSlot {
   // gpdb_sis_batch: kept / evaluated positions, the round's sample lists and counts (main stream, between pipeline calls;
   // read again by gpdb_sis_positions)
   SCR_SIS,
-  // host twins of gpdb_preprocess_depth / gpdb_subsample_clouds: the uploaded depth images, the uploaded mask
+  // host twins of gpdb_preprocess_depth / gpdb_subsample_clouds[_points] / gpdb_segment_plane[s]: the uploaded depth
+  // images, the uploaded mask, the eligible bytes on their way back
   SCR_UPLOAD,
+  // gpdb_segment_plane[s]: hypotheses, their inlier counts, the picked and refined planes (plane.cu)
+  SCR_PLANE,
   SCR_N
 };
 
@@ -444,10 +447,15 @@ int pre_voxelize_back(gpdb_ctx *ctx, CloudSet &s, const PreBatch &h, const int *
 int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format, const gpdb_depth_camera *cams,
                     const int *n_cameras, int B, const int *roff, const gpdb_preprocess_params &pp, int *poff,
                     cudaEvent_t ev_filter_done);
-// Cloud::subsample of every cloud of store s (has_src when d_mask is given; mask indexed by the store's raw_off): cloud
-// b's draw to d_out at soff[b] (host, B + 1); returns the total or an error
+// Cloud::subsample of every cloud of store s: cloud b's draw to d_out at soff[b] (host, B + 1); returns the total or an
+// error. d_mask: one byte per installed point (per_point), or per raw point indexed by the store's raw_off (has_src)
 int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned long long seed, const uint8_t *d_mask,
-                   int *d_out, int *soff);
+                   bool per_point, int *d_out, int *soff);
+
+// plane.cu (include/gpd_b200_plane.h). Segments every cloud of store s (cloud b with key pp.seed + b): planes[4B],
+// n_inliers[B] and n_hyp[B] (may be null) are host arrays, d_eligible (N bytes or null) device memory. Returns B.
+int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_params &pp, float *planes, int *n_inliers,
+                        int *n_hyp, uint8_t *d_eligible);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 

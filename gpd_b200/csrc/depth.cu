@@ -95,6 +95,11 @@ __global__ void k_sub_flag(int N, const int *off, int B, const int *src, const i
   }
   flag[g] = e;
 }
+// flag[g] = the mask byte of point g itself (a mask over the installed points)
+__global__ void k_sub_flag_points(int N, const uint8_t *mask, int *flag) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < N) flag[g] = mask[g] != 0;
+}
 // eligible point g -> position e = pos[g]: its key under seed + b, its cloud-local index j, and e itself (the sort's value)
 __global__ void k_sub_compact(int N, const int *off, int B, const int *flag, const int *pos, unsigned long long seed,
                               unsigned long long *keys, int *vals, int *ev) {
@@ -203,7 +208,7 @@ int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format,
 }
 
 int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned long long seed, const uint8_t *d_mask,
-                   int *d_out, int *soff) {
+                   bool per_point, int *d_out, int *soff) {
   const int tb = 256;
   const int B = s.n, N = s.points();
   // device: point offsets, raw offsets, eligible offsets, output offsets [B+1 each]
@@ -211,7 +216,7 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
   if (!d_off) return GPDB_ERR_CUDA;
   int *d_roff = d_off + B + 1, *d_eoff = d_roff + B + 1, *d_soff = d_eoff + B + 1;
   CUDA_TRY(cudaMemcpyAsync(d_off, s.off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if (d_mask)
+  if (d_mask && !per_point)
     CUDA_TRY(cudaMemcpyAsync(d_roff, s.raw_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   std::vector<int> eoff((size_t)B + 1, 0);
   int *flag = nullptr, *pos = nullptr;
@@ -219,7 +224,8 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
     flag = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * 2 * ((size_t)N + 1));
     if (!flag) return GPDB_ERR_CUDA;
     pos = flag + N + 1;
-    k_sub_flag<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_off, B, s.src, d_roff, d_mask, flag);
+    if (d_mask && per_point) k_sub_flag_points<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_mask, flag);
+    else k_sub_flag<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_off, B, s.src, d_roff, d_mask, flag);
     LAUNCH_CHECK();
     CUDA_TRY(cudaMemsetAsync(flag + N, 0, sizeof(int), ctx->stream));
     size_t tmp_bytes = 0;

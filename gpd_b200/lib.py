@@ -30,7 +30,9 @@ EXPORTS = [
     "gpdb_find_clusters_batch_device", "gpdb_sis_params_default", "gpdb_sis_batch", "gpdb_sis_batch_device",
     "gpdb_sis_positions", "gpdb_set_clouds_samples_device", "gpdb_hand_search_batch_device", "gpdb_detect_batch_device",
     "gpdb_images_batch_device", "gpdb_classify_device", "gpdb_preprocess_depth", "gpdb_preprocess_depth_device",
-    "gpdb_subsample_clouds", "gpdb_subsample_clouds_device",
+    "gpdb_subsample_clouds", "gpdb_subsample_clouds_device", "gpdb_plane_params_default", "gpdb_segment_plane",
+    "gpdb_segment_planes", "gpdb_segment_planes_device", "gpdb_subsample_clouds_points",
+    "gpdb_subsample_clouds_points_device",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -115,8 +117,9 @@ def lib():
     L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
-    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES}.items():
+    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES, **abi.PLANE_PROTOTYPES}.items():
         getattr(L, name).argtypes = argtypes
+    L.gpdb_plane_params_default.restype = None
     _LIB = L
     return L
 
@@ -169,6 +172,16 @@ def sis_params(**over):
             p.workspace[:] = list(v)
         else:
             setattr(p, k, v)
+    return p
+
+
+def plane_params(**over):
+    """gpdb_plane_params with the reference's values (gpdb_plane_params_default: threshold 0.01, 50 iterations,
+    probability 0.99, seed 0), overridden by keyword."""
+    p = abi.PlaneParams()
+    lib().gpdb_plane_params_default(C.byref(p))
+    for k, v in over.items():
+        setattr(p, k, v)
     return p
 
 
@@ -714,6 +727,74 @@ class Context:
         n = self._check(lib().gpdb_subsample_clouds_device(self.h, int(num_samples), C.c_uint64(int(seed)), pm,
                                                            C.c_void_p(out.data_ptr()) if room else None, _p(soff)))
         return soff, out[:n]
+
+    def subsample_clouds_points(self, num_samples, seed, point_mask=None):
+        """gpdb_subsample_clouds_points: subsample_clouds() with the mask over the installed points (one uint8 per point
+        of the batch, concatenated by cloud, e.g. segment_planes()' eligible bytes), so it also works after set_clouds().
+        Returns one int32 array per cloud."""
+        room = self._subsample_room(num_samples)
+        idx = np.zeros(max(room, 1), np.int32)
+        m = None if point_mask is None else np.ascontiguousarray(point_mask, dtype=np.uint8).ravel()
+        if m is not None and self._batch is not None and len(m) != int(self._batch[0][-1]):
+            raise ValueError(f"point_mask: {len(m)} bytes, need one per installed point ({int(self._batch[0][-1])})")
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        self._check(lib().gpdb_subsample_clouds_points(self.h, int(num_samples), C.c_uint64(int(seed)), _p(m), _p(idx),
+                                                       _p(soff)))
+        return [idx[soff[b]:soff[b + 1]].copy() for b in range(self._n_clouds)]
+
+    def subsample_clouds_points_tensors(self, num_samples, seed, d_point_mask=None):
+        """gpdb_subsample_clouds_points_device: subsample_clouds_points() with the mask (uint8 CUDA tensor, one byte per
+        installed point, or None) on the device. Returns (offsets, indices) as subsample_clouds_tensors()."""
+        import torch
+        dev = self.params.device
+        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
+        pm = None if d_point_mask is None else _device_arg("d_point_mask", d_point_mask, torch.uint8, dev, n_pts)
+        self._torch_stream()
+        room = self._subsample_room(num_samples)
+        out = torch.empty(room, dtype=torch.int32, device=f"cuda:{dev}")
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        n = self._check(lib().gpdb_subsample_clouds_points_device(self.h, int(num_samples), C.c_uint64(int(seed)), pm,
+                                                                  C.c_void_p(out.data_ptr()) if room else None, _p(soff)))
+        return soff, out[:n]
+
+    def segment_plane(self, pl=None):
+        """gpdb_segment_plane: the support plane of the single installed cloud (include/gpd_b200_plane.h). Returns
+        (plane [4] float32, NaN when the fit failed; n_inliers; eligible [N] uint8, 1 for the points off the plane)."""
+        pl = plane_params() if pl is None else pl
+        n = self._check(lib().gpdb_get_cloud(self.h, None, None, None))
+        plane = np.zeros(4, np.float32)
+        cnt = np.zeros(1, np.int32)
+        elig = np.zeros(max(n, 1), np.uint8)
+        self._check(lib().gpdb_segment_plane(self.h, C.byref(pl), _p(plane), _p(cnt), _p(elig)))
+        return plane, int(cnt[0]), elig[:n]
+
+    def _plane_outputs(self):
+        B = self._n_clouds
+        return np.zeros((max(B, 1), 4), np.float32), np.zeros(max(B, 1), np.int32), np.zeros(max(B, 1), np.int32)
+
+    def segment_planes(self, pl=None):
+        """gpdb_segment_planes: the support plane of every installed cloud (cloud b with key seed + b). Returns a dict:
+        planes [B, 4] float32, n_inliers [B], n_hypotheses [B] (RANSAC hypotheses evaluated) and eligible [N] uint8
+        (concatenated by cloud, the point_mask subsample_clouds_points() takes)."""
+        pl = plane_params() if pl is None else pl
+        planes, cnt, nh = self._plane_outputs()
+        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
+        elig = np.zeros(max(n_pts, 1), np.uint8)
+        B = self._check(lib().gpdb_segment_planes(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh), _p(elig)))
+        return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": elig[:n_pts]}
+
+    def segment_planes_tensors(self, pl=None):
+        """gpdb_segment_planes_device: segment_planes() with the eligible bytes in a uint8 CUDA tensor [N], on torch's
+        current stream; planes and counts are host arrays as in segment_planes()."""
+        import torch
+        pl = plane_params() if pl is None else pl
+        planes, cnt, nh = self._plane_outputs()
+        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
+        self._torch_stream()
+        elig = torch.empty(n_pts, dtype=torch.uint8, device=f"cuda:{self.params.device}")
+        B = self._check(lib().gpdb_segment_planes_device(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh),
+                                                         C.c_void_p(elig.data_ptr()) if n_pts else None))
+        return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": elig}
 
     def set_clouds_tensors(self, point_offsets, xyz, normals, n_cameras, view_points, cam_source=None):
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them

@@ -329,9 +329,9 @@ void gpdb_preprocess_params_default(gpdb_preprocess_params *p);
  * neighbours within normals_radius at one point is GPDB_ERR_CAPACITY; a voxel index of 2^21 or more on any axis
  * (cloud extent / voxel_size) is GPDB_ERR_INVALID. After either error, or a rejected cam_source, the context holds
  * no cloud until the next successful gpdb_set_cloud / gpdb_preprocess.
- * Not covered: refine_normals_k, remove_outliers, sample_above_plane (PCL filters outside the default cfg) and
- * Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch draws them on the device with
- * gpdb_subsample_clouds).
+ * Not covered: refine_normals_k, remove_outliers (PCL filters outside the default cfg), sample_above_plane (a separate
+ * step: gpdb_segment_plane) and Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch
+ * draws them on the device with gpdb_subsample_clouds).
  * Semantics that differ from the reference by specification (DESIGN.md "preprocessing"): the voxel set is an
  * exact set (the reference's std::set comparator is not a strict weak order), output order = descending index
  * of each voxel's first point (the reference's iteration order whenever its de-duplication succeeds). */
@@ -563,6 +563,51 @@ int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, con
 /* The same with the mask and the indices in device memory (sample_offsets_out stays a host array). */
 int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_mask,
                                  int32_t *d_sample_idx_out, int32_t *sample_offsets_out);
+
+/* --- the support plane: Cloud::sampleAbovePlane on the device (include/gpd_b200_plane.h) --------------------------------
+ * pcl::SACSegmentation's RANSAC plane fit with refit (cloud.cpp:407-435), restated with counter-based draws: fit the
+ * table plane of each installed cloud and mark the points off it, so that samples land on the objects. The recipe of a
+ * tabletop view: gpdb_preprocess_depth[_device] -> gpdb_segment_planes[_device] -> gpdb_subsample_clouds_points[_device]
+ * (the eligible bytes as the mask) -> gpdb_detect_batch_select[_device]. */
+typedef struct gpdb_plane_params {
+  double distance_threshold; /* inlier iff the point's distance is < this (0.01, cloud.cpp:418)                     */
+  int32_t max_iterations;    /* at most max_iterations + 1 hypotheses (50, SACSegmentation's default), 1..1024    */
+  double probability;        /* RANSAC's stop probability (0.99), in (0, 1)                                      */
+  uint64_t seed;             /* cloud b draws with key seed + b (the single cloud: seed)                         */
+} gpdb_plane_params;
+
+/* The values above. */
+void gpdb_plane_params_default(gpdb_plane_params *p);
+
+/* Segments the single installed cloud (gpdb_set_cloud / gpdb_preprocess) by the rules of gpd_b200_plane.h: plane_out[4]
+ * = (a, b, c, d) with ax + by + cz + d = 0 (all NaN when the fit failed: fewer than 3 points or no good sample),
+ * *n_inliers_out = the points within distance_threshold of it (0 when the fit failed), eligible_out [N] (may be NULL) = 1
+ * for every point off the plane, and 1 for every point when the fit failed or no point is off the plane. Nothing
+ * installed changes. No cloud is GPDB_ERR_STATE; a threshold that is not finite and positive, max_iterations outside
+ * 1..1024 and probability outside (0, 1) are GPDB_ERR_INVALID before any device work. Equal to gpdb_segment_planes on a
+ * batch of one. Returns 1. */
+int gpdb_segment_plane(gpdb_ctx *ctx, const gpdb_plane_params *pl, float plane_out[4], int32_t *n_inliers_out,
+                       uint8_t *eligible_out);
+/* The same for every cloud of the installed batch (cloud b with key seed + b; its result depends on nothing else):
+ * planes_out [4B], n_inliers_out [B], n_hypotheses_out [B] (may be NULL) = RANSAC hypotheses evaluated, eligible_out [N]
+ * (may be NULL, concatenated by cloud). No batch is GPDB_ERR_STATE. Nothing installed changes: the clouds, sample
+ * positions and SIS record stay. Returns B. */
+int gpdb_segment_planes(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                        int32_t *n_hypotheses_out, uint8_t *eligible_out);
+/* The same with d_eligible_out in device memory (the rules of the device-resident family); planes and counts stay host
+ * arrays. */
+int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                               int32_t *n_hypotheses_out, uint8_t *d_eligible_out);
+
+/* gpdb_subsample_clouds with the mask over the INSTALLED points: point_mask [N] (may be NULL) holds one byte per point of
+ * the batch, concatenated by cloud (the eligible bytes of gpdb_segment_planes), so it also works after
+ * gpdb_set_clouds[_device]. The draw rule is gpd_b200_depth.h 5 unchanged; point_mask = NULL equals gpdb_subsample_clouds
+ * with mask = NULL bit for bit. */
+int gpdb_subsample_clouds_points(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *point_mask,
+                                 int32_t *sample_idx_out, int32_t *sample_offsets_out);
+/* The same with the mask and the indices in device memory (sample_offsets_out stays a host array). */
+int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_point_mask,
+                                        int32_t *d_sample_idx_out, int32_t *sample_offsets_out);
 
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
