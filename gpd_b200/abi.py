@@ -209,6 +209,12 @@ PLANE_PROTOTYPES = {
     "gpdb_subsample_clouds_points_device": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
 }
 
+# gpdb_refine_normals[_clouds] (include/gpd_b200.h, rules in include/gpd_b200_refine.h)
+REFINE_PROTOTYPES = {
+    "gpdb_refine_normals": [C.c_void_p, C.c_int32, C.c_void_p],
+    "gpdb_refine_normals_clouds": [C.c_void_p, C.c_int32, C.c_void_p],
+}
+
 
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""

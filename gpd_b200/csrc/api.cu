@@ -15,6 +15,7 @@
 
 #include "../../include/gpd_b200_depth.h"
 #include "../../include/gpd_b200_plane.h"
+#include "../../include/gpd_b200_refine.h"
 #include "common.cuh"
 
 static char g_create_err[512] = "";
@@ -1903,6 +1904,40 @@ int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float
                                int32_t *n_hypotheses_out, uint8_t *d_eligible_out) {
   return segment_entry(ctx, "gpdb_segment_planes_device", false, pl, planes_out, n_inliers_out, n_hypotheses_out,
                        d_eligible_out, true);
+}
+
+}  // extern "C"
+
+// ---- the normal refinement (include/gpd_b200_refine.h) -----------------------------------------------------------------
+
+// gpdb_refine_normals / gpdb_refine_normals_clouds: the state and argument checks, then refine_normals_batch on the single
+// cloud (single) or the batch
+static int refine_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t k, int32_t *iterations_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (k < 1 || k > GPDB_REFINE_MAX_K) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: k must lie in 1..%d (got %d)", name, GPDB_REFINE_MAX_K, (int)k);
+    return GPDB_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  std::vector<int> iters((size_t)s.n);
+  rc = refine_normals_batch(ctx, s, k, iters.data());
+  if (rc < 0) return rc;
+  if (iterations_out) std::copy(iters.begin(), iters.end(), iterations_out);
+  return rc;
+}
+
+extern "C" {
+
+int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
+  return refine_entry(ctx, "gpdb_refine_normals", true, k, iterations_out);
+}
+
+int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
+  return refine_entry(ctx, "gpdb_refine_normals_clouds", false, k, iterations_out);
 }
 
 }  // extern "C"

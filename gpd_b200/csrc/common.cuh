@@ -239,6 +239,8 @@ enum ScratchSlot {
   SCR_UPLOAD,
   // gpdb_segment_plane[s]: hypotheses, their inlier counts, the picked and refined planes (plane.cu)
   SCR_PLANE,
+  // gpdb_refine_normals[_clouds]: the two float32 iterates, the errors, the neighbour lists, done flags and counts (refine.cu)
+  SCR_REFINE,
   SCR_N
 };
 
@@ -456,6 +458,10 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
 // n_inliers[B] and n_hyp[B] (may be null) are host arrays, d_eligible (N bytes or null) device memory. Returns B.
 int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_params &pp, float *planes, int *n_inliers,
                         int *n_hyp, uint8_t *d_eligible);
+// refine.cu (include/gpd_b200_refine.h). Refines the normals of every cloud of store s with k neighbours (1..128) and
+// refreshes the descriptors' nonunit flags; iters[B] (host) receives each cloud's iteration count. The stored normals
+// change only once every step before the final cast has succeeded. Returns B.
+int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 

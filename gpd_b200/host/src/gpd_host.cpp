@@ -803,6 +803,7 @@ GraspDetector::GraspDetector(const std::string &config_filename) {
     if (config_file.ExtractKeys()) {
       model_file = config_file.getValueOfKeyAsString("model_file", "");  // grasp_detector.cpp:130
       sample_above_plane_ = config_file.getValueOfKey<bool>("sample_above_plane", false);  // grasp_detector.cpp:54-55
+      refine_normals_k_ = config_file.getValueOfKey<int>("refine_normals_k", 0);  // grasp_detector.cpp:62-63
     }
   }
   if (relu_after_conv_of(model_file, weights_file, params_.image_num_channels)) params_.relu_after_conv = 1;
@@ -829,8 +830,8 @@ bool preprocessParamsFromConfig(const std::string &config_filename, gpdb_preproc
   pp.normals_radius = config_file.getValueOfKey<double>("normals_radius", 0.03);
   std::vector<double> ws = config_file.getValueOfKeyAsStdVectorDouble("workspace", "-1 1 -1 1 -1 1");
   for (size_t i = 0; i < 6 && i < ws.size(); i++) pp.workspace[i] = ws[i];
-  if (config_file.getValueOfKey<bool>("remove_outliers", false) || config_file.getValueOfKey<int>("refine_normals_k", 0) > 0)
-    printf("NOTE: remove_outliers / refine_normals_k are not part of the accelerated preprocessing: ignored\n");
+  if (config_file.getValueOfKey<bool>("remove_outliers", false))
+    printf("NOTE: remove_outliers is not part of the accelerated preprocessing: ignored\n");
   return true;
 }
 
@@ -852,6 +853,13 @@ void GraspDetector::preprocessPointCloud(util::Cloud &cloud) {
   gpdb_preprocess_timings(ctx_, ms);
   if (pp.voxelize) printf("Voxelized cloud: %d\n", n);
   if (pp.estimate_normals) printf("Calculated %d surface normals in %3.4fs (mode: GPU).\n", n, ms[4] * 1e-3);
+  if (refine_normals_k_ > 0 && n > 0) {  // candidates_generator.cpp:28-30, in place on the installed cloud
+    printf("Refining surface normals ...\n");
+    if (gpdb_refine_normals(ctx_, refine_normals_k_, nullptr) < 0) {
+      printf("ERROR: %s\n", gpdb_last_error(ctx_));
+      return;
+    }
+  }
   std::vector<float> xyz(3 * (size_t)n);
   std::vector<double> nrm(3 * (size_t)n);
   std::vector<int> cam((size_t)n * cloud.numCameras());
@@ -1192,6 +1200,13 @@ bool GraspDetector::preprocessPointClouds(std::vector<util::Cloud> &clouds) {
     return false;
   }
   const int N = poff[B];
+  if (refine_normals_k_ > 0) {  // refineNormals of every cloud in one call, each cloud on its own
+    printf("Refining surface normals ...\n");
+    if (gpdb_refine_normals_clouds(ctx_, refine_normals_k_, nullptr) < 0) {
+      printf("ERROR: %s\n", gpdb_last_error(ctx_));
+      return false;
+    }
+  }
   std::vector<float> pxyz(3 * (size_t)N);
   std::vector<double> pnrm(3 * (size_t)N);
   size_t ncam = 0;

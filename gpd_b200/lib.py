@@ -32,7 +32,7 @@ EXPORTS = [
     "gpdb_images_batch_device", "gpdb_classify_device", "gpdb_preprocess_depth", "gpdb_preprocess_depth_device",
     "gpdb_subsample_clouds", "gpdb_subsample_clouds_device", "gpdb_plane_params_default", "gpdb_segment_plane",
     "gpdb_segment_planes", "gpdb_segment_planes_device", "gpdb_subsample_clouds_points",
-    "gpdb_subsample_clouds_points_device",
+    "gpdb_subsample_clouds_points_device", "gpdb_refine_normals", "gpdb_refine_normals_clouds",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -117,7 +117,8 @@ def lib():
     L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
     L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
-    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES, **abi.PLANE_PROTOTYPES}.items():
+    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES, **abi.PLANE_PROTOTYPES,
+                           **abi.REFINE_PROTOTYPES}.items():
         getattr(L, name).argtypes = argtypes
     L.gpdb_plane_params_default.restype = None
     _LIB = L
@@ -795,6 +796,20 @@ class Context:
         B = self._check(lib().gpdb_segment_planes_device(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh),
                                                          C.c_void_p(elig.data_ptr()) if n_pts else None))
         return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": elig}
+
+    def refine_normals(self, k):
+        """gpdb_refine_normals: refines the normals of the single installed cloud in place with k nearest neighbours
+        (Cloud::refineNormals, include/gpd_b200_refine.h). Returns the iterations run; get_cloud() reads the normals."""
+        it = np.zeros(1, np.int32)
+        self._check(lib().gpdb_refine_normals(self.h, int(k), _p(it)))
+        return int(it[0])
+
+    def refine_normals_clouds(self, k):
+        """gpdb_refine_normals_clouds: refine_normals() for every installed cloud, each on its own. Returns the
+        iterations run per cloud, int32 [B]."""
+        it = np.zeros(max(self._n_clouds, 1), np.int32)
+        B = self._check(lib().gpdb_refine_normals_clouds(self.h, int(k), _p(it)))
+        return it[:B]
 
     def set_clouds_tensors(self, point_offsets, xyz, normals, n_cameras, view_points, cam_source=None):
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them

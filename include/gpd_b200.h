@@ -329,8 +329,8 @@ void gpdb_preprocess_params_default(gpdb_preprocess_params *p);
  * neighbours within normals_radius at one point is GPDB_ERR_CAPACITY; a voxel index of 2^21 or more on any axis
  * (cloud extent / voxel_size) is GPDB_ERR_INVALID. After either error, or a rejected cam_source, the context holds
  * no cloud until the next successful gpdb_set_cloud / gpdb_preprocess.
- * Not covered: refine_normals_k, remove_outliers (PCL filters outside the default cfg), sample_above_plane (a separate
- * step: gpdb_segment_plane) and Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch
+ * Not covered: remove_outliers (parsed by the reference but never run), refine_normals_k and sample_above_plane
+ * (separate steps: gpdb_refine_normals, then gpdb_segment_plane) and Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch
  * draws them on the device with gpdb_subsample_clouds).
  * Semantics that differ from the reference by specification (DESIGN.md "preprocessing"): the voxel set is an
  * exact set (the reference's std::set comparator is not a strict weak order), output order = descending index
@@ -598,6 +598,28 @@ int gpdb_segment_planes(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *plane
  * arrays. */
 int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
                                int32_t *n_hypotheses_out, uint8_t *d_eligible_out);
+
+/* --- the normal refinement: Cloud::refineNormals on the device (include/gpd_b200_refine.h) -----------------------------
+ * refine_normals_k > 0 (candidates_generator.cpp:28-30): every normal becomes the normalised sum of the normals of its
+ * point's k nearest neighbours, repeated until the mean change is small (pcl::NormalRefinement's defaults), so that noisy
+ * normals, those of depth images in particular, are smoothed before the local frames, the antipodal test and the
+ * normals channels of the images read them. The reference runs it between calculateNormals and sampleAbovePlane: e.g.
+ * gpdb_preprocess_depth[_device] -> gpdb_refine_normals_clouds -> gpdb_segment_planes[_device] -> ... */
+
+/* Refines the normals of the single installed cloud (any install: gpdb_set_cloud, gpdb_preprocess) in place by the
+ * rules of gpd_b200_refine.h with k nearest neighbours (the point itself included; every point when the cloud has fewer
+ * than k). *iterations_out (may be NULL) = iterations run (1..15; 0 for an empty cloud). gpdb_get_cloud reads the
+ * refined normals back; the store's other content derived from the normals (the per-cloud flag of normals not of unit
+ * length, which decides how the image stage folds a cell) is recomputed by the rule every install applies, so a refined
+ * cloud behaves as one installed with the refined normals. The call is not an install: sample positions stay, and the
+ * batch is untouched. k outside 1..128 (GPDB_REFINE_MAX_K: the neighbour lists take N * k int32 of device memory) is
+ * GPDB_ERR_INVALID, no cloud GPDB_ERR_STATE; after any error the stored normals are unchanged. Returns 1. */
+int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out);
+/* The same for every cloud of the installed batch (any install: gpdb_set_clouds[_device], gpdb_preprocess_clouds[_device],
+ * gpdb_preprocess_depth[_device]), each cloud on its own: its own neighbour lists, stop decision and iteration count,
+ * iterations_out [B] (may be NULL). Sample positions and the SIS record stay; the single cloud is untouched. No batch is
+ * GPDB_ERR_STATE. Returns B. */
+int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out);
 
 /* gpdb_subsample_clouds with the mask over the INSTALLED points: point_mask [N] (may be NULL) holds one byte per point of
  * the batch, concatenated by cloud (the eligible bytes of gpdb_segment_planes), so it also works after
