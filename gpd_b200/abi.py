@@ -215,6 +215,12 @@ REFINE_PROTOTYPES = {
     "gpdb_refine_normals_clouds": [C.c_void_p, C.c_int32, C.c_void_p],
 }
 
+# gpdb_remove_outliers[_clouds] (include/gpd_b200.h, rules in include/gpd_b200_outliers.h)
+OUTLIERS_PROTOTYPES = {
+    "gpdb_remove_outliers": [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p],
+    "gpdb_remove_outliers_clouds": [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p],
+}
+
 
 def default_preprocess_params(**over):
     """Reference defaults (cfg/eigen_params.cfg:16-21, grasp_detector.cpp:56-66)."""

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/gpd_b200_depth.h"
+#include "../../include/gpd_b200_outliers.h"
 #include "../../include/gpd_b200_plane.h"
 #include "../../include/gpd_b200_refine.h"
 #include "common.cuh"
@@ -1938,6 +1939,60 @@ int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
 
 int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
   return refine_entry(ctx, "gpdb_refine_normals_clouds", false, k, iterations_out);
+}
+
+}  // extern "C"
+
+// ---- the statistical outlier removal (include/gpd_b200_outliers.h) ----------------------------------------------------
+
+// gpdb_remove_outliers / gpdb_remove_outliers_clouds: the state and argument checks, then outliers_remove_batch on the
+// single cloud (single) or the batch. It reinstalls the store: the batch loses its SIS record, and any failure after the
+// checks leaves no cloud (no batch: drop_batch), as a failed install does. Returns the kept points (single) or B.
+static int outliers_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t mean_k, double stddev_mul,
+                          int32_t *offsets_out, double *stats_out, uint8_t *kept_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (mean_k < 1 || mean_k > GPDB_OUTLIERS_MAX_K) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mean_k must lie in 1..%d (got %d)", name, GPDB_OUTLIERS_MAX_K, (int)mean_k);
+    return GPDB_ERR_INVALID;
+  }
+  if (!std::isfinite(stddev_mul)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: stddev_mul must be finite", name);
+    return GPDB_ERR_INVALID;
+  }
+  std::vector<int> off((size_t)s.n + 1);
+  const cudaError_t e = cudaSetDevice(ctx->device);
+  if (e != cudaSuccess) {
+    gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s: cudaSetDevice -> %s", name, cudaGetErrorString(e));
+    rc = GPDB_ERR_CUDA;
+  } else {
+    rc = outliers_remove_batch(ctx, s, mean_k, stddev_mul, off.data(), stats_out, kept_out);
+  }
+  if (rc < 0) {
+    s.n = 0;
+    s.has_src = false;
+    if (!single) drop_batch(ctx);
+    return rc;
+  }
+  if (!single) gpdb_sis_forget(ctx);  // the SIS positions describe clouds that are gone
+  if (offsets_out) std::copy(off.begin(), off.end(), offsets_out);
+  if (!single) return rc;
+  if (off[1] == 0) s.n = 0;  // no point kept: no cloud, as gpdb_preprocess when its filter keeps none
+  return off[1];
+}
+
+extern "C" {
+
+int gpdb_remove_outliers(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, double stats_out[3], uint8_t *kept_out) {
+  return outliers_entry(ctx, "gpdb_remove_outliers", true, mean_k, stddev_mul, nullptr, stats_out, kept_out);
+}
+
+int gpdb_remove_outliers_clouds(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, int32_t *offsets_out,
+                                double *stats_out, uint8_t *kept_out) {
+  return outliers_entry(ctx, "gpdb_remove_outliers_clouds", false, mean_k, stddev_mul, offsets_out, stats_out, kept_out);
 }
 
 }  // extern "C"

@@ -239,8 +239,14 @@ enum ScratchSlot {
   SCR_UPLOAD,
   // gpdb_segment_plane[s]: hypotheses, their inlier counts, the picked and refined planes (plane.cu)
   SCR_PLANE,
-  // gpdb_refine_normals[_clouds]: the two float32 iterates, the errors, the neighbour lists, done flags and counts (refine.cu)
+  // gpdb_refine_normals[_clouds]: the two float32 iterates, the errors, done flags and counts (refine.cu)
   SCR_REFINE,
+  // the k-nearest-neighbour lists (refine_knn_lists, N * k int32) of gpdb_refine_normals[_clouds] and
+  // gpdb_remove_outliers[_clouds]: one grow-only buffer for both, the largest part of their memory
+  SCR_NBR,
+  // gpdb_remove_outliers[_clouds]: mean distances, statistics, keep flags and their scan, per-cloud counts and camera
+  // flags, the kept points gathered before they go back into the store (outliers.cu)
+  SCR_OUTLIERS,
   SCR_N
 };
 
@@ -462,6 +468,16 @@ int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_param
 // refreshes the descriptors' nonunit flags; iters[B] (host) receives each cloud's iteration count. The stored normals
 // change only once every step before the final cast has succeeded. Returns B.
 int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters);
+// refine.cu: rule 1 of gpd_b200_refine.h alone. nbr[g*k + r], r < min(k, N_b): the cloud-local index of the r-th
+// neighbour of concatenated point g of store s (device memory of N * k int32; k in 1..128).
+int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr);
+// outliers.cu (include/gpd_b200_outliers.h). Removes the statistical outliers of every cloud of store s with mean_k
+// neighbours (1..127) and reinstalls the kept points (grids, nonunit and all_seen flags as an install of them computes
+// them; sample positions dropped; the source indices and has_src kept). off[B+1] (host) receives the new point offsets;
+// stats[3B] (host, may be null) each cloud's mean, stddev and threshold; kept (host, may be null) one byte per point before
+// the call. Returns B, or an error after which s holds no cloud (s.n = 0), as after a failed install.
+int outliers_remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int *off, double *stats,
+                          uint8_t *kept);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 

@@ -263,21 +263,30 @@ __global__ void k_refine_commit(const CloudDesc *d, int B, int N, const int *ite
     }                                                    \
   } while (0)
 
-int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
-  const int B = s.n, N = s.points();
-  // SCR_REFINE: iterates float4[2N], errors float[N], lists int[N*k], done int[B], counts int[B]
-  const size_t n = (size_t)N;
-  float4 *buf0 = (float4 *)gpdb_scratch(ctx, SCR_REFINE,
-                                        sizeof(float4) * 2 * n + sizeof(float) * n + sizeof(int) * (n * k + 2 * (size_t)B));
-  if (!buf0) return GPDB_ERR_CUDA;
-  float4 *buf1 = buf0 + n;
-  float *err = (float *)(buf1 + n);
-  int *nbr = (int *)(err + n), *done = nbr + n * k, *d_iters = done + B;
-  CUDA_TRY(cudaMemsetAsync(done, 0, sizeof(int) * 2 * (size_t)B, ctx->stream));
-  const int tb = 256, nb = (N + tb - 1) / tb;
+int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr) {
+  const int N = s.points();
   if (N > 0) {
     k_refine_knn<<<(N + KNN_WARPS - 1) / KNN_WARPS, KNN_WARPS * 32, 0, ctx->stream>>>(s.view, s.table(), N, k, nbr);
     LAUNCH_CHECK();
+  }
+  return GPDB_OK;
+}
+
+int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
+  const int B = s.n, N = s.points();
+  // SCR_REFINE: iterates float4[2N], errors float[N], done int[B], counts int[B]; SCR_NBR: lists int[N*k]
+  const size_t n = (size_t)N;
+  float4 *buf0 = (float4 *)gpdb_scratch(ctx, SCR_REFINE, sizeof(float4) * 2 * n + sizeof(float) * n + sizeof(int) * 2 * (size_t)B);
+  int *nbr = (int *)gpdb_scratch(ctx, SCR_NBR, sizeof(int) * n * k);
+  if (!buf0 || !nbr) return GPDB_ERR_CUDA;
+  float4 *buf1 = buf0 + n;
+  float *err = (float *)(buf1 + n);
+  int *done = (int *)(err + n), *d_iters = done + B;
+  CUDA_TRY(cudaMemsetAsync(done, 0, sizeof(int) * 2 * (size_t)B, ctx->stream));
+  const int tb = 256, nb = (N + tb - 1) / tb;
+  const int rc0 = refine_knn_lists(ctx, s, k, nbr);
+  if (rc0 != GPDB_OK) return rc0;
+  if (N > 0) {
     k_refine_cast<<<nb, tb, 0, ctx->stream>>>(s.nrm, N, buf0);
     LAUNCH_CHECK();
   }

@@ -92,6 +92,11 @@ class Cloud {
   // be this processed cloud (GraspDetector::preprocessPointCloud installs it). The sample indices become the points off
   // the plane, or stay as they are when the fit fails or no point is off it. Prints the reference's messages.
   bool sampleAbovePlane(gpdb_ctx *ctx);
+  // Cloud::removeStatisticalOutliers (cloud.cpp:166-174) on the device: gpdb_remove_outliers with the reference's mean_k
+  // = 50 and stddev_mul = 1.0 on the single cloud of ctx, which must be this processed cloud. The kept points, their
+  // normals and camera sources replace the cloud's (the reference filters the points alone); the sample indices are
+  // invalidated. Prints the reference's message.
+  bool removeStatisticalOutliers(gpdb_ctx *ctx);
   // the same from one cloud's result of gpdb_segment_plane[s] (n_inliers, eligible bytes of its N points)
   void setAbovePlane(int n_inliers, const uint8_t *eligible);
   const std::vector<float> &getPoints() const { return points_; }       // packed x,y,z

@@ -421,6 +421,24 @@ bool Cloud::sampleAbovePlane(gpdb_ctx *ctx) {
   return true;
 }
 
+bool Cloud::removeStatisticalOutliers(gpdb_ctx *ctx) {
+  const int n = gpdb_remove_outliers(ctx, 50, 1.0, nullptr, nullptr);  // sor.setMeanK(50), sor.setStddevMulThresh(1.0)
+  if (n < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx));
+    return false;
+  }
+  std::vector<float> xyz(3 * (size_t)n);
+  std::vector<double> nrm(3 * (size_t)n);
+  std::vector<int> cam((size_t)n * numCameras());
+  if (n > 0 && gpdb_get_cloud(ctx, xyz.data(), nrm.data(), cam.data()) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx));
+    return false;
+  }
+  setProcessed(std::move(xyz), std::move(nrm), std::move(cam));
+  printf("Cloud after removing statistical outliers: %zu\n", size());
+  return true;
+}
+
 void Cloud::subsample(int num_samples) {
   if (!above_plane_.empty()) {  // subsampleSampleIndices (cloud.cpp:395-405): with replacement, fixed-seed generator
     sample_indices_ = above_plane_;

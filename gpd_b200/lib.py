@@ -33,6 +33,7 @@ EXPORTS = [
     "gpdb_subsample_clouds", "gpdb_subsample_clouds_device", "gpdb_plane_params_default", "gpdb_segment_plane",
     "gpdb_segment_planes", "gpdb_segment_planes_device", "gpdb_subsample_clouds_points",
     "gpdb_subsample_clouds_points_device", "gpdb_refine_normals", "gpdb_refine_normals_clouds",
+    "gpdb_remove_outliers", "gpdb_remove_outliers_clouds",
 ]
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
@@ -118,7 +119,7 @@ def lib():
     L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
     L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
     for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES, **abi.PLANE_PROTOTYPES,
-                           **abi.REFINE_PROTOTYPES}.items():
+                           **abi.REFINE_PROTOTYPES, **abi.OUTLIERS_PROTOTYPES}.items():
         getattr(L, name).argtypes = argtypes
     L.gpdb_plane_params_default.restype = None
     _LIB = L
@@ -810,6 +811,39 @@ class Context:
         it = np.zeros(max(self._n_clouds, 1), np.int32)
         B = self._check(lib().gpdb_refine_normals_clouds(self.h, int(k), _p(it)))
         return it[:B]
+
+    def remove_outliers(self, mean_k=50, stddev_mul=1.0):
+        """gpdb_remove_outliers: removes the statistical outliers of the single installed cloud and reinstalls the kept
+        points (Cloud::removeStatisticalOutliers, include/gpd_b200_outliers.h). Returns n_kept, the cloud's mean, stddev
+        and threshold, and kept, one byte per point before the call; get_cloud() reads the kept cloud."""
+        n = self._check(lib().gpdb_get_cloud(self.h, None, None, None))
+        stats = np.zeros(3, np.float64)
+        kept = np.zeros(n, np.uint8)
+        n_kept = self._check(lib().gpdb_remove_outliers(self.h, int(mean_k), float(stddev_mul), _p(stats), _p(kept)))
+        return {"n_kept": n_kept, "mean": float(stats[0]), "stddev": float(stats[1]), "threshold": float(stats[2]),
+                "kept": kept}
+
+    def remove_outliers_clouds(self, mean_k=50, stddev_mul=1.0):
+        """gpdb_remove_outliers_clouds: remove_outliers() for every installed cloud, each on its own. Returns offsets, the
+        new point offsets [B+1], stats [B, 3] (mean, stddev, threshold) and kept, one byte per point before the call.
+        Sample positions and the SIS record are dropped."""
+        B = self._n_clouds
+        n = int(self._batch[0][-1]) if self._batch is not None else 0
+        off = np.zeros(B + 1, np.int32)
+        stats = np.zeros((max(B, 1), 3), np.float64)
+        kept = np.zeros(n, np.uint8)
+        try:
+            self._check(lib().gpdb_remove_outliers_clouds(self.h, int(mean_k), float(stddev_mul), _p(off), _p(stats),
+                                                          _p(kept)))
+        except GpdbError as e:
+            # GPDB_ERR_INVALID / GPDB_ERR_STATE come before any device work and change nothing; after any other error the
+            # library holds no batch, and neither may this bookkeeping, which sizes the output buffers of later calls
+            if e.code not in (-1, -3):
+                self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None
+            raise
+        self._batch = (off,) + tuple(self._batch[1:])
+        self._sis_shape = None
+        return {"offsets": off, "stats": stats[:B], "kept": kept}
 
     def set_clouds_tensors(self, point_offsets, xyz, normals, n_cameras, view_points, cam_source=None):
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them

@@ -329,9 +329,10 @@ void gpdb_preprocess_params_default(gpdb_preprocess_params *p);
  * neighbours within normals_radius at one point is GPDB_ERR_CAPACITY; a voxel index of 2^21 or more on any axis
  * (cloud extent / voxel_size) is GPDB_ERR_INVALID. After either error, or a rejected cam_source, the context holds
  * no cloud until the next successful gpdb_set_cloud / gpdb_preprocess.
- * Not covered: remove_outliers (parsed by the reference but never run), refine_normals_k and sample_above_plane
- * (separate steps: gpdb_refine_normals, then gpdb_segment_plane) and Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch
- * draws them on the device with gpdb_subsample_clouds).
+ * Not covered: remove_outliers, refine_normals_k and sample_above_plane (separate steps: gpdb_remove_outliers, which the
+ * reference's preprocessing never runs although its cfg parses the key, gpdb_refine_normals, then gpdb_segment_plane) and
+ * Cloud::subsample (host-side RNG; the sample indices are an input of gpdb_detect; a batch draws them on the device with
+ * gpdb_subsample_clouds).
  * Semantics that differ from the reference by specification (DESIGN.md "preprocessing"): the voxel set is an
  * exact set (the reference's std::set comparator is not a strict weak order), output order = descending index
  * of each voxel's first point (the reference's iteration order whenever its de-duplication succeeds). */
@@ -620,6 +621,35 @@ int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out);
  * iterations_out [B] (may be NULL). Sample positions and the SIS record stay; the single cloud is untouched. No batch is
  * GPDB_ERR_STATE. Returns B. */
 int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out);
+
+/* --- the statistical outlier removal: Cloud::removeStatisticalOutliers on the device (include/gpd_b200_outliers.h) ------
+ * Removes the points whose mean distance to their mean_k nearest neighbours lies more than stddev_mul standard
+ * deviations above the cloud's mean of that distance (pcl::StatisticalOutlierRemoval; the reference's
+ * removeStatisticalOutliers uses mean_k = 50, stddev_mul = 1.0). Depth images are where such points come from: flying
+ * pixels at depth edges and isolated speckle, each a sample that finds no grasp, a point in the fingers' way and occupied
+ * cells in the grasp images. E.g. gpdb_preprocess_depth[_device] -> gpdb_remove_outliers_clouds ->
+ * gpdb_refine_normals_clouds -> gpdb_segment_planes[_device] -> ...
+ *
+ * The call is an install of the kept points: they keep their order, normals, camera masks and (after a preprocessing
+ * install) source indices, which still index the raw points, so per-pixel masks keep working; the grids, the nonunit
+ * flags and the flag of clouds whose every point every camera sees are recomputed as gpdb_set_clouds computes them, so
+ * the store behaves as one installed with the kept points. Sample positions are dropped. mean_k outside 1..127
+ * (GPDB_OUTLIERS_MAX_K) or a non-finite stddev_mul is GPDB_ERR_INVALID and no cloud GPDB_ERR_STATE; these errors change
+ * nothing. Any other error (a CUDA error, e.g. no device memory for the neighbour lists) leaves no cloud (the batch
+ * call: no batch, no sample positions, no SIS record), as a failed install does. A cloud of at most mean_k points keeps
+ * every point and reports NaN statistics (gpd_b200_outliers.h rule 5). */
+
+/* The single installed cloud (any install: gpdb_set_cloud, gpdb_preprocess); the batch is untouched. stats_out (may be
+ * NULL) = {mean, stddev, threshold}; kept_out (may be NULL) one byte per point before the call, 1 = kept. Returns the
+ * number of kept points; when none is kept the context holds no cloud, as after gpdb_preprocess keeping none. */
+int gpdb_remove_outliers(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, double stats_out[3], uint8_t *kept_out);
+/* Every cloud of the installed batch (any install: gpdb_set_clouds[_device], gpdb_preprocess_clouds[_device],
+ * gpdb_preprocess_depth[_device]), each on its own; the single cloud is untouched. offsets_out [B+1] (may be NULL) = the
+ * new point offsets, stats_out [3B] (may be NULL) each cloud's {mean, stddev, threshold}, kept_out [N before] (may be
+ * NULL) the kept bytes. The SIS record is dropped (gpdb_sis_positions is then GPDB_ERR_STATE). No batch is GPDB_ERR_STATE.
+ * Returns B. */
+int gpdb_remove_outliers_clouds(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, int32_t *offsets_out,
+                                double *stats_out, uint8_t *kept_out);
 
 /* gpdb_subsample_clouds with the mask over the INSTALLED points: point_mask [N] (may be NULL) holds one byte per point of
  * the batch, concatenated by cloud (the eligible bytes of gpdb_segment_planes), so it also works after
