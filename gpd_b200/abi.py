@@ -145,18 +145,6 @@ class SisParams(C.Structure):
     ]
 
 
-# Argument types of the device-resident calls that take sample positions, return every hand and make and classify grasp
-# images from device memory (include/gpd_b200.h, "device-resident batches"); every one returns int. Pointers are
-# c_void_p (host or device addresses), the result is a gpdb_result *.
-RESIDENT_PROTOTYPES = {
-    "gpdb_set_clouds_samples_device": [C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_hand_search_batch_device": [C.c_void_p] * 6 + [C.POINTER(Result)],
-    "gpdb_detect_batch_device": [C.c_void_p] * 7 + [C.POINTER(Result)],
-    "gpdb_images_batch_device": [C.c_void_p] * 4,
-    "gpdb_classify_device": [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
-}
-
-
 DEPTH_U16, DEPTH_F32 = 0, 1  # GPDB_DEPTH_U16 / GPDB_DEPTH_F32
 
 
@@ -177,17 +165,6 @@ class DepthCamera(C.Structure):
     ]
 
 
-# gpdb_preprocess_depth[_device], gpdb_subsample_clouds[_device] (include/gpd_b200.h)
-DEPTH_PROTOTYPES = {
-    "gpdb_preprocess_depth": [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                              C.POINTER(PreprocessParams), C.c_void_p],
-    "gpdb_preprocess_depth_device": [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                                     C.POINTER(PreprocessParams), C.c_void_p],
-    "gpdb_subsample_clouds": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_subsample_clouds_device": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
-}
-
-
 class PlaneParams(C.Structure):
     """gpdb_plane_params (include/gpd_b200.h, rules in include/gpd_b200_plane.h)."""
 
@@ -199,27 +176,102 @@ class PlaneParams(C.Structure):
     ]
 
 
-# gpdb_segment_plane[s][_device], gpdb_subsample_clouds_points[_device] (include/gpd_b200.h)
-PLANE_PROTOTYPES = {
-    "gpdb_plane_params_default": [C.POINTER(PlaneParams)],
-    "gpdb_segment_plane": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_segment_planes": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_segment_planes_device": [C.c_void_p, C.POINTER(PlaneParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_subsample_clouds_points": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
-    "gpdb_subsample_clouds_points_device": [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p],
+_vp, _i32, _int = C.c_void_p, C.c_int32, C.c_int
+_res, _pp, _sp, _pl = C.POINTER(Result), C.POINTER(PreprocessParams), C.POINTER(SisParams), C.POINTER(PlaneParams)
+
+# Every function of include/gpd_b200.h, in its order: name -> (restype, argtypes). A pointer is c_void_p (a host or
+# device address) unless it points to a boundary struct; tests/test_abi.py holds each entry against the declaration.
+PROTOTYPES = {
+    "gpdb_params_default": (None, [C.POINTER(Params)]),
+    "gpdb_create": (_int, [C.POINTER(Params), C.POINTER(_vp)]),
+    "gpdb_destroy": (None, [_vp]),
+    "gpdb_last_error": (C.c_char_p, [_vp]),
+    "gpdb_load_weights_dir": (_int, [_vp, C.c_char_p]),
+    "gpdb_load_weights_file": (_int, [_vp, C.c_char_p, C.c_char_p]),
+    "gpdb_read_weights_file": (_int, [C.c_char_p, C.c_char_p, _i32, _vp, _vp, C.c_char_p, _i32]),
+    "gpdb_set_weights": (_int, [_vp] * 9),
+    "gpdb_set_cloud": (_int, [_vp, _vp, _vp, _vp, _i32, _vp, _i32]),
+    "gpdb_set_samples": (_int, [_vp, _vp, _i32]),
+    "gpdb_detect": (_int, [_vp, _vp, _i32, _res]),
+    "gpdb_detect_select": (_int, [_vp, _vp, _i32, _i32, _res]),
+    "gpdb_detect_resident": (_int, [_vp, _vp, _i32, _vp, _vp, _res]),
+    "gpdb_set_clouds": (_int, [_vp, _i32] + [_vp] * 6),
+    "gpdb_detect_batch": (_int, [_vp, _vp, _vp, _res, _vp]),
+    "gpdb_detect_batch_select": (_int, [_vp, _vp, _vp, _i32, _res, _vp]),
+    "gpdb_set_clouds_samples": (_int, [_vp, _vp, _vp]),
+    "gpdb_hand_search_batch": (_int, [_vp, _vp, _vp, _res, _vp]),
+    "gpdb_set_stream": (_int, [_vp, _vp]),
+    "gpdb_set_overlap": (_int, [_vp, _i32]),
+    "gpdb_frames": (_int, [_vp, _vp, _i32, _vp, _vp]),
+    "gpdb_hand_search": (_int, [_vp, _vp, _i32, _res]),
+    "gpdb_images": (_int, [_vp, _vp, _i32, _vp]),
+    "gpdb_classify": (_int, [_vp, _vp, _i32, _vp, _vp]),
+    "gpdb_preprocess_params_default": (None, [_pp]),
+    "gpdb_preprocess": (_int, [_vp, _vp, _vp, _vp, _i32, _vp, _i32, _pp]),
+    "gpdb_get_cloud": (_int, [_vp, _vp, _vp, _vp]),
+    "gpdb_get_cloud_source_index": (_int, [_vp, _vp]),
+    "gpdb_preprocess_clouds": (_int, [_vp, _i32] + [_vp] * 6 + [_pp, _vp]),
+    "gpdb_get_clouds": (_int, [_vp] * 5),
+    "gpdb_preprocess_timings": (_int, [_vp, _vp]),
+    "gpdb_reevaluate": (_int, [_vp, _vp, _i32, _vp]),
+    "gpdb_find_clusters": (_int, [_vp, _vp, _i32, _i32, _vp]),
+    "gpdb_find_clusters_batch": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "gpdb_preprocess_clouds_device": (_int, [_vp, _i32] + [_vp] * 6 + [_pp, _vp]),
+    "gpdb_set_clouds_device": (_int, [_vp, _i32] + [_vp] * 6),
+    "gpdb_detect_batch_select_device": (_int, [_vp, _vp, _vp, _i32, _vp, _vp, _res]),
+    "gpdb_find_clusters_batch_device": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "gpdb_set_clouds_samples_device": (_int, [_vp, _vp, _vp]),
+    "gpdb_hand_search_batch_device": (_int, [_vp] * 6 + [_res]),
+    "gpdb_detect_batch_device": (_int, [_vp] * 7 + [_res]),
+    "gpdb_images_batch_device": (_int, [_vp] * 4),
+    "gpdb_classify_device": (_int, [_vp, _vp, _i32, _vp, _vp]),
+    "gpdb_sis_params_default": (None, [_sp]),
+    "gpdb_sis_batch": (_int, [_vp, _sp, _vp, _vp, _res, _vp]),
+    "gpdb_sis_batch_device": (_int, [_vp, _sp, _vp, _vp, _vp, _vp, _res]),
+    "gpdb_sis_positions": (_int, [_vp] * 6),
+    "gpdb_preprocess_depth": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp]),
+    "gpdb_preprocess_depth_device": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp]),
+    "gpdb_subsample_clouds": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
+    "gpdb_subsample_clouds_device": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
+    "gpdb_plane_params_default": (None, [_pl]),
+    "gpdb_segment_plane": (_int, [_vp, _pl, _vp, _vp, _vp]),
+    "gpdb_segment_planes": (_int, [_vp, _pl, _vp, _vp, _vp, _vp]),
+    "gpdb_segment_planes_device": (_int, [_vp, _pl, _vp, _vp, _vp, _vp]),
+    "gpdb_refine_normals": (_int, [_vp, _i32, _vp]),
+    "gpdb_refine_normals_clouds": (_int, [_vp, _i32, _vp]),
+    "gpdb_remove_outliers": (_int, [_vp, _i32, C.c_double, _vp, _vp]),
+    "gpdb_remove_outliers_clouds": (_int, [_vp, _i32, C.c_double, _vp, _vp, _vp]),
+    "gpdb_subsample_clouds_points": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
+    "gpdb_subsample_clouds_points_device": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
+    "gpdb_free_result": (None, [_res]),
+    "gpdb_comm_unique_id": (_int, [_vp]),
+    "gpdb_comm_init": (_int, [_vp, _vp, _i32, _i32]),
+    "gpdb_comm_destroy": (_int, [_vp]),
+    "gpdb_shard_bounds": (None, [_i32, _i32, _i32, _vp, _vp, _vp]),
+    "gpdb_set_cloud_bcast": (_int, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32]),
+    "gpdb_detect_sharded": (_int, [_vp, _vp, _i32, _res]),
+    "gpdb_detect_sharded_resident": (_int, [_vp, _vp, _i32, _i32, _vp, _res]),
+    "gpdb_slot_bytes": (C.c_int64, [_i32, _i32]),
+    "gpdb_last_timings": (_int, [_vp, _vp]),
+    "gpdb_debug_phase_cycles": (_int, [_vp, _int, _vp]),
+    "gpdb_debug_path_counts": (_int, [_vp, _vp]),
+    "gpdb_debug_lenet_layers": (_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "gpdb_build_info": (C.c_char_p, []),
 }
 
-# gpdb_refine_normals[_clouds] (include/gpd_b200.h, rules in include/gpd_b200_refine.h)
-REFINE_PROTOTYPES = {
-    "gpdb_refine_normals": [C.c_void_p, C.c_int32, C.c_void_p],
-    "gpdb_refine_normals_clouds": [C.c_void_p, C.c_int32, C.c_void_p],
-}
 
-# gpdb_remove_outliers[_clouds] (include/gpd_b200.h, rules in include/gpd_b200_outliers.h)
-OUTLIERS_PROTOTYPES = {
-    "gpdb_remove_outliers": [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p],
-    "gpdb_remove_outliers_clouds": [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p],
-}
+def set_fields(p, **over):
+    """Sets fields of a params struct by keyword and returns it. An array field takes all its values, except hand_axes,
+    which takes 1..MAX_HAND_AXES axes and sets num_hand_axes to their count."""
+    for k, v in over.items():
+        if k == "hand_axes":
+            p.num_hand_axes = len(v)
+            p.hand_axes[:len(v)] = list(v)
+        elif isinstance(getattr(p, k, None), C.Array):
+            getattr(p, k)[:] = list(v)
+        else:
+            setattr(p, k, v)
+    return p
 
 
 def default_preprocess_params(**over):
@@ -230,12 +282,7 @@ def default_preprocess_params(**over):
     p.normals_radius = 0.03
     p.voxelize = 1
     p.estimate_normals = 1
-    for k, v in over.items():
-        if k == "workspace":
-            p.workspace[:] = list(v)
-        else:
-            setattr(p, k, v)
-    return p
+    return set_fields(p, **over)
 
 
 def default_params(channels=15, **over):
@@ -268,17 +315,7 @@ def default_params(channels=15, **over):
     p.chunk_samples = 0
     p.keep_images = 0
     p.lenet_impl = 0
-    for k, v in over.items():
-        if k == "hand_axes":
-            p.num_hand_axes = len(v)
-            for i, a in enumerate(v):
-                p.hand_axes[i] = a
-        elif k in ("workspace_grasps", "direction"):
-            for i, a in enumerate(v):
-                getattr(p, k)[i] = a
-        else:
-            setattr(p, k, v)
-    return p
+    return set_fields(p, **over)
 
 
 def result_to_numpy(res, image_bytes):

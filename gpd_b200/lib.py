@@ -16,25 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("GPD_B200_LIB") or os.path.join(_HERE, "libgpd_b200.so")
 _LIB = None
 
-EXPORTS = [
-    "gpdb_params_default", "gpdb_create", "gpdb_destroy", "gpdb_last_error", "gpdb_load_weights_dir",
-    "gpdb_set_weights", "gpdb_set_cloud", "gpdb_detect", "gpdb_frames", "gpdb_hand_search", "gpdb_images",
-    "gpdb_classify", "gpdb_free_result", "gpdb_last_timings", "gpdb_build_info", "gpdb_detect_resident",
-    "gpdb_set_stream", "gpdb_debug_phase_cycles", "gpdb_preprocess_params_default", "gpdb_preprocess",
-    "gpdb_get_cloud", "gpdb_get_cloud_source_index", "gpdb_preprocess_timings", "gpdb_detect_select", "gpdb_load_weights_file", "gpdb_read_weights_file", "gpdb_set_samples",
-    "gpdb_comm_unique_id", "gpdb_comm_init", "gpdb_comm_destroy", "gpdb_shard_bounds", "gpdb_set_cloud_bcast",
-    "gpdb_detect_sharded", "gpdb_detect_sharded_resident", "gpdb_slot_bytes", "gpdb_find_clusters", "gpdb_reevaluate", "gpdb_set_overlap",
-    "gpdb_set_clouds", "gpdb_detect_batch", "gpdb_detect_batch_select", "gpdb_preprocess_clouds", "gpdb_get_clouds",
-    "gpdb_debug_path_counts", "gpdb_debug_lenet_layers", "gpdb_set_clouds_samples", "gpdb_hand_search_batch",
-    "gpdb_find_clusters_batch", "gpdb_preprocess_clouds_device", "gpdb_set_clouds_device", "gpdb_detect_batch_select_device",
-    "gpdb_find_clusters_batch_device", "gpdb_sis_params_default", "gpdb_sis_batch", "gpdb_sis_batch_device",
-    "gpdb_sis_positions", "gpdb_set_clouds_samples_device", "gpdb_hand_search_batch_device", "gpdb_detect_batch_device",
-    "gpdb_images_batch_device", "gpdb_classify_device", "gpdb_preprocess_depth", "gpdb_preprocess_depth_device",
-    "gpdb_subsample_clouds", "gpdb_subsample_clouds_device", "gpdb_plane_params_default", "gpdb_segment_plane",
-    "gpdb_segment_planes", "gpdb_segment_planes_device", "gpdb_subsample_clouds_points",
-    "gpdb_subsample_clouds_points_device", "gpdb_refine_normals", "gpdb_refine_normals_clouds",
-    "gpdb_remove_outliers", "gpdb_remove_outliers_clouds",
-]
+EXPORTS = list(abi.PROTOTYPES)
 
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
 PATH_EVENTS = ["frames_tier1", "frames_tier2", "hands_tile", "hands_global", "hands_full_slab", "images2_box",
@@ -57,71 +39,9 @@ def lib():
             f"{SO_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(nvcc, sm_90a). gpd_b200 has no CPU fallback.")
     L = C.CDLL(SO_PATH)
-    vp = C.c_void_p
-    L.gpdb_params_default.argtypes = [C.POINTER(abi.Params)]
-    L.gpdb_create.argtypes = [C.POINTER(abi.Params), C.POINTER(vp)]
-    L.gpdb_destroy.argtypes = [vp]
-    L.gpdb_last_error.restype = C.c_char_p
-    L.gpdb_last_error.argtypes = [vp]
-    L.gpdb_load_weights_dir.argtypes = [vp, C.c_char_p]
-    L.gpdb_set_weights.argtypes = [vp] + [vp] * 8
-    L.gpdb_load_weights_file.argtypes = [vp, C.c_char_p, C.c_char_p]
-    L.gpdb_read_weights_file.argtypes = [C.c_char_p, C.c_char_p, C.c_int32, vp, vp, C.c_char_p, C.c_int32]
-    L.gpdb_set_cloud.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32]
-    L.gpdb_detect.argtypes = [vp, vp, C.c_int32, C.POINTER(abi.Result)]
-    L.gpdb_hand_search.argtypes = [vp, vp, C.c_int32, C.POINTER(abi.Result)]
-    L.gpdb_detect_select.argtypes = [vp, vp, C.c_int32, C.c_int32, C.POINTER(abi.Result)]
-    L.gpdb_frames.argtypes = [vp, vp, C.c_int32, vp, vp]
-    L.gpdb_images.argtypes = [vp, vp, C.c_int32, vp]
-    L.gpdb_classify.argtypes = [vp, vp, C.c_int32, vp, vp]
-    L.gpdb_free_result.argtypes = [C.POINTER(abi.Result)]
-    L.gpdb_last_timings.argtypes = [vp, vp]
-    L.gpdb_build_info.restype = C.c_char_p
-    L.gpdb_detect_resident.argtypes = [vp, vp, C.c_int32, vp, vp, C.POINTER(abi.Result)]
-    L.gpdb_set_stream.argtypes = [vp, vp]
-    L.gpdb_debug_phase_cycles.argtypes = [vp, C.c_int, vp]
-    L.gpdb_debug_path_counts.argtypes = [vp, vp]
-    L.gpdb_debug_lenet_layers.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp]
-    L.gpdb_preprocess_params_default.argtypes = [C.POINTER(abi.PreprocessParams)]
-    L.gpdb_preprocess.argtypes = [vp, vp, vp, vp, C.c_int32, vp, C.c_int32, C.POINTER(abi.PreprocessParams)]
-    L.gpdb_get_cloud.argtypes = [vp, vp, vp, vp]
-    L.gpdb_set_samples.argtypes = [vp, vp, C.c_int32]
-    L.gpdb_get_cloud_source_index.argtypes = [vp, vp]
-    L.gpdb_preprocess_timings.argtypes = [vp, vp]
-    L.gpdb_comm_unique_id.argtypes = [vp]
-    L.gpdb_comm_init.argtypes = [vp, vp, C.c_int32, C.c_int32]
-    L.gpdb_comm_destroy.argtypes = [vp]
-    L.gpdb_shard_bounds.argtypes = [C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
-    L.gpdb_shard_bounds.restype = None
-    L.gpdb_set_cloud_bcast.argtypes = [vp, C.c_int32, vp, vp, vp, C.c_int32, vp, C.c_int32]
-    L.gpdb_detect_sharded.argtypes = [vp, vp, C.c_int32, C.POINTER(abi.Result)]
-    L.gpdb_detect_sharded_resident.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, C.POINTER(abi.Result)]
-    L.gpdb_slot_bytes.argtypes = [C.c_int32, C.c_int32]
-    L.gpdb_slot_bytes.restype = C.c_int64
-    L.gpdb_find_clusters.argtypes = [vp, vp, C.c_int32, C.c_int32, vp]
-    L.gpdb_reevaluate.argtypes = [vp, vp, C.c_int32, vp]
-    L.gpdb_set_overlap.argtypes = [vp, C.c_int32]
-    L.gpdb_set_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
-    L.gpdb_detect_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
-    L.gpdb_detect_batch_select.argtypes = [vp, vp, vp, C.c_int32, C.POINTER(abi.Result), vp]
-    L.gpdb_preprocess_clouds.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, C.POINTER(abi.PreprocessParams), vp]
-    L.gpdb_get_clouds.argtypes = [vp, vp, vp, vp, vp]
-    L.gpdb_set_clouds_samples.argtypes = [vp, vp, vp]
-    L.gpdb_hand_search_batch.argtypes = [vp, vp, vp, C.POINTER(abi.Result), vp]
-    L.gpdb_find_clusters_batch.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]
-    L.gpdb_preprocess_clouds_device.argtypes = L.gpdb_preprocess_clouds.argtypes
-    L.gpdb_set_clouds_device.argtypes = L.gpdb_set_clouds.argtypes
-    L.gpdb_detect_batch_select_device.argtypes = [vp, vp, vp, C.c_int32, vp, vp, C.POINTER(abi.Result)]
-    L.gpdb_find_clusters_batch_device.argtypes = L.gpdb_find_clusters_batch.argtypes
-    L.gpdb_sis_params_default.argtypes = [C.POINTER(abi.SisParams)]
-    L.gpdb_sis_params_default.restype = None
-    L.gpdb_sis_batch.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, C.POINTER(abi.Result), vp]
-    L.gpdb_sis_batch_device.argtypes = [vp, C.POINTER(abi.SisParams), vp, vp, vp, vp, C.POINTER(abi.Result)]
-    L.gpdb_sis_positions.argtypes = [vp, vp, vp, vp, vp, vp]
-    for name, argtypes in {**abi.RESIDENT_PROTOTYPES, **abi.DEPTH_PROTOTYPES, **abi.PLANE_PROTOTYPES,
-                           **abi.REFINE_PROTOTYPES, **abi.OUTLIERS_PROTOTYPES}.items():
-        getattr(L, name).argtypes = argtypes
-    L.gpdb_plane_params_default.restype = None
+    for name, (restype, argtypes) in abi.PROTOTYPES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _LIB = L
     return L
 
@@ -133,48 +53,24 @@ def _p(a):
 def default_params(**over):
     p = abi.Params()
     lib().gpdb_params_default(C.byref(p))
-    q = abi.default_params(p.image_num_channels)
-    for name, _ in abi.Params._fields_:  # the two defaults must agree (tests check it)
-        pass
     chan = over.pop("channels", None)
     if chan is not None:
         p.image_num_channels = chan
-    for k, v in over.items():
-        if k == "hand_axes":
-            p.num_hand_axes = len(v)
-            for i, a in enumerate(v):
-                p.hand_axes[i] = a
-        elif k in ("workspace_grasps", "direction"):
-            for i, a in enumerate(v):
-                getattr(p, k)[i] = a
-        else:
-            setattr(p, k, v)
-    del q
-    return p
+    return abi.set_fields(p, **over)
 
 
 def preprocess_params(**over):
     """gpdb_preprocess_params with the reference defaults (cfg/eigen_params.cfg:16-21), overridden by keyword."""
     p = abi.PreprocessParams()
     lib().gpdb_preprocess_params_default(C.byref(p))
-    for k, v in over.items():
-        if k == "workspace":
-            p.workspace[:] = list(v)
-        else:
-            setattr(p, k, v)
-    return p
+    return abi.set_fields(p, **over)
 
 
 def sis_params(**over):
     """gpdb_sis_params with the reference defaults (gpdb_sis_params_default), overridden by keyword (cfg key names)."""
     p = abi.SisParams()
     lib().gpdb_sis_params_default(C.byref(p))
-    for k, v in over.items():
-        if k == "workspace":
-            p.workspace[:] = list(v)
-        else:
-            setattr(p, k, v)
-    return p
+    return abi.set_fields(p, **over)
 
 
 def plane_params(**over):
@@ -182,9 +78,7 @@ def plane_params(**over):
     probability 0.99, seed 0), overridden by keyword."""
     p = abi.PlaneParams()
     lib().gpdb_plane_params_default(C.byref(p))
-    for k, v in over.items():
-        setattr(p, k, v)
-    return p
+    return abi.set_fields(p, **over)
 
 
 def read_weights_file(weights_file, channels, model_file=None):
@@ -441,14 +335,31 @@ class Context:
         n = self._check(lib().gpdb_find_clusters(self.h, _p(hands), len(hands), int(min_inliers), _p(out)))
         return out[:n].copy()
 
+    # ---- batch bookkeeping: what the library installed, kept here to size the outputs of later batch calls ----
+    def _drop_batch(self):
+        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None
+
+    def _install(self, call, offsets, n_cameras, view_points, n_raw=None):
+        """Runs call(), which installs a batch of len(n_cameras) clouds, and records that batch: offsets [B+1] are its
+        point offsets (read by set_clouds, written by the preprocessing calls), n_raw the raw points of a preprocessing
+        call, whose clouds keep source indices (None after set_clouds). A failed install leaves no batch in the library,
+        so none is recorded. Returns offsets."""
+        self._drop_batch()
+        self._check(call())
+        self._n_clouds = len(n_cameras)
+        self._batch = (offsets, n_cameras, view_points, n_raw is not None)
+        self._n_raw = n_raw
+        return offsets
+
+    def _n_points(self):
+        return int(self._batch[0][-1]) if self._batch is not None else 0
+
     def set_clouds(self, clouds):
         """gpdb_set_clouds: installs a batch of processed clouds (list of dicts as set_cloud takes) beside the single cloud."""
         pk = pack_clouds(clouds)
-        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed gpdb_set_clouds leaves no batch
-        self._check(lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
-                                          _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])))
-        self._n_clouds = len(clouds)
-        self._batch = (pk["offsets"], pk["n_cameras"], pk["view_points"], False)
+        self._install(lambda: lib().gpdb_set_clouds(self.h, len(clouds), _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
+                                                    _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"])),
+                      pk["offsets"], pk["n_cameras"], pk["view_points"])
 
     def preprocess_clouds(self, raw_clouds, pp=None, read_back=True):
         """gpdb_preprocess_clouds: preprocess() of every raw cloud (list of dicts: xyz, optional normals, optional
@@ -458,15 +369,11 @@ class Context:
         pk = pack_clouds(raw_clouds)
         if pp is None:
             pp = preprocess_params()
-        B = len(raw_clouds)
-        poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
-        self._check(lib().gpdb_preprocess_clouds(self.h, B, _p(pk["offsets"]), _p(pk["xyz"]), _p(pk["normals"]),
-                                                 _p(pk["cam_source"]), _p(pk["n_cameras"]), _p(pk["view_points"]), C.byref(pp),
-                                                 _p(poff)))
-        self._n_clouds = B
-        self._batch = (poff, pk["n_cameras"], pk["view_points"], True)
-        self._n_raw = int(pk["offsets"][-1])
+        poff = np.zeros(len(raw_clouds) + 1, np.int32)
+        self._install(lambda: lib().gpdb_preprocess_clouds(self.h, len(raw_clouds), _p(pk["offsets"]), _p(pk["xyz"]),
+                                                           _p(pk["normals"]), _p(pk["cam_source"]), _p(pk["n_cameras"]),
+                                                           _p(pk["view_points"]), C.byref(pp), _p(poff)),
+                      poff, pk["n_cameras"], pk["view_points"], int(pk["offsets"][-1]))
         return self.get_clouds() if read_back else poff
 
     def get_clouds(self):
@@ -625,27 +532,18 @@ class Context:
         off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, True)
         if pp is None:
             pp = preprocess_params()
-        B = len(ks)
-        poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
-        self._check(lib().gpdb_preprocess_clouds_device(self.h, B, _p(off), px, pn, pc, _p(ks), _p(vp), C.byref(pp), _p(poff)))
-        self._n_clouds = B
-        self._batch = (poff, ks, vp, True)
-        self._n_raw = int(off[-1])
-        return poff
+        poff = np.zeros(len(ks) + 1, np.int32)
+        return self._install(lambda: lib().gpdb_preprocess_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp),
+                                                                         C.byref(pp), _p(poff)),
+                             poff, ks, vp, int(off[-1]))
 
     def _install_depth(self, fn, n_cameras, cameras, fmt, ptr, pp):
         ks, arr, vps = _depth_cameras(n_cameras, cameras)
         if pp is None:
             pp = preprocess_params()
-        B = len(ks)
-        poff = np.zeros(B + 1, np.int32)
-        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
-        self._check(fn(self.h, B, _p(ks), C.cast(arr, C.c_void_p), int(fmt), ptr, C.byref(pp), _p(poff)))
-        self._n_clouds = B
-        self._batch = (poff, ks, vps, True)
-        self._n_raw = sum(int(c.width) * int(c.height) for c in arr[:len(cameras)])
-        return poff
+        poff = np.zeros(len(ks) + 1, np.int32)
+        return self._install(lambda: fn(self.h, len(ks), _p(ks), C.cast(arr, C.c_void_p), int(fmt), ptr, C.byref(pp), _p(poff)),
+                             poff, ks, vps, sum(int(c.width) * int(c.height) for c in arr[:len(cameras)]))
 
     def preprocess_depth(self, views, pp=None, read_back=True):
         """gpdb_preprocess_depth: preprocess_clouds() of views given as depth images. views: one list per view of
@@ -695,20 +593,35 @@ class Context:
         npts = np.diff(self._batch[0]).astype(np.int64) if self._batch is not None else np.zeros(0, np.int64)
         return int(npts.sum()) if num_samples == 0 else int(np.minimum(npts, max(int(num_samples), 0)).sum())
 
+    def _subsample(self, fn, num_samples, seed, name, mask, need, per):
+        # the host twins: a mask of `need` bytes (None: nothing to size it by, and the library reports the state error)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8).ravel()
+        if m is not None and need is not None and len(m) != need:
+            raise ValueError(f"{name}: {len(m)} bytes, need one per {per} ({need})")
+        idx = np.zeros(max(self._subsample_room(num_samples), 1), np.int32)
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        self._check(fn(self.h, int(num_samples), C.c_uint64(int(seed)), _p(m), _p(idx), _p(soff)))
+        return [idx[soff[b]:soff[b + 1]].copy() for b in range(self._n_clouds)]
+
+    def _subsample_tensors(self, fn, num_samples, seed, name, d_mask, need):
+        import torch
+        dev = self.params.device
+        pm = None if d_mask is None else _device_arg(name, d_mask, torch.uint8, dev, need)
+        self._torch_stream()
+        room = self._subsample_room(num_samples)
+        out = torch.empty(room, dtype=torch.int32, device=f"cuda:{dev}")
+        soff = np.zeros(self._n_clouds + 1, np.int32)
+        n = self._check(fn(self.h, int(num_samples), C.c_uint64(int(seed)), pm, C.c_void_p(out.data_ptr()) if room else None,
+                           _p(soff)))
+        return soff, out[:n]
+
     def subsample_clouds(self, num_samples, seed, mask=None):
         """gpdb_subsample_clouds: Cloud::subsample of every installed cloud (include/gpd_b200_depth.h 5): num_samples
         cloud-local point indices per cloud without replacement, ascending (0: every eligible point), drawn with key
         seed + b. mask: one uint8 per raw point (pixel) of the preprocessing call that installed the batch, concatenated
         by view, or None; only points whose source raw point has a nonzero byte are eligible. Returns one int32 array per
         cloud, as detect_batch takes them."""
-        room = self._subsample_room(num_samples)
-        idx = np.zeros(max(room, 1), np.int32)
-        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8).ravel()
-        if m is not None and self._n_raw is not None and len(m) != self._n_raw:
-            raise ValueError(f"mask: {len(m)} bytes, need one per raw point ({self._n_raw})")
-        soff = np.zeros(self._n_clouds + 1, np.int32)
-        self._check(lib().gpdb_subsample_clouds(self.h, int(num_samples), C.c_uint64(int(seed)), _p(m), _p(idx), _p(soff)))
-        return [idx[soff[b]:soff[b + 1]].copy() for b in range(self._n_clouds)]
+        return self._subsample(lib().gpdb_subsample_clouds, num_samples, seed, "mask", mask, self._n_raw, "raw point")
 
     def subsample_clouds_tensors(self, num_samples, seed, d_mask=None):
         """gpdb_subsample_clouds_device: subsample_clouds() with the mask (uint8 CUDA tensor, one byte per raw point, or
@@ -716,48 +629,22 @@ class Context:
         indices (cloud b's at offsets[b] .. offsets[b+1]-1), the CSR pair detect_batch_select_tensors / sis_batch_tensors
         take."""
         import torch
-        dev = self.params.device
-        if d_mask is not None:
-            n_raw = self._n_raw if self._n_raw is not None else (d_mask.numel() if isinstance(d_mask, torch.Tensor) else 0)
-            pm = _device_arg("d_mask", d_mask, torch.uint8, dev, int(n_raw))
-        else:
-            pm = None
-        self._torch_stream()
-        room = self._subsample_room(num_samples)
-        out = torch.empty(room, dtype=torch.int32, device=f"cuda:{dev}")
-        soff = np.zeros(self._n_clouds + 1, np.int32)
-        n = self._check(lib().gpdb_subsample_clouds_device(self.h, int(num_samples), C.c_uint64(int(seed)), pm,
-                                                           C.c_void_p(out.data_ptr()) if room else None, _p(soff)))
-        return soff, out[:n]
+        n_raw = self._n_raw if self._n_raw is not None else (d_mask.numel() if isinstance(d_mask, torch.Tensor) else 0)
+        return self._subsample_tensors(lib().gpdb_subsample_clouds_device, num_samples, seed, "d_mask", d_mask, int(n_raw))
 
     def subsample_clouds_points(self, num_samples, seed, point_mask=None):
         """gpdb_subsample_clouds_points: subsample_clouds() with the mask over the installed points (one uint8 per point
         of the batch, concatenated by cloud, e.g. segment_planes()' eligible bytes), so it also works after set_clouds().
         Returns one int32 array per cloud."""
-        room = self._subsample_room(num_samples)
-        idx = np.zeros(max(room, 1), np.int32)
-        m = None if point_mask is None else np.ascontiguousarray(point_mask, dtype=np.uint8).ravel()
-        if m is not None and self._batch is not None and len(m) != int(self._batch[0][-1]):
-            raise ValueError(f"point_mask: {len(m)} bytes, need one per installed point ({int(self._batch[0][-1])})")
-        soff = np.zeros(self._n_clouds + 1, np.int32)
-        self._check(lib().gpdb_subsample_clouds_points(self.h, int(num_samples), C.c_uint64(int(seed)), _p(m), _p(idx),
-                                                       _p(soff)))
-        return [idx[soff[b]:soff[b + 1]].copy() for b in range(self._n_clouds)]
+        need = self._n_points() if self._batch is not None else None
+        return self._subsample(lib().gpdb_subsample_clouds_points, num_samples, seed, "point_mask", point_mask, need,
+                               "installed point")
 
     def subsample_clouds_points_tensors(self, num_samples, seed, d_point_mask=None):
         """gpdb_subsample_clouds_points_device: subsample_clouds_points() with the mask (uint8 CUDA tensor, one byte per
         installed point, or None) on the device. Returns (offsets, indices) as subsample_clouds_tensors()."""
-        import torch
-        dev = self.params.device
-        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
-        pm = None if d_point_mask is None else _device_arg("d_point_mask", d_point_mask, torch.uint8, dev, n_pts)
-        self._torch_stream()
-        room = self._subsample_room(num_samples)
-        out = torch.empty(room, dtype=torch.int32, device=f"cuda:{dev}")
-        soff = np.zeros(self._n_clouds + 1, np.int32)
-        n = self._check(lib().gpdb_subsample_clouds_points_device(self.h, int(num_samples), C.c_uint64(int(seed)), pm,
-                                                                  C.c_void_p(out.data_ptr()) if room else None, _p(soff)))
-        return soff, out[:n]
+        return self._subsample_tensors(lib().gpdb_subsample_clouds_points_device, num_samples, seed, "d_point_mask",
+                                       d_point_mask, self._n_points())
 
     def segment_plane(self, pl=None):
         """gpdb_segment_plane: the support plane of the single installed cloud (include/gpd_b200_plane.h). Returns
@@ -770,33 +657,29 @@ class Context:
         self._check(lib().gpdb_segment_plane(self.h, C.byref(pl), _p(plane), _p(cnt), _p(elig)))
         return plane, int(cnt[0]), elig[:n]
 
-    def _plane_outputs(self):
-        B = self._n_clouds
-        return np.zeros((max(B, 1), 4), np.float32), np.zeros(max(B, 1), np.int32), np.zeros(max(B, 1), np.int32)
+    def _segment_planes(self, fn, pl, eligible, p_eligible):
+        pl = plane_params() if pl is None else pl
+        n = max(self._n_clouds, 1)
+        planes, cnt, nh = np.zeros((n, 4), np.float32), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        B = self._check(fn(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh), p_eligible))
+        return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": eligible}
 
     def segment_planes(self, pl=None):
         """gpdb_segment_planes: the support plane of every installed cloud (cloud b with key seed + b). Returns a dict:
         planes [B, 4] float32, n_inliers [B], n_hypotheses [B] (RANSAC hypotheses evaluated) and eligible [N] uint8
         (concatenated by cloud, the point_mask subsample_clouds_points() takes)."""
-        pl = plane_params() if pl is None else pl
-        planes, cnt, nh = self._plane_outputs()
-        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
+        n_pts = self._n_points()
         elig = np.zeros(max(n_pts, 1), np.uint8)
-        B = self._check(lib().gpdb_segment_planes(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh), _p(elig)))
-        return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": elig[:n_pts]}
+        return self._segment_planes(lib().gpdb_segment_planes, pl, elig[:n_pts], _p(elig))
 
     def segment_planes_tensors(self, pl=None):
         """gpdb_segment_planes_device: segment_planes() with the eligible bytes in a uint8 CUDA tensor [N], on torch's
         current stream; planes and counts are host arrays as in segment_planes()."""
         import torch
-        pl = plane_params() if pl is None else pl
-        planes, cnt, nh = self._plane_outputs()
-        n_pts = int(self._batch[0][-1]) if self._batch is not None else 0
+        n_pts = self._n_points()
         self._torch_stream()
         elig = torch.empty(n_pts, dtype=torch.uint8, device=f"cuda:{self.params.device}")
-        B = self._check(lib().gpdb_segment_planes_device(self.h, C.byref(pl), _p(planes), _p(cnt), _p(nh),
-                                                         C.c_void_p(elig.data_ptr()) if n_pts else None))
-        return {"planes": planes[:B], "n_inliers": cnt[:B], "n_hypotheses": nh[:B], "eligible": elig}
+        return self._segment_planes(lib().gpdb_segment_planes_device, pl, elig, C.c_void_p(elig.data_ptr()) if n_pts else None)
 
     def refine_normals(self, k):
         """gpdb_refine_normals: refines the normals of the single installed cloud in place with k nearest neighbours
@@ -828,10 +711,9 @@ class Context:
         new point offsets [B+1], stats [B, 3] (mean, stddev, threshold) and kept, one byte per point before the call.
         Sample positions and the SIS record are dropped."""
         B = self._n_clouds
-        n = int(self._batch[0][-1]) if self._batch is not None else 0
         off = np.zeros(B + 1, np.int32)
         stats = np.zeros((max(B, 1), 3), np.float64)
-        kept = np.zeros(n, np.uint8)
+        kept = np.zeros(self._n_points(), np.uint8)
         try:
             self._check(lib().gpdb_remove_outliers_clouds(self.h, int(mean_k), float(stddev_mul), _p(off), _p(stats),
                                                           _p(kept)))
@@ -839,9 +721,9 @@ class Context:
             # GPDB_ERR_INVALID / GPDB_ERR_STATE come before any device work and change nothing; after any other error the
             # library holds no batch, and neither may this bookkeeping, which sizes the output buffers of later calls
             if e.code not in (-1, -3):
-                self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None
+                self._drop_batch()
             raise
-        self._batch = (off,) + tuple(self._batch[1:])
+        self._batch = (off,) + self._batch[1:]
         self._sis_shape = None
         return {"offsets": off, "stats": stats[:B], "kept": kept}
 
@@ -849,10 +731,7 @@ class Context:
         """gpdb_set_clouds_device: set_clouds() from CUDA tensors, laid out as preprocess_clouds_tensors takes them
         (normals required)."""
         off, ks, vp, (px, pn, pc) = self._cloud_tensors(point_offsets, xyz, normals, cam_source, n_cameras, view_points, False)
-        self._n_clouds, self._batch, self._sis_shape, self._n_raw = 0, None, None, None  # a failed call leaves no batch
-        self._check(lib().gpdb_set_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp)))
-        self._n_clouds = len(ks)
-        self._batch = (off, ks, vp, False)
+        self._install(lambda: lib().gpdb_set_clouds_device(self.h, len(ks), _p(off), px, pn, pc, _p(ks), _p(vp)), off, ks, vp)
 
     def detect_batch_select_tensors(self, sample_offsets, d_sample_idx, k):
         """gpdb_detect_batch_select_device: the k best candidates of every installed cloud, for cloud-local sample indices
@@ -1012,10 +891,10 @@ class Context:
         lib().gpdb_preprocess_timings(self.h, _p(ms))
         return ms
 
-    def _result(self, fn, sample_idx):
+    def _result(self, fn, sample_idx, *args):
         sidx = np.ascontiguousarray(sample_idx, dtype=np.int32)
         res = abi.Result()
-        self._check(fn(self.h, _p(sidx), len(sidx), C.byref(res)))
+        self._check(fn(self.h, _p(sidx), len(sidx), *args, C.byref(res)))
         S, Cc = self.params.image_size, self.params.image_num_channels
         out = abi.result_to_numpy(res, S * S * Cc)
         lib().gpdb_free_result(C.byref(res))
@@ -1026,13 +905,7 @@ class Context:
 
     def detect_select(self, sample_idx, num_selected):
         """detectGrasps + selectGrasps: the num_selected best candidates, sorted on the device (gpdb_detect_select)."""
-        sidx = np.ascontiguousarray(sample_idx, dtype=np.int32)
-        res = abi.Result()
-        self._check(lib().gpdb_detect_select(self.h, _p(sidx), len(sidx), int(num_selected), C.byref(res)))
-        S, Cc = self.params.image_size, self.params.image_num_channels
-        out = abi.result_to_numpy(res, S * S * Cc)
-        lib().gpdb_free_result(C.byref(res))
-        return out
+        return self._result(lib().gpdb_detect_select, sample_idx, int(num_selected))
 
     def detect_select_raw(self, sidx_i32, num_selected, res):
         """Timed path for bench.py; caller frees `res`."""

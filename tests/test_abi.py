@@ -28,6 +28,49 @@ def test_library_exports_every_declared_symbol():
     assert set(lib.EXPORTS) == set(syms)
 
 
+# the structs passed by reference, typed as pointers to their mirrors; arrays of records (gpdb_pose, gpdb_depth_camera)
+# and every other pointer, host or device memory, are c_void_p, and a char * string is c_char_p
+BY_REF = {"gpdb_params": abi.Params, "gpdb_result": abi.Result, "gpdb_preprocess_params": abi.PreprocessParams,
+          "gpdb_sis_params": abi.SisParams, "gpdb_plane_params": abi.PlaneParams}
+SCALARS = {"void": None, "int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64,
+           "double": C.c_double}
+
+
+def header_prototypes():
+    """{name: (return type, [parameter declarations])} of every function include/gpd_b200.h declares."""
+    h = open(os.path.join(ROOT, "include", "gpd_b200.h")).read()
+    h = re.sub(r"/\*.*?\*/|//[^\n]*|^\s*#[^\n]*", "", h, flags=re.S | re.M)
+    out = {}
+    for ret, name, params in re.findall(r"([\w\s*]+?)\s*\b(gpdb_\w+)\s*\(([^)]*)\)\s*;", h):
+        params = [" ".join(p.split()) for p in params.split(",")]
+        out[name] = (" ".join(ret.split()), [] if params == ["void"] else params)
+    return out
+
+
+def ctype_of(decl):
+    """The ctypes type that passes a C value declared as `decl` (a parameter or a return type)."""
+    base = next(w for w in re.sub(r"[*\[\]]", " ", decl).split() if w != "const")
+    depth = decl.count("*") + decl.count("[")
+    if depth == 0:
+        return SCALARS[base]
+    if depth == 2:  # gpdb_ctx **ctx_out; float *const out[8]
+        return C.POINTER(C.c_void_p) if base == "gpdb_ctx" else C.c_void_p
+    if base in BY_REF:
+        return C.POINTER(BY_REF[base])
+    return C.c_char_p if base == "char" and "*" in decl else C.c_void_p
+
+
+def test_prototypes_match_the_header():
+    decls = header_prototypes()
+    assert len(decls) >= 70 and set(decls) == set(abi.PROTOTYPES)
+    for name, (ret, params) in decls.items():
+        restype, argtypes = abi.PROTOTYPES[name]
+        assert restype is ctype_of(ret), (name, ret, restype)
+        assert len(argtypes) == len(params), (name, params, argtypes)
+        for p, t in zip(params, argtypes):
+            assert t is ctype_of(p), (name, p, t)
+
+
 def test_struct_layouts_match_the_header():
     src = r'''
 #include <stdio.h>

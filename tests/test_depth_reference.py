@@ -1,6 +1,6 @@
-"""The numpy restatement of include/gpd_b200_depth.h (tests/depth_reference.py) and the ctypes mirror of its entry points,
-without a GPU: prototypes and struct layout against the headers, the float32 back-projection against float64, the raw-cloud
-numbering, and the sampling rule."""
+"""The numpy restatement of include/gpd_b200_depth.h (tests/depth_reference.py) and the ctypes mirror of its camera struct,
+without a GPU: struct layout against the header, the float32 back-projection against float64, the raw-cloud numbering, and
+the sampling rule. tests/test_abi.py holds the prototypes of the depth entry points against include/gpd_b200.h."""
 import ctypes as C
 import os
 import re
@@ -11,34 +11,10 @@ import depth_reference as dr
 from gpd_b200 import abi, lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_CALLS = ("gpdb_preprocess_depth", "gpdb_preprocess_depth_device", "gpdb_subsample_clouds", "gpdb_subsample_clouds_device")
 
 
 def header(name):
     return re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", name)).read(), flags=re.S)
-
-
-def declared_params(name):
-    m = re.search(r"\bint\s+" + name + r"\s*\(([^)]*)\)\s*;", header("gpd_b200.h"))
-    assert m, f"{name} is not declared as returning int"
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-def test_prototypes_match_the_header():
-    for name in NEW_CALLS:
-        params = declared_params(name)
-        argtypes = abi.DEPTH_PROTOTYPES[name]
-        assert len(argtypes) == len(params), name
-        for p, t in zip(params, argtypes):
-            if p.startswith("const gpdb_preprocess_params *"):
-                assert t is C.POINTER(abi.PreprocessParams), (name, p)
-            elif "*" in p:
-                assert t is C.c_void_p, (name, p)
-            elif p.startswith("uint64_t "):
-                assert t is C.c_uint64, (name, p)
-            else:
-                assert p.startswith("int32_t ") and t is C.c_int32, (name, p)
-        assert name in lib.EXPORTS
 
 
 def test_camera_struct_matches_the_header():

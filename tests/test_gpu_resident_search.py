@@ -5,12 +5,10 @@ gpdb_classify_device) through the tensor methods of lib.Context.
 The oracle of every device route is its host route on the same seeded inputs, bit for bit: the records (cloud-local
 sample slots), the per-cloud offsets, the dense flags and the score bit patterns of hand_search_batch / detect_batch, the
 images of detect_batch with keep_images = 1 and the scores and logits of classify. The errors must be the host twin's
-(code and message, up to the entry point's name). The first test runs without a GPU: it holds the ctypes prototypes of
-the five calls against their declarations in include/gpd_b200.h.
+(code and message, up to the entry point's name). tests/test_abi.py holds the ctypes prototypes of the five calls
+against their declarations in include/gpd_b200.h.
 """
 import ctypes as C
-import os
-import re
 
 import numpy as np
 import pytest
@@ -18,37 +16,12 @@ import pytest
 from conftest import load_weights
 from gpd_b200 import abi, lib, scenes
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ERR_INVALID, ERR_STATE = -1, -3
 K1 = [(0.0, 0.0, 0.0)]
 K2 = [(0.0, 0.0, 0.0), (0.3, 0.0, 0.0)]
 K3 = [(0.0, 0.0, 0.0), (0.3, 0.0, 0.0), (-0.3, 0.1, 0.0)]
 K8 = [(-0.3, -0.2, 0.0), (0.0, -0.2, 0.0), (0.3, -0.2, 0.0), (-0.3, 0.2, 0.0), (0.0, 0.2, 0.0), (0.3, 0.2, 0.0),
       (0.0, 0.0, 0.0), (0.15, 0.0, 0.1)]
-NEW_CALLS = ("gpdb_set_clouds_samples_device", "gpdb_hand_search_batch_device", "gpdb_detect_batch_device",
-             "gpdb_images_batch_device", "gpdb_classify_device")
-
-
-def declared_params(name):
-    h = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "gpd_b200.h")).read(), flags=re.S)
-    m = re.search(r"\bint\s+" + name + r"\s*\(([^)]*)\)\s*;", h)
-    assert m, f"{name} is not declared as returning int"
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-def test_prototypes_match_the_header():
-    for name in NEW_CALLS:
-        params = declared_params(name)
-        argtypes = abi.RESIDENT_PROTOTYPES[name]
-        assert len(argtypes) == len(params), name
-        for p, t in zip(params, argtypes):
-            if p.startswith("gpdb_result *"):
-                assert t is C.POINTER(abi.Result), (name, p)
-            elif "*" in p:
-                assert t is C.c_void_p, (name, p)
-            else:
-                assert p.startswith("int32_t ") and t is C.c_int32, (name, p)
-        assert name in lib.EXPORTS
 
 
 # ---- GPU ---------------------------------------------------------------------------------------------------------------
