@@ -214,6 +214,7 @@ PROTOTYPES = {
     "gpdb_get_clouds": (_int, [_vp] * 5),
     "gpdb_preprocess_timings": (_int, [_vp, _vp]),
     "gpdb_reevaluate": (_int, [_vp, _vp, _i32, _vp]),
+    "gpdb_reevaluate_batch": (_int, [_vp] * 4),
     "gpdb_find_clusters": (_int, [_vp, _vp, _i32, _i32, _vp]),
     "gpdb_find_clusters_batch": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _vp]),
     "gpdb_preprocess_clouds_device": (_int, [_vp, _i32] + [_vp] * 6 + [_pp, _vp]),
@@ -225,6 +226,7 @@ PROTOTYPES = {
     "gpdb_detect_batch_device": (_int, [_vp] * 7 + [_res]),
     "gpdb_images_batch_device": (_int, [_vp] * 4),
     "gpdb_classify_device": (_int, [_vp, _vp, _i32, _vp, _vp]),
+    "gpdb_reevaluate_batch_device": (_int, [_vp] * 4),
     "gpdb_sis_params_default": (None, [_sp]),
     "gpdb_sis_batch": (_int, [_vp, _sp, _vp, _vp, _res, _vp]),
     "gpdb_sis_batch_device": (_int, [_vp, _sp, _vp, _vp, _vp, _vp, _res]),

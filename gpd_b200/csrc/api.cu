@@ -2318,6 +2318,54 @@ int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n,
   return classify_batches(ctx, images_hwc, n, nullptr, logits_out, &layers);
 }
 
+namespace {
+
+// gpdb_reevaluate[_batch][_device] after their checks: HandSearch::reevaluateHypotheses of the hand_offsets[B] hands,
+// group b (hand_offsets[b] .. hand_offsets[b+1]) against cloud b of store s, in one k_label launch. The store is only
+// read: a batch borrows its soff for the group offsets, as gpdb_images_batch_device does. device: hands and labels are
+// device arrays, labelled in place; else they go through SCR_HANDS / SCR_LABELS.
+int label_hands(gpdb_ctx *ctx, const CloudSet &s, const int32_t *hand_offsets, gpdb_pose *hands, int32_t *labels,
+                bool device) {
+  const int n = hand_offsets[s.n];
+  if (n == 0) return 0;
+  gpdb_pose *d_h = hands;
+  int *d_l = labels;
+  if (!device) {
+    d_h = (gpdb_pose *)gpdb_scratch(ctx, SCR_HANDS, sizeof(gpdb_pose) * (size_t)n);
+    d_l = (int *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int) * (size_t)n);
+    if (!d_h || !d_l) return GPDB_ERR_CUDA;
+    CUDA_TRY(cudaMemcpyAsync(d_h, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (s.n > 1)
+    CUDA_TRY(cudaMemcpyAsync(s.soff, hand_offsets, sizeof(int) * ((size_t)s.n + 1), cudaMemcpyHostToDevice, ctx->stream));
+  int rc;
+  if ((rc = geo_label(ctx, s, d_h, n, d_l)) != GPDB_OK) return rc;
+  if (!device) {
+    CUDA_TRY(cudaMemcpyAsync(hands, d_h, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(labels, d_l, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return n;
+}
+
+int reevaluate_batch(gpdb_ctx *ctx, const char *name, const int32_t *hand_offsets, gpdb_pose *hands, int32_t *labels_out,
+                     bool device) {
+  int rc = gpdb_check_state(ctx, false, false);
+  if (rc != GPDB_OK) return rc;
+  if ((rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth")) != GPDB_OK) return rc;
+  if ((rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, ctx->many.n, "cloud")) != GPDB_OK) return rc;
+  if (hand_offsets[ctx->many.n] > 0 && (!hands || !labels_out)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s or %s", name, device ? "d_hands" : "hands",
+                   device ? "d_labels_out" : "labels_out");
+    return GPDB_ERR_INVALID;
+  }
+  if (device && (rc = check_device_ptrs(ctx, name, {{"d_hands", hands}, {"d_labels_out", labels_out}})) != GPDB_OK)
+    return rc;
+  return label_hands(ctx, ctx->many, hand_offsets, hands, labels_out, device);
+}
+
+}  // namespace
+
 int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_out) {
   int rc = gpdb_check_state(ctx, true, false);
   if (rc != GPDB_OK) return rc;
@@ -2325,16 +2373,16 @@ int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n, int32_t *labels_
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_reevaluate: bad arguments");
     return GPDB_ERR_INVALID;
   }
-  if (n == 0) return 0;
-  gpdb_pose *d_h = (gpdb_pose *)gpdb_scratch(ctx, SCR_HANDS, sizeof(gpdb_pose) * (size_t)n);
-  int *d_l = (int *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int) * (size_t)n);
-  if (!d_h || !d_l) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemcpyAsync(d_h, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = geo_reeval(ctx, d_h, n, d_l)) != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(hands, d_h, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(labels_out, d_l, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return n;
+  const int32_t hand_offsets[2] = {0, n};
+  return label_hands(ctx, ctx->one, hand_offsets, hands, labels_out, false);
+}
+
+int gpdb_reevaluate_batch(gpdb_ctx *ctx, const int32_t *hand_offsets, gpdb_pose *hands, int32_t *labels_out) {
+  return reevaluate_batch(ctx, "gpdb_reevaluate_batch", hand_offsets, hands, labels_out, false);
+}
+
+int gpdb_reevaluate_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, gpdb_pose *d_hands, int32_t *d_labels_out) {
+  return reevaluate_batch(ctx, "gpdb_reevaluate_batch_device", hand_offsets, d_hands, d_labels_out, true);
 }
 
 }  // extern "C"

@@ -144,7 +144,7 @@ struct CloudSet {
 #define GPDB_PROF_SLOTS 48
 enum PathEvent {
   PATH_FRAMES_T1, PATH_FRAMES_T2, PATH_HANDS_T2, PATH_HANDS_T3, PATH_HANDS_SLAB, PATH_IMG2_BOX, PATH_IMG2_NONUNIT, PATH_IMG_GL,
-  PATH_IMG2_CAST, PATH_IMG2_DRAW, PATH_IMG2_STASH, PATH_IMG_CAST, PATH_IMG_DRAW, PATH_IMG_STASH, PATH_IMG_BALL
+  PATH_IMG2_CAST, PATH_IMG2_DRAW, PATH_IMG2_STASH, PATH_IMG_CAST, PATH_IMG_DRAW, PATH_IMG_STASH, PATH_IMG_BALL, PATH_LABEL_WALK
 };
 
 #define CUDA_TRY(expr)                                                                        \
@@ -218,7 +218,7 @@ enum ScratchSlot {
   SCR_CAND, SCR_COUNT,
   // main stream: candidate scores (+ logits in gpdb_classify); images in the cv::Mat layout
   SCR_SCORES, SCR_HWC,
-  // gpdb_reevaluate: hands, labels. Clustering: dense + compacted records (+ uploaded hands); group offsets, counts, keep flags
+  // gpdb_reevaluate[_batch]: hands, labels. Clustering: dense + compacted records (+ uploaded hands); group offsets, counts, keep flags
   SCR_HANDS, SCR_LABELS,
   // global-memory fallbacks of the capacity tiers. Image stage (main stream): the box lists of k_images' last tier and
   // the overflow list of its shared-memory tier
@@ -415,8 +415,9 @@ int geo_hwc_to_p16(gpdb_ctx *ctx, const uint8_t *d_hwc, int n, uint8_t *d_p16);
 int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_scores, int nc, int slot0, int P,
                        float *d_pose_scores, gpdb_pose *d_cand_out);
 
-// HandSearch::reevaluateHypotheses: labels + half / full flags of the given hands against the single cloud
-int geo_reeval(gpdb_ctx *ctx, gpdb_pose *d_hands, int n, int *d_labels);
+// HandSearch::reevaluateHypotheses: labels + half / full flags of the given hands, hand i against the cloud of store s
+// whose group holds it (group offsets in s.soff, uploaded by the caller; a store of one cloud reads no offsets)
+int geo_label(gpdb_ctx *ctx, const CloudSet &s, gpdb_pose *d_hands, int n, int *d_labels);
 // Clustering::findClusters (remove_inliers = false) on each of G groups of hands (group g: d_goff[g] .. d_goff[g+1]-1,
 // device offsets): dense per-hand cluster records + keep flags (3 = cluster), for geo_compact; d_gcount[G] (zeroed here)
 // receives the clusters per group

@@ -21,7 +21,8 @@ EXPORTS = list(abi.PROTOTYPES)
 # gpdb_debug_path_counts: index of each event in the returned array (include/gpd_b200.h)
 PATH_EVENTS = ["frames_tier1", "frames_tier2", "hands_tile", "hands_global", "hands_full_slab", "images2_box",
                "images2_nonunit", "images_global", "images2_cast_in_place", "images2_draw_in_place", "images2_stash_full",
-               "images_cast_in_place", "images_draw_in_place", "images_voxel_list_full", "images_ball_record_full"]
+               "images_cast_in_place", "images_draw_in_place", "images_voxel_list_full", "images_ball_record_full",
+               "label_walk"]
 
 
 class GpdbError(RuntimeError):
@@ -450,6 +451,21 @@ class Context:
         self._check(lib().gpdb_find_clusters_batch(self.h, len(arrs), _p(hoff), _p(hands), int(min_inliers), _p(out), _p(coff)))
         return [out[coff[g]:coff[g + 1]].copy() for g in range(len(arrs))]
 
+    def reevaluate_batch(self, hand_lists):
+        """gpdb_reevaluate_batch: reevaluate() of every group of hands (one abi.POSE_DTYPE array per installed cloud, may
+        be empty) against its cloud in one call. Returns (labels, records): one int32 array and one re-labelled record
+        array per group."""
+        if self._batch is not None and len(hand_lists) != self._n_clouds:  # no batch: the library names the state error
+            raise ValueError(f"{len(hand_lists)} hand lists for a batch of {self._n_clouds} clouds (one list per cloud)")
+        arrs = [np.asarray(h, dtype=abi.POSE_DTYPE).ravel() for h in hand_lists]
+        hoff = np.zeros(len(arrs) + 1, np.int32)
+        hoff[1:] = np.cumsum([len(a) for a in arrs])
+        hands = np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros(0, abi.POSE_DTYPE))
+        labels = np.zeros(len(hands), np.int32)
+        self._check(lib().gpdb_reevaluate_batch(self.h, _p(hoff), _p(hands), _p(labels)))
+        return ([labels[hoff[g]:hoff[g + 1]].copy() for g in range(len(arrs))],
+                [hands[hoff[g]:hoff[g + 1]].copy() for g in range(len(arrs))])
+
     def detect_batch_select(self, sample_lists, num_selected):
         """gpdb_detect_batch_select: the num_selected best candidates of every cloud; returns one record array per cloud."""
         offsets, sidx = self._pack_batch_samples(sample_lists)
@@ -844,6 +860,21 @@ class Context:
         out = torch.empty((n, S, S, Cc), dtype=torch.uint8, device=f"cuda:{dev}")
         self._check(lib().gpdb_images_batch_device(self.h, _p(hoff), ph, C.c_void_p(out.data_ptr()) if n else None))
         return out
+
+    def reevaluate_batch_tensors(self, hand_offsets, hands):
+        """gpdb_reevaluate_batch_device: reevaluate_batch() of gpdb_pose records in a uint8 CUDA tensor [n, POSE_BYTES]
+        (group b, labelled against cloud b: rows hand_offsets[b] .. hand_offsets[b+1]-1, hand_offsets a host array of B+1
+        entries), e.g. detect_batch_tensors' records of another context. The records' half / full flags are updated in
+        place; returns the labels as an int32 CUDA tensor [n]."""
+        import torch
+        hoff = _host_i32("hand_offsets", hand_offsets, self._n_clouds + 1 if self._batch is not None else None)
+        dev = self.params.device
+        n = int(hoff[-1]) if len(hoff) else 0
+        ph = _device_arg("hands", hands, torch.uint8, dev, n * POSE_BYTES)
+        self._torch_stream()
+        labels = torch.empty(n, dtype=torch.int32, device=f"cuda:{dev}")
+        self._check(lib().gpdb_reevaluate_batch_device(self.h, _p(hoff), ph, C.c_void_p(labels.data_ptr()) if n else None))
+        return labels
 
     def classify_tensors(self, images):
         """gpdb_classify_device: classify() of uint8 CUDA images [n, S, S, C] (cv::Mat layout). Returns (scores [n], logits

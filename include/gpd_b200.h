@@ -386,6 +386,16 @@ int gpdb_preprocess_timings(const gpdb_ctx *ctx, double ms_out[6]);
  * half_antipodal / full_antipodal fields of the records are updated in place. Returns n. */
 int gpdb_reevaluate(gpdb_ctx *ctx, gpdb_pose *hands, int32_t n_hands, int32_t *labels_out);
 
+/* HandSearch::reevaluateHypotheses for every cloud of the installed batch in one call: group b, hands[hand_offsets[b] ..
+ * hand_offsets[b+1]), is re-labelled against cloud b (hand_offsets: B + 1 host entries starting at 0, never decreasing;
+ * an empty group is allowed). Fields read and written as gpdb_reevaluate; group b's records and labels are bit-equal to
+ * gpdb_reevaluate on those hands with cloud b installed alone. The hands may come from anywhere, e.g. the candidates of
+ * camera views detected in another context, labelled here against ground-truth clouds installed once. The call only
+ * reads the store: the batch, its sample positions and the SIS record are unchanged. Returns hand_offsets[B];
+ * GPDB_ERR_STATE when no batch is installed; malformed offsets or NULL arrays for a non-empty call are GPDB_ERR_INVALID
+ * before any device work, with the outputs untouched. */
+int gpdb_reevaluate_batch(gpdb_ctx *ctx, const int32_t *hand_offsets, gpdb_pose *hands, int32_t *labels_out);
+
 /* Replaces: Clustering::findClusters(hand_list, remove_inliers = false) (clustering.cpp:5-105; GraspDetector::detectGrasps
  * step 6, grasp_detector.cpp:283-301; SequentialImportanceSampling step 4) on the device: one warp per hand over the n
  * hands (n <= num_selected in detectGrasps), inliers folded in index order so that the running mean / variance are the
@@ -476,6 +486,11 @@ int gpdb_images_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, const g
 /* gpdb_classify on n images in device memory (d_images_hwc [n * S*S*C], HWC uint8): d_scores_out [n] and d_logits_out
  * [n * 2] (may be NULL) are written by the classifier directly. Bit-equal to gpdb_classify, for both lenet_impl values. */
 int gpdb_classify_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, int32_t n, float *d_scores_out, float *d_logits_out);
+
+/* gpdb_reevaluate_batch on device records: d_hands [hand_offsets[B]] are re-labelled in place and d_labels_out
+ * [hand_offsets[B]] receives the labels, bit-equal to the host twin. With images_batch_device this keeps the images and
+ * the labels of many views on the GPU (training data, INTEGRATION.md). */
+int gpdb_reevaluate_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, gpdb_pose *d_hands, int32_t *d_labels_out);
 
 /* --- sequential importance sampling: SequentialImportanceSampling::detectGrasps on the device ----------------------------
  * (sequential_importance_sampling.cpp:54-270) over every cloud of the installed batch (gpdb_set_clouds[_device] /
@@ -725,7 +740,8 @@ int gpdb_debug_phase_cycles(gpdb_ctx *ctx, int enable, uint64_t cycles_out[32]);
  *  [10] ... images whose shadow voxel stash overflowed
  *  [11] k_images shadow points cast in place  [12] ... draws evaluated in place  [13] ... images whose shadow voxel
  *       list overflowed  [14] ... shadow casts that walked the grid because the in-ball record (tile C) was full
- *  [15] unused, zero. */
+ *  [15] gpdb_reevaluate[_batch][_device] hands whose Antipodal passes walked the grid because the closing region held over
+ *       1 024 points (the neighbour-0 padding is not counted) */
 int gpdb_debug_path_counts(gpdb_ctx *ctx, uint64_t counts_out[16]);
 /* Development aid: gpdb_classify (same batching, same kernels of the implementation lenet_impl selects) that also returns
  * what each LeNet layer computed, in one layout for both implementations. images_hwc as gpdb_classify; outputs:
