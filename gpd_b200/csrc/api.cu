@@ -834,12 +834,13 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
     CUDA_TRY(cudaSetDevice(ctx->device));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     // ---- one upload of the concatenated raw arrays
-    const size_t raw_bytes = sizeof(float) * 3 * (size_t)M + (size_t)M + 16 + (normals ? sizeof(double) * 3 * (size_t)M : 0);
-    unsigned char *raw = (unsigned char *)gpdb_scratch(ctx, SCR_SIDX, raw_bytes);
-    if (!raw) return GPDB_ERR_CUDA;
-    double *nrm_up = normals ? (double *)raw : nullptr;
-    float *xyz_up = (float *)(raw + (normals ? sizeof(double) * 3 * (size_t)M : 0));
-    d_cam_raw = (uint8_t *)(xyz_up + 3 * (size_t)M);
+    double *nrm_up = nullptr;
+    float *xyz_up;
+    if (!gpdb_carve(ctx, SCR_SIDX, [&](Carve &c) {
+          if (normals) nrm_up = c.take<double>(3 * (size_t)M);
+          xyz_up = c.take<float>(3 * (size_t)M); d_cam_raw = c.take<uint8_t>((size_t)M + 16);
+        }))
+      return GPDB_ERR_CUDA;
     cudaEventRecord(ev[0], ctx->stream);
     CUDA_TRY(cudaMemcpyAsync(xyz_up, xyz, sizeof(float) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(d_cam_raw, cam.data(), (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
@@ -2397,17 +2398,22 @@ static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, cons
   for (int g = 0; g <= G; g++) cluster_offsets_out[g] = 0;
   if (n == 0) return 0;
   CUDA_TRY(cudaSetDevice(ctx->device));
-  gpdb_pose *d_dense = (gpdb_pose *)gpdb_scratch(ctx, SCR_HANDS, sizeof(gpdb_pose) * (size_t)n * (device ? 2 : 3));
-  int *d_goff = (int *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int) * (2 * (size_t)G + 1) + (size_t)n);
+  gpdb_pose *d_dense, *d_out, *d_up = nullptr;  // dense records, compacted records, the uploaded hands
+  int *d_goff, *d_gcount;
+  uint8_t *d_keep;
+  const bool ok = gpdb_carve(ctx, SCR_HANDS, [&](Carve &c) {
+                    d_dense = c.take<gpdb_pose>(n); d_out = c.take<gpdb_pose>(n);
+                    if (!device) d_up = c.take<gpdb_pose>(n);
+                  }) &&
+                  gpdb_carve(ctx, SCR_LABELS, [&](Carve &c) {
+                    d_goff = c.take<int>((size_t)G + 1); d_gcount = c.take<int>(G); d_keep = c.take<uint8_t>(n);
+                  });
   int *d_count = (int *)gpdb_scratch(ctx, SCR_COUNT, 64);
-  if (!d_dense || !d_goff || !d_count) return GPDB_ERR_CUDA;
-  gpdb_pose *d_out = d_dense + n;
-  int *d_gcount = d_goff + G + 1;
-  uint8_t *d_keep = (uint8_t *)(d_gcount + G);
+  if (!ok || !d_count) return GPDB_ERR_CUDA;
   const gpdb_pose *d_in = hands;
   if (!device) {
-    d_in = d_out + n;
-    CUDA_TRY(cudaMemcpyAsync(d_out + n, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    d_in = d_up;
+    CUDA_TRY(cudaMemcpyAsync(d_up, hands, sizeof(gpdb_pose) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   }
   CUDA_TRY(cudaMemcpyAsync(d_goff, hand_offsets, sizeof(int) * ((size_t)G + 1), cudaMemcpyHostToDevice, ctx->stream));
   int rc;
@@ -2482,20 +2488,23 @@ int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32
 
 // ---- sequential importance sampling (gpdb_sis_batch) ----------------------------------------------------------------
 
-// The arrays of SCR_SIS (doubles first): kept [3 * KC] with KC = n_init + B*R*S, evaluated [3 * B*R*S]; then the ints:
-// init offsets [B+1] and indices [n_init], kept counts [B], round counts [R*B], hand counts [B], the installed sample
-// list [KC]
+// The arrays of SCR_SIS for B clouds, R rounds of S positions and n_init initial samples: kept positions (KC = n_init +
+// B*R*S of them) and evaluated positions, the initial offsets and indices, the kept counts [B] followed by the round
+// counts [R*B] (ecount, zeroed with them), the hand counts and the installed sample list
 struct SisArena {
   double *kept, *eval;
   int *init_off, *init_idx, *kcount, *ecount, *hcount, *sidx;
 };
-static size_t sis_arena(int B, int R, int S, int n_init, void *base, SisArena *a) {
+static void sis_layout(Carve &c, int B, int R, int S, int n_init, SisArena &a) {
   const size_t RS = (size_t)R * S, KC = (size_t)n_init + (size_t)B * RS;
-  double *d = (double *)base;
-  int *i = (int *)(d + 3 * (KC + (size_t)B * RS));
-  if (a) *a = {d, d + 3 * KC, i, i + B + 1, i + B + 1 + n_init, i + 2 * B + 1 + n_init,
-               i + 2 * B + 1 + n_init + R * (size_t)B, i + 3 * B + 1 + n_init + R * (size_t)B};
-  return sizeof(double) * 3 * (KC + (size_t)B * RS) + sizeof(int) * (3 * (size_t)B + 1 + n_init + (size_t)R * B + KC);
+  a.kept = c.take<double>(3 * KC);
+  a.eval = c.take<double>(3 * (size_t)B * RS);
+  a.init_off = c.take<int>((size_t)B + 1);
+  a.init_idx = c.take<int>(n_init);
+  a.kcount = c.take<int>((size_t)B * (R + 1));
+  a.ecount = c.base ? a.kcount + B : nullptr;
+  a.hcount = c.take<int>(B);
+  a.sidx = c.take<int>(KC);
 }
 
 // The argument checks of gpdb_sis_batch[_device] after the state checks: parameters and offsets
@@ -2684,10 +2693,8 @@ static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp,
   }
   SisState &st = *ctx->sis;
   const int R = sp->num_iterations, S = sp->num_samples_per_iteration;
-  void *base = gpdb_scratch(ctx, SCR_SIS, sis_arena(B, R, S, n0, nullptr, nullptr));
-  if (!base) return GPDB_ERR_CUDA;
   SisArena a;
-  sis_arena(B, R, S, n0, base, &a);
+  if (!gpdb_carve(ctx, SCR_SIS, [&](Carve &c) { sis_layout(c, B, R, S, n0, a); })) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(a.init_off, init_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   if (n0 > 0)
     CUDA_TRY(cudaMemcpyAsync(a.init_idx, init_idx, sizeof(int) * (size_t)n0,
@@ -2739,7 +2746,7 @@ int gpdb_sis_positions(gpdb_ctx *ctx, int32_t *eval_offsets_out, int32_t *eval_r
   const SisState &st = *ctx->sis;
   const int B = st.B, R = st.R, S = st.S, RS = R * S;
   SisArena a;
-  sis_arena(B, R, S, st.init_off[B], ctx->scratch[SCR_SIS], &a);
+  carve_at(ctx->scratch[SCR_SIS], [&](Carve &c) { sis_layout(c, B, R, S, st.init_off[B], a); });
   CUDA_TRY(cudaSetDevice(ctx->device));
   // the evaluated and kept arenas, read once on the context's stream and unpacked on the host
   std::vector<double> ev(eval_xyz_out ? 3 * (size_t)B * RS : 0), kp(kept_xyz_out ? 3 * ((size_t)st.init_off[B] + (size_t)B * RS) : 0);

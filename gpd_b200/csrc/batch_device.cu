@@ -68,16 +68,6 @@ __global__ void k_image_hands(const gpdb_pose *in, int n, int base, gpdb_pose *o
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                                                                    \
-  do {                                                                                                    \
-    ctx->launches++;                                                                                      \
-    cudaError_t e__ = cudaGetLastError();                                                                 \
-    if (e__ != cudaSuccess) {                                                                             \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                                                                               \
-    }                                                                                                     \
-  } while (0)
-
 int batch_pack_cameras(gpdb_ctx *ctx, const int32_t *d_rows, const int *d_off, const long long *d_row_off, const int *d_k,
                        int B, int N, bool eq1, bool strict01, uint8_t *d_cam, int *d_all_seen,
                        unsigned long long *d_first_bad) {

@@ -157,6 +157,17 @@ enum PathEvent {
     }                                                                                         \
   } while (0)
 
+// after each kernel launch: counts it in ctx->launches and turns a launch error into GPDB_ERR_CUDA
+#define LAUNCH_CHECK()                                                                                    \
+  do {                                                                                                    \
+    ctx->launches++;                                                                                      \
+    cudaError_t e__ = cudaGetLastError();                                                                 \
+    if (e__ != cudaSuccess) {                                                                             \
+      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
+      return GPDB_ERR_CUDA;                                                                               \
+    }                                                                                                     \
+  } while (0)
+
 struct LenetWeights {  // device pointers, layouts documented in lenet_simt.cu
   float *c1w, *c1b, *c2w, *c2b, *i1w, *i1b, *i2w, *i2b;
   int C;
@@ -291,6 +302,36 @@ cudaEvent_t gpdb_st_begin(gpdb_ctx *ctx);
 void gpdb_st_end(gpdb_ctx *ctx, int stage, cudaEvent_t begin);
 void *gpdb_scratch(gpdb_ctx *ctx, ScratchSlot slot, size_t bytes);  // returns nullptr on failure (error set)
 
+// Several arrays in one buffer, each stated once. A layout is a callable that takes its arrays from a Carve, in order:
+// run with a null base it only adds up the bytes (carve_bytes), run over a buffer it assigns the pointers (carve_at),
+// so the size and the pointers cannot disagree. Each array starts at the alignment of its type, or at `align`.
+struct Carve {
+  unsigned char *base;
+  size_t at;
+  template <class T> T *take(size_t n, size_t align = alignof(T)) {
+    at = (at + align - 1) / align * align;
+    T *p = base ? reinterpret_cast<T *>(base + at) : nullptr;
+    at += sizeof(T) * n;
+    return p;
+  }
+};
+template <class Layout> size_t carve_bytes(Layout &&layout) {
+  Carve c{nullptr, 0};
+  layout(c);
+  return c.at;
+}
+template <class Layout> void carve_at(void *base, Layout &&layout) {
+  Carve c{static_cast<unsigned char *>(base), 0};
+  layout(c);
+}
+// scratch slot `slot` grown to the layout's bytes, then carved by it; false: no memory (error set)
+template <class Layout> bool gpdb_carve(gpdb_ctx *ctx, ScratchSlot slot, Layout &&layout) {
+  void *base = gpdb_scratch(ctx, slot, carve_bytes(layout));
+  if (!base) return false;
+  carve_at(base, layout);
+  return true;
+}
+
 // api.cu
 int gpdb_pipe_create(gpdb_ctx *ctx);
 void gpdb_pipe_destroy(gpdb_ctx *ctx);
@@ -344,6 +385,38 @@ __device__ __forceinline__ int csr_owner(const int *a, int n, long long x) {
     if (a[mid] <= x) lo = mid; else hi = mid;
   }
   return lo;
+}
+
+// One sequential fold over v[0 .. n) per CTA of THREADS threads: thread 0 applies add(v[j]) for j = 0, 1, .., n - 1
+// from one half of `stage` (double-buffered chunks of CHUNK values in shared memory, 16-byte aligned) while warps 1..
+// stage the next chunk into the other half, so the chain waits on shared loads only. Every thread of the CTA calls it;
+// it returns with the CTA synchronised.
+template <int THREADS, int CHUNK, class Add>
+__device__ __forceinline__ void ordered_fold(const float *v, int n, float (*stage)[CHUNK], Add &&add) {
+  const int nc = (n + CHUNK - 1) / CHUNK;
+  for (int j = threadIdx.x; j < min(n, CHUNK); j += THREADS) stage[0][j] = __ldg(v + j);
+  __syncthreads();
+  for (int c = 0; c < nc; c++) {
+    const int base = c * CHUNK;
+    if (threadIdx.x == 0) {
+      const float *p = stage[c & 1];
+      const int len = min(CHUNK, n - base);
+      int j = 0;
+#pragma unroll 4
+      for (; j + 4 <= len; j += 4) {
+        const float4 q = *reinterpret_cast<const float4 *>(p + j);
+        add(q.x);
+        add(q.y);
+        add(q.z);
+        add(q.w);
+      }
+      for (; j < len; j++) add(p[j]);
+    } else if (threadIdx.x >= 32 && c + 1 < nc) {
+      const int nb = base + CHUNK, nl = min(CHUNK, n - nb);
+      for (int j = threadIdx.x - 32; j < nl; j += THREADS - 32) stage[(c + 1) & 1][j] = __ldg(v + nb + j);
+    }
+    __syncthreads();
+  }
 }
 
 // batch_device.cu (the device-resident batch entry points). The checks lower *d_first_bad (set to all ones by the caller)
@@ -430,6 +503,9 @@ int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *
 // per-cloud bounds of xyz (cloud b: points d_off[b] .. d_off[b+1]-1, device offsets; `largest` points in the largest
 // cloud) -> bounds[6b .. 6b+5] (min x y z, max x y z as order-preserving ints; an empty cloud keeps INT_MAX / INT_MIN)
 int pre_bounds_batch(gpdb_ctx *ctx, const float *xyz, const int *d_off, int B, int largest, int *bounds);
+// the exclusive scan of n compaction flags: flag holds n + 1 ints (flag[n] is zeroed here), pos[0 .. n] receives the
+// positions and pos[n] the number of flagged entries; counts its 2 launches
+int scan_flags(gpdb_ctx *ctx, int *flag, int *pos, int n);
 // filters + voxelises a raw batch into the arenas of store s (reserved inside); poff[B+1] (host) = processed offsets
 int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw, const uint8_t *d_cam_raw,
                               const double *d_nrm_raw, int M, int B, const int *roff, const gpdb_preprocess_params &pp,

@@ -127,18 +127,6 @@ __global__ void k_sub_gather(int E, const int *pick, const int *ppos, const int 
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
-static size_t depth_camera_table_bytes(int C) { return sizeof(DepthCam) * (size_t)C + sizeof(int) * ((size_t)C + 1); }
-
 // Back-projection + filter of the pixels of B views (camera descriptions cams, view b has n_cameras[b] of them; raw
 // offsets roff = cumulative pixels per view), then the voxelise / emit back of preprocess.cu
 int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format, const gpdb_depth_camera *cams,
@@ -148,10 +136,12 @@ int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format,
   const int M = roff[B];
   int C = 0;
   for (int b = 0; b < B; b++) C += n_cameras[b];
-  // the camera table (behind the call's header): C DepthCam, then the pixel offsets of the cameras [C+1]
-  std::vector<unsigned char> h_tab(depth_camera_table_bytes(C));
-  DepthCam *tab = (DepthCam *)h_tab.data();
-  int *cam_off = (int *)(tab + C);
+  // the camera table: the cameras, then their pixel offsets [C+1]; staged on the host, copied behind the call's header
+  DepthCam *tab;
+  int *cam_off;
+  const auto table = [&](Carve &c) { tab = c.take<DepthCam>(C); cam_off = c.take<int>((size_t)C + 1); };
+  std::vector<unsigned char> h_tab(carve_bytes(table));
+  carve_at(h_tab.data(), table);
   cam_off[0] = 0;
   for (int b = 0, c = 0; b < B; b++)
     for (int k = 0; k < n_cameras[b]; k++, c++) {
@@ -172,32 +162,30 @@ int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format,
   int rc = pre_batch_header(ctx, B, roff, pp, h_tab.size(), h);
   if (rc != GPDB_OK) return rc;
   CUDA_TRY(cudaMemcpyAsync(h.extra, h_tab.data(), h_tab.size(), cudaMemcpyHostToDevice, ctx->stream));
-  const DepthCam *d_cams = (const DepthCam *)h.extra;
-  const int *d_cam_off = (const int *)(d_cams + C);
-  // per pixel: filter flag + its scan (M + 1 each), the camera mask
-  int *flag = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * 2 * ((size_t)M + 1));
-  if (!flag) return GPDB_ERR_CUDA;
-  int *pos = flag + M + 1;
+  carve_at(h.extra, table);  // tab and cam_off now address the device copy
+  const DepthCam *d_cams = tab;
+  const int *d_cam_off = cam_off;
+  // per pixel: filter flag + its scan, the camera mask
+  int *flag, *pos;
+  if (!gpdb_carve(ctx, SCR_KEYS, [&](Carve &c) {
+        flag = c.take<int>((size_t)M + 1); pos = c.take<int>((size_t)M + 1);
+      }))
+    return GPDB_ERR_CUDA;
   uint8_t *cam_raw = (uint8_t *)gpdb_scratch(ctx, SCR_SIDX, (size_t)M + 16);
   if (!cam_raw) return GPDB_ERR_CUDA;
   k_depth_flag<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_depth, format, M, d_cam_off, C, d_cams, h.ws, flag, cam_raw);
   LAUNCH_CHECK();
-  CUDA_TRY(cudaMemsetAsync(flag + M, 0, sizeof(int), ctx->stream));  // pos[M] = number of filtered points
-  size_t tmp_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, M + 1, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
-  if (!tmp) return GPDB_ERR_CUDA;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, M + 1, ctx->stream));
-  ctx->launches += 2;
+  if ((rc = scan_flags(ctx, flag, pos, M)) != GPDB_OK) return rc;  // pos[M] = number of filtered points
   if ((rc = pre_filter_offsets(ctx, pos, h, B)) != GPDB_OK) return rc;
   std::vector<int> foff((size_t)B + 1);
   CUDA_TRY(cudaMemcpyAsync(foff.data(), h.foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   // the filtered points alone: keep + xyz1, sized by the count just read back
   const int M1 = foff[B];
-  int *keep = (int *)gpdb_scratch(ctx, SCR_WORK_B, (sizeof(int) + 3 * sizeof(float)) * (size_t)M1);
-  if (!keep) return GPDB_ERR_CUDA;
-  float *xyz1 = (float *)(keep + M1);
+  int *keep;
+  float *xyz1;
+  if (!gpdb_carve(ctx, SCR_WORK_B, [&](Carve &c) { keep = c.take<int>(M1); xyz1 = c.take<float>(3 * (size_t)M1); }))
+    return GPDB_ERR_CUDA;
   if (M1 > 0) {
     k_depth_compact<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_depth, format, M, d_cam_off, C, d_cams, flag, pos, keep,
                                                                xyz1);
@@ -211,35 +199,33 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
                    bool per_point, int *d_out, int *soff) {
   const int tb = 256;
   const int B = s.n, N = s.points();
-  // device: point offsets, raw offsets, eligible offsets, output offsets [B+1 each]
-  int *d_off = (int *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(int) * 4 * ((size_t)B + 1));
-  if (!d_off) return GPDB_ERR_CUDA;
-  int *d_roff = d_off + B + 1, *d_eoff = d_roff + B + 1, *d_soff = d_eoff + B + 1;
+  // device: point offsets, raw offsets, eligible offsets, output offsets
+  int *d_off, *d_roff, *d_eoff, *d_soff;
+  if (!gpdb_carve(ctx, SCR_WORK_A, [&](Carve &c) {
+        d_off = c.take<int>((size_t)B + 1); d_roff = c.take<int>((size_t)B + 1); d_eoff = c.take<int>((size_t)B + 1);
+        d_soff = c.take<int>((size_t)B + 1);
+      }))
+    return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(d_off, s.off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   if (d_mask && !per_point)
     CUDA_TRY(cudaMemcpyAsync(d_roff, s.raw_off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   std::vector<int> eoff((size_t)B + 1, 0);
   int *flag = nullptr, *pos = nullptr;
   if (N > 0) {
-    flag = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * 2 * ((size_t)N + 1));
-    if (!flag) return GPDB_ERR_CUDA;
-    pos = flag + N + 1;
+    if (!gpdb_carve(ctx, SCR_KEYS, [&](Carve &c) {
+          flag = c.take<int>((size_t)N + 1); pos = c.take<int>((size_t)N + 1);
+        }))
+      return GPDB_ERR_CUDA;
     if (d_mask && per_point) k_sub_flag_points<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_mask, flag);
     else k_sub_flag<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_off, B, s.src, d_roff, d_mask, flag);
     LAUNCH_CHECK();
-    CUDA_TRY(cudaMemsetAsync(flag + N, 0, sizeof(int), ctx->stream));
-    size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, N + 1, ctx->stream);
-    void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
-    if (!tmp) return GPDB_ERR_CUDA;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, N + 1, ctx->stream));
-    ctx->launches += 2;
+    int rc = scan_flags(ctx, flag, pos, N);
+    if (rc != GPDB_OK) return rc;
     // eligible offsets eoff[b] = pos[off[b]] (the filtered-offsets kernel of preprocessing, on the point offsets)
     PreBatch h{};
     h.roff = d_off;
     h.foff = d_eoff;
-    const int rc = pre_filter_offsets(ctx, pos, h, B);
-    if (rc != GPDB_OK) return rc;
+    if ((rc = pre_filter_offsets(ctx, pos, h, B)) != GPDB_OK) return rc;
     CUDA_TRY(cudaMemcpyAsync(eoff.data(), d_eoff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   }
@@ -254,11 +240,14 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
   }
   const int n = soff[B];
   if (E == 0) return 0;
-  // keys, sorted keys (8 B); j, e, sorted e, pick flags + their scan (4 B); E each (E + 1 for the flags and the scan)
-  unsigned long long *keys = (unsigned long long *)gpdb_scratch(ctx, SCR_WORK_C, (size_t)E * (8 + 8 + 4 + 4 + 4 + 4 + 4) + 8);
-  if (!keys) return GPDB_ERR_CUDA;
-  unsigned long long *keys2 = keys + E;
-  int *vals = (int *)(keys2 + E), *ev = vals + E, *ev2 = ev + E, *pick = ev2 + E, *ppos = pick + E + 1;
+  // keys, sorted keys; j, e, sorted e; pick flags and their scan
+  unsigned long long *keys, *keys2;
+  int *vals, *ev, *ev2, *pick, *ppos;
+  if (!gpdb_carve(ctx, SCR_WORK_C, [&](Carve &c) {
+        keys = c.take<unsigned long long>(E); keys2 = c.take<unsigned long long>(E); vals = c.take<int>(E);
+        ev = c.take<int>(E); ev2 = c.take<int>(E); pick = c.take<int>((size_t)E + 1); ppos = c.take<int>((size_t)E + 1);
+      }))
+    return GPDB_ERR_CUDA;
   k_sub_compact<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(N, d_off, B, flag, pos, seed, keys, all ? d_out : vals,
                                                            all ? nullptr : ev);
   LAUNCH_CHECK();

@@ -2768,16 +2768,6 @@ __global__ void k_batch_sel_order(const int *sorted_vals, const int *cand_off, c
 // ================================================================================================
 // host launchers
 // ================================================================================================
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 __global__ void k_path_add(unsigned long long *prof, int e0, const int *n0, int e1, const int *n1) {
   // atomic: the hand search of the next chunk may run on its own stream beside the image kernels of this one
   atomicAdd(prof + GPDB_PROF_PATH + e0, (unsigned long long)(unsigned)*n0);
@@ -2793,18 +2783,25 @@ static int path_add(gpdb_ctx *ctx, int e0, const int *n0, int e1, const int *n1)
   return GPDB_OK;
 }
 
+// SCR_OVF for a tiered launch over n samples: the tier-1 overflow list and its count, the tier-2 list and its count
+static bool overflow_lists(gpdb_ctx *ctx, int n, int *&ovf, int *&ovf_count, int *&ovf2, int *&ovf2_count) {
+  return gpdb_carve(ctx, SCR_OVF, [&](Carve &c) {
+    ovf = c.take<int>(n); ovf_count = c.take<int>(1); ovf2 = c.take<int>(n); ovf2_count = c.take<int>(1);
+  });
+}
+
 template <bool BATCH>
 static int launch_frames(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int n, double *d_frames, uint8_t *d_valid) {
   const int cap0 = 128;  // ~44 points at the default nn_radius on a 3 mm cloud
   const size_t smem0 = (size_t)2 * LRF_WARPS * cap0 * sizeof(unsigned long long);
   const size_t smem1 = (size_t)2 * LRF_WARPS * LRF_CAP * sizeof(unsigned long long);
   CUDA_TRY(cudaFuncSetAttribute(k_frames<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * 2 * ((size_t)n + 1));
+  int *ovf, *ovf_count, *ovf2, *ovf2_count;
+  if (!overflow_lists(ctx, n, ovf, ovf_count, ovf2, ovf2_count)) return GPDB_ERR_CUDA;
   const int g2 = 37;  // tier 2: 148 warps, 2 x 8 B x LRF_CAP_GLOBAL each (38 MB of scratch)
   unsigned long long *gkeys =
       (unsigned long long *)gpdb_scratch(ctx, SCR_FRAMES_GL, sizeof(unsigned long long) * 2 * LRF_CAP_GLOBAL * (size_t)g2 * LRF_WARPS);
-  if (!ovf || !gkeys) return GPDB_ERR_CUDA;
-  int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
+  if (!gkeys) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
   const DevCloud &cl = s.view;
@@ -2840,10 +2837,10 @@ static int launch_hands(gpdb_ctx *ctx, const CloudSet &s, const int *d_sidx, int
                         const uint8_t *d_valid, gpdb_pose *d_poses, uint8_t *d_flags) {
   // per call, not once per process: function attributes belong to the current device's context (one context per GPU)
   CUDA_TRY(cudaFuncSetAttribute(k_hands<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, HANDS_CAP2 * 16));
-  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * 2 * ((size_t)n + 1));
+  int *ovf, *ovf_count, *ovf2, *ovf2_count;
+  if (!overflow_lists(ctx, n, ovf, ovf_count, ovf2, ovf2_count)) return GPDB_ERR_CUDA;
   float4 *glist = (float4 *)gpdb_scratch(ctx, SCR_HANDS_GL, sizeof(float4) * (size_t)HANDS_CAP3 * ctx->sm_count);
-  if (!ovf || !glist) return GPDB_ERR_CUDA;
-  int *ovf_count = ovf + n, *ovf2 = ovf + n + 1, *ovf2_count = ovf2 + n;
+  if (!glist) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
   const DevCloud &cl = s.view;
@@ -2879,9 +2876,9 @@ int geo_compact(gpdb_ctx *ctx, const gpdb_pose *d_poses, const uint8_t *d_flags,
     CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int), ctx->stream));
     return GPDB_OK;
   }
-  int *f01 = (int *)gpdb_scratch(ctx, SCR_KEYS, sizeof(int) * (size_t)n_poses * 2);
-  if (!f01) return GPDB_ERR_CUDA;
-  int *pos = f01 + n_poses;
+  int *f01, *pos;
+  if (!gpdb_carve(ctx, SCR_KEYS, [&](Carve &c) { f01 = c.take<int>(n_poses); pos = c.take<int>(n_poses); }))
+    return GPDB_ERR_CUDA;
   const int tb = 256, gb = (n_poses + tb - 1) / tb;
   k_flag01<<<gb, tb, 0, ctx->stream>>>(d_flags, n_poses, f01);
   LAUNCH_CHECK();
@@ -2947,9 +2944,9 @@ static int launch_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_ca
   const bool fast = S == 60 && (hp.C != 15 || (K <= 2 && bm + 2048 <= (size_t)BOX_CAP2 * 36)) && !(force && force[0] == '1');
   const int *d_work = nullptr, *d_work_n = nullptr;
   if (fast) {
-    int *ovf = (int *)gpdb_scratch(ctx, SCR_IMG_OVF, sizeof(int) * ((size_t)nc + 1));  // not SCR_OVF: the hand search of
-    if (!ovf) return GPDB_ERR_CUDA;                                                    // the next chunk may be writing it
-    int *ovf_count = ovf + nc;
+    int *ovf, *ovf_count;  // not SCR_OVF: the hand search of the next chunk may be writing it
+    if (!gpdb_carve(ctx, SCR_IMG_OVF, [&](Carve &c) { ovf = c.take<int>(nc); ovf_count = c.take<int>(1); }))
+      return GPDB_ERR_CUDA;
     CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
     const size_t smem2 = IMG2_DYN_SMEM;
     CUDA_TRY(cudaFuncSetAttribute(k_images2<BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
@@ -2961,12 +2958,13 @@ static int launch_images(gpdb_ctx *ctx, const CloudSet &s, const gpdb_pose *d_ca
   }
   // general tier (2 048-point box list in shared memory): everything, or the overflow list of the fast path; its own
   // overflow goes to a second list ...
-  int *ovf2 = (int *)gpdb_scratch(ctx, SCR_IMG_OVF2, sizeof(int) * ((size_t)nc + 1));
+  int *ovf2, *ovf2_count;
+  if (!gpdb_carve(ctx, SCR_IMG_OVF2, [&](Carve &c) { ovf2 = c.take<int>(nc); ovf2_count = c.take<int>(1); }))
+    return GPDB_ERR_CUDA;
   const int gl_cap = 32768;
   const size_t gl_slice = (size_t)gl_cap * 36 + (size_t)16 * S * S;
   unsigned char *gl = (unsigned char *)gpdb_scratch(ctx, SCR_IMG_GL, gl_slice * (size_t)ctx->sm_count);
-  if (!ovf2 || !gl) return GPDB_ERR_CUDA;
-  int *ovf2_count = ovf2 + nc;
+  if (!gl) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemsetAsync(ovf2_count, 0, sizeof(int), ctx->stream));
   const int grid = fast ? ctx->sm_count : std::min(nc, ctx->sm_count * 64);
   const int err = S == 60 ? launch_general<60, BATCH>(ctx, s, d_cand, nc, d_p16, smem, plane_bytes, list_bytes, grid, d_work,
@@ -3021,10 +3019,12 @@ int geo_clusters(gpdb_ctx *ctx, const gpdb_pose *d_hands, int n, const int *d_go
 
 int geo_select(gpdb_ctx *ctx, const gpdb_pose *d_cand, int n, int k, gpdb_pose *d_out) {
   if (n <= 0 || k <= 0) return GPDB_OK;
-  unsigned *keys = (unsigned *)gpdb_scratch(ctx, SCR_KEYS, sizeof(unsigned) * (size_t)n * 4);
-  if (!keys) return GPDB_ERR_CUDA;
-  unsigned *keys2 = keys + n;
-  int *vals = (int *)(keys2 + n), *vals2 = vals + n;
+  unsigned *keys, *keys2;
+  int *vals, *vals2;
+  if (!gpdb_carve(ctx, SCR_KEYS, [&](Carve &c) {
+        keys = c.take<unsigned>(n); keys2 = c.take<unsigned>(n); vals = c.take<int>(n); vals2 = c.take<int>(n);
+      }))
+    return GPDB_ERR_CUDA;
   k_select_keys<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, keys, vals);
   LAUNCH_CHECK();
   size_t tmp_bytes = 0;
@@ -3050,11 +3050,13 @@ int geo_scatter_scores(gpdb_ctx *ctx, const gpdb_pose *d_cand, const float *d_sc
 // cell bases on the device, one sort over (cloud, cell) for all clouds.
 int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
   const int B = s.n, N = s.points();
-  long long *ncell =
-      (long long *)gpdb_scratch(ctx, SCR_WORK_B, sizeof(long long) * 2 * ((size_t)B + 1) + sizeof(int) * (7 * (size_t)B + 1));
-  if (!ncell) return GPDB_ERR_CUDA;
-  long long *base = ncell + B + 1;
-  int *d_off = (int *)(base + B + 1), *bounds = d_off + B + 1;
+  long long *ncell, *base;  // cells per cloud and their scan
+  int *d_off, *bounds;
+  if (!gpdb_carve(ctx, SCR_WORK_B, [&](Carve &c) {
+        ncell = c.take<long long>((size_t)B + 1); base = c.take<long long>((size_t)B + 1);
+        d_off = c.take<int>((size_t)B + 1); bounds = c.take<int>(6 * (size_t)B);
+      }))
+    return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(d_off, s.off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   int largest = 0;
   for (int b = 0; b < B; b++) largest = std::max(largest, s.off[b + 1] - s.off[b]);
@@ -3088,9 +3090,11 @@ int geo_build_grid_batch(gpdb_ctx *ctx, CloudSet &s) {
     s.cell_cap = ncells + 1 + ncells / 4;
   }
   CUDA_TRY(cudaMemsetAsync(s.cell_start, 0, sizeof(int) * (ncells + 1), ctx->stream));
-  int *cid = (int *)gpdb_scratch(ctx, SCR_P16, sizeof(int) * (size_t)N * 4);
-  if (!cid) return GPDB_ERR_CUDA;
-  int *idx = cid + N, *cid2 = idx + N, *idx2 = cid2 + N;
+  int *cid, *idx, *cid2, *idx2;
+  if (!gpdb_carve(ctx, SCR_P16, [&](Carve &c) {
+        cid = c.take<int>(N); idx = c.take<int>(N); cid2 = c.take<int>(N); idx2 = c.take<int>(N);
+      }))
+    return GPDB_ERR_CUDA;
   const int tb = 256, gb = (N + tb - 1) / tb;
   size_t tmp2 = 0;
   tmp_bytes = 0;
@@ -3121,11 +3125,14 @@ int geo_select_batch(gpdb_ctx *ctx, CloudSet &s, const gpdb_pose *d_cand, int n,
   const int B = s.n;
   int *sel_off = s.sel;
   *d_out = nullptr;
-  unsigned long long *keys = (unsigned long long *)gpdb_scratch(
-      ctx, SCR_KEYS, sizeof(unsigned long long) * 2 * (size_t)n + sizeof(int) * (3 * (size_t)n + 2 * ((size_t)B + 1)));
-  if (!keys) return GPDB_ERR_CUDA;
-  unsigned long long *keys2 = keys + n;
-  int *vals = (int *)(keys2 + n), *vals2 = vals + n, *order = vals2 + n, *cand_off = order + n, *d_sel_off = cand_off + B + 1;
+  unsigned long long *keys, *keys2;
+  int *vals, *vals2, *order, *cand_off, *d_sel_off;
+  if (!gpdb_carve(ctx, SCR_KEYS, [&](Carve &c) {
+        keys = c.take<unsigned long long>(n); keys2 = c.take<unsigned long long>(n); vals = c.take<int>(n);
+        vals2 = c.take<int>(n); order = c.take<int>(n); cand_off = c.take<int>((size_t)B + 1);
+        d_sel_off = c.take<int>((size_t)B + 1);
+      }))
+    return GPDB_ERR_CUDA;
   k_batch_cand_off<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(d_cand, n, s.soff, B, cand_off);
   LAUNCH_CHECK();
   std::vector<int> coff((size_t)B + 1);

@@ -237,16 +237,6 @@ __global__ void k_ip2(const float *__restrict__ H, int n, const float *__restric
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 // Upload the reference's .bin layout (conv OIHW row-major, ip column-major (out,in)) and re-lay the conv
 // filters as [c][kh][kw][o] for the kernels above. ip1/ip2 are used as stored: W(o,k) at o + OUT*k.
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]) {

@@ -421,16 +421,6 @@ __global__ void __launch_bounds__(IP_NT, 1) k_ip1_tc(const __half *__restrict__ 
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 static float pow2_scale(float maxabs, float target) {
   if (!(maxabs > 0.0f)) return 1.0f;
   const float q = target / maxabs;

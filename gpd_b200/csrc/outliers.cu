@@ -13,7 +13,6 @@
 // store is left without a cloud, as a failed install leaves it. Compiled with -fmad=false: every operation of the
 // specification is rounded on its own.
 #include <cmath>
-#include <cub/cub.cuh>
 #include <vector>
 
 #include "../../include/gpd_b200_outliers.h"
@@ -47,8 +46,7 @@ __global__ void __launch_bounds__(TB) k_outlier_mean(const CloudDesc *d, int B, 
   dist[g] = gpdb_outlier_mean(s, mean_k);
 }
 
-// rules 3 and 5 for cloud b = blockIdx.x: stats[3b ..] = mean, stddev, threshold. Thread 0 adds chunk c from shared memory
-// while warps 1.. stage chunk c + 1, so the two chains wait on shared loads only.
+// rules 3 and 5 for cloud b = blockIdx.x: stats[3b ..] = mean, stddev, threshold
 __global__ void __launch_bounds__(STATS_THREADS) k_outlier_stats(const CloudDesc *d, const float *dist, int mean_k,
                                                                  double stddev_mul, double *stats) {
   __shared__ __align__(16) float s_d[2][STATS_CHUNK];
@@ -58,32 +56,9 @@ __global__ void __launch_bounds__(STATS_THREADS) k_outlier_stats(const CloudDesc
     if (threadIdx.x == 0) gpdb_outlier_stats(0.0, 0.0, n, mean_k, stddev_mul, stats + 3 * (size_t)b);
     return;
   }
-  const float *e = dist + d[b].off;
-  const int nc = (n + STATS_CHUNK - 1) / STATS_CHUNK;
-  for (int j = threadIdx.x; j < min(n, STATS_CHUNK); j += STATS_THREADS) s_d[0][j] = __ldg(e + j);
-  __syncthreads();
   double sum = 0.0, sq = 0.0;
-  for (int c = 0; c < nc; c++) {
-    const int base = c * STATS_CHUNK;
-    if (threadIdx.x == 0) {
-      const float *p = s_d[c & 1];
-      const int len = min(STATS_CHUNK, n - base);
-      int j = 0;
-#pragma unroll 2
-      for (; j + 4 <= len; j += 4) {
-        const float4 v = *reinterpret_cast<const float4 *>(p + j);
-        gpdb_outlier_stats_add(&sum, &sq, v.x);
-        gpdb_outlier_stats_add(&sum, &sq, v.y);
-        gpdb_outlier_stats_add(&sum, &sq, v.z);
-        gpdb_outlier_stats_add(&sum, &sq, v.w);
-      }
-      for (; j < len; j++) gpdb_outlier_stats_add(&sum, &sq, p[j]);
-    } else if (threadIdx.x >= 32 && c + 1 < nc) {
-      const int nb = base + STATS_CHUNK, nl = min(STATS_CHUNK, n - nb);
-      for (int j = threadIdx.x - 32; j < nl; j += STATS_THREADS - 32) s_d[(c + 1) & 1][j] = __ldg(e + nb + j);
-    }
-    __syncthreads();
-  }
+  ordered_fold<STATS_THREADS, STATS_CHUNK>(dist + d[b].off, n, s_d,
+                                           [&](float v) { gpdb_outlier_stats_add(&sum, &sq, v); });
   if (threadIdx.x == 0) gpdb_outlier_stats(sum, sq, n, mean_k, stddev_mul, stats + 3 * (size_t)b);
 }
 
@@ -131,86 +106,49 @@ __global__ void __launch_bounds__(TB) k_outlier_gather(int N, const int *flag, c
   src2[j] = src[g];
 }
 
-}  // namespace
-
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
-namespace {
-
-// SCR_OUTLIERS, in this order (8-byte blocks first): stats double[3B], gathered normals double[3N], gathered xyz
-// float[3N], mean distances float[N], flags and scan int[N+1] each, gathered src int[N], counts and camera flags int[B]
-// each, keep bytes [N], gathered camera masks [N]. The lists are SCR_NBR, shared with the normal refinement.
-struct OutlierScratch {
-  double *stats, *nrm2;
-  float *xyz2, *dist;
-  int *nbr, *flag, *pos, *src2, *cnt, *partial;
-  uint8_t *kept, *cam2;
-};
-
-int outlier_scratch(gpdb_ctx *ctx, size_t N, int B, int k, OutlierScratch &w) {
-  const size_t bytes = sizeof(double) * (3 * (size_t)B + 3 * N) + sizeof(float) * 4 * N +
-                       sizeof(int) * (2 * (N + 1) + N + 2 * (size_t)B) + 2 * N;
-  unsigned char *p = (unsigned char *)gpdb_scratch(ctx, SCR_OUTLIERS, bytes);
-  w.nbr = (int *)gpdb_scratch(ctx, SCR_NBR, sizeof(int) * N * k);
-  if (!p || !w.nbr) return GPDB_ERR_CUDA;
-  w.stats = (double *)p;
-  w.nrm2 = w.stats + 3 * (size_t)B;
-  w.xyz2 = (float *)(w.nrm2 + 3 * N);
-  w.dist = w.xyz2 + 3 * N;
-  w.flag = (int *)(w.dist + N);
-  w.pos = w.flag + N + 1;
-  w.src2 = w.pos + N + 1;
-  w.cnt = w.src2 + N;
-  w.partial = w.cnt + B;
-  w.kept = (uint8_t *)(w.partial + B);
-  w.cam2 = w.kept + N;
-  return GPDB_OK;
-}
-
 // outliers_remove_batch up to its result; an error may come after the store has been partly rewritten
 int remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int *off, double *stats, uint8_t *kept) {
   const int B = s.n, N = s.points(), k = mean_k + 1;
-  OutlierScratch w;
-  int rc = outlier_scratch(ctx, (size_t)N, B, k, w);
-  if (rc != GPDB_OK) return rc;
+  const size_t n = (size_t)N;
+  double *d_stats, *nrm2;
+  float *xyz2, *dist;
+  int *flag, *pos, *src2, *d_cnt;
+  uint8_t *d_kept, *cam2;
+  // xyz2 / nrm2 / src2 / cam2: the kept points, gathered
+  if (!gpdb_carve(ctx, SCR_OUTLIERS, [&](Carve &c) {
+        d_stats = c.take<double>(3 * (size_t)B); nrm2 = c.take<double>(3 * n); xyz2 = c.take<float>(3 * n);
+        dist = c.take<float>(n); flag = c.take<int>(n + 1); pos = c.take<int>(n + 1); src2 = c.take<int>(n);
+        d_cnt = c.take<int>(2 * (size_t)B);  // kept counts [B], then the camera flags [B]: one memset, one read-back
+        d_kept = c.take<uint8_t>(n); cam2 = c.take<uint8_t>(n);
+      }))
+    return GPDB_ERR_CUDA;
+  int *partial = d_cnt + B;
+  int *nbr = (int *)gpdb_scratch(ctx, SCR_NBR, sizeof(int) * n * k);  // shared with the normal refinement
+  if (!nbr) return GPDB_ERR_CUDA;
+  int rc;
   // the camera fields of the descriptors, for the reinstall; read back with the counts
   std::vector<CloudDesc> desc((size_t)B);
   std::vector<int> cnt(2 * (size_t)B);  // counts, then the camera flags
   CUDA_TRY(cudaMemcpyAsync(desc.data(), s.desc, sizeof(CloudDesc) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaMemsetAsync(w.cnt, 0, sizeof(int) * 2 * (size_t)B, ctx->stream));
+  CUDA_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(int) * 2 * (size_t)B, ctx->stream));
   const int nb = (N + TB - 1) / TB;
-  if ((rc = refine_knn_lists(ctx, s, k, w.nbr)) != GPDB_OK) return rc;
+  if ((rc = refine_knn_lists(ctx, s, k, nbr)) != GPDB_OK) return rc;
   if (N > 0) {
-    k_outlier_mean<<<nb, TB, 0, ctx->stream>>>(s.desc, B, N, s.xyz, w.nbr, mean_k, w.dist);
+    k_outlier_mean<<<nb, TB, 0, ctx->stream>>>(s.desc, B, N, s.xyz, nbr, mean_k, dist);
     LAUNCH_CHECK();
   }
-  k_outlier_stats<<<B, STATS_THREADS, 0, ctx->stream>>>(s.desc, w.dist, mean_k, stddev_mul, w.stats);
+  k_outlier_stats<<<B, STATS_THREADS, 0, ctx->stream>>>(s.desc, dist, mean_k, stddev_mul, d_stats);
   LAUNCH_CHECK();
   if (N > 0) {
-    k_outlier_mark<<<nb, TB, 0, ctx->stream>>>(s.desc, B, N, w.dist, w.stats, s.cam, w.flag, w.kept, w.cnt, w.partial);
+    k_outlier_mark<<<nb, TB, 0, ctx->stream>>>(s.desc, B, N, dist, d_stats, s.cam, flag, d_kept, d_cnt, partial);
     LAUNCH_CHECK();
-    CUDA_TRY(cudaMemsetAsync(w.flag + N, 0, sizeof(int), ctx->stream));
-    size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, w.flag, w.pos, N + 1, ctx->stream);
-    void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
-    if (!tmp) return GPDB_ERR_CUDA;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, w.flag, w.pos, N + 1, ctx->stream));
-    ctx->launches += 2;
-    k_outlier_gather<<<nb, TB, 0, ctx->stream>>>(N, w.flag, w.pos, s.xyz, s.nrm, s.cam, s.src, w.xyz2, w.nrm2, w.cam2,
-                                                 w.src2);
+    if ((rc = scan_flags(ctx, flag, pos, N)) != GPDB_OK) return rc;
+    k_outlier_gather<<<nb, TB, 0, ctx->stream>>>(N, flag, pos, s.xyz, s.nrm, s.cam, s.src, xyz2, nrm2, cam2, src2);
     LAUNCH_CHECK();
   }
-  CUDA_TRY(cudaMemcpyAsync(cnt.data(), w.cnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  if (stats) CUDA_TRY(cudaMemcpyAsync(stats, w.stats, sizeof(double) * 3 * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  if (kept && N > 0) CUDA_TRY(cudaMemcpyAsync(kept, w.kept, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int) * 2 * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  if (stats) CUDA_TRY(cudaMemcpyAsync(stats, d_stats, sizeof(double) * 3 * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
+  if (kept && N > 0) CUDA_TRY(cudaMemcpyAsync(kept, d_kept, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   off[0] = 0;
   for (int b = 0; b < B; b++) {
@@ -219,10 +157,10 @@ int remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int 
   }
   const size_t n2 = (size_t)off[B];
   const bool has_src = s.has_src;
-  CUDA_TRY(cudaMemcpyAsync(s.xyz, w.xyz2, sizeof(float) * 3 * n2, cudaMemcpyDeviceToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.nrm, w.nrm2, sizeof(double) * 3 * n2, cudaMemcpyDeviceToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.cam, w.cam2, n2, cudaMemcpyDeviceToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.src, w.src2, sizeof(int) * n2, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.xyz, xyz2, sizeof(float) * 3 * n2, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.nrm, nrm2, sizeof(double) * 3 * n2, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.cam, cam2, n2, cudaMemcpyDeviceToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.src, src2, sizeof(int) * n2, cudaMemcpyDeviceToDevice, ctx->stream));
   if ((rc = gpdb_install_clouds(ctx, s, desc.data(), off, B, true)) != GPDB_OK) return rc;
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   s.has_src = has_src;  // the raw offsets stay: src still indexes each cloud's raw points

@@ -250,16 +250,6 @@ __global__ void __launch_bounds__(256) k_plane_mark(const float *xyz, const int 
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_params &pp, float *planes, int *n_inliers,
                         int *n_hyp, uint8_t *d_eligible) {
   const int B = s.n, N = s.points(), H = pp.max_iterations + 1;
@@ -268,13 +258,15 @@ int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_param
   if ((double)tf >= pp.distance_threshold) tf = nextafterf(tf, -INFINITY);
   int largest = 0;
   for (int b = 0; b < B; b++) largest = std::max(largest, s.off[b + 1] - s.off[b]);
-  // SCR_PLANE: hypotheses float4[B*H], planes float4[B], counts int[B*H], offsets int[B+1], nh int[B], pick int[2B],
-  // final counts int[B]
   const size_t BH = (size_t)B * H;
-  float4 *hyp = (float4 *)gpdb_scratch(ctx, SCR_PLANE, sizeof(float4) * (BH + B) + sizeof(int) * (BH + 5 * (size_t)B + 1));
-  if (!hyp) return GPDB_ERR_CUDA;
-  float4 *d_planes = hyp + BH;
-  int *cnt = (int *)(d_planes + B), *d_off = cnt + BH, *nh = d_off + B + 1, *pick = nh + B, *fin = pick + 2 * B;
+  float4 *hyp, *d_planes;
+  int *cnt, *d_off, *nh, *pick, *fin;
+  if (!gpdb_carve(ctx, SCR_PLANE, [&](Carve &c) {
+        hyp = c.take<float4>(BH); d_planes = c.take<float4>(B); cnt = c.take<int>(BH);
+        d_off = c.take<int>((size_t)B + 1); nh = c.take<int>(B); pick = c.take<int>(2 * (size_t)B);
+        fin = c.take<int>(B);
+      }))
+    return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemcpyAsync(d_off, s.off, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   std::vector<int> h_nh((size_t)B, H);
   CUDA_TRY(cudaMemcpyAsync(nh, h_nh.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));

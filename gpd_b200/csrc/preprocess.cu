@@ -447,16 +447,6 @@ __global__ void k_bnonunit(const double *nrm, CloudDesc *d, int B, int N) {
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 // Normal estimation over the N points of store s (grids built): writes s.nrm.
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius) {
   const int N = s.points();
@@ -464,9 +454,9 @@ int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius) {
   const CloudTable tab = s.table();
   const float r2 = (float)(radius * radius);
   const float rf = (float)radius * 1.0001f + 1e-6f;
-  int *ovf = (int *)gpdb_scratch(ctx, SCR_OVF, sizeof(int) * ((size_t)N + 1));
-  if (!ovf) return GPDB_ERR_CUDA;
-  int *ovf_count = ovf + N;
+  int *ovf, *ovf_count;
+  if (!gpdb_carve(ctx, SCR_OVF, [&](Carve &c) { ovf = c.take<int>(N); ovf_count = c.take<int>(1); }))
+    return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemsetAsync(ovf_count, 0, sizeof(int), ctx->stream));
   const size_t sm1 = (size_t)NRM_WARPS * NRM_CAP1 * NRM_BYTES_PER, sm2 = (size_t)NRM_CAP2 * NRM_BYTES_PER;
   CUDA_TRY(cudaFuncSetAttribute(k_normals<NRM_WARPS, NRM_NB1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
@@ -508,21 +498,30 @@ int pre_bounds_batch(gpdb_ctx *ctx, const float *xyz, const int *d_off, int B, i
   return GPDB_OK;
 }
 
-// The header of a preprocessing call in SCR_WORK_A: workspace [6 doubles], raw / filtered / processed offsets [B+1 each],
-// bounds [6B], voxel error [2], then `extra` bytes for the caller (h.extra, 8-byte aligned). Uploads the workspace, the
-// raw offsets and the voxel error words.
+// The header of a preprocessing call in SCR_WORK_A, then `extra` bytes for the caller (h.extra, 8-byte aligned).
+// Uploads the workspace, the raw offsets and the voxel error words.
 int pre_batch_header(gpdb_ctx *ctx, int B, const int *roff, const gpdb_preprocess_params &pp, size_t extra, PreBatch &h) {
-  const size_t head = sizeof(double) * 6 + sizeof(int) * (3 * ((size_t)B + 1) + 6 * (size_t)B + 2);
-  const size_t head8 = (head + 7) / 8 * 8;
-  h.ws = (double *)gpdb_scratch(ctx, SCR_WORK_A, head8 + extra);
-  if (!h.ws) return GPDB_ERR_CUDA;
-  h.roff = (int *)(h.ws + 6), h.foff = h.roff + B + 1, h.poff = h.foff + B + 1, h.bounds = h.poff + B + 1;
-  h.verr = h.bounds + 6 * B;
-  h.extra = (unsigned char *)h.ws + head8;
+  if (!gpdb_carve(ctx, SCR_WORK_A, [&](Carve &c) {
+        h.ws = c.take<double>(6); h.roff = c.take<int>((size_t)B + 1); h.foff = c.take<int>((size_t)B + 1);
+        h.poff = c.take<int>((size_t)B + 1); h.bounds = c.take<int>(6 * (size_t)B); h.verr = c.take<int>(2);
+        h.extra = c.take<unsigned char>(extra, 8);
+      }))
+    return GPDB_ERR_CUDA;
   const int verr0[2] = {0, INT_MAX};
   CUDA_TRY(cudaMemcpyAsync(h.ws, pp.workspace, sizeof(double) * 6, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(h.roff, roff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(h.verr, verr0, sizeof(verr0), cudaMemcpyHostToDevice, ctx->stream));
+  return GPDB_OK;
+}
+
+int scan_flags(gpdb_ctx *ctx, int *flag, int *pos, int n) {
+  CUDA_TRY(cudaMemsetAsync(flag + n, 0, sizeof(int), ctx->stream));
+  size_t tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, n + 1, ctx->stream);
+  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
+  if (!tmp) return GPDB_ERR_CUDA;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, n + 1, ctx->stream));
+  ctx->launches += 2;
   return GPDB_OK;
 }
 
@@ -547,19 +546,16 @@ int pre_filter_voxelize_batch(gpdb_ctx *ctx, CloudSet &s, const float *d_xyz_raw
   PreBatch h;
   int rc = pre_batch_header(ctx, B, roff, pp, 0, h);
   if (rc != GPDB_OK) return rc;
-  int *flag = (int *)gpdb_scratch(ctx, SCR_WORK_B, sizeof(int) * (3 * (size_t)M + 2) + sizeof(float) * 3 * (size_t)M);
-  if (!flag) return GPDB_ERR_CUDA;
-  int *pos = flag + M + 1, *keep = pos + M + 1;
-  float *xyz1 = (float *)(keep + M);
+  int *flag, *pos, *keep;
+  float *xyz1;
+  if (!gpdb_carve(ctx, SCR_WORK_B, [&](Carve &c) {
+        flag = c.take<int>((size_t)M + 1); pos = c.take<int>((size_t)M + 1); keep = c.take<int>(M);
+        xyz1 = c.take<float>(3 * (size_t)M);
+      }))
+    return GPDB_ERR_CUDA;
   k_pre_flag<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, M, h.ws, flag);
   LAUNCH_CHECK();
-  CUDA_TRY(cudaMemsetAsync(flag + M, 0, sizeof(int), ctx->stream));  // pos[M] = number of filtered points
-  size_t tmp_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flag, pos, M + 1, ctx->stream);
-  void *tmp = gpdb_scratch(ctx, SCR_CUB, tmp_bytes);
-  if (!tmp) return GPDB_ERR_CUDA;
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, pos, M + 1, ctx->stream));
-  ctx->launches += 2;
+  if ((rc = scan_flags(ctx, flag, pos, M)) != GPDB_OK) return rc;  // pos[M] = number of filtered points
   k_pre_compact<<<(M + tb - 1) / tb, tb, 0, ctx->stream>>>(d_xyz_raw, flag, pos, M, keep, xyz1);
   LAUNCH_CHECK();
   if ((rc = pre_filter_offsets(ctx, pos, h, B)) != GPDB_OK) return rc;
@@ -596,15 +592,19 @@ int pre_voxelize_back(gpdb_ctx *ctx, CloudSet &s, const PreBatch &h, const int *
   for (int b = 0; b < B; b++) largest = std::max(largest, foff[b + 1] - foff[b]);
   int rc = pre_bounds_batch(ctx, xyz1, d_foff, B, largest, d_bounds);
   if (rc != GPDB_OK) return rc;
-  // sort buffers: keys x2 (8 B), vals x3, cloud of point, cloud keys x2, head, gid, gfirst, gbegin, group order vals x2
-  // (4 B each), group order keys x2 (8 B)
-  unsigned long long *keys = (unsigned long long *)gpdb_scratch(ctx, SCR_WORK_C, (size_t)M1 * (16 + 48 + 16));
-  if (!keys) return GPDB_ERR_CUDA;
-  unsigned long long *keys2 = keys + M1, *gord_k = keys2 + M1, *gord_k2 = gord_k + M1;
-  int *vals = (int *)(gord_k2 + M1), *vals2 = vals + M1, *vals3 = vals2 + M1, *cl_of = vals3 + M1;
-  unsigned *ck = (unsigned *)(cl_of + M1), *ck2 = ck + M1;
-  int *head = (int *)(ck2 + M1), *gid = head + M1, *gfirst = gid + M1, *gbegin = gfirst + M1, *gord_v = gbegin + M1;
-  int *gord_v2 = gord_v + M1;
+  // sort buffers: voxel keys and point indices, cloud keys, group heads / ids / first points / begins, group order
+  unsigned long long *keys, *keys2, *gord_k, *gord_k2;
+  int *vals, *vals2, *vals3, *cl_of, *head, *gid, *gfirst, *gbegin, *gord_v, *gord_v2;
+  unsigned *ck, *ck2;
+  if (!gpdb_carve(ctx, SCR_WORK_C, [&](Carve &c) {
+        const size_t m = (size_t)M1;
+        keys = c.take<unsigned long long>(m); keys2 = c.take<unsigned long long>(m);
+        gord_k = c.take<unsigned long long>(m); gord_k2 = c.take<unsigned long long>(m); vals = c.take<int>(m);
+        vals2 = c.take<int>(m); vals3 = c.take<int>(m); cl_of = c.take<int>(m); ck = c.take<unsigned>(m);
+        ck2 = c.take<unsigned>(m); head = c.take<int>(m); gid = c.take<int>(m); gfirst = c.take<int>(m);
+        gbegin = c.take<int>(m); gord_v = c.take<int>(m); gord_v2 = c.take<int>(m);
+      }))
+    return GPDB_ERR_CUDA;
   int cloud_bits = 0;
   while ((1 << cloud_bits) < B) cloud_bits++;
   k_bvox_keys<<<(M1 + tb - 1) / tb, tb, 0, ctx->stream>>>(xyz1, M1, d_foff, B, d_bounds, cell, keys, vals, cl_of, d_verr);

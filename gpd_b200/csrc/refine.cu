@@ -5,9 +5,9 @@
 //   k_refine_cast    the float32 input normals (rule 2)
 //   k_refine_iter    one thread per point of a cloud still iterating: the ordered neighbour sums, the refined normal and
 //                    its error (rules 3 and 4)
-//   k_refine_stop    one CTA per cloud still iterating: the sequential float32 mean of rule 4 (one thread adds, the
-//                    others stage the errors in shared memory), the iteration count and the cloud's done flag, so that
-//                    a batch runs its 15 iterations without reading back to the host
+//   k_refine_stop    one CTA per cloud still iterating: the sequential float32 mean of rule 4 (ordered_fold), the
+//                    iteration count and the cloud's done flag, so that a batch runs its 15 iterations without reading
+//                    back to the host
 //   k_refine_commit  the last iterate of every cloud, cast to double, into the store (rule 5)
 // The lists are N x k int32; the iterates ping-pong between two float4 arrays: iteration t reads buf[(t - 1) & 1] and
 // writes buf[t & 1], so a cloud done after m iterations holds its result in buf[m & 1]. Nothing in the store changes
@@ -197,7 +197,6 @@ __global__ void __launch_bounds__(256) k_refine_iter(const CloudDesc *d, int B, 
 
 // rule 4 after iteration t for cloud b = blockIdx.x, unless it is done: the float32 sum of its errors in index order (one
 // sequential chain, as std::accumulate), the mean, the count, the flag. A cloud without points is done at once (0).
-// Thread 0 adds chunk c from shared memory while warps 1.. stage chunk c + 1, so the chain waits on shared loads only.
 __global__ void __launch_bounds__(STOP_THREADS) k_refine_stop(const CloudDesc *d, const float *err, int t, int *done,
                                                               int *iters) {
   __shared__ __align__(16) float s_e[2][STOP_CHUNK];
@@ -208,32 +207,8 @@ __global__ void __launch_bounds__(STOP_THREADS) k_refine_stop(const CloudDesc *d
     if (threadIdx.x == 0) done[b] = 1;
     return;
   }
-  const float *e = err + d[b].off;
-  const int nc = (n + STOP_CHUNK - 1) / STOP_CHUNK;
-  for (int j = threadIdx.x; j < min(n, STOP_CHUNK); j += STOP_THREADS) s_e[0][j] = __ldg(e + j);
-  __syncthreads();
   float s = 0.0f;
-  for (int c = 0; c < nc; c++) {
-    const int base = c * STOP_CHUNK;
-    if (threadIdx.x == 0) {
-      const float *p = s_e[c & 1];
-      const int len = min(STOP_CHUNK, n - base);
-      int j = 0;
-#pragma unroll 4
-      for (; j + 4 <= len; j += 4) {
-        const float4 v = *reinterpret_cast<const float4 *>(p + j);
-        s = s + v.x;
-        s = s + v.y;
-        s = s + v.z;
-        s = s + v.w;
-      }
-      for (; j < len; j++) s = s + p[j];
-    } else if (threadIdx.x >= 32 && c + 1 < nc) {
-      const int nb = base + STOP_CHUNK, nl = min(STOP_CHUNK, n - nb);
-      for (int j = threadIdx.x - 32; j < nl; j += STOP_THREADS - 32) s_e[(c + 1) & 1][j] = __ldg(e + nb + j);
-    }
-    __syncthreads();
-  }
+  ordered_fold<STOP_THREADS, STOP_CHUNK>(err + d[b].off, n, s_e, [&](float v) { s = s + v; });
   if (threadIdx.x == 0) {
     iters[b] = t;
     if (s / (float)n < GPDB_REFINE_CONVERGENCE || t >= GPDB_REFINE_MAX_ITERATIONS) done[b] = 1;
@@ -253,16 +228,6 @@ __global__ void k_refine_commit(const CloudDesc *d, int B, int N, const int *ite
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                   \
-  do {                                                   \
-    ctx->launches++;                                     \
-    cudaError_t e__ = cudaGetLastError();                \
-    if (e__ != cudaSuccess) {                            \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                              \
-    }                                                    \
-  } while (0)
-
 int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr) {
   const int N = s.points();
   if (N > 0) {
@@ -274,14 +239,18 @@ int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr) {
 
 int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
   const int B = s.n, N = s.points();
-  // SCR_REFINE: iterates float4[2N], errors float[N], done int[B], counts int[B]; SCR_NBR: lists int[N*k]
   const size_t n = (size_t)N;
-  float4 *buf0 = (float4 *)gpdb_scratch(ctx, SCR_REFINE, sizeof(float4) * 2 * n + sizeof(float) * n + sizeof(int) * 2 * (size_t)B);
+  float4 *buf0, *buf1;
+  float *err;
+  int *done;
+  if (!gpdb_carve(ctx, SCR_REFINE, [&](Carve &c) {
+        buf0 = c.take<float4>(n); buf1 = c.take<float4>(n); err = c.take<float>(n);
+        done = c.take<int>(2 * (size_t)B);  // done flags [B], then iteration counts [B]: one memset
+      }))
+    return GPDB_ERR_CUDA;
+  int *d_iters = done + B;
   int *nbr = (int *)gpdb_scratch(ctx, SCR_NBR, sizeof(int) * n * k);
-  if (!buf0 || !nbr) return GPDB_ERR_CUDA;
-  float4 *buf1 = buf0 + n;
-  float *err = (float *)(buf1 + n);
-  int *done = (int *)(err + n), *d_iters = done + B;
+  if (!nbr) return GPDB_ERR_CUDA;
   CUDA_TRY(cudaMemsetAsync(done, 0, sizeof(int) * 2 * (size_t)B, ctx->stream));
   const int tb = 256, nb = (N + tb - 1) / tb;
   const int rc0 = refine_knn_lists(ctx, s, k, nbr);

@@ -131,16 +131,6 @@ __global__ void k_sis_filter(gpdb_pose *rec, int n, const int *soff, int B, doub
 
 }  // namespace
 
-#define LAUNCH_CHECK()                                                                                    \
-  do {                                                                                                    \
-    ctx->launches++;                                                                                      \
-    cudaError_t e__ = cudaGetLastError();                                                                 \
-    if (e__ != cudaSuccess) {                                                                             \
-      gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s:%d launch -> %s", __FILE__, __LINE__, cudaGetErrorString(e__)); \
-      return GPDB_ERR_CUDA;                                                                               \
-    }                                                                                                     \
-  } while (0)
-
 int sis_draw(gpdb_ctx *ctx, const SisDraw &q, int B, const CloudSet &s, const int *d_init_off, const int *d_init_idx,
              const double *d_kept, const int *d_kcount, int stage_cap, double *d_eval, int *d_ecount) {
   if (B == 0) return GPDB_OK;
