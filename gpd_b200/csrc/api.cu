@@ -525,67 +525,6 @@ int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *
   return rc;
 }
 
-// one cloud's camera masks: bit k of dst[i] set when seen(row i, entry k); returns the AND of the masks
-template <class Seen>
-static unsigned pack_rows(const int32_t *rows, int nb, int K, uint8_t *dst, Seen seen) {
-  unsigned seen_by_all = ~0u;
-  for (int i = 0; i < nb; i++) {
-    const int32_t *row = rows + (size_t)i * K;
-    unsigned m = 0;
-    for (int k = 0; k < K; k++) m |= (unsigned)seen(row[k]) << k;
-    dst[i] = (uint8_t)m;
-    seen_by_all &= m;
-  }
-  return seen_by_all;
-}
-
-// the camera fields of B descriptors: K_b and the 3 x K_b view point blocks, one after the other; the rest zeroed
-static void camera_descs(int B, const int32_t *n_cameras, const double *view_points, CloudDesc *desc) {
-  size_t vs = 0;  // running offset into view_points
-  for (int b = 0; b < B; b++) {
-    CloudDesc &D = desc[b];
-    memset(&D, 0, sizeof(D));
-    D.K = n_cameras[b];
-    for (int k = 0; k < D.K; k++)
-      for (int r = 0; r < 3; r++) D.vp[k][r] = view_points[vs + 3 * k + r];
-    vs += 3 * (size_t)D.K;
-  }
-}
-
-// entry (row, k) of cloud b's cam_source block is neither 0 nor 1, which only voxelisation accepts
-static int cam_source_error(gpdb_ctx *ctx, const char *name, int b, long long row, long long k, int v) {
-  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must be 0 or 1",
-                 name, b, (int)row, (int)k, v);
-  return GPDB_ERR_INVALID;
-}
-
-int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
-                      const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
-                      CloudDesc *desc) {
-  camera_descs(B, n_cameras, view_points, desc);
-  const int32_t *rows = cam_source;  // cloud b's N_b x K_b block
-  for (int b = 0; b < B; b++) {
-    CloudDesc &D = desc[b];
-    const int K = n_cameras[b];  // a local, not D's field: the byte stores to cam below may alias anything
-    const unsigned all = (1u << K) - 1;
-    const int nb = off[b + 1] - off[b];
-    uint8_t *dst = cam + off[b];
-    unsigned seen_by_all = all;
-    if (!rows)
-      memset(dst, (int)all, (size_t)nb);
-    else if (eq1)
-      seen_by_all = pack_rows(rows, nb, K, dst, [](int32_t v) { return v == 1; });
-    else
-      seen_by_all = pack_rows(rows, nb, K, dst, [](int32_t v) { return v > 0; });
-    if (rows && strict01)
-      for (size_t e = 0; e < (size_t)nb * K; e++)
-        if (rows[e] != 0 && rows[e] != 1) return cam_source_error(ctx, name, b, e / K, e % K, rows[e]);
-    if (rows) rows += (size_t)nb * K;
-    D.all_seen = (seen_by_all & all) == all ? 1 : 0;
-  }
-  return GPDB_OK;
-}
-
 // ---- the device-resident entry points (gpdb_*_device): bulk arrays in device memory, sizes and offsets on the host ----
 
 static const unsigned long long NO_BAD = ~0ull;  // the check word when no position offends
@@ -654,41 +593,28 @@ static int check_offsets(gpdb_ctx *ctx, const char *name, const char *label, con
   return GPDB_OK;
 }
 
-// The cloud-local indices idx[off[b] .. off[b+1]) of cloud b of the installed batch must lie in [0, N_b + M_b), M_b its
-// sample positions. A host list (d_off null) is checked here; a device list by batch_check_samples, with d_off the offsets
-// on the device. Either way the first offending position is named. init: the initial indices of gpdb_sis_batch, which
-// has dropped the positions (M_b = 0) and names the indices so.
-static int check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *idx,
+// The cloud-local indices d_idx[off[b] .. off[b+1]) of cloud b of the installed batch must lie in [0, N_b + M_b), M_b
+// its sample positions. The list d_idx and its offsets d_off are in device memory, off is the host copy of d_off;
+// batch_check_samples finds the first offending position, which the message names. init: the initial indices of
+// gpdb_sis_batch, which has dropped the positions (M_b = 0) and names the indices so.
+static int check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *d_idx,
                                const int *d_off) {
   const CloudSet &s = ctx->many;
   const int B = s.n, n = off[B];
+  if (n == 0) return GPDB_OK;
   std::vector<int> lim((size_t)B);
   for (int b = 0; b < B; b++) lim[b] = s.off[b + 1] - s.off[b] + s.positions(b);
-  unsigned long long bad = NO_BAD;
-  if (!d_off) {
-    for (int b = 0; b < B && bad == NO_BAD; b++)
-      for (int i = off[b]; i < off[b + 1]; i++)
-        if (idx[i] < 0 || idx[i] >= lim[b]) {
-          bad = i;
-          break;
-        }
-  } else if (n > 0) {
-    const int rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
-      CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
-      return batch_check_samples(ctx, idx, n, d_off, B, (const int *)d_lim, d_bad);
-    });
-    if (rc != GPDB_OK) return rc;
-  }
-  if (bad == NO_BAD) return GPDB_OK;
+  unsigned long long bad;
+  const int rc = first_bad(ctx, sizeof(int) * (size_t)B, &bad, [&](unsigned long long *d_bad, void *d_lim) -> int {
+    CUDA_TRY(cudaMemcpyAsync(d_lim, lim.data(), sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, ctx->stream));
+    return batch_check_samples(ctx, d_idx, n, d_off, B, (const int *)d_lim, d_bad);
+  });
+  if (rc != GPDB_OK || bad == NO_BAD) return rc;
   const int i = (int)bad;
   int b = 0, v = 0;
   while (off[b + 1] <= i) b++;
-  if (d_off) {
-    CUDA_TRY(cudaMemcpyAsync(&v, idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  } else {
-    v = idx[i];
-  }
+  CUDA_TRY(cudaMemcpyAsync(&v, d_idx + i, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   const int nb = s.off[b + 1] - s.off[b];
   if (init)
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: init index %d at position %d outside cloud %d (N = %d)", name, v, i, b, nb);
@@ -698,21 +624,29 @@ static int check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const
   return GPDB_ERR_INVALID;
 }
 
-// gpdb_pack_cameras with cam_source (d_rows) and cam (d_cam) in device memory: the masks and each cloud's all_seen are
-// computed by batch_pack_cameras, the descriptors' camera fields on the host; same rules, same error
-static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *d_rows,
-                               const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01,
-                               uint8_t *d_cam, CloudDesc *desc) {
-  camera_descs(B, n_cameras, view_points, desc);
+// Packs the camera-source matrices of B clouds (cloud b: off[b+1] - off[b] rows of n_cameras[b] entries, concatenated
+// in device memory as d_rows, or null: every camera sees every point) into d_cam, one bit per camera
+// (batch_pack_cameras), and fills desc[b].K / vp / all_seen. A camera sees a point when its entry is > 0 (eq1 false)
+// or == 1 (eq1 true); strict01 refuses entries other than 0 and 1 and names the first.
+static int pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *d_rows,
+                        const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *d_cam,
+                        CloudDesc *desc) {
   // behind the check word: element offsets of the cam_source blocks [B+1], point offsets [B+1], K_b [B], all_seen [B]
   const size_t bytes = sizeof(long long) * ((size_t)B + 1) + sizeof(int) * (3 * (size_t)B + 1);
   std::vector<unsigned char> h(bytes);
   long long *h_roff = (long long *)h.data();
   int *h_off = (int *)(h_roff + B + 1), *h_k = h_off + B + 1, *h_all = h_k + B;
   h_roff[0] = 0;
+  size_t vs = 0;  // running offset into view_points: cloud b's 3 x K_b block follows cloud b-1's
   for (int b = 0; b < B; b++) {
-    h_roff[b + 1] = h_roff[b] + (long long)(off[b + 1] - off[b]) * n_cameras[b];
-    h_k[b] = n_cameras[b];
+    CloudDesc &D = desc[b];
+    memset(&D, 0, sizeof(D));
+    D.K = n_cameras[b];
+    for (int k = 0; k < D.K; k++)
+      for (int r = 0; r < 3; r++) D.vp[k][r] = view_points[vs + 3 * k + r];
+    vs += 3 * (size_t)D.K;
+    h_roff[b + 1] = h_roff[b] + (long long)(off[b + 1] - off[b]) * D.K;
+    h_k[b] = D.K;
     h_all[b] = 1;
   }
   memcpy(h_off, off, sizeof(int) * ((size_t)B + 1));
@@ -733,62 +667,62 @@ static int pack_cameras_device(gpdb_ctx *ctx, const char *name, int B, const int
     CUDA_TRY(cudaMemcpyAsync(&v, d_rows + e, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     const long long r = (long long)e - h_roff[b];
-    return cam_source_error(ctx, name, b, r / n_cameras[b], r % n_cameras[b], v);
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: cam_source[%d][%d] = %d; without voxelisation entries must be 0 or 1",
+                   name, b, (int)(r / n_cameras[b]), (int)(r % n_cameras[b]), v);
+    return GPDB_ERR_INVALID;
   }
   for (int b = 0; b < B; b++) desc[b].all_seen = h_all[b];
   return GPDB_OK;
 }
 
-// point `point` of an install has a NaN or infinite coordinate
-static int nonfinite_error(gpdb_ctx *ctx, const char *name, unsigned long long point) {
-  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess first)",
-                 name, point);
-  return GPDB_ERR_INVALID;
+// The camera-source matrices of B clouds on the device (*d_rows): the caller's device array as it is (device, or null),
+// else the host matrices uploaded into SCR_UPLOAD
+static int cam_source_on_device(gpdb_ctx *ctx, int B, const int32_t *off, const int32_t *cam_source,
+                                const int32_t *n_cameras, bool device, const int32_t **d_rows) {
+  *d_rows = cam_source;
+  if (device || !cam_source) return GPDB_OK;
+  size_t n = 0;
+  for (int b = 0; b < B; b++) n += (size_t)(off[b + 1] - off[b]) * n_cameras[b];
+  int32_t *up = (int32_t *)gpdb_scratch(ctx, SCR_UPLOAD, sizeof(int32_t) * n);
+  if (!up) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemcpyAsync(up, cam_source, sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+  *d_rows = up;
+  return GPDB_OK;
 }
 
-// gpdb_set_clouds into store s after the argument checks (gpdb_set_cloud: `one`, a batch of one); `name` is the entry
-// point the errors name. A camera sees a point when its entry is > 0.
-static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t n_clouds, const int32_t *point_offsets,
-                      const float *xyz, const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
-                      const double *view_points) {
-  const int N = point_offsets[n_clouds];
-  for (size_t i = 0; i < 3 * (size_t)N; i++)
-    if (!std::isfinite(xyz[i])) return nonfinite_error(ctx, name, i / 3);
+int gpdb_stage_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int B, const int32_t *off, const float *xyz,
+                      const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
+                      const double *view_points, bool device, CloudDesc *desc) {
+  const int N = off[B];
+  const cudaMemcpyKind kind = device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   CUDA_TRY(cudaSetDevice(ctx->device));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  std::vector<uint8_t> cam((size_t)N);
-  std::vector<CloudDesc> desc((size_t)n_clouds);
-  int rc = gpdb_pack_cameras(ctx, name, n_clouds, point_offsets, cam_source, n_cameras, view_points, false, false,
-                             cam.data(), desc.data());
-  if (rc == GPDB_OK) rc = gpdb_cloud_reserve(ctx, s, (size_t)N, n_clouds);
+  int rc = gpdb_cloud_reserve(ctx, s, (size_t)N, B);
   if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(s.xyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.nrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.cam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-  rc = gpdb_install_clouds(ctx, s, desc.data(), point_offsets, n_clouds, true);
-  return rc == GPDB_OK ? n_clouds : rc;
-}
-
-// set_clouds from the caller's device arrays: the finiteness check and the camera masks run on the device, the points and
-// normals are copied device to device into the store
-static int set_clouds_device(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *point_offsets,
-                             const float *d_xyz, const double *d_normals, const int32_t *d_cam_source, const int32_t *n_cameras,
-                             const double *view_points) {
-  const int N = point_offsets[B];
-  CUDA_TRY(cudaSetDevice(ctx->device));
+  CUDA_TRY(cudaMemcpyAsync(s.xyz, xyz, sizeof(float) * 3 * (size_t)N, kind, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(s.nrm, normals, sizeof(double) * 3 * (size_t)N, kind, ctx->stream));
+  const int32_t *d_rows;
+  if ((rc = cam_source_on_device(ctx, B, off, cam_source, n_cameras, device, &d_rows)) != GPDB_OK) return rc;
   unsigned long long bad;
-  int rc = first_bad(ctx, 0, &bad, [&](unsigned long long *d_bad, void *) {
-    return batch_first_nonfinite(ctx, d_xyz, 3 * (long long)N, d_bad);
+  rc = first_bad(ctx, 0, &bad, [&](unsigned long long *d_bad, void *) {
+    return batch_first_nonfinite(ctx, s.xyz, 3 * (long long)N, d_bad);
   });
   if (rc != GPDB_OK) return rc;
-  if (bad != NO_BAD) return nonfinite_error(ctx, name, bad);
+  if (bad != NO_BAD) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: point %llu has a non-finite coordinate (run removeNans / gpdb_preprocess first)",
+                   name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  return pack_cameras(ctx, name, B, off, d_rows, n_cameras, view_points, false, false, s.cam, desc);
+}
+
+// gpdb_set_clouds[_device] into store s after the argument checks (gpdb_set_cloud: `one`, a batch of one); `name` is
+// the entry point the errors name
+static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *off, const float *xyz,
+                      const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
+                      const double *view_points, bool device) {
   std::vector<CloudDesc> desc((size_t)B);
-  rc = gpdb_cloud_reserve(ctx, s, (size_t)N, B);
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(s.xyz, d_xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyDeviceToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(s.nrm, d_normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyDeviceToDevice, ctx->stream));
-  rc = pack_cameras_device(ctx, name, B, point_offsets, d_cam_source, n_cameras, view_points, false, false, s.cam, desc.data());
-  if (rc == GPDB_OK) rc = gpdb_install_clouds(ctx, s, desc.data(), point_offsets, B, true);
+  int rc = gpdb_stage_clouds(ctx, s, name, B, off, xyz, normals, cam_source, n_cameras, view_points, device, desc.data());
+  if (rc == GPDB_OK) rc = gpdb_install_clouds(ctx, s, desc.data(), off, B, true);
   return rc == GPDB_OK ? B : rc;
 }
 
@@ -796,8 +730,8 @@ static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B
                               const gpdb_preprocess_params *pp, int32_t *poff);
 
 // gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); a failed call
-// leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays (read in place, the camera
-// masks packed on the device), else host arrays uploaded here.
+// leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays, read in place; else host
+// arrays uploaded here. Either way the camera masks are packed on the device.
 static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, const int32_t *roff, const float *xyz,
                              const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
                              const double *view_points, const gpdb_preprocess_params *pp, int32_t *poff,
@@ -815,39 +749,30 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   std::vector<CloudDesc> desc((size_t)B);
   const float *d_xyz_raw = xyz;
   const double *d_nrm_raw = normals;
-  uint8_t *d_cam_raw = nullptr;
-  std::vector<uint8_t> cam;
-  int rc;
-  if (device) {
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    d_cam_raw = (uint8_t *)gpdb_scratch(ctx, SCR_SIDX, (size_t)M + 16);
-    if (!d_cam_raw) return GPDB_ERR_CUDA;
-    cudaEventRecord(ev[0], ctx->stream);
-    rc = pack_cameras_device(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, d_cam_raw,
-                             desc.data());
-    if (rc != GPDB_OK) return rc;
-  } else {
-    cam.resize((size_t)M);
-    rc = gpdb_pack_cameras(ctx, name, B, roff, cam_source, n_cameras, view_points, true, !pp->voxelize, cam.data(),
-                           desc.data());
-    if (rc != GPDB_OK) return rc;
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    // ---- one upload of the concatenated raw arrays
-    double *nrm_up = nullptr;
-    float *xyz_up;
-    if (!gpdb_carve(ctx, SCR_SIDX, [&](Carve &c) {
+  float *xyz_up = nullptr;
+  double *nrm_up = nullptr;
+  uint8_t *d_cam_raw;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  if (!gpdb_carve(ctx, SCR_SIDX, [&](Carve &c) {
+        if (!device) {
           if (normals) nrm_up = c.take<double>(3 * (size_t)M);
-          xyz_up = c.take<float>(3 * (size_t)M); d_cam_raw = c.take<uint8_t>((size_t)M + 16);
-        }))
-      return GPDB_ERR_CUDA;
-    cudaEventRecord(ev[0], ctx->stream);
+          xyz_up = c.take<float>(3 * (size_t)M);
+        }
+        d_cam_raw = c.take<uint8_t>((size_t)M + 16);
+      }))
+    return GPDB_ERR_CUDA;
+  cudaEventRecord(ev[0], ctx->stream);
+  if (!device) {  // ---- one upload of the concatenated raw arrays
     CUDA_TRY(cudaMemcpyAsync(xyz_up, xyz, sizeof(float) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(d_cam_raw, cam.data(), (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
     if (normals) CUDA_TRY(cudaMemcpyAsync(nrm_up, normals, sizeof(double) * 3 * (size_t)M, cudaMemcpyHostToDevice, ctx->stream));
     d_xyz_raw = xyz_up;
     d_nrm_raw = nrm_up;
   }
+  const int32_t *d_rows;
+  int rc = cam_source_on_device(ctx, B, roff, cam_source, n_cameras, device, &d_rows);
+  if (rc == GPDB_OK)
+    rc = pack_cameras(ctx, name, B, roff, d_rows, n_cameras, view_points, true, !pp->voxelize, d_cam_raw, desc.data());
+  if (rc != GPDB_OK) return rc;
   for (CloudDesc &D : desc) D.all_seen = cam_source ? 0 : 1;  // without a camera-source matrix every camera sees every point
   cudaEventRecord(ev[1], ctx->stream);
   // ---- removeNans + filterWorkspace + voxelizeCloud of every cloud, into the store's arenas
@@ -972,7 +897,7 @@ int gpdb_set_cloud(gpdb_ctx *ctx, const float *xyz, const double *normals, const
   }
   ctx->one.n = 0;  // past the argument checks, a failed call leaves no cloud behind
   const int32_t off[2] = {0, N};
-  const int rc = set_clouds(ctx, ctx->one, "gpdb_set_cloud", 1, off, xyz, normals, cam_source, &K, view_points);
+  const int rc = set_clouds(ctx, ctx->one, "gpdb_set_cloud", 1, off, xyz, normals, cam_source, &K, view_points, false);
   return rc < 0 ? rc : GPDB_OK;
 }
 
@@ -1597,9 +1522,7 @@ static int clouds_entry(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const
   if (raw)
     return preprocess_clouds(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, pp,
                              processed_offsets_out, device);
-  if (device)
-    return set_clouds_device(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
-  return set_clouds(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points);
+  return set_clouds(ctx, s, name, n_clouds, point_offsets, xyz, normals, cam_source, n_cameras, view_points, device);
 }
 
 extern "C" {
@@ -2003,9 +1926,10 @@ namespace {
 // gpdb_detect_batch / gpdb_detect_batch_select / gpdb_hand_search_batch: checks the CSR sample lists against the installed
 // batch and runs them as ONE sample stream through the chunk pipeline (chunks span cloud boundaries); the records come back
 // with cloud-local sample slots, grouped by cloud (offsets_out). Only the classifying calls (with_images_and_scores) need
-// weights. device (gpdb_*_batch*_device): sample_idx and sel_out are device arrays, the sample lists are checked on the
-// device and the records stay there: the selection (select_k >= 0), or every record (select_k < 0, PIPE_ALL_CALLER) with the
-// dense flags / scores in the caller's d_flags / d_scores when those are given. sel_name names sel_out in the messages.
+// weights. The sample lists are checked on the device; host lists are uploaded first. device (gpdb_*_batch*_device):
+// sample_idx and sel_out are device arrays and the records stay there: the selection (select_k >= 0), or every record
+// (select_k < 0, PIPE_ALL_CALLER) with the dense flags / scores in the caller's d_flags / d_scores when those are
+// given. sel_name names sel_out in the messages.
 int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sample_idx, gpdb_result *out, int32_t *offsets_out,
               bool with_images_and_scores, int select_k, const char *name, bool device = false, gpdb_pose *sel_out = nullptr,
               const char *sel_name = "d_selected_out", uint8_t *d_flags = nullptr, float *d_scores = nullptr) {
@@ -2029,15 +1953,18 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, sel_name);
       return GPDB_ERR_INVALID;
     }
-    rc = check_device_ptrs(ctx, name, {{"d_sample_idx", sample_idx}, {sel_name, sel_out}, {"d_flags_out", d_flags},
-                                       {"d_scores_out", d_scores}});
-  } else {
-    rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, nullptr);
+    if ((rc = check_device_ptrs(ctx, name, {{"d_sample_idx", sample_idx}, {sel_name, sel_out}, {"d_flags_out", d_flags},
+                                            {"d_scores_out", d_scores}})) != GPDB_OK)
+      return rc;
+  } else if (n > 0) {  // host lists go through SCR_SIDX, where the pipeline reads them
+    int *d_sidx = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)n);
+    if (!d_sidx) return GPDB_ERR_CUDA;
+    CUDA_TRY(cudaMemcpyAsync(d_sidx, sample_idx, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+    sample_idx = d_sidx;
   }
-  if (rc != GPDB_OK) return rc;
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if (device && (rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, s.soff)) != GPDB_OK) return rc;
-  PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = device, .per_cloud = true,
+  if ((rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, s.soff)) != GPDB_OK) return rc;
+  PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = true, .per_cloud = true,
                     .classify = with_images_and_scores, .d_flags = d_flags, .d_scores = d_scores,
                     .dest = select_k < 0 ? (device ? PIPE_ALL_CALLER : PIPE_TO_HOST) : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
                     .select_k = select_k, .d_selected = sel_out};
@@ -2666,7 +2593,7 @@ static int sis_run(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init
   return n_out;
 }
 
-// gpdb_sis_batch[_device]: checks, the initial indices into the arena (checked on the host, or on the device), sis_run
+// gpdb_sis_batch[_device]: checks, the initial indices into the arena (checked there, on the device), sis_run
 static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp, const int32_t *init_offsets,
                      const int32_t *init_idx, bool device, gpdb_pose *d_hands_out, int32_t *hand_offsets_out,
                      gpdb_result *out) {
@@ -2688,8 +2615,6 @@ static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp,
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands_out", name);
       return GPDB_ERR_INVALID;
     }
-  } else if ((rc = check_cloud_indices(ctx, name, true, init_offsets, init_idx, nullptr)) != GPDB_OK) {
-    return rc;
   }
   SisState &st = *ctx->sis;
   const int R = sp->num_iterations, S = sp->num_samples_per_iteration;
@@ -2700,7 +2625,7 @@ static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp,
     CUDA_TRY(cudaMemcpyAsync(a.init_idx, init_idx, sizeof(int) * (size_t)n0,
                              device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaMemsetAsync(a.kcount, 0, sizeof(int) * (size_t)B * (R + 1), ctx->stream));  // kept and round counts
-  if (device && (rc = check_cloud_indices(ctx, name, true, init_offsets, a.init_idx, a.init_off)) != GPDB_OK) return rc;
+  if ((rc = check_cloud_indices(ctx, name, true, init_offsets, a.init_idx, a.init_off)) != GPDB_OK) return rc;
   st.B = B;
   st.R = R;
   st.S = S;

@@ -1,8 +1,8 @@
-// batch_device.cu — kernels of the device-resident batch entry points (gpdb_*_device, api.cu): camera-mask packing, the
-// finiteness and sample-index checks, cloud-local sample slots of records, and the caller's hands made addressable by the
-// image kernels. The checks write the lowest
-// offending position (atomicMin into a word the caller set to all ones), so that their error messages name what the
-// host loops of the host entry points name.
+// batch_device.cu — kernels of the installs and batch entry points (api.cu), host calls and gpdb_*_device twins
+// alike: camera-mask packing, the finiteness and sample-index checks, cloud-local sample slots of records, and the
+// caller's hands made addressable by the image kernels. The checks write the lowest
+// offending position (atomicMin into a word the caller set to all ones), so that their error messages name the first
+// offending point, entry or sample, as a sequential loop over the input would.
 #include <algorithm>
 
 #include "common.cuh"

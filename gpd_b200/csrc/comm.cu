@@ -10,10 +10,8 @@
 #include <nccl.h>
 
 #include <algorithm>
-#include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <vector>
 
 #include "common.cuh"
 
@@ -181,18 +179,18 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
   const bool is_root = cs.rank == root;
   // header: N, K, validity of the root's arguments, the view points
   double hdr[4 + 3 * GPDB_MAX_CAMERAS] = {0};
-  std::vector<uint8_t> cam;  // the root's camera masks (a camera sees a point when its entry is > 0, as gpdb_set_cloud)
+  double *d_hdr = (double *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(hdr));
+  if (!d_hdr) return GPDB_ERR_CUDA;
+  CloudSet &s = ctx->one;
+  s.n = 0;
   CloudDesc desc;
   if (is_root) {
-    bool ok = xyz && normals && view_points && N > 0 && K > 0 && K <= GPDB_MAX_CAMERAS;
-    if (ok)
-      for (size_t i = 0; i < 3 * (size_t)N && ok; i++) ok = std::isfinite(xyz[i]);
-    if (ok) {  // a failure here is reported through the header too: every rank waits in its broadcast
-      const int32_t off[2] = {0, N};
-      cam.resize((size_t)N);
-      ok = gpdb_pack_cameras(ctx, "gpdb_set_cloud_bcast", 1, off, cam_source, &K, view_points, false, false, cam.data(),
-                             &desc) == GPDB_OK;
-    }
+    // the root stages its cloud in its own store, checked and packed as gpdb_set_cloud does it; a failure is reported
+    // through the header too: every rank waits in its broadcast
+    const int32_t off[2] = {0, N};
+    const bool ok = xyz && normals && view_points && N > 0 && K > 0 && K <= GPDB_MAX_CAMERAS &&
+                    gpdb_stage_clouds(ctx, s, "gpdb_set_cloud_bcast", 1, off, xyz, normals, cam_source, &K, view_points,
+                                      false, &desc) == GPDB_OK;
     hdr[0] = ok ? N : -1;
     hdr[1] = K;
     if (ok) {
@@ -200,10 +198,6 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
       memcpy(hdr + 4, view_points, sizeof(double) * 3 * (size_t)K);
     }
   }
-  double *d_hdr = (double *)gpdb_scratch(ctx, SCR_WORK_A, sizeof(hdr));
-  if (!d_hdr) return GPDB_ERR_CUDA;
-  CloudSet &s = ctx->one;
-  s.n = 0;
   if (is_root) CUDA_TRY(cudaMemcpyAsync(d_hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, ctx->stream));
   NCCL_TRY(g_nccl.Broadcast(d_hdr, d_hdr, sizeof(hdr), ncclUint8, root, cs.comm, ctx->stream));
   CUDA_TRY(cudaMemcpyAsync(hdr, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, ctx->stream));
@@ -215,12 +209,7 @@ int gpdb_set_cloud_bcast(gpdb_ctx *ctx, int32_t root, const float *xyz, const do
   }
   N = (int32_t)hdr[0];
   K = (int32_t)hdr[1];
-  if ((rc = gpdb_cloud_reserve(ctx, s, (size_t)N, 1)) != GPDB_OK) return rc;
-  if (is_root) {
-    CUDA_TRY(cudaMemcpyAsync(s.xyz, xyz, sizeof(float) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(s.nrm, normals, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(s.cam, cam.data(), (size_t)N, cudaMemcpyHostToDevice, ctx->stream));
-  }
+  if (!is_root && (rc = gpdb_cloud_reserve(ctx, s, (size_t)N, 1)) != GPDB_OK) return rc;
   NCCL_TRY(g_nccl.GroupStart());
   NCCL_TRY(g_nccl.Broadcast(s.xyz, s.xyz, sizeof(float) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));
   NCCL_TRY(g_nccl.Broadcast(s.nrm, s.nrm, sizeof(double) * 3 * (size_t)N, ncclUint8, root, cs.comm, ctx->stream));

@@ -240,13 +240,14 @@ enum ScratchSlot {
   SCR_IMG_OVF,
   // k_frames last tier: the staged neighbourhood keys
   SCR_FRAMES_GL,
-  // device-resident entry points: the check word, then the per-cloud arrays of the check
+  // the device-side input checks of api.cu: the check word, then the per-cloud arrays of the check
   SCR_CHECK,
   // gpdb_sis_batch: kept / evaluated positions, the round's sample lists and counts (main stream, between pipeline calls;
   // read again by gpdb_sis_positions)
   SCR_SIS,
   // host twins of gpdb_preprocess_depth / gpdb_subsample_clouds[_points] / gpdb_segment_plane[s]: the uploaded depth
-  // images, the uploaded mask, the eligible bytes on their way back
+  // images, the uploaded mask, the eligible bytes on their way back; host installs and preprocessing calls: the
+  // uploaded camera-source matrices
   SCR_UPLOAD,
   // gpdb_segment_plane[s]: hypotheses, their inlier counts, the picked and refined planes (plane.cu)
   SCR_PLANE,
@@ -370,12 +371,15 @@ int gpdb_cloud_reserve(gpdb_ctx *ctx, CloudSet &s, size_t n, int n_clouds);
 // (host) carries K / vp / all_seen and receives the point range; uploads the descriptors and builds the grids. nonunit:
 // also set the descriptors' nonunit flags from the stored normals (false: the caller sets them once the normals exist).
 int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *off, int B, bool nonunit);
-// Packs the camera-source matrices of B clouds (cloud b: off[b+1] - off[b] rows of n_cameras[b] entries, concatenated,
-// or null: every camera sees every point) into cam (one bit per camera) and fills desc[b].K / vp / all_seen. A camera
-// sees a point when its entry is > 0 (eq1 false) or == 1 (eq1 true); strict01 refuses entries other than 0 and 1.
-int gpdb_pack_cameras(gpdb_ctx *ctx, const char *name, int B, const int32_t *off, const int32_t *cam_source,
-                      const int32_t *n_cameras, const double *view_points, bool eq1, bool strict01, uint8_t *cam,
-                      CloudDesc *desc);
+// The points of B clouds (cloud b: off[b] .. off[b+1]-1, host offsets) into store s, ready for gpdb_install_clouds:
+// reserves s, copies xyz and normals into it, then on the device refuses a non-finite coordinate (naming the first
+// point) and packs the camera-source matrices (cloud b: n_cameras[b] entries per point, concatenated; null: every
+// camera sees every point) into s.cam, a camera seeing a point when its entry is > 0; desc[b] receives K / vp /
+// all_seen. device: xyz, normals and cam_source are the caller's device arrays, else host arrays uploaded here
+// (cam_source into SCR_UPLOAD).
+int gpdb_stage_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int B, const int32_t *off, const float *xyz,
+                      const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
+                      const double *view_points, bool device, CloudDesc *desc);
 
 // largest b in [0, n) with a[b] <= x, for a non-decreasing a with a[0] <= x: the cloud that owns position x of a CSR array
 __device__ __forceinline__ int csr_owner(const int *a, int n, long long x) {
@@ -419,10 +423,10 @@ __device__ __forceinline__ void ordered_fold(const float *v, int n, float (*stag
   }
 }
 
-// batch_device.cu (the device-resident batch entry points). The checks lower *d_first_bad (set to all ones by the caller)
-// to the first offending position.
+// batch_device.cu (the installs and batch entry points, host and device twins). The checks lower *d_first_bad (set to
+// all ones by the caller) to the first offending position.
 // camera masks of N points in B clouds (point offsets d_off[B+1]; cloud b's N_b x K_b int32 block starts at entry
-// d_row_off[b] of d_rows, K_b = d_k[b]; d_rows null: every camera sees every point), as gpdb_pack_cameras packs them;
+// d_row_off[b] of d_rows, K_b = d_k[b]; d_rows null: every camera sees every point), seen as == 1 (eq1) or > 0;
 // d_all_seen[b] (1 on entry) drops to 0 when a point of cloud b misses a camera; strict01: first entry other than 0 / 1
 int batch_pack_cameras(gpdb_ctx *ctx, const int32_t *d_rows, const int *d_off, const long long *d_row_off, const int *d_k,
                        int B, int N, bool eq1, bool strict01, uint8_t *d_cam, int *d_all_seen,

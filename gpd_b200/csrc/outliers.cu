@@ -153,7 +153,7 @@ int remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int 
   off[0] = 0;
   for (int b = 0; b < B; b++) {
     off[b + 1] = off[b] + cnt[b];
-    desc[b].all_seen = !cnt[B + b];  // as gpdb_pack_cameras computes it for the kept points
+    desc[b].all_seen = !cnt[B + b];  // as batch_pack_cameras computes it for the kept points
   }
   const size_t n2 = (size_t)off[B];
   const bool has_src = s.has_src;

@@ -425,8 +425,8 @@ int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *han
  * (gpdb_set_stream: e.g. the framework's current stream, so that inputs made ready on it need no synchronisation) and, as
  * every entry point, returns once its outputs are complete: they may then be used on any stream.
  * Each call has the semantics, error codes, messages and failure rules of its host twin (a failed install leaves no batch,
- * the single cloud is never touched); its checks run on the device (non-finite coordinates, cam_source entries, sample
- * indices) and report the first offending point / entry / position, as the host loops do. */
+ * the single cloud is never touched); its checks are the host twin's, on the device (non-finite coordinates, cam_source
+ * entries, sample indices), and report the first offending point / entry / position. */
 
 /* gpdb_preprocess_clouds from device arrays: d_xyz [3M] float32, d_normals [3M] float64 or NULL, d_cam_source (the
  * N_b x K_b int32 blocks) or NULL; the raw arrays are read in place and the camera masks packed on the device. */
