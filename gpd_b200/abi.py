@@ -233,6 +233,10 @@ PROTOTYPES = {
     "gpdb_sis_positions": (_int, [_vp] * 6),
     "gpdb_preprocess_depth": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp]),
     "gpdb_preprocess_depth_device": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp]),
+    "gpdb_normals_organized": (_int, [_vp, _i32] + [_vp] * 6),
+    "gpdb_normals_organized_device": (_int, [_vp, _i32] + [_vp] * 6),
+    "gpdb_preprocess_depth_organized": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp, _vp]),
+    "gpdb_preprocess_depth_organized_device": (_int, [_vp, _i32, _vp, _vp, _i32, _vp, _pp, _vp, _vp]),
     "gpdb_subsample_clouds": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
     "gpdb_subsample_clouds_device": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
     "gpdb_plane_params_default": (None, [_pl]),

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
 #include <string>
 #include <utility>
@@ -727,7 +728,8 @@ static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, c
 }
 
 static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
-                              const gpdb_preprocess_params *pp, int32_t *poff);
+                              const gpdb_preprocess_params *pp, int32_t *poff,
+                              const std::function<int()> &after_normals = nullptr);
 
 // gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); a failed call
 // leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays, read in place; else host
@@ -783,9 +785,10 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
 
 // The steps of a preprocessing call after the filter and voxelisation (store s holds the processed points, poff[B+1] their
 // offsets, desc[B] the camera fields): install with one grid per cloud, normals, nonunit flags, stage timings, and the
-// raw offsets roff[B+1] the source indices refer to. A failure leaves no cloud in s.
+// raw offsets roff[B+1] the source indices refer to. after_normals (may be empty) runs between the normal estimation and
+// the nonunit flags, inside the normals' stage timing. A failure leaves no cloud in s.
 static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
-                              const gpdb_preprocess_params *pp, int32_t *poff) {
+                              const gpdb_preprocess_params *pp, int32_t *poff, const std::function<int()> &after_normals) {
   cudaEvent_t *ev = ctx->ev;
   cudaEventRecord(ev[3], ctx->stream);
   // ---- install, one grid per cloud
@@ -798,6 +801,10 @@ static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B
   auto tail = [&]() -> int {
     if (pp->estimate_normals) {
       const int r = pre_normals_batch(ctx, s, pp->normals_radius);
+      if (r != GPDB_OK) return r;
+    }
+    if (after_normals) {
+      const int r = after_normals();
       if (r != GPDB_OK) return r;
     }
     const int r = pre_nonunit_batch(ctx, s);
@@ -1624,9 +1631,11 @@ static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const in
 }
 
 // gpdb_preprocess_depth[_device] after the argument checks: d_depth in device memory (the host twin has uploaded it)
-static int preprocess_depth(gpdb_ctx *ctx, CloudSet &s, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
-                            int32_t format, const void *depth, bool device, const gpdb_preprocess_params *pp,
-                            const std::vector<int> &roff, int32_t *poff) {
+// organized: the normals of gpd_b200_organized.h rule 7 replace the radius estimates (n_fallback[B], host, may be null)
+static int preprocess_depth(gpdb_ctx *ctx, const char *name, CloudSet &s, int32_t B, const int32_t *n_cameras,
+                            const gpdb_depth_camera *cams, int32_t format, const void *depth, bool device,
+                            const gpdb_preprocess_params *pp, const std::vector<int> &roff, int32_t *poff, bool organized,
+                            int32_t *n_fallback) {
   cudaEvent_t *ev = ctx->ev;
   const int M = roff[B];
   CUDA_TRY(cudaSetDevice(ctx->device));
@@ -1651,20 +1660,55 @@ static int preprocess_depth(gpdb_ctx *ctx, CloudSet &s, int32_t B, const int32_t
   cudaEventRecord(ev[1], ctx->stream);
   int rc = pre_depth_batch(ctx, s, d_depth, format, cams, n_cameras, B, roff.data(), *pp, poff, ev[2]);
   if (rc != GPDB_OK) return rc;
-  return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff);
+  if (!organized) return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff);
+  // the host twin's images stay in SCR_UPLOAD until here: the install does not use that slot
+  return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff, [&]() {
+    return org_depth_normals(ctx, name, s, d_depth, format, cams, n_cameras, B, n_fallback);
+  });
 }
 
 static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const int32_t *n_cameras,
                        const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
-                       const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device) {
+                       const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device,
+                       bool organized = false, int32_t *n_fallback = nullptr) {
   if (!ctx) return GPDB_ERR_INVALID;
   drop_batch(ctx);
   std::vector<int> roff;
   int rc = check_depth_args(ctx, name, n_views, n_cameras, cameras, depth_format, depth, pp, processed_offsets_out, roff);
   if (rc == GPDB_OK && device) rc = check_device_ptrs(ctx, name, {{"d_depth", depth}});
   if (rc != GPDB_OK) return rc;
-  return preprocess_depth(ctx, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
-                          processed_offsets_out);
+  return preprocess_depth(ctx, name, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
+                          processed_offsets_out, organized, n_fallback);
+}
+
+// gpdb_normals_organized[_device]: the argument checks, then rules 2 - 5 of gpd_b200_organized.h on every cloud
+static int organized_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *W, const int32_t *H, const float *xyz,
+                           const float *view_points, float *normals_out, float *distance_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !W || !H || !xyz || !view_points || !normals_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, widths, heights, xyz, view_points, normals_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  long long total = 0;
+  for (int b = 0; b < B; b++) {
+    if (W[b] < 1 || H[b] < 1) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d is %d x %d (width and height must be at least 1)", name, b, W[b],
+                     H[b]);
+      return GPDB_ERR_INVALID;
+    }
+    total += (long long)W[b] * H[b];
+    if (total >= (1ll << 31)) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: the call holds 2^31 or more points", name, b);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  int rc = device ? check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals_out", normals_out},
+                                                  {"d_distance_out", distance_out}})
+                  : GPDB_OK;
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  rc = org_normals_batch(ctx, name, B, W, H, xyz, view_points, normals_out, distance_out, device);
+  return rc == GPDB_OK ? B : rc;
 }
 
 // gpdb_subsample_clouds[_device]: the state and argument checks, then the device draw (the host twin uploads the mask and
@@ -1734,6 +1778,35 @@ int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *
                                  int32_t *processed_offsets_out) {
   return depth_entry(ctx, "gpdb_preprocess_depth_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
                      processed_offsets_out, true);
+}
+
+int gpdb_normals_organized(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights, const float *xyz,
+                           const float *view_points, float *normals_out, float *distance_out) {
+  return organized_entry(ctx, "gpdb_normals_organized", n_clouds, widths, heights, xyz, view_points, normals_out,
+                         distance_out, false);
+}
+
+int gpdb_normals_organized_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights,
+                                  const float *d_xyz, const float *view_points, float *d_normals_out,
+                                  float *d_distance_out) {
+  return organized_entry(ctx, "gpdb_normals_organized_device", n_clouds, widths, heights, d_xyz, view_points,
+                         d_normals_out, d_distance_out, true);
+}
+
+int gpdb_preprocess_depth_organized(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
+                                    const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                    int32_t *n_fallback_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_organized", n_views, n_cameras, cameras, depth_format, depth, pp,
+                     processed_offsets_out, false, true, n_fallback_out);
+}
+
+int gpdb_preprocess_depth_organized_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                           const gpdb_depth_camera *cameras, int32_t depth_format, const void *d_depth,
+                                           const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                           int32_t *n_fallback_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_organized_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
+                     processed_offsets_out, true, true, n_fallback_out);
 }
 
 int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *mask, int32_t *sample_idx_out,

@@ -259,6 +259,12 @@ enum ScratchSlot {
   // gpdb_remove_outliers[_clouds]: mean distances, statistics, keep flags and their scan, per-cloud counts and camera
   // flags, the kept points gathered before they go back into the store (outliers.cu)
   SCR_OUTLIERS,
+  // gpdb_normals_organized[_device]: one group of images at a time, its image table, points, distance map, normals and
+  // integral tables (organized.cu)
+  SCR_ORGANIZED,
+  // gpdb_preprocess_depth_organized[_device]: the camera table, the views' first cameras, the fallback counts and the
+  // per-point organized flags (organized.cu)
+  SCR_ORGANIZED_DEPTH,
   SCR_N
 };
 
@@ -559,6 +565,17 @@ int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr);
 // the call. Returns B, or an error after which s holds no cloud (s.n = 0), as after a failed install.
 int outliers_remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int *off, double *stats,
                           uint8_t *kept);
+// organized.cu (include/gpd_b200_organized.h). Rules 2 - 5 on B organized clouds (cloud b: W[b] x H[b] points, view point
+// vp[3b..], concatenated in xyz): nrm_out [3 * pixels] and dist_out [pixels] (may be null). device: xyz and the outputs are
+// device arrays, else host arrays. `name` is the entry point the errors name.
+int org_normals_batch(gpdb_ctx *ctx, const char *name, int B, const int *W, const int *H, const float *xyz, const float *vp,
+                      float *nrm_out, float *dist_out, bool device);
+// Rules 6 and 7 on store s, just installed with radius normals by gpdb_preprocess_depth from the depth images d_depth
+// (device) of the B views with n_cameras[b] cameras cams: each point whose representative pixel has a finite organized
+// normal takes it in s.nrm; n_fallback[B] (host, may be null) receives the other points per view. The nonunit flags are
+// the caller's.
+int org_depth_normals(gpdb_ctx *ctx, const char *name, CloudSet &s, const void *d_depth, int format,
+                      const gpdb_depth_camera *cams, const int *n_cameras, int B, int *n_fallback);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
 

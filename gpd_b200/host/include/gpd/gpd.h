@@ -97,6 +97,15 @@ class Cloud {
   // normals and camera sources replace the cloud's (the reference filters the points alone); the sample indices are
   // invalidated. Prints the reference's message.
   bool removeStatisticalOutliers(gpdb_ctx *ctx);
+  // Cloud::calculateNormalsOrganized (cloud.cpp:479-495) on the device: gpdb_normals_organized on this cloud as its
+  // width x height organized cloud (a .pcd whose HEIGHT is > 1; NaN coordinates for missing points), the view point the
+  // first camera's. The normals become the float32 estimates widened to double, NaN where the estimator gives none.
+  // Prints the reference's messages; a cloud that is not organized keeps its normals and returns false.
+  bool calculateNormalsOrganized(gpdb_ctx *ctx);
+  // the reference's isOrganized(): height > 1 (the .pcd reader keeps WIDTH and HEIGHT; setProcessed makes it 1)
+  bool isOrganized() const { return height_ > 1 && (size_t)width_ * height_ == size(); }
+  int width() const { return width_; }
+  int height() const { return height_; }
   // the same from one cloud's result of gpdb_segment_plane[s] (n_inliers, eligible bytes of its N points)
   void setAbovePlane(int n_inliers, const uint8_t *eligible);
   const std::vector<float> &getPoints() const { return points_; }       // packed x,y,z
@@ -115,6 +124,7 @@ class Cloud {
   std::vector<int> sample_indices_;
   std::vector<int> above_plane_;  // the points off the support plane (sampleAbovePlane): the pool subsample draws from
   std::vector<double> samples_;
+  int width_{0}, height_{1};  // organized layout (.pcd WIDTH / HEIGHT); height 1: unorganized
   unsigned revision_{0};
   void touch();
 };

@@ -246,6 +246,8 @@ bool Cloud::loadPly(const std::string &filename) {
     std::cout << "Unsupported PLY format '" << format << "' (ascii and binary_little_endian are supported)\n";
     return false;
   }
+  width_ = (int)size();
+  height_ = 1;
   printf("Loaded point cloud with %zu points\n", size());
   return true;
 }
@@ -260,6 +262,7 @@ bool Cloud::loadPcd(const std::string &filename) {
   std::vector<std::string> fields, types;
   std::vector<int> sizes, counts;
   size_t npoints = 0;
+  long long pcd_width = 0, pcd_height = 1;
   std::string data_kind, line;
   while (std::getline(f, line)) {
     if (!line.empty() && line.back() == '\r') line.pop_back();
@@ -272,6 +275,8 @@ bool Cloud::loadPcd(const std::string &filename) {
     else if (tag == "TYPE") while (ss >> tok) types.push_back(tok);
     else if (tag == "COUNT") while (ss >> tok) counts.push_back(std::atoi(tok.c_str()));
     else if (tag == "POINTS") ss >> npoints;
+    else if (tag == "WIDTH") ss >> pcd_width;
+    else if (tag == "HEIGHT") ss >> pcd_height;
     else if (tag == "DATA") { ss >> data_kind; break; }
   }
   if (counts.empty()) counts.assign(fields.size(), 1);
@@ -294,7 +299,8 @@ bool Cloud::loadPcd(const std::string &filename) {
   normals_.clear();
   std::vector<double> row(fields.size());
   auto push = [&]() {
-    if (!std::isfinite(row[ix]) || !std::isfinite(row[iy]) || !std::isfinite(row[iz])) return;
+    // pcl::io::loadPCDFile keeps the NaN points of an organized cloud (HEIGHT > 1): they hold its layout
+    if (pcd_height <= 1 && (!std::isfinite(row[ix]) || !std::isfinite(row[iy]) || !std::isfinite(row[iz]))) return;
     points_.push_back((float)row[ix]); points_.push_back((float)row[iy]); points_.push_back((float)row[iz]);
     if (inx >= 0 && iny >= 0 && inz >= 0) {  // PCL normals are float32
       normals_.push_back((double)(float)row[inx]); normals_.push_back((double)(float)row[iny]); normals_.push_back((double)(float)row[inz]);
@@ -346,6 +352,10 @@ bool Cloud::loadPcd(const std::string &filename) {
     std::cout << "Unsupported .pcd DATA kind '" << data_kind << "' (ascii, binary and binary_compressed are supported)\n";
     return false;
   }
+  // an organized cloud keeps its layout when it matches the points read (pcl::PCLPointCloud2 width / height)
+  const bool organized = pcd_height > 1 && pcd_width > 0 && (size_t)(pcd_width * pcd_height) == size();
+  width_ = organized ? (int)pcd_width : (int)size();
+  height_ = organized ? (int)pcd_height : 1;
   printf("Loaded point cloud with %zu points\n", size());
   return true;
 }
@@ -384,6 +394,8 @@ void Cloud::setProcessed(std::vector<float> points, std::vector<double> normals,
   points_ = std::move(points);
   normals_ = std::move(normals);
   camera_source_ = std::move(camera_source);
+  width_ = (int)size();  // filterWorkspace / voxelizeCloud leave an unorganized cloud
+  height_ = 1;
   sample_indices_.clear();
   above_plane_.clear();
   touch();
@@ -436,6 +448,23 @@ bool Cloud::removeStatisticalOutliers(gpdb_ctx *ctx) {
   }
   setProcessed(std::move(xyz), std::move(nrm), std::move(cam));
   printf("Cloud after removing statistical outliers: %zu\n", size());
+  return true;
+}
+
+bool Cloud::calculateNormalsOrganized(gpdb_ctx *ctx) {
+  if (!isOrganized()) {
+    std::cout << "Error: point cloud is not organized!\n";
+    return false;
+  }
+  std::cout << "Using integral images for surface normals estimation ...\n";
+  const float vp[3] = {(float)view_points_[0], (float)view_points_[1], (float)view_points_[2]};  // setViewPoint: floats
+  std::vector<float> nrm(3 * size());
+  if (gpdb_normals_organized(ctx, 1, &width_, &height_, points_.data(), vp, nrm.data(), nullptr) < 0) {
+    printf("ERROR: %s\n", gpdb_last_error(ctx));
+    return false;
+  }
+  normals_.assign(nrm.begin(), nrm.end());
+  touch();
   return true;
 }
 

@@ -151,6 +151,48 @@ def _depth_cameras(n_cameras, cameras):
     return ks, arr, vps
 
 
+def _depth_views(views, name):
+    """(n_cameras, cameras, format, concatenated images) of the host depth views of preprocess_depth[_organized]."""
+    imgs, cams, ks = [], [], []
+    for view in views:
+        ks.append(len(view))
+        for img, cam in view:
+            imgs.append(np.asarray(img))
+            cams.append(cam)
+    dts = {a.dtype for a in imgs}
+    if len(dts) != 1 or next(iter(dts)) not in (np.dtype(np.uint16), np.dtype(np.float32)):
+        raise TypeError(f"{name}: need every image uint16 or every image float32, got {sorted(map(str, dts))}")
+    fmt = abi.DEPTH_U16 if next(iter(dts)) == np.uint16 else abi.DEPTH_F32
+    for i, (a, c) in enumerate(zip(imgs, cams)):
+        if a.shape != (c.height, c.width):
+            raise ValueError(f"{name}: image {i} has shape {a.shape}, its camera is {c.height} x {c.width}")
+    return ks, cams, fmt, np.ascontiguousarray(np.concatenate([a.ravel() for a in imgs]))
+
+
+def _organized_shapes(clouds, view_points):
+    """widths [B], heights [B] (int32) and view points [B, 3] (float32) of [H, W, 3] organized clouds."""
+    for i, c in enumerate(clouds):
+        if len(c.shape) != 3 or c.shape[2] != 3:
+            raise ValueError(f"clouds[{i}]: shape {tuple(c.shape)}, need [H, W, 3]")
+    H = np.array([c.shape[0] for c in clouds], np.int32)
+    W = np.array([c.shape[1] for c in clouds], np.int32)
+    B = len(clouds)
+    vp = np.zeros((B, 3), np.float32) if view_points is None else np.ascontiguousarray(view_points, np.float32).reshape(-1, 3)
+    if len(vp) != B:
+        raise ValueError(f"view_points: {len(vp)} rows, need one per cloud ({B})")
+    return W, H, np.ascontiguousarray(vp)
+
+
+def _organized_split(nrm, dist, W, H):
+    """The concatenated outputs of gpdb_normals_organized[_device] as per-cloud [H, W, 3] normals and [H, W] distances."""
+    ns, ds, o = [], [], 0
+    for w, h in zip(W.tolist(), H.tolist()):
+        ns.append(nrm[3 * o:3 * (o + w * h)].reshape(h, w, 3))
+        ds.append(None if dist is None else dist[o:o + w * h].reshape(h, w))
+        o += w * h
+    return ns, ds
+
+
 def pack_samples(sample_lists):
     """The CSR arrays of gpdb_detect_batch for one list of cloud-local sample indices per cloud: (offsets [B+1], indices)."""
     arrs = [np.asarray(s, dtype=np.int32).ravel() for s in sample_lists]
@@ -553,12 +595,15 @@ class Context:
                                                                          C.byref(pp), _p(poff)),
                              poff, ks, vp, int(off[-1]))
 
-    def _install_depth(self, fn, n_cameras, cameras, fmt, ptr, pp):
+    def _install_depth(self, fn, n_cameras, cameras, fmt, ptr, pp, fallback=None):
+        # fallback: the n_fallback_out array of the organized entry points, which take it as one more argument
         ks, arr, vps = _depth_cameras(n_cameras, cameras)
         if pp is None:
             pp = preprocess_params()
         poff = np.zeros(len(ks) + 1, np.int32)
-        return self._install(lambda: fn(self.h, len(ks), _p(ks), C.cast(arr, C.c_void_p), int(fmt), ptr, C.byref(pp), _p(poff)),
+        extra = () if fallback is None else (_p(fallback),)
+        return self._install(lambda: fn(self.h, len(ks), _p(ks), C.cast(arr, C.c_void_p), int(fmt), ptr, C.byref(pp), _p(poff),
+                                        *extra),
                              poff, ks, vps, sum(int(c.width) * int(c.height) for c in arr[:len(cameras)]))
 
     def preprocess_depth(self, views, pp=None, read_back=True):
@@ -567,30 +612,40 @@ class Context:
         GPDB_DEPTH_U16 / GPDB_DEPTH_F32), camera a depth_camera(). View b's raw cloud is its cameras' pixels concatenated
         (include/gpd_b200_depth.h), so src indexes those pixels. Installs the processed batch; returns one dict per view as
         preprocess_clouds() does, or the processed point offsets [B+1] when read_back is False."""
-        imgs, cams, ks = [], [], []
-        for view in views:
-            ks.append(len(view))
-            for img, cam in view:
-                imgs.append(np.asarray(img))
-                cams.append(cam)
-        dts = {a.dtype for a in imgs}
-        if len(dts) != 1 or next(iter(dts)) not in (np.dtype(np.uint16), np.dtype(np.float32)):
-            raise TypeError(f"preprocess_depth: need every image uint16 or every image float32, got {sorted(map(str, dts))}")
-        fmt = abi.DEPTH_U16 if next(iter(dts)) == np.uint16 else abi.DEPTH_F32
-        for i, (a, c) in enumerate(zip(imgs, cams)):
-            if a.shape != (c.height, c.width):
-                raise ValueError(f"preprocess_depth: image {i} has shape {a.shape}, its camera is {c.height} x {c.width}")
-        depth = np.ascontiguousarray(np.concatenate([a.ravel() for a in imgs]))
+        ks, cams, fmt, depth = _depth_views(views, "preprocess_depth")
         poff = self._install_depth(lib().gpdb_preprocess_depth, ks, cams, fmt, _p(depth), pp)
         return self.get_clouds() if read_back else poff
+
+    def preprocess_depth_organized(self, views, pp=None, read_back=True):
+        """gpdb_preprocess_depth_organized: preprocess_depth() with the integral-image normals of each camera's image
+        (include/gpd_b200_organized.h rule 7); a point without a finite one keeps its radius estimate. Returns
+        (what preprocess_depth() returns, the fallback points per view [B])."""
+        ks, cams, fmt, depth = _depth_views(views, "preprocess_depth_organized")
+        fb = np.zeros(len(ks), np.int32)
+        poff = self._install_depth(lib().gpdb_preprocess_depth_organized, ks, cams, fmt, _p(depth), pp, fb)
+        return (self.get_clouds() if read_back else poff), fb
 
     def preprocess_depth_tensors(self, n_cameras, cameras, d_depth, pp=None):
         """gpdb_preprocess_depth_device: preprocess_depth() of depth images held in ONE CUDA tensor, every camera's image
         back to back in camera order (n_cameras [B] per view, cameras the sum(n_cameras) depth_camera()s, view by view).
         The tensor's dtype selects the format: torch.uint16 (or int16 holding the same bits) or torch.float32. Installs the
         processed batch; returns its point offsets [B+1]."""
-        import torch
         cams = list(cameras)
+        fmt, ptr = self._depth_tensor(cams, d_depth)
+        return self._install_depth(lib().gpdb_preprocess_depth_device, n_cameras, cams, fmt, ptr, pp)
+
+    def preprocess_depth_organized_tensors(self, n_cameras, cameras, d_depth, pp=None):
+        """gpdb_preprocess_depth_organized_device: preprocess_depth_organized() of depth images held in one CUDA tensor,
+        as preprocess_depth_tensors() takes them. Returns (the processed point offsets [B+1], the fallback points per view
+        [B])."""
+        cams = list(cameras)
+        fmt, ptr = self._depth_tensor(cams, d_depth)
+        fb = np.zeros(len(_host_i32("n_cameras", n_cameras)), np.int32)
+        return self._install_depth(lib().gpdb_preprocess_depth_organized_device, n_cameras, cams, fmt, ptr, pp, fb), fb
+
+    def _depth_tensor(self, cams, d_depth):
+        """(format, device pointer) of the depth tensor of a *_tensors call whose cameras are cams."""
+        import torch
         n = sum(int(c.width) * int(c.height) for c in cams)
         if not isinstance(d_depth, torch.Tensor):
             raise ValueError(f"d_depth: need a tensor on cuda:{self.params.device}, got {type(d_depth).__name__}")
@@ -603,7 +658,40 @@ class Context:
             raise TypeError(f"d_depth: need torch.uint16 or torch.float32, got {d_depth.dtype}")
         ptr = _device_arg("d_depth", d_depth, dt, self.params.device, n)
         self._torch_stream()
-        return self._install_depth(lib().gpdb_preprocess_depth_device, n_cameras, cams, fmt, ptr, pp)
+        return fmt, ptr
+
+    def normals_organized(self, clouds, view_points=None):
+        """gpdb_normals_organized: Cloud::calculateNormalsOrganized (include/gpd_b200_organized.h) of organized clouds,
+        each a [H, W, 3] float32 array (NaN coordinates for a missing point), view_points [B, 3] (None: the origin).
+        Nothing installed changes. Returns (normals, distance maps): one [H, W, 3] float32 and one [H, W] float32 array
+        per cloud, NaN normals where the estimator gives none."""
+        arrs = [np.asarray(c, dtype=np.float32) for c in clouds]
+        W, H, vp = _organized_shapes(arrs, view_points)
+        xyz = np.ascontiguousarray(np.concatenate([a.ravel() for a in arrs])) if arrs else np.zeros(0, np.float32)
+        n = int((W.astype(np.int64) * H).sum())
+        nrm, dist = np.zeros(3 * n, np.float32), np.zeros(n, np.float32)
+        self._check(lib().gpdb_normals_organized(self.h, len(arrs), _p(W), _p(H), _p(xyz), _p(vp), _p(nrm), _p(dist)))
+        return _organized_split(nrm, dist, W, H)
+
+    def normals_organized_tensors(self, clouds, view_points=None, distance=True):
+        """gpdb_normals_organized_device: normals_organized() of [H, W, 3] float32 CUDA tensors (several are copied back to
+        back into one first). Returns lists of [H, W, 3] normal and [H, W] distance tensors (views of one output each;
+        distances None when distance is False)."""
+        import torch
+        ts = list(clouds)
+        W, H, vp = _organized_shapes(ts, view_points)
+        dev = self.params.device
+        for i, t in enumerate(ts):
+            _device_arg(f"clouds[{i}]", t, torch.float32, dev, t.numel())
+        xyz = ts[0].contiguous() if len(ts) == 1 else torch.cat([t.reshape(-1) for t in ts])
+        n = int((W.astype(np.int64) * H).sum())
+        nrm = torch.empty(3 * n, dtype=torch.float32, device=f"cuda:{dev}")
+        dist = torch.empty(n, dtype=torch.float32, device=f"cuda:{dev}") if distance else None
+        self._torch_stream()
+        self._check(lib().gpdb_normals_organized_device(self.h, len(ts), _p(W), _p(H), _device_arg("clouds", xyz, torch.float32, dev, 3 * n),
+                                                        _p(vp), _device_arg("normals", nrm, torch.float32, dev, 3 * n),
+                                                        _device_arg("distance", dist, torch.float32, dev, n, optional=True)))
+        return _organized_split(nrm, dist, W, H)
 
     def _subsample_room(self, num_samples):
         npts = np.diff(self._batch[0]).astype(np.int64) if self._batch is not None else np.zeros(0, np.int64)

@@ -565,6 +565,42 @@ int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *
                                  int32_t depth_format, const void *d_depth, const gpdb_preprocess_params *pp,
                                  int32_t *processed_offsets_out);
 
+/* --- organized clouds: Cloud::calculateNormalsOrganized on the device (include/gpd_b200_organized.h) ------------------
+ * pcl::IntegralImageNormalEstimation (COVARIANCE_MATRIX, smoothing size 20, PCL's defaults otherwise), the method the
+ * reference's calculateNormals picks for an organized cloud: each normal comes from a pixel window of at most 20 x 20
+ * that shrinks towards depth discontinuities, so it does not smooth across object silhouettes, and its cost per pixel
+ * does not depend on how many neighbours a point has. The reference's preprocessing never reaches it (its workspace
+ * filter makes the cloud unorganized), so it is a call of its own. */
+
+/* Normals of n_clouds organized clouds by the rules of gpd_b200_organized.h: cloud b is heights[b] x widths[b] float32
+ * points, row-major, NaN coordinates for a missing point, with view point view_points[3b .. 3b+2] (float32, host);
+ * the clouds lie back to back in xyz. normals_out [3 * points] receives the float32 normals (NaN where rule 5 gives none:
+ * the 20-pixel border, non-finite depth, a distance map value <= 2), distance_out [points] (may be NULL) the rule-3
+ * distance map. Nothing installed changes. GPDB_ERR_INVALID before any device work: n_clouds <= 0, a null array, a
+ * width or height < 1, 2^31 or more points in the call. Returns n_clouds. */
+int gpdb_normals_organized(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights, const float *xyz,
+                           const float *view_points, float *normals_out, float *distance_out);
+/* The same with xyz and the outputs in device memory (widths, heights and view_points stay host arrays). */
+int gpdb_normals_organized_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights,
+                                  const float *d_xyz, const float *view_points, float *d_normals_out,
+                                  float *d_distance_out);
+/* gpdb_preprocess_depth with the normals of gpd_b200_organized.h rule 7: a processed point whose representative pixel
+ * (gpdb_get_clouds' src) has a finite integral-image normal in its camera's image (camera frame, rotated to the world by
+ * the pose's R) takes it, with reverseNormals applied; every other point (a fallback: the image border, silhouettes,
+ * holes) keeps exactly the radius estimate gpdb_preprocess_depth gives it, so estimate_normals must be nonzero and
+ * normals_radius > 0. Points, camera sources, source indices and offsets are those of gpdb_preprocess_depth bit for bit,
+ * and so are the failure rules. n_fallback_out [B] (may be NULL) receives each view's fallback points.
+ * gpdb_preprocess_timings' ms[4] covers both normal methods. Returns B. */
+int gpdb_preprocess_depth_organized(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
+                                    const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                    int32_t *n_fallback_out);
+/* The same with the images in device memory. */
+int gpdb_preprocess_depth_organized_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                           const gpdb_depth_camera *cameras, int32_t depth_format, const void *d_depth,
+                                           const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                           int32_t *n_fallback_out);
+
 /* Replaces: Cloud::subsample (cloud.cpp:350-370) for every cloud of the installed batch, by the rule of gpd_b200_depth.h
  * 5: cloud b draws min(num_samples, eligible points) cloud-local point indices without replacement, in ascending order
  * (num_samples = 0: every eligible point). mask (may be NULL) holds one byte per raw point of the preprocessing call that
