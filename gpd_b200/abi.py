@@ -176,6 +176,27 @@ class PlaneParams(C.Structure):
     ]
 
 
+class TrainParams(C.Structure):
+    """gpdb_train_params (include/gpd_b200.h, rules in include/gpd_b200_train.h)."""
+
+    _fields_ = [
+        ("optimizer", C.c_int32),
+        ("lr", C.c_float),
+        ("momentum", C.c_float),
+        ("weight_decay", C.c_float),
+        ("beta1", C.c_float),
+        ("beta2", C.c_float),
+        ("eps", C.c_float),
+    ]
+
+
+class TrainDebug(C.Structure):
+    """gpdb_train_debug (include/gpd_b200.h): host buffers of gpdb_debug_train_step, any of them NULL."""
+
+    _fields_ = [(f, C.c_void_p) for f in ("pool1", "pool2", "ip1", "logits", "choice1", "choice2", "loss", "dlogits",
+                                          "dip1", "dpool2", "dpool1")] + [("grad", C.c_void_p * 8)]
+
+
 _vp, _i32, _int = C.c_void_p, C.c_int32, C.c_int
 _res, _pp, _sp, _pl = C.POINTER(Result), C.POINTER(PreprocessParams), C.POINTER(SisParams), C.POINTER(PlaneParams)
 
@@ -262,6 +283,12 @@ PROTOTYPES = {
     "gpdb_debug_phase_cycles": (_int, [_vp, _int, _vp]),
     "gpdb_debug_path_counts": (_int, [_vp, _vp]),
     "gpdb_debug_lenet_layers": (_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "gpdb_train_begin": (_int, [_vp] * 3),
+    "gpdb_train_step": (_int, [_vp, _vp, _vp, _i32, _vp]),
+    "gpdb_train_step_device": (_int, [_vp, _vp, _vp, _i32, _vp]),
+    "gpdb_train_weights": (_int, [_vp, _vp]),
+    "gpdb_write_weights_dir": (_int, [C.c_char_p, _i32, _vp]),
+    "gpdb_debug_train_step": (_int, [_vp, _vp, _vp, _i32, _vp]),
     "gpdb_build_info": (C.c_char_p, []),
 }
 

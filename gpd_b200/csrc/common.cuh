@@ -189,6 +189,7 @@ struct StageTimes;  // api.cu
 struct PipeState;   // api.cu: copy stream, events and the pinned result arenas of the chunk pipeline
 struct CommState;   // comm.cu: NCCL communicator (multi-GPU sharding)
 struct SisState;    // api.cu: host-side record of the last gpdb_sis_batch call (gpdb_sis_positions)
+struct TrainState;  // train.cu: the trained weights, the optimiser state and the step count (gpdb_train_begin)
 
 // The scratch buffers of a context (gpdb_scratch), each grown on demand and never shrunk. This enum is the whole slot
 // map: a buffer is addressed by its enumerator only, and a buffer several stages share is named for what it is, not for
@@ -265,6 +266,9 @@ enum ScratchSlot {
   // gpdb_preprocess_depth_organized[_device]: the camera table, the views' first cameras, the fallback counts and the
   // per-point organized flags (organized.cu)
   SCR_ORGANIZED_DEPTH,
+  // gpdb_train_step[_device] / gpdb_debug_train_step: one chunk's forward state, backward intermediates and per-image
+  // gradient partials (train.cu, train_scratch_bytes)
+  SCR_TRAIN,
   SCR_N
 };
 
@@ -280,6 +284,7 @@ struct gpdb_ctx {
   PipeState *pipe;
   CommState *comm;
   SisState *sis;
+  TrainState *train;
   int sm_count;
   int smem_optin;  // largest shared memory (dynamic + static) one block may opt in to, in bytes
   char err[512];
@@ -591,6 +596,23 @@ struct LenetLayers {
 // layers == nullptr (every production call): the kernels alone, nothing is read back
 int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits,
                   const LenetLayers *layers = nullptr);
+
+// The float32 SIMT forward (lenet_impl = 1) with the weights w (lenet_upload's layouts): pool1 p1 [n][20][28][28], pool2
+// p2 [n][7200] (k = c + 50 j), ip1 h3 [n][500], scores and logits. lenet_forward and the training forward both run it.
+int lenet_simt_run(gpdb_ctx *ctx, const LenetWeights &w, const uint8_t *d_images, int n, float *p1, float *p2, float *h3,
+                   float *d_scores, float *d_logits);
+
+// train.cu (include/gpd_b200_train.h)
+int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]);
+// one step on n device images / labels (labels already checked); d_loss_out / h_loss_out: device / host float or null; dbg: host outputs of a
+// debug step (n <= GPDB_TRAIN_CHUNK), which updates nothing
+int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, int n, float *d_loss_out,
+               float *h_loss_out, const gpdb_train_debug *dbg);
+int train_weights(gpdb_ctx *ctx, float *const out[8]);
+bool train_started(const gpdb_ctx *ctx);
+void train_free(gpdb_ctx *ctx);
+// the label check of a step: lowers *d_bad to the first label outside {0, 1}
+int train_check_labels(gpdb_ctx *ctx, const int32_t *d_labels, int n, unsigned long long *d_bad);
 
 // lenet_tc.cu (wgmma conv1 / conv2 / ip1)
 int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]);

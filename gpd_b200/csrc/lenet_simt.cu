@@ -291,10 +291,37 @@ static int read_layers(gpdb_ctx *ctx, int n, bool use_tc, const float *p1, const
   return GPDB_OK;
 }
 
+int lenet_simt_run(gpdb_ctx *ctx, const LenetWeights &w, const uint8_t *d_images, int n, float *p1, float *p2, float *h3,
+                   float *d_scores, float *d_logits) {
+  const int S = ctx->prm.image_size, C = ctx->prm.image_num_channels;
+  const int P1 = (S - 4) / 2, P2 = (P1 - 4) / 2, K = NF2 * P2 * P2;
+  const int relu = ctx->prm.relu_after_conv;
+  size_t sm1 = sizeof(float) * C * 25 * NF1 + (size_t)C * S * S;
+  size_t sm2 = sizeof(float) * (NF1 * 25 * NF2 + NF1 * P1 * P1);
+  CUDA_TRY(cudaFuncSetAttribute(k_conv1_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
+  CUDA_TRY(cudaFuncSetAttribute(k_conv2_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+  cudaEvent_t e1 = gpdb_st_begin(ctx);
+  k_conv1_pool<<<std::min(n, ctx->sm_count * 2), 224, sm1, ctx->stream>>>(d_images, n, S, C, w.c1w, w.c1b, relu, p1);
+  LAUNCH_CHECK();
+  gpdb_st_end(ctx, 5, e1);
+  cudaEvent_t e2 = gpdb_st_begin(ctx);
+  k_conv2_pool<<<std::min(n, ctx->sm_count), 240, sm2, ctx->stream>>>(p1, n, P1, w.c2w, w.c2b, relu, p2);
+  LAUNCH_CHECK();
+  gpdb_st_end(ctx, 6, e2);
+  cudaEvent_t e3 = gpdb_st_begin(ctx);
+  dim3 g3((n + 63) / 64, (NH + 63) / 64);
+  k_ip1<<<g3, 256, 0, ctx->stream>>>(p2, n, K, w.i1w, w.i1b, h3);
+  LAUNCH_CHECK();
+  k_ip2<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(h3, n, w.i2w, w.i2b, d_scores, d_logits);
+  LAUNCH_CHECK();
+  gpdb_st_end(ctx, 7, e3);
+  return GPDB_OK;
+}
+
 int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores, float *d_logits,
                   const LenetLayers *layers) {
   if (n <= 0) return GPDB_OK;
-  const int S = ctx->prm.image_size, C = ctx->prm.image_num_channels;
+  const int S = ctx->prm.image_size;
   const int P1 = (S - 4) / 2, P2 = (P1 - 4) / 2, K = NF2 * P2 * P2;
   if (S != 60) {  // 61..63 would also give ip1 7200 inputs, but the reference's network is built for 60 x 60
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "LeNet expects image_size 60 (ip1 input 7200), got %d (ip1 input %d)", S, K);
@@ -306,11 +333,6 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
   float *p2 = (float *)gpdb_scratch(ctx, SCR_WORK_B, use_tc ? lenet_tc_xc_bytes(n) : sizeof(float) * (size_t)n * K);
   float *h3 = (float *)gpdb_scratch(ctx, SCR_WORK_C, sizeof(float) * (size_t)n * NH);
   if (!p1 || !p2 || !h3) return GPDB_ERR_CUDA;
-  const int relu = ctx->prm.relu_after_conv;
-  size_t sm1 = sizeof(float) * C * 25 * NF1 + (size_t)C * S * S;
-  size_t sm2 = sizeof(float) * (NF1 * 25 * NF2 + NF1 * P1 * P1);
-  CUDA_TRY(cudaFuncSetAttribute(k_conv1_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
-  CUDA_TRY(cudaFuncSetAttribute(k_conv2_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
   if (use_tc) {
     int rc = lenet_tc_forward(ctx, d_images, n, p1, reinterpret_cast<__half *>(p2), h3);
     if (rc != GPDB_OK) return rc;
@@ -319,22 +341,8 @@ int lenet_forward(gpdb_ctx *ctx, const uint8_t *d_images, int n, float *d_scores
     LAUNCH_CHECK();
     gpdb_st_end(ctx, 7, e4);
     return layers ? read_layers(ctx, n, true, p1, p2, h3, *layers) : GPDB_OK;
-  } else {
-  cudaEvent_t e1 = gpdb_st_begin(ctx);
-  k_conv1_pool<<<std::min(n, ctx->sm_count * 2), 224, sm1, ctx->stream>>>(d_images, n, S, C, w.c1w, w.c1b, relu, p1);
-  LAUNCH_CHECK();
-  gpdb_st_end(ctx, 5, e1);
-  cudaEvent_t e2 = gpdb_st_begin(ctx);
-  k_conv2_pool<<<std::min(n, ctx->sm_count), 240, sm2, ctx->stream>>>(p1, n, P1, w.c2w, w.c2b, relu, p2);
-  LAUNCH_CHECK();
-  gpdb_st_end(ctx, 6, e2);
   }
-  cudaEvent_t e3 = gpdb_st_begin(ctx);
-  dim3 g3((n + 63) / 64, (NH + 63) / 64);
-  k_ip1<<<g3, 256, 0, ctx->stream>>>(p2, n, K, w.i1w, w.i1b, h3);
-  LAUNCH_CHECK();
-  k_ip2<<<(n * 32 + 255) / 256, 256, 0, ctx->stream>>>(h3, n, w.i2w, w.i2b, d_scores, d_logits);
-  LAUNCH_CHECK();
-  gpdb_st_end(ctx, 7, e3);
+  const int rc = lenet_simt_run(ctx, w, d_images, n, p1, p2, h3, d_scores, d_logits);
+  if (rc != GPDB_OK) return rc;
   return layers ? read_layers(ctx, n, false, p1, p2, h3, *layers) : GPDB_OK;
 }

@@ -265,4 +265,24 @@ int gpdb_load_weights_file(gpdb_ctx *ctx, const char *model_file, const char *we
   return gpdb_set_weights(ctx, a[0].data(), a[1].data(), a[2].data(), a[3].data(), a[4].data(), a[5].data(), a[6].data(), a[7].data());
 }
 
+// The .bin parameter directory, written: each array as raw little-endian float32, the layout gpdb_load_weights_dir and
+// readBinaryFileIntoVector (eigen_classifier.cpp:185-205) read.
+int gpdb_write_weights_dir(const char *dir, int32_t channels, const float *const w[8]) {
+  if (!dir || !*dir || !w || !(channels == 1 || channels == 3 || channels == 12 || channels == 15)) return GPDB_ERR_INVALID;
+  for (int i = 0; i < 8; i++)
+    if (!w[i]) return GPDB_ERR_INVALID;
+  const char *names[8] = {"conv1_weights", "conv1_biases", "conv2_weights", "conv2_biases",
+                          "ip1_weights",   "ip1_biases",   "ip2_weights",   "ip2_biases"};
+  const size_t sizes[8] = {(size_t)20 * channels * 25, 20, 50 * 20 * 25, 50, (size_t)500 * 7200, 500, 1000, 2};
+  std::string d = dir;
+  if (d.back() != '/') d += '/';
+  for (int i = 0; i < 8; i++) {
+    FILE *f = fopen((d + names[i] + ".bin").c_str(), "wb");
+    if (!f) return GPDB_ERR_IO;
+    const bool ok = fwrite(w[i], sizeof(float), sizes[i], f) == sizes[i];
+    if ((fclose(f) != 0) || !ok) return GPDB_ERR_IO;
+  }
+  return GPDB_OK;
+}
+
 }  // extern "C"

@@ -97,6 +97,40 @@ def read_weights_file(weights_file, channels, model_file=None):
     return arrs, relu.value
 
 
+def weight_sizes(channels):
+    """Values in each of the eight arrays of the .bin layout (gpdb_set_weights) for a network of `channels` inputs."""
+    return [20 * channels * 25, 20, 50 * 20 * 25, 50, 500 * 7200, 500, 1000, 2]
+
+
+def train_params(optimizer="sgd", lr=1e-5, momentum=0.9, weight_decay=0.0, betas=(0.9, 0.999), eps=1e-8):
+    """gpdb_train_params: optimizer "sgd" (torch.optim.SGD, dampening 0) or "adam" (torch.optim.Adam, L2 weight decay).
+    The defaults are the reference's pytorch/train_net.py (SGD, lr 1e-5, momentum 0.9)."""
+    opt = {"sgd": 0, "adam": 1}.get(optimizer)
+    if opt is None:
+        raise ValueError(f"optimizer: 'sgd' or 'adam', got {optimizer!r}")
+    return abi.TrainParams(opt, lr, momentum, weight_decay, betas[0], betas[1], eps)
+
+
+def _weight_ptrs(arrays, channels):
+    sizes = weight_sizes(channels)
+    if len(arrays) != 8:
+        raise ValueError(f"need 8 weight arrays, got {len(arrays)}")
+    arrs = [np.ascontiguousarray(a, dtype=np.float32).ravel() for a in arrays]
+    for i, (a, s) in enumerate(zip(arrs, sizes)):
+        if a.size != s:
+            raise ValueError(f"weight array {i}: {a.size} values, need {s} for {channels} channels")
+    return arrs, (C.c_void_p * 8)(*[a.ctypes.data for a in arrs])
+
+
+def write_weights_dir(d, channels, arrays):
+    """gpdb_write_weights_dir: the eight arrays as {conv1,conv2,ip1,ip2}_{weights,biases}.bin in the directory d, what
+    Context.load_weights_dir and the reference's EigenClassifier read."""
+    _, ptrs = _weight_ptrs(arrays, channels)
+    rc = lib().gpdb_write_weights_dir(os.fspath(d).encode(), int(channels), ptrs)
+    if rc != 0:
+        raise GpdbError(rc, f"gpdb_write_weights_dir({os.fspath(d)!r}, {channels}) failed")
+
+
 def pack_clouds(clouds):
     """The CSR arrays of gpdb_set_clouds / gpdb_preprocess_clouds for a list of cloud dicts (xyz [N, 3], normals [N, 3],
     optional cam_source [N, K], optional view_points [K, 3]): point offsets [B+1], xyz, normals (None when no cloud has
@@ -1072,6 +1106,61 @@ class Context:
         logits = np.zeros((n, 2), np.float32)
         self._check(lib().gpdb_classify(self.h, _p(images), n, _p(scores), _p(logits)))
         return scores, logits
+
+    def train_begin(self, params, init=None):
+        """gpdb_train_begin: start (or restart) training from the eight arrays `init`, or from the loaded weights when
+        None. The optimiser state and step count start at zero."""
+        C_ = self.params.image_num_channels
+        if init is None:
+            self._check(lib().gpdb_train_begin(self.h, C.c_void_p(C.addressof(params)), None))
+        else:
+            arrs, ptrs = _weight_ptrs(init, C_)
+            self._check(lib().gpdb_train_begin(self.h, C.c_void_p(C.addressof(params)), ptrs))
+
+    def train_step(self, images, labels):
+        """gpdb_train_step: one optimiser step on uint8 images [n, S, S, C] (cv::Mat layout) and labels in {0, 1};
+        returns the step's mean loss."""
+        images = np.ascontiguousarray(images, dtype=np.uint8)
+        labels = _host_i32("labels", labels, images.shape[0] if images.ndim else 0)
+        loss = C.c_float()
+        self._check(lib().gpdb_train_step(self.h, _p(images), _p(labels), len(labels), C.byref(loss)))
+        return loss.value
+
+    def train_step_tensors(self, images, labels):
+        """gpdb_train_step_device: train_step() on a uint8 CUDA tensor [n, S, S, C] and int32 CUDA labels [n]; returns
+        the loss as a 0-d float32 CUDA tensor, written on the device (no synchronisation)."""
+        import torch
+        dev = self.params.device
+        S, Cc = self.params.image_size, self.params.image_num_channels
+        n = images.shape[0] if isinstance(images, torch.Tensor) and images.dim() > 0 else 0
+        pi = _device_arg("images", images, torch.uint8, dev, n * S * S * Cc)
+        pl = _device_arg("labels", labels, torch.int32, dev, n)
+        self._torch_stream()
+        loss = torch.empty((), dtype=torch.float32, device=f"cuda:{dev}")
+        self._check(lib().gpdb_train_step_device(self.h, pi, pl, n, C.c_void_p(loss.data_ptr())))
+        return loss
+
+    def train_weights(self):
+        """gpdb_train_weights: the trained weights as eight float32 arrays in the .bin layout (set_weights takes them)."""
+        arrs = [np.zeros(s, np.float32) for s in weight_sizes(self.params.image_num_channels)]
+        self._check(lib().gpdb_train_weights(self.h, (C.c_void_p * 8)(*[a.ctypes.data for a in arrs])))
+        return arrs
+
+    def debug_train_step(self, images, labels):
+        """gpdb_debug_train_step: one step's forward state, backward intermediates and gradients (nothing updated), as a
+        dict of numpy arrays named as the fields of gpdb_train_debug; "grad" holds the eight gradients."""
+        images = np.ascontiguousarray(images, dtype=np.uint8)
+        n = images.shape[0]
+        labels = _host_i32("labels", labels, n)
+        shapes = {"pool1": ((n, 20, 28, 28), np.float32), "pool2": ((n, 7200), np.float32), "ip1": ((n, 500), np.float32),
+                  "logits": ((n, 2), np.float32), "choice1": ((n, 20, 28, 28), np.uint8), "choice2": ((n, 7200), np.uint8),
+                  "loss": ((n,), np.float32), "dlogits": ((n, 2), np.float32), "dip1": ((n, 500), np.float32),
+                  "dpool2": ((n, 7200), np.float32), "dpool1": ((n, 20, 28, 28), np.float32)}
+        out = {k: np.zeros(s, t) for k, (s, t) in shapes.items()}
+        out["grad"] = [np.zeros(s, np.float32) for s in weight_sizes(self.params.image_num_channels)]
+        dbg = abi.TrainDebug(*[out[k].ctypes.data for k in shapes], (C.c_void_p * 8)(*[a.ctypes.data for a in out["grad"]]))
+        self._check(lib().gpdb_debug_train_step(self.h, _p(images), _p(labels), n, C.c_void_p(C.addressof(dbg))))
+        return out
 
     def lenet_layers(self, images):
         """gpdb_debug_lenet_layers: classify() that also returns every layer the selected implementation computed, as a

@@ -790,6 +790,53 @@ int gpdb_debug_path_counts(gpdb_ctx *ctx, uint64_t counts_out[16]);
 int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n, float *pool1_out, double *pool2_out,
                             float *ip1_out, float *logits_out);
 
+/* ---- Training the classifier on the device (rules in include/gpd_b200_train.h) ------------------------------------------
+ * The context's network (image_num_channels, relu_after_conv, image_size 60) trained in float32 on the CUDA cores: the
+ * forward pass is gpdb_classify's with lenet_impl = 1, bit for bit. Training keeps its own weights: gpdb_classify uses
+ * the loaded ones until the caller passes gpdb_train_weights to gpdb_set_weights. */
+typedef struct gpdb_train_params {
+  int32_t optimizer;                /* 0 = SGD (torch.optim.SGD, dampening 0), 1 = Adam (torch.optim.Adam, L2 decay) */
+  float lr, momentum, weight_decay; /* momentum: SGD only */
+  float beta1, beta2, eps;          /* Adam only */
+} gpdb_train_params;
+/* Starts (or restarts) training: init = the eight arrays in the gpdb_set_weights layout, or NULL for the context's loaded
+ * weights (GPDB_ERR_STATE if none). Zeroes the optimiser state and the step count. Bad params (unknown optimizer, a
+ * non-finite or negative lr / momentum / weight_decay / eps, betas outside [0, 1)) or a NULL array: GPDB_ERR_INVALID,
+ * nothing changed. */
+int gpdb_train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]);
+/* One optimiser step on the mean cross-entropy of n >= 1 images (HWC uint8, as gpdb_classify) and labels in {0, 1}; the
+ * step's loss to *loss_out (may be NULL). Before gpdb_train_begin: GPDB_ERR_STATE. n <= 0, a NULL array, image_size other
+ * than 60 or a label outside {0, 1} (checked on the device, the message names the first): GPDB_ERR_INVALID. A failed step
+ * changes neither the weights, nor the optimiser state, nor the step count. */
+int gpdb_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n, float *loss_out);
+/* gpdb_train_step on device arrays; d_loss_out (may be NULL) is a device float. */
+int gpdb_train_step_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, const int32_t *d_labels, int32_t n,
+                           float *d_loss_out);
+/* The current trained weights, in the .bin layout (what gpdb_set_weights reads), to eight host arrays. */
+int gpdb_train_weights(gpdb_ctx *ctx, float *const out[8]);
+/* Writes {conv1,conv2,ip1,ip2}_{weights,biases}.bin into the directory dir (which must exist; a trailing '/' is optional):
+ * what gpdb_load_weights_dir and the reference's EigenClassifier read. Host only. channels other than 1, 3, 12, 15
+ * or a NULL argument: GPDB_ERR_INVALID; a file that cannot be written: GPDB_ERR_IO. */
+int gpdb_write_weights_dir(const char *dir, int32_t channels, const float *const w[8]);
+/* Development aid, like gpdb_debug_lenet_layers: one step's forward state, backward intermediates and gradients, nothing
+ * updated. n in 1..GPDB_TRAIN_CHUNK (include/gpd_b200_train.h); every output host memory, any of them NULL. */
+typedef struct gpdb_train_debug {
+  float *pool1;      /* [n][20][28][28]  as gpdb_debug_lenet_layers */
+  float *pool2;      /* [n][7200]        k = c + 50 j */
+  float *ip1;        /* [n][500] */
+  float *logits;     /* [n][2] */
+  uint8_t *choice1;  /* [n][20][28][28]  pooling choice of each pool1 value, 0..3 in row-major window order */
+  uint8_t *choice2;  /* [n][7200]        ... of each pool2 value, k = c + 50 j */
+  float *loss;       /* [n]              per-image losses */
+  float *dlogits;    /* [n][2] */
+  float *dip1;       /* [n][500]         d ip1 output, ReLU mask applied */
+  float *dpool2;     /* [n][7200]        d pool2 (before its mask), k = c + 50 j */
+  float *dpool1;     /* [n][20][28][28]  d pool1 (before its mask) */
+  float *grad[8];    /* the eight gradients, .bin layouts */
+} gpdb_train_debug;
+int gpdb_debug_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n,
+                          gpdb_train_debug *out);
+
 /* Version / build info string (arch, lenet implementation). */
 const char *gpdb_build_info(void);
 
