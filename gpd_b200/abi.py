@@ -270,6 +270,10 @@ PROTOTYPES = {
     "gpdb_remove_outliers_clouds": (_int, [_vp, _i32, C.c_double, _vp, _vp, _vp]),
     "gpdb_subsample_clouds_points": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
     "gpdb_subsample_clouds_points_device": (_int, [_vp, _i32, C.c_uint64, _vp, _vp, _vp]),
+    "gpdb_render_depth": (_int, [_vp, _i32] + [_vp] * 5 + [_vp, _i32, _vp, _vp]),
+    "gpdb_render_depth_device": (_int, [_vp, _i32] + [_vp] * 5 + [_vp, _i32, _vp, _vp]),
+    "gpdb_sample_meshes": (_int, [_vp, _i32] + [_vp] * 4 + [C.c_double, C.c_uint64] + [_vp] * 4),
+    "gpdb_sample_meshes_device": (_int, [_vp, _i32] + [_vp] * 4 + [C.c_double, C.c_uint64] + [_vp] * 4),
     "gpdb_free_result": (None, [_res]),
     "gpdb_comm_unique_id": (_int, [_vp]),
     "gpdb_comm_init": (_int, [_vp, _vp, _i32, _i32]),

@@ -1579,25 +1579,11 @@ int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t 
 
 // ---- depth images and Cloud::subsample (include/gpd_b200_depth.h) ------------------------------------------------------
 
-// the argument checks of gpdb_preprocess_depth[_device]; roff[B+1] receives the raw offsets (cumulative pixels per view)
-static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
-                            int32_t format, const void *depth, const gpdb_preprocess_params *pp, const int32_t *poff,
-                            std::vector<int> &roff) {
-  if (B <= 0 || !n_cameras || !cams || !depth || !pp || !poff) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth, params, processed_offsets_out",
-                   name);
-    return GPDB_ERR_INVALID;
-  }
-  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
-    return GPDB_ERR_INVALID;
-  }
-  if (!pp->estimate_normals) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
-    return GPDB_ERR_INVALID;
-  }
-  const int rc = check_preprocess_params(ctx, name, pp, nullptr);
-  if (rc != GPDB_OK) return rc;
+// The camera checks of gpdb_preprocess_depth[_device] and gpdb_render_depth[_device]: view b has n_cameras[b] (1..8)
+// cameras, each of them well formed, and the call holds fewer than 2^31 pixels; roff[B+1] receives the raw offsets
+// (cumulative pixels per view)
+static int check_depth_cameras(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras,
+                               const gpdb_depth_camera *cams, std::vector<int> &roff) {
   roff.assign((size_t)B + 1, 0);
   long long total = 0;
   for (int b = 0, c = 0; b < B; b++) {
@@ -1630,6 +1616,28 @@ static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const in
     roff[b + 1] = (int)total;
   }
   return GPDB_OK;
+}
+
+// the argument checks of gpdb_preprocess_depth[_device]; roff[B+1] receives the raw offsets (cumulative pixels per view)
+static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                            int32_t format, const void *depth, const gpdb_preprocess_params *pp, const int32_t *poff,
+                            std::vector<int> &roff) {
+  if (B <= 0 || !n_cameras || !cams || !depth || !pp || !poff) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth, params, processed_offsets_out",
+                   name);
+    return GPDB_ERR_INVALID;
+  }
+  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
+    return GPDB_ERR_INVALID;
+  }
+  if (!pp->estimate_normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
+    return GPDB_ERR_INVALID;
+  }
+  const int rc = check_preprocess_params(ctx, name, pp, nullptr);
+  if (rc != GPDB_OK) return rc;
+  return check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
 }
 
 // gpdb_preprocess_depth[_device] after the argument checks: d_depth in device memory (the host twin has uploaded it)
@@ -1766,6 +1774,180 @@ static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples,
   return n;
 }
 
+// ---- triangle meshes: depth images and surface samples (include/gpd_b200_render.h) ----------------------------------
+
+// the offsets of B meshes (rule 7): vertex_offsets and face_offsets start at 0 and never decrease, and the arrays they
+// address are given; `unit` names a mesh in the messages
+static int check_mesh_args(gpdb_ctx *ctx, const char *name, const char *unit, int32_t B, const int32_t *voff,
+                           const float *vertices, const int32_t *foff, const int32_t *faces) {
+  int rc = check_offsets(ctx, name, "vertex_offsets", voff, B, unit);
+  if (rc == GPDB_OK) rc = check_offsets(ctx, name, "face_offsets", foff, B, unit);
+  if (rc != GPDB_OK) return rc;
+  if ((voff[B] > 0 && !vertices) || (foff[B] > 0 && !faces)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null vertices or faces for %d vertices and %d faces", name, voff[B], foff[B]);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// rule 7's device checks of B meshes in device memory: a non-finite vertex or a face index outside its mesh's vertices,
+// the first of them named
+static int check_meshes(gpdb_ctx *ctx, const char *name, const char *unit, int B, const int32_t *voff, const int32_t *foff,
+                        const float *d_vtx, const int32_t *d_faces) {
+  const int V = voff[B], F = foff[B];
+  const size_t bytes = sizeof(int) * 2 * ((size_t)B + 1);
+  unsigned long long bad;
+  const int rc = first_bad(ctx, bytes, &bad, [&](unsigned long long *d_bad, void *d) -> int {
+    int *d_voff = (int *)d, *d_foff = d_voff + B + 1;
+    CUDA_TRY(cudaMemcpyAsync(d_voff, voff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(d_foff, foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+    return mesh_check(ctx, d_voff, d_foff, B, V, F, d_vtx, d_faces, d_bad);
+  });
+  if (rc != GPDB_OK || bad == NO_BAD) return rc;
+  int b = 0;
+  if (bad < (unsigned long long)V) {
+    while (voff[b + 1] <= (long long)bad) b++;
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: vertex %d has a non-finite coordinate", name, unit, b,
+                   (int)(bad - voff[b]));
+    return GPDB_ERR_INVALID;
+  }
+  const int f = (int)(bad - V);
+  while (foff[b + 1] <= f) b++;
+  int32_t tri[3];
+  CUDA_TRY(cudaMemcpyAsync(tri, d_faces + 3 * (size_t)f, sizeof(tri), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: face %d = (%d, %d, %d) indexes outside its %d vertices", name, unit, b,
+                 f - foff[b], tri[0], tri[1], tri[2], voff[b + 1] - voff[b]);
+  return GPDB_ERR_INVALID;
+}
+
+// gpdb_render_depth[_device]: the checks, then the device render (the host twin uploads the meshes into SCR_UPLOAD, renders
+// into it and copies the images back). Nothing installed changes.
+static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
+                        const int32_t *foff, const int32_t *faces, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                        int32_t format, void *depth_out, int32_t *face_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !n_cameras || !cams || !depth_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
+    return GPDB_ERR_INVALID;
+  }
+  std::vector<int> roff;
+  int rc = check_mesh_args(ctx, name, "view", B, voff, vertices, foff, faces);
+  if (rc == GPDB_OK) rc = check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
+  if (rc == GPDB_OK && device)
+    rc = check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_depth_out", depth_out},
+                                       {"d_face_out", face_out}});
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const size_t V = (size_t)voff[B], F = (size_t)foff[B], M = (size_t)roff[B];
+  const size_t elt = format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float);
+  const float *d_vtx = vertices;
+  const int32_t *d_faces = faces;
+  void *d_depth = depth_out;
+  int32_t *d_face = face_out;
+  if (!device) {
+    float *v;
+    int32_t *f;
+    unsigned char *dd;
+    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
+          v = c.take<float>(3 * V);
+          f = c.take<int32_t>(3 * F);
+          dd = c.take<unsigned char>(elt * M, 16);
+          d_face = face_out ? c.take<int32_t>(M) : nullptr;
+        }))
+      return GPDB_ERR_CUDA;
+    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
+    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
+    d_vtx = v, d_faces = f, d_depth = dd;
+  }
+  if ((rc = check_meshes(ctx, name, "view", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
+  rc = render_depth_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face);
+  if (rc != GPDB_OK) return rc;
+  if (!device) {
+    CUDA_TRY(cudaMemcpyAsync(depth_out, d_depth, elt * M, cudaMemcpyDeviceToHost, ctx->stream));
+    if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  return B;
+}
+
+// gpdb_sample_meshes[_device]: the checks, the count, then (xyz_out given) the points. The host twin uploads the meshes
+// into SCR_UPLOAD, and once the count is known carves the outputs behind them there (uploading again: a grown slot
+// starts empty). Nothing installed changes.
+static int sample_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
+                        const int32_t *foff, const int32_t *faces, double density, uint64_t seed, int32_t *poff_out,
+                        float *xyz_out, double *normals_out, int32_t *face_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !poff_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_meshes > 0 and point_offsets_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  if (!(density > 0.0) || !std::isfinite(density)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: density must be finite and > 0 (got %g)", name, density);
+    return GPDB_ERR_INVALID;
+  }
+  int rc = check_mesh_args(ctx, name, "mesh", B, voff, vertices, foff, faces);
+  if (rc == GPDB_OK && device)
+    rc = check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_xyz_out", xyz_out},
+                                       {"d_normals_out", normals_out}, {"d_face_out", face_out}});
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const size_t V = (size_t)voff[B], F = (size_t)foff[B];
+  const float *d_vtx = vertices;
+  const int32_t *d_faces = faces;
+  float *d_xyz = xyz_out;
+  double *d_nrm = normals_out;
+  int32_t *d_face = face_out;
+  // the host twin's buffers: the meshes, then n points of the outputs the caller asked for
+  auto upload = [&](size_t n) -> int {
+    float *v;
+    int32_t *f;
+    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
+          v = c.take<float>(3 * V);
+          f = c.take<int32_t>(3 * F);
+          d_xyz = c.take<float>(3 * n);
+          d_nrm = normals_out ? c.take<double>(3 * n) : nullptr;
+          d_face = face_out ? c.take<int32_t>(n) : nullptr;
+        }))
+      return GPDB_ERR_CUDA;
+    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
+    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
+    d_vtx = v, d_faces = f;
+    return GPDB_OK;
+  };
+  if (!device && (rc = upload(0)) != GPDB_OK) return rc;
+  if ((rc = check_meshes(ctx, name, "mesh", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
+  std::vector<int> poff((size_t)B + 1);
+  std::vector<long long> mesh_n((size_t)B);
+  const long long n = mesh_count_batch(ctx, B, voff, foff, d_vtx, d_faces, density, seed, poff.data(), mesh_n.data());
+  if (n < 0) return (int)n;
+  if (n >= (1ll << 31)) {
+    long long run = 0;
+    int b = 0;
+    while ((run += mesh_n[b]) < (1ll << 31)) b++;
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mesh %d: the call reaches 2^31 or more sampled points (lower the density)",
+                   name, b);
+    return GPDB_ERR_INVALID;
+  }
+  if (xyz_out && n > 0) {
+    if (!device && (rc = upload((size_t)n)) != GPDB_OK) return rc;
+    if ((rc = mesh_write_batch(ctx, B, foff, d_vtx, d_faces, seed, (int)n, d_xyz, d_nrm, d_face)) != GPDB_OK) return rc;
+    if (!device) {
+      CUDA_TRY(cudaMemcpyAsync(xyz_out, d_xyz, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+      if (normals_out)
+        CUDA_TRY(cudaMemcpyAsync(normals_out, d_nrm, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+      if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+  }
+  memcpy(poff_out, poff.data(), sizeof(int32_t) * ((size_t)B + 1));
+  return (int)n;
+}
+
 extern "C" {
 
 int gpdb_preprocess_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
@@ -1832,6 +2014,35 @@ int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint
                                         int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
   return subsample_entry(ctx, "gpdb_subsample_clouds_points_device", num_samples, seed, d_point_mask, d_sample_idx_out,
                          sample_offsets_out, true, true);
+}
+
+int gpdb_render_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                      const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                      const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out) {
+  return render_entry(ctx, "gpdb_render_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras,
+                      depth_format, depth_out, face_out, false);
+}
+
+int gpdb_render_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                             const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                             int32_t *d_face_out) {
+  return render_entry(ctx, "gpdb_render_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces, n_cameras,
+                      cameras, depth_format, d_depth_out, d_face_out, true);
+}
+
+int gpdb_sample_meshes(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *vertices,
+                       const int32_t *face_offsets, const int32_t *faces, double density, uint64_t seed,
+                       int32_t *point_offsets_out, float *xyz_out, double *normals_out, int32_t *face_out) {
+  return sample_entry(ctx, "gpdb_sample_meshes", n_meshes, vertex_offsets, vertices, face_offsets, faces, density, seed,
+                      point_offsets_out, xyz_out, normals_out, face_out, false);
+}
+
+int gpdb_sample_meshes_device(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *d_vertices,
+                              const int32_t *face_offsets, const int32_t *d_faces, double density, uint64_t seed,
+                              int32_t *point_offsets_out, float *d_xyz_out, double *d_normals_out, int32_t *d_face_out) {
+  return sample_entry(ctx, "gpdb_sample_meshes_device", n_meshes, vertex_offsets, d_vertices, face_offsets, d_faces, density,
+                      seed, point_offsets_out, d_xyz_out, d_normals_out, d_face_out, true);
 }
 
 }  // extern "C"

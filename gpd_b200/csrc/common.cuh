@@ -269,6 +269,10 @@ enum ScratchSlot {
   // gpdb_train_step[_device] / gpdb_debug_train_step: one chunk's forward state, backward intermediates and per-image
   // gradient partials (train.cu, train_scratch_bytes)
   SCR_TRAIN,
+  // gpdb_render_depth[_device]: one group of cameras at a time, its camera table, camera-frame vertices, face records,
+  // tile rectangles, running minimum and per-tile lists; gpdb_sample_meshes[_device]: the offsets, counts and their scan
+  // (render.cu)
+  SCR_RENDER,
   SCR_N
 };
 
@@ -583,6 +587,24 @@ int org_depth_normals(gpdb_ctx *ctx, const char *name, CloudSet &s, const void *
                       const gpdb_depth_camera *cams, const int *n_cameras, int B, int *n_fallback);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
+
+// render.cu (include/gpd_b200_render.h). B views (mesh b: vertices voff[b] .. voff[b+1]-1 of d_vtx, faces foff[b] ..
+// foff[b+1]-1 of d_faces, host offsets, checked) rendered by their n_cameras[b] cameras cams into d_depth (format) and
+// d_face (may be null), device arrays in the layout of gpdb_preprocess_depth.
+int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                       const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face);
+// rule 6's counts of B checked meshes: returns the total (an error when negative) and mesh_n[B] (host) each mesh's
+// count (each face's count clamped to 2^31); when the total is below 2^31, poff[B+1] (host) receives the point offsets
+// and SCR_RENDER keeps the per-face scan for mesh_write_batch
+long long mesh_count_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                           double density, unsigned long long seed, int *poff, long long *mesh_n);
+// the N points mesh_count_batch counted (the same meshes and seed): xyz, normals and faces (each but xyz may be null)
+int mesh_write_batch(gpdb_ctx *ctx, int B, const int *foff, const float *d_vtx, const int *d_faces, unsigned long long seed,
+                     int N, float *d_xyz, double *d_nrm, int *d_face);
+// rule 7's mesh checks (offsets d_voff / d_foff on the device): lowers *d_first_bad to the first vertex i with a
+// non-finite coordinate (position i) or face f with an index outside its view's vertices (position V + f)
+int mesh_check(gpdb_ctx *ctx, const int *d_voff, const int *d_foff, int B, int V, int F, const float *d_vtx,
+               const int *d_faces, unsigned long long *d_first_bad);
 
 // lenet_simt.cu
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);

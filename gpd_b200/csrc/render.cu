@@ -1,0 +1,487 @@
+// render.cu — depth images of triangle-mesh scenes and surface samples of the same meshes (include/gpd_b200_render.h):
+// gpdb_render_depth[_device] and gpdb_sample_meshes[_device].
+//
+// Rendering, per group of cameras:
+//   k_rnd_xform    one float64 camera-frame copy per (camera, vertex) (rule 2)
+//   k_rnd_setup    m0..m2, n and h once per (camera, face) (rule 4), and the screen tiles the face's conservative pixel
+//                  bounds touch
+//   k_rnd_bin      the (face, tile) pairs counted per tile, then, after an exact scan, filled into per-tile lists with
+//                  integer atomics: the list order is arbitrary, the resolve does not depend on it
+//   k_rnd_resolve  one CTA per (camera, tile), one thread per pixel: the lexicographic minimum of (t, face) over the
+//                  tile's list (rule 5), then the depth and face images
+// The cameras of a call are processed in groups whose per-camera arrays fit RND_GROUP_BYTES; a group's (face, tile)
+// pairs are resolved in chunks of at most the carved list length, the running minimum kept per pixel between chunks, so a
+// face covering every tile (a table) costs one list entry per tile and memory stays bounded.
+//
+// Sampling: k_mesh_count per face (rule 6's count, a 64-bit total), scan_flags over the counts once the total is known
+// to lie below 2^31, then k_mesh_write per point. Scratch: SCR_RENDER. Compiled with -fmad=false: every float64
+// operation is rounded on its own.
+#include <algorithm>
+#include <climits>
+#include <vector>
+
+#include "../../include/gpd_b200_render.h"
+#include "common.cuh"
+
+namespace {
+
+constexpr int RND_TILE = 16;                                 // tile edge in pixels: one thread per pixel
+constexpr int RND_THREADS = RND_TILE * RND_TILE;
+constexpr int RND_STAGE = 64;                                // face records a resolve CTA stages in shared memory at once
+constexpr size_t RND_GROUP_BYTES = size_t(256) << 20;        // per-camera arrays of one group
+constexpr long long RND_LIST_CAP = 32ll << 20;               // (face, tile) entries one chunk may hold
+constexpr double RND_PROJ_LIMIT = 16777216.0;                // 2^24: projected bounds beyond this take every tile
+
+// One camera of a group. Its vertices are xv .. xv + nv - 1 of the group's camera-frame vertices, its faces the items
+// item .. item + nf - 1, its tiles tile .. tile + tx*ty - 1; pix is its first pixel in the call's images.
+struct RndCam {
+  double pose[12];
+  double fx, fy, cx, cy, scale;
+  int W, H, tx, ty;
+  int vbase, nv, fbase, nf;
+  int xv, item, tile, pad;
+  long long pix;
+};
+
+// rule 2: q[i] for every (camera, vertex) of the group; xv_off[G+1] the cameras' first entries
+__global__ void k_rnd_xform(const RndCam *cams, const int *xv_off, int G, int n, const float *vtx, double *q) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const RndCam &c = cams[csr_owner(xv_off, G, i)];
+  const long long v = (long long)c.vbase + (i - c.xv);
+  const float p[3] = {vtx[3 * v], vtx[3 * v + 1], vtx[3 * v + 2]};
+  double o[3];
+  gpdb_render_to_camera(c.pose, p, o);
+  q[3 * (size_t)i] = o[0];
+  q[3 * (size_t)i + 1] = o[1];
+  q[3 * (size_t)i + 2] = o[2];
+}
+
+// The tiles a face may cover, inclusive, as (tx0, ty0, tx1, ty1); tx0 > tx1: none. Every tile of the image when a vertex
+// lies at or behind the camera plane, a projected bound is not finite or beyond 2^24 pixels, or an edge runs so close to
+// a ray through the eye that its m is within rounding of zero. Otherwise the projected bounding box grown by one pixel:
+// the coverage test of rule 4 is exact up to float64 roundings, many orders of magnitude below a pixel there.
+__device__ int4 rnd_tiles(const RndCam &c, const double *A, const double *B, const double *C, const double *rec) {
+  const int4 all = make_int4(0, 0, c.tx - 1, c.ty - 1);
+  const int4 none = make_int4(1, 0, 0, 0);
+  if (rec[9] == 0.0 && rec[10] == 0.0 && rec[11] == 0.0) return none;  // n = 0: s = 0 for every ray
+  const double *V[3] = {A, B, C};
+  double umin = INFINITY, umax = -INFINITY, vmin = INFINITY, vmax = -INFINITY;
+  for (int k = 0; k < 3; k++) {
+    const double *P = V[k], *Q = V[(k + 1) % 3], *m = rec + 3 * k;
+    if (!(P[2] > 0.0)) return all;
+    const double pm = fmax(fabs(P[0]), fmax(fabs(P[1]), fabs(P[2]))), qm = fmax(fabs(Q[0]), fmax(fabs(Q[1]), fabs(Q[2])));
+    const double mm = fmax(fabs(m[0]), fmax(fabs(m[1]), fabs(m[2])));
+    if (!(mm > 1.4901161193847656e-8 * (pm * qm))) return all;  // 2^-26
+    const double u = c.cx + c.fx * (P[0] / P[2]), v = c.cy + c.fy * (P[1] / P[2]);
+    umin = fmin(umin, u);
+    umax = fmax(umax, u);
+    vmin = fmin(vmin, v);
+    vmax = fmax(vmax, v);
+  }
+  if (!(fabs(umin) < RND_PROJ_LIMIT && fabs(umax) < RND_PROJ_LIMIT && fabs(vmin) < RND_PROJ_LIMIT &&
+        fabs(vmax) < RND_PROJ_LIMIT))
+    return all;
+  const int u0 = max((int)floor(umin) - 1, 0), u1 = min((int)ceil(umax) + 1, c.W - 1);
+  const int v0 = max((int)floor(vmin) - 1, 0), v1 = min((int)ceil(vmax) + 1, c.H - 1);
+  if (u0 > u1 || v0 > v1) return none;
+  return make_int4(u0 / RND_TILE, v0 / RND_TILE, u1 / RND_TILE, v1 / RND_TILE);
+}
+
+// rule 4's setup of every (camera, face) item of the group, its tile rectangle and its (face, tile) pairs; *pairs (zeroed
+// by the caller) receives their sum
+__global__ void k_rnd_setup(const RndCam *cams, const int *item_off, int G, int n, const int *faces, const double *q,
+                            double *rec, int4 *rect, int *count, unsigned long long *pairs) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const RndCam &c = cams[csr_owner(item_off, G, i)];
+  const long long f = (long long)c.fbase + (i - c.item);
+  const double *A = q + 3 * ((size_t)c.xv + faces[3 * f]);
+  const double *B = q + 3 * ((size_t)c.xv + faces[3 * f + 1]);
+  const double *C = q + 3 * ((size_t)c.xv + faces[3 * f + 2]);
+  double r[GPDB_RENDER_REC];
+  gpdb_render_setup(A, B, C, r);
+  for (int k = 0; k < GPDB_RENDER_REC; k++) rec[(size_t)GPDB_RENDER_REC * i + k] = r[k];
+  const int4 t = rnd_tiles(c, A, B, C, r);
+  rect[i] = t;
+  const int cnt = t.x > t.z ? 0 : (t.z - t.x + 1) * (t.w - t.y + 1);
+  count[i] = cnt;
+  if (cnt) atomicAdd(pairs, (unsigned long long)cnt);
+}
+
+// the (face, tile) pairs of items i0 .. i1-1: fill = false counts them per tile (cnt); fill = true writes item i into
+// tile t's list at pos[t] + atomicAdd(cnt[t], 1), cnt zeroed again by the caller
+__global__ void k_rnd_bin(const RndCam *cams, const int *item_off, int G, int i0, int i1, const int4 *rect, int *cnt,
+                          const int *pos, int *list, bool fill) {
+  const int i = i0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= i1) return;
+  const RndCam &c = cams[csr_owner(item_off, G, i)];
+  const int4 r = rect[i];
+  for (int y = r.y; y <= r.w; y++)
+    for (int x = r.x; x <= r.z; x++) {
+      const int t = c.tile + y * c.tx + x;
+      const int k = atomicAdd(cnt + t, 1);
+      if (fill) list[pos[t] + k] = i;
+    }
+}
+
+// One CTA per tile of the group: each thread keeps the lexicographic minimum of (t, face) of its pixel over the tile's
+// list, starting from none (first chunk) or from the running minimum (best_t / best_f), and writes either the running
+// minimum back or, after the last chunk, the depth and face images (rule 5).
+__global__ void __launch_bounds__(RND_THREADS) k_rnd_resolve(const RndCam *cams, const int *tile_off, int G,
+                                                             const double *rec, const int *pos, const int *list,
+                                                             bool first, bool last, double *best_t, int *best_f,
+                                                             const long long *pix_off, int format, void *depth,
+                                                             int *face_out) {
+  __shared__ double s_rec[RND_STAGE][GPDB_RENDER_REC];
+  __shared__ int s_face[RND_STAGE];
+  const int tile = blockIdx.x;
+  const int g = csr_owner(tile_off, G, tile);
+  const RndCam &c = cams[g];
+  const int lt = tile - c.tile;
+  const int u = (lt % c.tx) * RND_TILE + threadIdx.x % RND_TILE, v = (lt / c.tx) * RND_TILE + threadIdx.x / RND_TILE;
+  const bool in = u < c.W && v < c.H;
+  const long long gp = pix_off[g] + (long long)v * c.W + u;  // the pixel in the group's running minimum
+  double d[2];
+  gpdb_render_ray(u, v, c.fx, c.fy, c.cx, c.cy, d);
+  double bt = INFINITY;
+  int bf = -1;
+  if (!first && in) {
+    bt = best_t[gp];
+    bf = best_f[gp];
+  }
+  const int e0 = pos[tile], e1 = pos[tile + 1];
+  for (int base = e0; base < e1; base += RND_STAGE) {
+    const int m = min(RND_STAGE, e1 - base);
+    __syncthreads();
+    for (int k = threadIdx.x; k < m * GPDB_RENDER_REC; k += RND_THREADS) {
+      const int r = k / GPDB_RENDER_REC, w = k % GPDB_RENDER_REC;
+      s_rec[r][w] = rec[(size_t)GPDB_RENDER_REC * list[base + r] + w];
+    }
+    for (int k = threadIdx.x; k < m; k += RND_THREADS) s_face[k] = list[base + k] - c.item;
+    __syncthreads();
+    if (in)
+      for (int k = 0; k < m; k++) {
+        double t;
+        if (gpdb_render_hit(s_rec[k], d[0], d[1], &t) && (t < bt || (t == bt && s_face[k] < bf))) {
+          bt = t;
+          bf = s_face[k];
+        }
+      }
+  }
+  if (!in) return;
+  if (!last) {
+    best_t[gp] = bt;
+    best_f[gp] = bf;
+    return;
+  }
+  const long long o = c.pix + (long long)v * c.W + u;
+  bool ret = false;
+  const uint32_t raw = bf >= 0 ? gpdb_render_raw(bt, c.scale, format, &ret) : 0u;
+  if (format == GPDB_DEPTH_F32) static_cast<uint32_t *>(depth)[o] = raw;
+  else static_cast<uint16_t *>(depth)[o] = (uint16_t)raw;
+  if (face_out) face_out[o] = ret ? bf : -1;
+}
+
+// the cameras [first, last) of one group and their sizes
+struct RndGroup {
+  int first, last;
+  long long verts, items, pixels, tiles, pairs_max;  // pairs_max: the most (face, tile) pairs its faces can make
+};
+
+size_t rnd_camera_bytes(long long nv, long long nf, long long px, long long tiles) {
+  return nv * 3 * sizeof(double) + nf * (GPDB_RENDER_REC * sizeof(double) + sizeof(int4) + sizeof(int)) +
+         px * (sizeof(double) + sizeof(int)) + tiles * 2 * sizeof(int);
+}
+
+// The scratch of one group, sized for the largest: camera table, offsets, camera-frame vertices, face records, tile
+// rectangles and pair counts, the running minimum, the tile counts and positions, the pair total and the lists
+struct RndScratch {
+  RndCam *cams;
+  int *xv_off, *item_off, *tile_off;
+  long long *pix_off;
+  double *q, *rec, *best_t;
+  int4 *rect;
+  int *count, *best_f, *tcnt, *tpos, *list;
+  unsigned long long *pairs;
+};
+
+}  // namespace
+
+int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                       const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face) {
+  // the cameras of the call, view by view
+  int C = 0;
+  for (int b = 0; b < B; b++) C += n_cameras[b];
+  std::vector<RndCam> rc((size_t)C);
+  long long pix = 0;
+  for (int b = 0, k = 0; b < B; b++)
+    for (int j = 0; j < n_cameras[b]; j++, k++) {
+      const gpdb_depth_camera &D = cams[k];
+      RndCam &c = rc[k];
+      memset(&c, 0, sizeof(c));
+      for (int e = 0; e < 12; e++) c.pose[e] = D.pose[e];
+      c.fx = D.fx, c.fy = D.fy, c.cx = D.cx, c.cy = D.cy, c.scale = D.depth_scale;
+      c.W = D.width, c.H = D.height;
+      c.tx = (D.width + RND_TILE - 1) / RND_TILE, c.ty = (D.height + RND_TILE - 1) / RND_TILE;
+      c.vbase = voff[b], c.nv = voff[b + 1] - voff[b], c.fbase = foff[b], c.nf = foff[b + 1] - foff[b];
+      c.pix = pix;
+      pix += (long long)D.width * D.height;
+    }
+  // consecutive cameras, each group's per-camera arrays within RND_GROUP_BYTES (a larger camera is a group of its own)
+  std::vector<RndGroup> groups;
+  RndGroup cur{0, 0, 0, 0, 0, 0, 0};
+  for (int k = 0; k < C; k++) {
+    const RndCam &c = rc[k];
+    const long long px = (long long)c.W * c.H, tl = (long long)c.tx * c.ty;
+    if (cur.last > cur.first &&
+        rnd_camera_bytes(cur.verts + c.nv, cur.items + c.nf, cur.pixels + px, cur.tiles + tl) > RND_GROUP_BYTES) {
+      groups.push_back(cur);
+      cur = RndGroup{k, k, 0, 0, 0, 0, 0};
+    }
+    cur.last = k + 1;
+    cur.verts += c.nv, cur.items += c.nf, cur.pixels += px, cur.tiles += tl;
+    cur.pairs_max += (long long)c.nf * tl;
+  }
+  groups.push_back(cur);
+  long long g_max = 0, v_max = 0, i_max = 0, p_max = 0, t_max = 0, cap = 0;
+  for (const RndGroup &G : groups) {
+    g_max = std::max(g_max, (long long)(G.last - G.first));
+    v_max = std::max(v_max, G.verts), i_max = std::max(i_max, G.items);
+    p_max = std::max(p_max, G.pixels), t_max = std::max(t_max, G.tiles);
+    cap = std::max(cap, std::min(G.pairs_max, RND_LIST_CAP));
+  }
+  for (const RndCam &c : rc) cap = std::max(cap, (long long)c.tx * c.ty);  // one face's pairs always fit a chunk
+  if (v_max * 3 >= INT_MAX || i_max >= INT_MAX / GPDB_RENDER_REC || t_max >= INT_MAX) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_render_depth: a camera of %lld vertices, %lld faces and %lld tiles exceeds "
+                   "the int32 ranges of one group", v_max, i_max, t_max);
+    return GPDB_ERR_INVALID;
+  }
+  RndScratch s;
+  if (!gpdb_carve(ctx, SCR_RENDER, [&](Carve &c) {
+        s.cams = c.take<RndCam>(g_max);
+        s.xv_off = c.take<int>(g_max + 1);
+        s.item_off = c.take<int>(g_max + 1);
+        s.tile_off = c.take<int>(g_max + 1);
+        s.pix_off = c.take<long long>(g_max + 1);
+        s.q = c.take<double>(3 * v_max);
+        s.rec = c.take<double>(GPDB_RENDER_REC * i_max);
+        s.rect = c.take<int4>(i_max);
+        s.count = c.take<int>(i_max);
+        s.best_t = c.take<double>(p_max);
+        s.best_f = c.take<int>(p_max);
+        s.tcnt = c.take<int>(t_max + 1);
+        s.tpos = c.take<int>(t_max + 1);
+        s.pairs = c.take<unsigned long long>(1);
+        s.list = c.take<int>(cap);
+      }))
+    return GPDB_ERR_CUDA;
+  const int tb = 256;
+  for (const RndGroup &G : groups) {
+    const int n = G.last - G.first;
+    std::vector<RndCam> gc(rc.begin() + G.first, rc.begin() + G.last);
+    std::vector<int> xv((size_t)n + 1, 0), it((size_t)n + 1, 0), tl((size_t)n + 1, 0);
+    std::vector<long long> px((size_t)n + 1, 0);
+    for (int k = 0; k < n; k++) {
+      RndCam &c = gc[k];
+      c.xv = xv[k], c.item = it[k], c.tile = tl[k];
+      xv[k + 1] = xv[k] + c.nv;
+      it[k + 1] = it[k] + c.nf;
+      tl[k + 1] = tl[k] + c.tx * c.ty;
+      px[k + 1] = px[k] + (long long)c.W * c.H;
+    }
+    CUDA_TRY(cudaMemcpyAsync(s.cams, gc.data(), sizeof(RndCam) * n, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.xv_off, xv.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.item_off, it.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.tile_off, tl.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(s.pix_off, px.data(), sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemsetAsync(s.pairs, 0, sizeof(*s.pairs), ctx->stream));
+    const int NV = xv[n], NI = it[n], NT = tl[n];
+    if (NV > 0) {
+      k_rnd_xform<<<(NV + tb - 1) / tb, tb, 0, ctx->stream>>>(s.cams, s.xv_off, n, NV, d_vtx, s.q);
+      LAUNCH_CHECK();
+    }
+    if (NI > 0) {
+      k_rnd_setup<<<(NI + tb - 1) / tb, tb, 0, ctx->stream>>>(s.cams, s.item_off, n, NI, d_faces, s.q, s.rec, s.rect,
+                                                             s.count, s.pairs);
+      LAUNCH_CHECK();
+    }
+    unsigned long long pairs = 0;
+    CUDA_TRY(cudaMemcpyAsync(&pairs, s.pairs, sizeof(pairs), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    // chunks of consecutive items whose pairs fit the list: one chunk unless the group makes more than `cap` pairs
+    std::vector<int> cuts{0};
+    if ((long long)pairs > cap) {
+      std::vector<int> cnt((size_t)NI);
+      CUDA_TRY(cudaMemcpyAsync(cnt.data(), s.count, sizeof(int) * (size_t)NI, cudaMemcpyDeviceToHost, ctx->stream));
+      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+      long long run = 0;
+      for (int i = 0; i < NI; i++) {
+        if (run + cnt[i] > cap) {
+          cuts.push_back(i);
+          run = 0;
+        }
+        run += cnt[i];
+      }
+    }
+    cuts.push_back(NI);
+    for (size_t ch = 0; ch + 1 < cuts.size(); ch++) {
+      const int i0 = cuts[ch], i1 = cuts[ch + 1];
+      CUDA_TRY(cudaMemsetAsync(s.tcnt, 0, sizeof(int) * NT, ctx->stream));
+      if (i1 > i0) {
+        k_rnd_bin<<<(i1 - i0 + tb - 1) / tb, tb, 0, ctx->stream>>>(s.cams, s.item_off, n, i0, i1, s.rect, s.tcnt, nullptr,
+                                                                  nullptr, false);
+        LAUNCH_CHECK();
+      }
+      const int rc2 = scan_flags(ctx, s.tcnt, s.tpos, NT);
+      if (rc2 != GPDB_OK) return rc2;
+      CUDA_TRY(cudaMemsetAsync(s.tcnt, 0, sizeof(int) * NT, ctx->stream));
+      if (i1 > i0) {
+        k_rnd_bin<<<(i1 - i0 + tb - 1) / tb, tb, 0, ctx->stream>>>(s.cams, s.item_off, n, i0, i1, s.rect, s.tcnt, s.tpos,
+                                                                  s.list, true);
+        LAUNCH_CHECK();
+      }
+      k_rnd_resolve<<<NT, RND_THREADS, 0, ctx->stream>>>(s.cams, s.tile_off, n, s.rec, s.tpos, s.list, ch == 0,
+                                                         ch + 2 == cuts.size(), s.best_t, s.best_f, s.pix_off, format,
+                                                         d_depth, d_face);
+      LAUNCH_CHECK();
+    }
+  }
+  return GPDB_OK;
+}
+
+namespace {
+
+// rule 6's count of every face of the call (mesh b: faces foff[b] .. foff[b+1]-1, vertices from voff[b]); cnt[f] is the
+// count clamped to INT_MAX, total[b] (zeroed by the caller) the sum of mesh b's counts each clamped to 2^31, so the
+// totals reach 2^31 exactly when the call would hold 2^31 or more points
+__global__ void k_mesh_count(const int *voff, const int *foff, int B, int F, const float *vtx, const int *faces,
+                             double density, unsigned long long seed, int *cnt, unsigned long long *total) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const int b = csr_owner(foff, B, f);
+  const float *a = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f]);
+  const float *bb = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f + 1]);
+  const float *c = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f + 2]);
+  double n[3];
+  const double L = gpdb_mesh_face(a, bb, c, n);
+  const gpdb_u32x4 r = gpdb_mesh_draw(seed + (unsigned long long)b, (uint32_t)(f - foff[b]), 0u);
+  const double k = fmin(gpdb_mesh_count(L, density, gpdb_mesh_unit(r.x, r.y)), 2147483648.0);
+  cnt[f] = (int)fmin(k, 2147483647.0);
+  if (k > 0.0) atomicAdd(total + b, (unsigned long long)k);
+}
+
+// the points of the call: point i belongs to the face f with pos[f] <= i < pos[f+1] and is its point i - pos[f]
+__global__ void k_mesh_write(const int *voff, const int *foff, int B, int F, const float *vtx, const int *faces,
+                             unsigned long long seed, const int *pos, int N, float *xyz, double *nrm, int *face) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int f = csr_owner(pos, F, i);
+  const int b = csr_owner(foff, B, f);
+  const float *a = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f]);
+  const float *bb = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f + 1]);
+  const float *c = vtx + 3 * ((size_t)voff[b] + faces[3 * (size_t)f + 2]);
+  double n[3], p[3];
+  const double L = gpdb_mesh_face(a, bb, c, n);
+  const gpdb_u32x4 r = gpdb_mesh_draw(seed + (unsigned long long)b, (uint32_t)(f - foff[b]), (uint32_t)(i - pos[f] + 1));
+  gpdb_mesh_point(a, bb, c, gpdb_mesh_unit(r.x, r.y), gpdb_mesh_unit(r.z, r.w), p);
+  for (int k = 0; k < 3; k++) xyz[3 * (size_t)i + k] = (float)p[k];
+  if (nrm)
+    for (int k = 0; k < 3; k++) nrm[3 * (size_t)i + k] = n[k] / L;
+  if (face) face[i] = f - foff[b];
+}
+
+// the points offsets of the meshes: poff[b] = pos[foff[b]]
+__global__ void k_mesh_offsets(const int *pos, const int *foff, int B, int *poff) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b <= B) poff[b] = pos[foff[b]];
+}
+
+// SCR_RENDER of a sampling call: the offsets, the counts (scan_flags' flags), their scan and the total
+struct MeshScratch {
+  int *voff, *foff, *poff, *cnt, *pos;
+  unsigned long long *total;
+};
+
+bool mesh_carve(gpdb_ctx *ctx, int B, int F, MeshScratch &m) {
+  return gpdb_carve(ctx, SCR_RENDER, [&](Carve &c) {
+    m.voff = c.take<int>((size_t)B + 1);
+    m.foff = c.take<int>((size_t)B + 1);
+    m.poff = c.take<int>((size_t)B + 1);
+    m.cnt = c.take<int>((size_t)F + 1);
+    m.pos = c.take<int>((size_t)F + 1);
+    m.total = c.take<unsigned long long>(B);
+  });
+}
+
+}  // namespace
+
+long long mesh_count_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                           double density, unsigned long long seed, int *poff, long long *mesh_n) {
+  const int F = foff[B];
+  MeshScratch m;
+  if (!mesh_carve(ctx, B, F, m)) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemcpyAsync(m.voff, voff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(m.foff, foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemsetAsync(m.total, 0, sizeof(*m.total) * B, ctx->stream));
+  if (F > 0) {
+    k_mesh_count<<<(F + 255) / 256, 256, 0, ctx->stream>>>(m.voff, m.foff, B, F, d_vtx, d_faces, density, seed, m.cnt,
+                                                          m.total);
+    LAUNCH_CHECK();
+  }
+  CUDA_TRY(cudaMemcpyAsync(mesh_n, m.total, sizeof(long long) * B, cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  long long total = 0;
+  for (int b = 0; b < B; b++) total += mesh_n[b];
+  if (total >= (1ll << 31)) return total;  // the caller refuses the call; nothing was scanned
+  const int rc = scan_flags(ctx, m.cnt, m.pos, F);
+  if (rc != GPDB_OK) return rc;
+  k_mesh_offsets<<<(B + 1 + 255) / 256, 256, 0, ctx->stream>>>(m.pos, m.foff, B, m.poff);
+  LAUNCH_CHECK();
+  CUDA_TRY(cudaMemcpyAsync(poff, m.poff, sizeof(int) * ((size_t)B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return total;
+}
+
+int mesh_write_batch(gpdb_ctx *ctx, int B, const int *foff, const float *d_vtx, const int *d_faces, unsigned long long seed,
+                     int N, float *d_xyz, double *d_nrm, int *d_face) {
+  if (N == 0) return GPDB_OK;
+  MeshScratch m;
+  if (!mesh_carve(ctx, B, foff[B], m)) return GPDB_ERR_CUDA;  // the slot as mesh_count_batch left it
+  k_mesh_write<<<(N + 255) / 256, 256, 0, ctx->stream>>>(m.voff, m.foff, B, foff[B], d_vtx, d_faces, seed, m.pos, N, d_xyz,
+                                                        d_nrm, d_face);
+  LAUNCH_CHECK();
+  return GPDB_OK;
+}
+
+namespace {
+
+// rule 7's mesh checks: position i < V is vertex i (a non-finite coordinate), position V + f is face f (an index
+// outside its view's vertices)
+__global__ void k_mesh_check(const int *voff, const int *foff, int B, int V, int F, const float *vtx, const int *faces,
+                             unsigned long long *first_bad) {
+  const long long n = (long long)V + F;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (i < V) {
+      if (!isfinite(vtx[3 * i]) || !isfinite(vtx[3 * i + 1]) || !isfinite(vtx[3 * i + 2])) atomicMin(first_bad, i);
+      continue;
+    }
+    const int f = (int)(i - V), b = csr_owner(foff, B, f), nv = voff[b + 1] - voff[b];
+    for (int k = 0; k < 3; k++) {
+      const int v = faces[3 * (size_t)f + k];
+      if (v < 0 || v >= nv) atomicMin(first_bad, (unsigned long long)i);
+    }
+  }
+}
+
+}  // namespace
+
+int mesh_check(gpdb_ctx *ctx, const int *d_voff, const int *d_foff, int B, int V, int F, const float *d_vtx,
+               const int *d_faces, unsigned long long *d_first_bad) {
+  const long long n = (long long)V + F;
+  if (n == 0) return GPDB_OK;
+  const long long blocks = std::min((n + 255) / 256, (long long)ctx->sm_count * 16);
+  k_mesh_check<<<(int)blocks, 256, 0, ctx->stream>>>(d_voff, d_foff, B, V, F, d_vtx, d_faces, d_first_bad);
+  LAUNCH_CHECK();
+  return GPDB_OK;
+}

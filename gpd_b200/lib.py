@@ -162,6 +162,22 @@ def pack_clouds(clouds):
             "cam_source": cam, "n_cameras": ks, "view_points": np.ascontiguousarray(np.concatenate(vps))}
 
 
+def pack_meshes(meshes):
+    """The CSR arrays of gpdb_render_depth / gpdb_sample_meshes for a list of (vertices [V, 3], faces [F, 3]) meshes, faces
+    indexing their own mesh's vertices from 0: {"vertex_offsets" [B+1], "vertices" float32 [sum V, 3], "face_offsets"
+    [B+1], "faces" int32 [sum F, 3]}, each concatenated in mesh order."""
+    if not meshes:
+        raise ValueError("pack_meshes: need at least one mesh")
+    vs = [np.asarray(v, dtype=np.float32).reshape(-1, 3) for v, _ in meshes]
+    fs = [np.asarray(f, dtype=np.int32).reshape(-1, 3) for _, f in meshes]
+    voff = np.zeros(len(meshes) + 1, np.int32)
+    voff[1:] = np.cumsum([len(v) for v in vs])
+    foff = np.zeros(len(meshes) + 1, np.int32)
+    foff[1:] = np.cumsum([len(f) for f in fs])
+    return {"vertex_offsets": voff, "vertices": np.ascontiguousarray(np.concatenate(vs)),
+            "face_offsets": foff, "faces": np.ascontiguousarray(np.concatenate(fs))}
+
+
 def depth_camera(width, height, fx, fy, cx, cy, pose=None, depth_scale=0.001, min_depth=0.0, max_depth=float("inf")):
     """A gpdb_depth_camera (include/gpd_b200_depth.h): pinhole intrinsics in pixels, pose = camera-to-world [R | t] as a
     3 x 4 (or 4 x 4) array, identity when None; depth_scale in metres per stored unit (0.001 for uint16 millimetres, 1.0
@@ -693,6 +709,110 @@ class Context:
         ptr = _device_arg("d_depth", d_depth, dt, self.params.device, n)
         self._torch_stream()
         return fmt, ptr
+
+    # ---- triangle meshes (include/gpd_b200_render.h): depth images and surface samples; nothing is installed ----
+
+    def render_depth(self, meshes, cameras_per_view, dtype=np.float32, face_ids=False):
+        """gpdb_render_depth: depth images of mesh scenes. meshes: one (vertices [V, 3], faces [F, 3]) per view;
+        cameras_per_view: one list of depth_camera()s per view. dtype np.float32 (GPDB_DEPTH_F32) or np.uint16
+        (GPDB_DEPTH_U16). Returns one list of (image [height, width], camera) per view, what preprocess_depth() takes,
+        and with face_ids also one list of int32 face images per view (the view-local face each return hit, -1 where
+        the pixel has none)."""
+        fmt = {np.dtype(np.float32): abi.DEPTH_F32, np.dtype(np.uint16): abi.DEPTH_U16}.get(np.dtype(dtype))
+        if fmt is None:
+            raise TypeError(f"render_depth: dtype must be float32 or uint16, got {np.dtype(dtype)}")
+        if len(cameras_per_view) != len(meshes):
+            raise ValueError(f"cameras_per_view: {len(cameras_per_view)} lists, need one per mesh ({len(meshes)})")
+        m = pack_meshes(meshes)
+        ks, arr, _ = _depth_cameras([len(c) for c in cameras_per_view], [c for cs in cameras_per_view for c in cs])
+        cams = list(arr[:int(ks.sum())])
+        n = sum(int(c.width) * int(c.height) for c in cams)
+        depth = np.zeros(n, dtype)
+        face = np.zeros(n, np.int32) if face_ids else None
+        self._check(lib().gpdb_render_depth(self.h, len(ks), _p(m["vertex_offsets"]), _p(m["vertices"]),
+                                            _p(m["face_offsets"]), _p(m["faces"]), _p(ks), C.cast(arr, C.c_void_p), fmt,
+                                            _p(depth), _p(face)))
+        views, faces, o, k = [], [], 0, 0
+        for cs in cameras_per_view:
+            views.append([])
+            faces.append([])
+            for _ in cs:
+                c = cams[k]
+                h, w = int(c.height), int(c.width)
+                views[-1].append((depth[o:o + h * w].reshape(h, w), c))
+                faces[-1].append(None if face is None else face[o:o + h * w].reshape(h, w))
+                o, k = o + h * w, k + 1
+        return (views, faces) if face_ids else views
+
+    def render_depth_tensors(self, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras, dtype=None,
+                             face_ids=False):
+        """gpdb_render_depth_device: render_depth() of meshes held in CUDA tensors (vertices [V, 3] float32, faces
+        [F, 3] int32, concatenated as pack_meshes() lays them out; the offsets, n_cameras [B] and the sum(n_cameras)
+        cameras are host arrays). dtype torch.float32 (default) or torch.uint16. Returns ONE depth tensor holding every
+        camera's image back to back, as preprocess_depth_tensors() takes it, and with face_ids also the int32 face
+        tensor of the same length."""
+        import torch
+        dtype = torch.float32 if dtype is None else dtype
+        fmt = {torch.float32: abi.DEPTH_F32, torch.uint16: abi.DEPTH_U16}.get(dtype)
+        if fmt is None:
+            raise TypeError(f"render_depth_tensors: dtype must be torch.float32 or torch.uint16, got {dtype}")
+        voff, foff = _host_i32("vertex_offsets", vertex_offsets), _host_i32("face_offsets", face_offsets)
+        if len(voff) < 2 or len(foff) != len(voff):
+            raise ValueError(f"vertex_offsets / face_offsets: {len(voff)} / {len(foff)} entries, need B + 1 each (B >= 1)")
+        ks, arr, _ = _depth_cameras(n_cameras, cameras)
+        if len(ks) != len(voff) - 1:
+            raise ValueError(f"n_cameras: {len(ks)} entries, need one per view ({len(voff) - 1})")
+        dev = self.params.device
+        pv = _device_arg("vertices", vertices, torch.float32, dev, 3 * int(voff[-1]))
+        pf = _device_arg("faces", faces, torch.int32, dev, 3 * int(foff[-1]))
+        n = sum(int(c.width) * int(c.height) for c in arr[:int(ks.sum())])
+        depth = torch.empty(n, dtype=dtype, device=f"cuda:{dev}")
+        face = torch.empty(n, dtype=torch.int32, device=f"cuda:{dev}") if face_ids else None
+        self._torch_stream()
+        self._check(lib().gpdb_render_depth_device(self.h, len(ks), _p(voff), pv, _p(foff), pf, _p(ks),
+                                                   C.cast(arr, C.c_void_p), fmt, C.c_void_p(depth.data_ptr()),
+                                                   None if face is None else C.c_void_p(face.data_ptr())))
+        return (depth, face) if face_ids else depth
+
+    def sample_meshes(self, meshes, density, seed, face_ids=False):
+        """gpdb_sample_meshes: ground-truth clouds sampled from the surfaces of (vertices, faces) meshes at `density`
+        points per square metre, mesh b with the key seed + b. Returns (point_offsets [B+1], xyz [n, 3] float32, normals
+        [n, 3] float64 unit face normals[, face [n] int32 mesh-local faces]): what set_clouds() takes as clouds."""
+        m = pack_meshes(meshes)
+        B = len(meshes)
+        poff = np.zeros(B + 1, np.int32)
+        args = (self.h, B, _p(m["vertex_offsets"]), _p(m["vertices"]), _p(m["face_offsets"]), _p(m["faces"]),
+                C.c_double(float(density)), C.c_uint64(int(seed)), _p(poff))
+        n = self._check(lib().gpdb_sample_meshes(*args, None, None, None))
+        xyz, nrm = np.zeros((n, 3), np.float32), np.zeros((n, 3), np.float64)
+        face = np.zeros(n, np.int32) if face_ids else None
+        if n:
+            self._check(lib().gpdb_sample_meshes(*args, _p(xyz), _p(nrm), _p(face)))
+        return (poff, xyz, nrm, face) if face_ids else (poff, xyz, nrm)
+
+    def sample_meshes_tensors(self, vertex_offsets, vertices, face_offsets, faces, density, seed, face_ids=False):
+        """gpdb_sample_meshes_device: sample_meshes() of meshes held in CUDA tensors (as render_depth_tensors() takes
+        them). Returns (point_offsets [B+1] host, xyz [n, 3] float32, normals [n, 3] float64[, face [n] int32]) with the
+        point arrays on the device: what set_clouds_tensors() takes."""
+        import torch
+        voff, foff = _host_i32("vertex_offsets", vertex_offsets), _host_i32("face_offsets", face_offsets)
+        if len(voff) < 2 or len(foff) != len(voff):
+            raise ValueError(f"vertex_offsets / face_offsets: {len(voff)} / {len(foff)} entries, need B + 1 each (B >= 1)")
+        dev = self.params.device
+        pv = _device_arg("vertices", vertices, torch.float32, dev, 3 * int(voff[-1]))
+        pf = _device_arg("faces", faces, torch.int32, dev, 3 * int(foff[-1]))
+        self._torch_stream()
+        poff = np.zeros(len(voff), np.int32)
+        args = (self.h, len(voff) - 1, _p(voff), pv, _p(foff), pf, C.c_double(float(density)), C.c_uint64(int(seed)),
+                _p(poff))
+        n = self._check(lib().gpdb_sample_meshes_device(*args, None, None, None))
+        xyz = torch.empty((n, 3), dtype=torch.float32, device=f"cuda:{dev}")
+        nrm = torch.empty((n, 3), dtype=torch.float64, device=f"cuda:{dev}")
+        face = torch.empty(n, dtype=torch.int32, device=f"cuda:{dev}") if face_ids else None
+        if n:
+            self._check(lib().gpdb_sample_meshes_device(*args, C.c_void_p(xyz.data_ptr()), C.c_void_p(nrm.data_ptr()),
+                                                        None if face is None else C.c_void_p(face.data_ptr())))
+        return (poff, xyz, nrm, face) if face_ids else (poff, xyz, nrm)
 
     def normals_organized(self, clouds, view_points=None):
         """gpdb_normals_organized: Cloud::calculateNormalsOrganized (include/gpd_b200_organized.h) of organized clouds,

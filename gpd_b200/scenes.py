@@ -272,3 +272,87 @@ def load_weights_dir(d):
     names = ["conv1_weights", "conv1_biases", "conv2_weights", "conv2_biases", "ip1_weights", "ip1_biases",
              "ip2_weights", "ip2_biases"]
     return [np.fromfile(os.path.join(d, n + ".bin"), dtype=np.float32) for n in names]
+
+
+# ---- triangle-mesh scenes (gpdb_render_depth / gpdb_sample_meshes) -------------------------------------------------------
+
+def _outward(v, f, centre):
+    """faces f of the convex solid v wound so that (b - a) x (c - a) points away from its centre"""
+    a, b, c = v[f[:, 0]], v[f[:, 1]], v[f[:, 2]]
+    flip = (np.cross(b - a, c - a) * ((a + b + c) / 3 - centre)).sum(1) < 0
+    f = f.copy()
+    f[flip] = f[flip][:, [0, 2, 1]]
+    return f
+
+
+def _mesh_box(centre, half, yaw):
+    s = np.array([[x, y, z] for x in (-1, 1) for y in (-1, 1) for z in (-1, 1)], np.float64) * half
+    c, si = np.cos(yaw), np.sin(yaw)
+    R = np.array([[c, -si, 0.0], [si, c, 0.0], [0.0, 0.0, 1.0]])
+    v = s @ R.T + centre
+    quads = [(0, 1, 3, 2), (4, 6, 7, 5), (0, 4, 5, 1), (2, 3, 7, 6), (0, 2, 6, 4), (1, 5, 7, 3)]
+    f = np.array([t for q in quads for t in ((q[0], q[1], q[2]), (q[0], q[2], q[3]))], np.int64)
+    return v, _outward(v, f, centre)
+
+
+def _mesh_cylinder(cx, cy, z0, r, h, n):
+    th = np.arange(n) * (2 * np.pi / n)
+    ring = np.stack([cx + r * np.cos(th), cy + r * np.sin(th)], 1)
+    v = np.vstack([np.column_stack([ring, np.full(n, z0)]), np.column_stack([ring, np.full(n, z0 - h)]),
+                   [[cx, cy, z0], [cx, cy, z0 - h]]])
+    i, j = np.arange(n), (np.arange(n) + 1) % n
+    f = np.vstack([np.stack([i, j, n + j], 1), np.stack([i, n + j, n + i], 1),
+                   np.stack([np.full(n, 2 * n), j, i], 1), np.stack([np.full(n, 2 * n + 1), n + i, n + j], 1)])
+    return v, _outward(v, f, np.array([cx, cy, z0 - h / 2]))
+
+
+def _mesh_sphere(centre, r, n):
+    nu, nv = 2 * n, n
+    ph = np.arange(1, nv) * (np.pi / nv)
+    th = np.arange(nu) * (2 * np.pi / nu)
+    P, T = np.meshgrid(ph, th, indexing="ij")
+    ring = np.stack([np.sin(P) * np.cos(T), np.sin(P) * np.sin(T), np.cos(P)], -1).reshape(-1, 3)
+    v = centre + r * np.vstack([ring, [[0, 0, 1.0], [0, 0, -1.0]]])
+    top, bot = len(ring), len(ring) + 1
+    f = []
+    for a in range(nv - 1):
+        for k in range(nu):
+            p, q = a * nu + k, a * nu + (k + 1) % nu
+            if a == 0:
+                f.append((top, p, q))
+            if a == nv - 2:
+                f.append((bot, q, p))
+            else:
+                f.append((p, p + nu, q + nu))
+                f.append((p, q + nu, q))
+    return v, _outward(v, np.array(f, np.int64), centre)
+
+
+def mesh_table_scene(seed, n_objects=8, segments=24, table=(0.6, 0.45), tz=0.9):
+    """A seeded tabletop of triangle meshes in the frame of synthetic_table_scene (up is -z, the table top at z = tz,
+    cameras near the origin looking along +z): a 3 cm table slab plus n_objects closed, outward-wound boxes, cylinders
+    and UV spheres resting on it, 3-8 cm across, so the default hand (aperture up to 8.5 cm) fits most of them.
+    `segments` sets the tessellation (cylinder sides, sphere rings), the knob of the face count. Returns (vertices [V, 3]
+    float32, faces [F, 3] int32, object_id [F] int32: 0 for the table, 1..n_objects for the objects)."""
+    rng = np.random.default_rng(seed)
+    tx, ty = table
+    parts = [_mesh_box(np.array([0.0, 0.0, tz + 0.015]), np.array([tx / 2, ty / 2, 0.015]), 0.0)]
+    for _ in range(n_objects):
+        cx, cy = rng.uniform(-tx / 2 + 0.06, tx / 2 - 0.06), rng.uniform(-ty / 2 + 0.06, ty / 2 - 0.06)
+        kind = rng.integers(0, 3)
+        if kind == 0:
+            half = np.array([rng.uniform(0.015, 0.04), rng.uniform(0.015, 0.04), rng.uniform(0.02, 0.07)])
+            parts.append(_mesh_box(np.array([cx, cy, tz - half[2]]), half, rng.uniform(0, np.pi)))
+        elif kind == 1:
+            parts.append(_mesh_cylinder(cx, cy, tz, rng.uniform(0.015, 0.035), rng.uniform(0.04, 0.14), 2 * segments))
+        else:
+            r = rng.uniform(0.02, 0.04)
+            parts.append(_mesh_sphere(np.array([cx, cy, tz - r]), r, segments))
+    V, Fs, ids, base = [], [], [], 0
+    for k, (v, f) in enumerate(parts):
+        V.append(v)
+        Fs.append(f + base)
+        ids.append(np.full(len(f), k, np.int32))
+        base += len(v)
+    return (np.ascontiguousarray(np.vstack(V).astype(np.float32)), np.ascontiguousarray(np.vstack(Fs).astype(np.int32)),
+            np.concatenate(ids))

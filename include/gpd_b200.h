@@ -712,6 +712,44 @@ int gpdb_subsample_clouds_points(gpdb_ctx *ctx, int32_t num_samples, uint64_t se
 int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_point_mask,
                                         int32_t *d_sample_idx_out, int32_t *sample_offsets_out);
 
+/* --- training views from triangle meshes (include/gpd_b200_render.h) ----------------------------------------------------
+ * Depth images of mesh scenes in the layout gpdb_preprocess_depth[_device] consumes, and dense ground-truth clouds sampled
+ * from the same surfaces for gpdb_reevaluate_batch[_device]: meshes -> views -> candidates -> labels -> images -> weights
+ * with no dataset on disk. Neither call installs anything: the single cloud, the batch, its sample positions and the SIS
+ * record are untouched. The rules are specified in gpd_b200_render.h. */
+
+/* Renders n_views mesh scenes: view b has the float32 xyz vertices vertex_offsets[b] .. vertex_offsets[b+1]-1 of vertices
+ * (world frame) and the int32 index triples face_offsets[b] .. face_offsets[b+1]-1 of faces (0-based, into the view's own
+ * vertices); it is seen by n_cameras[b] (1..8) cameras, the sum of n_cameras host descriptions in cameras, view by view.
+ * depth_out receives every camera's image back to back in the same order (gpd_b200_render.h 5; format GPDB_DEPTH_U16 or
+ * GPDB_DEPTH_F32), face_out (may be NULL) one int32 per pixel: the view-local index of the face the pixel's return hit,
+ * -1 where it has none. GPDB_ERR_INVALID, the message naming the view, with nothing written: malformed offsets, a face
+ * index outside its view's vertices, a non-finite vertex, the camera checks of gpdb_preprocess_depth, an unknown format,
+ * 2^31 or more pixels in the call. Returns n_views. */
+int gpdb_render_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                      const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                      const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out);
+/* The same with vertices, faces and the outputs in device memory (offsets and cameras stay host arrays), on the context's
+ * stream. */
+int gpdb_render_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                             const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                             int32_t *d_face_out);
+/* Samples the surfaces of n_meshes meshes (laid out as the views of gpdb_render_depth) at density points per square metre,
+ * mesh b with the key seed + b (gpd_b200_render.h 6). point_offsets_out [B+1] (host) always receives the point offsets;
+ * xyz_out = NULL only counts, else xyz_out [3n] receives the float32 points, normals_out [3n] (may be NULL) the float64
+ * unit face normals that gpdb_set_clouds[_device] takes, face_out [n] (may be NULL) each point's mesh-local face. The call
+ * is deterministic, so a count followed by a fill agrees. GPDB_ERR_INVALID, the message naming the mesh, with nothing
+ * written: malformed offsets, a face index outside its mesh's vertices, a non-finite vertex, a density that is not
+ * finite and > 0, 2^31 or more points. Returns the number of points n. */
+int gpdb_sample_meshes(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *vertices,
+                       const int32_t *face_offsets, const int32_t *faces, double density, uint64_t seed,
+                       int32_t *point_offsets_out, float *xyz_out, double *normals_out, int32_t *face_out);
+/* The same with vertices, faces and the point arrays in device memory (the offsets stay host arrays). */
+int gpdb_sample_meshes_device(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *d_vertices,
+                              const int32_t *face_offsets, const int32_t *d_faces, double density, uint64_t seed,
+                              int32_t *point_offsets_out, float *d_xyz_out, double *d_normals_out, int32_t *d_face_out);
+
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
  * back for the next call. A result may outlive its context. */
