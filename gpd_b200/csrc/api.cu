@@ -2614,8 +2614,8 @@ int gpdb_debug_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_
   const char *name = "gpdb_debug_train_step";
   int rc = train_step_args(ctx, name, images_hwc, labels, n);
   if (rc != GPDB_OK) return rc;
-  if (!out || n > GPDB_TRAIN_CHUNK) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need an output struct and n <= %d", name, GPDB_TRAIN_CHUNK);
+  if (!out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need an output struct", name);
     return GPDB_ERR_INVALID;
   }
   return train_step_host(ctx, name, images_hwc, labels, n, nullptr, out);

@@ -627,7 +627,7 @@ int lenet_simt_run(gpdb_ctx *ctx, const LenetWeights &w, const uint8_t *d_images
 // train.cu (include/gpd_b200_train.h)
 int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]);
 // one step on n device images / labels (labels already checked); d_loss_out / h_loss_out: device / host float or null; dbg: host outputs of a
-// debug step (n <= GPDB_TRAIN_CHUNK), which updates nothing
+// debug step (any n, copied chunk by chunk), which updates nothing
 int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, int n, float *d_loss_out,
                float *h_loss_out, const gpdb_train_debug *dbg);
 int train_weights(gpdb_ctx *ctx, float *const out[8]);

@@ -465,6 +465,28 @@ int chunk(gpdb_ctx *ctx, TrainState &ts, ChunkBufs &b, const uint8_t *d_img, con
   return GPDB_OK;
 }
 
+// gpdb_debug_train_step: the per-image arrays of the chunk that just ran (images b0 .. b0 + nb of the step) to the
+// caller's arrays at image offset b0, before the next chunk overwrites the buffers
+int debug_copy_chunk(gpdb_ctx *ctx, const ChunkBufs &b, const gpdb_train_debug &dbg, int b0, int nb) {
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  auto get = [&](auto *dst, const void *src, size_t per_image) {
+    return dst ? cudaMemcpy(dst + per_image * b0, src, sizeof(*dst) * per_image * nb, cudaMemcpyDeviceToHost)
+               : cudaSuccess;
+  };
+  CUDA_TRY(get(dbg.pool1, b.p1, NF1 * P1 * P1));
+  CUDA_TRY(get(dbg.pool2, b.p2, K));
+  CUDA_TRY(get(dbg.ip1, b.h3, NH));
+  CUDA_TRY(get(dbg.logits, b.logits, 2));
+  CUDA_TRY(get(dbg.choice1, b.ch1, NF1 * P1 * P1));
+  CUDA_TRY(get(dbg.choice2, b.ch2, K));
+  CUDA_TRY(get(dbg.loss, b.loss, 1));
+  CUDA_TRY(get(dbg.dlogits, b.dz, 2));
+  CUDA_TRY(get(dbg.dip1, b.dh, NH));
+  CUDA_TRY(get(dbg.dpool2, b.dx, K));
+  CUDA_TRY(get(dbg.dpool1, b.dp1, NF1 * P1 * P1));
+  return GPDB_OK;
+}
+
 bool params_ok(const gpdb_train_params &p) {
   auto nonneg = [](float x) { return std::isfinite(x) && x >= 0.0f; };
   if (p.optimizer != 0 && p.optimizer != 1) return false;
@@ -571,26 +593,12 @@ int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, 
   for (int b0 = 0; b0 < n; b0 += GPDB_TRAIN_CHUNK) {
     const int nb = std::min(GPDB_TRAIN_CHUNK, n - b0);
     TRY(chunk(ctx, ts, b, d_images + isz * b0, d_labels + b0, nb, n, b0 == 0, b0 + nb == n, d_loss_out));
+    if (dbg) TRY(debug_copy_chunk(ctx, b, *dbg, b0, nb));
   }
-  if (dbg) {  // n <= GPDB_TRAIN_CHUNK: one chunk, its buffers hold every intermediate
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    auto get = [&](void *dst, const void *src, size_t bytes) {
-      return dst ? cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) : cudaSuccess;
-    };
-    const size_t fn = sizeof(float) * n;
-    CUDA_TRY(get(dbg->pool1, b.p1, fn * NF1 * P1 * P1));
-    CUDA_TRY(get(dbg->pool2, b.p2, fn * K));
-    CUDA_TRY(get(dbg->ip1, b.h3, fn * NH));
-    CUDA_TRY(get(dbg->logits, b.logits, fn * 2));
-    CUDA_TRY(get(dbg->choice1, b.ch1, (size_t)n * NF1 * P1 * P1));
-    CUDA_TRY(get(dbg->choice2, b.ch2, (size_t)n * K));
-    CUDA_TRY(get(dbg->loss, b.loss, fn));
-    CUDA_TRY(get(dbg->dlogits, b.dz, fn * 2));
-    CUDA_TRY(get(dbg->dip1, b.dh, fn * NH));
-    CUDA_TRY(get(dbg->dpool2, b.dx, fn * K));
-    CUDA_TRY(get(dbg->dpool1, b.dp1, fn * NF1 * P1 * P1));
+  if (dbg) {  // the gradients once, after the last chunk has chained onto them
     for (int i = 0; i < 8; i++)
-      CUDA_TRY(get(dbg->grad[i], ts.g + ts.off[i], sizeof(float) * ts.len[i]));
+      if (dbg->grad[i])
+        CUDA_TRY(cudaMemcpy(dbg->grad[i], ts.g + ts.off[i], sizeof(float) * ts.len[i], cudaMemcpyDeviceToHost));
     return GPDB_OK;
   }
   const gpdb_train_params &p = ts.p;

@@ -857,7 +857,10 @@ int gpdb_train_weights(gpdb_ctx *ctx, float *const out[8]);
  * or a NULL argument: GPDB_ERR_INVALID; a file that cannot be written: GPDB_ERR_IO. */
 int gpdb_write_weights_dir(const char *dir, int32_t channels, const float *const w[8]);
 /* Development aid, like gpdb_debug_lenet_layers: one step's forward state, backward intermediates and gradients, nothing
- * updated. n in 1..GPDB_TRAIN_CHUNK (include/gpd_b200_train.h); every output host memory, any of them NULL. */
+ * updated. Any n >= 1: a step of more than GPDB_TRAIN_CHUNK images (include/gpd_b200_train.h) runs in chunks as
+ * gpdb_train_step does, and each chunk's per-image arrays are copied out at their image offset before the next chunk
+ * runs; the gradients are those of the whole step. Every output host memory, any of them NULL; a NULL struct:
+ * GPDB_ERR_INVALID. */
 typedef struct gpdb_train_debug {
   float *pool1;      /* [n][20][28][28]  as gpdb_debug_lenet_layers */
   float *pool2;      /* [n][7200]        k = c + 50 j */

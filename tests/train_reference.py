@@ -60,14 +60,18 @@ def mean_loss_f32(losses):
     return F(s / F(len(losses)))
 
 
-def dlogits_f32(z, y, n):
-    """rule 4: z [m, 2], y [m], n the step's image count"""
+def probs_f32(z):
+    """rule 4: the probabilities (p0, p1) of logits z [m, 2]"""
     z0, z1 = z[:, 0].astype(F), z[:, 1].astype(F)
     e = _vec("expf", -np.abs(z1 - z0))
     s = F(1) + e
     pb, ps = F(1) / s, e / s
-    p1 = np.where(z1 >= z0, pb, ps)
-    p0 = np.where(z1 >= z0, ps, pb)
+    return np.where(z1 >= z0, ps, pb), np.where(z1 >= z0, pb, ps)
+
+
+def dlogits_f32(z, y, n):
+    """rule 4: z [m, 2], y [m], n the step's image count"""
+    p0, p1 = probs_f32(z)
     nf = F(n)
     return np.stack([(p0 - (y == 0).astype(F)) / nf, (p1 - (y == 1).astype(F)) / nf], 1).astype(F)
 
@@ -239,17 +243,23 @@ def dlogits64(z, y, n):
     return (p - np.eye(2)[np.asarray(y)]) / n
 
 
-def backward64(images, labels, w, relu, dev=None):
+def backward64(images, labels, w, relu, dev=None, n_step=None):
     """every backward stage in float64. dev: a dict of the device's own stage inputs (keys of gpdb_train_debug: pool1,
     pool2 (k order), ip1, logits, choice1 ([n, 20, 28, 28]), choice2 (k order), dlogits, dip1, dpool2, dpool1); each
-    stage then starts from the device's input to it. Returns the stages and the eight gradients in the .bin layouts."""
+    stage then starts from the device's input to it. n_step: the image count of the whole step when images are a slice
+    of it (the gradients of a step are the sums of its slices' gradients). Returns the stages and the eight gradients in
+    the .bin layouts."""
     C = images.shape[-1]
-    n = len(labels)
+    n = n_step or len(labels)
     w1, b1, w2, b2, W1, B1, W2, B2 = arrays64(w, C)
     dev = dev or {}
     ch1 = dev.get("choice1")
     ch2 = None if dev.get("choice2") is None else unflat(np.asarray(dev["choice2"]))
-    f = forward64(images, w, relu, ch1, ch2, dev.get("pool1"))
+    if all(k in dev for k in ("pool1", "pool2", "ip1", "logits", "choice1", "choice2")):
+        # every forward value is given: only the input and the choices are needed
+        f = {"x": chw(images), "ch1": ch1, "ch2": ch2, "p1": None, "xf": None, "h": None, "z": None}
+    else:
+        f = forward64(images, w, relu, ch1, ch2, dev.get("pool1"))
     g = lambda k, v: np.asarray(dev[k], np.float64) if k in dev else v  # noqa: E731
     h, xf, p1, p2 = g("ip1", f["h"]), g("pool2", f["xf"]), g("pool1", f["p1"]), unflat(g("pool2", f["xf"]))
     dz = dlogits64(g("logits", f["z"]), labels, n)
@@ -274,11 +284,12 @@ def backward64(images, labels, w, relu, dev=None):
             "g2": g2, "g1": g1, "grad": grads, "h": h, "xf": xf, "p1": p1, "dz_in": dzi, "dh_in": dhi}
 
 
-def bounds(images, labels, w, relu, st):
+def bounds(images, labels, w, relu, st, n_step=None):
     """per-stage error bounds of the device's float32 arithmetic for the stages of backward64(..., dev) (each on the
-    device's own input), and of the eight gradients"""
+    device's own input), and of the eight gradients; n_step as backward64 (the bound of a step's gradient is the sum of
+    its slices' bounds)"""
     C = images.shape[-1]
-    n = len(labels)
+    n = n_step or len(labels)
     w1, b1, w2, b2, W1, B1, W2, B2 = arrays64(w, C)
     tiny = 2.0 ** -140
     dz, dh, h, xf, p1 = np.abs(st["dz_in"]), np.abs(st["dh_in"]), np.abs(st["h"]), np.abs(st["xf"]), np.abs(st["p1"])
@@ -303,6 +314,21 @@ def bounds(images, labels, w, relu, st):
         gamma(n) * dz.sum(0) + tiny,
     ]
     return out
+
+
+def step_grad_bounds(images, labels, w, relu, dev, slice_size=64):
+    """(the eight float64 gradients of backward64(..., dev), their bounds) for a whole step, summed over slices of
+    slice_size images: the float64 windows of a few hundred images would take gigabytes"""
+    n = len(labels)
+    ref, bnd = [0.0] * 8, [0.0] * 8
+    for s in range(0, n, slice_size):
+        sl = slice(s, s + slice_size)
+        d = {k: np.asarray(v)[sl] for k, v in dev.items() if k != "grad"}
+        st = backward64(images[sl], labels[sl], w, relu, d, n_step=n)
+        b = bounds(images[sl], labels[sl], w, relu, st, n_step=n)
+        ref = [r + g for r, g in zip(ref, st["grad"])]
+        bnd = [r + g for r, g in zip(bnd, b["grad"])]
+    return ref, bnd
 
 
 def torch_grads64(images, labels, w, relu):
