@@ -165,6 +165,13 @@ class DepthCamera(C.Structure):
     ]
 
 
+class SensorParams(C.Structure):
+    """gpdb_sensor_params (include/gpd_b200.h, rules in include/gpd_b200_sensor.h): every field 0 is a clean render."""
+
+    _fields_ = [(f, C.c_double) for f in ("baseline", "lateral_sigma", "disparity_sigma", "disparity_step",
+                                          "min_cos_incidence", "shadow_tolerance", "dropout")]
+
+
 class PlaneParams(C.Structure):
     """gpdb_plane_params (include/gpd_b200.h, rules in include/gpd_b200_plane.h)."""
 
@@ -274,6 +281,10 @@ PROTOTYPES = {
     "gpdb_render_depth_device": (_int, [_vp, _i32] + [_vp] * 5 + [_vp, _i32, _vp, _vp]),
     "gpdb_sample_meshes": (_int, [_vp, _i32] + [_vp] * 4 + [C.c_double, C.c_uint64] + [_vp] * 4),
     "gpdb_sample_meshes_device": (_int, [_vp, _i32] + [_vp] * 4 + [C.c_double, C.c_uint64] + [_vp] * 4),
+    "gpdb_sensor_params_default": (None, [_vp]),
+    "gpdb_render_sensor_depth": (_int, [_vp, _i32] + [_vp] * 5 + [_vp, _i32, _vp, _vp, _vp, C.c_uint64]),
+    "gpdb_render_sensor_depth_device": (_int, [_vp, _i32] + [_vp] * 5 + [_vp, _i32, _vp, _vp, _vp, C.c_uint64]),
+    "gpdb_debug_sensor_table": (_int, [_vp]),
     "gpdb_free_result": (None, [_res]),
     "gpdb_comm_unique_id": (_int, [_vp]),
     "gpdb_comm_init": (_int, [_vp, _vp, _i32, _i32]),

@@ -18,6 +18,7 @@
 #include "../../include/gpd_b200_outliers.h"
 #include "../../include/gpd_b200_plane.h"
 #include "../../include/gpd_b200_refine.h"
+#include "../../include/gpd_b200_sensor.h"
 #include "../../include/gpd_b200_train.h"
 #include "common.cuh"
 
@@ -1821,11 +1822,46 @@ static int check_meshes(gpdb_ctx *ctx, const char *name, const char *unit, int B
   return GPDB_ERR_INVALID;
 }
 
-// gpdb_render_depth[_device]: the checks, then the device render (the host twin uploads the meshes into SCR_UPLOAD, renders
-// into it and copies the images back). Nothing installed changes.
+// gpd_b200_sensor.h rule 9's parameter checks
+static int check_sensor_params(gpdb_ctx *ctx, const char *name, const gpdb_sensor_params *sp) {
+  if (!sp) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need sensor (gpdb_sensor_params_default for a clean render)", name);
+    return GPDB_ERR_INVALID;
+  }
+  const struct {
+    const char *name;
+    double v;
+  } f[] = {{"baseline", sp->baseline},
+           {"lateral_sigma", sp->lateral_sigma},
+           {"disparity_sigma", sp->disparity_sigma},
+           {"disparity_step", sp->disparity_step},
+           {"min_cos_incidence", sp->min_cos_incidence},
+           {"shadow_tolerance", sp->shadow_tolerance},
+           {"dropout", sp->dropout}};
+  const char *bad = nullptr;
+  for (const auto &e : f)
+    if (!(e.v >= 0.0) || !std::isfinite(e.v)) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s must be finite and >= 0 (got %g)", name, e.name, e.v);
+      return GPDB_ERR_INVALID;
+    }
+  if (sp->dropout > 1.0) bad = "dropout must lie in [0, 1]";
+  else if (sp->shadow_tolerance >= 1.0) bad = "shadow_tolerance must be < 1";
+  else if (sp->min_cos_incidence > 1.0) bad = "min_cos_incidence must be <= 1";
+  else if ((sp->disparity_sigma > 0.0 || sp->disparity_step > 0.0) && !(sp->baseline > 0.0))
+    bad = "disparity_sigma and disparity_step need a baseline > 0";
+  if (bad) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s", name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// gpdb_render_depth[_device] and (sensor) gpdb_render_sensor_depth[_device]: the checks, then the device render (the host
+// twin uploads the meshes into SCR_UPLOAD, renders into it and copies the images back). Nothing installed changes.
 static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
                         const int32_t *foff, const int32_t *faces, const int32_t *n_cameras, const gpdb_depth_camera *cams,
-                        int32_t format, void *depth_out, int32_t *face_out, bool device) {
+                        int32_t format, void *depth_out, int32_t *face_out, bool device, bool sensor = false,
+                        const gpdb_sensor_params *sp = nullptr, uint64_t seed = 0) {
   if (!ctx) return GPDB_ERR_INVALID;
   if (B <= 0 || !n_cameras || !cams || !depth_out) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth_out", name);
@@ -1835,6 +1871,7 @@ static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
     return GPDB_ERR_INVALID;
   }
+  if (sensor && check_sensor_params(ctx, name, sp) != GPDB_OK) return GPDB_ERR_INVALID;
   std::vector<int> roff;
   int rc = check_mesh_args(ctx, name, "view", B, voff, vertices, foff, faces);
   if (rc == GPDB_OK) rc = check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
@@ -1865,7 +1902,8 @@ static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_
     d_vtx = v, d_faces = f, d_depth = dd;
   }
   if ((rc = check_meshes(ctx, name, "view", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
-  rc = render_depth_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face);
+  rc = sensor ? render_sensor_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, sp, seed)
+              : render_depth_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face);
   if (rc != GPDB_OK) return rc;
   if (!device) {
     CUDA_TRY(cudaMemcpyAsync(depth_out, d_depth, elt * M, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2029,6 +2067,32 @@ int gpdb_render_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vert
                              int32_t *d_face_out) {
   return render_entry(ctx, "gpdb_render_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces, n_cameras,
                       cameras, depth_format, d_depth_out, d_face_out, true);
+}
+
+void gpdb_sensor_params_default(gpdb_sensor_params *p) {
+  if (p) memset(p, 0, sizeof(*p));
+}
+
+int gpdb_render_sensor_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                             const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out,
+                             const gpdb_sensor_params *sensor, uint64_t seed) {
+  return render_entry(ctx, "gpdb_render_sensor_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras,
+                      cameras, depth_format, depth_out, face_out, false, true, sensor, seed);
+}
+
+int gpdb_render_sensor_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                                    const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                                    int32_t *d_face_out, const gpdb_sensor_params *sensor, uint64_t seed) {
+  return render_entry(ctx, "gpdb_render_sensor_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces,
+                      n_cameras, cameras, depth_format, d_depth_out, d_face_out, true, true, sensor, seed);
+}
+
+int gpdb_debug_sensor_table(double *table_out) {
+  if (!table_out) return GPDB_ERR_INVALID;
+  memcpy(table_out, sensor_table(), sizeof(double) * GPDB_SENSOR_TABLE);
+  return GPDB_SENSOR_TABLE;
 }
 
 int gpdb_sample_meshes(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *vertices,

@@ -593,6 +593,12 @@ int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud 
 // d_face (may be null), device arrays in the layout of gpdb_preprocess_depth.
 int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
                        const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face);
+// The same seen by the structured-light sensor sp (include/gpd_b200_sensor.h, checked), view b with the key seed + b.
+int render_sensor_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                        const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face,
+                        const gpdb_sensor_params *sp, unsigned long long seed);
+// gpd_b200_sensor.h rule 2's table (GPDB_SENSOR_TABLE doubles, host), built on first use
+const double *sensor_table();
 // rule 6's counts of B checked meshes: returns the total (an error when negative) and mesh_n[B] (host) each mesh's
 // count (each face's count clamped to 2^31); when the total is below 2^31, poff[B+1] (host) receives the point offsets
 // and SCR_RENDER keeps the per-face scan for mesh_write_batch

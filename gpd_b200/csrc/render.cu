@@ -13,6 +13,13 @@
 // pairs are resolved in chunks of at most the carved list length, the running minimum kept per pixel between chunks, so a
 // face covering every tile (a table) costs one list entry per tile and memory stays bounded.
 //
+// Sensor views (include/gpd_b200_sensor.h): with a baseline every camera is followed by its projector, a camera of the
+// same intrinsics whose pose is shifted along the camera's +x, and the two always share a group, so the projector's
+// image counts toward the group's bytes. Every chunk's resolve then keeps the running minimum, and after the group's
+// last chunk
+//   k_sensor       one thread per camera pixel: rules 1-8, reading the camera's and the projector's (t, face) minima and
+//                  the hit face's vertices, then the depth and face images
+//
 // Sampling: k_mesh_count per face (rule 6's count, a 64-bit total), scan_flags over the counts once the total is known
 // to lie below 2^31, then k_mesh_write per point. Scratch: SCR_RENDER. Compiled with -fmad=false: every float64
 // operation is rounded on its own.
@@ -21,6 +28,7 @@
 #include <vector>
 
 #include "../../include/gpd_b200_render.h"
+#include "../../include/gpd_b200_sensor.h"
 #include "common.cuh"
 
 namespace {
@@ -183,6 +191,37 @@ __global__ void __launch_bounds__(RND_THREADS) k_rnd_resolve(const RndCam *cams,
   if (face_out) face_out[o] = ret ? bf : -1;
 }
 
+// One camera of a sensor group: its entry in the group's camera table, its projector's (-1: none), its index within its
+// view and its view's key
+struct SensorCam {
+  int cam, proj, k, pad;
+  unsigned long long key;
+};
+
+// rules 1-8 of every pixel of the group's n sensor cameras (spix_off[n+1]: their first pixels, N in all) from the
+// running minima the resolve left, then the depth and face images (rule 8)
+__global__ void k_sensor(const RndCam *cams, const SensorCam *sc, const int *spix_off, int n, int N, const double *best_t,
+                         const int *best_f, const long long *pix_off, const float *vtx, const int *faces, const double *T,
+                         gpdb_sensor_params sp, int format, void *depth, int *face_out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int j = csr_owner(spix_off, n, i);
+  const SensorCam &s = sc[j];
+  const RndCam &c = cams[s.cam];
+  const int p = i - spix_off[j], u = p % c.W, v = p / c.W;
+  const long long o = pix_off[s.cam], po = s.proj >= 0 ? pix_off[s.proj] : o;
+  double z = 0.0;
+  const int f = gpdb_sensor_pixel(&sp, T, s.key, (uint32_t)s.k, u, v, c.W, c.H, c.fx, c.fy, c.cx, c.cy, c.pose,
+                                  best_t + o, best_f + o, best_t + po, best_f + po, vtx + 3 * (size_t)c.vbase,
+                                  faces + 3 * (size_t)c.fbase, &z);
+  bool ret = false;
+  const uint32_t raw = f >= 0 ? gpdb_render_raw(z, c.scale, format, &ret) : 0u;
+  const long long out = c.pix + p;
+  if (format == GPDB_DEPTH_F32) static_cast<uint32_t *>(depth)[out] = raw;
+  else static_cast<uint16_t *>(depth)[out] = (uint16_t)raw;
+  if (face_out) face_out[out] = ret ? f : -1;
+}
+
 // the cameras [first, last) of one group and their sizes
 struct RndGroup {
   int first, last;
@@ -204,21 +243,39 @@ struct RndScratch {
   int4 *rect;
   int *count, *best_f, *tcnt, *tpos, *list;
   unsigned long long *pairs;
+  // sensor views only: the table, the group's sensor cameras and their first pixels
+  double *table;
+  SensorCam *scam;
+  int *spix_off;
 };
 
-}  // namespace
+// The table of gpd_b200_sensor.h rule 2, built once
+const double *sensor_table_host() {
+  static const std::vector<double> T = [] {
+    std::vector<double> t(GPDB_SENSOR_TABLE);
+    gpdb_sensor_table_build(t.data());
+    return t;
+  }();
+  return T.data();
+}
 
-int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
-                       const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face) {
+// The render of a call (sp null) or of a sensor call (sp given, view b with the key seed + b): camera k of the call is
+// entry k * per of the camera table, and with a baseline (per = 2) entry k * per + 1 is its projector
+int render_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                 const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face,
+                 const gpdb_sensor_params *sp, unsigned long long seed) {
+  const int per = sp && sp->baseline > 0.0 ? 2 : 1;
   // the cameras of the call, view by view
   int C = 0;
   for (int b = 0; b < B; b++) C += n_cameras[b];
-  std::vector<RndCam> rc((size_t)C);
+  std::vector<RndCam> rc((size_t)C * per);
+  std::vector<SensorCam> sc((size_t)C);
   long long pix = 0;
   for (int b = 0, k = 0; b < B; b++)
     for (int j = 0; j < n_cameras[b]; j++, k++) {
       const gpdb_depth_camera &D = cams[k];
-      RndCam &c = rc[k];
+      sc[k] = SensorCam{0, -1, j, 0, seed + (unsigned long long)b};
+      RndCam &c = rc[(size_t)k * per];
       memset(&c, 0, sizeof(c));
       for (int e = 0; e < 12; e++) c.pose[e] = D.pose[e];
       c.fx = D.fx, c.fy = D.fy, c.cx = D.cx, c.cy = D.cy, c.scale = D.depth_scale;
@@ -227,21 +284,32 @@ int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, c
       c.vbase = voff[b], c.nv = voff[b + 1] - voff[b], c.fbase = foff[b], c.nf = foff[b + 1] - foff[b];
       c.pix = pix;
       pix += (long long)D.width * D.height;
+      if (per == 2) {
+        RndCam &p = rc[(size_t)k * per + 1];
+        p = c;
+        gpdb_sensor_projector_pose(c.pose, sp->baseline, p.pose);
+        p.pix = -1;  // never written out
+      }
     }
-  // consecutive cameras, each group's per-camera arrays within RND_GROUP_BYTES (a larger camera is a group of its own)
+  // consecutive cameras (with their projectors), each group's per-camera arrays within RND_GROUP_BYTES (a larger camera
+  // is a group of its own)
   std::vector<RndGroup> groups;
   RndGroup cur{0, 0, 0, 0, 0, 0, 0};
-  for (int k = 0; k < C; k++) {
-    const RndCam &c = rc[k];
-    const long long px = (long long)c.W * c.H, tl = (long long)c.tx * c.ty;
+  for (int k = 0; k < C * per; k += per) {
+    long long nv = 0, nf = 0, px = 0, tl = 0, pm = 0;
+    for (int e = k; e < k + per; e++) {
+      const RndCam &c = rc[e];
+      const long long ct = (long long)c.tx * c.ty;
+      nv += c.nv, nf += c.nf, px += (long long)c.W * c.H, tl += ct, pm += (long long)c.nf * ct;
+    }
     if (cur.last > cur.first &&
-        rnd_camera_bytes(cur.verts + c.nv, cur.items + c.nf, cur.pixels + px, cur.tiles + tl) > RND_GROUP_BYTES) {
+        rnd_camera_bytes(cur.verts + nv, cur.items + nf, cur.pixels + px, cur.tiles + tl) > RND_GROUP_BYTES) {
       groups.push_back(cur);
       cur = RndGroup{k, k, 0, 0, 0, 0, 0};
     }
-    cur.last = k + 1;
-    cur.verts += c.nv, cur.items += c.nf, cur.pixels += px, cur.tiles += tl;
-    cur.pairs_max += (long long)c.nf * tl;
+    cur.last = k + per;
+    cur.verts += nv, cur.items += nf, cur.pixels += px, cur.tiles += tl;
+    cur.pairs_max += pm;
   }
   groups.push_back(cur);
   long long g_max = 0, v_max = 0, i_max = 0, p_max = 0, t_max = 0, cap = 0;
@@ -274,8 +342,16 @@ int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, c
         s.tpos = c.take<int>(t_max + 1);
         s.pairs = c.take<unsigned long long>(1);
         s.list = c.take<int>(cap);
+        if (sp) {
+          s.table = c.take<double>(GPDB_SENSOR_TABLE);
+          s.scam = c.take<SensorCam>(g_max);
+          s.spix_off = c.take<int>(g_max + 1);
+        }
       }))
     return GPDB_ERR_CUDA;
+  if (sp)
+    CUDA_TRY(cudaMemcpyAsync(s.table, sensor_table_host(), sizeof(double) * GPDB_SENSOR_TABLE, cudaMemcpyHostToDevice,
+                             ctx->stream));
   const int tb = 256;
   for (const RndGroup &G : groups) {
     const int n = G.last - G.first;
@@ -341,14 +417,48 @@ int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, c
                                                                   s.list, true);
         LAUNCH_CHECK();
       }
+      // a sensor call keeps the running minimum after the last chunk too: k_sensor reads it
       k_rnd_resolve<<<NT, RND_THREADS, 0, ctx->stream>>>(s.cams, s.tile_off, n, s.rec, s.tpos, s.list, ch == 0,
-                                                         ch + 2 == cuts.size(), s.best_t, s.best_f, s.pix_off, format,
-                                                         d_depth, d_face);
+                                                         !sp && ch + 2 == cuts.size(), s.best_t, s.best_f, s.pix_off,
+                                                         format, d_depth, d_face);
+      LAUNCH_CHECK();
+    }
+    if (sp) {
+      // the group's cameras (every per-th entry) and their first pixels
+      const int ns = n / per;
+      std::vector<SensorCam> gs((size_t)ns);
+      std::vector<int> sp_off((size_t)ns + 1, 0);
+      for (int j = 0; j < ns; j++) {
+        gs[j] = sc[(size_t)(G.first / per + j)];
+        gs[j].cam = j * per;
+        gs[j].proj = per == 2 ? j * per + 1 : -1;
+        sp_off[j + 1] = sp_off[j] + gc[j * per].W * gc[j * per].H;
+      }
+      CUDA_TRY(cudaMemcpyAsync(s.scam, gs.data(), sizeof(SensorCam) * ns, cudaMemcpyHostToDevice, ctx->stream));
+      CUDA_TRY(cudaMemcpyAsync(s.spix_off, sp_off.data(), sizeof(int) * (ns + 1), cudaMemcpyHostToDevice, ctx->stream));
+      const int N = sp_off[ns];
+      k_sensor<<<(N + tb - 1) / tb, tb, 0, ctx->stream>>>(s.cams, s.scam, s.spix_off, ns, N, s.best_t, s.best_f, s.pix_off,
+                                                          d_vtx, d_faces, s.table, *sp, format, d_depth, d_face);
       LAUNCH_CHECK();
     }
   }
   return GPDB_OK;
 }
+
+}  // namespace
+
+int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                       const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face) {
+  return render_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, nullptr, 0);
+}
+
+int render_sensor_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
+                        const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face,
+                        const gpdb_sensor_params *sp, unsigned long long seed) {
+  return render_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, sp, seed);
+}
+
+const double *sensor_table() { return sensor_table_host(); }
 
 namespace {
 

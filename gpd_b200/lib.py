@@ -82,6 +82,28 @@ def plane_params(**over):
     return abi.set_fields(p, **over)
 
 
+def sensor_params(**fields):
+    """gpdb_sensor_params (include/gpd_b200_sensor.h): every field 0 (a clean render, gpdb_sensor_params_default),
+    overridden by keyword: baseline (m), lateral_sigma, disparity_sigma, disparity_step (pixels), min_cos_incidence,
+    shadow_tolerance, dropout."""
+    p = abi.SensorParams()
+    lib().gpdb_sensor_params_default(C.c_void_p(C.addressof(p)))
+    for k in fields:
+        if k not in dict(abi.SensorParams._fields_):
+            raise TypeError(f"sensor_params: unknown field {k!r}")
+    return abi.set_fields(p, **fields)
+
+
+def debug_sensor_table():
+    """gpdb_debug_sensor_table: the float64 inverse-normal table [4097] the sensor draws interpolate (gpd_b200_sensor.h 2).
+    Needs no device."""
+    t = np.zeros(4097, np.float64)
+    rc = lib().gpdb_debug_sensor_table(_p(t))
+    if rc != len(t):
+        raise GpdbError(rc, "gpdb_debug_sensor_table failed")
+    return t
+
+
 def read_weights_file(weights_file, channels, model_file=None):
     """Host-side import of a .caffemodel or an OpenVINO IR into the eight arrays of the .bin layout (no device needed).
     Returns (arrays, relu_layers)."""
@@ -718,9 +740,26 @@ class Context:
         (GPDB_DEPTH_U16). Returns one list of (image [height, width], camera) per view, what preprocess_depth() takes,
         and with face_ids also one list of int32 face images per view (the view-local face each return hit, -1 where
         the pixel has none)."""
+        return self._render_views("render_depth", lib().gpdb_render_depth, (), meshes, cameras_per_view, dtype, face_ids)
+
+    def render_sensor_depth(self, meshes, cameras_per_view, sensor, seed, dtype=np.float32, face_ids=False):
+        """gpdb_render_sensor_depth: render_depth() seen by the structured-light sensor `sensor` (a sensor_params()),
+        view b with the key seed + b (include/gpd_b200_sensor.h): projector shadows, grazing-angle dropouts, disparity
+        noise and quantisation, lateral jitter and dropout. Returns what render_depth() returns; with sensor_params()'s
+        zeros it equals render_depth() bit for bit."""
+        return self._render_views("render_sensor_depth", lib().gpdb_render_sensor_depth, self._sensor_args(sensor, seed),
+                                  meshes, cameras_per_view, dtype, face_ids)
+
+    @staticmethod
+    def _sensor_args(sensor, seed):
+        if not isinstance(sensor, abi.SensorParams):
+            raise TypeError(f"sensor: need a sensor_params(), got {type(sensor).__name__}")
+        return (C.c_void_p(C.addressof(sensor)), C.c_uint64(int(seed) % 2 ** 64))
+
+    def _render_views(self, name, fn, extra, meshes, cameras_per_view, dtype, face_ids):
         fmt = {np.dtype(np.float32): abi.DEPTH_F32, np.dtype(np.uint16): abi.DEPTH_U16}.get(np.dtype(dtype))
         if fmt is None:
-            raise TypeError(f"render_depth: dtype must be float32 or uint16, got {np.dtype(dtype)}")
+            raise TypeError(f"{name}: dtype must be float32 or uint16, got {np.dtype(dtype)}")
         if len(cameras_per_view) != len(meshes):
             raise ValueError(f"cameras_per_view: {len(cameras_per_view)} lists, need one per mesh ({len(meshes)})")
         m = pack_meshes(meshes)
@@ -729,9 +768,8 @@ class Context:
         n = sum(int(c.width) * int(c.height) for c in cams)
         depth = np.zeros(n, dtype)
         face = np.zeros(n, np.int32) if face_ids else None
-        self._check(lib().gpdb_render_depth(self.h, len(ks), _p(m["vertex_offsets"]), _p(m["vertices"]),
-                                            _p(m["face_offsets"]), _p(m["faces"]), _p(ks), C.cast(arr, C.c_void_p), fmt,
-                                            _p(depth), _p(face)))
+        self._check(fn(self.h, len(ks), _p(m["vertex_offsets"]), _p(m["vertices"]), _p(m["face_offsets"]), _p(m["faces"]),
+                       _p(ks), C.cast(arr, C.c_void_p), fmt, _p(depth), _p(face), *extra))
         views, faces, o, k = [], [], 0, 0
         for cs in cameras_per_view:
             views.append([])
@@ -751,11 +789,24 @@ class Context:
         cameras are host arrays). dtype torch.float32 (default) or torch.uint16. Returns ONE depth tensor holding every
         camera's image back to back, as preprocess_depth_tensors() takes it, and with face_ids also the int32 face
         tensor of the same length."""
+        return self._render_tensors("render_depth_tensors", lib().gpdb_render_depth_device, (), vertex_offsets, vertices,
+                                    face_offsets, faces, n_cameras, cameras, dtype, face_ids)
+
+    def render_sensor_depth_tensors(self, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras, sensor, seed,
+                                    dtype=None, face_ids=False):
+        """gpdb_render_sensor_depth_device: render_sensor_depth() of meshes held in CUDA tensors, laid out as
+        render_depth_tensors() takes them. Returns what render_depth_tensors() returns."""
+        return self._render_tensors("render_sensor_depth_tensors", lib().gpdb_render_sensor_depth_device,
+                                    self._sensor_args(sensor, seed), vertex_offsets, vertices, face_offsets, faces,
+                                    n_cameras, cameras, dtype, face_ids)
+
+    def _render_tensors(self, name, fn, extra, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras, dtype,
+                        face_ids):
         import torch
         dtype = torch.float32 if dtype is None else dtype
         fmt = {torch.float32: abi.DEPTH_F32, torch.uint16: abi.DEPTH_U16}.get(dtype)
         if fmt is None:
-            raise TypeError(f"render_depth_tensors: dtype must be torch.float32 or torch.uint16, got {dtype}")
+            raise TypeError(f"{name}: dtype must be torch.float32 or torch.uint16, got {dtype}")
         voff, foff = _host_i32("vertex_offsets", vertex_offsets), _host_i32("face_offsets", face_offsets)
         if len(voff) < 2 or len(foff) != len(voff):
             raise ValueError(f"vertex_offsets / face_offsets: {len(voff)} / {len(foff)} entries, need B + 1 each (B >= 1)")
@@ -769,9 +820,8 @@ class Context:
         depth = torch.empty(n, dtype=dtype, device=f"cuda:{dev}")
         face = torch.empty(n, dtype=torch.int32, device=f"cuda:{dev}") if face_ids else None
         self._torch_stream()
-        self._check(lib().gpdb_render_depth_device(self.h, len(ks), _p(voff), pv, _p(foff), pf, _p(ks),
-                                                   C.cast(arr, C.c_void_p), fmt, C.c_void_p(depth.data_ptr()),
-                                                   None if face is None else C.c_void_p(face.data_ptr())))
+        self._check(fn(self.h, len(ks), _p(voff), pv, _p(foff), pf, _p(ks), C.cast(arr, C.c_void_p), fmt,
+                       C.c_void_p(depth.data_ptr()), None if face is None else C.c_void_p(face.data_ptr()), *extra))
         return (depth, face) if face_ids else depth
 
     def sample_meshes(self, meshes, density, seed, face_ids=False):

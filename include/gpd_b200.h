@@ -750,6 +750,40 @@ int gpdb_sample_meshes_device(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *ve
                               const int32_t *face_offsets, const int32_t *d_faces, double density, uint64_t seed,
                               int32_t *point_offsets_out, float *d_xyz_out, double *d_normals_out, int32_t *d_face_out);
 
+/* The structured-light sensor model of gpdb_render_sensor_depth[_device] (rules in gpd_b200_sensor.h). Every field 0
+ * (gpdb_sensor_params_default) is a clean render. */
+typedef struct gpdb_sensor_params {
+  double baseline;          /* metres from the camera to the projector along the camera's +x; 0 disables rules 5, 6 */
+  double lateral_sigma;     /* pixels: the spread of the pixel each return is read from (rule 3)                  */
+  double disparity_sigma;   /* pixels: the spread of the disparity (rule 6)                                       */
+  double disparity_step;    /* pixels: the disparity quantum; 0 means no quantisation (rule 6)                    */
+  double min_cos_incidence; /* no return below this cosine of the incidence angle; 0 disables rule 4             */
+  double shadow_tolerance;  /* relative depth slack of the projector's visibility test (rule 5), < 1             */
+  double dropout;           /* the probability in [0, 1] of dropping a return (rule 7)                            */
+} gpdb_sensor_params;
+
+/* Every field 0: a clean render. */
+void gpdb_sensor_params_default(gpdb_sensor_params *p);
+
+/* gpdb_render_depth's arguments, then the sensor model and the seed: the same images seen as a structured-light sensor
+ * sees them (projector shadows, grazing-angle dropouts, quantised disparity noise, lateral jitter, dropout), view b with
+ * the key seed + b (gpd_b200_sensor.h). With every sensor field 0 the outputs equal gpdb_render_depth's bit for bit.
+ * GPDB_ERR_INVALID, nothing written: gpdb_render_depth's errors, sensor NULL, and the parameter rules of
+ * gpd_b200_sensor.h 9. Returns n_views. */
+int gpdb_render_sensor_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                             const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out,
+                             const gpdb_sensor_params *sensor, uint64_t seed);
+/* The same with vertices, faces and the outputs in device memory (offsets, cameras and the sensor model stay host
+ * memory), on the context's stream. */
+int gpdb_render_sensor_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                                    const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                                    int32_t *d_face_out, const gpdb_sensor_params *sensor, uint64_t seed);
+/* Development aid: the float64 inverse-normal table of gpd_b200_sensor.h rule 2 (table_out [4097], host), the bytes the
+ * device interpolates. Needs no device. Returns 4097. */
+int gpdb_debug_sensor_table(double *table_out);
+
 /* Replaces: freeMemoryGrasps (detect_grasps_python.cpp:598-601). The arrays of a result live in page-locked host memory
  * owned by the library (the device writes them directly, overlapped with compute); gpdb_free_result hands that memory
  * back for the next call. A result may outlive its context. */
