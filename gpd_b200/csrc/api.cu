@@ -1,6 +1,9 @@
-// api.cu — the C-ABI of libgpd_b200.so (include/gpd_b200.h): context, cloud upload, the chunked
-// detect pipeline and the stage-level entry points. Host-side logic only; kernels live in
-// geometry.cu / lenet_simt.cu / lenet_tc.cu. There is no CPU fallback anywhere in this library.
+// api.cu — the C-ABI of libgpd_b200.so (include/gpd_b200.h): the context, the cloud store, the checks the other entry
+// points share (common.cuh), the chunked detect pipeline and the detect / hand-search / frames / images / classify /
+// reevaluate / cluster entry points. Host-side logic only; their kernels live in geometry.cu / lenet_simt.cu /
+// lenet_tc.cu. The depth, mesh, organized-normal, plane, refinement, outlier, training and SIS entry points sit beside
+// their kernels, in depth.cu / render.cu / organized.cu / plane.cu / refine.cu / outliers.cu / train.cu / sis.cu.
+// There is no CPU fallback anywhere in this library.
 #include <atomic>
 #include <cfloat>
 #include <cmath>
@@ -14,12 +17,6 @@
 #include <utility>
 #include <vector>
 
-#include "../../include/gpd_b200_depth.h"
-#include "../../include/gpd_b200_outliers.h"
-#include "../../include/gpd_b200_plane.h"
-#include "../../include/gpd_b200_refine.h"
-#include "../../include/gpd_b200_sensor.h"
-#include "../../include/gpd_b200_train.h"
 #include "common.cuh"
 
 static char g_create_err[512] = "";
@@ -48,19 +45,6 @@ void gpdb_st_end(gpdb_ctx *ctx, int stage, cudaEvent_t begin) {
   cudaEvent_t e = ctx->st->get();
   cudaEventRecord(e, ctx->stream);
   ctx->st->spans.push_back({stage, begin, e});
-}
-// What the last SIS call evaluated and kept, for gpdb_sis_positions (gpdb_sis_batch): the counts on
-// the host, the positions in SCR_SIS
-struct SisState {
-  bool valid = false;
-  int B = 0, R = 0, S = 0;
-  std::vector<int> init_off;  // [B + 1] initial samples per cloud (they size the kept arena)
-  std::vector<int> ecount;    // [R * B] round-major, as the device holds them
-  std::vector<int> koff;      // [B + 1] kept positions per cloud
-};
-// a new batch, or a SIS call that fails, leaves nothing for gpdb_sis_positions to read
-static void gpdb_sis_forget(gpdb_ctx *ctx) {
-  if (ctx->sis) ctx->sis->valid = false;
 }
 
 static void st_collect(gpdb_ctx *ctx, double *ms) {
@@ -406,7 +390,7 @@ void gpdb_destroy(gpdb_ctx *ctx) {
   cudaFree(ctx->d_prof);
   cudaFree(ctx->d_qtab);
   cudaFree(ctx->d_sel);
-  delete ctx->sis;
+  sis_free(ctx);
   cloud_free(ctx->one);
   cloud_free(ctx->many);
   float *w[8] = {ctx->w.c1w, ctx->w.c1b, ctx->w.c2w, ctx->w.c2b, ctx->w.i1w, ctx->w.i1b, ctx->w.i2w, ctx->w.i2b};
@@ -531,11 +515,8 @@ int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *
 
 // ---- the device-resident entry points (gpdb_*_device): bulk arrays in device memory, sizes and offsets on the host ----
 
-static const unsigned long long NO_BAD = ~0ull;  // the check word when no position offends
-
-// every non-null pointer must be device (or managed) memory of the context's device; runs before any device work
-static int check_device_ptrs(gpdb_ctx *ctx, const char *name,
-                             std::initializer_list<std::pair<const char *, const void *>> ptrs) {
+int gpdb_check_device_ptrs(gpdb_ctx *ctx, const char *name,
+                           std::initializer_list<std::pair<const char *, const void *>> ptrs) {
   for (const auto &p : ptrs) {
     if (!p.second) continue;
     cudaPointerAttributes a;
@@ -549,42 +530,22 @@ static int check_device_ptrs(gpdb_ctx *ctx, const char *name,
   return GPDB_OK;
 }
 
-// The check-word protocol of the device-side checks. The word, at the head of SCR_CHECK, is set to all ones;
-// enqueue(d_bad, d_extra) queues the kernel that lowers it to the first offending position, with `extra` bytes behind the
-// word for the check's own arrays; *bad receives the word (NO_BAD: nothing offends) once the stream has drained.
-template <class Enqueue>
-static int first_bad(gpdb_ctx *ctx, size_t extra, unsigned long long *bad, Enqueue enqueue) {
-  unsigned long long *d_bad = (unsigned long long *)gpdb_scratch(ctx, SCR_CHECK, sizeof(*d_bad) + extra);
-  if (!d_bad) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
-  const int rc = enqueue(d_bad, d_bad + 1);
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(bad, d_bad, sizeof(*bad), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return GPDB_OK;
-}
-
 // ---- the checks shared by the batch entry points and their _device twins ----------------------------------------------
 
-// what every call that installs a batch does first: a failed call leaves no batch, no sample positions and no SIS record
-// behind (the SIS positions describe clouds that are gone); the single cloud is never touched
-static void drop_batch(gpdb_ctx *ctx) {
+void gpdb_drop_batch(gpdb_ctx *ctx) {
   ctx->many.n = 0;
   ctx->many.has_src = false;
   ctx->many.n_samples = 0;
-  gpdb_sis_forget(ctx);
+  sis_forget(ctx);
 }
 
-// GPDB_ERR_STATE unless a batch is installed; hint names the calls that install one
-static int need_batch(gpdb_ctx *ctx, const char *name, const char *hint) {
+int gpdb_need_batch(gpdb_ctx *ctx, const char *name, const char *hint) {
   if (ctx->many.n) return GPDB_OK;
   gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: no batch of clouds: call %s first", name, hint);
   return GPDB_ERR_STATE;
 }
 
-// CSR offsets off[B+1] (the array `label`) from the host: they start at 0 and never decrease; entry b belongs to the b-th
-// `unit` (cloud or group). A call whose start message lists other arguments too checks the start itself first.
-static int check_offsets(gpdb_ctx *ctx, const char *name, const char *label, const int32_t *off, int B, const char *unit) {
+int gpdb_check_offsets(gpdb_ctx *ctx, const char *name, const char *label, const int32_t *off, int B, const char *unit) {
   if (!off || off[0] != 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need %s[%d] starting at 0", name, label, B + 1);
     return GPDB_ERR_INVALID;
@@ -597,12 +558,8 @@ static int check_offsets(gpdb_ctx *ctx, const char *name, const char *label, con
   return GPDB_OK;
 }
 
-// The cloud-local indices d_idx[off[b] .. off[b+1]) of cloud b of the installed batch must lie in [0, N_b + M_b), M_b
-// its sample positions. The list d_idx and its offsets d_off are in device memory, off is the host copy of d_off;
-// batch_check_samples finds the first offending position, which the message names. init: the initial indices of
-// gpdb_sis_batch, which has dropped the positions (M_b = 0) and names the indices so.
-static int check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *d_idx,
-                               const int *d_off) {
+int gpdb_check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *d_idx,
+                             const int *d_off) {
   const CloudSet &s = ctx->many;
   const int B = s.n, n = off[B];
   if (n == 0) return GPDB_OK;
@@ -730,10 +687,6 @@ static int set_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32_t B, c
   return rc == GPDB_OK ? B : rc;
 }
 
-static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
-                              const gpdb_preprocess_params *pp, int32_t *poff,
-                              const std::function<int()> &after_normals = nullptr);
-
 // gpdb_preprocess_clouds into store s after the argument checks (gpdb_preprocess: `one`, a batch of one); a failed call
 // leaves no cloud in s. device: xyz, normals and cam_source are the caller's device arrays, read in place; else host
 // arrays uploaded here. Either way the camera masks are packed on the device.
@@ -783,15 +736,11 @@ static int preprocess_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int32
   // ---- removeNans + filterWorkspace + voxelizeCloud of every cloud, into the store's arenas
   rc = pre_filter_voxelize_batch(ctx, s, d_xyz_raw, d_cam_raw, d_nrm_raw, M, B, roff, *pp, poff, ev[2]);
   if (rc != GPDB_OK) return rc;
-  return preprocess_install(ctx, s, desc.data(), B, roff, pp, poff);
+  return gpdb_preprocess_install(ctx, s, desc.data(), B, roff, pp, poff);
 }
 
-// The steps of a preprocessing call after the filter and voxelisation (store s holds the processed points, poff[B+1] their
-// offsets, desc[B] the camera fields): install with one grid per cloud, normals, nonunit flags, stage timings, and the
-// raw offsets roff[B+1] the source indices refer to. after_normals (may be empty) runs between the normal estimation and
-// the nonunit flags, inside the normals' stage timing. A failure leaves no cloud in s.
-static int preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
-                              const gpdb_preprocess_params *pp, int32_t *poff, const std::function<int()> &after_normals) {
+int gpdb_preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
+                            const gpdb_preprocess_params *pp, int32_t *poff, const std::function<int()> &after_normals) {
   cudaEvent_t *ev = ctx->ev;
   cudaEventRecord(ev[3], ctx->stream);
   // ---- install, one grid per cloud
@@ -855,8 +804,7 @@ static int get_clouds(gpdb_ctx *ctx, CloudSet &s, float *xyz_out, double *normal
   return (int)N;
 }
 
-// drops the sample positions of store s and makes its arena hold n positions (grown, never shrunk)
-static int reserve_samples(gpdb_ctx *ctx, CloudSet &s, int n) {
+int gpdb_reserve_samples(gpdb_ctx *ctx, CloudSet &s, int n) {
   CUDA_TRY(cudaSetDevice(ctx->device));
   s.n_samples = 0;
   if ((size_t)n > s.samples_cap) {
@@ -874,7 +822,7 @@ static int reserve_samples(gpdb_ctx *ctx, CloudSet &s, int n) {
 
 // replaces the sample positions of store s by n host positions (3 x n, column-major; n == 0: none)
 static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int n) {
-  const int rc = reserve_samples(ctx, s, n);
+  const int rc = gpdb_reserve_samples(ctx, s, n);
   if (rc != GPDB_OK || n == 0) return rc;
   CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
@@ -882,8 +830,7 @@ static int upload_samples(gpdb_ctx *ctx, CloudSet &s, const double *samples, int
   return GPDB_OK;
 }
 
-// the preprocessing parameters, against the caller's normals (null: none)
-static int check_preprocess_params(gpdb_ctx *ctx, const char *name, const gpdb_preprocess_params *pp, const double *normals) {
+int gpdb_check_preprocess_params(gpdb_ctx *ctx, const char *name, const gpdb_preprocess_params *pp, const double *normals) {
   if (!pp->estimate_normals && !normals) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals = 0 needs the caller's normals", name);
     return GPDB_ERR_INVALID;
@@ -929,7 +876,7 @@ int gpdb_preprocess(gpdb_ctx *ctx, const float *xyz, const double *normals, cons
                    GPDB_MAX_CAMERAS);
     return GPDB_ERR_INVALID;
   }
-  int rc = check_preprocess_params(ctx, "gpdb_preprocess", pp, normals);
+  int rc = gpdb_check_preprocess_params(ctx, "gpdb_preprocess", pp, normals);
   if (rc != GPDB_OK) return rc;
   const int32_t roff[2] = {0, M};
   int32_t poff[2] = {0, 0};
@@ -967,16 +914,16 @@ static int set_clouds_samples(gpdb_ctx *ctx, const char *name, const int32_t *po
   if (!ctx) return GPDB_ERR_INVALID;
   CloudSet &s = ctx->many;
   s.n_samples = 0;  // past this point, a failed call leaves no positions behind
-  int rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds");
+  int rc = gpdb_need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds");
   if (rc != GPDB_OK) return rc;
   const int B = s.n;
-  if ((rc = check_offsets(ctx, name, "pos_offsets", pos_offsets, B, "cloud")) != GPDB_OK) return rc;
+  if ((rc = gpdb_check_offsets(ctx, name, "pos_offsets", pos_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int M = pos_offsets[B];
   if (M > 0 && !samples) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null samples_xyz for %d positions", name, M);
     return GPDB_ERR_INVALID;
   }
-  if (device && (rc = check_device_ptrs(ctx, name, {{"d_samples_xyz", samples}})) != GPDB_OK) return rc;
+  if (device && (rc = gpdb_check_device_ptrs(ctx, name, {{"d_samples_xyz", samples}})) != GPDB_OK) return rc;
   memcpy(s.pos, pos_offsets, sizeof(int) * ((size_t)B + 1));
   // each descriptor's first position: one strided copy into the pos field of the B device descriptors
   CUDA_TRY(cudaSetDevice(ctx->device));
@@ -986,7 +933,7 @@ static int set_clouds_samples(gpdb_ctx *ctx, const char *name, const int32_t *po
     rc = upload_samples(ctx, s, samples, M);
     return rc < 0 ? rc : M;
   }
-  if ((rc = reserve_samples(ctx, s, M)) != GPDB_OK) return rc;
+  if ((rc = gpdb_reserve_samples(ctx, s, M)) != GPDB_OK) return rc;
   if (M > 0)
     CUDA_TRY(cudaMemcpyAsync(s.samples, samples, sizeof(double) * 3 * (size_t)M, cudaMemcpyDeviceToDevice, ctx->stream));
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
@@ -1505,7 +1452,7 @@ static int clouds_entry(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const
                         const double *normals, const int32_t *cam_source, const int32_t *n_cameras, const double *view_points,
                         const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool raw, bool device) {
   if (!ctx) return GPDB_ERR_INVALID;
-  drop_batch(ctx);
+  gpdb_drop_batch(ctx);
   if (n_clouds <= 0 || !point_offsets || !n_cameras || !xyz || !view_points || point_offsets[0] != 0 ||
       (raw ? !pp || !processed_offsets_out : !normals)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, point_offsets (starting at 0), n_cameras, xyz, %s", name,
@@ -1524,9 +1471,9 @@ static int clouds_entry(gpdb_ctx *ctx, const char *name, int32_t n_clouds, const
       return GPDB_ERR_INVALID;
     }
   }
-  int rc = raw ? check_preprocess_params(ctx, name, pp, normals) : GPDB_OK;
+  int rc = raw ? gpdb_check_preprocess_params(ctx, name, pp, normals) : GPDB_OK;
   if (rc == GPDB_OK && device)
-    rc = check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals", normals}, {"d_cam_source", cam_source}});
+    rc = gpdb_check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals", normals}, {"d_cam_source", cam_source}});
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
   if (raw)
@@ -1567,706 +1514,13 @@ int gpdb_preprocess_clouds_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t
 
 int gpdb_get_clouds(gpdb_ctx *ctx, float *xyz_out, double *normals_out, int32_t *cam_source_out, int32_t *src_out) {
   if (!ctx) return GPDB_ERR_INVALID;
-  const int rc = need_batch(ctx, "gpdb_get_clouds", "gpdb_set_clouds / gpdb_preprocess_clouds");
+  const int rc = gpdb_need_batch(ctx, "gpdb_get_clouds", "gpdb_set_clouds / gpdb_preprocess_clouds");
   if (rc != GPDB_OK) return rc;
   if (src_out && !ctx->many.has_src) {
     gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_get_clouds: source indices exist after gpdb_preprocess_clouds only");
     return GPDB_ERR_STATE;
   }
   return get_clouds(ctx, ctx->many, xyz_out, normals_out, cam_source_out, src_out);
-}
-
-}  // extern "C"
-
-// ---- depth images and Cloud::subsample (include/gpd_b200_depth.h) ------------------------------------------------------
-
-// The camera checks of gpdb_preprocess_depth[_device] and gpdb_render_depth[_device]: view b has n_cameras[b] (1..8)
-// cameras, each of them well formed, and the call holds fewer than 2^31 pixels; roff[B+1] receives the raw offsets
-// (cumulative pixels per view)
-static int check_depth_cameras(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras,
-                               const gpdb_depth_camera *cams, std::vector<int> &roff) {
-  roff.assign((size_t)B + 1, 0);
-  long long total = 0;
-  for (int b = 0, c = 0; b < B; b++) {
-    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d has %d cameras (1 <= cameras <= %d)", name, b, n_cameras[b],
-                     GPDB_MAX_CAMERAS);
-      return GPDB_ERR_INVALID;
-    }
-    for (int k = 0; k < n_cameras[b]; k++, c++) {
-      const gpdb_depth_camera &D = cams[c];
-      const char *bad = nullptr;
-      bool finite = std::isfinite(D.fx) && std::isfinite(D.fy) && std::isfinite(D.cx) && std::isfinite(D.cy);
-      for (int e = 0; e < 12; e++) finite = finite && std::isfinite(D.pose[e]);
-      if (D.width < 1 || D.height < 1) bad = "width and height must be at least 1";
-      else if (!finite) bad = "non-finite intrinsics or pose";
-      else if (!(D.fx > 0.0) || !(D.fy > 0.0)) bad = "fx and fy must be positive";
-      else if (!(D.depth_scale > 0.0) || !std::isfinite(D.depth_scale)) bad = "depth_scale must be finite and positive";
-      else if (!(D.min_depth >= 0.0)) bad = "min_depth must be >= 0";
-      else if (!(D.max_depth > D.min_depth)) bad = "max_depth must exceed min_depth";
-      if (bad) {
-        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d (camera %d of the call): %s", name, b, k, c, bad);
-        return GPDB_ERR_INVALID;
-      }
-      total += (long long)D.width * D.height;
-      if (total >= (1ll << 31)) {
-        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d: the call holds 2^31 or more pixels", name, b, k);
-        return GPDB_ERR_INVALID;
-      }
-    }
-    roff[b + 1] = (int)total;
-  }
-  return GPDB_OK;
-}
-
-// the argument checks of gpdb_preprocess_depth[_device]; roff[B+1] receives the raw offsets (cumulative pixels per view)
-static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
-                            int32_t format, const void *depth, const gpdb_preprocess_params *pp, const int32_t *poff,
-                            std::vector<int> &roff) {
-  if (B <= 0 || !n_cameras || !cams || !depth || !pp || !poff) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth, params, processed_offsets_out",
-                   name);
-    return GPDB_ERR_INVALID;
-  }
-  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
-    return GPDB_ERR_INVALID;
-  }
-  if (!pp->estimate_normals) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
-    return GPDB_ERR_INVALID;
-  }
-  const int rc = check_preprocess_params(ctx, name, pp, nullptr);
-  if (rc != GPDB_OK) return rc;
-  return check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
-}
-
-// gpdb_preprocess_depth[_device] after the argument checks: d_depth in device memory (the host twin has uploaded it)
-// organized: the normals of gpd_b200_organized.h rule 7 replace the radius estimates (n_fallback[B], host, may be null)
-static int preprocess_depth(gpdb_ctx *ctx, const char *name, CloudSet &s, int32_t B, const int32_t *n_cameras,
-                            const gpdb_depth_camera *cams, int32_t format, const void *depth, bool device,
-                            const gpdb_preprocess_params *pp, const std::vector<int> &roff, int32_t *poff, bool organized,
-                            int32_t *n_fallback) {
-  cudaEvent_t *ev = ctx->ev;
-  const int M = roff[B];
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  cudaEventRecord(ev[0], ctx->stream);
-  const void *d_depth = depth;
-  if (!device) {
-    const size_t bytes = (size_t)M * (format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float));
-    void *up = gpdb_scratch(ctx, SCR_UPLOAD, bytes);
-    if (!up) return GPDB_ERR_CUDA;
-    CUDA_TRY(cudaMemcpyAsync(up, depth, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    d_depth = up;
-  }
-  // the camera fields of the descriptors: view point k = t of camera k; one-hot camera sources, as a cam_source matrix
-  std::vector<CloudDesc> desc((size_t)B);
-  for (int b = 0, c = 0; b < B; b++) {
-    CloudDesc &D = desc[b];
-    memset(&D, 0, sizeof(D));
-    D.K = n_cameras[b];
-    for (int k = 0; k < D.K; k++, c++)
-      for (int r = 0; r < 3; r++) D.vp[k][r] = cams[c].pose[4 * r + 3];
-  }
-  cudaEventRecord(ev[1], ctx->stream);
-  int rc = pre_depth_batch(ctx, s, d_depth, format, cams, n_cameras, B, roff.data(), *pp, poff, ev[2]);
-  if (rc != GPDB_OK) return rc;
-  if (!organized) return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff);
-  // the host twin's images stay in SCR_UPLOAD until here: the install does not use that slot
-  return preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff, [&]() {
-    return org_depth_normals(ctx, name, s, d_depth, format, cams, n_cameras, B, n_fallback);
-  });
-}
-
-static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const int32_t *n_cameras,
-                       const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
-                       const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device,
-                       bool organized = false, int32_t *n_fallback = nullptr) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  drop_batch(ctx);
-  std::vector<int> roff;
-  int rc = check_depth_args(ctx, name, n_views, n_cameras, cameras, depth_format, depth, pp, processed_offsets_out, roff);
-  if (rc == GPDB_OK && device) rc = check_device_ptrs(ctx, name, {{"d_depth", depth}});
-  if (rc != GPDB_OK) return rc;
-  return preprocess_depth(ctx, name, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
-                          processed_offsets_out, organized, n_fallback);
-}
-
-// gpdb_normals_organized[_device]: the argument checks, then rules 2 - 5 of gpd_b200_organized.h on every cloud
-static int organized_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *W, const int32_t *H, const float *xyz,
-                           const float *view_points, float *normals_out, float *distance_out, bool device) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  if (B <= 0 || !W || !H || !xyz || !view_points || !normals_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, widths, heights, xyz, view_points, normals_out", name);
-    return GPDB_ERR_INVALID;
-  }
-  long long total = 0;
-  for (int b = 0; b < B; b++) {
-    if (W[b] < 1 || H[b] < 1) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d is %d x %d (width and height must be at least 1)", name, b, W[b],
-                     H[b]);
-      return GPDB_ERR_INVALID;
-    }
-    total += (long long)W[b] * H[b];
-    if (total >= (1ll << 31)) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: the call holds 2^31 or more points", name, b);
-      return GPDB_ERR_INVALID;
-    }
-  }
-  int rc = device ? check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals_out", normals_out},
-                                                  {"d_distance_out", distance_out}})
-                  : GPDB_OK;
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  rc = org_normals_batch(ctx, name, B, W, H, xyz, view_points, normals_out, distance_out, device);
-  return rc == GPDB_OK ? B : rc;
-}
-
-// gpdb_subsample_clouds[_device]: the state and argument checks, then the device draw (the host twin uploads the mask and
-// copies the indices back)
-static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples, uint64_t seed, const uint8_t *mask,
-                           int32_t *idx_out, int32_t *offsets_out, bool device, bool per_point = false) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  CloudSet &s = ctx->many;
-  int rc = need_batch(ctx, name, "gpdb_preprocess_depth / gpdb_preprocess_clouds");
-  if (rc != GPDB_OK) return rc;
-  if (num_samples < 0 || !offsets_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need num_samples >= 0 (got %d) and sample_offsets_out", name, num_samples);
-    return GPDB_ERR_INVALID;
-  }
-  if (mask && !per_point && !s.has_src) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: a mask needs the source indices of a preprocessing call (gpdb_preprocess_depth "
-                   "/ gpdb_preprocess_clouds); the batch was installed by gpdb_set_clouds", name);
-    return GPDB_ERR_STATE;
-  }
-  const int B = s.n;
-  long long room = 0;
-  for (int b = 0; b < B; b++) {
-    const int nb = s.off[b + 1] - s.off[b];
-    room += num_samples == 0 ? nb : std::min(num_samples, nb);
-  }
-  if (room > 0 && !idx_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, device ? "d_sample_idx_out" : "sample_idx_out");
-    return GPDB_ERR_INVALID;
-  }
-  if (device && (rc = check_device_ptrs(ctx, name, {{"d_mask", mask}, {"d_sample_idx_out", idx_out}})) != GPDB_OK) return rc;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  const uint8_t *d_mask = mask;
-  int *d_out = idx_out;
-  if (!device) {
-    if (mask) {
-      const size_t M = per_point ? (size_t)s.points() : (size_t)s.raw_off[B];
-      uint8_t *up = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, M);
-      if (!up) return GPDB_ERR_CUDA;
-      CUDA_TRY(cudaMemcpyAsync(up, mask, M, cudaMemcpyHostToDevice, ctx->stream));
-      d_mask = up;
-    }
-    d_out = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)room);
-    if (!d_out) return GPDB_ERR_CUDA;
-  }
-  std::vector<int> soff((size_t)B + 1);
-  const int n = sub_draw_batch(ctx, s, num_samples, seed, d_mask, per_point, d_out, soff.data());
-  if (n < 0) return n;
-  if (!device && n > 0) {
-    CUDA_TRY(cudaMemcpyAsync(idx_out, d_out, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  }
-  memcpy(offsets_out, soff.data(), sizeof(int) * ((size_t)B + 1));
-  return n;
-}
-
-// ---- triangle meshes: depth images and surface samples (include/gpd_b200_render.h) ----------------------------------
-
-// the offsets of B meshes (rule 7): vertex_offsets and face_offsets start at 0 and never decrease, and the arrays they
-// address are given; `unit` names a mesh in the messages
-static int check_mesh_args(gpdb_ctx *ctx, const char *name, const char *unit, int32_t B, const int32_t *voff,
-                           const float *vertices, const int32_t *foff, const int32_t *faces) {
-  int rc = check_offsets(ctx, name, "vertex_offsets", voff, B, unit);
-  if (rc == GPDB_OK) rc = check_offsets(ctx, name, "face_offsets", foff, B, unit);
-  if (rc != GPDB_OK) return rc;
-  if ((voff[B] > 0 && !vertices) || (foff[B] > 0 && !faces)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null vertices or faces for %d vertices and %d faces", name, voff[B], foff[B]);
-    return GPDB_ERR_INVALID;
-  }
-  return GPDB_OK;
-}
-
-// rule 7's device checks of B meshes in device memory: a non-finite vertex or a face index outside its mesh's vertices,
-// the first of them named
-static int check_meshes(gpdb_ctx *ctx, const char *name, const char *unit, int B, const int32_t *voff, const int32_t *foff,
-                        const float *d_vtx, const int32_t *d_faces) {
-  const int V = voff[B], F = foff[B];
-  const size_t bytes = sizeof(int) * 2 * ((size_t)B + 1);
-  unsigned long long bad;
-  const int rc = first_bad(ctx, bytes, &bad, [&](unsigned long long *d_bad, void *d) -> int {
-    int *d_voff = (int *)d, *d_foff = d_voff + B + 1;
-    CUDA_TRY(cudaMemcpyAsync(d_voff, voff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-    CUDA_TRY(cudaMemcpyAsync(d_foff, foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-    return mesh_check(ctx, d_voff, d_foff, B, V, F, d_vtx, d_faces, d_bad);
-  });
-  if (rc != GPDB_OK || bad == NO_BAD) return rc;
-  int b = 0;
-  if (bad < (unsigned long long)V) {
-    while (voff[b + 1] <= (long long)bad) b++;
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: vertex %d has a non-finite coordinate", name, unit, b,
-                   (int)(bad - voff[b]));
-    return GPDB_ERR_INVALID;
-  }
-  const int f = (int)(bad - V);
-  while (foff[b + 1] <= f) b++;
-  int32_t tri[3];
-  CUDA_TRY(cudaMemcpyAsync(tri, d_faces + 3 * (size_t)f, sizeof(tri), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: face %d = (%d, %d, %d) indexes outside its %d vertices", name, unit, b,
-                 f - foff[b], tri[0], tri[1], tri[2], voff[b + 1] - voff[b]);
-  return GPDB_ERR_INVALID;
-}
-
-// gpd_b200_sensor.h rule 9's parameter checks
-static int check_sensor_params(gpdb_ctx *ctx, const char *name, const gpdb_sensor_params *sp) {
-  if (!sp) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need sensor (gpdb_sensor_params_default for a clean render)", name);
-    return GPDB_ERR_INVALID;
-  }
-  const struct {
-    const char *name;
-    double v;
-  } f[] = {{"baseline", sp->baseline},
-           {"lateral_sigma", sp->lateral_sigma},
-           {"disparity_sigma", sp->disparity_sigma},
-           {"disparity_step", sp->disparity_step},
-           {"min_cos_incidence", sp->min_cos_incidence},
-           {"shadow_tolerance", sp->shadow_tolerance},
-           {"dropout", sp->dropout}};
-  const char *bad = nullptr;
-  for (const auto &e : f)
-    if (!(e.v >= 0.0) || !std::isfinite(e.v)) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s must be finite and >= 0 (got %g)", name, e.name, e.v);
-      return GPDB_ERR_INVALID;
-    }
-  if (sp->dropout > 1.0) bad = "dropout must lie in [0, 1]";
-  else if (sp->shadow_tolerance >= 1.0) bad = "shadow_tolerance must be < 1";
-  else if (sp->min_cos_incidence > 1.0) bad = "min_cos_incidence must be <= 1";
-  else if ((sp->disparity_sigma > 0.0 || sp->disparity_step > 0.0) && !(sp->baseline > 0.0))
-    bad = "disparity_sigma and disparity_step need a baseline > 0";
-  if (bad) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s", name, bad);
-    return GPDB_ERR_INVALID;
-  }
-  return GPDB_OK;
-}
-
-// gpdb_render_depth[_device] and (sensor) gpdb_render_sensor_depth[_device]: the checks, then the device render (the host
-// twin uploads the meshes into SCR_UPLOAD, renders into it and copies the images back). Nothing installed changes.
-static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
-                        const int32_t *foff, const int32_t *faces, const int32_t *n_cameras, const gpdb_depth_camera *cams,
-                        int32_t format, void *depth_out, int32_t *face_out, bool device, bool sensor = false,
-                        const gpdb_sensor_params *sp = nullptr, uint64_t seed = 0) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  if (B <= 0 || !n_cameras || !cams || !depth_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth_out", name);
-    return GPDB_ERR_INVALID;
-  }
-  if (format != GPDB_DEPTH_U16 && format != GPDB_DEPTH_F32) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
-    return GPDB_ERR_INVALID;
-  }
-  if (sensor && check_sensor_params(ctx, name, sp) != GPDB_OK) return GPDB_ERR_INVALID;
-  std::vector<int> roff;
-  int rc = check_mesh_args(ctx, name, "view", B, voff, vertices, foff, faces);
-  if (rc == GPDB_OK) rc = check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
-  if (rc == GPDB_OK && device)
-    rc = check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_depth_out", depth_out},
-                                       {"d_face_out", face_out}});
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  const size_t V = (size_t)voff[B], F = (size_t)foff[B], M = (size_t)roff[B];
-  const size_t elt = format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float);
-  const float *d_vtx = vertices;
-  const int32_t *d_faces = faces;
-  void *d_depth = depth_out;
-  int32_t *d_face = face_out;
-  if (!device) {
-    float *v;
-    int32_t *f;
-    unsigned char *dd;
-    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
-          v = c.take<float>(3 * V);
-          f = c.take<int32_t>(3 * F);
-          dd = c.take<unsigned char>(elt * M, 16);
-          d_face = face_out ? c.take<int32_t>(M) : nullptr;
-        }))
-      return GPDB_ERR_CUDA;
-    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
-    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
-    d_vtx = v, d_faces = f, d_depth = dd;
-  }
-  if ((rc = check_meshes(ctx, name, "view", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
-  rc = sensor ? render_sensor_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, sp, seed)
-              : render_depth_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face);
-  if (rc != GPDB_OK) return rc;
-  if (!device) {
-    CUDA_TRY(cudaMemcpyAsync(depth_out, d_depth, elt * M, cudaMemcpyDeviceToHost, ctx->stream));
-    if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  }
-  return B;
-}
-
-// gpdb_sample_meshes[_device]: the checks, the count, then (xyz_out given) the points. The host twin uploads the meshes
-// into SCR_UPLOAD, and once the count is known carves the outputs behind them there (uploading again: a grown slot
-// starts empty). Nothing installed changes.
-static int sample_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
-                        const int32_t *foff, const int32_t *faces, double density, uint64_t seed, int32_t *poff_out,
-                        float *xyz_out, double *normals_out, int32_t *face_out, bool device) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  if (B <= 0 || !poff_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_meshes > 0 and point_offsets_out", name);
-    return GPDB_ERR_INVALID;
-  }
-  if (!(density > 0.0) || !std::isfinite(density)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: density must be finite and > 0 (got %g)", name, density);
-    return GPDB_ERR_INVALID;
-  }
-  int rc = check_mesh_args(ctx, name, "mesh", B, voff, vertices, foff, faces);
-  if (rc == GPDB_OK && device)
-    rc = check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_xyz_out", xyz_out},
-                                       {"d_normals_out", normals_out}, {"d_face_out", face_out}});
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  const size_t V = (size_t)voff[B], F = (size_t)foff[B];
-  const float *d_vtx = vertices;
-  const int32_t *d_faces = faces;
-  float *d_xyz = xyz_out;
-  double *d_nrm = normals_out;
-  int32_t *d_face = face_out;
-  // the host twin's buffers: the meshes, then n points of the outputs the caller asked for
-  auto upload = [&](size_t n) -> int {
-    float *v;
-    int32_t *f;
-    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
-          v = c.take<float>(3 * V);
-          f = c.take<int32_t>(3 * F);
-          d_xyz = c.take<float>(3 * n);
-          d_nrm = normals_out ? c.take<double>(3 * n) : nullptr;
-          d_face = face_out ? c.take<int32_t>(n) : nullptr;
-        }))
-      return GPDB_ERR_CUDA;
-    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
-    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
-    d_vtx = v, d_faces = f;
-    return GPDB_OK;
-  };
-  if (!device && (rc = upload(0)) != GPDB_OK) return rc;
-  if ((rc = check_meshes(ctx, name, "mesh", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
-  std::vector<int> poff((size_t)B + 1);
-  std::vector<long long> mesh_n((size_t)B);
-  const long long n = mesh_count_batch(ctx, B, voff, foff, d_vtx, d_faces, density, seed, poff.data(), mesh_n.data());
-  if (n < 0) return (int)n;
-  if (n >= (1ll << 31)) {
-    long long run = 0;
-    int b = 0;
-    while ((run += mesh_n[b]) < (1ll << 31)) b++;
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mesh %d: the call reaches 2^31 or more sampled points (lower the density)",
-                   name, b);
-    return GPDB_ERR_INVALID;
-  }
-  if (xyz_out && n > 0) {
-    if (!device && (rc = upload((size_t)n)) != GPDB_OK) return rc;
-    if ((rc = mesh_write_batch(ctx, B, foff, d_vtx, d_faces, seed, (int)n, d_xyz, d_nrm, d_face)) != GPDB_OK) return rc;
-    if (!device) {
-      CUDA_TRY(cudaMemcpyAsync(xyz_out, d_xyz, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
-      if (normals_out)
-        CUDA_TRY(cudaMemcpyAsync(normals_out, d_nrm, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
-      if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    }
-  }
-  memcpy(poff_out, poff.data(), sizeof(int32_t) * ((size_t)B + 1));
-  return (int)n;
-}
-
-extern "C" {
-
-int gpdb_preprocess_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
-                          int32_t depth_format, const void *depth, const gpdb_preprocess_params *pp,
-                          int32_t *processed_offsets_out) {
-  return depth_entry(ctx, "gpdb_preprocess_depth", n_views, n_cameras, cameras, depth_format, depth, pp,
-                     processed_offsets_out, false);
-}
-
-int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
-                                 int32_t depth_format, const void *d_depth, const gpdb_preprocess_params *pp,
-                                 int32_t *processed_offsets_out) {
-  return depth_entry(ctx, "gpdb_preprocess_depth_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
-                     processed_offsets_out, true);
-}
-
-int gpdb_normals_organized(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights, const float *xyz,
-                           const float *view_points, float *normals_out, float *distance_out) {
-  return organized_entry(ctx, "gpdb_normals_organized", n_clouds, widths, heights, xyz, view_points, normals_out,
-                         distance_out, false);
-}
-
-int gpdb_normals_organized_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights,
-                                  const float *d_xyz, const float *view_points, float *d_normals_out,
-                                  float *d_distance_out) {
-  return organized_entry(ctx, "gpdb_normals_organized_device", n_clouds, widths, heights, d_xyz, view_points,
-                         d_normals_out, d_distance_out, true);
-}
-
-int gpdb_preprocess_depth_organized(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
-                                    const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
-                                    const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
-                                    int32_t *n_fallback_out) {
-  return depth_entry(ctx, "gpdb_preprocess_depth_organized", n_views, n_cameras, cameras, depth_format, depth, pp,
-                     processed_offsets_out, false, true, n_fallback_out);
-}
-
-int gpdb_preprocess_depth_organized_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
-                                           const gpdb_depth_camera *cameras, int32_t depth_format, const void *d_depth,
-                                           const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
-                                           int32_t *n_fallback_out) {
-  return depth_entry(ctx, "gpdb_preprocess_depth_organized_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
-                     processed_offsets_out, true, true, n_fallback_out);
-}
-
-int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *mask, int32_t *sample_idx_out,
-                          int32_t *sample_offsets_out) {
-  return subsample_entry(ctx, "gpdb_subsample_clouds", num_samples, seed, mask, sample_idx_out, sample_offsets_out, false);
-}
-
-int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_mask,
-                                 int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
-  return subsample_entry(ctx, "gpdb_subsample_clouds_device", num_samples, seed, d_mask, d_sample_idx_out,
-                         sample_offsets_out, true);
-}
-
-int gpdb_subsample_clouds_points(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *point_mask,
-                                 int32_t *sample_idx_out, int32_t *sample_offsets_out) {
-  return subsample_entry(ctx, "gpdb_subsample_clouds_points", num_samples, seed, point_mask, sample_idx_out,
-                         sample_offsets_out, false, true);
-}
-
-int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_point_mask,
-                                        int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
-  return subsample_entry(ctx, "gpdb_subsample_clouds_points_device", num_samples, seed, d_point_mask, d_sample_idx_out,
-                         sample_offsets_out, true, true);
-}
-
-int gpdb_render_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
-                      const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
-                      const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out) {
-  return render_entry(ctx, "gpdb_render_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras,
-                      depth_format, depth_out, face_out, false);
-}
-
-int gpdb_render_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
-                             const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
-                             const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
-                             int32_t *d_face_out) {
-  return render_entry(ctx, "gpdb_render_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces, n_cameras,
-                      cameras, depth_format, d_depth_out, d_face_out, true);
-}
-
-void gpdb_sensor_params_default(gpdb_sensor_params *p) {
-  if (p) memset(p, 0, sizeof(*p));
-}
-
-int gpdb_render_sensor_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
-                             const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
-                             const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out,
-                             const gpdb_sensor_params *sensor, uint64_t seed) {
-  return render_entry(ctx, "gpdb_render_sensor_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras,
-                      cameras, depth_format, depth_out, face_out, false, true, sensor, seed);
-}
-
-int gpdb_render_sensor_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
-                                    const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
-                                    const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
-                                    int32_t *d_face_out, const gpdb_sensor_params *sensor, uint64_t seed) {
-  return render_entry(ctx, "gpdb_render_sensor_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces,
-                      n_cameras, cameras, depth_format, d_depth_out, d_face_out, true, true, sensor, seed);
-}
-
-int gpdb_debug_sensor_table(double *table_out) {
-  if (!table_out) return GPDB_ERR_INVALID;
-  memcpy(table_out, sensor_table(), sizeof(double) * GPDB_SENSOR_TABLE);
-  return GPDB_SENSOR_TABLE;
-}
-
-int gpdb_sample_meshes(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *vertices,
-                       const int32_t *face_offsets, const int32_t *faces, double density, uint64_t seed,
-                       int32_t *point_offsets_out, float *xyz_out, double *normals_out, int32_t *face_out) {
-  return sample_entry(ctx, "gpdb_sample_meshes", n_meshes, vertex_offsets, vertices, face_offsets, faces, density, seed,
-                      point_offsets_out, xyz_out, normals_out, face_out, false);
-}
-
-int gpdb_sample_meshes_device(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *d_vertices,
-                              const int32_t *face_offsets, const int32_t *d_faces, double density, uint64_t seed,
-                              int32_t *point_offsets_out, float *d_xyz_out, double *d_normals_out, int32_t *d_face_out) {
-  return sample_entry(ctx, "gpdb_sample_meshes_device", n_meshes, vertex_offsets, d_vertices, face_offsets, d_faces, density,
-                      seed, point_offsets_out, d_xyz_out, d_normals_out, d_face_out, true);
-}
-
-}  // extern "C"
-
-// ---- the support plane (include/gpd_b200_plane.h) ----------------------------------------------------------------------
-
-// gpdb_segment_plane / gpdb_segment_planes[_device]: the state and argument checks, then plane_segment_batch on the
-// single cloud (single) or the batch. The host twins let the eligible bytes come back through SCR_UPLOAD.
-static int segment_entry(gpdb_ctx *ctx, const char *name, bool single, const gpdb_plane_params *pl, float *planes_out,
-                         int32_t *n_inliers_out, int32_t *n_hyp_out, uint8_t *eligible_out, bool device) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  CloudSet &s = single ? ctx->one : ctx->many;
-  int rc = single ? gpdb_check_state(ctx, true, false)
-                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
-  if (rc != GPDB_OK) return rc;
-  if (!pl || !planes_out || !n_inliers_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need params, %s and n_inliers_out", name, single ? "plane_out" : "planes_out");
-    return GPDB_ERR_INVALID;
-  }
-  const char *bad = nullptr;
-  if (!std::isfinite(pl->distance_threshold) || !(pl->distance_threshold > 0.0))
-    bad = "distance_threshold must be finite and positive";
-  else if (pl->max_iterations < 1 || pl->max_iterations > GPDB_PLANE_MAX_ITERATIONS)
-    bad = "max_iterations must lie in 1..1024";
-  else if (!(pl->probability > 0.0 && pl->probability < 1.0))
-    bad = "probability must lie in (0, 1)";
-  if (bad) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s", name, bad);
-    return GPDB_ERR_INVALID;
-  }
-  if (device && (rc = check_device_ptrs(ctx, name, {{"d_eligible_out", eligible_out}})) != GPDB_OK) return rc;
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  const int N = s.points();
-  uint8_t *d_elig = eligible_out;
-  if (!device && eligible_out) {
-    d_elig = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, (size_t)N + 16);
-    if (!d_elig) return GPDB_ERR_CUDA;
-  }
-  rc = plane_segment_batch(ctx, s, *pl, planes_out, n_inliers_out, n_hyp_out, d_elig);
-  if (rc < 0) return rc;
-  if (!device && eligible_out && N > 0) {
-    CUDA_TRY(cudaMemcpyAsync(eligible_out, d_elig, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  }
-  return rc;
-}
-
-extern "C" {
-
-void gpdb_plane_params_default(gpdb_plane_params *p) {
-  if (!p) return;
-  p->distance_threshold = 0.01;
-  p->max_iterations = 50;
-  p->probability = 0.99;
-  p->seed = 0;
-}
-
-int gpdb_segment_plane(gpdb_ctx *ctx, const gpdb_plane_params *pl, float plane_out[4], int32_t *n_inliers_out,
-                       uint8_t *eligible_out) {
-  return segment_entry(ctx, "gpdb_segment_plane", true, pl, plane_out, n_inliers_out, nullptr, eligible_out, false);
-}
-
-int gpdb_segment_planes(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
-                        int32_t *n_hypotheses_out, uint8_t *eligible_out) {
-  return segment_entry(ctx, "gpdb_segment_planes", false, pl, planes_out, n_inliers_out, n_hypotheses_out, eligible_out,
-                       false);
-}
-
-int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
-                               int32_t *n_hypotheses_out, uint8_t *d_eligible_out) {
-  return segment_entry(ctx, "gpdb_segment_planes_device", false, pl, planes_out, n_inliers_out, n_hypotheses_out,
-                       d_eligible_out, true);
-}
-
-}  // extern "C"
-
-// ---- the normal refinement (include/gpd_b200_refine.h) -----------------------------------------------------------------
-
-// gpdb_refine_normals / gpdb_refine_normals_clouds: the state and argument checks, then refine_normals_batch on the single
-// cloud (single) or the batch
-static int refine_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t k, int32_t *iterations_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  CloudSet &s = single ? ctx->one : ctx->many;
-  int rc = single ? gpdb_check_state(ctx, true, false)
-                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
-  if (rc != GPDB_OK) return rc;
-  if (k < 1 || k > GPDB_REFINE_MAX_K) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: k must lie in 1..%d (got %d)", name, GPDB_REFINE_MAX_K, (int)k);
-    return GPDB_ERR_INVALID;
-  }
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  std::vector<int> iters((size_t)s.n);
-  rc = refine_normals_batch(ctx, s, k, iters.data());
-  if (rc < 0) return rc;
-  if (iterations_out) std::copy(iters.begin(), iters.end(), iterations_out);
-  return rc;
-}
-
-extern "C" {
-
-int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
-  return refine_entry(ctx, "gpdb_refine_normals", true, k, iterations_out);
-}
-
-int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
-  return refine_entry(ctx, "gpdb_refine_normals_clouds", false, k, iterations_out);
-}
-
-}  // extern "C"
-
-// ---- the statistical outlier removal (include/gpd_b200_outliers.h) ----------------------------------------------------
-
-// gpdb_remove_outliers / gpdb_remove_outliers_clouds: the state and argument checks, then outliers_remove_batch on the
-// single cloud (single) or the batch. It reinstalls the store: the batch loses its SIS record, and any failure after the
-// checks leaves no cloud (no batch: drop_batch), as a failed install does. Returns the kept points (single) or B.
-static int outliers_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t mean_k, double stddev_mul,
-                          int32_t *offsets_out, double *stats_out, uint8_t *kept_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  CloudSet &s = single ? ctx->one : ctx->many;
-  int rc = single ? gpdb_check_state(ctx, true, false)
-                  : need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
-  if (rc != GPDB_OK) return rc;
-  if (mean_k < 1 || mean_k > GPDB_OUTLIERS_MAX_K) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mean_k must lie in 1..%d (got %d)", name, GPDB_OUTLIERS_MAX_K, (int)mean_k);
-    return GPDB_ERR_INVALID;
-  }
-  if (!std::isfinite(stddev_mul)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: stddev_mul must be finite", name);
-    return GPDB_ERR_INVALID;
-  }
-  std::vector<int> off((size_t)s.n + 1);
-  const cudaError_t e = cudaSetDevice(ctx->device);
-  if (e != cudaSuccess) {
-    gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s: cudaSetDevice -> %s", name, cudaGetErrorString(e));
-    rc = GPDB_ERR_CUDA;
-  } else {
-    rc = outliers_remove_batch(ctx, s, mean_k, stddev_mul, off.data(), stats_out, kept_out);
-  }
-  if (rc < 0) {
-    s.n = 0;
-    s.has_src = false;
-    if (!single) drop_batch(ctx);
-    return rc;
-  }
-  if (!single) gpdb_sis_forget(ctx);  // the SIS positions describe clouds that are gone
-  if (offsets_out) std::copy(off.begin(), off.end(), offsets_out);
-  if (!single) return rc;
-  if (off[1] == 0) s.n = 0;  // no point kept: no cloud, as gpdb_preprocess when its filter keeps none
-  return off[1];
-}
-
-extern "C" {
-
-int gpdb_remove_outliers(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, double stats_out[3], uint8_t *kept_out) {
-  return outliers_entry(ctx, "gpdb_remove_outliers", true, mean_k, stddev_mul, nullptr, stats_out, kept_out);
-}
-
-int gpdb_remove_outliers_clouds(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, int32_t *offsets_out,
-                                double *stats_out, uint8_t *kept_out) {
-  return outliers_entry(ctx, "gpdb_remove_outliers_clouds", false, mean_k, stddev_mul, offsets_out, stats_out, kept_out);
 }
 
 }  // extern "C"
@@ -2286,13 +1540,13 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
   int rc = gpdb_check_state(ctx, false, with_images_and_scores);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
-  if ((rc = need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
+  if ((rc = gpdb_need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
   const int B = s.n;
   if (!out || !sample_offsets || sample_offsets[0] != 0) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need out and sample_offsets[%d] starting at 0", name, B + 1);
     return GPDB_ERR_INVALID;
   }
-  if ((rc = check_offsets(ctx, name, "sample_offsets", sample_offsets, B, "cloud")) != GPDB_OK) return rc;
+  if ((rc = gpdb_check_offsets(ctx, name, "sample_offsets", sample_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int n = sample_offsets[B];
   if (n > 0 && !sample_idx) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null sample_idx", name);
@@ -2303,8 +1557,8 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
       gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, sel_name);
       return GPDB_ERR_INVALID;
     }
-    if ((rc = check_device_ptrs(ctx, name, {{"d_sample_idx", sample_idx}, {sel_name, sel_out}, {"d_flags_out", d_flags},
-                                            {"d_scores_out", d_scores}})) != GPDB_OK)
+    if ((rc = gpdb_check_device_ptrs(ctx, name, {{"d_sample_idx", sample_idx}, {sel_name, sel_out}, {"d_flags_out", d_flags},
+                                                 {"d_scores_out", d_scores}})) != GPDB_OK)
       return rc;
   } else if (n > 0) {  // host lists go through SCR_SIDX, where the pipeline reads them
     int *d_sidx = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)n);
@@ -2313,7 +1567,7 @@ int run_batch(gpdb_ctx *ctx, const int32_t *sample_offsets, const int32_t *sampl
     sample_idx = d_sidx;
   }
   CUDA_TRY(cudaMemcpyAsync(s.soff, sample_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, s.soff)) != GPDB_OK) return rc;
+  if ((rc = gpdb_check_cloud_indices(ctx, name, false, sample_offsets, sample_idx, s.soff)) != GPDB_OK) return rc;
   PipeRequest rq = {.store = &s, .sample_idx = sample_idx, .n = n, .samples_on_device = true, .per_cloud = true,
                     .classify = with_images_and_scores, .d_flags = d_flags, .d_scores = d_scores,
                     .dest = select_k < 0 ? (device ? PIPE_ALL_CALLER : PIPE_TO_HOST) : device ? PIPE_TOP_DEVICE : PIPE_TOP_HOST,
@@ -2408,15 +1662,15 @@ int gpdb_images_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, const g
   int rc = gpdb_check_state(ctx, false, false);
   if (rc != GPDB_OK) return rc;
   CloudSet &s = ctx->many;
-  if ((rc = need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
+  if ((rc = gpdb_need_batch(ctx, name, "gpdb_set_clouds")) != GPDB_OK) return rc;
   const int B = s.n;
-  if ((rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, B, "cloud")) != GPDB_OK) return rc;
+  if ((rc = gpdb_check_offsets(ctx, name, "hand_offsets", hand_offsets, B, "cloud")) != GPDB_OK) return rc;
   const int n = hand_offsets[B];
   if (n > 0 && (!d_hands || !d_images_out)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands or d_images_out", name);
     return GPDB_ERR_INVALID;
   }
-  if ((rc = check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_images_out", d_images_out}})) != GPDB_OK) return rc;
+  if ((rc = gpdb_check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_images_out", d_images_out}})) != GPDB_OK) return rc;
   if (n == 0) return 0;
   CUDA_TRY(cudaMemcpyAsync(s.soff, hand_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
   const size_t isz = (size_t)ctx->hp.S * ctx->hp.S * ctx->hp.C, psz = (size_t)ctx->hp.S * ctx->hp.S * 16;
@@ -2578,8 +1832,8 @@ int gpdb_classify_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, int32_t n, 
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: bad arguments", name);
     return GPDB_ERR_INVALID;
   }
-  rc = check_device_ptrs(ctx, name, {{"d_images_hwc", d_images_hwc}, {"d_scores_out", d_scores_out},
-                                     {"d_logits_out", d_logits_out}});
+  rc = gpdb_check_device_ptrs(ctx, name, {{"d_images_hwc", d_images_hwc}, {"d_scores_out", d_scores_out},
+                                          {"d_logits_out", d_logits_out}});
   if (rc != GPDB_OK) return rc;
   return classify_batches(ctx, d_images_hwc, n, d_scores_out, d_logits_out, nullptr, true);
 }
@@ -2594,109 +1848,6 @@ int gpdb_debug_lenet_layers(gpdb_ctx *ctx, const uint8_t *images_hwc, int32_t n,
   }
   const LenetLayers layers = {pool1_out, pool2_out, ip1_out};
   return classify_batches(ctx, images_hwc, n, nullptr, logits_out, &layers);
-}
-
-// ---- training (train.cu, include/gpd_b200_train.h) ------------------------------------------------------------------------
-
-int gpdb_train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]) {
-  int rc = gpdb_check_state(ctx, false, false);
-  if (rc != GPDB_OK) return rc;
-  return train_begin(ctx, p, init);
-}
-
-namespace {
-
-// the checks of a training step before any device work: begun, a 60 x 60 network, n >= 1, the arrays given
-int train_step_args(gpdb_ctx *ctx, const char *name, const void *images, const void *labels, int32_t n) {
-  int rc = gpdb_check_state(ctx, false, false);
-  if (rc != GPDB_OK) return rc;
-  if (!train_started(ctx)) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: call gpdb_train_begin first", name);
-    return GPDB_ERR_STATE;
-  }
-  if (ctx->prm.image_size != 60) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: LeNet expects image_size 60, got %d", name, ctx->prm.image_size);
-    return GPDB_ERR_INVALID;
-  }
-  if (n <= 0 || !images || !labels) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: bad arguments (n = %d)", name, n);
-    return GPDB_ERR_INVALID;
-  }
-  return GPDB_OK;
-}
-
-// the device check of the labels, then the step: a label outside {0, 1} fails the step before anything changes
-int train_step_checked(gpdb_ctx *ctx, const char *name, const uint8_t *d_images, const int32_t *d_labels, int32_t n,
-                       float *d_loss_out, float *h_loss_out, const gpdb_train_debug *dbg) {
-  unsigned long long bad;
-  int rc = first_bad(ctx, 0, &bad, [&](unsigned long long *d_bad, void *) {
-    return train_check_labels(ctx, d_labels, n, d_bad);
-  });
-  if (rc != GPDB_OK) return rc;
-  if (bad != NO_BAD) {
-    int32_t v = 0;
-    CUDA_TRY(cudaMemcpy(&v, d_labels + bad, sizeof(v), cudaMemcpyDeviceToHost));
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: labels[%llu] = %d is not 0 or 1", name, bad, v);
-    return GPDB_ERR_INVALID;
-  }
-  return train_step(ctx, d_images, d_labels, n, d_loss_out, h_loss_out, dbg);
-}
-
-// host twins: upload images and labels (SCR_HWC / SCR_LABELS), then the device path
-int train_step_host(gpdb_ctx *ctx, const char *name, const uint8_t *images_hwc, const int32_t *labels, int32_t n,
-                    float *loss_out, const gpdb_train_debug *dbg) {
-  const size_t isz = (size_t)60 * 60 * ctx->prm.image_num_channels * n;
-  uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz);
-  int32_t *d_lab = (int32_t *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int32_t) * (size_t)n);
-  if (!d_img || !d_lab) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemcpyAsync(d_img, images_hwc, isz, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(d_lab, labels, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  return train_step_checked(ctx, name, d_img, d_lab, n, nullptr, loss_out, dbg);
-}
-
-}  // namespace
-
-int gpdb_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n, float *loss_out) {
-  const char *name = "gpdb_train_step";
-  int rc = train_step_args(ctx, name, images_hwc, labels, n);
-  if (rc != GPDB_OK) return rc;
-  return train_step_host(ctx, name, images_hwc, labels, n, loss_out, nullptr);
-}
-
-int gpdb_train_step_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, const int32_t *d_labels, int32_t n,
-                           float *d_loss_out) {
-  const char *name = "gpdb_train_step_device";
-  int rc = train_step_args(ctx, name, d_images_hwc, d_labels, n);
-  if (rc != GPDB_OK) return rc;
-  rc = check_device_ptrs(ctx, name, {{"d_images_hwc", d_images_hwc}, {"d_labels", d_labels}, {"d_loss_out", d_loss_out}});
-  if (rc != GPDB_OK) return rc;
-  return train_step_checked(ctx, name, d_images_hwc, d_labels, n, d_loss_out, nullptr, nullptr);
-}
-
-int gpdb_debug_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n,
-                          gpdb_train_debug *out) {
-  const char *name = "gpdb_debug_train_step";
-  int rc = train_step_args(ctx, name, images_hwc, labels, n);
-  if (rc != GPDB_OK) return rc;
-  if (!out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need an output struct", name);
-    return GPDB_ERR_INVALID;
-  }
-  return train_step_host(ctx, name, images_hwc, labels, n, nullptr, out);
-}
-
-int gpdb_train_weights(gpdb_ctx *ctx, float *const out[8]) {
-  int rc = gpdb_check_state(ctx, false, false);
-  if (rc != GPDB_OK) return rc;
-  if (!train_started(ctx)) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_train_weights: call gpdb_train_begin first");
-    return GPDB_ERR_STATE;
-  }
-  if (!out || !out[0] || !out[1] || !out[2] || !out[3] || !out[4] || !out[5] || !out[6] || !out[7]) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_train_weights: null output array");
-    return GPDB_ERR_INVALID;
-  }
-  return train_weights(ctx, out);
 }
 
 namespace {
@@ -2733,14 +1884,15 @@ int reevaluate_batch(gpdb_ctx *ctx, const char *name, const int32_t *hand_offset
                      bool device) {
   int rc = gpdb_check_state(ctx, false, false);
   if (rc != GPDB_OK) return rc;
-  if ((rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth")) != GPDB_OK) return rc;
-  if ((rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, ctx->many.n, "cloud")) != GPDB_OK) return rc;
+  if ((rc = gpdb_need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth")) != GPDB_OK)
+    return rc;
+  if ((rc = gpdb_check_offsets(ctx, name, "hand_offsets", hand_offsets, ctx->many.n, "cloud")) != GPDB_OK) return rc;
   if (hand_offsets[ctx->many.n] > 0 && (!hands || !labels_out)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s or %s", name, device ? "d_hands" : "hands",
                    device ? "d_labels_out" : "labels_out");
     return GPDB_ERR_INVALID;
   }
-  if (device && (rc = check_device_ptrs(ctx, name, {{"d_hands", hands}, {"d_labels_out", labels_out}})) != GPDB_OK)
+  if (device && (rc = gpdb_check_device_ptrs(ctx, name, {{"d_hands", hands}, {"d_labels_out", labels_out}})) != GPDB_OK)
     return rc;
   return label_hands(ctx, ctx->many, hand_offsets, hands, labels_out, device);
 }
@@ -2768,12 +1920,8 @@ int gpdb_reevaluate_batch_device(gpdb_ctx *ctx, const int32_t *hand_offsets, gpd
 
 }  // extern "C"
 
-// gpdb_find_clusters_batch after the argument checks (gpdb_find_clusters: one group): the clusters of all G groups in one
-// k_clusters launch, compacted in hand order, so group g's are clusters_out[cluster_offsets_out[g] ..
-// cluster_offsets_out[g+1]); returns their total. device: hands are device arrays (no copy of the hands); clusters_out
-// may be host or device memory
-static int find_clusters(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
-                         gpdb_pose *clusters_out, int32_t *cluster_offsets_out, bool device = false) {
+int gpdb_cluster_groups(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
+                        gpdb_pose *clusters_out, int32_t *cluster_offsets_out, bool device) {
   const int n = hand_offsets[G];
   for (int g = 0; g <= G; g++) cluster_offsets_out[g] = 0;
   if (n == 0) return 0;
@@ -2821,7 +1969,7 @@ int gpdb_find_clusters(gpdb_ctx *ctx, const gpdb_pose *hands, int32_t n, int32_t
   }
   const int32_t hand_offsets[2] = {0, n};
   int32_t cluster_offsets[2];
-  return find_clusters(ctx, 1, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets);
+  return gpdb_cluster_groups(ctx, 1, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets);
 }
 
 }  // extern "C"
@@ -2834,7 +1982,7 @@ static int check_groups_args(gpdb_ctx *ctx, const char *name, int32_t n_groups, 
                    "cluster_offsets_out", name);
     return GPDB_ERR_INVALID;
   }
-  const int rc = check_offsets(ctx, name, "hand_offsets", hand_offsets, n_groups, "group");
+  const int rc = gpdb_check_offsets(ctx, name, "hand_offsets", hand_offsets, n_groups, "group");
   if (rc != GPDB_OK) return rc;
   if (hand_offsets[n_groups] > 0 && (!hands || !clusters_out)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null hands or clusters_out", name);
@@ -2851,7 +1999,7 @@ int gpdb_find_clusters_batch(gpdb_ctx *ctx, int32_t n_groups, const int32_t *han
   const int rc = check_groups_args(ctx, "gpdb_find_clusters_batch", n_groups, hand_offsets, hands, clusters_out,
                                    cluster_offsets_out);
   if (rc != GPDB_OK) return rc;
-  return find_clusters(ctx, n_groups, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets_out);
+  return gpdb_cluster_groups(ctx, n_groups, hand_offsets, hands, min_inliers, clusters_out, cluster_offsets_out);
 }
 
 int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32_t *hand_offsets, const gpdb_pose *d_hands,
@@ -2859,297 +2007,9 @@ int gpdb_find_clusters_batch_device(gpdb_ctx *ctx, int32_t n_groups, const int32
   if (!ctx) return GPDB_ERR_INVALID;
   const char *name = "gpdb_find_clusters_batch_device";
   int rc = check_groups_args(ctx, name, n_groups, hand_offsets, d_hands, d_clusters_out, cluster_offsets_out);
-  if (rc == GPDB_OK) rc = check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_clusters_out", d_clusters_out}});
+  if (rc == GPDB_OK) rc = gpdb_check_device_ptrs(ctx, name, {{"d_hands", d_hands}, {"d_clusters_out", d_clusters_out}});
   if (rc != GPDB_OK) return rc;
-  return find_clusters(ctx, n_groups, hand_offsets, d_hands, min_inliers, d_clusters_out, cluster_offsets_out, true);
-}
-
-}  // extern "C"
-
-// ---- sequential importance sampling (gpdb_sis_batch) ----------------------------------------------------------------
-
-// The arrays of SCR_SIS for B clouds, R rounds of S positions and n_init initial samples: kept positions (KC = n_init +
-// B*R*S of them) and evaluated positions, the initial offsets and indices, the kept counts [B] followed by the round
-// counts [R*B] (ecount, zeroed with them), the hand counts and the installed sample list
-struct SisArena {
-  double *kept, *eval;
-  int *init_off, *init_idx, *kcount, *ecount, *hcount, *sidx;
-};
-static void sis_layout(Carve &c, int B, int R, int S, int n_init, SisArena &a) {
-  const size_t RS = (size_t)R * S, KC = (size_t)n_init + (size_t)B * RS;
-  a.kept = c.take<double>(3 * KC);
-  a.eval = c.take<double>(3 * (size_t)B * RS);
-  a.init_off = c.take<int>((size_t)B + 1);
-  a.init_idx = c.take<int>(n_init);
-  a.kcount = c.take<int>((size_t)B * (R + 1));
-  a.ecount = c.base ? a.kcount + B : nullptr;
-  a.hcount = c.take<int>(B);
-  a.sidx = c.take<int>(KC);
-}
-
-// The argument checks of gpdb_sis_batch[_device] after the state checks: parameters and offsets
-static int check_sis_args(gpdb_ctx *ctx, const char *name, int B, const gpdb_sis_params *sp, const int32_t *init_offsets,
-                          const void *init_idx, const void *out, const int32_t *hand_offsets_out) {
-  if (!sp || !init_offsets || init_offsets[0] != 0 || !out || !hand_offsets_out) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need params, init_offsets[%d] starting at 0, a result and hand_offsets_out",
-                   name, B + 1);
-    return GPDB_ERR_INVALID;
-  }
-  if (sp->num_iterations < 0 || sp->num_samples_per_iteration < 0 || sp->min_inliers < 0) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: num_iterations, num_samples_per_iteration and min_inliers must not be negative",
-                   name);
-    return GPDB_ERR_INVALID;
-  }
-  if (!(sp->prob_rand_samples >= 0.0 && sp->prob_rand_samples <= 1.0)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: prob_rand_samples = %g outside [0, 1]", name, sp->prob_rand_samples);
-    return GPDB_ERR_INVALID;
-  }
-  if (!(std::isfinite(sp->standard_deviation) && sp->standard_deviation > 0.0)) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: standard_deviation = %g must be finite and positive", name,
-                   sp->standard_deviation);
-    return GPDB_ERR_INVALID;
-  }
-  if (sp->sampling_method != 0 && sp->sampling_method != 1) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sampling_method = %d (0 sum of Gaussians, 1 max of Gaussians)", name,
-                   sp->sampling_method);
-    return GPDB_ERR_INVALID;
-  }
-  const int rc = check_offsets(ctx, name, "init_offsets", init_offsets, B, "cloud");
-  if (rc != GPDB_OK) return rc;
-  if (init_offsets[B] > 0 && !init_idx) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null init_idx", name);
-    return GPDB_ERR_INVALID;
-  }
-  const long long kc = (long long)init_offsets[B] + (long long)B * sp->num_iterations * sp->num_samples_per_iteration;
-  if (kc * ctx->hp.P > INT32_MAX) {
-    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %lld positions of %d poses exceed the 2^31 records of one call", name, kc,
-                   ctx->hp.P);
-    return GPDB_ERR_INVALID;
-  }
-  return GPDB_OK;
-}
-
-// The hand search of the CSR list d_sidx (offsets in s.soff, n samples) and the kept-set update it implies
-static int sis_search(gpdb_ctx *ctx, CloudSet &s, const int *d_sidx, int n, const SisArena &a, int RS) {
-  gpdb_result r;
-  PipeRequest rq = {.store = &s, .sample_idx = d_sidx, .n = n, .samples_on_device = true, .per_cloud = true,
-                    .classify = false, .dest = PIPE_STAY};
-  const int rc = gpdb_run_pipeline(ctx, rq, &r);
-  if (rc < 0) return rc;
-  return sis_keep(ctx, s, rq.d_flags, d_sidx, a.init_off, RS, a.kept, a.kcount);
-}
-
-// Installs, as gpdb_set_clouds_samples would, cloud b's cnt[b] positions of src (see sis_install) straight into the
-// store's sample arena, with the sample list N_b + j; h_cnt (host) gives the offsets. Returns the number of positions.
-static int sis_install_positions(gpdb_ctx *ctx, CloudSet &s, const SisArena &a, const int *h_cnt, const double *src,
-                                 int stride, int add, const int *init_off, const int *d_cnt) {
-  const int B = s.n;
-  s.pos[0] = 0;
-  for (int b = 0; b < B; b++) s.pos[b + 1] = s.pos[b] + h_cnt[b];
-  int rc = reserve_samples(ctx, s, s.pos[B]);
-  if (rc != GPDB_OK) return rc;
-  CUDA_TRY(cudaMemcpyAsync(s.soff, s.pos, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = sis_install(ctx, s, src, stride, add, init_off, d_cnt, s.soff, s.samples, a.sidx)) != GPDB_OK) return rc;
-  s.n_samples = s.pos[B];
-  return s.n_samples;
-}
-
-// gpdb_sis_batch[_device] after the checks: d_init_idx already in the arena. dest (host or device) receives the records,
-// out the counts and timings.
-static int sis_run(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const SisArena &a, gpdb_pose *dest,
-                   bool dest_on_host, int32_t *hand_offsets_out, gpdb_result *out) {
-  CloudSet &s = ctx->many;
-  SisState &st = *ctx->sis;
-  const int B = s.n, R = sp->num_iterations, S = sp->num_samples_per_iteration, RS = R * S, P = ctx->hp.P;
-  const int64_t launches0 = ctx->launches;
-  // 1. the initial hand sets (:68-79)
-  CUDA_TRY(cudaMemcpyAsync(s.soff, init_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  int rc = sis_search(ctx, s, a.init_idx, init_offsets[B], a, RS);
-  if (rc != GPDB_OK) return rc;
-  std::vector<int> h_cnt((size_t)B);
-  CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.kcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  bool any_active = false;
-  for (int c : h_cnt) any_active |= c > 0;
-  // 2. the rounds (:109-160): draws, then the hand search at the drawn positions
-  SisDraw q = {R, S, 0, 0, sp->sampling_method, 0, sp->standard_deviation, {}, sp->seed};
-  q.n_rand = (int)(sp->prob_rand_samples * S);
-  q.n_gauss = S - q.n_rand;
-  for (int k = 0; k < 6; k++) q.ws[k] = sp->workspace[k];
-  int max_init = 0;
-  for (int b = 0; b < B; b++) max_init = std::max(max_init, init_offsets[b + 1] - init_offsets[b]);
-  for (int r = 0; r < R && any_active; r++) {
-    q.round = r;
-    const int stage_cap = std::min(max_init + r * S, 1920);  // 45 KB: with the scan storage inside the 48 KB default
-    if ((rc = sis_draw(ctx, q, B, s, a.init_off, a.init_idx, a.kept, a.kcount, stage_cap, a.eval, a.ecount)) != GPDB_OK)
-      return rc;
-    CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.ecount + (size_t)r * B, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost,
-                             ctx->stream));
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    const int n = sis_install_positions(ctx, s, a, h_cnt.data(), a.eval, RS, r * S, nullptr, a.ecount + (size_t)r * B);
-    if (n < 0) return n;
-    if (n > 0 && (rc = sis_search(ctx, s, a.sidx, n, a, RS)) != GPDB_OK) return rc;
-  }
-  // 3. classify at every kept position (:168-170), keep score > min_score
-  st.ecount.resize((size_t)R * B);
-  CUDA_TRY(cudaMemcpyAsync(h_cnt.data(), a.kcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaMemcpyAsync(st.ecount.data(), a.ecount, sizeof(int) * st.ecount.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  const int M = sis_install_positions(ctx, s, a, h_cnt.data(), a.kept, RS, 0, a.init_off, a.kcount);
-  if (M < 0) return M;
-  st.koff.assign(s.pos, s.pos + B + 1);
-  PipeRequest rq = {.store = &s, .sample_idx = a.sidx, .n = M, .samples_on_device = true, .per_cloud = true, .classify = true,
-                    .dest = PIPE_ALL_DEVICE};
-  if ((rc = gpdb_run_pipeline(ctx, rq, out)) < 0) return rc;
-  const int total = out->n_total_candidates;
-  uint8_t *d_keep = (uint8_t *)gpdb_scratch(ctx, SCR_FLAGS, (size_t)total);
-  gpdb_pose *d_filt = (gpdb_pose *)gpdb_scratch(ctx, SCR_POSES, sizeof(gpdb_pose) * (size_t)total);
-  int *d_count = (int *)gpdb_scratch(ctx, SCR_COUNT, 64);
-  if (!d_keep || !d_filt || !d_count) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemsetAsync(a.hcount, 0, sizeof(int) * (size_t)B, ctx->stream));
-  if ((rc = sis_filter(ctx, ctx->d_sel, total, s.soff, B, sp->min_score, d_keep, a.hcount)) != GPDB_OK) return rc;
-  if ((rc = geo_compact(ctx, ctx->d_sel, d_keep, total, d_filt, d_count)) != GPDB_OK) return rc;
-  std::vector<int32_t> hoff((size_t)B + 1, 0);
-  CUDA_TRY(cudaMemcpyAsync(hoff.data() + 1, a.hcount, sizeof(int) * (size_t)B, cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  for (int b = 0; b < B; b++) hoff[b + 1] += hoff[b];
-  int n_out = hoff[B];
-  if (dest_on_host) dest = n_out ? (gpdb_pose *)malloc(sizeof(gpdb_pose) * (size_t)n_out) : nullptr;
-  if (n_out && !dest) {
-    gpdb_set_error(ctx, GPDB_ERR_CUDA, "out of host memory for %d records", n_out);
-    return GPDB_ERR_CUDA;
-  }
-  // 4. cluster (:177-179)
-  if (sp->min_inliers > 0) {
-    n_out = find_clusters(ctx, B, hoff.data(), d_filt, sp->min_inliers, dest, hand_offsets_out, true);
-  } else {
-    memcpy(hand_offsets_out, hoff.data(), sizeof(int32_t) * ((size_t)B + 1));
-    if (n_out) {
-      cudaError_t e = cudaMemcpyAsync(dest, d_filt, sizeof(gpdb_pose) * (size_t)n_out, cudaMemcpyDefault, ctx->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-      if (e != cudaSuccess) {
-        gpdb_set_error(ctx, GPDB_ERR_CUDA, "copy of the %d records: %s", n_out, cudaGetErrorString(e));
-        n_out = GPDB_ERR_CUDA;
-      }
-    }
-  }
-  if (n_out < 0) {
-    if (dest_on_host) free(dest);
-    return n_out;
-  }
-  st.valid = true;
-  out->n_samples = M;
-  out->poses_per_sample = P;
-  out->n_candidates = n_out;
-  out->candidates = dest_on_host ? dest : nullptr;
-  out->kernel_launches = ctx->launches - launches0;
-  return n_out;
-}
-
-// gpdb_sis_batch[_device]: checks, the initial indices into the arena (checked there, on the device), sis_run
-static int sis_batch(gpdb_ctx *ctx, const char *name, const gpdb_sis_params *sp, const int32_t *init_offsets,
-                     const int32_t *init_idx, bool device, gpdb_pose *d_hands_out, int32_t *hand_offsets_out,
-                     gpdb_result *out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  CloudSet &s = ctx->many;
-  s.n_samples = 0;  // a failed call leaves no positions behind, and no SIS positions to read back
-  gpdb_sis_forget(ctx);
-  int rc = gpdb_check_state(ctx, false, true);
-  if (rc != GPDB_OK) return rc;
-  if (!ctx->sis) ctx->sis = new SisState();
-  if ((rc = need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds")) != GPDB_OK) return rc;
-  const int B = s.n;
-  if ((rc = check_sis_args(ctx, name, B, sp, init_offsets, init_idx, out, hand_offsets_out)) != GPDB_OK) return rc;
-  const int n0 = init_offsets[B];
-  if (device) {
-    if ((rc = check_device_ptrs(ctx, name, {{"d_init_idx", init_idx}, {"d_hands_out", d_hands_out}})) != GPDB_OK) return rc;
-    const long long kc = (long long)n0 + (long long)B * sp->num_iterations * sp->num_samples_per_iteration;
-    if (kc > 0 && !d_hands_out) {
-      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null d_hands_out", name);
-      return GPDB_ERR_INVALID;
-    }
-  }
-  SisState &st = *ctx->sis;
-  const int R = sp->num_iterations, S = sp->num_samples_per_iteration;
-  SisArena a;
-  if (!gpdb_carve(ctx, SCR_SIS, [&](Carve &c) { sis_layout(c, B, R, S, n0, a); })) return GPDB_ERR_CUDA;
-  CUDA_TRY(cudaMemcpyAsync(a.init_off, init_offsets, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
-  if (n0 > 0)
-    CUDA_TRY(cudaMemcpyAsync(a.init_idx, init_idx, sizeof(int) * (size_t)n0,
-                             device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_TRY(cudaMemsetAsync(a.kcount, 0, sizeof(int) * (size_t)B * (R + 1), ctx->stream));  // kept and round counts
-  if ((rc = check_cloud_indices(ctx, name, true, init_offsets, a.init_idx, a.init_off)) != GPDB_OK) return rc;
-  st.B = B;
-  st.R = R;
-  st.S = S;
-  st.init_off.assign(init_offsets, init_offsets + B + 1);
-  rc = sis_run(ctx, sp, init_offsets, a, d_hands_out, !device, hand_offsets_out, out);
-  if (rc < 0) {
-    s.n_samples = 0;
-    st.valid = false;
-  }
-  return rc;
-}
-
-extern "C" {
-
-void gpdb_sis_params_default(gpdb_sis_params *p) {
-  memset(p, 0, sizeof(*p));
-  p->num_iterations = 5;
-  p->num_samples_per_iteration = 50;
-  p->prob_rand_samples = 0.3;
-  p->standard_deviation = 0.02;
-  const double ws[6] = {-1, 1, -1, 1, -1, 1};
-  for (int i = 0; i < 6; i++) p->workspace[i] = ws[i];
-  p->min_inliers = 1;
-}
-
-int gpdb_sis_batch(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *init_idx,
-                   gpdb_result *out, int32_t *hand_offsets_out) {
-  return sis_batch(ctx, "gpdb_sis_batch", sp, init_offsets, init_idx, false, nullptr, hand_offsets_out, out);
-}
-
-int gpdb_sis_batch_device(gpdb_ctx *ctx, const gpdb_sis_params *sp, const int32_t *init_offsets, const int32_t *d_init_idx,
-                          gpdb_pose *d_hands_out, int32_t *hand_offsets_out, gpdb_result *stats) {
-  return sis_batch(ctx, "gpdb_sis_batch_device", sp, init_offsets, d_init_idx, true, d_hands_out, hand_offsets_out, stats);
-}
-
-int gpdb_sis_positions(gpdb_ctx *ctx, int32_t *eval_offsets_out, int32_t *eval_round_counts_out, double *eval_xyz_out,
-                       int32_t *kept_offsets_out, double *kept_xyz_out) {
-  if (!ctx) return GPDB_ERR_INVALID;
-  if (!ctx->sis || !ctx->sis->valid) {
-    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_sis_positions: no successful gpdb_sis_batch call on this context");
-    return GPDB_ERR_STATE;
-  }
-  const SisState &st = *ctx->sis;
-  const int B = st.B, R = st.R, S = st.S, RS = R * S;
-  SisArena a;
-  carve_at(ctx->scratch[SCR_SIS], [&](Carve &c) { sis_layout(c, B, R, S, st.init_off[B], a); });
-  CUDA_TRY(cudaSetDevice(ctx->device));
-  // the evaluated and kept arenas, read once on the context's stream and unpacked on the host
-  std::vector<double> ev(eval_xyz_out ? 3 * (size_t)B * RS : 0), kp(kept_xyz_out ? 3 * ((size_t)st.init_off[B] + (size_t)B * RS) : 0);
-  if (!ev.empty()) CUDA_TRY(cudaMemcpyAsync(ev.data(), a.eval, sizeof(double) * ev.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  if (!kp.empty()) CUDA_TRY(cudaMemcpyAsync(kp.data(), a.kept, sizeof(double) * kp.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  if (eval_offsets_out || eval_round_counts_out || eval_xyz_out) {
-    size_t o = 0;
-    if (eval_offsets_out) eval_offsets_out[0] = 0;
-    for (int b = 0; b < B; b++) {
-      for (int r = 0; r < R; r++) {
-        const int c = st.ecount[(size_t)r * B + b];
-        if (eval_round_counts_out) eval_round_counts_out[(size_t)b * R + r] = c;
-        if (eval_xyz_out) memcpy(eval_xyz_out + 3 * o, ev.data() + 3 * ((size_t)b * R + r) * S, sizeof(double) * 3 * c);
-        o += c;
-      }
-      if (eval_offsets_out) eval_offsets_out[b + 1] = (int32_t)o;
-    }
-  }
-  if (kept_offsets_out) memcpy(kept_offsets_out, st.koff.data(), sizeof(int32_t) * ((size_t)B + 1));
-  if (kept_xyz_out)  // cloud b's kept positions start at position init_off[b] + b*R*S of the arena
-    for (int b = 0; b < B; b++)
-      memcpy(kept_xyz_out + 3 * (size_t)st.koff[b], kp.data() + 3 * ((size_t)st.init_off[b] + (size_t)b * RS),
-             sizeof(double) * 3 * (size_t)(st.koff[b + 1] - st.koff[b]));
-  return B;
+  return gpdb_cluster_groups(ctx, n_groups, hand_offsets, d_hands, min_inliers, d_clusters_out, cluster_offsets_out, true);
 }
 
 void gpdb_free_result(gpdb_result *r) {

@@ -16,6 +16,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
+#include <initializer_list>
+#include <utility>
+#include <vector>
+
 #include "../../include/gpd_b200.h"
 #include "../../include/gpd_b200_shadow.h"
 
@@ -188,7 +193,7 @@ struct LenetTc {  // tensor-core (wgmma) weight blobs, lenet_tc.cu
 struct StageTimes;  // api.cu
 struct PipeState;   // api.cu: copy stream, events and the pinned result arenas of the chunk pipeline
 struct CommState;   // comm.cu: NCCL communicator (multi-GPU sharding)
-struct SisState;    // api.cu: host-side record of the last gpdb_sis_batch call (gpdb_sis_positions)
+struct SisState;    // sis.cu: host-side record of the last gpdb_sis_batch call (gpdb_sis_positions)
 struct TrainState;  // train.cu: the trained weights, the optimiser state and the step count (gpdb_train_begin)
 
 // The scratch buffers of a context (gpdb_scratch), each grown on demand and never shrunk. This enum is the whole slot
@@ -241,7 +246,7 @@ enum ScratchSlot {
   SCR_IMG_OVF,
   // k_frames last tier: the staged neighbourhood keys
   SCR_FRAMES_GL,
-  // the device-side input checks of api.cu: the check word, then the per-cloud arrays of the check
+  // the device-side input checks (first_bad): the check word, then the per-cloud arrays of the check
   SCR_CHECK,
   // gpdb_sis_batch: kept / evaluated positions, the round's sample lists and counts (main stream, between pipeline calls;
   // read again by gpdb_sis_positions)
@@ -395,6 +400,55 @@ int gpdb_install_clouds(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, const int *
 int gpdb_stage_clouds(gpdb_ctx *ctx, CloudSet &s, const char *name, int B, const int32_t *off, const float *xyz,
                       const double *normals, const int32_t *cam_source, const int32_t *n_cameras,
                       const double *view_points, bool device, CloudDesc *desc);
+// every non-null pointer must be device (or managed) memory of the context's device; runs before any device work
+int gpdb_check_device_ptrs(gpdb_ctx *ctx, const char *name,
+                           std::initializer_list<std::pair<const char *, const void *>> ptrs);
+static const unsigned long long NO_BAD = ~0ull;  // the check word when no position offends
+// The check-word protocol of the device-side checks. The word, at the head of SCR_CHECK, is set to all ones;
+// enqueue(d_bad, d_extra) queues the kernel that lowers it to the first offending position, with `extra` bytes behind the
+// word for the check's own arrays; *bad receives the word (NO_BAD: nothing offends) once the stream has drained.
+template <class Enqueue>
+static int first_bad(gpdb_ctx *ctx, size_t extra, unsigned long long *bad, Enqueue enqueue) {
+  unsigned long long *d_bad = (unsigned long long *)gpdb_scratch(ctx, SCR_CHECK, sizeof(*d_bad) + extra);
+  if (!d_bad) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemsetAsync(d_bad, 0xFF, sizeof(*d_bad), ctx->stream));
+  const int rc = enqueue(d_bad, d_bad + 1);
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaMemcpyAsync(bad, d_bad, sizeof(*bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  return GPDB_OK;
+}
+// what every call that installs a batch does first: a failed call leaves no batch, no sample positions and no SIS record
+// behind (the SIS positions describe clouds that are gone); the single cloud is never touched
+void gpdb_drop_batch(gpdb_ctx *ctx);
+// GPDB_ERR_STATE unless a batch is installed; hint names the calls that install one
+int gpdb_need_batch(gpdb_ctx *ctx, const char *name, const char *hint);
+// CSR offsets off[B+1] (the array `label`) from the host: they start at 0 and never decrease; entry b belongs to the b-th
+// `unit` (cloud or group). A call whose start message lists other arguments too checks the start itself first.
+int gpdb_check_offsets(gpdb_ctx *ctx, const char *name, const char *label, const int32_t *off, int B, const char *unit);
+// The cloud-local indices d_idx[off[b] .. off[b+1]) of cloud b of the installed batch must lie in [0, N_b + M_b), M_b
+// its sample positions. The list d_idx and its offsets d_off are in device memory, off is the host copy of d_off;
+// batch_check_samples finds the first offending position, which the message names. init: the initial indices of
+// gpdb_sis_batch, which has dropped the positions (M_b = 0) and names the indices so.
+int gpdb_check_cloud_indices(gpdb_ctx *ctx, const char *name, bool init, const int32_t *off, const int32_t *d_idx,
+                             const int *d_off);
+// the preprocessing parameters, against the caller's normals (null: none)
+int gpdb_check_preprocess_params(gpdb_ctx *ctx, const char *name, const gpdb_preprocess_params *pp, const double *normals);
+// The steps of a preprocessing call after the filter and voxelisation (store s holds the processed points, poff[B+1] their
+// offsets, desc[B] the camera fields): install with one grid per cloud, normals, nonunit flags, stage timings, and the
+// raw offsets roff[B+1] the source indices refer to. after_normals (may be empty) runs between the normal estimation and
+// the nonunit flags, inside the normals' stage timing. A failure leaves no cloud in s.
+int gpdb_preprocess_install(gpdb_ctx *ctx, CloudSet &s, CloudDesc *desc, int B, const int32_t *roff,
+                            const gpdb_preprocess_params *pp, int32_t *poff,
+                            const std::function<int()> &after_normals = nullptr);
+// drops the sample positions of store s and makes its arena hold n positions (grown, never shrunk)
+int gpdb_reserve_samples(gpdb_ctx *ctx, CloudSet &s, int n);
+// gpdb_find_clusters_batch after the argument checks (gpdb_find_clusters: one group): the clusters of all G groups in one
+// k_clusters launch, compacted in hand order, so group g's are clusters_out[cluster_offsets_out[g] ..
+// cluster_offsets_out[g+1]); returns their total. device: hands are device arrays (no copy of the hands); clusters_out
+// may be host or device memory
+int gpdb_cluster_groups(gpdb_ctx *ctx, int G, const int32_t *hand_offsets, const gpdb_pose *hands, int min_inliers,
+                        gpdb_pose *clusters_out, int32_t *cluster_offsets_out, bool device = false);
 
 // largest b in [0, n) with a[b] <= x, for a non-decreasing a with a[0] <= x: the cloud that owns position x of a CSR array
 __device__ __forceinline__ int csr_owner(const int *a, int n, long long x) {
@@ -457,32 +511,10 @@ int batch_local_slots(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, const int *d_
 // the store's soff (gpdb_images_batch_device)
 int batch_image_hands(gpdb_ctx *ctx, const gpdb_pose *d_in, int n, int base, gpdb_pose *d_out);
 
-// sis.cu (gpdb_sis_batch, include/gpd_b200_sis.h). Per cloud b of a batch with R rounds of S positions and initial
-// offsets init_off[B+1] (device), the kept arena holds room for init_off[b+1] - init_off[b] + R*S positions from position
-// init_off[b] + b*R*S, the evaluated arena S positions per (cloud, round) from (b*R + r)*S; kcount[b] counts the kept
-// positions, ecount[r*B + b] the positions of round r.
-struct SisDraw {
-  int R, S, n_gauss, n_rand, method, round;
-  double sigma, ws[6];
-  unsigned long long seed;
-};
-// the draws of round q.round for every cloud with a kept position (one CTA per cloud); stage_cap: kept positions a CTA may
-// stage in shared memory
-int sis_draw(gpdb_ctx *ctx, const SisDraw &q, int B, const CloudSet &s, const int *d_init_off, const int *d_init_idx,
-             const double *d_kept, const int *d_kcount, int stage_cap, double *d_eval, int *d_ecount);
-// appends, per cloud and in sample order, the position of every sample of the CSR list d_sidx (offsets s.soff) with a
-// VALID|FILTERED pose in the dense flags [n * P] to the cloud's kept positions
-int sis_keep(gpdb_ctx *ctx, const CloudSet &s, const uint8_t *d_flags, const int *d_sidx, const int *d_init_off, int RS,
-             double *d_kept, int *d_kcount);
-// the positions to install, as gpdb_set_clouds_samples would lay them out: cloud b's d_cnt[b] positions from position
-// b*stride + add (+ d_init_off[b] when given) of d_src go to d_dst (the store's sample arena) at d_soff[b],
-// d_sidx[d_soff[b] + j] = N_b + j, and the descriptors' first position becomes d_soff[b]
-int sis_install(gpdb_ctx *ctx, CloudSet &s, const double *d_src, int stride, int add, const int *d_init_off,
-                const int *d_cnt, const int *d_soff, double *d_dst, int *d_sidx);
-// the final score filter over n records of a batch call (stream sample slots, offsets d_soff): keep flag 3 where
-// score > min_score, sample slots made cloud-local, d_hcount[b] (zeroed by the caller) counts cloud b's kept records
-int sis_filter(gpdb_ctx *ctx, gpdb_pose *d_rec, int n, const int *d_soff, int B, double min_score, uint8_t *d_keep,
-               int *d_hcount);
+// sis.cu (gpdb_sis_batch[_device], gpdb_sis_positions; include/gpd_b200_sis.h)
+// a new batch, or a SIS call that fails, leaves nothing for gpdb_sis_positions to read
+void sis_forget(gpdb_ctx *ctx);
+void sis_free(gpdb_ctx *ctx);  // gpdb_destroy: the SIS record
 
 // geometry.cu
 // builds the per-cloud grids of store s (its s.n descriptors hold off / N) and fills the descriptors' grid fields
@@ -545,72 +577,26 @@ int pre_filter_offsets(gpdb_ctx *ctx, const int *pos, const PreBatch &h, int B);
 int pre_voxelize_back(gpdb_ctx *ctx, CloudSet &s, const PreBatch &h, const int *foff, const int *keep, const float *xyz1,
                       const uint8_t *d_cam_raw, const double *d_nrm_raw, int B, const gpdb_preprocess_params &pp, int *poff);
 
-// depth.cu (include/gpd_b200_depth.h). The depth front of preprocessing: back-projection fused into the NaN / workspace
-// filter, then pre_voxelize_back. C cameras (d_cams, a device table written by depth_camera_table), cam_off[C+1] their
-// pixel offsets in the call (host), B views with raw offsets roff[B+1] (host, cumulative pixels per view).
-int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format, const gpdb_depth_camera *cams,
-                    const int *n_cameras, int B, const int *roff, const gpdb_preprocess_params &pp, int *poff,
-                    cudaEvent_t ev_filter_done);
-// Cloud::subsample of every cloud of store s: cloud b's draw to d_out at soff[b] (host, B + 1); returns the total or an
-// error. d_mask: one byte per installed point (per_point), or per raw point indexed by the store's raw_off (has_src)
-int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned long long seed, const uint8_t *d_mask,
-                   bool per_point, int *d_out, int *soff);
+// depth.cu (include/gpd_b200_depth.h)
+// the depth format of gpdb_preprocess_depth[_device] and gpdb_render_depth[_device]: GPDB_DEPTH_U16 or GPDB_DEPTH_F32
+int check_depth_format(gpdb_ctx *ctx, const char *name, int32_t format);
+// The camera checks of gpdb_preprocess_depth[_device] and gpdb_render_depth[_device]: view b has n_cameras[b] (1..8)
+// cameras, each of them well formed, and the call holds fewer than 2^31 pixels; roff[B+1] receives the raw offsets
+// (cumulative pixels per view)
+int check_depth_cameras(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras,
+                        const gpdb_depth_camera *cams, std::vector<int> &roff);
 
-// plane.cu (include/gpd_b200_plane.h). Segments every cloud of store s (cloud b with key pp.seed + b): planes[4B],
-// n_inliers[B] and n_hyp[B] (may be null) are host arrays, d_eligible (N bytes or null) device memory. Returns B.
-int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_params &pp, float *planes, int *n_inliers,
-                        int *n_hyp, uint8_t *d_eligible);
-// refine.cu (include/gpd_b200_refine.h). Refines the normals of every cloud of store s with k neighbours (1..128) and
-// refreshes the descriptors' nonunit flags; iters[B] (host) receives each cloud's iteration count. The stored normals
-// change only once every step before the final cast has succeeded. Returns B.
-int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters);
-// refine.cu: rule 1 of gpd_b200_refine.h alone. nbr[g*k + r], r < min(k, N_b): the cloud-local index of the r-th
+// refine.cu (include/gpd_b200_refine.h): rule 1 alone. nbr[g*k + r], r < min(k, N_b): the cloud-local index of the r-th
 // neighbour of concatenated point g of store s (device memory of N * k int32; k in 1..128).
 int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr);
-// outliers.cu (include/gpd_b200_outliers.h). Removes the statistical outliers of every cloud of store s with mean_k
-// neighbours (1..127) and reinstalls the kept points (grids, nonunit and all_seen flags as an install of them computes
-// them; sample positions dropped; the source indices and has_src kept). off[B+1] (host) receives the new point offsets;
-// stats[3B] (host, may be null) each cloud's mean, stddev and threshold; kept (host, may be null) one byte per point before
-// the call. Returns B, or an error after which s holds no cloud (s.n = 0), as after a failed install.
-int outliers_remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int *off, double *stats,
-                          uint8_t *kept);
-// organized.cu (include/gpd_b200_organized.h). Rules 2 - 5 on B organized clouds (cloud b: W[b] x H[b] points, view point
-// vp[3b..], concatenated in xyz): nrm_out [3 * pixels] and dist_out [pixels] (may be null). device: xyz and the outputs are
-// device arrays, else host arrays. `name` is the entry point the errors name.
-int org_normals_batch(gpdb_ctx *ctx, const char *name, int B, const int *W, const int *H, const float *xyz, const float *vp,
-                      float *nrm_out, float *dist_out, bool device);
-// Rules 6 and 7 on store s, just installed with radius normals by gpdb_preprocess_depth from the depth images d_depth
-// (device) of the B views with n_cameras[b] cameras cams: each point whose representative pixel has a finite organized
-// normal takes it in s.nrm; n_fallback[B] (host, may be null) receives the other points per view. The nonunit flags are
-// the caller's.
+// organized.cu (include/gpd_b200_organized.h). Rules 6 and 7 on store s, just installed with radius normals by
+// gpdb_preprocess_depth from the depth images d_depth (device) of the B views with n_cameras[b] cameras cams: each point
+// whose representative pixel has a finite organized normal takes it in s.nrm; n_fallback[B] (host, may be null) receives
+// the other points per view. The nonunit flags are the caller's.
 int org_depth_normals(gpdb_ctx *ctx, const char *name, CloudSet &s, const void *d_depth, int format,
                       const gpdb_depth_camera *cams, const int *n_cameras, int B, int *n_fallback);
 int pre_normals_batch(gpdb_ctx *ctx, CloudSet &s, double radius);  // normals of the installed store (grids built)
 int pre_nonunit_batch(gpdb_ctx *ctx, CloudSet &s);                 // per-cloud nonunit flags of the store, in the descriptors
-
-// render.cu (include/gpd_b200_render.h). B views (mesh b: vertices voff[b] .. voff[b+1]-1 of d_vtx, faces foff[b] ..
-// foff[b+1]-1 of d_faces, host offsets, checked) rendered by their n_cameras[b] cameras cams into d_depth (format) and
-// d_face (may be null), device arrays in the layout of gpdb_preprocess_depth.
-int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
-                       const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face);
-// The same seen by the structured-light sensor sp (include/gpd_b200_sensor.h, checked), view b with the key seed + b.
-int render_sensor_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
-                        const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face,
-                        const gpdb_sensor_params *sp, unsigned long long seed);
-// gpd_b200_sensor.h rule 2's table (GPDB_SENSOR_TABLE doubles, host), built on first use
-const double *sensor_table();
-// rule 6's counts of B checked meshes: returns the total (an error when negative) and mesh_n[B] (host) each mesh's
-// count (each face's count clamped to 2^31); when the total is below 2^31, poff[B+1] (host) receives the point offsets
-// and SCR_RENDER keeps the per-face scan for mesh_write_batch
-long long mesh_count_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
-                           double density, unsigned long long seed, int *poff, long long *mesh_n);
-// the N points mesh_count_batch counted (the same meshes and seed): xyz, normals and faces (each but xyz may be null)
-int mesh_write_batch(gpdb_ctx *ctx, int B, const int *foff, const float *d_vtx, const int *d_faces, unsigned long long seed,
-                     int N, float *d_xyz, double *d_nrm, int *d_face);
-// rule 7's mesh checks (offsets d_voff / d_foff on the device): lowers *d_first_bad to the first vertex i with a
-// non-finite coordinate (position i) or face f with an index outside its view's vertices (position V + f)
-int mesh_check(gpdb_ctx *ctx, const int *d_voff, const int *d_foff, int B, int V, int F, const float *d_vtx,
-               const int *d_faces, unsigned long long *d_first_bad);
 
 // lenet_simt.cu
 int lenet_upload(gpdb_ctx *ctx, const float *const w[8]);
@@ -631,16 +617,7 @@ int lenet_simt_run(gpdb_ctx *ctx, const LenetWeights &w, const uint8_t *d_images
                    float *d_scores, float *d_logits);
 
 // train.cu (include/gpd_b200_train.h)
-int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]);
-// one step on n device images / labels (labels already checked); d_loss_out / h_loss_out: device / host float or null; dbg: host outputs of a
-// debug step (any n, copied chunk by chunk), which updates nothing
-int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, int n, float *d_loss_out,
-               float *h_loss_out, const gpdb_train_debug *dbg);
-int train_weights(gpdb_ctx *ctx, float *const out[8]);
-bool train_started(const gpdb_ctx *ctx);
 void train_free(gpdb_ctx *ctx);
-// the label check of a step: lowers *d_bad to the first label outside {0, 1}
-int train_check_labels(gpdb_ctx *ctx, const int32_t *d_labels, int n, unsigned long long *d_bad);
 
 // lenet_tc.cu (wgmma conv1 / conv2 / ip1)
 int lenet_tc_upload(gpdb_ctx *ctx, const float *const w[8]);

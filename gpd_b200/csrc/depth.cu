@@ -8,8 +8,12 @@
 //     segmented radix sort of (key, eligible position) per cloud, k_sub_pick (each cloud's first k) and a scan +
 //     k_sub_gather of the picks, which restores ascending j.
 // Compiled with -fmad=false: every float32 / float64 operation of the back-projection is rounded on its own.
+// The entry points gpdb_preprocess_depth[_organized][_device] and gpdb_subsample_clouds[_points][_device], with their
+// argument checks, follow the kernels; the depth-format and camera checks are render.cu's too.
 #include <cfloat>
 #include <climits>
+#include <cmath>
+#include <cstring>
 #include <cub/cub.cuh>
 #include <vector>
 
@@ -125,8 +129,6 @@ __global__ void k_sub_gather(int E, const int *pick, const int *ppos, const int 
   if (e < E && pick[e]) out[ppos[e]] = vals[e];
 }
 
-}  // namespace
-
 // Back-projection + filter of the pixels of B views (camera descriptions cams, view b has n_cameras[b] of them; raw
 // offsets roff = cumulative pixels per view), then the voxelise / emit back of preprocess.cu
 int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format, const gpdb_depth_camera *cams,
@@ -195,6 +197,8 @@ int pre_depth_batch(gpdb_ctx *ctx, CloudSet &s, const void *d_depth, int format,
   return pre_voxelize_back(ctx, s, h, foff.data(), keep, xyz1, cam_raw, nullptr, B, pp, poff);
 }
 
+// Cloud::subsample of every cloud of store s: cloud b's draw to d_out at soff[b] (host, B + 1); returns the total or an
+// error. d_mask: one byte per installed point (per_point), or per raw point indexed by the store's raw_off (has_src)
 int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned long long seed, const uint8_t *d_mask,
                    bool per_point, int *d_out, int *soff) {
   const int tb = 256;
@@ -276,3 +280,230 @@ int sub_draw_batch(gpdb_ctx *ctx, const CloudSet &s, int num_samples, unsigned l
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return n;
 }
+
+}  // namespace
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+int check_depth_format(gpdb_ctx *ctx, const char *name, int32_t format) {
+  if (format == GPDB_DEPTH_U16 || format == GPDB_DEPTH_F32) return GPDB_OK;
+  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: unknown depth format %d (GPDB_DEPTH_U16 = 0, GPDB_DEPTH_F32 = 1)", name, format);
+  return GPDB_ERR_INVALID;
+}
+
+int check_depth_cameras(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras,
+                        const gpdb_depth_camera *cams, std::vector<int> &roff) {
+  roff.assign((size_t)B + 1, 0);
+  long long total = 0;
+  for (int b = 0, c = 0; b < B; b++) {
+    if (n_cameras[b] <= 0 || n_cameras[b] > GPDB_MAX_CAMERAS) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d has %d cameras (1 <= cameras <= %d)", name, b, n_cameras[b],
+                     GPDB_MAX_CAMERAS);
+      return GPDB_ERR_INVALID;
+    }
+    for (int k = 0; k < n_cameras[b]; k++, c++) {
+      const gpdb_depth_camera &D = cams[c];
+      const char *bad = nullptr;
+      bool finite = std::isfinite(D.fx) && std::isfinite(D.fy) && std::isfinite(D.cx) && std::isfinite(D.cy);
+      for (int e = 0; e < 12; e++) finite = finite && std::isfinite(D.pose[e]);
+      if (D.width < 1 || D.height < 1) bad = "width and height must be at least 1";
+      else if (!finite) bad = "non-finite intrinsics or pose";
+      else if (!(D.fx > 0.0) || !(D.fy > 0.0)) bad = "fx and fy must be positive";
+      else if (!(D.depth_scale > 0.0) || !std::isfinite(D.depth_scale)) bad = "depth_scale must be finite and positive";
+      else if (!(D.min_depth >= 0.0)) bad = "min_depth must be >= 0";
+      else if (!(D.max_depth > D.min_depth)) bad = "max_depth must exceed min_depth";
+      if (bad) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d (camera %d of the call): %s", name, b, k, c, bad);
+        return GPDB_ERR_INVALID;
+      }
+      total += (long long)D.width * D.height;
+      if (total >= (1ll << 31)) {
+        gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: view %d camera %d: the call holds 2^31 or more pixels", name, b, k);
+        return GPDB_ERR_INVALID;
+      }
+    }
+    roff[b + 1] = (int)total;
+  }
+  return GPDB_OK;
+}
+
+// the argument checks of gpdb_preprocess_depth[_device]; roff[B+1] receives the raw offsets (cumulative pixels per view)
+static int check_depth_args(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                            int32_t format, const void *depth, const gpdb_preprocess_params *pp, const int32_t *poff,
+                            std::vector<int> &roff) {
+  if (B <= 0 || !n_cameras || !cams || !depth || !pp || !poff) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth, params, processed_offsets_out",
+                   name);
+    return GPDB_ERR_INVALID;
+  }
+  if (check_depth_format(ctx, name, format) != GPDB_OK) return GPDB_ERR_INVALID;
+  if (!pp->estimate_normals) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: estimate_normals must be 1 (depth images carry no normals)", name);
+    return GPDB_ERR_INVALID;
+  }
+  const int rc = gpdb_check_preprocess_params(ctx, name, pp, nullptr);
+  if (rc != GPDB_OK) return rc;
+  return check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
+}
+
+// gpdb_preprocess_depth[_device] after the argument checks: d_depth in device memory (the host twin has uploaded it)
+// organized: the normals of gpd_b200_organized.h rule 7 replace the radius estimates (n_fallback[B], host, may be null)
+static int preprocess_depth(gpdb_ctx *ctx, const char *name, CloudSet &s, int32_t B, const int32_t *n_cameras,
+                            const gpdb_depth_camera *cams, int32_t format, const void *depth, bool device,
+                            const gpdb_preprocess_params *pp, const std::vector<int> &roff, int32_t *poff, bool organized,
+                            int32_t *n_fallback) {
+  cudaEvent_t *ev = ctx->ev;
+  const int M = roff[B];
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  cudaEventRecord(ev[0], ctx->stream);
+  const void *d_depth = depth;
+  if (!device) {
+    const size_t bytes = (size_t)M * (format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float));
+    void *up = gpdb_scratch(ctx, SCR_UPLOAD, bytes);
+    if (!up) return GPDB_ERR_CUDA;
+    CUDA_TRY(cudaMemcpyAsync(up, depth, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    d_depth = up;
+  }
+  // the camera fields of the descriptors: view point k = t of camera k; one-hot camera sources, as a cam_source matrix
+  std::vector<CloudDesc> desc((size_t)B);
+  for (int b = 0, c = 0; b < B; b++) {
+    CloudDesc &D = desc[b];
+    memset(&D, 0, sizeof(D));
+    D.K = n_cameras[b];
+    for (int k = 0; k < D.K; k++, c++)
+      for (int r = 0; r < 3; r++) D.vp[k][r] = cams[c].pose[4 * r + 3];
+  }
+  cudaEventRecord(ev[1], ctx->stream);
+  int rc = pre_depth_batch(ctx, s, d_depth, format, cams, n_cameras, B, roff.data(), *pp, poff, ev[2]);
+  if (rc != GPDB_OK) return rc;
+  if (!organized) return gpdb_preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff);
+  // the host twin's images stay in SCR_UPLOAD until here: the install does not use that slot
+  return gpdb_preprocess_install(ctx, s, desc.data(), B, roff.data(), pp, poff, [&]() {
+    return org_depth_normals(ctx, name, s, d_depth, format, cams, n_cameras, B, n_fallback);
+  });
+}
+
+static int depth_entry(gpdb_ctx *ctx, const char *name, int32_t n_views, const int32_t *n_cameras,
+                       const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
+                       const gpdb_preprocess_params *pp, int32_t *processed_offsets_out, bool device,
+                       bool organized = false, int32_t *n_fallback = nullptr) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  gpdb_drop_batch(ctx);
+  std::vector<int> roff;
+  int rc = check_depth_args(ctx, name, n_views, n_cameras, cameras, depth_format, depth, pp, processed_offsets_out, roff);
+  if (rc == GPDB_OK && device) rc = gpdb_check_device_ptrs(ctx, name, {{"d_depth", depth}});
+  if (rc != GPDB_OK) return rc;
+  return preprocess_depth(ctx, name, ctx->many, n_views, n_cameras, cameras, depth_format, depth, device, pp, roff,
+                          processed_offsets_out, organized, n_fallback);
+}
+
+// gpdb_subsample_clouds[_device]: the state and argument checks, then the device draw (the host twin uploads the mask and
+// copies the indices back)
+static int subsample_entry(gpdb_ctx *ctx, const char *name, int32_t num_samples, uint64_t seed, const uint8_t *mask,
+                           int32_t *idx_out, int32_t *offsets_out, bool device, bool per_point = false) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = ctx->many;
+  int rc = gpdb_need_batch(ctx, name, "gpdb_preprocess_depth / gpdb_preprocess_clouds");
+  if (rc != GPDB_OK) return rc;
+  if (num_samples < 0 || !offsets_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need num_samples >= 0 (got %d) and sample_offsets_out", name, num_samples);
+    return GPDB_ERR_INVALID;
+  }
+  if (mask && !per_point && !s.has_src) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: a mask needs the source indices of a preprocessing call (gpdb_preprocess_depth "
+                   "/ gpdb_preprocess_clouds); the batch was installed by gpdb_set_clouds", name);
+    return GPDB_ERR_STATE;
+  }
+  const int B = s.n;
+  long long room = 0;
+  for (int b = 0; b < B; b++) {
+    const int nb = s.off[b + 1] - s.off[b];
+    room += num_samples == 0 ? nb : std::min(num_samples, nb);
+  }
+  if (room > 0 && !idx_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null %s", name, device ? "d_sample_idx_out" : "sample_idx_out");
+    return GPDB_ERR_INVALID;
+  }
+  if (device && (rc = gpdb_check_device_ptrs(ctx, name, {{"d_mask", mask}, {"d_sample_idx_out", idx_out}})) != GPDB_OK)
+    return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const uint8_t *d_mask = mask;
+  int *d_out = idx_out;
+  if (!device) {
+    if (mask) {
+      const size_t M = per_point ? (size_t)s.points() : (size_t)s.raw_off[B];
+      uint8_t *up = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, M);
+      if (!up) return GPDB_ERR_CUDA;
+      CUDA_TRY(cudaMemcpyAsync(up, mask, M, cudaMemcpyHostToDevice, ctx->stream));
+      d_mask = up;
+    }
+    d_out = (int *)gpdb_scratch(ctx, SCR_SIDX, sizeof(int) * (size_t)room);
+    if (!d_out) return GPDB_ERR_CUDA;
+  }
+  std::vector<int> soff((size_t)B + 1);
+  const int n = sub_draw_batch(ctx, s, num_samples, seed, d_mask, per_point, d_out, soff.data());
+  if (n < 0) return n;
+  if (!device && n > 0) {
+    CUDA_TRY(cudaMemcpyAsync(idx_out, d_out, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  memcpy(offsets_out, soff.data(), sizeof(int) * ((size_t)B + 1));
+  return n;
+}
+
+extern "C" {
+
+int gpdb_preprocess_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                          int32_t depth_format, const void *depth, const gpdb_preprocess_params *pp,
+                          int32_t *processed_offsets_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth", n_views, n_cameras, cameras, depth_format, depth, pp,
+                     processed_offsets_out, false);
+}
+
+int gpdb_preprocess_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras, const gpdb_depth_camera *cameras,
+                                 int32_t depth_format, const void *d_depth, const gpdb_preprocess_params *pp,
+                                 int32_t *processed_offsets_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
+                     processed_offsets_out, true);
+}
+
+int gpdb_preprocess_depth_organized(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, const void *depth,
+                                    const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                    int32_t *n_fallback_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_organized", n_views, n_cameras, cameras, depth_format, depth, pp,
+                     processed_offsets_out, false, true, n_fallback_out);
+}
+
+int gpdb_preprocess_depth_organized_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *n_cameras,
+                                           const gpdb_depth_camera *cameras, int32_t depth_format, const void *d_depth,
+                                           const gpdb_preprocess_params *pp, int32_t *processed_offsets_out,
+                                           int32_t *n_fallback_out) {
+  return depth_entry(ctx, "gpdb_preprocess_depth_organized_device", n_views, n_cameras, cameras, depth_format, d_depth, pp,
+                     processed_offsets_out, true, true, n_fallback_out);
+}
+
+int gpdb_subsample_clouds(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *mask, int32_t *sample_idx_out,
+                          int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds", num_samples, seed, mask, sample_idx_out, sample_offsets_out, false);
+}
+
+int gpdb_subsample_clouds_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_mask,
+                                 int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_device", num_samples, seed, d_mask, d_sample_idx_out,
+                         sample_offsets_out, true);
+}
+
+int gpdb_subsample_clouds_points(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *point_mask,
+                                 int32_t *sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_points", num_samples, seed, point_mask, sample_idx_out,
+                         sample_offsets_out, false, true);
+}
+
+int gpdb_subsample_clouds_points_device(gpdb_ctx *ctx, int32_t num_samples, uint64_t seed, const uint8_t *d_point_mask,
+                                        int32_t *d_sample_idx_out, int32_t *sample_offsets_out) {
+  return subsample_entry(ctx, "gpdb_subsample_clouds_points_device", num_samples, seed, d_point_mask, d_sample_idx_out,
+                         sample_offsets_out, true, true);
+}
+
+}  // extern "C"

@@ -8,7 +8,8 @@
 //
 // The images of a call are processed in groups whose tables fit ORG_GROUP_BYTES; a group's points (host twin), distance
 // map, normals (host twin) and tables are carved from one scratch slot (SCR_ORGANIZED), sized once for the largest group.
-// Compiled with -fmad=false: every float32 / float64 operation is rounded on its own.
+// Compiled with -fmad=false: every float32 / float64 operation is rounded on its own. The entry points
+// gpdb_normals_organized[_device], with their argument checks, follow the kernels.
 #include <cfloat>
 #include <algorithm>
 #include <climits>
@@ -368,8 +369,9 @@ int org_scratch(gpdb_ctx *ctx, const char *name, const std::vector<OrgGroup> &gr
   return org_carve(ctx, n_max, p_max, (int)e_max, own_xyz, own_dist, own_nrm, o) ? GPDB_OK : GPDB_ERR_CUDA;
 }
 
-}  // namespace
-
+// Rules 2 - 5 on B organized clouds (cloud b: W[b] x H[b] points, view point vp[3b..], concatenated in xyz): nrm_out
+// [3 * pixels] and dist_out [pixels] (may be null). device: xyz and the outputs are device arrays, else host arrays.
+// `name` is the entry point the errors name.
 int org_normals_batch(gpdb_ctx *ctx, const char *name, int B, const int *W, const int *H, const float *xyz, const float *vp,
                       float *nrm_out, float *dist_out, bool device) {
   const std::vector<OrgGroup> groups = org_groups(B, W, H);
@@ -397,6 +399,8 @@ int org_normals_batch(gpdb_ctx *ctx, const char *name, int B, const int *W, cons
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return GPDB_OK;
 }
+
+}  // namespace
 
 int org_depth_normals(gpdb_ctx *ctx, const char *name, CloudSet &s, const void *d_depth, int format,
                       const gpdb_depth_camera *cams, const int *n_cameras, int B, int *n_fallback) {
@@ -465,3 +469,52 @@ int org_depth_normals(gpdb_ctx *ctx, const char *name, CloudSet &s, const void *
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return GPDB_OK;
 }
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+// gpdb_normals_organized[_device]: the argument checks, then rules 2 - 5 of gpd_b200_organized.h on every cloud
+static int organized_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *W, const int32_t *H, const float *xyz,
+                           const float *view_points, float *normals_out, float *distance_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !W || !H || !xyz || !view_points || !normals_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_clouds > 0, widths, heights, xyz, view_points, normals_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  long long total = 0;
+  for (int b = 0; b < B; b++) {
+    if (W[b] < 1 || H[b] < 1) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d is %d x %d (width and height must be at least 1)", name, b, W[b],
+                     H[b]);
+      return GPDB_ERR_INVALID;
+    }
+    total += (long long)W[b] * H[b];
+    if (total >= (1ll << 31)) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: cloud %d: the call holds 2^31 or more points", name, b);
+      return GPDB_ERR_INVALID;
+    }
+  }
+  int rc = device ? gpdb_check_device_ptrs(ctx, name, {{"d_xyz", xyz}, {"d_normals_out", normals_out},
+                                                       {"d_distance_out", distance_out}})
+                  : GPDB_OK;
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  rc = org_normals_batch(ctx, name, B, W, H, xyz, view_points, normals_out, distance_out, device);
+  return rc == GPDB_OK ? B : rc;
+}
+
+extern "C" {
+
+int gpdb_normals_organized(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights, const float *xyz,
+                           const float *view_points, float *normals_out, float *distance_out) {
+  return organized_entry(ctx, "gpdb_normals_organized", n_clouds, widths, heights, xyz, view_points, normals_out,
+                         distance_out, false);
+}
+
+int gpdb_normals_organized_device(gpdb_ctx *ctx, int32_t n_clouds, const int32_t *widths, const int32_t *heights,
+                                  const float *d_xyz, const float *view_points, float *d_normals_out,
+                                  float *d_distance_out) {
+  return organized_entry(ctx, "gpdb_normals_organized_device", n_clouds, widths, heights, d_xyz, view_points,
+                         d_normals_out, d_distance_out, true);
+}
+
+}  // extern "C"

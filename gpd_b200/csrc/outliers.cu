@@ -11,7 +11,9 @@
 // The gathered arrays go back into the store's arenas and the store is reinstalled with the new offsets, which rebuilds
 // the grids and the nonunit flags; each cloud's all_seen flag is recomputed from the kept masks. Whatever step fails, the
 // store is left without a cloud, as a failed install leaves it. Compiled with -fmad=false: every operation of the
-// specification is rounded on its own.
+// specification is rounded on its own. The entry points gpdb_remove_outliers and gpdb_remove_outliers_clouds, with their
+// checks, follow the kernels.
+#include <algorithm>
 #include <cmath>
 #include <vector>
 
@@ -167,8 +169,11 @@ int remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int 
   return B;
 }
 
-}  // namespace
-
+// Removes the statistical outliers of every cloud of store s with mean_k neighbours (1..127) and reinstalls the kept
+// points (grids, nonunit and all_seen flags as an install of them computes them; sample positions dropped; the source
+// indices and has_src kept). off[B+1] (host) receives the new point offsets; stats[3B] (host, may be null) each cloud's
+// mean, stddev and threshold; kept (host, may be null) one byte per point before the call. Returns B, or an error after
+// which s holds no cloud (s.n = 0), as after a failed install.
 int outliers_remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_mul, int *off, double *stats,
                           uint8_t *kept) {
   const int rc = remove_batch(ctx, s, mean_k, stddev_mul, off, stats, kept);
@@ -178,3 +183,59 @@ int outliers_remove_batch(gpdb_ctx *ctx, CloudSet &s, int mean_k, double stddev_
   }
   return rc;
 }
+
+}  // namespace
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+// gpdb_remove_outliers / gpdb_remove_outliers_clouds: the state and argument checks, then outliers_remove_batch on the
+// single cloud (single) or the batch. It reinstalls the store: the batch loses its SIS record, and any failure after the
+// checks leaves no cloud (no batch: gpdb_drop_batch), as a failed install does. Returns the kept points (single) or B.
+static int outliers_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t mean_k, double stddev_mul,
+                          int32_t *offsets_out, double *stats_out, uint8_t *kept_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : gpdb_need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (mean_k < 1 || mean_k > GPDB_OUTLIERS_MAX_K) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mean_k must lie in 1..%d (got %d)", name, GPDB_OUTLIERS_MAX_K, (int)mean_k);
+    return GPDB_ERR_INVALID;
+  }
+  if (!std::isfinite(stddev_mul)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: stddev_mul must be finite", name);
+    return GPDB_ERR_INVALID;
+  }
+  std::vector<int> off((size_t)s.n + 1);
+  const cudaError_t e = cudaSetDevice(ctx->device);
+  if (e != cudaSuccess) {
+    gpdb_set_error(ctx, GPDB_ERR_CUDA, "%s: cudaSetDevice -> %s", name, cudaGetErrorString(e));
+    rc = GPDB_ERR_CUDA;
+  } else {
+    rc = outliers_remove_batch(ctx, s, mean_k, stddev_mul, off.data(), stats_out, kept_out);
+  }
+  if (rc < 0) {
+    s.n = 0;
+    s.has_src = false;
+    if (!single) gpdb_drop_batch(ctx);
+    return rc;
+  }
+  if (!single) sis_forget(ctx);  // the SIS positions describe clouds that are gone
+  if (offsets_out) std::copy(off.begin(), off.end(), offsets_out);
+  if (!single) return rc;
+  if (off[1] == 0) s.n = 0;  // no point kept: no cloud, as gpdb_preprocess when its filter keeps none
+  return off[1];
+}
+
+extern "C" {
+
+int gpdb_remove_outliers(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, double stats_out[3], uint8_t *kept_out) {
+  return outliers_entry(ctx, "gpdb_remove_outliers", true, mean_k, stddev_mul, nullptr, stats_out, kept_out);
+}
+
+int gpdb_remove_outliers_clouds(gpdb_ctx *ctx, int32_t mean_k, double stddev_mul, int32_t *offsets_out,
+                                double *stats_out, uint8_t *kept_out) {
+  return outliers_entry(ctx, "gpdb_remove_outliers_clouds", false, mean_k, stddev_mul, offsets_out, stats_out, kept_out);
+}
+
+}  // extern "C"

@@ -9,6 +9,7 @@
 //                  sums of computeMeanAndCovarianceMatrix and pcl::eigen33 (the k_normals code, pcl_eigen33.cuh).
 //   k_plane_mark   one thread per point: the final threshold test, the eligible bytes, per-cloud inlier counts.
 // Compiled with -fmad=false: every float32 / float64 operation of the specification is rounded on its own.
+// The entry points gpdb_segment_plane and gpdb_segment_planes[_device], with their checks, follow the kernels.
 #include <cfloat>
 #include <climits>
 #include <cmath>
@@ -248,8 +249,8 @@ __global__ void __launch_bounds__(256) k_plane_mark(const float *xyz, const int 
   if (live && hits && (threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(fin + b, __popc(hits));
 }
 
-}  // namespace
-
+// Segments every cloud of store s (cloud b with key pp.seed + b): planes[4B], n_inliers[B] and n_hyp[B] (may be null) are
+// host arrays, d_eligible (N bytes or null) device memory. Returns B.
 int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_params &pp, float *planes, int *n_inliers,
                         int *n_hyp, uint8_t *d_eligible) {
   const int B = s.n, N = s.points(), H = pp.max_iterations + 1;
@@ -302,3 +303,77 @@ int plane_segment_batch(gpdb_ctx *ctx, const CloudSet &s, const gpdb_plane_param
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return B;
 }
+
+}  // namespace
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+// gpdb_segment_plane / gpdb_segment_planes[_device]: the state and argument checks, then plane_segment_batch on the
+// single cloud (single) or the batch. The host twins let the eligible bytes come back through SCR_UPLOAD.
+static int segment_entry(gpdb_ctx *ctx, const char *name, bool single, const gpdb_plane_params *pl, float *planes_out,
+                         int32_t *n_inliers_out, int32_t *n_hyp_out, uint8_t *eligible_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : gpdb_need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (!pl || !planes_out || !n_inliers_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need params, %s and n_inliers_out", name, single ? "plane_out" : "planes_out");
+    return GPDB_ERR_INVALID;
+  }
+  const char *bad = nullptr;
+  if (!std::isfinite(pl->distance_threshold) || !(pl->distance_threshold > 0.0))
+    bad = "distance_threshold must be finite and positive";
+  else if (pl->max_iterations < 1 || pl->max_iterations > GPDB_PLANE_MAX_ITERATIONS)
+    bad = "max_iterations must lie in 1..1024";
+  else if (!(pl->probability > 0.0 && pl->probability < 1.0))
+    bad = "probability must lie in (0, 1)";
+  if (bad) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s", name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  if (device && (rc = gpdb_check_device_ptrs(ctx, name, {{"d_eligible_out", eligible_out}})) != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const int N = s.points();
+  uint8_t *d_elig = eligible_out;
+  if (!device && eligible_out) {
+    d_elig = (uint8_t *)gpdb_scratch(ctx, SCR_UPLOAD, (size_t)N + 16);
+    if (!d_elig) return GPDB_ERR_CUDA;
+  }
+  rc = plane_segment_batch(ctx, s, *pl, planes_out, n_inliers_out, n_hyp_out, d_elig);
+  if (rc < 0) return rc;
+  if (!device && eligible_out && N > 0) {
+    CUDA_TRY(cudaMemcpyAsync(eligible_out, d_elig, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  return rc;
+}
+
+extern "C" {
+
+void gpdb_plane_params_default(gpdb_plane_params *p) {
+  if (!p) return;
+  p->distance_threshold = 0.01;
+  p->max_iterations = 50;
+  p->probability = 0.99;
+  p->seed = 0;
+}
+
+int gpdb_segment_plane(gpdb_ctx *ctx, const gpdb_plane_params *pl, float plane_out[4], int32_t *n_inliers_out,
+                       uint8_t *eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_plane", true, pl, plane_out, n_inliers_out, nullptr, eligible_out, false);
+}
+
+int gpdb_segment_planes(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                        int32_t *n_hypotheses_out, uint8_t *eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_planes", false, pl, planes_out, n_inliers_out, n_hypotheses_out, eligible_out,
+                       false);
+}
+
+int gpdb_segment_planes_device(gpdb_ctx *ctx, const gpdb_plane_params *pl, float *planes_out, int32_t *n_inliers_out,
+                               int32_t *n_hypotheses_out, uint8_t *d_eligible_out) {
+  return segment_entry(ctx, "gpdb_segment_planes_device", false, pl, planes_out, n_inliers_out, n_hypotheses_out,
+                       d_eligible_out, true);
+}
+
+}  // extern "C"

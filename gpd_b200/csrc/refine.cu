@@ -12,6 +12,8 @@
 // The lists are N x k int32; the iterates ping-pong between two float4 arrays: iteration t reads buf[(t - 1) & 1] and
 // writes buf[t & 1], so a cloud done after m iterations holds its result in buf[m & 1]. Nothing in the store changes
 // before k_refine_commit. Compiled with -fmad=false: every float32 operation of the specification is rounded on its own.
+// The entry points gpdb_refine_normals and gpdb_refine_normals_clouds, with their checks, follow the kernels.
+#include <algorithm>
 #include <cfloat>
 #include <climits>
 #include <cmath>
@@ -237,7 +239,10 @@ int refine_knn_lists(gpdb_ctx *ctx, const CloudSet &s, int k, int *nbr) {
   return GPDB_OK;
 }
 
-int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
+// Refines the normals of every cloud of store s with k neighbours (1..128) and refreshes the descriptors' nonunit flags;
+// iters[B] (host) receives each cloud's iteration count. The stored normals change only once every step before the final
+// cast has succeeded. Returns B.
+static int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
   const int B = s.n, N = s.points();
   const size_t n = (size_t)N;
   float4 *buf0, *buf1;
@@ -278,3 +283,37 @@ int refine_normals_batch(gpdb_ctx *ctx, CloudSet &s, int k, int *iters) {
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   return B;
 }
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+// gpdb_refine_normals / gpdb_refine_normals_clouds: the state and argument checks, then refine_normals_batch on the single
+// cloud (single) or the batch
+static int refine_entry(gpdb_ctx *ctx, const char *name, bool single, int32_t k, int32_t *iterations_out) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  CloudSet &s = single ? ctx->one : ctx->many;
+  int rc = single ? gpdb_check_state(ctx, true, false)
+                  : gpdb_need_batch(ctx, name, "gpdb_set_clouds / gpdb_preprocess_clouds / gpdb_preprocess_depth");
+  if (rc != GPDB_OK) return rc;
+  if (k < 1 || k > GPDB_REFINE_MAX_K) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: k must lie in 1..%d (got %d)", name, GPDB_REFINE_MAX_K, (int)k);
+    return GPDB_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  std::vector<int> iters((size_t)s.n);
+  rc = refine_normals_batch(ctx, s, k, iters.data());
+  if (rc < 0) return rc;
+  if (iterations_out) std::copy(iters.begin(), iters.end(), iterations_out);
+  return rc;
+}
+
+extern "C" {
+
+int gpdb_refine_normals(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
+  return refine_entry(ctx, "gpdb_refine_normals", true, k, iterations_out);
+}
+
+int gpdb_refine_normals_clouds(gpdb_ctx *ctx, int32_t k, int32_t *iterations_out) {
+  return refine_entry(ctx, "gpdb_refine_normals_clouds", false, k, iterations_out);
+}
+
+}  // extern "C"

@@ -23,8 +23,13 @@
 // Sampling: k_mesh_count per face (rule 6's count, a 64-bit total), scan_flags over the counts once the total is known
 // to lie below 2^31, then k_mesh_write per point. Scratch: SCR_RENDER. Compiled with -fmad=false: every float64
 // operation is rounded on its own.
+//
+// The entry points gpdb_render_depth[_device], gpdb_render_sensor_depth[_device] and gpdb_sample_meshes[_device], with
+// their checks and the host twins' uploads, follow the kernels.
 #include <algorithm>
 #include <climits>
+#include <cmath>
+#include <cstring>
 #include <vector>
 
 #include "../../include/gpd_b200_render.h"
@@ -249,8 +254,8 @@ struct RndScratch {
   int *spix_off;
 };
 
-// The table of gpd_b200_sensor.h rule 2, built once
-const double *sensor_table_host() {
+// gpd_b200_sensor.h rule 2's table (GPDB_SENSOR_TABLE doubles, host), built on first use
+const double *sensor_table() {
   static const std::vector<double> T = [] {
     std::vector<double> t(GPDB_SENSOR_TABLE);
     gpdb_sensor_table_build(t.data());
@@ -350,7 +355,7 @@ int render_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const f
       }))
     return GPDB_ERR_CUDA;
   if (sp)
-    CUDA_TRY(cudaMemcpyAsync(s.table, sensor_table_host(), sizeof(double) * GPDB_SENSOR_TABLE, cudaMemcpyHostToDevice,
+    CUDA_TRY(cudaMemcpyAsync(s.table, sensor_table(), sizeof(double) * GPDB_SENSOR_TABLE, cudaMemcpyHostToDevice,
                              ctx->stream));
   const int tb = 256;
   for (const RndGroup &G : groups) {
@@ -445,22 +450,20 @@ int render_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const f
   return GPDB_OK;
 }
 
-}  // namespace
-
+// B views (mesh b: vertices voff[b] .. voff[b+1]-1 of d_vtx, faces foff[b] .. foff[b+1]-1 of d_faces, host offsets,
+// checked) rendered by their n_cameras[b] cameras cams into d_depth (format) and d_face (may be null), device arrays in the
+// layout of gpdb_preprocess_depth.
 int render_depth_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
                        const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face) {
   return render_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, nullptr, 0);
 }
 
+// The same seen by the structured-light sensor sp (include/gpd_b200_sensor.h, checked), view b with the key seed + b.
 int render_sensor_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
                         const int *n_cameras, const gpdb_depth_camera *cams, int format, void *d_depth, int *d_face,
                         const gpdb_sensor_params *sp, unsigned long long seed) {
   return render_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, sp, seed);
 }
-
-const double *sensor_table() { return sensor_table_host(); }
-
-namespace {
 
 // rule 6's count of every face of the call (mesh b: faces foff[b] .. foff[b+1]-1, vertices from voff[b]); cnt[f] is the
 // count clamped to INT_MAX, total[b] (zeroed by the caller) the sum of mesh b's counts each clamped to 2^31, so the
@@ -524,8 +527,9 @@ bool mesh_carve(gpdb_ctx *ctx, int B, int F, MeshScratch &m) {
   });
 }
 
-}  // namespace
-
+// rule 6's counts of B checked meshes: returns the total (an error when negative) and mesh_n[B] (host) each mesh's
+// count (each face's count clamped to 2^31); when the total is below 2^31, poff[B+1] (host) receives the point offsets
+// and SCR_RENDER keeps the per-face scan for mesh_write_batch
 long long mesh_count_batch(gpdb_ctx *ctx, int B, const int *voff, const int *foff, const float *d_vtx, const int *d_faces,
                            double density, unsigned long long seed, int *poff, long long *mesh_n) {
   const int F = foff[B];
@@ -553,6 +557,7 @@ long long mesh_count_batch(gpdb_ctx *ctx, int B, const int *voff, const int *fof
   return total;
 }
 
+// the N points mesh_count_batch counted (the same meshes and seed): xyz, normals and faces (each but xyz may be null)
 int mesh_write_batch(gpdb_ctx *ctx, int B, const int *foff, const float *d_vtx, const int *d_faces, unsigned long long seed,
                      int N, float *d_xyz, double *d_nrm, int *d_face) {
   if (N == 0) return GPDB_OK;
@@ -563,8 +568,6 @@ int mesh_write_batch(gpdb_ctx *ctx, int B, const int *foff, const float *d_vtx, 
   LAUNCH_CHECK();
   return GPDB_OK;
 }
-
-namespace {
 
 // rule 7's mesh checks: position i < V is vertex i (a non-finite coordinate), position V + f is face f (an index
 // outside its view's vertices)
@@ -584,8 +587,8 @@ __global__ void k_mesh_check(const int *voff, const int *foff, int B, int V, int
   }
 }
 
-}  // namespace
-
+// rule 7's mesh checks (offsets d_voff / d_foff on the device): lowers *d_first_bad to the first vertex i with a
+// non-finite coordinate (position i) or face f with an index outside its view's vertices (position V + f)
 int mesh_check(gpdb_ctx *ctx, const int *d_voff, const int *d_foff, int B, int V, int F, const float *d_vtx,
                const int *d_faces, unsigned long long *d_first_bad) {
   const long long n = (long long)V + F;
@@ -595,3 +598,272 @@ int mesh_check(gpdb_ctx *ctx, const int *d_voff, const int *d_foff, int B, int V
   LAUNCH_CHECK();
   return GPDB_OK;
 }
+
+}  // namespace
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+// the offsets of B meshes (rule 7): vertex_offsets and face_offsets start at 0 and never decrease, and the arrays they
+// address are given; `unit` names a mesh in the messages
+static int check_mesh_args(gpdb_ctx *ctx, const char *name, const char *unit, int32_t B, const int32_t *voff,
+                           const float *vertices, const int32_t *foff, const int32_t *faces) {
+  int rc = gpdb_check_offsets(ctx, name, "vertex_offsets", voff, B, unit);
+  if (rc == GPDB_OK) rc = gpdb_check_offsets(ctx, name, "face_offsets", foff, B, unit);
+  if (rc != GPDB_OK) return rc;
+  if ((voff[B] > 0 && !vertices) || (foff[B] > 0 && !faces)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: null vertices or faces for %d vertices and %d faces", name, voff[B], foff[B]);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// rule 7's device checks of B meshes in device memory: a non-finite vertex or a face index outside its mesh's vertices,
+// the first of them named
+static int check_meshes(gpdb_ctx *ctx, const char *name, const char *unit, int B, const int32_t *voff, const int32_t *foff,
+                        const float *d_vtx, const int32_t *d_faces) {
+  const int V = voff[B], F = foff[B];
+  const size_t bytes = sizeof(int) * 2 * ((size_t)B + 1);
+  unsigned long long bad;
+  const int rc = first_bad(ctx, bytes, &bad, [&](unsigned long long *d_bad, void *d) -> int {
+    int *d_voff = (int *)d, *d_foff = d_voff + B + 1;
+    CUDA_TRY(cudaMemcpyAsync(d_voff, voff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(d_foff, foff, sizeof(int) * ((size_t)B + 1), cudaMemcpyHostToDevice, ctx->stream));
+    return mesh_check(ctx, d_voff, d_foff, B, V, F, d_vtx, d_faces, d_bad);
+  });
+  if (rc != GPDB_OK || bad == NO_BAD) return rc;
+  int b = 0;
+  if (bad < (unsigned long long)V) {
+    while (voff[b + 1] <= (long long)bad) b++;
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: vertex %d has a non-finite coordinate", name, unit, b,
+                   (int)(bad - voff[b]));
+    return GPDB_ERR_INVALID;
+  }
+  const int f = (int)(bad - V);
+  while (foff[b + 1] <= f) b++;
+  int32_t tri[3];
+  CUDA_TRY(cudaMemcpyAsync(tri, d_faces + 3 * (size_t)f, sizeof(tri), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: %s %d: face %d = (%d, %d, %d) indexes outside its %d vertices", name, unit, b,
+                 f - foff[b], tri[0], tri[1], tri[2], voff[b + 1] - voff[b]);
+  return GPDB_ERR_INVALID;
+}
+
+// gpd_b200_sensor.h rule 9's parameter checks
+static int check_sensor_params(gpdb_ctx *ctx, const char *name, const gpdb_sensor_params *sp) {
+  if (!sp) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need sensor (gpdb_sensor_params_default for a clean render)", name);
+    return GPDB_ERR_INVALID;
+  }
+  const struct {
+    const char *name;
+    double v;
+  } f[] = {{"baseline", sp->baseline},
+           {"lateral_sigma", sp->lateral_sigma},
+           {"disparity_sigma", sp->disparity_sigma},
+           {"disparity_step", sp->disparity_step},
+           {"min_cos_incidence", sp->min_cos_incidence},
+           {"shadow_tolerance", sp->shadow_tolerance},
+           {"dropout", sp->dropout}};
+  const char *bad = nullptr;
+  for (const auto &e : f)
+    if (!(e.v >= 0.0) || !std::isfinite(e.v)) {
+      gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s must be finite and >= 0 (got %g)", name, e.name, e.v);
+      return GPDB_ERR_INVALID;
+    }
+  if (sp->dropout > 1.0) bad = "dropout must lie in [0, 1]";
+  else if (sp->shadow_tolerance >= 1.0) bad = "shadow_tolerance must be < 1";
+  else if (sp->min_cos_incidence > 1.0) bad = "min_cos_incidence must be <= 1";
+  else if ((sp->disparity_sigma > 0.0 || sp->disparity_step > 0.0) && !(sp->baseline > 0.0))
+    bad = "disparity_sigma and disparity_step need a baseline > 0";
+  if (bad) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: sensor: %s", name, bad);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// gpdb_render_depth[_device] and (sensor) gpdb_render_sensor_depth[_device]: the checks, then the device render (the host
+// twin uploads the meshes into SCR_UPLOAD, renders into it and copies the images back). Nothing installed changes.
+static int render_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
+                        const int32_t *foff, const int32_t *faces, const int32_t *n_cameras, const gpdb_depth_camera *cams,
+                        int32_t format, void *depth_out, int32_t *face_out, bool device, bool sensor = false,
+                        const gpdb_sensor_params *sp = nullptr, uint64_t seed = 0) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !n_cameras || !cams || !depth_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_views > 0, n_cameras, cameras, depth_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  if (check_depth_format(ctx, name, format) != GPDB_OK) return GPDB_ERR_INVALID;
+  if (sensor && check_sensor_params(ctx, name, sp) != GPDB_OK) return GPDB_ERR_INVALID;
+  std::vector<int> roff;
+  int rc = check_mesh_args(ctx, name, "view", B, voff, vertices, foff, faces);
+  if (rc == GPDB_OK) rc = check_depth_cameras(ctx, name, B, n_cameras, cams, roff);
+  if (rc == GPDB_OK && device)
+    rc = gpdb_check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_depth_out", depth_out},
+                                            {"d_face_out", face_out}});
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const size_t V = (size_t)voff[B], F = (size_t)foff[B], M = (size_t)roff[B];
+  const size_t elt = format == GPDB_DEPTH_U16 ? sizeof(uint16_t) : sizeof(float);
+  const float *d_vtx = vertices;
+  const int32_t *d_faces = faces;
+  void *d_depth = depth_out;
+  int32_t *d_face = face_out;
+  if (!device) {
+    float *v;
+    int32_t *f;
+    unsigned char *dd;
+    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
+          v = c.take<float>(3 * V);
+          f = c.take<int32_t>(3 * F);
+          dd = c.take<unsigned char>(elt * M, 16);
+          d_face = face_out ? c.take<int32_t>(M) : nullptr;
+        }))
+      return GPDB_ERR_CUDA;
+    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
+    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
+    d_vtx = v, d_faces = f, d_depth = dd;
+  }
+  if ((rc = check_meshes(ctx, name, "view", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
+  rc = sensor ? render_sensor_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face, sp, seed)
+              : render_depth_batch(ctx, B, voff, foff, d_vtx, d_faces, n_cameras, cams, format, d_depth, d_face);
+  if (rc != GPDB_OK) return rc;
+  if (!device) {
+    CUDA_TRY(cudaMemcpyAsync(depth_out, d_depth, elt * M, cudaMemcpyDeviceToHost, ctx->stream));
+    if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * M, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  }
+  return B;
+}
+
+// gpdb_sample_meshes[_device]: the checks, the count, then (xyz_out given) the points. The host twin uploads the meshes
+// into SCR_UPLOAD, and once the count is known carves the outputs behind them there (uploading again: a grown slot
+// starts empty). Nothing installed changes.
+static int sample_entry(gpdb_ctx *ctx, const char *name, int32_t B, const int32_t *voff, const float *vertices,
+                        const int32_t *foff, const int32_t *faces, double density, uint64_t seed, int32_t *poff_out,
+                        float *xyz_out, double *normals_out, int32_t *face_out, bool device) {
+  if (!ctx) return GPDB_ERR_INVALID;
+  if (B <= 0 || !poff_out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need n_meshes > 0 and point_offsets_out", name);
+    return GPDB_ERR_INVALID;
+  }
+  if (!(density > 0.0) || !std::isfinite(density)) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: density must be finite and > 0 (got %g)", name, density);
+    return GPDB_ERR_INVALID;
+  }
+  int rc = check_mesh_args(ctx, name, "mesh", B, voff, vertices, foff, faces);
+  if (rc == GPDB_OK && device)
+    rc = gpdb_check_device_ptrs(ctx, name, {{"d_vertices", vertices}, {"d_faces", faces}, {"d_xyz_out", xyz_out},
+                                            {"d_normals_out", normals_out}, {"d_face_out", face_out}});
+  if (rc != GPDB_OK) return rc;
+  CUDA_TRY(cudaSetDevice(ctx->device));
+  const size_t V = (size_t)voff[B], F = (size_t)foff[B];
+  const float *d_vtx = vertices;
+  const int32_t *d_faces = faces;
+  float *d_xyz = xyz_out;
+  double *d_nrm = normals_out;
+  int32_t *d_face = face_out;
+  // the host twin's buffers: the meshes, then n points of the outputs the caller asked for
+  auto upload = [&](size_t n) -> int {
+    float *v;
+    int32_t *f;
+    if (!gpdb_carve(ctx, SCR_UPLOAD, [&](Carve &c) {
+          v = c.take<float>(3 * V);
+          f = c.take<int32_t>(3 * F);
+          d_xyz = c.take<float>(3 * n);
+          d_nrm = normals_out ? c.take<double>(3 * n) : nullptr;
+          d_face = face_out ? c.take<int32_t>(n) : nullptr;
+        }))
+      return GPDB_ERR_CUDA;
+    if (V) CUDA_TRY(cudaMemcpyAsync(v, vertices, sizeof(float) * 3 * V, cudaMemcpyHostToDevice, ctx->stream));
+    if (F) CUDA_TRY(cudaMemcpyAsync(f, faces, sizeof(int32_t) * 3 * F, cudaMemcpyHostToDevice, ctx->stream));
+    d_vtx = v, d_faces = f;
+    return GPDB_OK;
+  };
+  if (!device && (rc = upload(0)) != GPDB_OK) return rc;
+  if ((rc = check_meshes(ctx, name, "mesh", B, voff, foff, d_vtx, d_faces)) != GPDB_OK) return rc;
+  std::vector<int> poff((size_t)B + 1);
+  std::vector<long long> mesh_n((size_t)B);
+  const long long n = mesh_count_batch(ctx, B, voff, foff, d_vtx, d_faces, density, seed, poff.data(), mesh_n.data());
+  if (n < 0) return (int)n;
+  if (n >= (1ll << 31)) {
+    long long run = 0;
+    int b = 0;
+    while ((run += mesh_n[b]) < (1ll << 31)) b++;
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: mesh %d: the call reaches 2^31 or more sampled points (lower the density)",
+                   name, b);
+    return GPDB_ERR_INVALID;
+  }
+  if (xyz_out && n > 0) {
+    if (!device && (rc = upload((size_t)n)) != GPDB_OK) return rc;
+    if ((rc = mesh_write_batch(ctx, B, foff, d_vtx, d_faces, seed, (int)n, d_xyz, d_nrm, d_face)) != GPDB_OK) return rc;
+    if (!device) {
+      CUDA_TRY(cudaMemcpyAsync(xyz_out, d_xyz, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+      if (normals_out)
+        CUDA_TRY(cudaMemcpyAsync(normals_out, d_nrm, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, ctx->stream));
+      if (face_out) CUDA_TRY(cudaMemcpyAsync(face_out, d_face, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+      CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+  }
+  memcpy(poff_out, poff.data(), sizeof(int32_t) * ((size_t)B + 1));
+  return (int)n;
+}
+
+extern "C" {
+
+int gpdb_render_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                      const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                      const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out) {
+  return render_entry(ctx, "gpdb_render_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras, cameras,
+                      depth_format, depth_out, face_out, false);
+}
+
+int gpdb_render_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                             const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                             int32_t *d_face_out) {
+  return render_entry(ctx, "gpdb_render_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces, n_cameras,
+                      cameras, depth_format, d_depth_out, d_face_out, true);
+}
+
+void gpdb_sensor_params_default(gpdb_sensor_params *p) {
+  if (p) memset(p, 0, sizeof(*p));
+}
+
+int gpdb_render_sensor_depth(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *vertices,
+                             const int32_t *face_offsets, const int32_t *faces, const int32_t *n_cameras,
+                             const gpdb_depth_camera *cameras, int32_t depth_format, void *depth_out, int32_t *face_out,
+                             const gpdb_sensor_params *sensor, uint64_t seed) {
+  return render_entry(ctx, "gpdb_render_sensor_depth", n_views, vertex_offsets, vertices, face_offsets, faces, n_cameras,
+                      cameras, depth_format, depth_out, face_out, false, true, sensor, seed);
+}
+
+int gpdb_render_sensor_depth_device(gpdb_ctx *ctx, int32_t n_views, const int32_t *vertex_offsets, const float *d_vertices,
+                                    const int32_t *face_offsets, const int32_t *d_faces, const int32_t *n_cameras,
+                                    const gpdb_depth_camera *cameras, int32_t depth_format, void *d_depth_out,
+                                    int32_t *d_face_out, const gpdb_sensor_params *sensor, uint64_t seed) {
+  return render_entry(ctx, "gpdb_render_sensor_depth_device", n_views, vertex_offsets, d_vertices, face_offsets, d_faces,
+                      n_cameras, cameras, depth_format, d_depth_out, d_face_out, true, true, sensor, seed);
+}
+
+int gpdb_debug_sensor_table(double *table_out) {
+  if (!table_out) return GPDB_ERR_INVALID;
+  memcpy(table_out, sensor_table(), sizeof(double) * GPDB_SENSOR_TABLE);
+  return GPDB_SENSOR_TABLE;
+}
+
+int gpdb_sample_meshes(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *vertices,
+                       const int32_t *face_offsets, const int32_t *faces, double density, uint64_t seed,
+                       int32_t *point_offsets_out, float *xyz_out, double *normals_out, int32_t *face_out) {
+  return sample_entry(ctx, "gpdb_sample_meshes", n_meshes, vertex_offsets, vertices, face_offsets, faces, density, seed,
+                      point_offsets_out, xyz_out, normals_out, face_out, false);
+}
+
+int gpdb_sample_meshes_device(gpdb_ctx *ctx, int32_t n_meshes, const int32_t *vertex_offsets, const float *d_vertices,
+                              const int32_t *face_offsets, const int32_t *d_faces, double density, uint64_t seed,
+                              int32_t *point_offsets_out, float *d_xyz_out, double *d_normals_out, int32_t *d_face_out) {
+  return sample_entry(ctx, "gpdb_sample_meshes_device", n_meshes, vertex_offsets, d_vertices, face_offsets, d_faces, density,
+                      seed, point_offsets_out, d_xyz_out, d_normals_out, d_face_out, true);
+}
+
+}  // extern "C"

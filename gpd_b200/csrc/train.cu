@@ -10,7 +10,8 @@
 //   k_conv2_wgrad / k_conv1_wgrad  per-image weight and bias gradients over the pooled positions; k_colsum chains them
 //   k_dpool1     d pool1 from d conv2 (one fixed order over filter, kh, kw)
 // then one element-wise optimiser kernel over the eight parameter arrays. No atomics on floats anywhere: every sum has
-// one order, so identical call sequences give identical weights.
+// one order, so identical call sequences give identical weights. The entry points gpdb_train_begin,
+// gpdb_train_step[_device], gpdb_debug_train_step and gpdb_train_weights, with their checks, follow the kernels.
 #include <algorithm>
 #include <cmath>
 
@@ -497,7 +498,7 @@ bool params_ok(const gpdb_train_params &p) {
 
 }  // namespace
 
-bool train_started(const gpdb_ctx *ctx) { return ctx->train != nullptr; }
+static bool train_started(const gpdb_ctx *ctx) { return ctx->train != nullptr; }
 
 void train_free(gpdb_ctx *ctx) {
   if (!ctx->train) return;
@@ -506,7 +507,7 @@ void train_free(gpdb_ctx *ctx) {
   ctx->train = nullptr;
 }
 
-int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]) {
+static int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]) {
   if (!p || !params_ok(*p)) {
     gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_train_begin: bad training parameters");
     return GPDB_ERR_INVALID;
@@ -576,14 +577,17 @@ int train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const in
   return GPDB_OK;
 }
 
-int train_check_labels(gpdb_ctx *ctx, const int32_t *d_labels, int n, unsigned long long *d_bad) {
+// the label check of a step: lowers *d_bad to the first label outside {0, 1}
+static int train_check_labels(gpdb_ctx *ctx, const int32_t *d_labels, int n, unsigned long long *d_bad) {
   k_check_labels<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_labels, n, d_bad);
   LAUNCH_CHECK();
   return GPDB_OK;
 }
 
-int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, int n, float *d_loss_out,
-               float *h_loss_out, const gpdb_train_debug *dbg) {
+// one step on n device images / labels (labels already checked); d_loss_out / h_loss_out: device / host float or null;
+// dbg: host outputs of a debug step (any n, copied chunk by chunk), which updates nothing
+static int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, int n, float *d_loss_out,
+                      float *h_loss_out, const gpdb_train_debug *dbg) {
   TrainState &ts = *ctx->train;
   const int C = ts.C, chunk_n = std::min(n, GPDB_TRAIN_CHUNK);
   ChunkBufs b;
@@ -622,10 +626,117 @@ int train_step(gpdb_ctx *ctx, const uint8_t *d_images, const int32_t *d_labels, 
   return GPDB_OK;
 }
 
-int train_weights(gpdb_ctx *ctx, float *const out[8]) {
+static int train_weights(gpdb_ctx *ctx, float *const out[8]) {
   const TrainState &ts = *ctx->train;
   CUDA_TRY(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < 8; i++)
     CUDA_TRY(cudaMemcpy(out[i], ts.w + ts.off[i], sizeof(float) * ts.len[i], cudaMemcpyDeviceToHost));
   return GPDB_OK;
 }
+
+// ---- entry points: argument checks, host-twin uploads and the C-ABI calls -------------------------------------------
+
+extern "C" {
+
+int gpdb_train_begin(gpdb_ctx *ctx, const gpdb_train_params *p, const float *const init[8]) {
+  int rc = gpdb_check_state(ctx, false, false);
+  if (rc != GPDB_OK) return rc;
+  return train_begin(ctx, p, init);
+}
+
+namespace {
+
+// the checks of a training step before any device work: begun, a 60 x 60 network, n >= 1, the arrays given
+int train_step_args(gpdb_ctx *ctx, const char *name, const void *images, const void *labels, int32_t n) {
+  int rc = gpdb_check_state(ctx, false, false);
+  if (rc != GPDB_OK) return rc;
+  if (!train_started(ctx)) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "%s: call gpdb_train_begin first", name);
+    return GPDB_ERR_STATE;
+  }
+  if (ctx->prm.image_size != 60) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: LeNet expects image_size 60, got %d", name, ctx->prm.image_size);
+    return GPDB_ERR_INVALID;
+  }
+  if (n <= 0 || !images || !labels) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: bad arguments (n = %d)", name, n);
+    return GPDB_ERR_INVALID;
+  }
+  return GPDB_OK;
+}
+
+// the device check of the labels, then the step: a label outside {0, 1} fails the step before anything changes
+int train_step_checked(gpdb_ctx *ctx, const char *name, const uint8_t *d_images, const int32_t *d_labels, int32_t n,
+                       float *d_loss_out, float *h_loss_out, const gpdb_train_debug *dbg) {
+  unsigned long long bad;
+  int rc = first_bad(ctx, 0, &bad, [&](unsigned long long *d_bad, void *) {
+    return train_check_labels(ctx, d_labels, n, d_bad);
+  });
+  if (rc != GPDB_OK) return rc;
+  if (bad != NO_BAD) {
+    int32_t v = 0;
+    CUDA_TRY(cudaMemcpy(&v, d_labels + bad, sizeof(v), cudaMemcpyDeviceToHost));
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: labels[%llu] = %d is not 0 or 1", name, bad, v);
+    return GPDB_ERR_INVALID;
+  }
+  return train_step(ctx, d_images, d_labels, n, d_loss_out, h_loss_out, dbg);
+}
+
+// host twins: upload images and labels (SCR_HWC / SCR_LABELS), then the device path
+int train_step_host(gpdb_ctx *ctx, const char *name, const uint8_t *images_hwc, const int32_t *labels, int32_t n,
+                    float *loss_out, const gpdb_train_debug *dbg) {
+  const size_t isz = (size_t)60 * 60 * ctx->prm.image_num_channels * n;
+  uint8_t *d_img = (uint8_t *)gpdb_scratch(ctx, SCR_HWC, isz);
+  int32_t *d_lab = (int32_t *)gpdb_scratch(ctx, SCR_LABELS, sizeof(int32_t) * (size_t)n);
+  if (!d_img || !d_lab) return GPDB_ERR_CUDA;
+  CUDA_TRY(cudaMemcpyAsync(d_img, images_hwc, isz, cudaMemcpyHostToDevice, ctx->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_lab, labels, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+  return train_step_checked(ctx, name, d_img, d_lab, n, nullptr, loss_out, dbg);
+}
+
+}  // namespace
+
+int gpdb_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n, float *loss_out) {
+  const char *name = "gpdb_train_step";
+  int rc = train_step_args(ctx, name, images_hwc, labels, n);
+  if (rc != GPDB_OK) return rc;
+  return train_step_host(ctx, name, images_hwc, labels, n, loss_out, nullptr);
+}
+
+int gpdb_train_step_device(gpdb_ctx *ctx, const uint8_t *d_images_hwc, const int32_t *d_labels, int32_t n,
+                           float *d_loss_out) {
+  const char *name = "gpdb_train_step_device";
+  int rc = train_step_args(ctx, name, d_images_hwc, d_labels, n);
+  if (rc != GPDB_OK) return rc;
+  rc = gpdb_check_device_ptrs(ctx, name, {{"d_images_hwc", d_images_hwc}, {"d_labels", d_labels}, {"d_loss_out", d_loss_out}});
+  if (rc != GPDB_OK) return rc;
+  return train_step_checked(ctx, name, d_images_hwc, d_labels, n, d_loss_out, nullptr, nullptr);
+}
+
+int gpdb_debug_train_step(gpdb_ctx *ctx, const uint8_t *images_hwc, const int32_t *labels, int32_t n,
+                          gpdb_train_debug *out) {
+  const char *name = "gpdb_debug_train_step";
+  int rc = train_step_args(ctx, name, images_hwc, labels, n);
+  if (rc != GPDB_OK) return rc;
+  if (!out) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "%s: need an output struct", name);
+    return GPDB_ERR_INVALID;
+  }
+  return train_step_host(ctx, name, images_hwc, labels, n, nullptr, out);
+}
+
+int gpdb_train_weights(gpdb_ctx *ctx, float *const out[8]) {
+  int rc = gpdb_check_state(ctx, false, false);
+  if (rc != GPDB_OK) return rc;
+  if (!train_started(ctx)) {
+    gpdb_set_error(ctx, GPDB_ERR_STATE, "gpdb_train_weights: call gpdb_train_begin first");
+    return GPDB_ERR_STATE;
+  }
+  if (!out || !out[0] || !out[1] || !out[2] || !out[3] || !out[4] || !out[5] || !out[6] || !out[7]) {
+    gpdb_set_error(ctx, GPDB_ERR_INVALID, "gpdb_train_weights: null output array");
+    return GPDB_ERR_INVALID;
+  }
+  return train_weights(ctx, out);
+}
+
+}  // extern "C"
